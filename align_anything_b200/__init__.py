@@ -1,5 +1,5 @@
 """align_anything_b200 -- the RLHF loss hot path of PKU-Alignment/align-anything (per-token
-log-prob extraction, DPO pairwise loss, PPO rollout scoring) as hand-written sm_100a CUDA behind a
+log-prob extraction, DPO pairwise loss, PPO rollout scoring) as hand-written sm_90a CUDA behind a
 C ABI (include/aa_b200.h), with a Python host layer that mirrors the reference's own names:
 
     align_anything_b200.utils.tools            <-> align_anything/utils/tools.py

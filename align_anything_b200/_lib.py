@@ -151,7 +151,7 @@ def require_cuda(*tensors: torch.Tensor) -> torch.device:
             continue
         if not t.is_cuda:
             raise RuntimeError(
-                'align_anything_b200 runs on a B200 (sm_100a) only: got a tensor on '
+                'align_anything_b200 runs on an H100 (sm_90a) only: got a tensor on '
                 f'{t.device}.  There is deliberately no CPU fallback.'
             )
         if dev is None:

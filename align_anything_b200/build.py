@@ -1,10 +1,10 @@
-"""Build recipe for libaa_b200.so (hand-written sm_100a CUDA behind a C ABI).
+"""Build recipe for libaa_b200.so (hand-written sm_90a CUDA behind a C ABI).
 
     python -m align_anything_b200.build          # incremental
     python -m align_anything_b200.build --force
 
-nvcc cross-compiles without a GPU.  The .so is written next to the sources (in-tree, git-ignored)
-so that it travels to the GPU box with the repo snapshot.
+nvcc cross-compiles without a GPU.  The .so is written next to the sources (in-tree, git-ignored), where
+_lib.py loads it from.
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ LIB = os.path.join(CSRC, 'libaa_b200.so')
 OBJ_DIR = os.path.join(CSRC, 'build')
 SOURCES = ['capi.cu', 'logprob.cu', 'logprob_fused.cu', 'dpo.cu', 'score_head.cu', 'ppo.cu', 'layout.cu', 'linear_logprob.cu', 'linear_backward.cu']
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a',
+    '-gencode', 'arch=compute_90a,code=sm_90a',
     '-O3', '-lineinfo', '-std=c++17',
     '-Xcompiler', '-fPIC',
     '-Xptxas', '-v',
@@ -70,7 +70,7 @@ def build_experiment(tag: str, defines: list[str]) -> str:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every .cu for sm_100a and link libaa_b200.so.  Returns the library path."""
+    """Compile every .cu for sm_90a and link libaa_b200.so.  Returns the library path."""
     if not force and is_fresh():
         return LIB
     nvcc = _nvcc()
@@ -88,7 +88,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [nvcc, '-gencode', 'arch=compute_100a,code=sm_100a', '-shared', '-o', LIB, *objs]
+    cmd = [nvcc, '-gencode', 'arch=compute_90a,code=sm_90a', '-shared', '-o', LIB, *objs]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f'link failed:\n{r.stdout}\n{r.stderr}')

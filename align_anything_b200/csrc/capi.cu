@@ -26,11 +26,11 @@ int sm_count() {
   static thread_local int cached_dev = -1;
   static thread_local int cached = 0;
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (dev != cached_dev) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
     cached = n;
     cached_dev = dev;
   }
@@ -53,8 +53,8 @@ extern "C" int aa_device_info(int *sm_count, int *max_smem_optin) {
   int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-  if (major != 10) {
-    aa::set_error("aa_device_info: device %d is sm_%d%d; libaa_b200 is built for sm_100a only", dev,
+  if (major != 9 || minor != 0) {
+    aa::set_error("aa_device_info: device %d is sm_%d%d; libaa_b200 is built for sm_90a (H100) only", dev,
                   major, minor);
     return AA_ERR_UNSUPPORTED;
   }

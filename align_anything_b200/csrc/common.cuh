@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for libaa_b200 (sm_100a only).
+// common.cuh -- shared device helpers for libaa_b200 (sm_90a only).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -9,8 +9,8 @@
 
 #include "../../include/aa_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libaa_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libaa_b200 is written for sm_90a (H100) only"
 #endif
 
 namespace aa {
@@ -140,7 +140,7 @@ __device__ __forceinline__ uint4 ldg_stream(const uint4 *p) {
       : "l"(p));
   return r;
 }
-// store policy (compile-time experiment knob, see tools/sweep_k1.py): 0 = .cs (evict-first),
+// store policy (compile-time experiment knob): 0 = .cs (evict-first),
 // 1 = default write-back, 2 = .L1::no_allocate, 3 = .wt
 #ifndef AA_STG_POLICY
 #define AA_STG_POLICY 0
@@ -163,38 +163,21 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return r;
 }
 
-// ---- packed fp32 pairs (Blackwell f32x2: FADD2 / FMUL2 / FFMA2, one issue slot for two lanes of math) ----
-// The log-prob kernels are bound by instruction issue once the SM clock drops under the power cap
-// (1.72 GHz sustained vs 1.95 GHz burst), so the per-element fp32 ops are issued two at a time.
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 f2_pack(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
+// ---- fp32 pairs: the per-element math of the log-prob kernels is written two lanes at a time --------------
+// sm_90 has no packed fp32 instructions, so each pair op is two scalar round-to-nearest ops.  The __f*_rn
+// intrinsics are never contracted into FMAs, which the Veltkamp rounding below depends on.
+typedef float2 f32x2;
+__device__ __forceinline__ f32x2 f2_pack(float lo, float hi) { return make_float2(lo, hi); }
 __device__ __forceinline__ void f2_unpack(f32x2 v, float &lo, float &hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
+  lo = v.x;
+  hi = v.y;
 }
 __device__ __forceinline__ f32x2 f2_splat(float v) { return f2_pack(v, v); }
-__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2 f2_sub(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
+__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 f2_sub(f32x2 a, f32x2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 __device__ __forceinline__ f32x2 f2_ex2(f32x2 t) {
   float a, b;
@@ -202,13 +185,13 @@ __device__ __forceinline__ f32x2 f2_ex2(f32x2 t) {
   return f2_pack(ex2_approx(a), ex2_approx(b));
 }
 // Round both lanes to 8 significant bits (= bf16 round-to-nearest) WITHOUT the conversion unit:
-// Veltkamp splitting, hi = c - (c - x) with c = x * (2^16 + 1).  Three FMA-pipe ops per pair instead
-// of an F2FP round trip on the XU pipe (which MUFU.EX2 already keeps ~70% busy in the backward).
+// Veltkamp splitting, hi = c - (c - x) with c = x * (2^16 + 1).  FMA-pipe ops instead of a conversion
+// round trip, which shares its pipe with MUFU.EX2.
 // Bit-identical to __float2bfloat16_rn for normal numbers (checked on 5M samples); inputs must be
 // finite (callers clamp -inf logits to -1e30 first).
-// `zero2` must be a RUN-TIME +0.0 pair (kernel parameter): ptxas contracts mul.rn.f32x2 + sub.rn.f32x2
-// into FFMA2 (observed with CUDA 12.9: d = fma(x, 65537, -x)), which destroys the split; producing c
-// with an FMA whose addend the compiler cannot see through leaves nothing to contract.
+// `zero2` must be a RUN-TIME +0.0 pair (kernel parameter): ptxas may contract a multiply and a subtract
+// into an FMA (d = fma(x, 65537, -x)), which destroys the split; producing c with an FMA whose addend
+// the compiler cannot see through leaves nothing to contract.
 __device__ __forceinline__ f32x2 f2_round_bf16(f32x2 x, f32x2 zero2) {
   const f32x2 c = f2_fma(x, f2_splat(65537.f), zero2);
   return f2_sub(c, f2_sub(c, x));
@@ -222,8 +205,7 @@ __device__ __forceinline__ f32x2 f2_round_f16(f32x2 x, f32x2 zero2) {
 // 2^t on the FMA / ALU pipes (no MUFU): Cody-Waite split t = n + f, f in [-0.5, 0.5], degree-5 minimax
 // polynomial with c0 == 1 exactly (so 2^0 == 1 exactly, like MUFU.EX2), exponent patched in with one
 // integer add.  Max relative error 1.9e-7 (MUFU.EX2: 2^-22 = 2.4e-7).  An experiment to unload the
-// MUFU pipe (16/clk/SM on B200, 73% busy in the forward per ncu); it measured slower (logprob.cu,
-// AA_FWD_POLY_WORDS) and is off by default.
+// MUFU pipe (16/clk/SM); it is off by default (logprob.cu, AA_FWD_POLY_WORDS).
 __device__ __forceinline__ float ex2_poly(float t) {
   float tc;
   asm("max.NaN.f32 %0, %1, %2;" : "=f"(tc) : "f"(t), "f"(-126.f));  // NaN stays NaN

@@ -4,10 +4,10 @@
 //   d(weight) (V, H) += dlogits^T (V, n) . hidden (n, H)            aa_linear_dweight
 //
 // i.e. the autograd of the model's `nn.Linear` lm_head (callers trainers/text_to_text/dpo.py:128, ppo.py:338) given the
-// d(logits) tile that K6b (linear_logprob.cu) recomputes on the tensor cores.  Both run on the K6 pipeline -- warp 0 =
-// TMA producer into a 4-stage 128-byte-swizzled ring, warp 1 = tcgen05.mma issuer (M128 N256 K16, fp32 accumulators in
-// TMEM, two 256-column accumulators alternating), warps 2-5 = epilogue straight out of TMEM -- as ONE persistent kernel
-// template whose operands may be K-major or MN-major:
+// d(logits) tile that K6b (linear_logprob.cu) recomputes on the tensor cores.  Both run on the K6 pipeline (wgmma.cuh) --
+// a producer thread streams TMA boxes into a 4-stage 128-byte-swizzled ring, two consumer warpgroups multiply with
+// wgmma m64n256k16 into fp32 registers and write their 64 x 256 slice of the tile -- as ONE persistent kernel template
+// whose operands may be K-major or MN-major:
 //
 //   d(hidden): A = dlogits, K-major (K = vocabulary, contiguous);  B = weight seen as (N = H, K = V): H is the contiguous
 //              index of `weight`, so B is MN-major -- no transposed or padded copy of the 1 GB weight is ever made;
@@ -15,7 +15,7 @@
 //   d(weight): A = dlogits seen as (M = V, K = n) and B = hidden seen as (N = H, K = n): both MN-major.
 //
 // MN-major tiles are brought in as 64-wide boxes (one swizzle span) of BK rows each; the shared-memory descriptors
-// (umma.cuh) describe that layout directly, the instruction descriptor carries the a_major / b_major bits.
+// (wgmma.cuh) describe that layout directly, the transpose bits of the instruction select it.
 // Persistent grid: CTA b walks tiles b, b + grid, ... with the N tiles of one M tile adjacent, so the CTAs resident
 // together share their A strip through L2.  d(weight) accumulates across row chunks in an fp32 buffer (read-modify-write
 // in the epilogue) and is rounded to bf16 once, by the last chunk -- like a single GEMM over all rows.
@@ -23,16 +23,12 @@
 
 #include <atomic>
 
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace aa {
 namespace lmbwd {
 
-using namespace umma;
-
-constexpr int STAGES = 4;
-constexpr int THREADS = 192;  // warp 0 TMA, warp 1 MMA, warps 2..5 epilogue
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /* alignment slack */ + 256 /* barriers */;
+using namespace wg;
 
 struct GemmParams {
   int M, N, K;               // C (M x N) = A (M x K) . B (N x K)^T
@@ -65,35 +61,24 @@ __global__ void __launch_bounds__(THREADS, 1)
   uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t *full = reinterpret_cast<uint64_t *>(tiles + STAGES * STAGE_BYTES);
   uint64_t *empty = full + STAGES;
-  uint64_t *acc_full = empty + STAGES;  // [2]
-  uint64_t *acc_empty = acc_full + 2;   // [2]
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_tiles = p.tiles_m * p.tiles_n;
   const int k_blocks = (p.K + BK - 1) / BK;
-  constexpr uint32_t kIdesc = instr_desc(A_MN, B_MN);
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(full + i, 1);
-      mbar_init(empty + i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(acc_full + i, 1);
-      mbar_init(acc_empty + i, 128);
+      mbar_init(empty + i, CONSUMER_THREADS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc_512(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (threadIdx.x >= CONSUMER_THREADS) {
     // ------------------------------- TMA producer -------------------------------
-    if (lane == 0) {
+    producer_regs();
+    if (warp == CONSUMER_THREADS / 32 && lane == 0) {
       int64_t it = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         int mt, nt;
@@ -101,8 +86,7 @@ __global__ void __launch_bounds__(THREADS, 1)
         const int m0 = mt * BM, n0 = nt * BN;
         for (int kb = 0; kb < k_blocks; ++kb, ++it) {
           const int s = static_cast<int>(it % STAGES);
-          const uint32_t ph = static_cast<uint32_t>((it / STAGES) & 1);
-          mbar_wait(empty + s, ph ^ 1u);
+          mbar_wait(empty + s, static_cast<uint32_t>((it / STAGES) & 1) ^ 1u);
           uint8_t *a = tiles + s * STAGE_BYTES, *b = a + A_BYTES;
           mbar_expect_tx(full + s, STAGE_BYTES);
           if (A_MN) {  // inner coordinate = M, outer = K rows; one box per 64-wide M chunk
@@ -120,300 +104,36 @@ __global__ void __launch_bounds__(THREADS, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------- MMA issuer ---------------------------------
-    if (lane == 0) {
-      int64_t it = 0;
-      int lt = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
-        const int acc = lt & 1;
-        const uint32_t aph = static_cast<uint32_t>((lt >> 1) & 1);
-        mbar_wait(acc_empty + acc, aph ^ 1u);  // the epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_c = tmem_base + static_cast<uint32_t>(acc * BN);
-        for (int kb = 0; kb < k_blocks; ++kb, ++it) {
-          const int s = static_cast<int>(it % STAGES);
-          const uint32_t ph = static_cast<uint32_t>((it / STAGES) & 1);
-          mbar_wait(full + s, ph);
-          tc_fence_after();
-          const uint32_t a = smem_u32(tiles + s * STAGE_BYTES), b = a + A_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k)
-            mma_f16(tmem_c, operand_desc<A_MN>(a, k), operand_desc<B_MN>(b, k), kIdesc, (kb | k) != 0 ? 1u : 0u);
-          mma_commit(empty + s);  // frees the ring stage once these MMAs have read it
-        }
-        mma_commit(acc_full + acc);  // accumulator complete
-      }
-    }
-  } else {
-    // ------------------------------- epilogue: one thread per row ----------------
-    const int q = warp & 3;  // TMEM lane quadrant this warp may read
-    int lt = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
-      int mt, nt;
-      tile_coords(p, tile, mt, nt);
-      const int m0 = mt * BM, n0 = nt * BN;
-      const int acc = lt & 1;
-      const uint32_t aph = static_cast<uint32_t>((lt >> 1) & 1);
-      const int64_t row = static_cast<int64_t>(m0) + q * 32 + lane;
-      const bool live = row < p.M;
-      mbar_wait(acc_full + acc, aph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * BN);
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        const int col0 = n0 + c * 32;
-        if (col0 >= p.N) break;  // warp-uniform (N is a multiple of 32)
-        uint32_t v[32];
-        tmem_ld32(taddr + static_cast<uint32_t>(c * 32), v);
-        if (!live) continue;
-        float *acc_row = p.c_f32 ? p.c_f32 + row * p.ldc_f32 + col0 : nullptr;
-        if (p.beta) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 o = *reinterpret_cast<const float4 *>(acc_row + j);
-            v[j] = __float_as_uint(__uint_as_float(v[j]) + o.x);
-            v[j + 1] = __float_as_uint(__uint_as_float(v[j + 1]) + o.y);
-            v[j + 2] = __float_as_uint(__uint_as_float(v[j + 2]) + o.z);
-            v[j + 3] = __float_as_uint(__uint_as_float(v[j + 3]) + o.w);
-          }
-        }
-        if (p.c_bf16) {
-          uint4 *dst = reinterpret_cast<uint4 *>(p.c_bf16 + row * p.ldc_bf16 + col0);
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            dst[j / 8] = make_uint4(pack2<__nv_bfloat16>(__uint_as_float(v[j]), __uint_as_float(v[j + 1])),
-                                    pack2<__nv_bfloat16>(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3])),
-                                    pack2<__nv_bfloat16>(__uint_as_float(v[j + 4]), __uint_as_float(v[j + 5])),
-                                    pack2<__nv_bfloat16>(__uint_as_float(v[j + 6]), __uint_as_float(v[j + 7])));
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<uint4 *>(acc_row + j) = make_uint4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(acc_empty + acc);
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc_512(tmem_base);
-}
-
-// ---- CTA-pair form (default; AA_B200_GEMM_PAIR=0 selects the single-CTA kernel above) --------------------------------
-// Verified on a B200 (tools/r2/gemm_diag.py operand-map probes, tests/test_gpu_parity.py) and faster than the single-CTA
-// form on the 16 376 x 128512 x 4096 backward: d(hidden) 13.6 -> 12.2 ms (1266 -> 1411 TFLOP/s), d(weight) 14.6 -> 13.8 ms.
-// The same GEMM on CTA PAIRS (tcgen05 cta_group::2): the two CTAs of a cluster own one 256 x 256 output tile.  Each
-// holds its 128 rows of A, its HALF of the B tile (128 of the 256 N rows) and its 128 x 256 slice of the accumulator
-// in its own TMEM; the leader (cluster rank 0) issues M = 256 MMAs that read both CTAs' shared memory.  Per k-block a
-// CTA stages 32 KB instead of 48 KB, so the ring is 6 deep instead of 4 (1.6 us instead of 1.1 us of latency cover at
-// the MMA rate) and the L2 -> SM operand traffic of the B tile is halved.  Synchronisation:
-//   full[s]      (leader's)  one arrive.expect_tx by the leader's producer for BOTH CTAs' bytes; both producers' TMA
-//                            loads complete on it (cp.async.bulk.tensor ... cta_group::2 may credit the peer's barrier)
-//   empty[s], acc_full[a]    (one per CTA) tcgen05.commit.cta_group::2 ... multicast::cluster arrives on both at once
-//   acc_empty[a] (leader's)  256 arrivals: the leader's epilogue threads locally, the peer's through shared::cluster
-constexpr int PAIR_STAGES = 6;
-constexpr int PAIR_B_BYTES = B_BYTES / 2;
-constexpr int PAIR_STAGE_BYTES = A_BYTES + PAIR_B_BYTES;
-constexpr int PAIR_SMEM_BYTES = PAIR_STAGES * PAIR_STAGE_BYTES + 1024 + 256;
-
-template <int A_MN, int B_MN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(THREADS, 1)
-    lm_head_bwd_gemm_pair_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                                 const GemmParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t *full = reinterpret_cast<uint64_t *>(tiles + PAIR_STAGES * PAIR_STAGE_BYTES);
-  uint64_t *empty = full + PAIR_STAGES;
-  uint64_t *acc_full = empty + PAIR_STAGES;  // [2]
-  uint64_t *acc_empty = acc_full + 2;        // [2]
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int n_clusters = gridDim.x / 2, cluster_id = blockIdx.x / 2;
-  const int total_tiles = p.tiles_m * p.tiles_n;  // tiles of 256 x 256
-  const int k_blocks = (p.K + BK - 1) / BK;
-  constexpr uint32_t kIdesc = instr_desc_pair(A_MN, B_MN);
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < PAIR_STAGES; ++i) {
-      mbar_init(full + i, 1);
-      mbar_init(empty + i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(acc_full + i, 1);
-      mbar_init(acc_empty + i, 256);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) tmem_alloc_512_pair(tmem_slot);
-  tc_fence_before();
-  cluster_sync_all();  // barriers initialised and TMEM allocated in both CTAs before anybody signals across
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ------------------------------- TMA producer (both CTAs) -------------------
-    if (lane == 0) {
-      int64_t it = 0;
-      for (int tile = cluster_id; tile < total_tiles; tile += n_clusters) {
-        int mt, nt;
-        tile_coords(p, tile, mt, nt);
-        const int m0 = mt * (2 * BM) + static_cast<int>(rank) * BM;
-        const int n0 = nt * BN + static_cast<int>(rank) * (BN / 2);
-        for (int kb = 0; kb < k_blocks; ++kb, ++it) {
-          const int s = static_cast<int>(it % PAIR_STAGES);
-          const uint32_t ph = static_cast<uint32_t>((it / PAIR_STAGES) & 1);
-          mbar_wait(empty + s, ph ^ 1u);
-          uint8_t *a = tiles + s * PAIR_STAGE_BYTES, *b = a + A_BYTES;
-          if (leader) mbar_expect_tx(full + s, 2 * PAIR_STAGE_BYTES);
-          const uint32_t bar = mapa_u32(full + s, 0);
-          if (A_MN) {
+  // ------------------------------- consumers: wgmma + epilogue ----------------------------
+  consumer_regs();
+  const int w = threadIdx.x >> 7, t = threadIdx.x & 127;
+  float acc[ACC];
+  int64_t it = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    int mt, nt;
+    tile_coords(p, tile, mt, nt);
+    const int m0 = mt * BM + 64 * w, n0 = nt * BN;
+    consume_tile<A_MN, B_MN>(acc, tiles, full, empty, k_blocks, it, w);
 #pragma unroll
-            for (int c = 0; c < BM / 64; ++c) tma_load_2d_pair(a + c * (BK * 128), &map_a, m0 + 64 * c, kb * BK, bar);
-          } else {
-            tma_load_2d_pair(a, &map_a, kb * BK, m0, bar);
-          }
-          if (B_MN) {
-#pragma unroll
-            for (int c = 0; c < BN / 128; ++c) tma_load_2d_pair(b + c * (BK * 128), &map_b, n0 + 64 * c, kb * BK, bar);
-          } else {
-            tma_load_2d_pair(b, &map_b, kb * BK, n0, bar);  // box of BN / 2 rows (the host builds the map so)
-          }
-        }
+    for (int i = 0; i < ACC; i += 2) {  // (i, i + 1): one row, two adjacent columns
+      const int64_t row = m0 + frag_row(t, i);
+      const int col = n0 + frag_col(t, i);
+      if (row >= p.M || col >= p.N) continue;  // N is a multiple of 64: a pair never straddles it
+      float v0 = acc[i], v1 = acc[i + 1];
+      if (p.beta) {
+        const float2 o = *reinterpret_cast<const float2 *>(p.c_f32 + row * p.ldc_f32 + col);
+        v0 += o.x;
+        v1 += o.y;
       }
-    }
-  } else if (warp == 1) {
-    // ------------------------------- MMA issuer (leader CTA only) ---------------
-    if (leader && lane == 0) {
-      int64_t it = 0;
-      int lt = 0;
-      for (int tile = cluster_id; tile < total_tiles; tile += n_clusters, ++lt) {
-        const int acc = lt & 1;
-        const uint32_t aph = static_cast<uint32_t>((lt >> 1) & 1);
-        mbar_wait(acc_empty + acc, aph ^ 1u);  // both CTAs' epilogues have drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_c = tmem_base + static_cast<uint32_t>(acc * BN);
-        for (int kb = 0; kb < k_blocks; ++kb, ++it) {
-          const int s = static_cast<int>(it % PAIR_STAGES);
-          const uint32_t ph = static_cast<uint32_t>((it / PAIR_STAGES) & 1);
-          mbar_wait(full + s, ph);
-          tc_fence_after();
-          const uint32_t a = smem_u32(tiles + s * PAIR_STAGE_BYTES), b = a + A_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k)
-            mma_f16_pair(tmem_c, operand_desc<A_MN>(a, k), operand_desc<B_MN>(b, k), kIdesc, (kb | k) != 0 ? 1u : 0u);
-          mma_commit_pair(empty + s);  // frees this ring stage in BOTH CTAs
-        }
-        mma_commit_pair(acc_full + acc);  // accumulator complete, both CTAs' epilogues may read
-      }
-    }
-  } else {
-    // ------------------------------- epilogue (both CTAs, own 128 rows) ---------
-    const int q = warp & 3;
-    int lt = 0;
-    for (int tile = cluster_id; tile < total_tiles; tile += n_clusters, ++lt) {
-      int mt, nt;
-      tile_coords(p, tile, mt, nt);
-      const int m0 = mt * (2 * BM) + static_cast<int>(rank) * BM, n0 = nt * BN;
-      const int acc = lt & 1;
-      const uint32_t aph = static_cast<uint32_t>((lt >> 1) & 1);
-      const int64_t row = static_cast<int64_t>(m0) + q * 32 + lane;
-      const bool live = row < p.M;
-      mbar_wait(acc_full + acc, aph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * BN);
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        const int col0 = n0 + c * 32;
-        if (col0 >= p.N) break;
-        uint32_t v[32];
-        tmem_ld32(taddr + static_cast<uint32_t>(c * 32), v);
-        if (!live) continue;
-        float *acc_row = p.c_f32 ? p.c_f32 + row * p.ldc_f32 + col0 : nullptr;
-        if (p.beta) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 o = *reinterpret_cast<const float4 *>(acc_row + j);
-            v[j] = __float_as_uint(__uint_as_float(v[j]) + o.x);
-            v[j + 1] = __float_as_uint(__uint_as_float(v[j + 1]) + o.y);
-            v[j + 2] = __float_as_uint(__uint_as_float(v[j + 2]) + o.z);
-            v[j + 3] = __float_as_uint(__uint_as_float(v[j + 3]) + o.w);
-          }
-        }
-        if (p.c_bf16) {
-          uint4 *dst = reinterpret_cast<uint4 *>(p.c_bf16 + row * p.ldc_bf16 + col0);
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            dst[j / 8] = make_uint4(pack2<__nv_bfloat16>(__uint_as_float(v[j]), __uint_as_float(v[j + 1])),
-                                    pack2<__nv_bfloat16>(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3])),
-                                    pack2<__nv_bfloat16>(__uint_as_float(v[j + 4]), __uint_as_float(v[j + 5])),
-                                    pack2<__nv_bfloat16>(__uint_as_float(v[j + 6]), __uint_as_float(v[j + 7])));
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<uint4 *>(acc_row + j) = make_uint4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        }
-      }
-      tc_fence_before();
-      if (leader)
-        mbar_arrive(acc_empty + acc);
+      if (p.c_bf16)
+        *reinterpret_cast<uint32_t *>(p.c_bf16 + row * p.ldc_bf16 + col) = pack2<__nv_bfloat16>(v0, v1);
       else
-        mbar_arrive_cluster(mapa_u32(acc_empty + acc, 0));
+        *reinterpret_cast<float2 *>(p.c_f32 + row * p.ldc_f32 + col) = make_float2(v0, v1);
     }
   }
-
-  tc_fence_before();
-  cluster_sync_all();  // nobody leaves (or frees TMEM) while the peer may still signal / read across
-  if (warp == 1) tmem_dealloc_512_pair(tmem_base);
-}
-
-template <int A_MN, int B_MN>
-static int launch_pair(const CUtensorMap &map_a, const CUtensorMap &map_b, GemmParams p, cudaStream_t st, const char *who) {
-  auto kern = lm_head_bwd_gemm_pair_kernel<A_MN, B_MN>;
-  static std::atomic<bool> configured{false};
-  if (!configured.load(std::memory_order_relaxed)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PAIR_SMEM_BYTES);
-    if (e != cudaSuccess) {
-      set_error("%s: %s", who, cudaGetErrorString(e));
-      return static_cast<int>(e);
-    }
-    configured.store(true, std::memory_order_relaxed);
-  }
-  p.tiles_m = (p.M + 2 * BM - 1) / (2 * BM);  // 256-row tiles
-  const int total = p.tiles_m * p.tiles_n;
-  // how many CTA pairs can be resident at once (a pair needs both SMs of one TPC; not every TPC of a 148-SM part has two)
-  static std::atomic<int> max_pairs{0};
-  int cap = max_pairs.load(std::memory_order_relaxed);
-  if (cap == 0) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(static_cast<unsigned>(sm_count() / 2 * 2));
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = PAIR_SMEM_BYTES;
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = 2;
-    attr.val.clusterDim.y = 1;
-    attr.val.clusterDim.z = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) {
-      cudaGetLastError();
-      n = sm_count() / 2;
-    }
-    cap = n;
-    max_pairs.store(cap, std::memory_order_relaxed);
-  }
-  const int pairs = total < cap ? total : cap;
-  kern<<<2 * pairs, THREADS, PAIR_SMEM_BYTES, st>>>(map_a, map_b, p);
-  return check_launch(who);
 }
 
 // tile-order override for sweeps, read once: AA_B200_GEMM_BAND_DH / _DW = N tiles per band (0 = all N tiles, one band)
@@ -421,14 +141,6 @@ static int band_env(int which) {
   static const int v[2] = {[] { const char *e = getenv("AA_B200_GEMM_BAND_DH"); return e ? atoi(e) : 0; }(),
                            [] { const char *e = getenv("AA_B200_GEMM_BAND_DW"); return e ? atoi(e) : 0; }()};
   return v[which];
-}
-
-static bool use_pairs() {
-  static const bool on = [] {
-    const char *e = getenv("AA_B200_GEMM_PAIR");
-    return !e || atoi(e) > 0;
-  }();
-  return on;
 }
 
 template <int A_MN, int B_MN>
@@ -467,18 +179,17 @@ extern "C" int aa_linear_dhidden(const void *dlogits, int64_t n_rows, int64_t ld
                  weight_row_stride % 8 == 0 && weight_row_stride >= H && d_hidden_row_stride % 8 == 0 &&
                  d_hidden_row_stride >= H,
              AA_ERR_ALIGN, "aa_linear_dhidden: operands must be 16-byte aligned with 16-byte row strides");
-  AA_REQUIRE(n_rows < (int64_t(1) << 31) - umma::BM, AA_ERR_UNSUPPORTED, "aa_linear_dhidden: too many rows");
+  AA_REQUIRE(n_rows < (int64_t(1) << 31) - wg::BM, AA_ERR_UNSUPPORTED, "aa_linear_dhidden: too many rows");
   CUtensorMap map_a, map_b;
   // A = dlogits (n_rows, ld): K-major, box 64 (K) x 128 rows.  Columns [V, ld) are zero (K6b writes them so).
-  int rc = umma::make_map_2d(&map_a, dlogits, ld, n_rows, ld, umma::BM, "aa_linear_dhidden");
+  int rc = wg::make_map_2d(&map_a, dlogits, ld, n_rows, ld, wg::BM, "aa_linear_dhidden");
   if (rc) return rc;
   // B = weight (V, H) read as (N = H contiguous, K = V rows): MN-major, box 64 (N) x 64 (K rows); rows >= V read as zero
-  rc = umma::make_map_2d(&map_b, weight, H, V, weight_row_stride, umma::BK, "aa_linear_dhidden");
+  rc = wg::make_map_2d(&map_b, weight, H, V, weight_row_stride, wg::BK, "aa_linear_dhidden");
   if (rc) return rc;
   lmbwd::GemmParams p{static_cast<int>(n_rows), H, static_cast<int>(ld), static_cast<__nv_bfloat16 *>(d_hidden),
-                      d_hidden_row_stride, nullptr, 0, 0, static_cast<int>((n_rows + umma::BM - 1) / umma::BM),
-                      (H + umma::BN - 1) / umma::BN, lmbwd::band_env(0)};
-  if (lmbwd::use_pairs()) return lmbwd::launch_pair<0, 1>(map_a, map_b, p, static_cast<cudaStream_t>(stream), "aa_linear_dhidden(pair)");
+                      d_hidden_row_stride, nullptr, 0, 0, static_cast<int>((n_rows + wg::BM - 1) / wg::BM),
+                      (H + wg::BN - 1) / wg::BN, lmbwd::band_env(0)};
   return lmbwd::launch<0, 1>(map_a, map_b, p, static_cast<cudaStream_t>(stream), "aa_linear_dhidden");
 }
 
@@ -496,17 +207,16 @@ extern "C" int aa_linear_dweight(const void *dlogits, int64_t n_rows, int64_t ld
                  (!acc_f32 || (acc_row_stride % 4 == 0 && acc_row_stride >= H)) &&
                  (!d_weight || (d_weight_row_stride % 8 == 0 && d_weight_row_stride >= H)),
              AA_ERR_ALIGN, "aa_linear_dweight: operands must be 16-byte aligned with 16-byte row strides");
-  AA_REQUIRE(n_rows < (int64_t(1) << 31) - umma::BK, AA_ERR_UNSUPPORTED, "aa_linear_dweight: too many rows");
+  AA_REQUIRE(n_rows < (int64_t(1) << 31) - wg::BK, AA_ERR_UNSUPPORTED, "aa_linear_dweight: too many rows");
   CUtensorMap map_a, map_b;
   // A = dlogits (n_rows, ld) read as (M = vocabulary contiguous, K = rows): MN-major
-  int rc = umma::make_map_2d(&map_a, dlogits, ld, n_rows, ld, umma::BK, "aa_linear_dweight");
+  int rc = wg::make_map_2d(&map_a, dlogits, ld, n_rows, ld, wg::BK, "aa_linear_dweight");
   if (rc) return rc;
   // B = hidden (n_rows, H) read as (N = H contiguous, K = rows): MN-major
-  rc = umma::make_map_2d(&map_b, hidden, H, n_rows, hidden_row_stride, umma::BK, "aa_linear_dweight");
+  rc = wg::make_map_2d(&map_b, hidden, H, n_rows, hidden_row_stride, wg::BK, "aa_linear_dweight");
   if (rc) return rc;
   lmbwd::GemmParams p{V, H, static_cast<int>(n_rows), static_cast<__nv_bfloat16 *>(d_weight), d_weight_row_stride, acc_f32,
-                      acc_row_stride, accumulate ? 1 : 0, (V + umma::BM - 1) / umma::BM, (H + umma::BN - 1) / umma::BN,
+                      acc_row_stride, accumulate ? 1 : 0, (V + wg::BM - 1) / wg::BM, (H + wg::BN - 1) / wg::BN,
                       lmbwd::band_env(1)};
-  if (lmbwd::use_pairs()) return lmbwd::launch_pair<1, 1>(map_a, map_b, p, static_cast<cudaStream_t>(stream), "aa_linear_dweight(pair)");
   return lmbwd::launch<1, 1>(map_a, map_b, p, static_cast<cudaStream_t>(stream), "aa_linear_dweight");
 }

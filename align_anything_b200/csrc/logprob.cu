@@ -417,8 +417,7 @@ __global__ void __launch_bounds__(THREADS) logprob_bwd_kernel(const BwdParams p)
 }
 
 // ---- K1b, chunked (experiment, selected with tuning kernel digit 2): the gradient tile is swept in
-// address order.  MEASURED SLOWER on B200 than the one-CTA-per-row kernel above (4.4-5.4 TB/s vs
-// 5.7-6.0 TB/s at V = 128257, tools/sweep_k1.py) -- kept for study, not the default.
+// address order.  An experiment, not the default: it was slower than the one-CTA-per-row kernel above.
 // The backward needs no per-row reduction (max / logsum come from the forward), so a row does not
 // have to be owned by one CTA.  Work unit = (row, chunk of THREADS*UNROLL 16-byte vectors);
 // consecutive CTAs take consecutive units, so at any moment the whole grid reads and writes one
@@ -563,11 +562,10 @@ __global__ void __launch_bounds__(THREADS)
 }
 
 // ---- K1b, TMA-staged (default for 16-byte-phase-compatible tiles) ---------------------------------
-// Micro-benchmark on B200 (tools/micro/copy_bw.cu, 8 GiB read + 8 GiB write): the same one-CTA-per-row
-// access structure as the LDG kernel above tops out at 5.97-6.30 TB/s for a PURE copy, while the copy
-// engine (cp.async.bulk global->smem, smem->global, 64 KB in flight per SM) reaches 6.59 TB/s =
-// cudaMemcpy speed.  So the backward moves its data with the TMA engine in both directions and the SM
-// only touches shared memory:
+// A pure copy with the one-CTA-per-row access structure of the LDG kernel above stays below what the copy
+// engine (cp.async.bulk global->smem, smem->global, 64 KB in flight per SM) reaches, which is cudaMemcpy
+// speed.  So the backward moves its data with the TMA engine in both directions and the SM only touches
+// shared memory:
 //   producer lane : RowRec -> cp.async.bulk loads of 16 KB chunks of the row's aligned body into a ring
 //                   (full mbarriers, expect_tx), and -- lagging LAG chunks behind -- cp.async.bulk
 //                   STORES of the chunks the consumers have finished (done mbarriers); zero rows are
@@ -779,9 +777,8 @@ static int launch_fwd(const FwdParams &p, cudaStream_t st) {
       default: break;
     }
   }
-  // default (16-bit logits): 128 threads x 8 vectors in flight, 16 CTAs/SM.  Measured in the sustained
-  // full-size bench (bench.py, 33.6 GB tile, SM clock ~1.75-1.85 GHz under the power cap):
-  // 128x8x16 -> 6.20 TB/s, 256x4x6 -> 5.70-5.75 TB/s; burst (tools/sweep_k1.py): 6.8 vs 6.4 TB/s.
+  // default (16-bit logits): 128 threads x 8 vectors in flight, 16 CTAs/SM -- the read-only stream likes many bytes
+  // in flight (the shapes above are the alternatives selected with aa_logprob_set_tuning).
   if constexpr (sizeof(T) == 2) return launch_fwd_shape<T, 128, 8>(p, fwd_ctas() > 0 ? fwd_ctas() : 16, st);
   return launch_fwd_shape<T, 256, 4>(p, per_sm, st);
 }
@@ -874,8 +871,6 @@ static int launch_bwd_tma_shape(const BwdParams &p, int mode, int per_sm, RowRec
 // shape codes of the TMA-staged backward (stages x stage size, lag, default CTAs/SM):
 //   0 (default): 4 x 8 KB, lag 3, 3 CTAs/SM   1: 4 x 16 KB, lag 2, 2   2: 4 x 8 KB, lag 3, 3 (= default)
 //   3: 6 x 8 KB, lag 4, 2                     4: 3 x 16 KB, lag 2, 2   5: 8 x 8 KB, lag 6, 2   6: 4 x 16 KB, lag 3, 2
-// Measured (bench.py, sustained, 67.2 GB per launch): 4x8KB/lag3 x3 CTAs -> 10.37 ms = 6.48 TB/s (0.986 of the
-// measured copy peak); x4 CTAs 5.92; 4x16KB/lag3 x2 CTAs 6.38, x3 5.69; 6x8KB x3 5.94; LDG row kernel 5.79.
 template <typename T>
 static int launch_bwd_tma(const BwdParams &p, int mode, RowRec *rec, cudaStream_t st) {
   const int shape = (bwd_variant() / 10) % 10;
@@ -906,11 +901,8 @@ static int launch_bwd(const BwdParams &p, int mode, cudaStream_t st) {
     }
   }
   // default (16-bit logits).  The read+write stream is sensitive to how much is in flight per SM and the
-  // optimum depends on the compute per byte of the variant (tools/sweep_k1.py, V = 128257, reproducible
-  // to 1%; torch's copy_ reaches 6.6 TB/s on the same boxes):
-  //   FAITHFUL (Veltkamp rounding, ~7 instr/elem): 512 thr x 4 vec x 3 CTAs/SM -> 5.74 TB/s sustained in
-  //     bench.py (5.86-5.91 burst); 512x2x4 -> 5.44 sustained (5.89 burst); 512x2x3 -> 5.40 burst.
-  //   F32 mode (~3.5 instr/elem): 512x2x3 -> 5.93 TB/s burst (x4: 5.56).
+  // optimum depends on the compute per byte of the variant: FAITHFUL (Veltkamp rounding, ~7 instr/elem)
+  // 512 thr x 4 vec x 3 CTAs/SM, F32 mode (~3.5 instr/elem) 512 x 2 x 3.
   if constexpr (sizeof(T) == 2) {
     if (mode == AA_MODE_FAITHFUL) return launch_bwd_shape<T, 512, 4>(p, mode, bwd_ctas() > 0 ? bwd_ctas() : 3, st);
     return launch_bwd_shape<T, 512, 2>(p, mode, bwd_ctas() > 0 ? bwd_ctas() : 3, st);
@@ -1047,7 +1039,7 @@ extern "C" int aa_logprob_bwd(const void *logits, int logits_dtype, int64_t row_
       case AA_F32: return launch_bwd_tma<float>(p, mode, rec, st);
     }
   }
-  if (row_scratch && (bwd_variant() % 10) == 2) {  // kernel digit 2: address-ordered chunked sweep (slower on B200, kept for study)
+  if (row_scratch && (bwd_variant() % 10) == 2) {  // kernel digit 2: address-ordered chunked sweep (an experiment, slower)
     AA_REQUIRE((reinterpret_cast<uintptr_t>(row_scratch) & 15) == 0, AA_ERR_ALIGN,
                "aa_logprob_bwd: row_scratch must be 16-byte aligned");
     RowRec *rec = static_cast<RowRec *>(row_scratch);

@@ -563,26 +563,17 @@ __global__ void __launch_bounds__(256) scale_tile_kernel(T *__restrict__ tile, i
 }
 
 // ---- host side ----------------------------------------------------------------------------
-// Shape of the persistent kernel (experiment switch AA_B200_FUSED_SHAPE, read once).  Measured on the C4 actor tile
-// (32 x 513 x 152064 bf16, 8695 scored rows; K1 -> K5 -> K1b: 1.72 ms), zero rows interleaved:
-//   6 (default): 992 consumers (31 warps + the producer warp = 1024 threads), 6 x 31 KB stages, lag 4, 1 CTA/SM: 1.41 ms
-//                (1.37 ms after call M: ring positions stepped by hand instead of a 64-bit `it % 6`, two stages per
-//                fold in phase A, F2FP rounding in phase B),
-//                DRAM reads 2.72 GB = the scored rows ONCE (the second pass hits L2), 4.93 GB written
-//   1: 512 consumers, 8 x 16 KB, lag 6, 1 CTA/SM: 1.44     4: 992 consumers, 8 x 15.5 KB, lag 6, 1 CTA/SM: 1.47
-//   0: 256 consumers, 8 x 8 KB, lag 6, 2 CTAs/SM: 1.59-1.62 (two rows in flight per SM: a third of the second pass
-//      misses L2, 3.5-4.1 GB read)     5: 480 consumers, 8 x 7.5 KB, 2 CTAs/SM: 1.61
-//   2: 256 consumers, 4 x 8 KB, lag 3, 3 CTAs/SM (K1b's shape): 1.70     3: 256 consumers, 8 x 16 KB, 1 CTA/SM: 1.91
-//   7: 736 consumers, 8 x 11.5 KB, 1 CTA/SM: 1.71 (before the interleaving)
-// One CTA per SM keeps 148 rows (45 MB) between the two passes; the kernel is bound by the MUFU / conversion pipe and
-// instruction issue (two exp per logit + the bf16 pack), not by HBM: ncu shows 47 % XU, IPC 2.5 at the 1.4 GHz the power
-// cap leaves.  AA_B200_FUSED_CTAS overrides the CTAs/SM, AA_B200_FUSED_HINT=0 drops the L2 policies (-10 % with two CTAs
-// per SM, +-0 with one), AA_B200_FUSED_INTERLEAVE=0 puts the zero rows after the scored rows (1.63 ms for shape 6).
-// LOST (profiles/r02_k1f_experiments.txt, call J): phase A straight from global memory as in K1 (LDG.128, no staging) plus
-// a dedicated warp writing the zero rows with st.global: 1.59 ms (30 consumer warps per SM do not hide the DRAM latency
-// of the LDG pass: IPC 2.0, and a fifth of the second pass misses L2) -- removed from the source.
-// ncu --set full of the default shape (profiles/r02_ncu_k1f_summary.md): DRAM 70 %, issue slots 65 % busy, FMA-heavy
-// pipe 57 %, XU 48 %; stalls: 21 % not selected, 18 % waiting for a chunk, 12 % math pipe, 10 % MIO.
+// Shape of the persistent kernel (experiment switch AA_B200_FUSED_SHAPE, read once), zero rows interleaved:
+//   6 (default): 992 consumers (31 warps + the producer warp = 1024 threads), 6 x 31 KB stages, lag 4, 1 CTA/SM
+//   1: 512 consumers, 8 x 16 KB, lag 6, 1 CTA/SM           4: 992 consumers, 8 x 15.5 KB, lag 6, 1 CTA/SM
+//   0: 256 consumers, 8 x 8 KB, lag 6, 2 CTAs/SM           5: 480 consumers, 8 x 7.5 KB, 2 CTAs/SM
+//   2: 256 consumers, 4 x 8 KB, lag 3, 3 CTAs/SM (K1b's shape)     3: 256 consumers, 8 x 16 KB, 1 CTA/SM
+//   7: 736 consumers, 8 x 11.5 KB, 1 CTA/SM
+// One CTA per SM keeps 132 rows (40 MB of 152064-token bf16 rows) between the two passes, inside the 50 MB L2, so the
+// second pass is an L2 hit; with two rows in flight per SM part of it misses.  The kernel is bound by the MUFU /
+// conversion pipe and instruction issue (two exp per logit + the bf16 pack) rather than by HBM.  AA_B200_FUSED_CTAS
+// overrides the CTAs/SM, AA_B200_FUSED_HINT=0 drops the L2 policies, AA_B200_FUSED_INTERLEAVE=0 puts the zero rows
+// after the scored rows.
 static int env_int(const char *name, int dflt) {
   const char *v = std::getenv(name);
   return (v && *v) ? std::atoi(v) : dflt;

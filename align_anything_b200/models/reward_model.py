@@ -1,4 +1,4 @@
-"""The scalar-head tail of the reference's reward / critic models on the sm_100a kernels (K3).
+"""The scalar-head tail of the reference's reward / critic models on the sm_90a kernels (K3).
 
 `ScoreModelOutput` has the fields of align_anything/models/reward_model.py:22-32.  The backbones
 (HF transformers) are untouched; only what follows `outputs.hidden_states[-1]` is replaced:

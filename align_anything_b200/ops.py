@@ -2,7 +2,7 @@
 
 Every function cites the reference function whose arithmetic it replaces (paths relative to
 the reference's align_anything/).  PyTorch is used for device memory, streams and autograd
-plumbing only; all arithmetic on the path runs in the hand-written sm_100a kernels.
+plumbing only; all arithmetic on the path runs in the hand-written sm_90a kernels.
 
 `mode`:
   'faithful' (default for 16-bit tensors) -- fp32 arithmetic, rounded to the tensor dtype at the
@@ -27,7 +27,7 @@ __all__ = [
 ]
 
 _REROUTE_TO_BASE = os.environ.get('AA_B200_REROUTE_BASE', '1') != '0'
-_K6B = os.environ.get('AA_B200_K6B', '1') != '0'  # 0: lm_head path with gradient through chunked cuBLAS + K1 / K1b instead of the tcgen05 kernels
+_K6B = os.environ.get('AA_B200_K6B', '1') != '0'  # 0: lm_head path with gradient through chunked cuBLAS + K1 / K1b instead of the tensor-core kernels
 _K6 = os.environ.get('AA_B200_K6', '1') != '0'  # 0: no-grad lm_head scoring through chunked cuBLAS + K1 instead of K6
 _ZERO_SPANS = os.environ.get('AA_B200_ZERO_SPANS', '1') != '0'  # 0: K1b zero-fills every unscored tile row itself
 _FUSED_ACTOR = os.environ.get('AA_B200_FUSED_ACTOR', '1') != '0'  # 0: the PPO actor node runs K1 -> K5 -> K1b instead of the single-pass K1f
@@ -36,9 +36,8 @@ _FUSED_ACTOR = os.environ.get('AA_B200_FUSED_ACTOR', '1') != '0'  # 0: the PPO a
 # small entries to fp16 underflow -- exactly what loss scaling is there to prevent.  bf16 / fp32 have the exponent range.
 _FUSED_F16 = os.environ.get('AA_B200_FUSED_F16', '0') == '1'
 # K1f keeps ONE row per SM in flight (that is what makes its second pass an L2 hit), so its per-row costs -- two block
-# reductions, the boundary thread, ring fill / drain -- weigh more the shorter the row is.  Measured on 32 x 513 x V bf16
-# actor tiles (profiles/r02_k1f_experiments.txt, call V): V = 32064: 0.83x of the two-pass path, 65536: 0.93x,
-# 128256: 1.15x, 152064: 1.25x.  Rows below this many bytes keep K1 -> loss kernel -> K1b.
+# reductions, the boundary thread, ring fill / drain -- weigh more the shorter the row is, and a short-vocabulary row
+# (32064 tokens) is faster on the two-pass path.  Rows below this many bytes keep K1 -> loss kernel -> K1b.
 _FUSED_MIN_ROW_BYTES = int(os.environ.get('AA_B200_FUSED_MIN_ROW_BYTES', str(192 * 1024)))
 _FUSED_GRPO = os.environ.get('AA_B200_FUSED_GRPO', '1') != '0'  # 0: the GRPO loss runs K1 -> loss kernel -> K1b instead of the single-pass K1f
 _FUSED_CE = os.environ.get('AA_B200_FUSED_CE', '1') != '0'  # 0: causal_lm_loss runs K1 -> mean NLL -> K1b instead of the single-pass K1f
@@ -444,8 +443,8 @@ def _mm_f32(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
 
 def _pad_vocab(weight: torch.Tensor):
     """Weight with the vocabulary padded (zero rows) to a 16-byte multiple of logits per row.  V = 128257 is odd: a
-    (rows, V) logits buffer then has 2-byte aligned rows, cuBLAS falls back to its unaligned kernels (measured
-    124 TFLOP/s instead of ~1400 on B200) and K1 / K1b lose their 16-byte fast paths."""
+    (rows, V) logits buffer then has 2-byte aligned rows, cuBLAS falls back to its unaligned kernels and K1 / K1b lose
+    their 16-byte fast paths."""
     V, H = weight.shape
     q = 16 // weight.element_size()
     Vp = (V + q - 1) // q * q
@@ -514,7 +513,7 @@ class _LinearLogProbFn(torch.autograd.Function):
 
 class _LinearLogProbK6Fn(torch.autograd.Function):
     """The tensor-core path (bf16, H % 64 == 0; default).  Forward = K6 (no logits at all, saves (max, logsum) per row).
-    Backward per row chunk = three tcgen05 kernels on one (chunk, ld) bf16 d(logits) buffer: K6b recomputes the logits
+    Backward per row chunk = three tensor-core (wgmma) kernels on one (chunk, ld) bf16 d(logits) buffer: K6b recomputes the logits
     tile and turns it into d(logits) in its epilogue; aa_linear_dhidden = d(logits) @ W with W consumed MN-major in
     place; aa_linear_dweight accumulates d(logits)^T @ hidden in fp32 across chunks and rounds once at the end.  No
     library GEMM, no padded / transposed copy of the weight."""
@@ -591,7 +590,7 @@ def linear_token_log_probs(hidden: torch.Tensor, weight: torch.Tensor, labels: t
 
 def fused_linear_token_log_probs(hidden: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor,
                                  mode: str | None = None, return_stats: bool = False):
-    """K6 (tcgen05): log_softmax(hidden @ weight.T)[label] per row in ONE kernel, no logits tile, for rows that
+    """K6 (wgmma): log_softmax(hidden @ weight.T)[label] per row in ONE kernel, no logits tile, for rows that
     carry NO gradient (reference model / rollout scoring).  hidden (N, H) bf16, weight (V, H) bf16, H % 64 == 0."""
     L.require_cuda(hidden, weight, labels)
     if hidden.dim() != 2 or weight.dim() != 2 or hidden.size(1) != weight.size(1) or labels.shape != hidden.shape[:1]:
@@ -605,7 +604,7 @@ def fused_linear_token_log_probs(hidden: torch.Tensor, weight: torch.Tensor, lab
     out = torch.empty(N, dtype=torch.bfloat16 if mode_code == L.MODE_FAITHFUL else torch.float32, device=hidden.device)
     stats = torch.empty((2, max(N, 1)), dtype=torch.float32, device=hidden.device) if return_stats else None
     sc = _device_scratch(hidden.device)
-    partial = torch.empty(3 * max(148 * 128, 16 * N), dtype=torch.float32, device=hidden.device)  # split-vocabulary statistics
+    partial = torch.empty(3 * max(132 * 128, 16 * N), dtype=torch.float32, device=hidden.device)  # split-vocabulary statistics
     L.check(L.lib().aa_linear_logprob_fwd(
         hidden.data_ptr(), N, hidden.size(1), hidden.stride(0), weight.data_ptr(), V, weight.stride(0), labels.data_ptr(),
         out.data_ptr(), L.dtype_code(out.dtype), L.ptr(stats[0]) if return_stats else None,
@@ -665,7 +664,7 @@ def _tails_from_hidden(hidden, weight, labels_padded, lens, counts, first_pos, l
     lab = labels_padded[:, lab_shift:lab_shift + W].reshape(-1).index_select(0, dst)
     needs_grad = torch.is_grad_enabled() and (hidden.requires_grad or weight.requires_grad)
     if not needs_grad and _K6 and hidden.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16 and H % 64 == 0:
-        lp = fused_linear_token_log_probs(rows, weight, lab, mode)  # K6: one tcgen05 kernel, no logits at all
+        lp = fused_linear_token_log_probs(rows, weight, lab, mode)  # K6: one tensor-core kernel, no logits at all
     else:
         lp = linear_token_log_probs(rows, weight, lab, chunk_rows, mode)
     return torch.zeros(n * W, dtype=lp.dtype, device=dev).index_copy(0, dst, lp).view(n, W)

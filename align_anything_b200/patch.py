@@ -1,4 +1,4 @@
-"""Graft the B200 hot path into an importable `align_anything` (the reference) in place:
+"""Graft the H100 hot path into an importable `align_anything` (the reference) in place:
 
     import align_anything_b200.patch as p; p.install()
 
@@ -159,7 +159,7 @@ def install(trainers: bool = True, models: bool = True) -> dict[str, list[str]]:
             elif modname in _PPO_TARGETS or modname in _GRPO_TARGETS:
                 _saved.append((cls, 'mode', cls.__dict__.get('mode', None)))
                 setattr(cls, 'mode', None)
-                if modname in _PPO_TARGETS:  # helpers the grafted rl_step calls + the B200-side entry points
+                if modname in _PPO_TARGETS:  # helpers the grafted rl_step calls + the H100-side entry points
                     helpers = ('_actor_logits', '_tail_log_probs', 'score_rollout', 'postprocess_generation')
                     if src is not _TextPPO:  # multimodal: the post-generate bookkeeping of actor_step is ours too
                         helpers += ('actor_step',)

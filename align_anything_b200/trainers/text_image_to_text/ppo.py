@@ -1,4 +1,4 @@
-"""Multimodal PPO rollout and rl_step on the B200 kernels -- mirror of
+"""Multimodal PPO rollout and rl_step on the H100 kernels -- mirror of
 align_anything/trainers/text_image_to_text/ppo.py (move_padding_left :56-87, actor_step :174-204,
 rollout :206-269, rl_step :271-379); the audio trainer (text_audio_to_text/ppo.py:217-277) runs the same
 arithmetic per micro-batch (`micro_batched_rollout`).
@@ -39,7 +39,7 @@ class PPOTrainer(_TextPPOTrainer):
     # first TypeError switches the option off); one that ignores it returns the whole tile, which works the same.
     tail_logits = True
     # Opt-in (SURVEY.md 8f rank 1): no logits tile at all.  The models are asked for their last hidden states
-    # (`output_hidden_states=True, logits_to_keep=1`); rollout scoring (no gradient) runs K6, one tcgen05 kernel per
+    # (`output_hidden_states=True, logits_to_keep=1`); rollout scoring (no gradient) runs K6, one tensor-core kernel per
     # model, the actor's rl_step K6 + K6b + the two backward GEMMs (ops.tail_log_probs_from_hidden).
     fused_lm_head = False
     lm_head_chunk_rows = None

@@ -1,4 +1,4 @@
-"""Safe RLHF-V (PPO-Lagrangian with a cost model) on the B200 kernels -- mirror of the loss half of
+"""Safe RLHF-V (PPO-Lagrangian with a cost model) on the H100 kernels -- mirror of the loss half of
 align_anything/trainers/text_image_to_text/saferlhf.py: actor_step :289-319, rollout :343-430,
 actor_loss_fn_with_cost :432-451, add_kl_divergence_regularization_with_cost :453-481, rl_step :483-675
 (get_advantages_and_returns :772-793 is the text trainer's).  `model.generate`, cost_model_step / reward_model_step

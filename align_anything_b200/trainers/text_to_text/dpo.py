@@ -1,4 +1,4 @@
-"""DPO loss / step on the B200 kernels -- mirror of align_anything/trainers/text_to_text/dpo.py
+"""DPO loss / step on the H100 kernels -- mirror of align_anything/trainers/text_to_text/dpo.py
 (DPOTrainer.compute_log_probs :122-142, .loss :144-203, .train_step :205-237).
 
 The methods read exactly what the reference's methods read from `self`:

@@ -1,4 +1,4 @@
-"""GRPO loss / step on the B200 kernels -- mirror of align_anything/trainers/text_to_text/grpo.py
+"""GRPO loss / step on the H100 kernels -- mirror of align_anything/trainers/text_to_text/grpo.py
 (GRPOTrainer._get_per_token_logps :199-210, the arithmetic of .train_step :268-318).  Generation
 (`generate_completions`) and reward computation (`compute_rewards`: a reward-model forward) are out of
 scope and stay in the reference; the methods below read self.actor_model, self.actor_reference_model,

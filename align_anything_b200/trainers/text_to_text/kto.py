@@ -1,4 +1,4 @@
-"""KTO loss on the B200 kernels -- mirror of align_anything/trainers/text_to_text/kto.py
+"""KTO loss on the H100 kernels -- mirror of align_anything/trainers/text_to_text/kto.py
 (KTOTrainer.loss :83-159, .train_step :161-192; compute_kl :49-81 calls compute_log_probs, i.e. K1).
 Reads self.cfgs.train_cfgs.{scale_coeff, scale_better, scale_worse} and self.kl."""
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""ORPO loss on the B200 kernels -- mirror of align_anything/trainers/text_to_text/orpo.py
+"""ORPO loss on the H100 kernels -- mirror of align_anything/trainers/text_to_text/orpo.py
 (ORPOTrainer.loss :41-113, .train_step :115-146).  Reads self.cfgs.train_cfgs.scale_coeff."""
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""PPO rollout scoring and rl_step on the B200 kernels -- mirror of
+"""PPO rollout scoring and rl_step on the H100 kernels -- mirror of
 align_anything/trainers/text_to_text/ppo.py (reward_model_step :224-242, rollout :244-289,
 actor_loss_fn :291-307, rl_step :309-398, get_advantages_and_returns :487-508, critic_loss_fn
 :510-526, add_kl_divergence_regularization :528-547).

@@ -1,4 +1,4 @@
-"""Reward-model training loss / step on the B200 kernels -- mirror of
+"""Reward-model training loss / step on the H100 kernels -- mirror of
 align_anything/trainers/text_to_text/rm.py (RMTrainer.loss :97-132, .train_step :133-152).  The model
 forward goes through the K3 score head (models.reward_model); the pairwise log-sigmoid loss, its
 regularisation term, the accuracy and the gradient w.r.t. the end scores come from one launch."""

@@ -1,4 +1,4 @@
-"""SFT loss / step on the B200 kernels -- mirror of align_anything/trainers/text_to_text/sft.py
+"""SFT loss / step on the H100 kernels -- mirror of align_anything/trainers/text_to_text/sft.py
 (SupervisedTrainer.loss :95-98, .train_step :100-109).  The reference takes `outputs.loss` from the HF
 model, which upcasts the whole logits tile to fp32 and materialises a (rows, V) log-softmax; here the
 model is called WITHOUT labels and the cross-entropy comes from K1 + the mean-NLL epilogue

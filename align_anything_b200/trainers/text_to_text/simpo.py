@@ -1,4 +1,4 @@
-"""SimPO loss on the B200 kernels -- mirror of align_anything/trainers/text_to_text/simpo.py
+"""SimPO loss on the H100 kernels -- mirror of align_anything/trainers/text_to_text/simpo.py
 (SimPOTrainer.loss :41-108, .train_step :110-141).  Reads self.cfgs.train_cfgs.{scale_coeff, gamma}."""
 from __future__ import annotations
 

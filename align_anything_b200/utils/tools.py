@@ -1,5 +1,5 @@
 """Same names and signatures as the hot-path helpers of align_anything/utils/tools.py; bodies run on
-the sm_100a kernels (align_anything_b200.ops)."""
+the sm_90a kernels (align_anything_b200.ops)."""
 from __future__ import annotations
 
 import torch

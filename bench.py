@@ -1,28 +1,34 @@
 #!/usr/bin/env python
-"""bench.py -- RLHF loss hot path on B200: preference-pairs/s (DPO) and scored rollout-tokens/s (PPO) on synthetic
+"""bench.py -- RLHF loss hot path on H100: preference-pairs/s (DPO) and scored rollout-tokens/s (PPO) on synthetic
 batches shaped like BASELINE.json's configs.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C2|C3|C4|C5]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
 
-    C2 (default, the headline): Llama-3-8B shapes text->text DPO, V = 128257, seq_len 2048, 32 pairs/step, bf16
+    C2 (default, the headline): Llama-3-8B shapes text->text DPO, V = 128257, seq_len 2048, 16 pairs/step, bf16
     C3: LLaVA-1.5-7B shapes text+image->text DPO, V = 32064, seq_len 2048, 576 image positions in the prompt
     C4: Qwen2-VL-7B shapes text+image->text PPO (actor + critic + RM), V = 152064, H = 3584, 512-token responses
-    C5: Qwen2-Audio-7B shapes text+audio->text DPO, V = 156032, seq_len 4096, 750 audio positions in the prompt
+    C5: Qwen2-Audio-7B shapes text+audio->text DPO, V = 156032, seq_len 4096, 4 pairs/step, 750 audio positions in the prompt
+    (per GPU, the policy and reference logits and the gradient tile of a step stay resident: C2 holds 50 GB of them,
+    C5 31 GB, so that each fits the 80 GB of an H100 next to the other buffers of the run)
     (C1, OPT-125M on CPU, is the reference's own plumbing case: tests/, not a bench line)
 
 One JSON line on rank 0 per invocation: `--config X` makes X the line's metric / value / e2e / roofline /
-cpu_baseline; the default C2 line also carries compact results of C3, C4 and C5 under `other_configs` (the driver
-runs the default command only) unless --no-other-configs.  A "step" = one pass of the loss path over one batch whose
+cpu_baseline; the default C2 line also carries compact results of C3, C4 and C5 under `other_configs` unless
+--no-other-configs.  A "step" = one pass of the loss path over one batch whose
 logits / hidden states are resident in HBM (model forwards, generation and the optimizer are third-party code outside
 the path, SURVEY.md section 8d):
   DPO step = label extraction + K1(policy) + K1(reference) + K2 + K1b (row prep + TMA-staged tile sweep) + packed all-reduce
   PPO step = rollout scoring (K3 x2, K1 x2) + rl_step (K4, K1, K5, K1b, K3 fwd/bwd, K5, pack, all-reduce)
 `value` times the path with CUDA events; `e2e` drives the public trainer API with the batch (input_ids, attention_mask /
 prompt + generated sequence) in pinned HOST memory copied to the device inside the timed region and the metrics read
-back to the host every step.  `--impl reference` times the reference's CPU path (the oracle port of it:
-/root/reference is absent on the GPU box) on the host cores, same `config` object.
+back to the host every step.  `--impl reference` times the reference's CPU path (the oracle port of it) on the host
+cores, same `config` object.
+
+`--dump-outputs DIR` writes, after the timed steps, what the headline path returned in its last timed step as
+DIR/<name>.npy (float32 / float64; a fixed, seeded sample of the gradient tile), so that two builds can be compared
+output for output: the inputs depend only on the arguments.
 """
 from __future__ import annotations
 
@@ -41,10 +47,10 @@ if ROOT not in sys.path:
 import torch  # noqa: E402
 
 CONFIGS = {
-    'C2': dict(kind='dpo', model='Llama-3-8B (vocab 128257 after <pad> resize)', modality='text', V=128257, L=2048, pairs=32,
+    'C2': dict(kind='dpo', model='Llama-3-8B (vocab 128257 after <pad> resize)', modality='text', V=128257, L=2048, pairs=16,
                modal=0, dense=True),
     'C3': dict(kind='dpo', model='LLaVA-1.5-7B', modality='image', V=32064, L=2048, pairs=32, modal=576, dense=False),
-    'C5': dict(kind='dpo', model='Qwen2-Audio-7B', modality='audio', V=156032, L=4096, pairs=8, modal=750, dense=False),
+    'C5': dict(kind='dpo', model='Qwen2-Audio-7B', modality='audio', V=156032, L=4096, pairs=4, modal=750, dense=False),
     'C4': dict(kind='ppo', model='Qwen2-VL-7B', modality='image', V=152064, H=3584, prompt_len=512, max_response=512,
                prompts_per_rank=32, pad=151643),
 }
@@ -70,6 +76,8 @@ def parse():
     ap.add_argument('--no-lm-head', action='store_true')
     ap.add_argument('--no-sft', action='store_true')
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', default='', metavar='DIR',
+                    help='write the outputs of the last timed step of the headline path to DIR/<name>.npy')
     ap.add_argument('--cpu-seconds', type=float, default=12.0, help='target CPU time of the cpu_baseline sample')
     ap.add_argument('--variant', type=int, default=-1, help='K1 variant override (aa_logprob_set_tuning)')
     ap.add_argument('--ctas-per-sm', type=int, default=0)
@@ -147,7 +155,7 @@ def sum_over_ranks(x: float, world) -> float:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
@@ -211,7 +219,27 @@ def peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return float(p['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs, copy bandwidth)'
-    return 6650.0, 'fallback (B200_PROFILING.md, 6.65 TB/s)'
+    return 3350.0, 'fallback (H100 SXM data sheet, 3.35 TB/s)'
+
+
+def seeded_sample(t, n=1 << 22, seed=0):
+    """n elements of `t` at fixed pseudo-random positions (the same for the same shape), in index order."""
+    flat = t.reshape(-1)
+    if flat.numel() <= n:
+        return flat
+    idx = torch.randint(0, flat.numel(), (n,), generator=torch.Generator().manual_seed(seed)).sort().values
+    return flat[idx.to(flat.device)]
+
+
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: one DIR/<name>.npy per array, float64 arrays as float64 and everything else as float32."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        t = torch.as_tensor(a).detach()
+        t = t.double() if t.dtype == torch.float64 else t.float()
+        np.save(os.path.join(out_dir, f'{name}.npy'), t.cpu().numpy())
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -370,11 +398,14 @@ def dpo_bench(args, c, rank, world, device, extras=True):
         torch.cuda.synchronize()
         t0.record()
         for k in range(args.steps):
-            step(k)
+            last = step(k)
         t1.record()
         torch.cuda.synchronize()
         barrier(world)
         clocks = sampler.stop() if (variant == main and rank == 0) else None
+        if variant == main and extras and rank == 0 and args.dump_outputs:
+            dump_outputs(args.dump_outputs, {'dpo_packed_metrics': last, 'dpo_log_probs': lp, 'dpo_row_stats': stat,
+                                             'dpo_grad_logits_sample': seeded_sample(grad)})
         ms = max_over_ranks(t0.elapsed_time(t1), world) / args.steps
         fwd_ms = statistics.mean((e[0].elapsed_time(e[1]) + e[1].elapsed_time(e[2])) / 2 for e in ev)
         k2_ms = statistics.mean(e[2].elapsed_time(e[3]) for e in ev)
@@ -476,7 +507,7 @@ def eager_gpu_dpo(policy, ref, ids, lens, B, pad, strip=True, skip=False, sample
 def lm_head_bench(args, c, device, pairs=4, H=4096):
     """SURVEY.md 8f rank 1: lm_head x log-prob with and without the (rows, V) logits tile, on a reduced C2 batch
     (`pairs` pairs, dense): forward + backward of sum(log-probs) down to hidden states and the lm_head weight
-    (`fused`: K6 forward, K6b + aa_linear_dhidden + aa_linear_dweight backward -- all tcgen05, no library GEMM), the
+    (`fused`: K6 forward, K6b + aa_linear_dhidden + aa_linear_dweight backward -- all wgmma, no library GEMM), the
     no-gradient scoring path (K6 alone), and `dpo_fused_lm_head`: DPOTrainer(fused_lm_head=True).train_step end to end
     with the batch in pinned host memory."""
     from types import SimpleNamespace
@@ -519,7 +550,7 @@ def lm_head_bench(args, c, device, pairs=4, H=4096):
     rows = sum(r - 1 for r in lens)
     flops = 2 * rows * H * V
     out['fused']['tflops_over_4_gemm_passes'] = 4 * flops / out['fused']['ms'] / 1e9
-    out['fused']['path'] = 'K6 fwd; K6b + aa_linear_dhidden + aa_linear_dweight bwd (tcgen05, no library GEMM)' if ops._K6B else 'chunked cuBLAS + K1/K1b'
+    out['fused']['path'] = 'K6 fwd; K6b + aa_linear_dhidden + aa_linear_dweight bwd (wgmma, no library GEMM)' if ops._K6B else 'chunked cuBLAS + K1/K1b'
 
     def timed(fn, reps=3):
         fn()
@@ -532,7 +563,7 @@ def lm_head_bench(args, c, device, pairs=4, H=4096):
         torch.cuda.synchronize()
         return t0.elapsed_time(t1) / reps
 
-    # reference-model / rollout scoring (no gradient): K6 (one tcgen05 kernel) vs cuBLAS logits + K1
+    # reference-model / rollout scoring (no gradient): K6 (one wgmma kernel) vs cuBLAS logits + K1
     with torch.no_grad():
         ms_k6 = timed(lambda: ops.sequence_log_probs_from_hidden(hidden, weight, ids, lens, pad))
         ms_lib = timed(lambda: ops.sequence_log_probs(torch.nn.functional.linear(hidden, weight), ids, lens, pad))
@@ -545,7 +576,7 @@ def lm_head_bench(args, c, device, pairs=4, H=4096):
         'roofline': {'bound': 'tensor', 'achieved': flops / ms_k6 / 1e9, 'peak': tpeak, 'unit': 'TFLOP/s',
                      'frac': (flops / ms_k6 / 1e9 / tpeak) if tpeak else None,
                      'traffic': tr_k6[0] * (rows * H * 2 + V * H * 2) if tr_k6[0] else None, 'traffic_source': tr_k6[1],
-                     'kernel': 'linear_logprob_kernel<false> (K6: TMA + tcgen05.mma + LSE epilogue from TMEM)',
+                     'kernel': 'linear_logprob_kernel<false> (K6: TMA + wgmma + LSE epilogue on the accumulator registers)',
                      'peak_source': 'measured (MEASURED_PEAKS.json bf16_tflops: cuBLAS 8192^3 burst; kernel timed alone)',
                      'peak_sustained': tpeak_sustained,
                      'note': 'K6 time includes the row gather / scatter glue of sequence_log_probs_from_hidden'}}
@@ -592,7 +623,7 @@ def lm_head_bench(args, c, device, pairs=4, H=4096):
         'roofline': {'bound': 'tensor', 'achieved': gemm_flops / e2e_ms / 1e9, 'peak': tpeak_sustained, 'unit': 'TFLOP/s',
                      'frac': (gemm_flops / e2e_ms / 1e9 / tpeak_sustained) if tpeak_sustained else None, 'traffic': None,
                      'note': '5 GEMM passes of 2*rows*H*V flops per step (policy forward / recompute / d hidden / d weight + reference '
-                             'forward), all on hand-written tcgen05 kernels; peak = sustained cuBLAS bf16 (a long step)'},
+                             'forward), all on hand-written wgmma kernels; peak = sustained cuBLAS bf16 (a long step)'},
         'loss': m['train/loss']}
     out['config'] = {'pairs': pairs, 'rows': rows, 'H': H, 'V': V, 'gemm_tflop_per_pass': flops / 1e12,
                      'note': 'forward + backward to d(hidden), d(weight); the fused path runs 4 GEMM passes (forward, '
@@ -689,9 +720,10 @@ def ppo_port_step(O, actor, refl, critic_h, rm_h, w_c, w_r, seq, prompt, pad, le
     return out
 
 
-def ppo_bench(args, rank, world, device, tail=None):
+def ppo_bench(args, rank, world, device, tail=None, dump=False):
     """BASELINE configs[3].  tail: None = the trainer's default (`PPOTrainer.tail_logits`), True / False force the
-    tail tile (actor / reference asked for the last max(R)+1 positions only, HF `logits_to_keep`) or the full tile."""
+    tail tile (actor / reference asked for the last max(R)+1 positions only, HF `logits_to_keep`) or the full tile.
+    dump: write the last timed step's metrics for --dump-outputs."""
     from types import SimpleNamespace
 
     from align_anything_b200.models.reward_model import score_model_outputs
@@ -755,6 +787,9 @@ def ppo_bench(args, rank, world, device, tail=None):
         torch.cuda.synchronize()
         w1 = time.perf_counter()
         barrier(world)
+        if not e2e and dump and rank == 0:  # the timed path of the C4 line: rl_step's metrics of the last step
+            names = sorted(k for k, v in metrics.items() if isinstance(v, (int, float, torch.Tensor)))
+            dump_outputs(args.dump_outputs, {'ppo_metrics': torch.tensor([float(metrics[k]) for k in names], dtype=torch.float64)})
         ms_dev = max_over_ranks(t0.elapsed_time(t1), world) / args.steps
         ms_wall = max_over_ranks((w1 - w0) * 1e3, world) / args.steps
         out[label] = (ms_dev, ms_wall)
@@ -882,8 +917,8 @@ def cpu_ppo_tokens_per_s(target_s, threads):
 
 
 def reference_arm(args):
-    """--impl reference: the reference's own CPU implementation of the path.  /root/reference is not on the GPU box and
-    the reference is pure Python on torch, so this runs the oracle port of it (oracle/ref_port.py, pinned bit-exactly on
+    """--impl reference: the reference's own CPU implementation of the path.  The reference is pure Python on torch,
+    so this runs the oracle port of it (oracle/ref_port.py, pinned bit-exactly on
     the reference's outputs) on the host cores.  Each step = one bounded sample; same `config` object as our arm."""
     rank = int(os.environ.get('RANK', '0'))
     if rank != 0:
@@ -941,7 +976,7 @@ def dpo_line(args, name, c, dpo, world, cpu):
         'vs_baseline': None, 'dtype': 'bf16', 'data': 'synthetic',
         'config': config_object(name, c, world),
         'details': {'pairs_per_rank': dpo['B'], 'scored_rows_per_rank': d['rows_per_rank'],
-                    'l2': 'inputs (2 x %.1f GB logits tiles per rank) are far larger than the 126 MB L2; no flush needed'
+                    'l2': 'inputs (2 x %.1f GB logits tiles per rank) are far larger than the 50 MB L2; no flush needed'
                           % (2 * dpo['B'] * c['L'] * V * 2 / 1e9),
                     'rounding': 'faithful (reference bf16 rounding points)', 'collective': dpo['collective'],
                     'allreduce_check': dpo.get('allreduce_check')},
@@ -953,8 +988,8 @@ def dpo_line(args, name, c, dpo, world, cpu):
         'roofline': {'bound': 'hbm', 'achieved': d['fwd_gbs'], 'peak': hbm_peak, 'unit': 'GB/s', 'frac': d['fwd_gbs'] / hbm_peak,
                      'traffic': (t_f[0] * d['rows_per_rank'] * V * 2) if t_f[0] else None, 'traffic_source': t_f[1],
                      'kernel': 'logprob_fwd_kernel (K1)', 'peak_source': peak_src,
-                     'bytes_per_launch': d['rows_per_rank'] * V * 2, 'launch_ms': d['fwd_ms'], 'peak_nominal': 8000.0,
-                     'frac_of_nominal': d['fwd_gbs'] / 8000.0},
+                     'bytes_per_launch': d['rows_per_rank'] * V * 2, 'launch_ms': d['fwd_ms'], 'peak_nominal': 3350.0,
+                     'frac_of_nominal': d['fwd_gbs'] / 3350.0},
         'roofline_bwd': {'bound': 'hbm', 'achieved': d['bwd_gbs'], 'peak': hbm_peak, 'unit': 'GB/s',
                          'frac': d['bwd_gbs'] / hbm_peak, 'kernel': 'logprob_bwd_tma_kernel (K1b)', 'launch_ms': d['bwd_ms'],
                          'bytes_per_launch': 2 * d['rows_per_rank'] * V * 2,
@@ -988,7 +1023,7 @@ def main():
         reference_arm(args)
         return
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py --impl ours needs a B200: the product path has no CPU fallback')
+        raise SystemExit('bench.py --impl ours needs an H100: the product path has no CPU fallback')
     rank, world, local = init_dist(args.gpus)
     device = torch.device('cuda', local)
     from align_anything_b200 import _lib as Lb
@@ -1015,7 +1050,7 @@ def main():
         return {'value': v, 'unit': 'tokens/s', 'cores': cpu_ppo_tokens_per_s.threads_used, 'kind': 'port', 'sample': sample}
 
     def run_ppo(full):
-        ppo = ppo_bench(args, rank, world, device)
+        ppo = ppo_bench(args, rank, world, device, dump=bool(args.dump_outputs) and args.config == 'C4')
         torch.cuda.empty_cache()
         if full:
             other = ppo_bench(args, rank, world, device, tail=not ppo['config']['tail_logits'])

@@ -1,5 +1,5 @@
 /*
- * aa_b200.h -- C ABI of libaa_b200.so: the B200 (sm_100a) implementation of
+ * aa_b200.h -- C ABI of libaa_b200.so: the H100 (sm_90a) implementation of
  * align-anything's RLHF loss hot path.
  *
  * The reference (PKU-Alignment/align-anything) has NO FFI layer for this path:
@@ -122,7 +122,7 @@ int aa_logprob_fwd(const void *logits, int logits_dtype, int64_t row_stride, int
  * at grad_logits + seg_tile_row[s]*grad_row_stride, followed by the `n_extra_zero_rows` tile rows
  * listed in `extra_zero_rows` (device, int64), which are zero-filled.  A caller that knows the row
  * layout on the host uses this form together with aa_zero_rows: long zero spans go to the copy
- * engine (cudaMemsetAsync: 7.4 TB/s on B200 vs 6.45 TB/s for stores issued by a kernel), isolated
+ * engine (cudaMemsetAsync, faster than stores issued by a kernel), isolated
  * zero rows are listed, and the kernel's static row stride sees equally expensive rows first.
  * FAITHFUL mode recomputes softmax_j as exp(round_dtype((x_j - max) - logsum)), which is what
  * the reference's backward sees (it re-reads the ROUNDED log-softmax output).
@@ -415,12 +415,12 @@ int aa_allreduce_packed(const float *src, float *dst, int32_t n, const aa_coll *
  * nn.Linear lm_head; callers trainers/text_to_text/dpo.py:128 (reference model), ppo.py:266-267 (rollout))
  * without the (n_rows, V) logits tile.  hidden (n_rows, H) and weight (V, H) are bf16, K-major, rows
  * 16-byte aligned (strides in elements, multiples of 8), H a multiple of 64; V is arbitrary (128257 works:
- * the odd leading dimension only exists in the tile that is never written).  tcgen05.mma (M128 N256 K16,
- * fp32 accumulators in TMEM), operands staged by TMA into a 4-stage 128-byte-swizzled ring, epilogue =
- * online (max, sum-exp) + label pick straight out of TMEM.  FAITHFUL: each logit is rounded to bf16 before
+ * the odd leading dimension only exists in the tile that is never written).  wgmma (m64n256k16 per warpgroup,
+ * fp32 accumulators in registers), operands staged by TMA into a 4-stage 128-byte-swizzled ring, epilogue =
+ * online (max, sum-exp) + label pick on the accumulator registers.  FAITHFUL: each logit is rounded to bf16 before
  * the softmax (the rounding point of nn.Linear) and the result is rounded to bf16.  stat_max / stat_logsum
  * (optional, n_rows fp32 each) receive the row statistics.  `partial` (optional, `partial_floats` fp32 of
- * device scratch; 3 * 148 * 128 always suffices): with fewer 128-row tiles than SMs the vocabulary is also
+ * device scratch; 3 * 132 * 128 always suffices on a 132-SM H100): with fewer 128-row tiles than SMs the vocabulary is also
  * split across CTAs and the per-split (max, sum, label logit) are merged by a second tiny launch.  Needs a driver that exports
  * cuTensorMapEncodeTiled (resolved at run time; the library does not link libcuda).
  * Work: 2 * n_rows * H * V flops; HBM: weight + hidden read ~once (the weight sweep stays in L2).
@@ -442,8 +442,8 @@ int aa_linear_dlogits(const void *hidden, int64_t n_rows, int32_t H, int64_t hid
                       int grad_rows_dtype, void *dlogits, int64_t ld, int mode, void *stream);
 
 /* The two GEMMs that finish that backward: the autograd of the model's nn.Linear lm_head (callers
- * trainers/text_to_text/dpo.py:128, ppo.py:338) given the d(logits) buffer of aa_linear_dlogits.  Same tcgen05 / TMEM / TMA
- * pipeline as K6 (M128 N256 K16, fp32 accumulation), persistent grid, operands read in place:
+ * trainers/text_to_text/dpo.py:128, ppo.py:338) given the d(logits) buffer of aa_linear_dlogits.  Same wgmma / TMA
+ * pipeline as K6 (128 x 256 tiles, fp32 accumulation), persistent grid, operands read in place:
  *   aa_linear_dhidden:  d_hidden (n_rows, H) bf16 = dlogits (n_rows, ld) . weight (V, H)       [columns >= V of dlogits
  *                       must be zero; the weight is consumed MN-major, vocabulary rows >= V are zero-filled by TMA]
  *   aa_linear_dweight:  (V, H) result = [acc_f32 if accumulate] + dlogits^T . hidden (n_rows, H), both operands MN-major.

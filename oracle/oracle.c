@@ -4,7 +4,7 @@
  * RLHF loss path, independent of PyTorch.  Used by tests/ to cross-check oracle/ref_port.py (which
  * is pinned bit-exactly on the reference's golden vectors) and, through it, the CUDA kernels.
  * Only tests/, __graft_entry__ and bench.py's CPU legs may load this; the product never does.
- * Paths below are relative to /root/reference/align_anything/.
+ * Paths below are relative to the reference's align_anything/ directory.
  */
 #include <math.h>
 #include <stdint.h>

@@ -5,13 +5,12 @@ on CPU) of the reference's RLHF loss hot path.  The reference defines its
 results as "whatever these ATen ops return in the input dtype" -- including the
 bf16 rounding points -- so the restatement uses the same ops in the same order
 and dtype, one function per reference function, each citing the reference
-file:line it follows (paths relative to /root/reference/align_anything/).
+file:line it follows (paths relative to the reference's align_anything/ directory).
 
-Pinned: `tests/test_oracle_vs_reference.py` runs every function here against
-the *unmodified* reference (imported through oracle/ref_shim.py) whenever
-/root/reference is present, and `tests/golden/*.pt` (generated from the
-reference by tests/golden/make_golden.py) pin it on the GPU box where the
-reference is absent.
+Pinned: `tests/golden/*.pt`, generated from the *unmodified* reference by
+tests/golden/make_golden.py (through oracle/ref_shim.py), hold the reference's
+outputs; `tests/test_oracle_golden.py` and `tests/test_oracle_vs_reference.py`
+compare every function here against them.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl
 reference legs may import this module.  Nothing under align_anything_b200/
@@ -440,7 +439,7 @@ def ppo_mm_rl_step(
 # --------------------------------------------------------------------------------------
 # f4 -- the `outputs.loss` consumed by SupervisedTrainer.loss (trainers/text_to_text/sft.py:95-98) and
 #       PPOTrainer.ptx_step (trainers/text_to_text/ppo.py:400-408).  The arithmetic lives in a third-party
-#       dependency that is NOT under /root/reference: transformers (pyproject.toml:37 pins ">=4.50.0";
+#       dependency that is NOT part of the reference: transformers (pyproject.toml:37 pins ">=4.50.0";
 #       installed here 5.5.0), `transformers.loss.loss_utils.ForCausalLMLoss`: logits upcast to fp32,
 #       labels padded with ignore_index and shifted by one, mean cross-entropy over labels != ignore_index.
 #       Pinned by tests/golden/sft.pt (a tiny LlamaForCausalLM run through the real HF forward).

@@ -1,11 +1,10 @@
 """TEST INFRASTRUCTURE ONLY -- bootstrap that imports the *unmodified* reference
-(PKU-Alignment/align-anything, mounted read-only at /root/reference) in the
-authoring container so that the oracle port (oracle/ref_port.py) can be pinned
-against the reference's own functions and golden vectors can be generated
+(a checkout of PKU-Alignment/align-anything named by AA_REFERENCE_ROOT) so that
+golden vectors of the reference's own functions can be generated
 (tests/golden/make_golden.py).
 
-/root/reference does NOT exist on the GPU box: nothing under `-m gpu` tests,
-`__graft_entry__.smoke()` or `bench.py` imports this module.  It touches no
+Nothing in tests/, `__graft_entry__.smoke()` or `bench.py` imports this module:
+they read the stored golden vectors instead.  It touches no
 reference file; it only arranges `sys.modules` so that the reference's heavy
 optional dependencies (deepspeed, accelerate, peft, diffusers, librosa, ray,
 bitsandbytes) resolve to permissive stubs -- none of them is on the arithmetic
@@ -20,13 +19,13 @@ import types
 from types import SimpleNamespace
 from unittest.mock import MagicMock
 
-REF = os.environ.get('AA_REFERENCE_ROOT', '/root/reference')
+REF = os.environ.get('AA_REFERENCE_ROOT', '')
 
 _installed = False
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(REF, 'align_anything'))
+    return bool(REF) and os.path.isdir(os.path.join(REF, 'align_anything'))
 
 
 class _Stub(types.ModuleType):

@@ -1,4 +1,5 @@
-"""pytest config: `gpu` marker (tests needing a B200) + shared helpers."""
+"""pytest config: `gpu` marker (tests needing an H100) + shared helpers."""
+import glob
 import os
 import sys
 
@@ -10,15 +11,30 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box via gpurun)')
-    config.addinivalue_line('markers', 'reference: needs /root/reference (authoring container only)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100)')
 
 
 @pytest.fixture(scope='session')
 def golden():
     import torch
 
+    def merge(dst, src):
+        for k, v in src.items():
+            if isinstance(v, dict) and isinstance(dst.get(k), dict):
+                merge(dst[k], v)
+            else:
+                dst[k] = v
+
     def load(name):
-        return torch.load(os.path.join(ROOT, 'tests', 'golden', f'{name}.pt'), weights_only=False)
+        path = os.path.join(ROOT, 'tests', 'golden', f'{name}.pt')
+        if os.path.exists(path):
+            return torch.load(path, weights_only=False)
+        # stored as parts of < 1 MB each (tests/golden/make_golden.py `save`)
+        parts = glob.glob(os.path.join(ROOT, 'tests', 'golden', f'{name}.[0-9]*.pt'))
+        assert parts, f'no golden {name}'
+        data = {}
+        for part in sorted(parts, key=lambda p: int(p.rsplit('.', 2)[1])):
+            merge(data, torch.load(part, weights_only=False))
+        return data
 
     return load

@@ -1,5 +1,5 @@
-"""TEST INFRASTRUCTURE ONLY -- a stand-in `align_anything` module tree for the GPU box, where /root/reference does
-not exist.  It has the reference's module paths, class names and method names for the PPO recipes, with
+"""TEST INFRASTRUCTURE ONLY -- a stand-in `align_anything` module tree, so that the graft can be tested without the
+reference's sources.  It has the reference's module paths, class names and method names for the PPO recipes, with
 
   * the methods `align_anything_b200.patch.install()` is expected to REPLACE written as `raise AssertionError` bodies
     (so a test that runs the loop proves the graft took), and

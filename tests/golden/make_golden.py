@@ -1,14 +1,16 @@
-"""Generate tests/golden/*.pt by running the UNMODIFIED reference (/root/reference, imported
-through oracle/ref_shim.py) on small seeded inputs.  Run in the authoring container only:
+"""Generate tests/golden/*.pt by running the UNMODIFIED reference (a checkout of PKU-Alignment/align-anything named
+by AA_REFERENCE_ROOT, imported through oracle/ref_shim.py) on small seeded inputs:
 
-    python tests/golden/make_golden.py
+    AA_REFERENCE_ROOT=<checkout> python tests/golden/make_golden.py [name ...]
 
 The fixtures hold inputs AND the reference's outputs, so the oracle port and the CUDA path
-can be checked on the GPU box where /root/reference does not exist.  Sizes are tiny (odd
+can be checked without the reference.  A fixture larger than 1 MB is stored as parts
+<name>.<i>.pt that tests/conftest.py merges back.  Sizes are tiny (odd
 vocab 1031 to exercise the unaligned-row path; bf16 and fp32 variants).
 """
 from __future__ import annotations
 
+import glob
 import os
 import sys
 from types import SimpleNamespace
@@ -473,20 +475,98 @@ def golden_grpo(gen):
     return out
 
 
+def golden_reference_ports(gen):
+    """The reference's outputs on the seeded inputs of tests/test_oracle_vs_reference.py (which rebuilds the inputs)."""
+    sys.path.insert(0, os.path.join(ROOT, 'tests'))
+    import test_oracle_vs_reference as T
+
+    ref_shim.install()
+    out = {'dpo': {}, 'ppo': {}}
+    for dtype in (torch.bfloat16, torch.float32):
+        for seed in range(4):
+            pol, ref, ids, lens, pad = T.dpo_case(seed, dtype)
+            case = {}
+            for modality in T.MODALITIES:
+                leaf = pol.clone().requires_grad_(True)
+                tr = ref_shim.make_dpo_trainer(leaf, ref, pad, 0.1, modality)
+                want = tr.loss({'input_ids': ids, 'attention_mask': ids != pad, 'meta_info': {'response_lens': lens}})
+                want['loss'].backward()
+                case[modality] = {'loss': {k: v.detach() for k, v in want.items()}, 'grad': leaf.grad}
+            out['dpo'][f'{T.DTYPE_NAMES[dtype]}_{seed}'] = case
+    for seed in range(3):
+        cases = {}
+        for dtype, vdtype, modality, x in T.ppo_cases(seed):
+            p, s, mask = ref_shim.make_ppo_trainer(modality=modality), x['start'], x['mask']
+            r1 = p.add_kl_divergence_regularization(x['reward'], x['lp'], x['rlp'], mask)
+            a1, t1 = p.get_advantages_and_returns(x['vals'], r1, mask, s)
+            cases[f'{T.DTYPE_NAMES[dtype]}_{T.DTYPE_NAMES[vdtype]}_{modality}'] = dict(
+                rewards=r1, advantages=a1, returns=t1,
+                actor_loss=p.actor_loss_fn(x['nlp'][:, s:], x['lp'][:, s:], a1, mask[:, s:]),
+                critic_loss=p.critic_loss_fn(x['nv'][:, s:], x['vals'][:, s:], t1, mask[:, s:]))
+        out['ppo'][seed] = cases
+    out['layout'] = ref_shim.tools().move_padding_left(T.layout_case(), 0)
+    return out
+
+
+PART_BYTES = 900 * 1024  # every stored file stays under 1 MB
+
+
+def _leaves(d, path=()):
+    if isinstance(d, dict) and d:
+        for k, v in d.items():
+            yield from _leaves(v, path + (k,))
+    else:
+        yield path, d
+
+
+def _nbytes(v):
+    if torch.is_tensor(v):
+        return v.numel() * v.element_size()
+    if isinstance(v, (list, tuple)):
+        return sum(_nbytes(x) for x in v)
+    if isinstance(v, dict):
+        return sum(_nbytes(x) for x in v.values())
+    return 64
+
+
+def save(name, data):
+    """<name>.pt, or -- above PART_BYTES -- parts <name>.0.pt, <name>.1.pt, ... each holding a disjoint set of the
+    nested dict's leaves (tensors are cloned, so that a view does not drag its whole storage into the file)."""
+    for old in glob.glob(os.path.join(OUT, f'{name}.pt')) + glob.glob(os.path.join(OUT, f'{name}.[0-9]*.pt')):
+        os.remove(old)
+    parts, cur, size = [], {}, 0
+    for path, v in _leaves(data):
+        n = _nbytes(v)
+        if cur and size + n > PART_BYTES:
+            parts.append(cur)
+            cur, size = {}, 0
+        d = cur
+        for k in path[:-1]:
+            d = d.setdefault(k, {})
+        d[path[-1]] = v.clone() if torch.is_tensor(v) else v
+        size += n
+    parts.append(cur)
+    paths = [os.path.join(OUT, f'{name}.pt')] if len(parts) == 1 else [os.path.join(OUT, f'{name}.{i}.pt') for i in range(len(parts))]
+    for part, path in zip(parts, paths):
+        torch.save(part, path)
+        assert os.path.getsize(path) < 1 << 20, (path, os.path.getsize(path))
+    return paths
+
+
 def main():
     gen = torch.Generator().manual_seed(20260922)
     only = sys.argv[1:]
     parts = {
         'logprob': golden_logprob, 'dpo': golden_dpo, 'ppo': golden_ppo, 'ppo_step': golden_ppo_step,
         'layout': golden_layout, 'score_head': golden_score_head, 'score_head_mm': golden_score_head_mm, 'sft': golden_sft, 'grpo': golden_grpo, 'pairwise': golden_pairwise, 'saferlhf': golden_saferlhf,
+        'reference_ports': golden_reference_ports,
     }
     for name, fn in parts.items():
         if only and name not in only:
             continue
         data = fn(gen)
-        path = os.path.join(OUT, f'{name}.pt')
-        torch.save(data, path)
-        print(name, os.path.getsize(path) // 1024, 'KiB', [k for k in data])
+        paths = save(name, data)
+        print(name, sum(os.path.getsize(p) for p in paths) // 1024, 'KiB in', len(paths), 'file(s)', [k for k in data])
 
 
 if __name__ == '__main__':

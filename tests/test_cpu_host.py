@@ -121,10 +121,10 @@ def test_library_exports_every_declared_symbol():
     assert declared == set(_lib.EXPORTED_SYMBOLS), declared ^ set(_lib.EXPORTED_SYMBOLS)
     m = re.search(r"#define AA_B200_ABI_VERSION (\d+)", header)
     assert handle.aa_abi_version() == int(m.group(1)) == 3
-    # only sm_100a code in the binary
+    # only sm_90a code in the binary
     r = subprocess.run(['cuobjdump', '-lelf', path], capture_output=True, text=True)
     if r.returncode == 0 and r.stdout.strip():
-        assert 'sm_100a' in r.stdout and not re.search(r'sm_(?!100a)\d+', r.stdout), r.stdout
+        assert 'sm_90a' in r.stdout and not re.search(r'sm_(?!90a)\d+', r.stdout), r.stdout
 
 
 def test_argument_errors_need_no_gpu():

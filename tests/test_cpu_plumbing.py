@@ -3,7 +3,7 @@ a stand-in that validates every call against the declared ctypes signature (argu
 kinds) and returns 0, `require_cuda` is disabled and `torch.empty` zero-fills, so every trainer path can be driven end
 to end on CPU tensors.  What this pins: the host logic -- argument marshalling for every entry point on the DPO / PPO /
 lm_head paths, autograd wiring of the fused nodes, the graft (patch.install on a reference-shaped tree), dict keys,
-scalar-only metric dicts -- i.e. everything that would otherwise only fail on the GPU box."""
+scalar-only metric dicts -- i.e. everything that would otherwise only fail on the GPU."""
 import ctypes
 import math
 import sys

@@ -1,5 +1,5 @@
 """Drop-in test of the graft under the reference's own `train()` loop (VERDICT r1, task 1): `patch.install()` on a
-reference-shaped module tree (tests/fake_reference_tree.py; /root/reference does not exist on the GPU box), then
+reference-shaped module tree (tests/fake_reference_tree.py: the reference's sources are not needed), then
 `train()` = rollout -> rl_step -> Logger.log per micro-batch with fake engines and a fake `generate`.  What is
 asserted: the grafted `rollout` / `actor_step` / `rl_step` are ours, the text trainer's `actor_step` and every
 `reward_model_step` stay the tree's own, every value that reaches the tensorboard-style writer is a Python scalar,

@@ -1,5 +1,5 @@
-"""Multi-GPU tests (need >= 2 CUDA devices: `gpurun --gpus 2 -- python -m pytest tests/test_gpu_multi.py -m gpu`;
-skipped on the single-GPU box the driver uses)."""
+"""Multi-GPU tests (need >= 2 CUDA devices: `python -m pytest tests/test_gpu_multi.py -m gpu` on a machine with two or
+more GPUs; skipped on a single GPU)."""
 import os
 import subprocess
 import sys
