@@ -62,7 +62,7 @@ __host__ __device__ __forceinline__ int64_t bwd_work_rows(const BwdParams &p) {
   return p.n_tile_rows > 0 ? p.n_tile_rows : p.n_rows + p.n_extra;
 }
 
-// ---- K1 forward, variant 0: direct vectorised LDG ---------------------------------------
+// ---- K1 forward, LDG: direct vectorised loads (rows of 128 KB and more, see launch_fwd) -------------
 template <typename T, int THREADS, int UNROLL>
 __global__ void __launch_bounds__(THREADS) logprob_fwd_kernel(const FwdParams p) {
   constexpr int E = Traits<T>::kVec;
@@ -142,98 +142,144 @@ __global__ void __launch_bounds__(THREADS) logprob_fwd_kernel(const FwdParams p)
   }
 }
 
-// ---- K1 forward, variant 1: TMA engine (cp.async.bulk, 1-D) staged through shared memory ------------
-// One producer lane streams the 16-byte-aligned body of each row into a ring of shared-memory stages
-// with cp.async.bulk (SASS: UBLKCP), completion signalled on mbarriers; eight consumer warps read
-// the stages with conflict-free LDS.128 and run the same online softmax.  The ring runs across row
-// boundaries, so the copy engine is already fetching the next row while the consumers reduce the
-// current one.  Tensor maps are not needed (and could not describe V = 128257 anyway: a TMA tensor map
-// wants 16-byte row strides); the 1-D bulk copy only needs the 16-byte-aligned body that the head /
-// tail peel already isolates.
+// ---- K1 forward, default: rows streamed through a cp.async.bulk ring ---------------------------------
+// One producer lane walks the CTA's rows and owns everything that needs a dependent global load: segment
+// lookup, logits pointer, label, ignore_index test.  Ignored rows it writes itself (output 0, no traffic);
+// for every other row it hands a descriptor to the consumers through a small shared-memory queue and
+// streams the row's 16-byte-aligned body into a ring of shared-memory stages with cp.async.bulk (SASS:
+// UBLKCP), completion signalled on mbarriers.  The ring runs across row boundaries, so the copy engine is
+// already fetching the next row while the consumers reduce the current one.  Eight consumer warps read the
+// stages with conflict-free LDS.128 and run the online softmax of the LDG kernel above.  The label logit is
+// picked out of the staged chunk that holds it; only the (< 8 element) head / tail of an odd-V row and a
+// label outside the aligned body are scalar loads, issued at row start and consumed at row end.  The
+// row-end merge costs one named barrier over the consumers (the (m, s) scratch is double-buffered).
+// Tensor maps are not needed (and could not describe V = 128257 anyway: a TMA tensor map wants 16-byte
+// row strides); the 1-D bulk copy only needs the 16-byte-aligned body that the head / tail peel isolates.
+struct __align__(16) FwdRowDesc {
+  const void *x;    // logits row; nullptr: no more rows for this CTA
+  int64_t out_idx;  // element index in p.out
+  int64_t row;      // flat row index (p.stat_max / p.stat_logsum)
+  int32_t y;        // label column, -1 when out of range
+};
+constexpr int kFwdDescs = 8;  // descriptor queue depth (rows the producer may run ahead of the consumers)
+
+template <int CONSUMERS, int STAGES, int UNROLL>
+constexpr size_t fwd_ring_smem() {
+  return static_cast<size_t>(STAGES) * CONSUMERS * UNROLL * 16 + 2 * STAGES * sizeof(uint64_t) +
+         2 * kFwdDescs * sizeof(uint64_t) + kFwdDescs * sizeof(FwdRowDesc);
+}
 
 template <typename T, int CONSUMERS, int STAGES, int UNROLL>
-__global__ void __launch_bounds__(CONSUMERS + 32) logprob_fwd_bulk_kernel(const FwdParams p) {
+__global__ void __launch_bounds__(CONSUMERS + 32) logprob_fwd_ring_kernel(const FwdParams p) {
   constexpr int E = Traits<T>::kVec;
+  constexpr int NW = CONSUMERS / kWarp;
   constexpr int STAGE_VECS = CONSUMERS * UNROLL;
   extern __shared__ __align__(128) uint8_t smem_raw[];
   uint4 *ring = reinterpret_cast<uint4 *>(smem_raw);
   uint64_t *full = reinterpret_cast<uint64_t *>(smem_raw + static_cast<size_t>(STAGES) * STAGE_VECS * 16);
   uint64_t *empty = full + STAGES;
-  __shared__ float sh_m[32], sh_s[32];
+  uint64_t *dfull = empty + STAGES;
+  uint64_t *dempty = dfull + kFwdDescs;
+  FwdRowDesc *desc = reinterpret_cast<FwdRowDesc *>(dempty + kFwdDescs);
+  __shared__ float sh_m[2][NW], sh_s[2][NW], sh_xy[2];
   const int tid = threadIdx.x;
-  const T *__restrict__ logits = reinterpret_cast<const T *>(p.logits);
   const int V = p.V;
-  const f32x2 L2 = f2_splat(p.log2e);
   if (tid == 0) {
     for (int i = 0; i < STAGES; ++i) {
       bulk::mbar_init(full + i, 1);
-      bulk::mbar_init(empty + i, CONSUMERS / kWarp);
+      bulk::mbar_init(empty + i, NW);
+    }
+    for (int i = 0; i < kFwdDescs; ++i) {
+      bulk::mbar_init(dfull + i, 1);
+      bulk::mbar_init(dempty + i, NW);
     }
     bulk::fence_barrier_init();
   }
   __syncthreads();
-  int stage = 0;
-  uint32_t phase = 0;
-  const int64_t n_rows = min(p.n_rows, __ldg(p.map.seg_cum + p.map.n_seg));  // device-built plans: see the LDG kernel
+  int stage = 0, dq = 0;
+  uint32_t phase = 0, dphase = 0;
 
   if (tid >= CONSUMERS) {
-    // ---------------- producer warp: one elected lane drives the copy engine ----------------
-    if (tid == CONSUMERS) {
-      for (int64_t row = blockIdx.x; row < n_rows; row += gridDim.x) {
+    // ---------------- producer warp: one elected lane ----------------
+    if (tid != CONSUMERS) return;
+    const T *__restrict__ logits = reinterpret_cast<const T *>(p.logits);
+    // p.n_rows is an upper bound when the plan was built on the device: see the LDG kernel
+    const int64_t n_rows = min(p.n_rows, __ldg(p.map.seg_cum + p.map.n_seg));
+    int64_t seg_lo = 0, seg_hi = 0, logit_off = 0, label_off = 0, out_off = 0;
+    for (int64_t row = blockIdx.x; row < n_rows; row += gridDim.x) {
+      if (row >= seg_hi) {  // rows only move forward: search the plan on a segment change only
         const int seg = upper_segment(p.map.seg_cum, p.map.n_seg, row);
-        const int64_t j = row - __ldg(p.map.seg_cum + seg);
-        const T *x = logits + __ldg(p.map.seg_logit_off + seg) + j * p.row_stride;
-        if (p.use_ignore && __ldg(p.labels + __ldg(p.map.seg_label_off + seg) + j) == p.ignore_index) continue;
-        const int mis = static_cast<int>((reinterpret_cast<uintptr_t>(x) & 15) / sizeof(T));
-        const int head = mis ? min(E - mis, V) : 0;
-        const int nvec = (V - head) / E;
-        const uint4 *body = reinterpret_cast<const uint4 *>(x + head);
-        for (int v0 = 0; v0 < nvec; v0 += STAGE_VECS) {
-          const int n = min(STAGE_VECS, nvec - v0);
-          bulk::mbar_wait(empty + stage, phase ^ 1u);
-          bulk::mbar_expect_tx(full + stage, static_cast<uint32_t>(n) * 16u);
-          bulk::bulk_g2s(ring + static_cast<size_t>(stage) * STAGE_VECS, body + v0, static_cast<uint32_t>(n) * 16u,
-                         full + stage);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
+        seg_lo = __ldg(p.map.seg_cum + seg);
+        seg_hi = __ldg(p.map.seg_cum + seg + 1);
+        logit_off = __ldg(p.map.seg_logit_off + seg);
+        label_off = __ldg(p.map.seg_label_off + seg);
+        out_off = __ldg(p.map.seg_out_off + seg);
       }
-    }
-    return;
-  }
-
-  // ---------------- consumer warps ----------------
-  for (int64_t row = blockIdx.x; row < n_rows; row += gridDim.x) {
-    const int seg = upper_segment(p.map.seg_cum, p.map.n_seg, row);
-    const int64_t j = row - __ldg(p.map.seg_cum + seg);
-    const T *x = logits + __ldg(p.map.seg_logit_off + seg) + j * p.row_stride;
-    const int64_t y = __ldg(p.labels + __ldg(p.map.seg_label_off + seg) + j);
-    if (p.use_ignore && y == p.ignore_index) {
-      if (tid == 0) {
-        store_from_float(p.out, __ldg(p.map.seg_out_off + seg) + j, p.out_dtype, 0.f);
+      const int64_t j = row - seg_lo;
+      const int64_t y = __ldg(p.labels + label_off + j);
+      if (p.use_ignore && y == p.ignore_index) {  // ignored position (cross-entropy ignore_index): no traffic
+        store_from_float(p.out, out_off + j, p.out_dtype, 0.f);
         if (p.stat_max) {
           p.stat_max[row] = 0.f;
           p.stat_logsum[row] = 0.f;
         }
+        continue;
       }
-      continue;
+      const T *x = logits + logit_off + j * p.row_stride;
+      bulk::mbar_wait(dempty + dq, dphase ^ 1u);
+      desc[dq] = FwdRowDesc{x, out_off + j, row, (y >= 0 && y < V) ? static_cast<int32_t>(y) : -1};
+      bulk::mbar_arrive(dfull + dq);
+      if (++dq == kFwdDescs) {
+        dq = 0;
+        dphase ^= 1u;
+      }
+      const int mis = static_cast<int>((reinterpret_cast<uintptr_t>(x) & 15) / sizeof(T));
+      const int head = mis ? min(E - mis, V) : 0;
+      const int nvec = (V - head) / E;
+      const uint4 *body = reinterpret_cast<const uint4 *>(x + head);
+      for (int v0 = 0; v0 < nvec; v0 += STAGE_VECS) {
+        const uint32_t bytes = static_cast<uint32_t>(min(STAGE_VECS, nvec - v0)) * 16u;
+        bulk::mbar_wait(empty + stage, phase ^ 1u);
+        bulk::mbar_expect_tx(full + stage, bytes);
+        bulk::bulk_g2s(ring + static_cast<size_t>(stage) * STAGE_VECS, body + v0, bytes, full + stage);
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      }
     }
-    float xy = 0.f;
-    bool y_ok = true;
-    if (tid == 0) {
-      y_ok = (y >= 0) && (y < V);
-      xy = y_ok ? Traits<T>::to_float(x[y]) : NAN;
+    bulk::mbar_wait(dempty + dq, dphase ^ 1u);
+    desc[dq].x = nullptr;
+    bulk::mbar_arrive(dfull + dq);
+    return;
+  }
+
+  // ---------------- consumer warps ----------------
+  const f32x2 L2 = f2_splat(p.log2e);
+  const int lane = tid & 31, wid = tid >> 5;
+  for (int par = 0;; par ^= 1) {
+    bulk::mbar_wait(dfull + dq, dphase);
+    const FwdRowDesc d = desc[dq];
+    __syncwarp();
+    if (lane == 0) bulk::mbar_arrive(dempty + dq);
+    if (++dq == kFwdDescs) {
+      dq = 0;
+      dphase ^= 1u;
     }
+    if (d.x == nullptr) break;
+    const T *x = reinterpret_cast<const T *>(d.x);
     const int mis = static_cast<int>((reinterpret_cast<uintptr_t>(x) & 15) / sizeof(T));
     const int head = mis ? min(E - mis, V) : 0;
     const int nvec = (V - head) / E;
     const int tail0 = head + nvec * E;
-    float m = -INFINITY, s = 0.f;
-    if (tid < head) lse_push(m, s, Traits<T>::to_float(x[tid]));
-    if (tid < V - tail0) lse_push(m, s, Traits<T>::to_float(x[tail0 + tid]));
+    const int yb = (d.y >= head && d.y < tail0) ? d.y - head : -1;  // label offset in the aligned body
+    const int yv = yb >= 0 ? yb / E : -1;
+    // scalar loads: issued now, consumed after the body has streamed by
+    const float hx = tid < head ? Traits<T>::to_float(x[tid]) : -INFINITY;
+    const float tx = tid < V - tail0 ? Traits<T>::to_float(x[tail0 + tid]) : -INFINITY;
+    const float xy_peel = (tid == 0 && d.y >= 0 && yb < 0) ? Traits<T>::to_float(x[d.y]) : 0.f;
 
+    float m = -INFINITY, s = 0.f;
     for (int v0 = 0; v0 < nvec; v0 += STAGE_VECS) {
       const int n = min(STAGE_VECS, nvec - v0);
       bulk::mbar_wait(full + stage, phase);
@@ -243,59 +289,69 @@ __global__ void __launch_bounds__(CONSUMERS + 32) logprob_fwd_bulk_kernel(const 
       for (int u = 0; u < UNROLL; ++u) {
         const int k = tid + u * CONSUMERS;
         v[u] = (k < n) ? buf[k] : bulk::neg_inf_vec<T>();
+        if (v0 + k == yv) {  // the label column lies in this vector
+          const int e = yb - yv * E;
+          float lo, hi;
+          if constexpr (sizeof(T) == 4) {
+            lo = hi = __uint_as_float(get_word(v[u], e));
+          } else {
+            unpack2<T>(get_word(v[u], e >> 1), lo, hi);
+          }
+          sh_xy[par] = (e & 1) ? hi : lo;
+        }
       }
       // order this warp's generic-proxy reads of the stage before the copy engine's next write to it
       // (compute-sanitizer racecheck reports the WAR pair without the proxy fence)
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
-      if ((tid & 31) == 0) bulk::mbar_arrive(empty + stage);  // this warp's reads of the stage are done
+      if (lane == 0) bulk::mbar_arrive(empty + stage);  // this warp's reads of the stage are done
       fold_batch<T, UNROLL>(v, m, s, L2);
       if (++stage == STAGES) {
         stage = 0;
         phase ^= 1u;
       }
     }
+    lse_push(m, s, hx);
+    lse_push(m, s, tx);
 
-    // merge the partials of the CONSUMERS threads (named barrier 1: the producer warp is not part of it)
-    {
-      constexpr int NW = CONSUMERS / kWarp;
-      const int lane = tid & 31, wid = tid >> 5;
+    // merge the partials of the CONSUMERS threads.  Named barrier 1 leaves the producer out; the scratch is
+    // double-buffered by row parity, so warp 0 reading this row's partials cannot race the next row's writes
+    // (those come after the next row's barrier, which warp 0 reaches only when it is done here).
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      float m2 = __shfl_xor_sync(0xffffffffu, m, o);
+      float s2 = __shfl_xor_sync(0xffffffffu, s, o);
+      lse_merge(m, s, m2, s2);
+    }
+    if (lane == 0) {
+      sh_m[par][wid] = m;
+      sh_s[par][wid] = s;
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
+    if (wid == 0) {
+      m = lane < NW ? sh_m[par][lane] : -INFINITY;
+      s = lane < NW ? sh_s[par][lane] : 0.f;
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
         float m2 = __shfl_xor_sync(0xffffffffu, m, o);
         float s2 = __shfl_xor_sync(0xffffffffu, s, o);
         lse_merge(m, s, m2, s2);
       }
-      if (lane == 0) {
-        sh_m[wid] = m;
-        sh_s[wid] = s;
-      }
-      asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
-      if (wid == 0) {
-        m = lane < NW ? sh_m[lane] : -INFINITY;
-        s = lane < NW ? sh_s[lane] : 0.f;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          float m2 = __shfl_xor_sync(0xffffffffu, m, o);
-          float s2 = __shfl_xor_sync(0xffffffffu, s, o);
-          lse_merge(m, s, m2, s2);
+      if (tid == 0) {
+        const float logsum = logf(s);
+        const float xy = yb >= 0 ? sh_xy[par] : xy_peel;
+        float lp = (xy - m) - logsum;  // same association as ATen's `x - max - log(sum)`
+        if (d.y < 0) {
+          lp = NAN;
+          if (p.status) atomicOr(p.status, AA_STATUS_LABEL_OOB);
+        }
+        store_from_float(p.out, d.out_idx, p.out_dtype, lp);
+        if (p.stat_max) {
+          p.stat_max[d.row] = m;
+          p.stat_logsum[d.row] = logsum;
         }
       }
     }
-    if (tid == 0) {
-      const float logsum = logf(s);
-      float lp = (xy - m) - logsum;
-      if (!y_ok) {
-        lp = NAN;
-        if (p.status) atomicOr(p.status, AA_STATUS_LABEL_OOB);
-      }
-      store_from_float(p.out, __ldg(p.map.seg_out_off + seg) + j, p.out_dtype, lp);
-      if (p.stat_max) {
-        p.stat_max[row] = m;
-        p.stat_logsum[row] = logsum;
-      }
-    }
-    asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");  // sh_m / sh_s reuse
   }
 }
 
@@ -731,56 +787,65 @@ static inline int bwd_ctas() {
   return g_bwd_variant.load(std::memory_order_relaxed) >= 0 ? g_bwd_ctas_per_sm.load(std::memory_order_relaxed) : fwd_ctas();
 }
 
-// tuning: g_variant = kernel variant (units digit) + 10 * shape code:
-//   shape 0: 256 thr x 4 vec   1: 256 x 8   2: 512 x 4   3: 128 x 8   4: 256 x 2   5: 512 x 2
-template <typename T, int THREADS, int UNROLL>
-static int launch_fwd_shape(const FwdParams &p, int per_sm, cudaStream_t st) {
-  int64_t grid = static_cast<int64_t>(sm_count()) * per_sm;
-  if (grid > p.n_rows) grid = p.n_rows;
-  logprob_fwd_kernel<T, THREADS, UNROLL><<<static_cast<unsigned>(grid), THREADS, 0, st>>>(p);
+// Persistent forward grids are sized to what is resident at once: a second wave of a grid-strided kernel streams
+// its rows with fewer CTAs per SM.  The occupancy is asked once per kernel instance (`resident` is the caller's
+// cache; the library runs on one device model).  The tuning's ctas_per_sm can only lower the count.
+template <typename K>
+static int fwd_grid(K kern, int threads, size_t smem, std::atomic<int> &resident, int64_t n_rows, unsigned &grid) {
+  int per_sm = resident.load(std::memory_order_relaxed);
+  if (per_sm == 0) {  // a race computes the same value twice, harmlessly
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem);
+    if (e != cudaSuccess || per_sm < 1) {
+      set_error("aa_logprob_fwd: no resident CTA of %d threads with %zu B of shared memory: %s", threads, smem,
+                cudaGetErrorString(e));
+      return e != cudaSuccess ? static_cast<int>(e) : AA_ERR_UNSUPPORTED;
+    }
+    resident.store(per_sm, std::memory_order_relaxed);
+  }
+  if (fwd_ctas() > 0 && fwd_ctas() < per_sm) per_sm = fwd_ctas();
+  const int64_t g = static_cast<int64_t>(sm_count()) * per_sm;
+  grid = static_cast<unsigned>(g < n_rows ? g : n_rows);
+  return 0;
+}
+
+template <typename T>
+static int launch_fwd_ldg(const FwdParams &p, cudaStream_t st) {
+  constexpr int THREADS = 512, UNROLL = 4;
+  auto kern = logprob_fwd_kernel<T, THREADS, UNROLL>;
+  static std::atomic<int> resident{0};
+  unsigned grid = 0;
+  int rc = fwd_grid(kern, THREADS, 0, resident, p.n_rows, grid);
+  if (rc) return rc;
+  kern<<<grid, THREADS, 0, st>>>(p);
+  return check_launch("aa_logprob_fwd(ldg)");
+}
+
+template <typename T>
+static int launch_fwd_ring(const FwdParams &p, cudaStream_t st) {
+  constexpr int CONSUMERS = 256, STAGES = 4, UNROLL = 4;  // 4 stages x 16 KB; 3 CTAs per SM are resident
+  constexpr size_t smem = fwd_ring_smem<CONSUMERS, STAGES, UNROLL>();
+  auto kern = logprob_fwd_ring_kernel<T, CONSUMERS, STAGES, UNROLL>;
+  static std::atomic<int> resident{0};
+  unsigned grid = 0;
+  int rc = fwd_grid(kern, CONSUMERS + 32, smem, resident, p.n_rows, grid);
+  if (rc) return rc;
+  kern<<<grid, CONSUMERS + 32, smem, st>>>(p);
   return check_launch("aa_logprob_fwd");
 }
 
-template <typename T>
-static int launch_fwd_bulk(const FwdParams &p, cudaStream_t st) {
-  constexpr int CONSUMERS = 256, STAGES = 4, UNROLL = 4;
-  constexpr size_t smem = static_cast<size_t>(STAGES) * CONSUMERS * UNROLL * 16 + 2 * STAGES * sizeof(uint64_t);
-  auto kern = logprob_fwd_bulk_kernel<T, CONSUMERS, STAGES, UNROLL>;
-  static std::atomic<bool> configured{false};  // the attribute is idempotent: a race sets it twice, harmlessly
-  if (!configured.load(std::memory_order_relaxed)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) {
-      set_error("aa_logprob_fwd(bulk): cannot reserve %zu B of shared memory: %s", smem, cudaGetErrorString(e));
-      return static_cast<int>(e);
-    }
-    configured.store(true, std::memory_order_relaxed);
-  }
-  const int per_sm = fwd_ctas() > 0 ? fwd_ctas() : 3;
-  int64_t grid = static_cast<int64_t>(sm_count()) * per_sm;
-  if (grid > p.n_rows) grid = p.n_rows;
-  kern<<<static_cast<unsigned>(grid), CONSUMERS + 32, smem, st>>>(p);
-  return check_launch("aa_logprob_fwd(bulk)");
-}
+// Which forward streams a row is decided by the row's length.  Measured on an H100 SXM at 400 W (DESIGN.md section
+// 3.1): rows of 256 KB and more (V = 128257 / 156032 in bf16) move faster through the LDG kernel at 4 CTAs x 512
+// threads per SM (C2: 5.7 ms against 5.9-6.1 ms for the ring), 64 KB rows (V = 32064) through the ring (C3: 0.55 ms
+// against 0.62 ms).  Tuning kernel digit 1 forces the ring, digit 2 the LDG kernel.
+constexpr int64_t kFwdLdgMinRowBytes = 128 * 1024;
 
 template <typename T>
 static int launch_fwd(const FwdParams &p, cudaStream_t st) {
-  if ((fwd_variant() % 10) == 1) return launch_fwd_bulk<T>(p, st);
-  const int shape = (fwd_variant() / 10) % 10;
-  const int per_sm = fwd_ctas() > 0 ? fwd_ctas() : 6;
-  if constexpr (sizeof(T) == 2) {
-    switch (shape) {
-      case 1: return launch_fwd_shape<T, 256, 8>(p, per_sm, st);
-      case 2: return launch_fwd_shape<T, 512, 4>(p, fwd_ctas() > 0 ? fwd_ctas() : 3, st);
-      case 3: return launch_fwd_shape<T, 128, 8>(p, fwd_ctas() > 0 ? fwd_ctas() : 12, st);
-      case 4: return launch_fwd_shape<T, 256, 2>(p, per_sm, st);
-      case 5: return launch_fwd_shape<T, 512, 2>(p, fwd_ctas() > 0 ? fwd_ctas() : 3, st);
-      default: break;
-    }
-  }
-  // default (16-bit logits): 128 threads x 8 vectors in flight, 16 CTAs/SM -- the read-only stream likes many bytes
-  // in flight (the shapes above are the alternatives selected with aa_logprob_set_tuning).
-  if constexpr (sizeof(T) == 2) return launch_fwd_shape<T, 128, 8>(p, fwd_ctas() > 0 ? fwd_ctas() : 16, st);
-  return launch_fwd_shape<T, 256, 4>(p, per_sm, st);
+  const int digit = fwd_variant() % 10;
+  if (digit == 2 || (digit != 1 && static_cast<int64_t>(p.V) * sizeof(T) >= kFwdLdgMinRowBytes))
+    return launch_fwd_ldg<T>(p, st);
+  return launch_fwd_ring<T>(p, st);
 }
 
 template <typename T, int THREADS, int UNROLL>

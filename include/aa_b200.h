@@ -71,8 +71,8 @@ const char *aa_last_error(void);
 /* Number of SMs / max dynamic smem of the current device (for host-side grid sizing). */
 int aa_device_info(int *sm_count, int *max_smem_optin);
 /* Tuning / diagnostic knobs (process-wide).  variant = kernel digit + 10 * shape code.
- *   forward  kernel digit: 0 = vectorised LDG (default), 1 = cp.async.bulk staged through shared memory;
- *            shape: 0 = default (128 threads x 8 vectors x 16 CTAs/SM), 1 = 256x8, 2 = 512x4, 3 = 128x8, 4 = 256x2, 5 = 512x2.
+ *   forward  kernel digit: 0 / 3 = chosen by row length (default), 1 = cp.async.bulk ring through shared memory,
+ *            2 = vectorised LDG; no shape codes (each kernel has one launch shape, grid = resident CTAs).
  *   backward kernel digit: 0 / 1 = TMA-staged (cp.async.bulk loads AND stores through a shared-memory ring;
  *            the default whenever row_scratch is given), 2 = experimental address-ordered chunked sweep,
  *            3 = one-CTA-per-row LDG/STG kernel (also used when row_scratch == NULL);
