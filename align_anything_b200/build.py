@@ -55,20 +55,6 @@ def is_fresh() -> bool:
     return os.path.exists(LIB) and os.path.exists(stamp_file) and open(stamp_file).read().strip() == _stamp()
 
 
-def build_experiment(tag: str, defines: list[str]) -> str:
-    """Build a side copy libaa_b200.<tag>.so with extra -D flags (tuning experiments only; select it
-    at run time with AA_B200_LIB=<path>)."""
-    nvcc = _nvcc()
-    out = os.path.join(CSRC, f'libaa_b200.{tag}.so')
-    srcs = [os.path.join(CSRC, s) for s in SOURCES]
-    flags = [f for f in NVCC_FLAGS if f not in ('-Xptxas', '-v')]
-    cmd = [nvcc, *flags, *[f'-D{d}' for d in defines], '-I', INCLUDE, '-shared', '-o', out, *srcs]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(f'nvcc failed:\n{r.stdout}\n{r.stderr}')
-    return out
-
-
 def build(force: bool = False, verbose: bool = False) -> str:
     """Compile every .cu for sm_90a and link libaa_b200.so.  Returns the library path."""
     if not force and is_fresh():

@@ -120,41 +120,17 @@ __device__ __forceinline__ void round_bf16_pair(float &a, float &b) {
 }
 
 // ---- streaming 128-bit global access (read-once / write-once tiles) ---------------------
-// load policy (compile-time experiment knob): 0 = nc + L1::no_allocate + L2::256B prefetch (default),
-// 1 = same without the 256B prefetch hint, 2 = L2::evict_first, 3 = L1::no_allocate + L2::evict_first + 256B
-#ifndef AA_LDG_POLICY
-#define AA_LDG_POLICY 0
-#endif
+// loads: nc + L1::no_allocate + L2::256B prefetch
 __device__ __forceinline__ uint4 ldg_stream(const uint4 *p) {
   uint4 r;
-#if AA_LDG_POLICY == 0
   asm("ld.global.nc.L1::no_allocate.L2::256B.v4.u32 {%0,%1,%2,%3}, [%4];"
-#elif AA_LDG_POLICY == 1
-  asm("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-#elif AA_LDG_POLICY == 2
-  asm("ld.global.nc.L1::no_allocate.L2::evict_first.v4.u32 {%0,%1,%2,%3}, [%4];"
-#else
-  asm("ld.global.nc.L1::no_allocate.L2::evict_first.L2::256B.v4.u32 {%0,%1,%2,%3}, [%4];"
-#endif
       : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
       : "l"(p));
   return r;
 }
-// store policy (compile-time experiment knob): 0 = .cs (evict-first),
-// 1 = default write-back, 2 = .L1::no_allocate, 3 = .wt
-#ifndef AA_STG_POLICY
-#define AA_STG_POLICY 0
-#endif
+// stores: .cs (evict-first)
 __device__ __forceinline__ void stg_stream(uint4 *p, const uint4 &v) {
-#if AA_STG_POLICY == 0
   asm volatile("st.global.cs.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-#elif AA_STG_POLICY == 1
-  asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-#elif AA_STG_POLICY == 2
-  asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-#else
-  asm volatile("st.global.wt.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-#endif
 }
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -200,47 +176,6 @@ __device__ __forceinline__ f32x2 f2_round_bf16(f32x2 x, f32x2 zero2) {
 __device__ __forceinline__ f32x2 f2_round_f16(f32x2 x, f32x2 zero2) {
   const f32x2 c = f2_fma(x, f2_splat(8193.f), zero2);
   return f2_sub(c, f2_sub(c, x));
-}
-
-// 2^t on the FMA / ALU pipes (no MUFU): Cody-Waite split t = n + f, f in [-0.5, 0.5], degree-5 minimax
-// polynomial with c0 == 1 exactly (so 2^0 == 1 exactly, like MUFU.EX2), exponent patched in with one
-// integer add.  Max relative error 1.9e-7 (MUFU.EX2: 2^-22 = 2.4e-7).  An experiment to unload the
-// MUFU pipe (16/clk/SM); it is off by default (logprob.cu, AA_FWD_POLY_WORDS).
-__device__ __forceinline__ float ex2_poly(float t) {
-  float tc;
-  asm("max.NaN.f32 %0, %1, %2;" : "=f"(tc) : "f"(t), "f"(-126.f));  // NaN stays NaN
-  const float r = tc + 12582912.f;                                    // 1.5 * 2^23: rounds to nearest integer
-  const float f = tc - (r - 12582912.f);
-  float p = 1.328307088e-03f;
-  p = fmaf(p, f, 9.671507403e-03f);
-  p = fmaf(p, f, 5.550670624e-02f);
-  p = fmaf(p, f, 2.402224243e-01f);
-  p = fmaf(p, f, 6.931470037e-01f);
-  p = fmaf(p, f, 1.0f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(r) << 23));
-}
-
-// Packed version of ex2_poly: two lanes per instruction for the range reduction and the Horner chain.
-__device__ __forceinline__ f32x2 f2_ex2_poly(f32x2 t) {
-  float ta, tb;
-  f2_unpack(t, ta, tb);
-  asm("max.NaN.f32 %0, %1, %2;" : "=f"(ta) : "f"(ta), "f"(-126.f));
-  asm("max.NaN.f32 %0, %1, %2;" : "=f"(tb) : "f"(tb), "f"(-126.f));
-  const f32x2 tc = f2_pack(ta, tb);
-  const f32x2 magic = f2_splat(12582912.f);
-  const f32x2 r = f2_add(tc, magic);
-  const f32x2 f = f2_sub(tc, f2_sub(r, magic));
-  f32x2 p = f2_splat(1.328307088e-03f);
-  p = f2_fma(p, f, f2_splat(9.671507403e-03f));
-  p = f2_fma(p, f, f2_splat(5.550670624e-02f));
-  p = f2_fma(p, f, f2_splat(2.402224243e-01f));
-  p = f2_fma(p, f, f2_splat(6.931470037e-01f));
-  p = f2_fma(p, f, f2_splat(1.0f));
-  float pa, pb, ra, rb;
-  f2_unpack(p, pa, pb);
-  f2_unpack(r, ra, rb);
-  return f2_pack(__int_as_float(__float_as_int(pa) + (__float_as_int(ra) << 23)),
-                 __int_as_float(__float_as_int(pb) + (__float_as_int(rb) << 23)));
 }
 
 // ---- warp / block reductions ------------------------------------------------------------

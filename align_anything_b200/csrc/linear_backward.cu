@@ -19,8 +19,6 @@
 // Persistent grid: CTA b walks tiles b, b + grid, ... with the N tiles of one M tile adjacent, so the CTAs resident
 // together share their A strip through L2.  d(weight) accumulates across row chunks in an fp32 buffer (read-modify-write
 // in the epilogue) and is rounded to bf16 once, by the last chunk -- like a single GEMM over all rows.
-#include <stdlib.h>
-
 #include <atomic>
 
 #include "wgmma.cuh"
@@ -38,19 +36,12 @@ struct GemmParams {
   int64_t ldc_f32;
   int beta;                  // != 0: add the fp32 accumulator's current contents
   int tiles_m, tiles_n;
-  int n_band;                // tile order: bands of n_band N tiles, all M tiles of a band before the next band (0 = one band)
 };
 
-// linear tile id -> (M tile, N tile).  Within a band the N tiles of one M tile are adjacent, so co-resident CTAs share the A
-// strip; a band narrower than tiles_n shrinks the B working set that every wave of M tiles re-reads (d(weight): the
-// 67 MB hidden chunk does not survive in L2 next to the streaming d(logits) strips, half of it does).
+// linear tile id -> (M tile, N tile).  The N tiles of one M tile are adjacent, so co-resident CTAs share the A strip.
 __device__ __forceinline__ void tile_coords(const GemmParams &p, int tile, int &mt, int &nt) {
-  const int nb = p.n_band > 0 && p.n_band < p.tiles_n ? p.n_band : p.tiles_n;
-  const int per_band = p.tiles_m * nb;
-  const int band = tile / per_band, rem = tile - band * per_band;
-  const int width = min(nb, p.tiles_n - band * nb);
-  mt = rem / width;
-  nt = band * nb + rem % width;
+  mt = tile / p.tiles_n;
+  nt = tile % p.tiles_n;
 }
 
 template <int A_MN, int B_MN>
@@ -136,13 +127,6 @@ __global__ void __launch_bounds__(THREADS, 1)
   }
 }
 
-// tile-order override for sweeps, read once: AA_B200_GEMM_BAND_DH / _DW = N tiles per band (0 = all N tiles, one band)
-static int band_env(int which) {
-  static const int v[2] = {[] { const char *e = getenv("AA_B200_GEMM_BAND_DH"); return e ? atoi(e) : 0; }(),
-                           [] { const char *e = getenv("AA_B200_GEMM_BAND_DW"); return e ? atoi(e) : 0; }()};
-  return v[which];
-}
-
 template <int A_MN, int B_MN>
 static int launch(const CUtensorMap &map_a, const CUtensorMap &map_b, const GemmParams &p, cudaStream_t st, const char *who) {
   auto kern = lm_head_bwd_gemm_kernel<A_MN, B_MN>;
@@ -189,7 +173,7 @@ extern "C" int aa_linear_dhidden(const void *dlogits, int64_t n_rows, int64_t ld
   if (rc) return rc;
   lmbwd::GemmParams p{static_cast<int>(n_rows), H, static_cast<int>(ld), static_cast<__nv_bfloat16 *>(d_hidden),
                       d_hidden_row_stride, nullptr, 0, 0, static_cast<int>((n_rows + wg::BM - 1) / wg::BM),
-                      (H + wg::BN - 1) / wg::BN, lmbwd::band_env(0)};
+                      (H + wg::BN - 1) / wg::BN};
   return lmbwd::launch<0, 1>(map_a, map_b, p, static_cast<cudaStream_t>(stream), "aa_linear_dhidden");
 }
 
@@ -216,7 +200,6 @@ extern "C" int aa_linear_dweight(const void *dlogits, int64_t n_rows, int64_t ld
   rc = wg::make_map_2d(&map_b, hidden, H, n_rows, hidden_row_stride, wg::BK, "aa_linear_dweight");
   if (rc) return rc;
   lmbwd::GemmParams p{V, H, static_cast<int>(n_rows), static_cast<__nv_bfloat16 *>(d_weight), d_weight_row_stride, acc_f32,
-                      acc_row_stride, accumulate ? 1 : 0, (V + wg::BM - 1) / wg::BM, (H + wg::BN - 1) / wg::BN,
-                      lmbwd::band_env(1)};
+                      acc_row_stride, accumulate ? 1 : 0, (V + wg::BM - 1) / wg::BM, (H + wg::BN - 1) / wg::BN};
   return lmbwd::launch<1, 1>(map_a, map_b, p, static_cast<cudaStream_t>(stream), "aa_linear_dweight");
 }

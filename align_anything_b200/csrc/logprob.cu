@@ -472,14 +472,10 @@ __global__ void __launch_bounds__(THREADS) logprob_bwd_kernel(const BwdParams p)
   }
 }
 
-// ---- K1b, chunked (experiment, selected with tuning kernel digit 2): the gradient tile is swept in
-// address order.  An experiment, not the default: it was slower than the one-CTA-per-row kernel above.
-// The backward needs no per-row reduction (max / logsum come from the forward), so a row does not
-// have to be owned by one CTA.  Work unit = (row, chunk of THREADS*UNROLL 16-byte vectors);
-// consecutive CTAs take consecutive units, so at any moment the whole grid reads and writes one
-// compact window of the tile that moves through memory in address order (what a plain copy does),
-// instead of gridDim different rows 256 KB apart.  A tiny prep kernel resolves each row once
-// (segment search, label, saved stats, upstream gradient) into a 32-byte record.
+// ---- K1b, TMA-staged (default whenever row_scratch is given) -------------------------------------
+// The backward needs no per-row reduction (max / logsum come from the forward).  A tiny prep kernel
+// resolves each row once (segment search, label, saved stats, upstream gradient) into a 32-byte record,
+// so the TMA kernel below reads one record per row instead of searching the row plan.
 struct __align__(16) RowRec {
   int64_t x_off;   // element offset of the logits row
   int64_t g_row;   // row index in the gradient tile
@@ -541,88 +537,11 @@ __global__ void bwd_row_prep_kernel(const BwdParams p, RowRec *__restrict__ rec)
   rec[slot] = r;
 }
 
-template <typename T, int THREADS, int UNROLL, bool FAITHFUL>
-__global__ void __launch_bounds__(THREADS)
-    logprob_bwd_chunk_kernel(const T *__restrict__ logits, T *__restrict__ grad, int64_t grad_row_stride, int V,
-                             const RowRec *__restrict__ rec, int64_t n_work, int upr, float zero) {
-  constexpr int E = Traits<T>::kVec;
-  constexpr int CH = THREADS * UNROLL;
-  const int tid = threadIdx.x;
-  const int64_t n_units = n_work * upr;
-  for (int64_t u = blockIdx.x; u < n_units; u += gridDim.x) {
-    const int64_t r = u / upr;
-    const int c = static_cast<int>(u - r * upr);
-    const int4 r0 = __ldg(reinterpret_cast<const int4 *>(rec + r));
-    const int4 r1 = __ldg(reinterpret_cast<const int4 *>(rec + r) + 1);
-    const int64_t x_off = (static_cast<int64_t>(static_cast<uint32_t>(r0.y)) << 32) | static_cast<uint32_t>(r0.x);
-    const int64_t g_row = (static_cast<int64_t>(static_cast<uint32_t>(r0.w)) << 32) | static_cast<uint32_t>(r0.z);
-    const float m = __int_as_float(r1.x), logsum = __int_as_float(r1.y), g = __int_as_float(r1.z);
-    const int y = r1.w;
-    T *g_out = grad + g_row * grad_row_stride;
-    const int mis = static_cast<int>((reinterpret_cast<uintptr_t>(g_out) & 15) / sizeof(T));
-    // vector v of the row's 16-byte-aligned span covers elements [v*E - mis, v*E - mis + E)
-    uint4 *gspan = reinterpret_cast<uint4 *>(g_out - mis);
-    const int v0 = c * CH + tid;
-    if (y == -2) {
-#pragma unroll
-      for (int q = 0; q < UNROLL; ++q) {
-        const int v = v0 + q * THREADS;
-        const int e0 = v * E - mis;
-        if (e0 >= 0 && e0 + E <= V) {
-          stg_stream(gspan + v, make_uint4(0, 0, 0, 0));
-        } else {
-          for (int e = max(e0, 0); e < min(e0 + E, V); ++e) g_out[e] = Traits<T>::from_float(0.f);
-        }
-      }
-      continue;
-    }
-    const T *x = logits + x_off;
-    const float lse = m + logsum;
-    const float c_f32 = -lse * kLog2e;
-    const float neg_g = FAITHFUL ? -g : -g * ex2_approx(fmaf(-lse, kLog2e, -c_f32));
-    const GradConsts gk = make_grad_consts(m, logsum, c_f32, neg_g, zero);
-    const bool same_phase = ((reinterpret_cast<uintptr_t>(x) ^ reinterpret_cast<uintptr_t>(g_out)) & 15) == 0;
-    if (same_phase) {
-      const uint4 *xspan = reinterpret_cast<const uint4 *>(x - mis);
-      const int yv = (y >= 0) ? (y + mis) / E : -1;
-      uint4 val[UNROLL];
-#pragma unroll
-      for (int q = 0; q < UNROLL; ++q) {
-        const int v = v0 + q * THREADS;
-        const int e0 = v * E - mis;
-        if (e0 >= 0 && e0 + E <= V) val[q] = ldg_stream(xspan + v);
-      }
-#pragma unroll
-      for (int q = 0; q < UNROLL; ++q) {
-        const int v = v0 + q * THREADS;
-        const int e0 = v * E - mis;
-        if (e0 >= 0 && e0 + E <= V) {
-          uint4 o = vec_grad<T, FAITHFUL>(val[q], gk);
-          if (v == yv) patch_label<T, FAITHFUL>(o, val[q], y - e0, m, logsum, c_f32, neg_g, g);
-          stg_stream(gspan + v, o);
-        } else {  // row head / tail: the vector sticks out of the row
-          for (int e = max(e0, 0); e < min(e0 + E, V); ++e)
-            g_out[e] = Traits<T>::from_float(
-                grad_of<T, FAITHFUL>(Traits<T>::to_float(x[e]), m, logsum, c_f32, neg_g, g, e == y));
-        }
-      }
-    } else {
-      // logits view and gradient tile disagree on the 16-byte phase of this row: element loop
-      const int e_lo = max(c * CH * E - mis, 0);
-      const int e_hi = min((c + 1) * CH * E - mis, V);
-      for (int e = e_lo + tid; e < e_hi; e += THREADS)
-        g_out[e] = Traits<T>::from_float(
-            grad_of<T, FAITHFUL>(Traits<T>::to_float(x[e]), m, logsum, c_f32, neg_g, g, e == y));
-    }
-  }
-}
-
-// ---- K1b, TMA-staged (default for 16-byte-phase-compatible tiles) ---------------------------------
 // A pure copy with the one-CTA-per-row access structure of the LDG kernel above stays below what the copy
 // engine (cp.async.bulk global->smem, smem->global, 64 KB in flight per SM) reaches, which is cudaMemcpy
 // speed.  So the backward moves its data with the TMA engine in both directions and the SM only touches
 // shared memory:
-//   producer lane : RowRec -> cp.async.bulk loads of 16 KB chunks of the row's aligned body into a ring
+//   producer lane : RowRec -> cp.async.bulk loads of stage-sized chunks of the row's aligned body into a ring
 //                   (full mbarriers, expect_tx), and -- lagging LAG chunks behind -- cp.async.bulk
 //                   STORES of the chunks the consumers have finished (done mbarriers); zero rows are
 //                   stored straight from a zeroed shared-memory buffer, no SM data path at all;
@@ -772,20 +691,15 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
 // ---- host side ----------------------------------------------------------------------------
 // Tuning knobs of the DIAGNOSTIC entry points aa_logprob_set_tuning{,_bwd}: process-wide by design (sweeps set them once,
 // before a run; the trainers never touch them).  Atomics make a setter racing with launches on another thread well
-// defined: such a launch may see the old or the new shape, both valid -- results never depend on the knobs.
-static std::atomic<int> g_variant{0};        // forward (and backward unless overridden)
+// defined: such a launch may see the old or the new kernel, both valid -- results never depend on the knobs.
+static std::atomic<int> g_variant{0};        // forward: 0 / 3 by row length, 1 ring, 2 LDG
 static std::atomic<int> g_ctas_per_sm{0};
-static std::atomic<int> g_bwd_variant{-1};   // -1: follow the forward setting
+static std::atomic<int> g_bwd_variant{0};    // backward: -1 / 0 / 1 TMA-staged, 3 LDG row kernel
 static std::atomic<int> g_bwd_ctas_per_sm{0};
 static inline int fwd_variant() { return g_variant.load(std::memory_order_relaxed); }
 static inline int fwd_ctas() { return g_ctas_per_sm.load(std::memory_order_relaxed); }
-static inline int bwd_variant() {
-  const int v = g_bwd_variant.load(std::memory_order_relaxed);
-  return v >= 0 ? v : fwd_variant();
-}
-static inline int bwd_ctas() {
-  return g_bwd_variant.load(std::memory_order_relaxed) >= 0 ? g_bwd_ctas_per_sm.load(std::memory_order_relaxed) : fwd_ctas();
-}
+static inline int bwd_variant() { return g_bwd_variant.load(std::memory_order_relaxed); }
+static inline int bwd_ctas() { return g_bwd_ctas_per_sm.load(std::memory_order_relaxed); }
 
 // Persistent forward grids are sized to what is resident at once: a second wave of a grid-strided kernel streams
 // its rows with fewer CTAs per SM.  The occupancy is asked once per kernel instance (`resident` is the caller's
@@ -837,73 +751,30 @@ static int launch_fwd_ring(const FwdParams &p, cudaStream_t st) {
 // Which forward streams a row is decided by the row's length.  Measured on an H100 SXM at 400 W (DESIGN.md section
 // 3.1): rows of 256 KB and more (V = 128257 / 156032 in bf16) move faster through the LDG kernel at 4 CTAs x 512
 // threads per SM (C2: 5.7 ms against 5.9-6.1 ms for the ring), 64 KB rows (V = 32064) through the ring (C3: 0.55 ms
-// against 0.62 ms).  Tuning kernel digit 1 forces the ring, digit 2 the LDG kernel.
+// against 0.62 ms).  Tuning variant 1 forces the ring, variant 2 the LDG kernel.
 constexpr int64_t kFwdLdgMinRowBytes = 128 * 1024;
 
 template <typename T>
 static int launch_fwd(const FwdParams &p, cudaStream_t st) {
-  const int digit = fwd_variant() % 10;
-  if (digit == 2 || (digit != 1 && static_cast<int64_t>(p.V) * sizeof(T) >= kFwdLdgMinRowBytes))
+  const int variant = fwd_variant();
+  if (variant == 2 || (variant != 1 && static_cast<int64_t>(p.V) * sizeof(T) >= kFwdLdgMinRowBytes))
     return launch_fwd_ldg<T>(p, st);
   return launch_fwd_ring<T>(p, st);
 }
 
-template <typename T, int THREADS, int UNROLL>
-static int launch_bwd_shape(const BwdParams &p, int mode, int per_sm, cudaStream_t st) {
+template <typename T, int THREADS, int UNROLL, bool FAITHFUL>
+static int launch_bwd_shape(const BwdParams &p, int per_sm, cudaStream_t st) {
   const int64_t n_work = bwd_work_rows(p);
   int64_t grid = static_cast<int64_t>(sm_count()) * per_sm;
   if (grid > n_work) grid = n_work;
-  const bool faithful = (mode == AA_MODE_FAITHFUL) && sizeof(T) == 2;
-  if (faithful)
-    logprob_bwd_kernel<T, THREADS, UNROLL, true><<<static_cast<unsigned>(grid), THREADS, 0, st>>>(p);
-  else
-    logprob_bwd_kernel<T, THREADS, UNROLL, false><<<static_cast<unsigned>(grid), THREADS, 0, st>>>(p);
+  logprob_bwd_kernel<T, THREADS, UNROLL, FAITHFUL><<<static_cast<unsigned>(grid), THREADS, 0, st>>>(p);
   return check_launch("aa_logprob_bwd");
 }
 
-template <typename T, int THREADS, int UNROLL>
-static int launch_bwd_chunk_shape(const BwdParams &p, int mode, int per_sm, RowRec *rec, cudaStream_t st) {
-  constexpr int E = Traits<T>::kVec;
-  const int64_t n_work = bwd_work_rows(p);
-  bwd_row_prep_kernel<<<static_cast<unsigned>((n_work + 255) / 256), 256, 0, st>>>(p, rec);
-  int rc = check_launch("aa_logprob_bwd(prep)");
-  if (rc) return rc;
-  const int span_vecs = (p.V + 2 * (E - 1)) / E + 1;
-  const int upr = (span_vecs + THREADS * UNROLL - 1) / (THREADS * UNROLL);
-  const int64_t n_units = n_work * upr;
-  int64_t grid = static_cast<int64_t>(sm_count()) * per_sm;
-  if (grid > n_units) grid = n_units;
-  const bool faithful = (mode == AA_MODE_FAITHFUL) && sizeof(T) == 2;
-  const T *lg = reinterpret_cast<const T *>(p.logits);
-  T *gr = reinterpret_cast<T *>(p.grad_logits);
-  if (faithful)
-    logprob_bwd_chunk_kernel<T, THREADS, UNROLL, true>
-        <<<static_cast<unsigned>(grid), THREADS, 0, st>>>(lg, gr, p.grad_row_stride, p.V, rec, n_work, upr, p.zero);
-  else
-    logprob_bwd_chunk_kernel<T, THREADS, UNROLL, false>
-        <<<static_cast<unsigned>(grid), THREADS, 0, st>>>(lg, gr, p.grad_row_stride, p.V, rec, n_work, upr, p.zero);
-  return check_launch("aa_logprob_bwd(chunk)");
-}
-
+// TMA-staged backward: 256 consumers, 4 stages x 8 KB, lag 3, 3 CTAs/SM.
 template <typename T>
-static int launch_bwd_chunk(const BwdParams &p, int mode, RowRec *rec, cudaStream_t st) {
-  const int shape = (bwd_variant() / 10) % 10;
-  const int per_sm = bwd_ctas() > 0 ? bwd_ctas() : 8;
-  if constexpr (sizeof(T) == 2) {
-    switch (shape) {
-      case 1: return launch_bwd_chunk_shape<T, 256, 8>(p, mode, per_sm, rec, st);
-      case 2: return launch_bwd_chunk_shape<T, 512, 4>(p, mode, bwd_ctas() > 0 ? bwd_ctas() : 4, rec, st);
-      case 3: return launch_bwd_chunk_shape<T, 128, 8>(p, mode, bwd_ctas() > 0 ? bwd_ctas() : 16, rec, st);
-      case 4: return launch_bwd_chunk_shape<T, 256, 2>(p, mode, per_sm, rec, st);
-      case 5: return launch_bwd_chunk_shape<T, 512, 2>(p, mode, bwd_ctas() > 0 ? bwd_ctas() : 4, rec, st);
-      default: break;
-    }
-  }
-  return launch_bwd_chunk_shape<T, 256, 4>(p, mode, per_sm, rec, st);
-}
-
-template <typename T, int CONSUMERS, int STAGES, int UNROLL, int LAG>
-static int launch_bwd_tma_shape(const BwdParams &p, int mode, int per_sm, RowRec *rec, cudaStream_t st) {
+static int launch_bwd_tma(const BwdParams &p, int mode, RowRec *rec, cudaStream_t st) {
+  constexpr int CONSUMERS = 256, STAGES = 4, UNROLL = 2, LAG = 3;
   const int64_t n_work = bwd_work_rows(p);
   bwd_row_prep_kernel<<<static_cast<unsigned>((n_work + 255) / 256), 256, 0, st>>>(p, rec);
   int rc = check_launch("aa_logprob_bwd(prep)");
@@ -922,6 +793,7 @@ static int launch_bwd_tma_shape(const BwdParams &p, int mode, int per_sm, RowRec
     }
     configured.store(true, std::memory_order_relaxed);
   }
+  const int per_sm = bwd_ctas() > 0 ? bwd_ctas() : 3;
   int64_t grid = static_cast<int64_t>(sm_count()) * per_sm;
   if (grid > n_work) grid = n_work;
   const T *lg = reinterpret_cast<const T *>(p.logits);
@@ -933,46 +805,17 @@ static int launch_bwd_tma_shape(const BwdParams &p, int mode, int per_sm, RowRec
   return check_launch("aa_logprob_bwd(tma)");
 }
 
-// shape codes of the TMA-staged backward (stages x stage size, lag, default CTAs/SM):
-//   0 (default): 4 x 8 KB, lag 3, 3 CTAs/SM   1: 4 x 16 KB, lag 2, 2   2: 4 x 8 KB, lag 3, 3 (= default)
-//   3: 6 x 8 KB, lag 4, 2                     4: 3 x 16 KB, lag 2, 2   5: 8 x 8 KB, lag 6, 2   6: 4 x 16 KB, lag 3, 2
-template <typename T>
-static int launch_bwd_tma(const BwdParams &p, int mode, RowRec *rec, cudaStream_t st) {
-  const int shape = (bwd_variant() / 10) % 10;
-  const int c = bwd_ctas();
-  switch (shape) {
-    case 1: return launch_bwd_tma_shape<T, 256, 4, 4, 2>(p, mode, c > 0 ? c : 2, rec, st);
-    case 3: return launch_bwd_tma_shape<T, 256, 6, 2, 4>(p, mode, c > 0 ? c : 2, rec, st);
-    case 4: return launch_bwd_tma_shape<T, 256, 3, 4, 2>(p, mode, c > 0 ? c : 2, rec, st);
-    case 5: return launch_bwd_tma_shape<T, 256, 8, 2, 6>(p, mode, c > 0 ? c : 2, rec, st);
-    case 6: return launch_bwd_tma_shape<T, 256, 4, 4, 3>(p, mode, c > 0 ? c : 2, rec, st);
-    default: break;
-  }
-  return launch_bwd_tma_shape<T, 256, 4, 2, 3>(p, mode, c > 0 ? c : 3, rec, st);
-}
-
+// One-CTA-per-row LDG/STG backward.  The read+write stream is sensitive to how much is in flight per SM and the
+// optimum depends on the compute per byte: 16-bit FAITHFUL (Veltkamp rounding, ~7 instr/elem) 512 thr x 4 vec x
+// 3 CTAs/SM, 16-bit F32 mode (~3.5 instr/elem) 512 x 2 x 3, fp32 logits 256 x 4 x 4.
 template <typename T>
 static int launch_bwd(const BwdParams &p, int mode, cudaStream_t st) {
-  const int shape = (bwd_variant() / 10) % 10;
-  const int per_sm = bwd_ctas() > 0 ? bwd_ctas() : 6;
+  const int c = bwd_ctas();
   if constexpr (sizeof(T) == 2) {
-    switch (shape) {
-      case 1: return launch_bwd_shape<T, 256, 8>(p, mode, per_sm, st);
-      case 2: return launch_bwd_shape<T, 512, 4>(p, mode, bwd_ctas() > 0 ? bwd_ctas() : 3, st);
-      case 3: return launch_bwd_shape<T, 128, 8>(p, mode, bwd_ctas() > 0 ? bwd_ctas() : 12, st);
-      case 4: return launch_bwd_shape<T, 256, 2>(p, mode, per_sm, st);
-      case 5: return launch_bwd_shape<T, 512, 2>(p, mode, bwd_ctas() > 0 ? bwd_ctas() : 3, st);
-      default: break;
-    }
+    if (mode == AA_MODE_FAITHFUL) return launch_bwd_shape<T, 512, 4, true>(p, c > 0 ? c : 3, st);
+    return launch_bwd_shape<T, 512, 2, false>(p, c > 0 ? c : 3, st);
   }
-  // default (16-bit logits).  The read+write stream is sensitive to how much is in flight per SM and the
-  // optimum depends on the compute per byte of the variant: FAITHFUL (Veltkamp rounding, ~7 instr/elem)
-  // 512 thr x 4 vec x 3 CTAs/SM, F32 mode (~3.5 instr/elem) 512 x 2 x 3.
-  if constexpr (sizeof(T) == 2) {
-    if (mode == AA_MODE_FAITHFUL) return launch_bwd_shape<T, 512, 4>(p, mode, bwd_ctas() > 0 ? bwd_ctas() : 3, st);
-    return launch_bwd_shape<T, 512, 2>(p, mode, bwd_ctas() > 0 ? bwd_ctas() : 3, st);
-  }
-  return launch_bwd_shape<T, 256, 4>(p, mode, bwd_ctas() > 0 ? bwd_ctas() : 4, st);
+  return launch_bwd_shape<T, 256, 4, false>(p, c > 0 ? c : 4, st);
 }
 
 }  // namespace aa
@@ -980,17 +823,16 @@ static int launch_bwd(const BwdParams &p, int mode, cudaStream_t st) {
 using namespace aa;
 
 extern "C" int aa_logprob_set_tuning(int variant, int ctas_per_sm) {
-  AA_REQUIRE(variant >= 0 && variant < 100 && variant % 10 <= 3, AA_ERR_ARG,
-             "aa_logprob_set_tuning: variant = kernel digit (0..3) + 10 * shape code");
+  AA_REQUIRE(variant >= 0 && variant <= 3, AA_ERR_ARG,
+             "aa_logprob_set_tuning: variant = 0 / 3 (by row length), 1 (ring) or 2 (LDG)");
   g_variant = variant;
   g_ctas_per_sm = ctas_per_sm;
-  g_bwd_variant = -1;
   return AA_OK;
 }
 
 extern "C" int aa_logprob_set_tuning_bwd(int variant, int ctas_per_sm) {
-  AA_REQUIRE(variant >= -1 && variant < 100 && (variant < 0 || variant % 10 <= 3), AA_ERR_ARG,
-             "aa_logprob_set_tuning_bwd: variant = -1 (follow forward) or kernel + 10 * shape code");
+  AA_REQUIRE(variant == -1 || variant == 0 || variant == 1 || variant == 3, AA_ERR_ARG,
+             "aa_logprob_set_tuning_bwd: variant = -1 / 0 / 1 (TMA-staged) or 3 (LDG row kernel)");
   g_bwd_variant = variant;
   g_bwd_ctas_per_sm = ctas_per_sm;
   return AA_OK;
@@ -1094,7 +936,7 @@ extern "C" int aa_logprob_bwd(const void *logits, int logits_dtype, int64_t row_
               n_rows, seg_tile_row, stat_max, stat_logsum, grad_rows, grad_rows_dtype, grad_seg,
               grad_scale, grad_scale_dtype, grad_logits, grad_row_stride, n_tile_rows, 0.0f, extra_zero_rows, n_extra_zero_rows};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (row_scratch && (bwd_variant() % 10) <= 1) {  // kernel digit 0 / 1: TMA-staged backward (the default)
+  if (row_scratch && bwd_variant() != 3) {  // TMA-staged backward (the default); tuning variant 3 takes the LDG kernel
     AA_REQUIRE((reinterpret_cast<uintptr_t>(row_scratch) & 15) == 0, AA_ERR_ALIGN,
                "aa_logprob_bwd: row_scratch must be 16-byte aligned");
     RowRec *rec = static_cast<RowRec *>(row_scratch);
@@ -1102,16 +944,6 @@ extern "C" int aa_logprob_bwd(const void *logits, int logits_dtype, int64_t row_
       case AA_BF16: return launch_bwd_tma<__nv_bfloat16>(p, mode, rec, st);
       case AA_F16: return launch_bwd_tma<__half>(p, mode, rec, st);
       case AA_F32: return launch_bwd_tma<float>(p, mode, rec, st);
-    }
-  }
-  if (row_scratch && (bwd_variant() % 10) == 2) {  // kernel digit 2: address-ordered chunked sweep (an experiment, slower)
-    AA_REQUIRE((reinterpret_cast<uintptr_t>(row_scratch) & 15) == 0, AA_ERR_ALIGN,
-               "aa_logprob_bwd: row_scratch must be 16-byte aligned");
-    RowRec *rec = static_cast<RowRec *>(row_scratch);
-    switch (logits_dtype) {
-      case AA_BF16: return launch_bwd_chunk<__nv_bfloat16>(p, mode, rec, st);
-      case AA_F16: return launch_bwd_chunk<__half>(p, mode, rec, st);
-      case AA_F32: return launch_bwd_chunk<float>(p, mode, rec, st);
     }
   }
   switch (logits_dtype) {

@@ -16,7 +16,7 @@
 //   per scored row, one CTA:   phase A  stream the row through a shared-memory ring (cp.async.bulk), online softmax
 //                              boundary one thread: log-prob -> actor_token() -> g = d loss / d log-prob
 //                              phase B  stream the SAME row again -- 304 KB at V = 152064, read a few microseconds ago
-//                                       by this CTA, so the copy engine finds it in the 126 MB L2 (phase-A loads carry
+//                                       by this CTA, so the copy engine finds it in the 50 MB L2 (phase-A loads carry
 //                                       an L2 evict_last policy, phase-B loads and the stores evict_first) --
 //                                       g * (onehot - softmax) in place in shared memory, cp.async.bulk stores.
 //
@@ -25,7 +25,6 @@
 // log-probs this kernel writes (a 16 us launch); autograd's backward returns the tile produced here, multiplied in
 // place by the incoming scalar only if that is not 1 (aa_scale_tile: every CTA reads the scalar and leaves).
 #include <atomic>
-#include <cstdlib>
 
 #include "common.cuh"
 #include "logprob_math.cuh"
@@ -58,8 +57,7 @@ struct FusedActorParams {
   int64_t grad_row_stride;
   int32_t *status;
   float log2e, zero;
-  int hint;  // L2 policy of the bulk copies: 0 none, 1 phase A evict_last / phase B + stores evict_first
-  int interleave;  // > 0: size of the persistent grid -- the work list alternates `interleave` scored rows / zero rows
+  int interleave;  // size of the persistent grid: the work list alternates `interleave` scored rows / zero rows
   // kind 1 (cross-entropy, aa_logprob_ce_fused): every row whose label != ignore_index has the SAME upstream gradient
   // *ce_coeff = -loss_scale / n_valid (written by ce_coeff_kernel); old / adv / mask are unused
   // kind 2 (GRPO, aa_logprob_grpo_fused): old = reference log-probs, adv = ONE fp32 advantage per segment, clip = beta,
@@ -75,7 +73,7 @@ struct FusedActorParams {
 // instruction issue / MUFU (two exp per logit in one kernel), the zero rows are pure copy-engine stores: the list
 // alternates G scored rows and G zero rows (G = grid size), so every CTA's producer lane fires the stores of a zero
 // row while its consumer warps are still busy with the scored row before it -- the zero rows ride in the DRAM
-// bandwidth the compute-bound rows leave unused.  (interleave == 0: scored rows first, zero rows after, as in K1b.)
+// bandwidth the compute-bound rows leave unused.
 struct __align__(16) FusedRec {
   int64_t x_off;    // element offset of the logits row
   int64_t g_row;    // row index in the gradient tile
@@ -105,18 +103,14 @@ __global__ void __launch_bounds__(256) fused_actor_prep_kernel(const FusedActorP
   const int64_t j = work - __ldg(p.seg_tile_row + seg);
   const bool scored = j >= 0 && j < n;
   const int64_t scored_before = first_flat + min(max(j, static_cast<int64_t>(0)), n);
+  const int64_t G = p.interleave, Z = static_cast<int64_t>(p.map.n_seg) * p.seq - total;
   int64_t slot;
-  if (p.interleave > 0) {
-    const int64_t G = p.interleave, Z = static_cast<int64_t>(p.map.n_seg) * p.seq - total;
-    if (scored) {
-      const int64_t i = first_flat + j;
-      slot = i + min((i / G) * G, Z);                // zero rows of the earlier rounds come first
-    } else {
-      const int64_t z = work - scored_before;
-      slot = min((z / G + 1) * G, total) + z;        // scored rows of this and the earlier rounds come first
-    }
+  if (scored) {
+    const int64_t i = first_flat + j;
+    slot = i + min((i / G) * G, Z);                // zero rows of the earlier rounds come first
   } else {
-    slot = scored ? first_flat + j : total + (work - scored_before);
+    const int64_t z = work - scored_before;
+    slot = min((z / G + 1) * G, total) + z;        // scored rows of this and the earlier rounds come first
   }
   FusedRec r;
   r.x_off = 0; r.g_row = work; r.out_idx = 0; r.old = 0.f; r.adv = 0.f; r.g_rs = 0.f; r.y = -2; r.flat = 0; r.on = 0;
@@ -165,11 +159,6 @@ __device__ __forceinline__ void bulk_g2s_hint(void *dst_smem, const void *src_gm
       "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
       : "memory");
 }
-__device__ __forceinline__ void bulk_s2g(void *dst_gmem, const void *src_smem, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst_gmem), "r"(smem_u32(src_smem)),
-               "r"(bytes)
-               : "memory");
-}
 __device__ __forceinline__ void bulk_s2g_hint(void *dst_gmem, const void *src_smem, uint32_t bytes, uint64_t pol) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(dst_gmem),
                "r"(smem_u32(src_smem)), "r"(bytes), "l"(pol)
@@ -182,12 +171,9 @@ __device__ __forceinline__ void commit_group() { asm volatile("cp.async.bulk.com
 // (+ two ALU unpacks) instead of the Veltkamp split on the FMA pipe (FFMA2 + 2 FADD2): the same bits for finite values,
 // -inf logits need no clamp (HMNMX2), and three instructions per pair move from the FMA-heavy pipe -- the busiest one
 // of this kernel, 57 % -- to the ALU pipe (36 %).  K1b keeps the split: it is HBM-bound with the XU pipe as runner-up.
-#ifndef AA_K1F_PACK_ROUND
-#define AA_K1F_PACK_ROUND 1
-#endif
 template <typename T, bool FAITHFUL>
 __device__ __forceinline__ uint4 vec_grad_pk(const uint4 &v, const GradConsts &k) {
-  if constexpr (sizeof(T) == 4 || !FAITHFUL || !AA_K1F_PACK_ROUND) {
+  if constexpr (sizeof(T) == 4 || !FAITHFUL) {
     return vec_grad<T, FAITHFUL>(v, k);
   } else {
     const uint32_t w[4] = {v.x, v.y, v.z, v.w};
@@ -248,13 +234,9 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
     auto retire_one = [&]() {
       const int s = rt_stage;
       bulk::mbar_wait(done + s, rt_phase);
-      if (st_bytes[s]) {
-        void *dst = reinterpret_cast<void *>(st_dst[s]);
-        if (p.hint)
-          bulk::bulk_s2g_hint(dst, ring + static_cast<size_t>(s) * STAGE_VECS, st_bytes[s], pol_drop);
-        else
-          bulk::bulk_s2g(dst, ring + static_cast<size_t>(s) * STAGE_VECS, st_bytes[s]);
-      }
+      if (st_bytes[s])
+        bulk::bulk_s2g_hint(reinterpret_cast<void *>(st_dst[s]), ring + static_cast<size_t>(s) * STAGE_VECS, st_bytes[s],
+                            pol_drop);
       bulk::commit_group();  // one (possibly empty) group per chunk: wait_group.read below counts chunks
       --inflight;
       if (++rt_stage == STAGES) {
@@ -269,10 +251,7 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
     auto zero_some = [&](int max_chunks) {
       while (zq_left > 0 && max_chunks-- > 0) {
         const int n = min(STAGE_VECS, zq_left);
-        if (p.hint)
-          bulk::bulk_s2g_hint(zq_dst, zero_buf, static_cast<uint32_t>(n) * 16u, pol_drop);
-        else
-          bulk::bulk_s2g(zq_dst, zero_buf, static_cast<uint32_t>(n) * 16u);
+        bulk::bulk_s2g_hint(zq_dst, zero_buf, static_cast<uint32_t>(n) * 16u, pol_drop);
         zq_dst += n;
         zq_left -= n;
       }
@@ -306,11 +285,8 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
             st_dst[s] = reinterpret_cast<uint64_t>(gbody + v0);
             st_bytes[s] = ph ? bytes : 0u;
             bulk::mbar_expect_tx(full + s, bytes);
-            if (p.hint)
-              bulk::bulk_g2s_hint(ring + static_cast<size_t>(s) * STAGE_VECS, xbody + v0, bytes, full + s,
-                                  ph ? pol_drop : pol_keep);
-            else
-              bulk::bulk_g2s(ring + static_cast<size_t>(s) * STAGE_VECS, xbody + v0, bytes, full + s);
+            bulk::bulk_g2s_hint(ring + static_cast<size_t>(s) * STAGE_VECS, xbody + v0, bytes, full + s,
+                                ph ? pol_drop : pol_keep);
             ++inflight;
             if (++ld_stage == STAGES) ld_stage = 0;
             zero_some(1);  // joins the group of the next retired chunk
@@ -563,25 +539,14 @@ __global__ void __launch_bounds__(256) scale_tile_kernel(T *__restrict__ tile, i
 }
 
 // ---- host side ----------------------------------------------------------------------------
-// Shape of the persistent kernel (experiment switch AA_B200_FUSED_SHAPE, read once), zero rows interleaved:
-//   6 (default): 992 consumers (31 warps + the producer warp = 1024 threads), 6 x 31 KB stages, lag 4, 1 CTA/SM
-//   1: 512 consumers, 8 x 16 KB, lag 6, 1 CTA/SM           4: 992 consumers, 8 x 15.5 KB, lag 6, 1 CTA/SM
-//   0: 256 consumers, 8 x 8 KB, lag 6, 2 CTAs/SM           5: 480 consumers, 8 x 7.5 KB, 2 CTAs/SM
-//   2: 256 consumers, 4 x 8 KB, lag 3, 3 CTAs/SM (K1b's shape)     3: 256 consumers, 8 x 16 KB, 1 CTA/SM
-//   7: 736 consumers, 8 x 11.5 KB, 1 CTA/SM
-// One CTA per SM keeps 132 rows (40 MB of 152064-token bf16 rows) between the two passes, inside the 50 MB L2, so the
-// second pass is an L2 hit; with two rows in flight per SM part of it misses.  The kernel is bound by the MUFU /
-// conversion pipe and instruction issue (two exp per logit + the bf16 pack) rather than by HBM.  AA_B200_FUSED_CTAS
-// overrides the CTAs/SM, AA_B200_FUSED_HINT=0 drops the L2 policies, AA_B200_FUSED_INTERLEAVE=0 puts the zero rows
-// after the scored rows.
-static int env_int(const char *name, int dflt) {
-  const char *v = std::getenv(name);
-  return (v && *v) ? std::atoi(v) : dflt;
-}
-
-template <typename T, int CONSUMERS, int STAGES, int UNROLL, int LAG>
-static int launch_fused_shape(const FusedActorParams &p, int mode, int per_sm, FusedRec *rec, int64_t n_work,
-                              cudaStream_t st) {
+// One launch shape: 992 consumers (31 warps + the producer warp = 1024 threads), 6 x 31 KB stages, lag 4, 1 CTA/SM, zero
+// rows interleaved with the scored rows.  One CTA per SM keeps 132 rows (40 MB of 152064-token bf16 rows) between the
+// two passes, inside the 50 MB L2, so the second pass is an L2 hit; with two rows in flight per SM part of it misses.
+// The kernel is bound by the MUFU / conversion pipe and instruction issue (two exp per logit + the bf16 pack) rather
+// than by HBM.
+template <typename T>
+static int launch_fused_kernel(const FusedActorParams &p, int mode, FusedRec *rec, int64_t n_work, cudaStream_t st) {
+  constexpr int CONSUMERS = 992, STAGES = 6, UNROLL = 2, LAG = 4;
   constexpr size_t smem = static_cast<size_t>(STAGES + 1) * CONSUMERS * UNROLL * 16 + STAGES * (8 + 8 + 8 + 4) + 16;
   const bool faithful = (mode == AA_MODE_FAITHFUL) && sizeof(T) == 2;
   auto kf = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, true>;
@@ -596,11 +561,10 @@ static int launch_fused_shape(const FusedActorParams &p, int mode, int per_sm, F
     }
     configured.store(true, std::memory_order_relaxed);
   }
-  int64_t grid = static_cast<int64_t>(sm_count()) * per_sm;
+  int64_t grid = sm_count();
   if (grid > n_work) grid = n_work;
-  static const int interleave = env_int("AA_B200_FUSED_INTERLEAVE", 1);
   FusedActorParams q = p;
-  q.interleave = interleave ? static_cast<int>(grid) : 0;
+  q.interleave = static_cast<int>(grid);
   const dim3 pgrid((q.seq + 255) / 256, q.map.n_seg);
   fused_actor_prep_kernel<<<pgrid, 256, 0, st>>>(q, rec);
   int rc = check_launch("aa_logprob_actor_fused(prep)");
@@ -612,21 +576,38 @@ static int launch_fused_shape(const FusedActorParams &p, int mode, int per_sm, F
   return check_launch("aa_logprob_actor_fused");
 }
 
-template <typename T>
-static int launch_fused(const FusedActorParams &p, int mode, FusedRec *rec, int64_t n_work, cudaStream_t st) {
-  static const int shape = env_int("AA_B200_FUSED_SHAPE", 6);
-  static const int ctas = env_int("AA_B200_FUSED_CTAS", 0);
-  switch (shape) {
-    case 0: return launch_fused_shape<T, 256, 8, 2, 6>(p, mode, ctas > 0 ? ctas : 2, rec, n_work, st);
-    case 1: return launch_fused_shape<T, 512, 8, 2, 6>(p, mode, ctas > 0 ? ctas : 1, rec, n_work, st);
-    case 2: return launch_fused_shape<T, 256, 4, 2, 3>(p, mode, ctas > 0 ? ctas : 3, rec, n_work, st);
-    case 3: return launch_fused_shape<T, 256, 8, 4, 6>(p, mode, ctas > 0 ? ctas : 1, rec, n_work, st);
-    case 4: return launch_fused_shape<T, 992, 8, 1, 6>(p, mode, ctas > 0 ? ctas : 1, rec, n_work, st);
-    case 5: return launch_fused_shape<T, 480, 8, 1, 6>(p, mode, ctas > 0 ? ctas : 2, rec, n_work, st);
-    case 7: return launch_fused_shape<T, 736, 8, 1, 6>(p, mode, ctas > 0 ? ctas : 1, rec, n_work, st);
-    default: break;
+static int launch_fused(const FusedActorParams &p, int logits_dtype, int mode, FusedRec *rec, int64_t n_work,
+                        cudaStream_t st) {
+  switch (logits_dtype) {
+    case AA_BF16: return launch_fused_kernel<__nv_bfloat16>(p, mode, rec, n_work, st);
+    case AA_F16: return launch_fused_kernel<__half>(p, mode, rec, n_work, st);
+    case AA_F32: return launch_fused_kernel<float>(p, mode, rec, n_work, st);
   }
-  return launch_fused_shape<T, 992, 6, 2, 4>(p, mode, ctas > 0 ? ctas : 1, rec, n_work, st);
+  return AA_ERR_DTYPE;
+}
+
+// The fields every kind sets; each entry point adds its own and the kind.
+static FusedActorParams fused_params(const void *logits, int64_t row_stride, int32_t V, const int64_t *labels,
+                                     int32_t n_segments, const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                                     const int64_t *seg_out_off, const int64_t *seg_cum, const int64_t *seg_tile_row,
+                                     int64_t n_tile_rows, void *log_probs, int lp_dtype, void *grad_logits,
+                                     int64_t grad_row_stride, int32_t *status) {
+  FusedActorParams p{};
+  p.logits = logits;
+  p.row_stride = row_stride;
+  p.V = V;
+  p.labels = labels;
+  p.map = RowMap{seg_logit_off, seg_label_off, seg_out_off, seg_cum, n_segments};
+  p.seg_tile_row = seg_tile_row;
+  p.seq = static_cast<int>(n_tile_rows / n_segments);
+  p.out = log_probs;
+  p.out_dtype = lp_dtype;
+  p.grad = grad_logits;
+  p.grad_row_stride = grad_row_stride;
+  p.status = status;
+  p.log2e = kLog2e;
+  p.zero = 0.0f;
+  return p;
 }
 
 static inline bool fdtype_ok(int dt) { return dt == AA_BF16 || dt == AA_F16 || dt == AA_F32; }
@@ -659,21 +640,25 @@ extern "C" int aa_logprob_actor_fused(const void *logits, int logits_dtype, int6
   AA_REQUIRE(n_tile_rows / n_segments < (1ll << 31) && n_tile_rows < (1ll << 31), AA_ERR_ARG,
              "aa_logprob_actor_fused: tile too large");
   const bool f = (mode == AA_MODE_FAITHFUL);
-  static const int hint = env_int("AA_B200_FUSED_HINT", 1);
-  FusedActorParams p{logits, row_stride, V, labels,
-                     RowMap{seg_logit_off, seg_label_off, seg_out_off, seg_cum, n_segments}, seg_tile_row,
-                     static_cast<int>(n_tile_rows / n_segments), log_probs, lp_dtype, stat_max, stat_logsum,
-                     old_log_probs, old_stride, advantages, adv_stride, adv_dtype, mask, mask_stride, W,
-                     clip_range_ratio, f ? lp_dtype : AA_F32, f ? promote_dt(lp_dtype, adv_dtype) : AA_F32,
-                     grad_logits, grad_row_stride, status, kLog2e, 0.0f, hint, 0, 0, 0, nullptr, nullptr, nullptr};
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  FusedRec *rec = static_cast<FusedRec *>(row_scratch);
-  switch (logits_dtype) {
-    case AA_BF16: return launch_fused<__nv_bfloat16>(p, mode, rec, n_tile_rows, st);
-    case AA_F16: return launch_fused<__half>(p, mode, rec, n_tile_rows, st);
-    case AA_F32: return launch_fused<float>(p, mode, rec, n_tile_rows, st);
-  }
-  return AA_ERR_DTYPE;
+  FusedActorParams p = fused_params(logits, row_stride, V, labels, n_segments, seg_logit_off, seg_label_off, seg_out_off,
+                                    seg_cum, seg_tile_row, n_tile_rows, log_probs, lp_dtype, grad_logits,
+                                    grad_row_stride, status);
+  p.kind = 0;
+  p.stat_max = stat_max;
+  p.stat_logsum = stat_logsum;
+  p.old = old_log_probs;
+  p.old_stride = old_stride;
+  p.adv = advantages;
+  p.adv_stride = adv_stride;
+  p.adv_dtype = adv_dtype;
+  p.mask = mask;
+  p.mask_stride = mask_stride;
+  p.W = W;
+  p.clip = clip_range_ratio;
+  p.rx = f ? lp_dtype : AA_F32;
+  p.rp = f ? promote_dt(lp_dtype, adv_dtype) : AA_F32;
+  return launch_fused(p, logits_dtype, mode, static_cast<FusedRec *>(row_scratch), n_tile_rows,
+                      static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int aa_logprob_ce_fused(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
@@ -691,23 +676,17 @@ extern "C" int aa_logprob_ce_fused(const void *logits, int logits_dtype, int64_t
   AA_REQUIRE((reinterpret_cast<uintptr_t>(row_scratch) & 15) == 0, AA_ERR_ALIGN,
              "aa_logprob_ce_fused: row_scratch must be 16-byte aligned");
   AA_REQUIRE(n_tile_rows < (1ll << 31), AA_ERR_ARG, "aa_logprob_ce_fused: tile too large");
-  static const int hint = env_int("AA_B200_FUSED_HINT", 1);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ce_coeff_kernel<<<1, 1024, 0, st>>>(labels, n_labels, ignore_index, loss_scale, coeff_scratch);
   int rc = check_launch("aa_logprob_ce_fused(count)");
   if (rc) return rc;
-  FusedActorParams p{logits, row_stride, V, labels,
-                     RowMap{seg_logit_off, seg_label_off, seg_out_off, seg_cum, n_segments}, seg_tile_row,
-                     static_cast<int>(n_tile_rows / n_segments), log_probs, AA_F32, nullptr, nullptr,
-                     nullptr, 0, nullptr, 0, AA_F32, nullptr, 0, 0, 0.f, AA_F32, AA_F32,
-                     grad_logits, grad_row_stride, status, kLog2e, 0.0f, hint, 0, 1, ignore_index, coeff_scratch, nullptr, nullptr};
-  FusedRec *rec = static_cast<FusedRec *>(row_scratch);
-  switch (logits_dtype) {
-    case AA_BF16: return launch_fused<__nv_bfloat16>(p, AA_MODE_F32, rec, n_tile_rows, st);
-    case AA_F16: return launch_fused<__half>(p, AA_MODE_F32, rec, n_tile_rows, st);
-    case AA_F32: return launch_fused<float>(p, AA_MODE_F32, rec, n_tile_rows, st);
-  }
-  return AA_ERR_DTYPE;
+  FusedActorParams p = fused_params(logits, row_stride, V, labels, n_segments, seg_logit_off, seg_label_off, seg_out_off,
+                                    seg_cum, seg_tile_row, n_tile_rows, log_probs, AA_F32, grad_logits,
+                                    grad_row_stride, status);
+  p.kind = 1;
+  p.ignore_index = ignore_index;
+  p.ce_coeff = coeff_scratch;
+  return launch_fused(p, logits_dtype, AA_MODE_F32, static_cast<FusedRec *>(row_scratch), n_tile_rows, st);
 }
 
 extern "C" int aa_logprob_grpo_fused(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
@@ -729,24 +708,23 @@ extern "C" int aa_logprob_grpo_fused(const void *logits, int logits_dtype, int64
              "aa_logprob_grpo_fused: row_scratch must be 16-byte aligned");
   AA_REQUIRE(n_tile_rows < (1ll << 31), AA_ERR_ARG, "aa_logprob_grpo_fused: tile too large");
   const bool f = (mode == AA_MODE_FAITHFUL);
-  static const int hint = env_int("AA_B200_FUSED_HINT", 1);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   grpo_mask_kernel<128><<<n_segments, 128, 0, st>>>(completion_tokens, tok_stride, n_segments, K, eos_id, row_end, total, counter);
   int rc = check_launch("aa_logprob_grpo_fused(mask)");
   if (rc) return rc;
-  FusedActorParams p{logits, row_stride, V, labels,
-                     RowMap{seg_logit_off, seg_label_off, seg_out_off, seg_cum, n_segments}, seg_tile_row,
-                     static_cast<int>(n_tile_rows / n_segments), log_probs, lp_dtype, nullptr, nullptr,
-                     ref_log_probs, ref_stride, advantages, 0, AA_F32, nullptr, 0, K, beta, f ? lp_dtype : AA_F32,
-                     f ? lp_dtype : AA_F32, grad_logits, grad_row_stride, status, kLog2e, 0.0f, hint, 0, 2, 0, nullptr,
-                     row_end, total};
-  FusedRec *rec = static_cast<FusedRec *>(row_scratch);
-  switch (logits_dtype) {
-    case AA_BF16: return launch_fused<__nv_bfloat16>(p, mode, rec, n_tile_rows, st);
-    case AA_F16: return launch_fused<__half>(p, mode, rec, n_tile_rows, st);
-    case AA_F32: return launch_fused<float>(p, mode, rec, n_tile_rows, st);
-  }
-  return AA_ERR_DTYPE;
+  FusedActorParams p = fused_params(logits, row_stride, V, labels, n_segments, seg_logit_off, seg_label_off, seg_out_off,
+                                    seg_cum, seg_tile_row, n_tile_rows, log_probs, lp_dtype, grad_logits,
+                                    grad_row_stride, status);
+  p.kind = 2;
+  p.old = ref_log_probs;
+  p.old_stride = ref_stride;
+  p.adv = advantages;
+  p.clip = beta;
+  p.rx = f ? lp_dtype : AA_F32;
+  p.rp = f ? lp_dtype : AA_F32;
+  p.row_end = row_end;
+  p.total = total;
+  return launch_fused(p, logits_dtype, mode, static_cast<FusedRec *>(row_scratch), n_tile_rows, st);
 }
 
 extern "C" int aa_scale_tile(void *tile, int dtype, int64_t n, const void *scale, int scale_dtype, void *stream) {

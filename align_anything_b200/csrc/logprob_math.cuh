@@ -46,9 +46,6 @@ __device__ __forceinline__ float vec_max<float>(const uint4 &v) {
                fmaxf(__uint_as_float(v.z), __uint_as_float(v.w)));
 }
 
-#ifndef AA_FWD_POLY_WORDS
-#define AA_FWD_POLY_WORDS 0  // words (of 4 per 16-B vector) whose exp2 runs on the FMA pipe instead of MUFU
-#endif
 // acc += 2^((x - mref)*log2e) for the 8 (or 4) elements of the vector, two lanes at a time (f32x2).
 // Subtract first, then scale: x - m is exact for the maximum, so its term is exactly 1 (common.cuh).
 template <typename T>
@@ -62,8 +59,7 @@ __device__ __forceinline__ void vec_expsum(const uint4 &v, f32x2 mref2, f32x2 L2
     for (int i = 0; i < 4; ++i) {
       float lo, hi;
       unpack2<T>(w[i], lo, hi);
-      const f32x2 t = f2_mul(f2_sub(f2_pack(lo, hi), mref2), L2);
-      const f32x2 e = (i >= 4 - AA_FWD_POLY_WORDS) ? f2_ex2_poly(t) : f2_ex2(t);
+      const f32x2 e = f2_ex2(f2_mul(f2_sub(f2_pack(lo, hi), mref2), L2));
       if (i & 1)
         acc1 = f2_add(acc1, e);
       else

@@ -70,16 +70,16 @@ int aa_abi_version(void);
 const char *aa_last_error(void);
 /* Number of SMs / max dynamic smem of the current device (for host-side grid sizing). */
 int aa_device_info(int *sm_count, int *max_smem_optin);
-/* Tuning / diagnostic knobs (process-wide).  variant = kernel digit + 10 * shape code.
- *   forward  kernel digit: 0 / 3 = chosen by row length (default), 1 = cp.async.bulk ring through shared memory,
- *            2 = vectorised LDG; no shape codes (each kernel has one launch shape, grid = resident CTAs).
- *   backward kernel digit: 0 / 1 = TMA-staged (cp.async.bulk loads AND stores through a shared-memory ring;
- *            the default whenever row_scratch is given), 2 = experimental address-ordered chunked sweep,
- *            3 = one-CTA-per-row LDG/STG kernel (also used when row_scratch == NULL);
- *            shape (TMA): 0 = 4 stages x 8 KB, lag 3, 3 CTAs/SM (default); see logprob.cu for the others.
- * ctas_per_sm <= 0 keeps the default persistent-grid size. */
+/* Tuning / diagnostic knobs (process-wide).  Each kernel has one launch shape; the variant only picks the kernel.
+ *   K1 forward (aa_logprob_set_tuning): 0 / 3 = chosen by row length (default), 1 = cp.async.bulk ring through
+ *            shared memory, 2 = vectorised LDG; the grid is the resident CTA count.
+ *   K1b backward (aa_logprob_set_tuning_bwd): -1 / 0 / 1 = TMA-staged (cp.async.bulk loads AND stores through a
+ *            shared-memory ring, 4 stages x 8 KB, lag 3, 3 CTAs/SM; the default whenever row_scratch is given),
+ *            3 = one-CTA-per-row LDG/STG kernel (also used when row_scratch == NULL).
+ * Any other variant is AA_ERR_ARG.  ctas_per_sm <= 0 keeps the default persistent-grid size; the forward's can only
+ * lower it. */
 int aa_logprob_set_tuning(int variant, int ctas_per_sm);
-/* Same, for K1b only (variant -1: follow aa_logprob_set_tuning). */
+/* Same, for K1b only; the two settings are independent. */
 int aa_logprob_set_tuning_bwd(int variant, int ctas_per_sm);
 
 /* ---------------------------------------------------------------------------------------
@@ -129,8 +129,9 @@ int aa_logprob_fwd(const void *logits, int logits_dtype, int64_t row_stride, int
  * row_scratch: 16-byte aligned device scratch of 32 bytes per work row (n_tile_rows, or
  * n_rows + n_extra_zero_rows when n_tile_rows == 0).  With it the backward is TMA-staged: a tiny prep kernel resolves every row into a
  * 32-byte record, then a persistent kernel moves the tile with cp.async.bulk in both directions through
- * a shared-memory ring (6.48 TB/s sustained at V = 128257 vs 5.8 TB/s for the LDG/STG kernel that runs
- * when row_scratch == NULL).
+ * a shared-memory ring (6.48 TB/s sustained at V = 128257 vs 5.8 TB/s for the LDG/STG kernel).
+ * row_scratch == NULL (or tuning variant 3) runs the one-CTA-per-row LDG/STG kernel, which computes the
+ * same tile bit for bit.
  * Algorithmic HBM traffic: 2 * V * sizeof(logit) per scored row (+ V * sizeof per zero row).
  * ------------------------------------------------------------------------------------- */
 int aa_logprob_bwd(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,

@@ -135,6 +135,9 @@ def test_argument_errors_need_no_gpu():
     assert rc == -2 and b'bad sizes' in lib.aa_last_error()
     rc = lib.aa_logprob_set_tuning(7, 0)  # kernel digit 7 is invalid
     assert rc == -2
+    assert lib.aa_logprob_set_tuning(12, 0) == -2  # a variant names a kernel (0..3); there are no shape codes
+    assert lib.aa_logprob_set_tuning_bwd(2, 0) == -2  # backward kernels: -1 / 0 / 1 (TMA-staged), 3 (LDG)
+    assert lib.aa_logprob_set_tuning_bwd(11, 0) == -2
     with pytest.raises(RuntimeError):
         _lib.check(rc)
     # entry points added later in the round: argument validation happens before any CUDA call
