@@ -64,6 +64,8 @@ _SIGS = {
     'aa_ppo_prep': (c_int, [_P, _P, c_int, c_int64, _P, _P, c_int, c_int64, _P, c_int64, c_int32, c_int32,
                             c_int32, c_float, c_float, c_float, c_float, c_int, _P, c_int, _P, _P, c_int, _P,
                             _P, _P]),
+    'aa_ppo_returns': (c_int, [_P, c_int, c_int64, _P, c_int64, c_int32, c_int32, c_int32, c_int, c_int32, c_float,
+                               c_int, c_int, _P, _P, c_int, _P, _P]),
     'aa_ppo_actor_loss': (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, c_int32,
                                   c_int32, c_float, c_int, _P, _P, c_int64, _P, _P, _P]),
     'aa_ppo_critic_loss': (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, c_int32,

@@ -6,6 +6,8 @@
 // K5  aa_ppo_actor_loss  : clipped-ratio surrogate (:291-307) forward + backward in one launch.
 //     aa_ppo_critic_loss : clipped value loss (:510-526) forward + backward in one launch.
 //     aa_masked_mean     : utils/tools.py:460-467.
+// K4r aa_ppo_returns     : Multi-PPO's reinforce / rloo / reinforce_baseline / group_norm returns
+//                          (trainers/text_to_text/multi_ppo.py:510-591) on K4's shaped rewards.
 //     aa_ppo_pack_metrics: the ten local scalars of :360-381 packed for ONE all-reduce.
 //
 // These touch ~10 floats per token: latency-bound, not bandwidth-bound.  The point is launch
@@ -189,6 +191,168 @@ __global__ void __launch_bounds__(32) ppo_prep_kernel(const PrepParams p) {
     rs[5] = static_cast<float>(end);
     rs[6] = 0.f;
     rs[7] = 0.f;
+  }
+}
+
+// ---- K4r: Multi-PPO returns (trainers/text_to_text/multi_ppo.py:510-591) ----------------------------------
+// The four non-GAE estimators.  `rewards` is K4's (B, W) `old_rewards`; the reference masks it, applies the group
+// statistic, then runs `cumulative_returns`, a Python loop over t with a float32 carry.  Group quirk (SURVEY H9): the
+// estimators reshape the (B, W) TOKEN-reward matrix to (-1, n), so a group is n consecutive elements of the flattened
+// tensor -- it may straddle rows, prompt positions take part, pad positions take part as zeros.
+struct ReturnsParams {
+  const void *rew;
+  int rew_dtype;
+  int64_t rew_stride;
+  const uint8_t *mask;
+  int64_t mask_stride;
+  int B, W, start, est, n;
+  float gamma;
+  int r;         // rounding code: the rewards dtype (faithful) or AA_F32
+  int mask_out;  // 1: outputs *= mask (get_advantages_and_returns); 0: cumulative_returns on its own
+  void *adv, *ret;
+  int out_dtype;
+  float *row_stats;
+};
+
+// rewards * sequence_mask at flat index f of the (B, W) matrix (exact: r or a signed zero)
+__device__ __forceinline__ float masked_reward(const ReturnsParams &p, int64_t f) {
+  const int64_t b = f / p.W, t = f - b * p.W;
+  const float r = load_as_float(p.rew, b * p.rew_stride + t, p.rew_dtype);
+  return p.mask[b * p.mask_stride + t] ? r : r * 0.f;
+}
+
+// Welford state of ATen's std reduction (mean, m2, count)
+struct Welford {
+  float mean, m2, nf;
+};
+__device__ __forceinline__ Welford welford_one(float x) { return {x, 0.f, 1.f}; }
+__device__ __forceinline__ Welford welford_combine(Welford a, Welford b) {
+  const float d = __fsub_rn(b.mean, a.mean), nn = __fadd_rn(a.nf, b.nf), r = __fdiv_rn(b.nf, nn);
+  return {__fmaf_rn(d, r, a.mean), __fmaf_rn(__fmul_rn(__fmul_rn(d, d), a.nf), r, __fadd_rn(a.m2, b.m2)), nn};
+}
+
+// Group sum and unbiased std of the n flat elements from g0, in the order ATen's reduction combines them for a
+// contiguous inner dimension of n < 16: bw = largest power of two <= n lanes, lane j holds elements j and j + bw,
+// then a shuffle tree over the lanes.  Larger groups are folded sequentially (the same value up to fp32 rounding).
+__device__ __forceinline__ void group_stats(const ReturnsParams &p, int64_t g0, bool want_std, float &sum, float &sd) {
+  const int n = p.n;
+  if (n >= 16) {
+    Welford w = welford_one(masked_reward(p, g0));
+    sum = w.mean;
+    for (int k = 1; k < n; ++k) {
+      const float v = masked_reward(p, g0 + k);
+      sum = __fadd_rn(sum, v);
+      if (want_std) {
+        const float nf = __fadd_rn(w.nf, 1.f), d = __fsub_rn(v, w.mean);
+        const float m = __fadd_rn(w.mean, __fdiv_rn(d, nf));
+        w = {m, __fmaf_rn(d, __fsub_rn(v, m), w.m2), nf};
+      }
+    }
+    sd = __fsqrt_rn(__fdiv_rn(w.m2, static_cast<float>(n - 1)));
+    return;
+  }
+  const int bw = n >= 8 ? 8 : n >= 4 ? 4 : n >= 2 ? 2 : 1;
+  float s[8];
+  Welford w[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    if (j < bw) {
+      const float a = masked_reward(p, g0 + j);
+      const float b = (j + bw < n) ? masked_reward(p, g0 + j + bw) : 0.f;
+      s[j] = (j + bw < n) ? __fadd_rn(a, b) : a;
+      w[j] = (j + bw < n) ? welford_combine(welford_one(a), welford_one(b)) : welford_one(a);
+    }
+  }
+#pragma unroll
+  for (int off = 1; off < 8; off <<= 1) {
+#pragma unroll
+    for (int j = 0; j + off < 8; j += 2 * off) {
+      if (j + off < bw) {
+        s[j] = __fadd_rn(s[j], s[j + off]);
+        if (want_std) w[j] = welford_combine(w[j], w[j + off]);
+      }
+    }
+  }
+  sum = s[0];
+  sd = want_std ? __fsqrt_rn(__fdiv_rn(w[0].m2, static_cast<float>(n - 1))) : 0.f;
+}
+
+// the estimator's value at flat index f, with the rounding points of the eager ops (r = rounding code):
+//   rloo               : r - round(round(round(sum) - r) * (1 / (n - 1)))   (ATen divides by a scalar via its reciprocal)
+//   reinforce_baseline : r - round(sum * (1 / n))                           (the mean reduction's fp32 factor)
+//   group_norm         : round(r - mean) / round(round(std) + 1e-9)         (std: unbiased, Welford in fp32)
+__device__ __forceinline__ float estimator_value(const ReturnsParams &p, int64_t f) {
+  const float x = masked_reward(p, f);
+  if (p.est == AA_EST_REINFORCE) return x;
+  const int n = p.n, rc = p.r;
+  const int64_t g0 = (f / n) * n;
+  float sum, sd;
+  group_stats(p, g0, p.est == AA_EST_GROUP_NORM, sum, sd);
+  if (p.est == AA_EST_GROUP_NORM) {
+    const float mu = round_to(__fmul_rn(sum, __fdiv_rn(1.f, static_cast<float>(n))), rc);
+    return round_to(__fdiv_rn(round_to(__fsub_rn(x, mu), rc), round_to(__fadd_rn(round_to(sd, rc), 1e-9f), rc)), rc);
+  }
+  if (p.est == AA_EST_RLOO) {
+    const float loo = round_to(__fsub_rn(round_to(sum, rc), x), rc);
+    const float base = round_to(__fmul_rn(loo, __fdiv_rn(1.f, static_cast<float>(n - 1))), rc);
+    return round_to(__fsub_rn(x, base), rc);
+  }
+  const float mu = round_to(__fmul_rn(sum, __fdiv_rn(1.f, static_cast<float>(n))), rc);  // reinforce_baseline
+  return round_to(__fsub_rn(x, mu), rc);
+}
+
+// one warp per sample: the estimator values of positions start..W-1 are staged in shared memory, the float32 carry
+// c = r_t + gamma * c runs in order on one lane (one multiply, one add, each rounded: nothing contracts to an FMA), and
+// all lanes store.  The chain runs over the whole response width: a masked position is `0 * value`, which is NaN where
+// the estimator gave NaN (fp16 group_norm of a constant group: 1e-9 rounds to 0 in fp16), and that reaches every
+// earlier return in the reference too.
+__global__ void __launch_bounds__(32) ppo_returns_kernel(const ReturnsParams p) {
+  extern __shared__ float sh[];
+  const int b = blockIdx.x, lane = threadIdx.x;
+  const int W = p.W, start = p.start, nr = W - start;
+  const uint8_t *mrow = p.mask + b * p.mask_stride;
+  const int64_t row0 = static_cast<int64_t>(b) * W, ao = static_cast<int64_t>(b) * nr;
+  for (int t = start + lane; t < W; t += kWarp) {
+    float v = estimator_value(p, row0 + t);
+    if (!mrow[t]) v = v * 0.f;  // cumulative_returns masks again: `mask * rewards`
+    sh[t - start] = v;
+  }
+  __syncwarp();
+  if (lane == 0) {
+    const float g = p.gamma;
+    float c = 0.f;
+    int t = nr - 1;
+    for (; t >= 3; t -= 4) {
+      const float r0 = sh[t], r1 = sh[t - 1], r2 = sh[t - 2], r3 = sh[t - 3];
+      const float c0 = __fadd_rn(r0, __fmul_rn(g, c));
+      const float c1 = __fadd_rn(r1, __fmul_rn(g, c0));
+      const float c2 = __fadd_rn(r2, __fmul_rn(g, c1));
+      c = __fadd_rn(r3, __fmul_rn(g, c2));
+      sh[t] = round_to(c0, p.r); sh[t - 1] = round_to(c1, p.r); sh[t - 2] = round_to(c2, p.r); sh[t - 3] = round_to(c, p.r);
+    }
+    for (; t >= 0; --t) {
+      c = __fadd_rn(sh[t], __fmul_rn(g, c));
+      sh[t] = round_to(c, p.r);  // `returns[:, t] = cumulative_return` stores in the rewards dtype; the carry stays fp32
+    }
+  }
+  __syncwarp();
+  float sum = 0.f, cnt = 0.f;
+  for (int t = start + lane; t < W; t += kWarp) {
+    const bool on = mrow[t] != 0;
+    const float v = (on || !p.mask_out) ? sh[t - start] : sh[t - start] * 0.f;  // `advantages *= mask`, `returns *= mask`
+    store_from_float(p.adv, ao + (t - start), p.out_dtype, v);
+    store_from_float(p.ret, ao + (t - start), p.out_dtype, v);
+    if (on) {
+      sum += v;
+      cnt += 1.f;
+    }
+  }
+  sum = warp_sum(sum);
+  cnt = warp_sum(cnt);
+  if (lane == 0 && p.row_stats) {  // K4's lanes 3 / 4: masked row means of advantages and returns
+    float *rs = p.row_stats + static_cast<int64_t>(b) * 8;
+    rs[3] = sum / cnt;
+    rs[4] = sum / cnt;
   }
 }
 
@@ -519,6 +683,42 @@ extern "C" int aa_ppo_prep(const void *log_probs, const void *ref_log_probs, int
   }
   ppo_prep_kernel<<<B, 32, smem, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("aa_ppo_prep");
+}
+
+extern "C" int aa_ppo_returns(const void *rewards, int rew_dtype, int64_t rew_row_stride, const uint8_t *mask,
+                              int64_t mask_row_stride, int32_t B, int32_t W, int32_t start, int estimator,
+                              int32_t n_samples_per_prompt, float gamma, int mode, int mask_outputs, void *advantages,
+                              void *returns, int out_dtype, float *row_stats, void *stream) {
+  AA_REQUIRE(B > 0 && W > 0 && start >= 0 && start < W, AA_ERR_ARG, "aa_ppo_returns: bad sizes (B=%d W=%d start=%d)", B,
+             W, start);
+  AA_REQUIRE(rewards && mask && advantages && returns && advantages != returns, AA_ERR_ARG,
+             "aa_ppo_returns: null or aliased pointer");
+  AA_REQUIRE(rew_row_stride >= W && mask_row_stride >= W, AA_ERR_ARG, "aa_ppo_returns: row strides must be >= W");
+  AA_REQUIRE(estimator >= AA_EST_REINFORCE && estimator <= AA_EST_GROUP_NORM, AA_ERR_ARG,
+             "aa_ppo_returns: unknown estimator code %d", estimator);
+  const bool group = estimator != AA_EST_REINFORCE;
+  AA_REQUIRE(n_samples_per_prompt >= (group ? 2 : 1), AA_ERR_ARG,
+             "aa_ppo_returns: n_samples_per_prompt=%d (the group estimators need n > 1)", n_samples_per_prompt);
+  AA_REQUIRE(!group || (static_cast<int64_t>(B) * W) % n_samples_per_prompt == 0, AA_ERR_ARG,
+             "aa_ppo_returns: B*W=%lld is not a multiple of n_samples_per_prompt=%d",
+             static_cast<long long>(B) * W, n_samples_per_prompt);
+  AA_REQUIRE(dtype_ok(rew_dtype) && dtype_ok(out_dtype), AA_ERR_DTYPE, "aa_ppo_returns: bad dtype");
+  const size_t smem = static_cast<size_t>(W - start) * sizeof(float);
+  AA_REQUIRE(smem <= 200 * 1024, AA_ERR_UNSUPPORTED, "aa_ppo_returns: W - start = %d does not fit in shared memory",
+             W - start);
+  const bool f = (mode == AA_MODE_FAITHFUL);
+  ReturnsParams p{rewards, rew_dtype, rew_row_stride, mask, mask_row_stride, B, W, start, estimator,
+                  n_samples_per_prompt, gamma, f ? rew_dtype : AA_F32, mask_outputs != 0, advantages, returns, out_dtype,
+                  row_stats};
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(ppo_returns_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (e != cudaSuccess) {
+      set_error("aa_ppo_returns: %s", cudaGetErrorString(e));
+      return static_cast<int>(e);
+    }
+  }
+  ppo_returns_kernel<<<B, 32, smem, static_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("aa_ppo_returns");
 }
 
 static int promote(int a, int b) { return (a == b) ? a : AA_F32; }

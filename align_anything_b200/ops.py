@@ -21,7 +21,7 @@ from . import _lib as L
 
 __all__ = [
     'gather_log_probabilities', 'masked_mean', 'sequence_log_probs', 'RowPlan', 'DeviceLens', 'DevicePlan', 'as_device_lens', 'rollout_layout', 'response_tail_log_probs', 'response_tail_log_probs_pair', 'dpo_loss_from_log_probs',
-    'dpo_fused_loss', 'score_head', 'score_end', 'kl_rewards_and_gae', 'gae_from_rewards', 'actor_loss', 'critic_loss',
+    'dpo_fused_loss', 'score_head', 'score_end', 'kl_rewards_and_gae', 'gae_from_rewards', 'estimator_returns', 'actor_loss', 'critic_loss',
     'move_padding_left', 'count_nonpad', 'strip_pad_tail', 'ppo_pack_metrics', 'check_status', 'raise_for_status', 'status_lane', 'causal_lm_loss', 'rm_pair_loss', 'group_advantages', 'grpo_loss', 'tail_token_log_probs', 'pair_slices', 'slice_sums', 'tail_rows', 'linear_token_log_probs',
     'sequence_log_probs_from_hidden', 'fused_linear_token_log_probs', 'tail_log_probs_from_hidden', 'tail_actor_loss', 'tail_critic_loss', 'lm_head_weight',
 ]
@@ -1479,6 +1479,59 @@ def gae_from_rewards(values, rewards, sequence_mask, start: int, gamma: float, g
         rew.data_ptr(), L.dtype_code(rew.dtype), adv.data_ptr(), ret.data_ptr(), L.dtype_code(adv_dtype),
         row_stats.data_ptr(), sc['status'].data_ptr(), L.stream_ptr(dev)))
     return adv, ret, row_stats
+
+
+ESTIMATORS = {'reinforce': 0, 'rloo': 1, 'reinforce_baseline': 2, 'group_norm': 3}  # include/aa_b200.h AA_EST_*
+
+
+def estimator_returns(rewards, sequence_mask, start: int, estimator: str, n_samples_per_prompt: int, gamma: float,
+                      mode: str | None = None, row_stats=None, mask_outputs: bool = True):
+    """Multi-PPO's get_advantages_and_returns for the non-GAE estimators (trainers/text_to_text/multi_ppo.py:510-591:
+    the group statistic, then cumulative_returns) in ONE launch (K4r).  `rewards` is the (B, W) output of
+    add_kl_divergence_regularization.  Returns (advantages, returns), both (B, W - start) in the rewards dtype ('f32'
+    mode: fp32).  With `row_stats` (K4's (B, 8) fp32 output) lanes 3 and 4 are overwritten with the masked row means
+    of the new advantages and returns, so ppo_pack_metrics reports them.  mask_outputs=False with 'reinforce' is
+    `cumulative_returns` on its own: the returns are not multiplied by the mask afterwards.
+
+    The grouping is the reference's: `rewards.reshape(-1, n)` of the (B, W) token rewards, i.e. n consecutive flat
+    elements (SURVEY.md H9).  Errors are raised here, before the launch, like the reference raises them."""
+    if estimator == 'gae':
+        raise ValueError("estimator_returns: 'gae' is K4's scan (kl_rewards_and_gae / gae_from_rewards)")
+    if estimator not in ESTIMATORS:
+        raise ValueError(f'Unknown estimator: {estimator}')
+    n = int(n_samples_per_prompt)
+    group = estimator != 'reinforce'
+    if group and n < 2:
+        raise ValueError(f'{estimator} requires n_samples_per_prompt > 1')
+    if n < 1:
+        raise ValueError(f'n_samples_per_prompt must be >= 1, got {n}')
+    if rewards.dim() != 2 or tuple(sequence_mask.shape) != tuple(rewards.shape):
+        raise ValueError(f'rewards {tuple(rewards.shape)} and sequence_mask {tuple(sequence_mask.shape)} must share one '
+                         f'(B, W) shape')
+    B, W = rewards.shape
+    if group and (B * W) % n != 0:  # what `rewards.reshape(-1, n)` raises
+        raise RuntimeError(f"shape '[-1, {n}]' is invalid for input of size {B * W}")
+    if not 0 <= int(start) < W:
+        raise ValueError(f'start={start} must lie in [0, {W})')
+    L.require_cuda(rewards, sequence_mask, row_stats)
+    dev = rewards.device
+    rew = rewards.detach()
+    if rew.dtype not in (torch.float32, torch.bfloat16, torch.float16):
+        rew = rew.float()
+    rew = rew.contiguous()
+    mask = _contiguous_last(sequence_mask.to(torch.bool))
+    mode_code = _mode_code(mode, rew.dtype)
+    out_dtype = rew.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
+    adv = torch.empty((B, W - int(start)), dtype=out_dtype, device=dev)
+    ret = torch.empty((B, W - int(start)), dtype=out_dtype, device=dev)
+    if row_stats is not None and (row_stats.dtype != torch.float32 or tuple(row_stats.shape) != (B, 8)
+                                  or not row_stats.is_contiguous()):
+        raise ValueError(f'row_stats must be a contiguous fp32 (B, 8) tensor, got {row_stats.dtype} {tuple(row_stats.shape)}')
+    L.check(L.lib().aa_ppo_returns(
+        rew.data_ptr(), L.dtype_code(rew.dtype), rew.stride(0), mask.data_ptr(), mask.stride(0), B, W, int(start),
+        ESTIMATORS[estimator], n, float(gamma), mode_code, int(bool(mask_outputs)), adv.data_ptr(), ret.data_ptr(), L.dtype_code(out_dtype),
+        L.ptr(row_stats), L.stream_ptr(dev)))
+    return adv, ret
 
 
 def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=None):

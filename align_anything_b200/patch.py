@@ -10,6 +10,9 @@ swaps, without touching any reference file,
     get_advantages_and_returns, rl_step, ptx_step} of the text / image / audio / video trainers, and the
     multimodal trainers' actor_step (its post-generate bookkeeping); `reward_model_step` and the text trainer's
     actor_step (generate + mask) stay the reference's,
+  * the same methods plus cumulative_returns of the text Multi-PPO trainer (trainers/text_to_text/multi_ppo.py:
+    the five advantage estimators on K4 / K4r); its actor_step, reward_model_step and split_ptx_micro_batches stay
+    the reference's,
   * SupervisedTrainer.{loss, train_step} of the text / image / audio SFT trainers (cross-entropy from K1),
   * GRPOTrainer.{_get_per_token_logps, train_step} and RMTrainer.{loss, train_step} of the text trainers,
   * SimPOTrainer / ORPOTrainer / KTOTrainer.{loss, train_step} (they inherit the patched DPOTrainer.compute_log_probs),
@@ -31,6 +34,7 @@ from .trainers.text_image_to_text.saferlhf import SafeRLHFVTrainer as _SafeV
 from .trainers.text_to_text.dpo import DPOTrainer as _TextDPO
 from .trainers.text_to_text.grpo import GRPOTrainer as _GRPO
 from .trainers.text_to_text.kto import KTOTrainer as _KTO
+from .trainers.text_to_text.multi_ppo import PPOTrainer as _MultiPPO
 from .trainers.text_to_text.orpo import ORPOTrainer as _ORPO
 from .trainers.text_to_text.ppo import PPOTrainer as _TextPPO
 from .trainers.text_to_text.rm import RMTrainer as _RM
@@ -43,7 +47,7 @@ _saved: list[tuple[object, str, object]] = []
 _TOOL_NAMES = ('gather_log_probabilities', 'masked_mean', 'move_padding_left')
 _DPO_METHODS = ('compute_log_probs', 'loss', 'train_step', '_hidden_and_head')
 _PPO_METHODS = ('rollout', 'actor_loss_fn', 'critic_loss_fn', 'add_kl_divergence_regularization',
-                'get_advantages_and_returns', 'rl_step', 'ptx_step')
+                'get_advantages_and_returns', 'rl_step', 'ptx_step', 'cumulative_returns')  # the last: Multi-PPO only
 _SFT_METHODS = ('loss', 'train_step')
 _GRPO_METHODS = ('_get_per_token_logps', 'step_from_rollout', 'train_step')
 _RM_METHODS = ('loss', 'train_step')
@@ -59,6 +63,7 @@ _PPO_TARGETS = {
     'align_anything.trainers.text_image_to_text.ppo': _MMPPO,
     'align_anything.trainers.text_audio_to_text.ppo': _AudioPPO,
     'align_anything.trainers.text_video_to_text.ppo': _MMPPO,
+    'align_anything.trainers.text_to_text.multi_ppo': _MultiPPO,
 }
 _SFT_TARGETS = {
     'align_anything.trainers.text_to_text.sft': _SFT,
@@ -161,7 +166,7 @@ def install(trainers: bool = True, models: bool = True) -> dict[str, list[str]]:
                 setattr(cls, 'mode', None)
                 if modname in _PPO_TARGETS:  # helpers the grafted rl_step calls + the H100-side entry points
                     helpers = ('_actor_logits', '_tail_log_probs', 'score_rollout', 'postprocess_generation')
-                    if src is not _TextPPO:  # multimodal: the post-generate bookkeeping of actor_step is ours too
+                    if src not in (_TextPPO, _MultiPPO):  # multimodal: the post-generate bookkeeping of actor_step is ours too
                         helpers += ('actor_step',)
                     for m in helpers:
                         fn = next((b.__dict__[m] for b in src.__mro__ if m in b.__dict__), None)

@@ -269,6 +269,25 @@ int aa_ppo_prep(const void *log_probs, const void *ref_log_probs, int lp_dtype, 
                 float *row_stats, int32_t *status, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * K4r  Multi-PPO returns, one launch: trainers/text_to_text/multi_ppo.py:510-591
+ * (get_advantages_and_returns + cumulative_returns, a Python loop over t in the reference) for
+ * the four non-GAE estimators.  `rewards` is K4's (B, W) `old_rewards` (row stride in elements),
+ * mask is torch.bool (B, W).  The group estimators reshape the flattened (B, W) token rewards to
+ * (-1, n): a group is n consecutive flat elements, possibly spanning rows (SURVEY.md H9), so
+ * B * W must be a multiple of n.  The carry c = r_t + gamma * c is float32; each c is stored
+ * rounded to the rewards dtype (FAITHFUL) and, with mask_outputs != 0, multiplied by the mask
+ * (get_advantages_and_returns; mask_outputs == 0 is cumulative_returns on its own).
+ *   advantages, returns : (B, W - start) contiguous, `out_dtype` (equal tensors; separate buffers)
+ *   row_stats           : optional fp32 [B][8] in K4's layout; lanes 3 and 4 are overwritten with
+ *                         the masked row means of advantages and returns, the rest is untouched
+ * ------------------------------------------------------------------------------------- */
+enum { AA_EST_REINFORCE = 0, AA_EST_RLOO = 1, AA_EST_REINFORCE_BASELINE = 2, AA_EST_GROUP_NORM = 3 };
+int aa_ppo_returns(const void *rewards, int rew_dtype, int64_t rew_row_stride, const uint8_t *mask,
+                   int64_t mask_row_stride, int32_t B, int32_t W, int32_t start, int estimator,
+                   int32_t n_samples_per_prompt, float gamma, int mode, int mask_outputs, void *advantages,
+                   void *returns, int out_dtype, float *row_stats, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * K5  PPO losses, forward AND backward in one launch each (the backward is elementwise).
  * actor : trainers/text_to_text/ppo.py:291-307  (+ utils/tools.py:460-467 masked_mean)
  * critic: trainers/text_to_text/ppo.py:510-526
