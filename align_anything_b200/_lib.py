@@ -56,6 +56,7 @@ _SIGS = {
     'aa_pair_slices': (c_int, [_P, c_int64, _P, c_int, c_int64, c_int32, c_int32, _P, _P, _P]),
     'aa_slice_sums': (c_int, [_P, c_int, c_int64, c_int32, c_int32, _P, c_int, _P, _P]),
     'aa_rm_pair_loss': (c_int, [_P, c_int32, c_float, _P, _P, _P]),
+    'aa_cost_pair_loss': (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int32, c_float, c_float, c_int, _P, _P, _P, _P]),
     'aa_score_head_fwd': (c_int, [_P, c_int, c_int64, c_int32, c_int64, _P, _P, c_int, c_int, _P]),
     'aa_score_end': (c_int, [_P, c_int, c_int64, _P, c_int, c_int64, c_int32, c_int32, _P, _P, _P, c_int,
                              c_int64, c_int64, c_int32, _P, _P, _P]),

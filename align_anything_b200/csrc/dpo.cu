@@ -299,6 +299,85 @@ __global__ void __launch_bounds__(THREADS)
   }
 }
 
+// ---- cost-model pairwise loss (Safe RLHF's cost model; sibling of the RM loss) -----------------------------
+// trainers/text_to_text/cost_model.py:97-144, with h / l the higher- / lower-cost end scores (dtype E):
+//   cost   = -mean(logsigmoid(h * sb)) - mean(logsigmoid(l * sw))      sb / sw: is_better_safe / is_worse_safe
+//   loss   = scale * cost - mean(logsigmoid(h - l)) [+ reg * mean(square(stack([l, h])))]
+// The signs arrive cast to their product dtype Pb = result_type(h, sb) (E or fp32), likewise Pw; the cost and the
+// loss are then in Pc = promote(Pb, Pw).  FAITHFUL rounds to E / Pb / Pw / Pc wherever the eager ops round; every
+// product is __fmul_rn so that no rounding point is contracted away.  One CTA: forward, accuracy AND d loss / d
+// end_scores in the same launch.  A separate kernel from the RM loss: RM's arithmetic (fp32 only) stays as it is.
+struct CostParams {
+  const void *scores;
+  const void *better_signs;
+  const void *worse_signs;
+  int score_dt, better_dt, worse_dt;
+  int n_pairs;
+  float scale, reg;
+  int faithful;
+  void *loss;     // 0-dim, dtype Pc
+  float *stats;   // [loss, accuracy]
+  void *grad;     // optional, [2B] in E
+};
+
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS) cost_pair_loss_kernel(const CostParams p) {
+  __shared__ float scratch[33];
+  const int B = p.n_pairs, E = p.score_dt;
+  const int out_dt = (p.better_dt == AA_F32 || p.worse_dt == AA_F32) ? AA_F32 : E;
+  const int re = p.faithful ? E : AA_F32, rb = p.faithful ? p.better_dt : AA_F32;
+  const int rw = p.faithful ? p.worse_dt : AA_F32, rc = p.faithful ? out_dt : AA_F32;
+  const float inv_b = 1.f / static_cast<float>(B), inv_2b = 1.f / static_cast<float>(2 * B);
+  const bool use_reg = p.reg > 0.f;
+  // autograd's chain from d loss = 1, each gradient cast to its input's dtype at the promotion points
+  // (a mean's backward multiplies by the fp32 reciprocal of the count, as ATen CUDA divides by a scalar)
+  const float g_cost = round_to(p.scale, rc);                                     // MulBackward(scale)
+  const float g_lsb = round_to(__fmul_rn(-round_to(g_cost, rb), inv_b), rb);      // Sub -> Neg -> MeanBackward
+  const float g_lsw = round_to(__fmul_rn(-round_to(g_cost, rw), inv_b), rw);      // Sub(other) -> MeanBackward
+  const float g_lso = round_to(-inv_b, re);                                       // Neg -> MeanBackward
+  const float g_sq = round_to(__fmul_rn(round_to(p.reg, re), inv_2b), re);        // MulBackward(reg) -> MeanBackward
+  float s_b = 0.f, s_w = 0.f, s_o = 0.f, s_sq = 0.f, s_acc = 0.f;
+  for (int i = threadIdx.x; i < B; i += THREADS) {
+    const float h = load_as_float(p.scores, i, E), l = load_as_float(p.scores, B + i, E);
+    const float sb = load_as_float(p.better_signs, i, p.better_dt), sw = load_as_float(p.worse_signs, i, p.worse_dt);
+    const float hb = round_to(__fmul_rn(h, sb), rb), lw = round_to(__fmul_rn(l, sw), rw), z = round_to(h - l, re);
+    s_b += round_to(log_sigmoid(hb), rb);
+    s_w += round_to(log_sigmoid(lw), rw);
+    s_o += round_to(log_sigmoid(z), re);
+    s_sq += round_to(__fmul_rn(h, h), re) + round_to(__fmul_rn(l, l), re);
+    s_acc += (h > l) ? 1.f : 0.f;
+    if (p.grad) {
+      // the engine adds the contributions in reverse order of creation: reg (stack), then h - l, then the cost term
+      const float gz = round_to(__fmul_rn(g_lso, dlog_sigmoid(z)), re);
+      float gh = gz, gl = -gz;
+      if (use_reg) {
+        gh = round_to(round_to(__fmul_rn(g_sq, round_to(2.f * h, re)), re) + gz, re);
+        gl = round_to(round_to(__fmul_rn(g_sq, round_to(2.f * l, re)), re) - gz, re);
+      }
+      // MulBackward(h * sb): (grad * sb) in Pb, then cast to E
+      const float ch = round_to(round_to(__fmul_rn(round_to(__fmul_rn(g_lsb, dlog_sigmoid(hb)), rb), sb), rb), re);
+      const float cl = round_to(round_to(__fmul_rn(round_to(__fmul_rn(g_lsw, dlog_sigmoid(lw)), rw), sw), rw), re);
+      store_from_float(p.grad, i, E, round_to(gh + ch, re));
+      store_from_float(p.grad, B + i, E, round_to(gl + cl, re));
+    }
+  }
+  s_b = block_sum<THREADS>(s_b, scratch);
+  s_w = block_sum<THREADS>(s_w, scratch);
+  s_o = block_sum<THREADS>(s_o, scratch);
+  s_sq = block_sum<THREADS>(s_sq, scratch);
+  s_acc = block_sum<THREADS>(s_acc, scratch);
+  if (threadIdx.x == 0) {
+    const float mb = round_to(__fmul_rn(s_b, inv_b), rb), mw = round_to(__fmul_rn(s_w, inv_b), rw);
+    const float mo = round_to(__fmul_rn(s_o, inv_b), re);
+    const float cost = round_to(-mb - mw, rc);
+    float loss = round_to(round_to(__fmul_rn(p.scale, cost), rc) - mo, rc);
+    if (use_reg) loss = round_to(loss + round_to(__fmul_rn(p.reg, round_to(__fmul_rn(s_sq, inv_2b), re)), re), rc);
+    store_from_float(p.loss, 0, out_dt, loss);  // f32 mode: the fp32 result, rounded once to the reference's dtype
+    p.stats[0] = loss;                          // f32 mode: unrounded
+    p.stats[1] = s_acc * inv_b;  // (h > l).float().mean() is fp32 in the reference
+  }
+}
+
 }  // namespace aa
 
 using namespace aa;
@@ -326,6 +405,24 @@ extern "C" int aa_rm_pair_loss(const float *end_scores, int32_t n_pairs, float r
   rm_pair_loss_kernel<256><<<1, 256, 0, static_cast<cudaStream_t>(stream)>>>(end_scores, n_pairs, regularization, out,
                                                                             grad_end_scores);
   return check_launch("aa_rm_pair_loss");
+}
+
+extern "C" int aa_cost_pair_loss(const void *end_scores, int score_dtype, const void *better_signs, int better_dtype,
+                                 const void *worse_signs, int worse_dtype, int32_t n_pairs, float scale_coeff,
+                                 float regularization, int mode, void *loss, float *stats, void *grad_end_scores,
+                                 void *stream) {
+  AA_REQUIRE(n_pairs > 0, AA_ERR_ARG, "aa_cost_pair_loss: bad sizes");
+  AA_REQUIRE(end_scores && better_signs && worse_signs && loss && stats, AA_ERR_ARG, "aa_cost_pair_loss: null pointer");
+  AA_REQUIRE(score_dtype == AA_BF16 || score_dtype == AA_F16 || score_dtype == AA_F32, AA_ERR_DTYPE,
+             "aa_cost_pair_loss: bad dtype %d", score_dtype);
+  AA_REQUIRE((better_dtype == score_dtype || better_dtype == AA_F32) && (worse_dtype == score_dtype || worse_dtype == AA_F32),
+             AA_ERR_DTYPE, "aa_cost_pair_loss: bad sign dtype %d / %d for end-score dtype %d", better_dtype, worse_dtype,
+             score_dtype);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_cost_pair_loss: bad mode %d", mode);
+  const CostParams p{end_scores, better_signs, worse_signs, score_dtype, better_dtype, worse_dtype, n_pairs,
+                     scale_coeff, regularization, mode == AA_MODE_FAITHFUL, loss, stats, grad_end_scores};
+  cost_pair_loss_kernel<256><<<1, 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("aa_cost_pair_loss");
 }
 
 extern "C" int aa_strip_pad_tail(const int64_t *input_ids, int32_t n_samples, int32_t L,

@@ -22,7 +22,7 @@ from . import _lib as L
 __all__ = [
     'gather_log_probabilities', 'masked_mean', 'sequence_log_probs', 'RowPlan', 'DeviceLens', 'DevicePlan', 'as_device_lens', 'rollout_layout', 'response_tail_log_probs', 'response_tail_log_probs_pair', 'dpo_loss_from_log_probs',
     'dpo_fused_loss', 'score_head', 'score_end', 'kl_rewards_and_gae', 'gae_from_rewards', 'estimator_returns', 'actor_loss', 'critic_loss',
-    'move_padding_left', 'count_nonpad', 'strip_pad_tail', 'ppo_pack_metrics', 'check_status', 'raise_for_status', 'status_lane', 'causal_lm_loss', 'rm_pair_loss', 'group_advantages', 'grpo_loss', 'tail_token_log_probs', 'pair_slices', 'slice_sums', 'tail_rows', 'linear_token_log_probs',
+    'move_padding_left', 'count_nonpad', 'strip_pad_tail', 'ppo_pack_metrics', 'check_status', 'raise_for_status', 'status_lane', 'causal_lm_loss', 'rm_pair_loss', 'cost_pair_loss','group_advantages', 'grpo_loss', 'tail_token_log_probs', 'pair_slices', 'slice_sums', 'tail_rows', 'linear_token_log_probs',
     'sequence_log_probs_from_hidden', 'fused_linear_token_log_probs', 'tail_log_probs_from_hidden', 'tail_actor_loss', 'tail_critic_loss', 'lm_head_weight',
 ]
 
@@ -1163,6 +1163,68 @@ def rm_pair_loss(end_scores: torch.Tensor, regularization: float = 0.0) -> dict[
     loss, out = _RmPairLossFn.apply(flat, regularization)
     higher, lower = flat.detach().chunk(2)
     return {'loss': loss, 'accuracy': out[1], 'higher_end_reward': higher, 'lower_end_reward': lower, '_stats': out}
+
+
+# ---- cost-model pairwise loss -------------------------------------------------------------------------
+class _CostPairLossFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, end_scores, better, worse, scale_coeff, regularization, mode_code, out_dtype):
+        n = end_scores.numel()
+        dev = end_scores.device
+        loss = torch.empty((), dtype=out_dtype, device=dev)
+        stats = torch.empty(2, dtype=torch.float32, device=dev)
+        grad = torch.empty(n, dtype=end_scores.dtype, device=dev)
+        L.check(L.lib().aa_cost_pair_loss(end_scores.data_ptr(), L.dtype_code(end_scores.dtype), better.data_ptr(),
+                                          L.dtype_code(better.dtype), worse.data_ptr(), L.dtype_code(worse.dtype), n // 2,
+                                          float(scale_coeff), float(regularization), mode_code, loss.data_ptr(),
+                                          stats.data_ptr(), grad.data_ptr(), L.stream_ptr(dev)))
+        ctx.save_for_backward(grad)
+        ctx.mark_non_differentiable(stats)
+        return loss, stats
+
+    @staticmethod
+    def backward(ctx, g, _):
+        (grad,) = ctx.saved_tensors
+        return grad * g, None, None, None, None, None, None
+
+
+def cost_pair_loss(end_scores: torch.Tensor, better_signs, worse_signs, scale_coeff: float, regularization: float = 0.0,
+                   mode: str | None = None) -> dict[str, torch.Tensor]:
+    """The loss tail of CMTrainer.loss (trainers/text_to_text/cost_model.py:111-144): end_scores (2B,) or (2B, 1) in
+    bf16 / f16 / fp32, higher-cost rows first; better_signs / worse_signs are meta_info's is_better_safe /
+    is_worse_safe lists -> {'loss', 'accuracy', 'higher_end_reward', 'lower_end_reward', '_stats'}; one launch for
+    forward + backward.
+
+    Each sign list becomes a tensor through `torch.tensor(list)` as in the reference, so its dtype (int64, fp32 or
+    bool) decides the arithmetic: h * sb is in torch.result_type(h, sb), and the loss is fp32 as soon as one product
+    is.  The loss has the reference's dtype in both modes.  A sign list whose length is not B raises RuntimeError
+    (the reference's broadcast would accept a one-element list; the collator never produces one).  Every error is
+    raised on the host, before the launch."""
+    flat = end_scores.reshape(-1)
+    if flat.numel() % 2:
+        raise ValueError('end_scores must hold 2B values (higher-cost rows first, lower-cost second)')
+    B = flat.numel() // 2
+    flat = flat.contiguous()
+    sb, sw = torch.tensor(better_signs), torch.tensor(worse_signs)
+    for name, s in (('is_better_safe', sb), ('is_worse_safe', sw)):
+        if s.dim() != 1 or s.numel() != B:
+            raise RuntimeError(f'{name} holds {s.numel()} values for {B} pairs: the sizes of the end scores '
+                               f'and the signs must match')
+    L.require_cuda(end_scores)
+    sb, sw = sb.to(torch.result_type(flat, sb)), sw.to(torch.result_type(flat, sw))
+    # both sign vectors go to the device in ONE copy (the second starts 4-byte aligned)
+    off = (sb.numel() * sb.element_size() + 3) // 4 * 4
+    host = torch.zeros(off + sw.numel() * sw.element_size(), dtype=torch.uint8)
+    host[:sb.numel() * sb.element_size()] = sb.view(torch.uint8)
+    host[off:] = sw.view(torch.uint8)
+    signs = host.to(flat.device)
+    d_sb, d_sw = signs[:sb.numel() * sb.element_size()].view(sb.dtype), signs[off:].view(sw.dtype)
+    out_dtype = torch.promote_types(sb.dtype, sw.dtype)
+    loss, stats = _CostPairLossFn.apply(flat, d_sb, d_sw, scale_coeff, regularization,
+                                        _mode_code(mode, flat.dtype), out_dtype)
+    higher, lower = flat.detach().chunk(2)
+    return {'loss': loss, 'accuracy': stats[1], 'higher_end_reward': higher, 'lower_end_reward': lower,
+            '_stats': stats}
 
 
 # ---- causal-LM cross-entropy (SFT loss, PPO ptx term) -------------------------------------------------

@@ -14,7 +14,10 @@ swaps, without touching any reference file,
     the five advantage estimators on K4 / K4r); its actor_step, reward_model_step and split_ptx_micro_batches stay
     the reference's,
   * SupervisedTrainer.{loss, train_step} of the text / image / audio SFT trainers (cross-entropy from K1),
-  * GRPOTrainer.{_get_per_token_logps, train_step} and RMTrainer.{loss, train_step} of the text trainers,
+  * GRPOTrainer.{_get_per_token_logps, train_step} of the text trainer, RMTrainer.{loss, train_step} of the text /
+    audio / video trainers (the audio and video trainers override `loss` with the text arithmetic, so their own `loss`
+    is replaced too; the image trainers inherit both) and CMTrainer.{loss, train_step} of the text cost-model
+    trainer (Safe RLHF's signed cost loss in one launch; the image cost-model trainer inherits both),
   * SimPOTrainer / ORPOTrainer / KTOTrainer.{loss, train_step} (they inherit the patched DPOTrainer.compute_log_probs),
   * SafeRLHFVTrainer.{actor_step, rollout, actor_loss_fn_with_cost, add_kl_divergence_regularization_with_cost,
     rl_step} (text+image),
@@ -31,6 +34,7 @@ from .trainers.text_audio_to_text.dpo import DPOTrainer as _AudioDPO
 from .trainers.text_audio_to_text.ppo import PPOTrainer as _AudioPPO
 from .trainers.text_image_to_text.ppo import PPOTrainer as _MMPPO
 from .trainers.text_image_to_text.saferlhf import SafeRLHFVTrainer as _SafeV
+from .trainers.text_to_text.cost_model import CMTrainer as _CM
 from .trainers.text_to_text.dpo import DPOTrainer as _TextDPO
 from .trainers.text_to_text.grpo import GRPOTrainer as _GRPO
 from .trainers.text_to_text.kto import KTOTrainer as _KTO
@@ -71,7 +75,12 @@ _SFT_TARGETS = {
     'align_anything.trainers.text_audio_to_text.sft': _SFT,
 }
 _GRPO_TARGETS = {'align_anything.trainers.text_to_text.grpo': _GRPO}
-_RMT_TARGETS = {'align_anything.trainers.text_to_text.rm': _RM}
+_RMT_TARGETS = {
+    'align_anything.trainers.text_to_text.rm': _RM,
+    'align_anything.trainers.text_audio_to_text.rm': _RM,
+    'align_anything.trainers.text_video_to_text.rm': _RM,
+    'align_anything.trainers.text_to_text.cost_model': _CM,
+}
 _SLICED_TARGETS = {
     'align_anything.trainers.text_to_text.simpo': ('SimPOTrainer', _SimPO),
     'align_anything.trainers.text_to_text.orpo': ('ORPOTrainer', _ORPO),
@@ -145,7 +154,7 @@ def install(trainers: bool = True, models: bool = True) -> dict[str, list[str]]:
                     done.setdefault(modname, []).append(n)
             cls = (getattr(mod, 'DPOTrainer', None) or getattr(mod, 'PPOTrainer', None)
                    or getattr(mod, 'SupervisedTrainer', None) or getattr(mod, 'GRPOTrainer', None)
-                   or getattr(mod, 'RMTrainer', None))
+                   or getattr(mod, 'RMTrainer', None) or getattr(mod, 'CMTrainer', None))
             if cls is None:
                 continue
             methods = (_DPO_METHODS if modname in _DPO_TARGETS else _PPO_METHODS if modname in _PPO_TARGETS else

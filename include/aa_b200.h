@@ -217,6 +217,25 @@ int aa_rm_pair_loss(const float *end_scores, int32_t n_pairs, float regularizati
                     float *grad_end_scores, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Cost-model pairwise loss (Safe RLHF's cost model; sibling of the RM loss).  Replaces the loss tail of
+ * trainers/text_to_text/cost_model.py:97-144 (inherited by text_image_to_text/cost_model.py):
+ *   end_scores [2*n_pairs] in score_dtype E (bf16 / f16 / f32; higher-cost rows first, lower second),
+ *   better_signs / worse_signs [n_pairs]: is_better_safe / is_worse_safe cast to their product dtype with E
+ *     (torch.result_type of the end scores and the sign tensor): E, or AA_F32 for float signs;
+ *   loss   = scale_coeff * (-mean(logsigmoid(h * sb)) - mean(logsigmoid(l * sw))) - mean(logsigmoid(h - l))
+ *            [+ regularization * mean(square(all 2B scores)) when regularization > 0],
+ *            written as one element of dtype AA_F32 if either sign dtype is AA_F32, else E;
+ *   stats  fp32 [2] = {loss, accuracy = mean(h > l)}  (the RM stats layout);
+ *   grad_end_scores (optional) [2*n_pairs] in E = d loss / d end_scores.
+ * FAITHFUL rounds where the eager ops round, and the gradient restates autograd's chain and casts;
+ * AA_MODE_F32 keeps fp32 throughout and rounds the loss and the gradient once (stats[0] keeps the fp32 loss).
+ * One CTA.
+ * ------------------------------------------------------------------------------------- */
+int aa_cost_pair_loss(const void *end_scores, int score_dtype, const void *better_signs, int better_dtype,
+                      const void *worse_signs, int worse_dtype, int32_t n_pairs, float scale_coeff,
+                      float regularization, int mode, void *loss, float *stats, void *grad_end_scores, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * K3  scalar score head of the reward / critic models: scores[r] = <hidden[r,:], w>.
  * Replaces `self.score_head(last_hidden_state)` (models/llama.py:62-63, opt.py, llava.py:62-63,
  * qwen2_vl.py:59-60, qwen2_audio.py:77-78).  FAITHFUL: fp32 dot rounded to the hidden dtype
