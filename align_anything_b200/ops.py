@@ -309,16 +309,18 @@ def _launch_bwd(logits, labels, plan: RowPlan, stat_max, stat_logsum, grad_rows,
     dev = logits.device
     p = plan.ptrs()
     V = logits.size(-1)
+    grad_row_stride = V if grad_row_stride is None else int(grad_row_stride)
     n_tile_rows, extra, n_extra = plan.n_tile_rows, None, 0
     if n_tile_rows > 0 and _ZERO_SPANS and plan.host_layout:
         # the row layout is known on the host: long zero spans -> copy engine, isolated zero rows -> listed after the
-        # scored rows (equal-cost rows first under the kernel's static stride), instead of "every tile row is work"
+        # scored rows (equal-cost rows first under the kernel's static stride), instead of "every tile row is work".
+        # A pitched tile is cleared row by row (its pad columns are not the kernel's to touch)
         import ctypes
 
         if plan.n_zero_spans:
-            L.check(L.lib().aa_zero_rows(grad_logits.data_ptr(), L.dtype_code(grad_logits.dtype), V, V, plan.n_tile_rows,
-                                         ctypes.cast(plan.zero_spans, ctypes.c_void_p), plan.n_zero_spans,
-                                         L.stream_ptr(dev)))
+            L.check(L.lib().aa_zero_rows(grad_logits.data_ptr(), L.dtype_code(grad_logits.dtype), grad_row_stride, V,
+                                         plan.n_tile_rows, ctypes.cast(plan.zero_spans, ctypes.c_void_p),
+                                         plan.n_zero_spans, L.stream_ptr(dev)))
         n_tile_rows, extra, n_extra = 0, plan.extra_zero_rows, plan.n_extra
     if scratch is None:  # 32 bytes per work row: the RowRec table of the TMA-staged K1b
         n_work = n_tile_rows if n_tile_rows > 0 else plan.n_rows + n_extra
@@ -329,8 +331,7 @@ def _launch_bwd(logits, labels, plan: RowPlan, stat_max, stat_logsum, grad_rows,
         plan.n_seg, plan.n_rows, p[0], p[1], p[2], p[3], p[4], stat_max.data_ptr(), stat_logsum.data_ptr(),
         L.ptr(grad_rows), L.dtype_code(grad_rows.dtype) if grad_rows is not None else L.AA_F32,
         L.ptr(grad_seg), L.ptr(grad_scale), L.dtype_code(grad_scale.dtype) if grad_scale is not None else L.AA_F32,
-        grad_logits.data_ptr(), V if grad_row_stride is None else int(grad_row_stride),
-        n_tile_rows, L.ptr(extra), n_extra,
+        grad_logits.data_ptr(), grad_row_stride, n_tile_rows, L.ptr(extra), n_extra,
         L.ptr(scratch), mode_code, L.stream_ptr(dev)))
 
 
