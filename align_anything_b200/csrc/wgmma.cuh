@@ -196,9 +196,19 @@ inline int make_map_2d(CUtensorMap *map, const void *base, int64_t inner, int64_
   const cuuint64_t strides[1] = {static_cast<cuuint64_t>(row_stride) * 2};
   const cuuint32_t box[2] = {static_cast<cuuint32_t>(BK), static_cast<cuuint32_t>(box_rows)};
   const cuuint32_t elem[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(base), dims, strides, box, elem,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  auto encode = [&] {
+    return fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(base), dims, strides, box, elem,
+              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  };
+  CUresult r = encode();
+  if (r == CUDA_ERROR_INVALID_CONTEXT) {
+    // The driver call needs a current context, and a thread whose first CUDA work is this launch has none yet (the
+    // autograd engine's device thread when the lm_head backward is the first node it runs).  cudaSetDevice binds the
+    // device's primary context to the thread, as the runtime's own first launch would.
+    int dev = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess && cudaSetDevice(dev) == cudaSuccess) r = encode();
+  }
   if (r != CUDA_SUCCESS) {
     set_error("%s: cuTensorMapEncodeTiled failed (%d)", who, static_cast<int>(r));
     return AA_ERR_ARG;
