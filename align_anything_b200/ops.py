@@ -23,7 +23,7 @@ __all__ = [
     'gather_log_probabilities', 'masked_mean', 'sequence_log_probs', 'RowPlan', 'DeviceLens', 'DevicePlan', 'as_device_lens', 'rollout_layout', 'response_tail_log_probs', 'response_tail_log_probs_pair', 'dpo_loss_from_log_probs',
     'dpo_fused_loss', 'score_head', 'score_end', 'kl_rewards_and_gae', 'gae_from_rewards', 'estimator_returns', 'actor_loss', 'critic_loss',
     'move_padding_left', 'count_nonpad', 'strip_pad_tail', 'ppo_pack_metrics', 'check_status', 'raise_for_status', 'status_lane', 'causal_lm_loss', 'rm_pair_loss', 'cost_pair_loss','group_advantages', 'grpo_loss', 'tail_token_log_probs', 'pair_slices', 'slice_sums', 'tail_rows', 'linear_token_log_probs',
-    'sequence_log_probs_from_hidden', 'fused_linear_token_log_probs', 'tail_log_probs_from_hidden', 'tail_actor_loss', 'tail_critic_loss', 'lm_head_weight',
+    'sequence_log_probs_from_hidden', 'fused_linear_token_log_probs', 'tail_log_probs_from_hidden', 'dense_log_probs_from_hidden', 'tail_actor_loss', 'tail_critic_loss', 'lm_head_weight',
 ]
 
 _REROUTE_TO_BASE = os.environ.get('AA_B200_REROUTE_BASE', '1') != '0'
@@ -696,6 +696,24 @@ def tail_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, input
     seq = hidden.size(1)
     labels = strip_pad_tail(input_ids, lens, 0, strip=False)  # (B, max R): input_ids[b, -R_b:]
     return _tails_from_hidden(hidden, weight, labels, lens, list(lens), [seq - 1 - r for r in lens], 0, chunk_rows, mode)
+
+
+def dense_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, input_ids: torch.Tensor, start: int,
+                                chunk_rows: int | None = None, mode: str | None = None) -> torch.Tensor:
+    """`gather_log_probabilities(F.linear(hidden, weight)[:, :-1], input_ids[:, 1:])[:, start:]` from the last hidden
+    states (B, L, H) and the lm_head weight (V, H), without the (B, L, V) logits tile: every sample scores the same rows,
+    hidden positions [start, L - 1) against tokens [start + 1, L).  The text PPO rollout (start = 0), its rl_step
+    (start = prompt_idx) and GRPO (start = L - 1 - logits_to_keep) all read this.  Without a gradient the rows go to K6;
+    with one to linear_token_log_probs.  -> (B, L - 1 - start), the dtype gather_log_probabilities returns."""
+    L.require_cuda(hidden, weight, input_ids)
+    if hidden.dim() != 3 or input_ids.shape != hidden.shape[:2]:
+        raise ValueError('expected hidden (B, L, H) and input_ids (B, L)')
+    B, seq = input_ids.shape
+    start = int(start)
+    if not 0 <= start <= seq - 1:
+        raise ValueError(f'start = {start} lies outside [0, {seq - 1}] for sequences of {seq}')
+    W = seq - 1 - start
+    return _tails_from_hidden(hidden, weight, input_ids, (W,) * B, [W] * B, [start] * B, start + 1, chunk_rows, mode)
 
 
 class _LogProbViewFn(torch.autograd.Function):

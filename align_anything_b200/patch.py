@@ -14,7 +14,8 @@ swaps, without touching any reference file,
     the five advantage estimators on K4 / K4r); its actor_step, reward_model_step and split_ptx_micro_batches stay
     the reference's,
   * SupervisedTrainer.{loss, train_step} of the text / image / audio SFT trainers (cross-entropy from K1),
-  * GRPOTrainer.{_get_per_token_logps, train_step} of the text trainer, RMTrainer.{loss, train_step} of the text /
+  * GRPOTrainer.{_get_per_token_logps, train_step} of the text trainer (the PPO and GRPO classes also get the
+    `fused_lm_head` / `lm_head_chunk_rows` switches, off), RMTrainer.{loss, train_step} of the text /
     audio / video trainers (the audio and video trainers override `loss` with the text arithmetic, so their own `loss`
     is replaced too; the image trainers inherit both) and CMTrainer.{loss, train_step} of the text cost-model
     trainer (Safe RLHF's signed cost loss in one launch; the image cost-model trainer inherits both),
@@ -187,6 +188,10 @@ def install(trainers: bool = True, models: bool = True) -> dict[str, list[str]]:
                         if hasattr(src, attr):
                             _saved.append((cls, attr, cls.__dict__.get(attr, None)))
                             setattr(cls, attr, getattr(src, attr))
+                else:  # the switch the grafted step_from_rollout / _get_per_token_logps read
+                    for attr in ('fused_lm_head', 'lm_head_chunk_rows'):
+                        _saved.append((cls, attr, cls.__dict__.get(attr, None)))
+                        setattr(cls, attr, getattr(src, attr))
             elif modname in _SFT_TARGETS:
                 _saved.append((cls, 'ignore_index', cls.__dict__.get('ignore_index', None)))
                 setattr(cls, 'ignore_index', -100)

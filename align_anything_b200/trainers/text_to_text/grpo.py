@@ -11,12 +11,18 @@ import torch
 
 from ... import ops
 from ...utils.multi_process import all_reduce_packed
+from .ppo import hidden_log_probs, lm_head_of
 
 __all__ = ['GRPOTrainer']
 
 
 class GRPOTrainer:
     mode = None
+    # Opt-in: no (B * G, L, V) logits tile.  Both models are asked for their last hidden states (`output_hidden_states=
+    # True, logits_to_keep=1`); the reference model's completion rows run through K6, the policy's through K6 + K6b + the
+    # two backward GEMMs (ops.dense_log_probs_from_hidden), then the GRPO loss kernel (ops.grpo_loss).
+    fused_lm_head = False
+    lm_head_chunk_rows = None
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, tokenizer=None, *, beta=None,
                  num_generations=None) -> None:
@@ -31,12 +37,19 @@ class GRPOTrainer:
     # -- trainers/text_to_text/grpo.py:199-210 ---------------------------------------------------
     def _get_per_token_logps(self, model, input_ids, attention_mask, logits_to_keep):
         """Log-probs of the last `logits_to_keep` tokens: one K1 launch on the model's logits (the reference
-        slices, log-softmaxes the whole (B, K, V) tile and gathers)."""
+        slices, log-softmaxes the whole (B, K, V) tile and gathers).  With fused_lm_head: from the hidden states."""
+        if self.fused_lm_head:
+            return hidden_log_probs(model, {'input_ids': input_ids, 'attention_mask': attention_mask}, input_ids,
+                                    input_ids.size(1) - 1 - logits_to_keep, lm_head_of(model), self.lm_head_chunk_rows,
+                                    self.mode)
         logits = model(input_ids=input_ids, attention_mask=attention_mask).logits
         return ops.tail_token_log_probs(logits, input_ids, logits_to_keep, mode=self.mode)
 
     # -- the arithmetic of train_step, trainers/text_to_text/grpo.py:268-318 ---------------------------
     def step_from_rollout(self, sequences: torch.Tensor, prompt_length: int, rewards: torch.Tensor) -> dict[str, Any]:
+        if self.fused_lm_head:  # refuse a head the fused path would get wrong before anything runs
+            for model in (self.actor_reference_model, self.actor_model):
+                lm_head_of(model)
         advantages = ops.group_advantages(rewards, self.num_generations)  # (B * G, 1)
         attention_mask = (sequences != self.tokenizer.pad_token_id).long()
         logits_to_keep = sequences.size(1) - prompt_length
@@ -45,9 +58,14 @@ class GRPOTrainer:
         with torch.no_grad():
             ref_per_token_logps = self._get_per_token_logps(self.actor_reference_model, sequences, attention_mask,
                                                             logits_to_keep)
-        logits = self.actor_model(input_ids=sequences, attention_mask=attention_mask).logits
-        loss, _, _ = ops.grpo_loss_from_logits(logits, sequences, logits_to_keep, ref_per_token_logps, advantages,
-                                               self.tokenizer.eos_token_id, self.beta, mode=self.mode)
+        if self.fused_lm_head:  # the composed path: K1f needs a logits tile
+            per_token_logps = self._get_per_token_logps(self.actor_model, sequences, attention_mask, logits_to_keep)
+            loss, _ = ops.grpo_loss(per_token_logps, ref_per_token_logps, advantages, sequences[:, -logits_to_keep:],
+                                    self.tokenizer.eos_token_id, self.beta, mode=self.mode)
+        else:
+            logits = self.actor_model(input_ids=sequences, attention_mask=attention_mask).logits
+            loss, _, _ = ops.grpo_loss_from_logits(logits, sequences, logits_to_keep, ref_per_token_logps, advantages,
+                                                   self.tokenizer.eos_token_id, self.beta, mode=self.mode)
         self.actor_model.zero_grad()
         self.actor_model.backward(loss)
         self.actor_model.step()

@@ -9,6 +9,9 @@ then K4r (ops.estimator_returns) for the group statistic and the discounted retu
 where the reference loops over every response position.  The group estimators keep the reference's grouping of the
 flattened (B, W) token rewards (SURVEY.md H9).
 
+`fused_lm_head` (inherited from the text trainer) covers all five estimators: rollout scoring is the text trainer's
+score_rollout, and both rl_step branches take the actor node of the text trainer (actor_loss_node).
+
 Reads, besides what the text trainer reads, `self.advantage_estimator` and `self.n_samples_per_prompt`.
 """
 from __future__ import annotations
@@ -19,7 +22,7 @@ import torch
 
 from ... import ops
 from ...utils.multi_process import all_reduce_packed, fused_allreduce
-from .ppo import METRIC_KEYS
+from .ppo import METRIC_KEYS, actor_loss_node, lm_head_of
 from .ppo import PPOTrainer as _TextPPOTrainer
 
 __all__ = ['PPOTrainer']
@@ -97,6 +100,7 @@ class PPOTrainer(_TextPPOTrainer):
         start = training_batch['prompt_idx']
         input_ids = inference_batch['input_ids']
         sequence_mask = inference_batch['attention_mask'][:, 1:]
+        head = lm_head_of(self.actor_model) if self.fused_lm_head else None  # refusals before any launch
 
         # K4 gives the KL-shaped rewards, the metric row sums and the status word (its GAE output is not used); K4r
         # then writes the estimator's advantages / returns and their row means into lanes 3 / 4 of row_stats
@@ -107,10 +111,8 @@ class PPOTrainer(_TextPPOTrainer):
             old_rewards, sequence_mask, start, self.advantage_estimator, self.n_samples_per_prompt, self.gamma,
             mode=self.mode, row_stats=row_stats)
 
-        logits = self.actor_model(**inference_batch, use_cache=False).logits
-        actor_loss, _, actor_loss32 = ops.dense_actor_loss(logits, input_ids, start, old_log_probs[:, start:],
-                                                           reward_advantages, sequence_mask[:, start:],
-                                                           self.clip_range_ratio, mode=self.mode)
+        actor_loss, actor_loss32 = actor_loss_node(self, inference_batch, input_ids, start, head, old_log_probs,
+                                                   reward_advantages, sequence_mask)
         self.actor_model.backward(actor_loss)
         self.actor_model.step()
 

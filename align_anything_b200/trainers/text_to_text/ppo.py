@@ -26,8 +26,46 @@ METRIC_KEYS = ('train/actor_loss', 'train/reward_critic_loss', 'train/reward', '
                'train/mean_generated_length', 'train/max_generated_length')
 
 
+def lm_head_of(model) -> torch.Tensor:
+    """The lm_head weight of an engine (or bare module) for the fused lm_head path; ops.lm_head_weight refuses the heads
+    that path would get wrong (ZeRO-3 placeholder, bias, soft-capping / logit scaling)."""
+    return ops.lm_head_weight(getattr(model, 'module', model))
+
+
+def hidden_log_probs(model, batch, input_ids, start, weight, chunk_rows, mode, **kw) -> torch.Tensor:
+    """`gather_log_probabilities(model(**batch).logits[:, :-1], input_ids[:, 1:])[:, start:]` from the model's last
+    hidden states: the lm_head runs on one position inside the model and on the scored rows in ops, no logits tile."""
+    out = model(**batch, output_hidden_states=True, logits_to_keep=1, **kw)
+    return ops.dense_log_probs_from_hidden(out.hidden_states[-1], weight, input_ids, start, chunk_rows=chunk_rows,
+                                           mode=mode)
+
+
+def actor_loss_node(tr, inference_batch, input_ids, start, head, old_log_probs, advantages, sequence_mask):
+    """The actor loss of the text rl_step over the rows `[start:]` -> (loss, the loss for ppo_pack_metrics).  `head`:
+    the lm_head weight when `tr.fused_lm_head` is on, else None.  A function rather than a method, so that the grafted
+    rl_step of the reference's classes finds it without being grafted itself."""
+    if head is not None:  # K6 + K6b + backward GEMMs for the log-probs, then K5
+        log_probs = hidden_log_probs(tr.actor_model, inference_batch, input_ids, start, head, tr.lm_head_chunk_rows,
+                                     tr.mode, use_cache=False)
+        loss = ops.actor_loss(log_probs, old_log_probs[:, start:], advantages, sequence_mask[:, start:],
+                              tr.clip_range_ratio, mode=tr.mode)
+        return loss, loss
+    logits = tr.actor_model(**inference_batch, use_cache=False).logits
+    # the reference scores every position and then slices `[:, start:]` (:338-346); only those rows are ever used, so
+    # only they are read here.  One autograd node (K1f): log-probs, d loss / d log-prob and the gradient tile in a
+    # single pass over the response rows; the prompt rows of the tile are written as zeros by the same kernel.
+    loss, _, loss32 = ops.dense_actor_loss(logits, input_ids, start, old_log_probs[:, start:], advantages,
+                                           sequence_mask[:, start:], tr.clip_range_ratio, mode=tr.mode)
+    return loss, loss32
+
+
 class PPOTrainer:
     mode = None  # None -> 'faithful'
+    # Opt-in: no (B, L, V) logits tile.  The models are asked for their last hidden states (`output_hidden_states=True,
+    # logits_to_keep=1`); rollout scoring (no gradient) runs K6 once per model, the actor's rl_step K6 + K6b + the two
+    # backward GEMMs and then K5 (ops.dense_log_probs_from_hidden -> ops.actor_loss).  ptx_step keeps its logits.
+    fused_lm_head = False
+    lm_head_chunk_rows = None
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, reward_model=None,
                  reward_critic_model=None, tokenizer=None, reward_tokenizer=None, *, kl_coeff=0.02,
@@ -134,14 +172,24 @@ class PPOTrainer:
     def score_rollout(self, actor_batch, prompt_len: int) -> tuple[dict, dict]:
         """Everything rollout() does after generation for one mini-batch: reward / critic scoring and
         the actor / reference log-probs of every next token."""
+        if self.fused_lm_head:  # refuse a head the fused path would get wrong before anything runs
+            heads = (lm_head_of(self.actor_model), lm_head_of(self.actor_reference_model))
         reward_batch = self.reward_model_step(actor_batch)
-        logits = self.actor_model(**actor_batch).logits
-        ref_logits = self.actor_reference_model(**actor_batch).logits
         ids = actor_batch['input_ids']
+        if self.fused_lm_head:  # every position, prompt and pad included: the width the tile path stores
+            log_probs = hidden_log_probs(self.actor_model, actor_batch, ids, 0, heads[0], self.lm_head_chunk_rows,
+                                         self.mode)
+            ref_log_probs = hidden_log_probs(self.actor_reference_model, actor_batch, ids, 0, heads[1],
+                                             self.lm_head_chunk_rows, self.mode)
+        else:
+            logits = self.actor_model(**actor_batch).logits
+            ref_logits = self.actor_reference_model(**actor_batch).logits
+            log_probs = ops.gather_log_probabilities(logits[:, :-1], ids[:, 1:], mode=self.mode)
+            ref_log_probs = ops.gather_log_probabilities(ref_logits[:, :-1], ids[:, 1:], mode=self.mode)
         training = {
             'prompt_idx': prompt_len - 1,
-            'log_probs': ops.gather_log_probabilities(logits[:, :-1], ids[:, 1:], mode=self.mode),
-            'ref_log_probs': ops.gather_log_probabilities(ref_logits[:, :-1], ids[:, 1:], mode=self.mode),
+            'log_probs': log_probs,
+            'ref_log_probs': ref_log_probs,
             'reward': reward_batch['reward'],
             'reward_values': reward_batch['reward_values'],
         }
@@ -172,18 +220,14 @@ class PPOTrainer:
         start = training_batch['prompt_idx']
         input_ids = inference_batch['input_ids']
         sequence_mask = inference_batch['attention_mask'][:, 1:]
+        head = lm_head_of(self.actor_model) if self.fused_lm_head else None  # refusals before any launch
 
         old_rewards, reward_advantages, reward_returns, row_stats = ops.kl_rewards_and_gae(
             reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, start, self.kl_coeff,
             self.clip_range_score, self.gamma, self.gae_lambda, mode=self.mode)
 
-        logits = self.actor_model(**inference_batch, use_cache=False).logits
-        # the reference scores every position and then slices `[:, start:]` (:338-346); only those rows are ever used, so
-        # only they are read here.  One autograd node (K1f): log-probs, d loss / d log-prob and the gradient tile in a
-        # single pass over the response rows; the prompt rows of the tile are written as zeros by the same kernel.
-        actor_loss, _, actor_loss32 = ops.dense_actor_loss(logits, input_ids, start, old_log_probs[:, start:],
-                                                           reward_advantages, sequence_mask[:, start:],
-                                                           self.clip_range_ratio, mode=self.mode)
+        actor_loss, actor_loss32 = actor_loss_node(self, inference_batch, input_ids, start, head, old_log_probs,
+                                                   reward_advantages, sequence_mask)
         self.actor_model.backward(actor_loss)
         self.actor_model.step()
 
