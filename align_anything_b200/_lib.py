@@ -50,6 +50,8 @@ _SIGS = {
     'aa_linear_dweight': (c_int, [_P, c_int64, c_int64, _P, c_int32, c_int64, c_int32, _P, c_int64, c_int32, _P, c_int64, _P]),
     'aa_linear_logprob_fwd': (c_int, [_P, c_int64, c_int32, c_int64, _P, c_int32, c_int64, _P, _P, c_int, _P, _P, _P, c_int64,
                                       c_int, _P, _P]),
+    'aa_linear_logits': (c_int, [_P, c_int64, c_int32, c_int64, _P, c_int32, c_int64, _P, _P, c_int, _P, _P, _P, c_int64,
+                                 c_int, _P, _P, c_int64, _P]),
     'aa_strip_pad_tail': (c_int, [_P, c_int32, c_int32, c_int64, c_int64, c_int, _P, _P, c_int64, _P, _P]),
     'aa_dpo_loss': (c_int, [_P, _P, c_int, c_int32, c_int32, c_int64, c_float, c_int, _P, c_int32, c_int64,
                             _P, _P, _P, _P, POINTER(AaColl), _P, _P, _P]),

@@ -41,12 +41,19 @@ struct Params {
   float *partial;                 // v_splits > 1: (row, split) -> {max, sum, label logit}
 };
 
-// d(logits) tile store of K6b: the upstream gradient per row and the padded bf16 buffer
+// the tile store of K6b (d(logits)) and K6s (the logits): the upstream gradient per row (K6b) and the padded bf16 buffer
 struct GradParams {
   const void *grad_rows;  // upstream d loss / d logp per row
   int grad_rows_dtype;
   __nv_bfloat16 *dlogits; // (n_rows, ld) bf16, ld >= ceil(V / 256) * 256, multiple of 8
   int64_t ld;
+};
+
+// what the consumer warpgroups do with a finished 128 x 256 logits tile
+enum class Epi : int {
+  Lse,      // K6: fold it into the row's running (max, sum-exp, label logit)
+  DLogits,  // K6b: turn it into d(logits) with the statistics K6 saved and store it
+  Logits,   // K6s: both K6's fold and a store of the bf16-rounded logits
 };
 
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
@@ -59,12 +66,13 @@ __device__ __forceinline__ void lse_merge(float &m, float &s, float m_o, float s
   m = mn;
 }
 
-// K6 (DLOGITS = false) and K6b (DLOGITS = true) are ONE kernel: same TMA producer, same wgmma main loop; they differ in
-// what the consumer warpgroups do with a finished 128 x 256 logits tile -- fold it into the running (max, sum-exp,
-// label logit) of the row, or turn it into d(logits) with the statistics K6 saved and store it as bf16.
+// K6, K6b and K6s are ONE kernel: same TMA producer, same wgmma main loop; they differ in what the consumer
+// warpgroups do with a finished 128 x 256 logits tile (Epi) -- fold it into the running (max, sum-exp, label logit) of
+// the row, turn it into d(logits) with the statistics K6 saved and store it as bf16, or (K6s) fold it AND store the
+// bf16-rounded logits, so that the logits of a loss whose gradient seed is known in the forward cost one GEMM pass.
 // Each consumer thread holds 2 rows x 64 columns of the tile (wgmma.cuh, frag_row / frag_col); the 4 threads of a quad
 // share a row, so the per-row statistics are per-thread partials merged across the quad once, at the end.
-template <bool DLOGITS>
+template <Epi EPI>
 __global__ void __launch_bounds__(THREADS, 1)
     linear_logprob_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                           const Params p, const GradParams gp) {
@@ -136,8 +144,13 @@ __global__ void __launch_bounds__(THREADS, 1)
   }
   float acc[ACC];
   int64_t it = 0;
-  if constexpr (!DLOGITS) {
-    // ------------------------------- K6 epilogue: online log-sum-exp ----------------
+  if constexpr (EPI != Epi::DLogits) {
+    // ------------------------------- K6 / K6s epilogue: online log-sum-exp ----------------
+    // K6s rounds every logit to bf16 whatever the mode (the stored tile is bf16, and the statistics must describe it);
+    // the mode then only decides whether the log-prob is rounded.  K6s's pad columns of the last tile are stored as +0.
+    __nv_bfloat16 *lrow[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) lrow[r] = gp.dlogits + (live[r] ? row[r] : 0) * gp.ld;
     if ((t & 3) == 0 && p.status) {
 #pragma unroll
       for (int r = 0; r < 2; ++r)
@@ -172,7 +185,7 @@ __global__ void __launch_bounds__(THREADS, 1)
         float cmax = -INFINITY;
 #pragma unroll
         for (int i = 2 * r; i < ACC; i += 4) cmax = fmaxf(cmax, fmaxf(acc[i], acc[i + 1]));
-        if (p.faithful) cmax = bf16_round(cmax);
+        if (EPI == Epi::Logits || p.faithful) cmax = bf16_round(cmax);
         if (cmax > m[r]) {  // m == -inf implies s == 0
           s[r] *= ex2_approx((m[r] - cmax) * kLog2e);
           m[r] = cmax;
@@ -181,7 +194,15 @@ __global__ void __launch_bounds__(THREADS, 1)
 #pragma unroll
         for (int i = 2 * r; i < ACC; i += 4) {
           float x0 = acc[i], x1 = acc[i + 1];
-          if (p.faithful) round_bf16_pair(x0, x1);
+          if constexpr (EPI == Epi::Logits) {  // ONE rounding serves the store and the fold
+            const uint32_t w = pack2<__nv_bfloat16>(x0, x1);
+            unpack2<__nv_bfloat16>(w, x0, x1);
+            const int col = col_base + frag_col(t, i);
+            if (live[r])
+              *reinterpret_cast<uint32_t *>(lrow[r] + col) = col + 1 < p.V ? w : (col < p.V ? (w & 0xffffu) : 0u);
+          } else {
+            if (p.faithful) round_bf16_pair(x0, x1);
+          }
           add += ex2_approx((x0 - m[r]) * kLog2e) + ex2_approx((x1 - m[r]) * kLog2e);
         }
         s[r] += add;
@@ -189,7 +210,7 @@ __global__ void __launch_bounds__(THREADS, 1)
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      if (p.faithful) x_label[r] = bf16_round(x_label[r]);
+      if (EPI == Epi::Logits || p.faithful) x_label[r] = bf16_round(x_label[r]);
 #pragma unroll
       for (int o = 1; o <= 2; o <<= 1) {
         const float m_o = __shfl_xor_sync(0xffffffffu, m[r], o), s_o = __shfl_xor_sync(0xffffffffu, s[r], o);
@@ -275,7 +296,7 @@ static int make_map(CUtensorMap *map, const void *base, int64_t rows, int H, int
   return make_map_2d(map, base, H, rows, row_stride, box_rows, "aa_linear_logprob_fwd");
 }
 
-// ---- host: scheduling and launch shared by K6 / K6b ------------------------------------------------------------------
+// ---- host: scheduling and launch shared by K6 / K6b / K6s -----------------------------------------------------------
 // One CTA owns 128 rows x a range of vocabulary tiles and keeps (max, sum) in registers.  The L2 working set decides
 // the speed: the 1 MB hidden-state tile of every resident CTA is re-read for each vocabulary tile, and all of them plus
 // the weight tiles do not fit the 50 MB L2.  So the resident wave is shaped as `group` row units x `splits` vocabulary
@@ -324,7 +345,7 @@ static Schedule make_schedule(int64_t n_rows, int V, bool may_split, int64_t par
   return sc;
 }
 
-template <bool DLOGITS>
+template <Epi EPI>
 static int launch(const void *hidden, int64_t n_rows, int H, int64_t hidden_row_stride, const void *weight, int V,
                   int64_t weight_row_stride, Params p, const GradParams &gp, const Schedule &sc, cudaStream_t st,
                   const char *who) {
@@ -338,7 +359,7 @@ static int launch(const void *hidden, int64_t n_rows, int H, int64_t hidden_row_
   p.group_tiles = static_cast<int>(sc.group);
   p.m_tiles = static_cast<int>(sc.units);
   const unsigned units = static_cast<unsigned>(sc.n_groups * sc.group * sc.splits);
-  auto kern = linear_logprob_kernel<DLOGITS>;
+  auto kern = linear_logprob_kernel<EPI>;
   static std::atomic<bool> configured{false};  // once per process (idempotent; a race sets it twice, harmlessly)
   if (!configured.load(std::memory_order_relaxed)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
@@ -351,6 +372,34 @@ static int launch(const void *hidden, int64_t n_rows, int H, int64_t hidden_row_
   kern<<<units, THREADS, SMEM_BYTES, st>>>(map_a, map_b, p, gp);
   return check_launch(who);
 }
+
+// K6 / K6s: argument checks, the launch and (split vocabulary) the merge of the per-split statistics
+template <Epi EPI>
+static int forward(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride, const void *weight,
+                   int32_t V, int64_t weight_row_stride, const int64_t *labels, void *out, int out_dtype,
+                   float *stat_max, float *stat_logsum, float *partial, int64_t partial_floats, int mode,
+                   int32_t *status, const GradParams &gp, void *stream, const char *who) {
+  AA_REQUIRE(n_rows >= 0 && H > 0 && V > 0, AA_ERR_ARG, "%s: bad sizes", who);
+  if (n_rows == 0) return AA_OK;
+  AA_REQUIRE(hidden && weight && labels && out, AA_ERR_ARG, "%s: null pointer", who);
+  AA_REQUIRE(H % BK == 0, AA_ERR_UNSUPPORTED, "%s: H=%d must be a multiple of %d", who, H, BK);
+  AA_REQUIRE((reinterpret_cast<uintptr_t>(hidden) & 15) == 0 && (reinterpret_cast<uintptr_t>(weight) & 15) == 0 &&
+                 hidden_row_stride % 8 == 0 && weight_row_stride % 8 == 0 && hidden_row_stride >= H && weight_row_stride >= H,
+             AA_ERR_ALIGN, "%s: operands must be 16-byte aligned with 16-byte row strides", who);
+  AA_REQUIRE(out_dtype == AA_BF16 || out_dtype == AA_F32, AA_ERR_DTYPE, "%s: out must be bf16 or f32", who);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "%s: bad mode", who);
+  AA_REQUIRE(n_rows < (int64_t(1) << 31) - BM, AA_ERR_UNSUPPORTED, "%s: too many rows", who);
+  const Schedule sc = make_schedule(n_rows, V, partial != nullptr, partial_floats);
+  Params p{labels, n_rows, V, H, out, out_dtype, stat_max, stat_logsum, mode == AA_MODE_FAITHFUL ? 1 : 0, status,
+           1, 1, 1, 1, 1, 1, partial};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = launch<EPI>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, p, gp, sc, st, who);
+  p.v_splits = static_cast<int>(sc.splits);  // the merge kernel reads the split count
+  const int64_t splits = sc.splits;
+  if (rc || splits == 1) return rc;
+  linear_logprob_merge_kernel<<<static_cast<unsigned>((n_rows + 255) / 256), 256, 0, st>>>(p);
+  return check_launch(EPI == Epi::Logits ? "aa_linear_logits(merge)" : "aa_linear_logprob_fwd(merge)");
+}
 }  // namespace k6
 }  // namespace aa
 
@@ -360,29 +409,27 @@ extern "C" int aa_linear_logprob_fwd(const void *hidden, int64_t n_rows, int32_t
                                      const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
                                      void *out, int out_dtype, float *stat_max, float *stat_logsum, float *partial,
                                      int64_t partial_floats, int mode, int32_t *status, void *stream) {
-  AA_REQUIRE(n_rows >= 0 && H > 0 && V > 0, AA_ERR_ARG, "aa_linear_logprob_fwd: bad sizes");
-  if (n_rows == 0) return AA_OK;
-  AA_REQUIRE(hidden && weight && labels && out, AA_ERR_ARG, "aa_linear_logprob_fwd: null pointer");
-  AA_REQUIRE(H % k6::BK == 0, AA_ERR_UNSUPPORTED, "aa_linear_logprob_fwd: H=%d must be a multiple of %d", H, k6::BK);
-  AA_REQUIRE((reinterpret_cast<uintptr_t>(hidden) & 15) == 0 && (reinterpret_cast<uintptr_t>(weight) & 15) == 0 &&
-                 hidden_row_stride % 8 == 0 && weight_row_stride % 8 == 0 && hidden_row_stride >= H && weight_row_stride >= H,
-             AA_ERR_ALIGN, "aa_linear_logprob_fwd: operands must be 16-byte aligned with 16-byte row strides");
-  AA_REQUIRE(out_dtype == AA_BF16 || out_dtype == AA_F32, AA_ERR_DTYPE, "aa_linear_logprob_fwd: out must be bf16 or f32");
-  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_linear_logprob_fwd: bad mode");
-  AA_REQUIRE(n_rows < (int64_t(1) << 31) - k6::BM, AA_ERR_UNSUPPORTED, "aa_linear_logprob_fwd: too many rows");
-  const k6::Schedule sc = k6::make_schedule(n_rows, V, partial != nullptr, partial_floats);
-  k6::Params p{labels, n_rows, V, H, out, out_dtype, stat_max, stat_logsum, mode == AA_MODE_FAITHFUL ? 1 : 0, status,
-               1, 1, 1, 1, 1, 1, partial};
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = k6::launch<false>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, p,
-                             k6::GradParams{nullptr, AA_F32, nullptr, 0}, sc, st, "aa_linear_logprob_fwd");
-  p.v_splits = static_cast<int>(sc.splits);  // the merge kernel reads the split count
-  const int64_t splits = sc.splits;
-  if (rc || splits == 1) return rc;
-  k6::linear_logprob_merge_kernel<<<static_cast<unsigned>((n_rows + 255) / 256), 256, 0, st>>>(p);
-  return check_launch("aa_linear_logprob_fwd(merge)");
+  return k6::forward<k6::Epi::Lse>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, labels, out,
+                                   out_dtype, stat_max, stat_logsum, partial, partial_floats, mode, status,
+                                   k6::GradParams{nullptr, AA_F32, nullptr, 0}, stream, "aa_linear_logprob_fwd");
 }
 
+extern "C" int aa_linear_logits(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
+                                const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
+                                void *out, int out_dtype, float *stat_max, float *stat_logsum, float *partial,
+                                int64_t partial_floats, int mode, int32_t *status, void *logits, int64_t ld,
+                                void *stream) {
+  if (n_rows > 0) {
+    AA_REQUIRE(logits, AA_ERR_ARG, "aa_linear_logits: null pointer");
+    const int64_t all_tiles = (static_cast<int64_t>(V) + k6::BN - 1) / k6::BN;
+    AA_REQUIRE(V > 0 && ld >= all_tiles * k6::BN && ld % 8 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0,
+               AA_ERR_ALIGN, "aa_linear_logits: ld must be >= ceil(V / 256) * 256, a multiple of 8, buffer 16-byte aligned");
+  }
+  return k6::forward<k6::Epi::Logits>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, labels, out,
+                                      out_dtype, stat_max, stat_logsum, partial, partial_floats, mode, status,
+                                      k6::GradParams{nullptr, AA_F32, static_cast<__nv_bfloat16 *>(logits), ld}, stream,
+                                      "aa_linear_logits");
+}
 
 extern "C" int aa_linear_dlogits(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
                                  const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
@@ -407,6 +454,6 @@ extern "C" int aa_linear_dlogits(const void *hidden, int64_t n_rows, int32_t H, 
   k6::Params p{labels, n_rows, V, H, nullptr, AA_BF16, const_cast<float *>(stat_max), const_cast<float *>(stat_logsum),
                mode == AA_MODE_FAITHFUL ? 1 : 0, nullptr, 1, 1, 1, 1, 1, 1, nullptr};
   k6::GradParams gp{grad_rows, grad_rows_dtype, static_cast<__nv_bfloat16 *>(dlogits), ld};
-  return k6::launch<true>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, p, gp, sc,
+  return k6::launch<k6::Epi::DLogits>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, p, gp, sc,
                           static_cast<cudaStream_t>(stream), "aa_linear_dlogits");
 }

@@ -24,6 +24,7 @@ __all__ = [
     'dpo_fused_loss', 'score_head', 'score_end', 'kl_rewards_and_gae', 'gae_from_rewards', 'estimator_returns', 'actor_loss', 'critic_loss',
     'move_padding_left', 'count_nonpad', 'strip_pad_tail', 'ppo_pack_metrics', 'check_status', 'raise_for_status', 'status_lane', 'causal_lm_loss', 'rm_pair_loss', 'cost_pair_loss','group_advantages', 'grpo_loss', 'tail_token_log_probs', 'pair_slices', 'slice_sums', 'tail_rows', 'linear_token_log_probs',
     'sequence_log_probs_from_hidden', 'fused_linear_token_log_probs', 'tail_log_probs_from_hidden', 'dense_log_probs_from_hidden', 'tail_actor_loss', 'tail_critic_loss', 'lm_head_weight',
+    'causal_lm_loss_from_hidden', 'causal_lm_valid_rows',
 ]
 
 _REROUTE_TO_BASE = os.environ.get('AA_B200_REROUTE_BASE', '1') != '0'
@@ -1344,6 +1345,157 @@ def causal_lm_loss_scaled(logits: torch.Tensor, labels: torch.Tensor, loss_scale
     on the multiplication; log the second."""
     logits, shift = _shifted_labels(logits, labels, ignore_index)
     return _CausalLMLossFn.apply(logits, shift, int(ignore_index), float(loss_scale))
+
+
+# ---- causal-LM cross-entropy from the last hidden states (fused lm_head SFT) ---------------------------------------
+def causal_lm_valid_rows(labels: torch.Tensor, ignore_index: int = -100):
+    """The rows a causal-LM cross-entropy scores: flat position b * L + t, t < L - 1, with labels[b, t + 1] !=
+    ignore_index (prompt and padding rows never meet the head).  ONE `nonzero`, so ONE host read: SupervisedTrainer
+    takes it before the model forward, when the queue is already drained by the previous step's read.
+    -> (index (N,) int64 on the labels' device, N)."""
+    B, seq = labels.shape
+    valid = torch.zeros((B, seq), dtype=torch.bool, device=labels.device)
+    valid[:, :-1] = labels[:, 1:] != int(ignore_index)
+    idx = valid.view(-1).nonzero().view(-1)
+    return idx, int(idx.numel())
+
+
+def _ce_chunks(N: int, V: int, chunk_rows: int | None):
+    """Row chunks (r0, n) of the fused lm_head cross-entropy.  Default: two (chunk, ld) bf16 buffers (the logits and
+    d(logits) of one chunk) of about 1 GB each, together what the single d(logits) buffer of the K6b backward holds;
+    then equal chunks of whole 256-row tiles, as in _LinearLogProbK6Fn.backward."""
+    ld = (V + 255) // 256 * 256
+    if chunk_rows is None:
+        chunk_rows = max(128, (1 << 30) // (ld * 2) // 128 * 128)
+    chunk = int(chunk_rows)
+    if chunk < 1:
+        raise ValueError(f'chunk_rows must be positive, got {chunk_rows}')
+    if N == 0:
+        return []
+    n_chunks = (N + chunk - 1) // chunk
+    chunk = min(chunk, (-(-N // n_chunks) + 255) // 256 * 256)
+    return [(r0, min(chunk, N - r0)) for r0 in range(0, N, chunk)]
+
+
+def _ce_loss_launch(logp, labels, n, ignore_index, out, dev):
+    partial = torch.empty(512, dtype=torch.float32, device=dev)
+    L.check(L.lib().aa_nll_mean(logp.data_ptr(), L.AA_F32, labels.data_ptr(), n, int(ignore_index), out[0:1].data_ptr(),
+                                out[1:2].data_ptr(), partial.data_ptr(), _device_scratch(dev)['counter'][4:5].data_ptr(),
+                                L.stream_ptr(dev)))
+
+
+class _LinearCrossEntropyFn(torch.autograd.Function):
+    """Mean NLL of log_softmax(rows @ weight.T) at `lab` over the N valid rows, times `loss_scale`, where the gradient is
+    formed in the FORWARD: every row's upstream gradient is the host constant -loss_scale / N, so per row chunk
+      K6s   the GEMM once: the bf16 logits into `lbuf`, (max, logsum, fp32 log-prob) from the same rounded values;
+      K1b   f32 mode, `lbuf` -> `dbuf`: ATen's fp32 softmax gradient of the upcast logits, cast to bf16 (ForCausalLMLoss);
+      aa_linear_dhidden / aa_linear_dweight on `dbuf` (d(weight) accumulated in fp32 across chunks, rounded once)
+    -- three GEMM passes over 2 * N * H * V instead of K6 + K6b + the two backward GEMMs.  K1b runs out of place: its
+    kernels read `logits` and write `grad` through __restrict__ / non-coherent loads.  The backward only scales the two
+    gradients by the incoming scalar (aa_scale_tile; nothing to do when it is 1) and hands them over, once.
+    Without a gradient (neither input needs one; causal_lm_loss_from_hidden detaches both under torch.no_grad, since
+    needs_input_grad follows requires_grad and not the grad mode): K6s and the loss only.  K6s still stores each logits
+    chunk, into a `lbuf` that nothing reads then (about 1 GB at the default chunk): the price of statistics over the
+    bf16-rounded logits, which K6 only offers with a bf16-rounded log-prob.  N == 0: the loss aa_nll_mean gives over all-ignored labels (what
+    causal_lm_loss returns then), zero gradients.  -> (loss_scale * loss, loss)."""
+
+    @staticmethod
+    def forward(ctx, rows, weight, lab, shift_flat, ignore_index, loss_scale, chunk_rows):
+        N, (V, H) = rows.size(0), weight.shape
+        dev = rows.device
+        need_h, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        out = torch.empty(2, dtype=torch.float32, device=dev)  # [loss, -1 / n_valid]
+        d_rows = d_weight = None
+        if N == 0:
+            _ce_loss_launch(torch.zeros(shift_flat.numel(), dtype=torch.float32, device=dev), shift_flat,
+                            shift_flat.numel(), ignore_index, out, dev)
+            d_rows = torch.zeros_like(rows) if need_h else None
+            d_weight = torch.zeros_like(weight) if need_w else None
+        else:
+            chunks = _ce_chunks(N, V, chunk_rows)
+            ld, cmax = (V + 255) // 256 * 256, max(n for _, n in chunks)
+            lib, st, sc = L.lib(), L.stream_ptr(dev), _device_scratch(dev)
+            logp = torch.empty(N, dtype=torch.float32, device=dev)
+            stats = torch.empty((2, N), dtype=torch.float32, device=dev)
+            partial = torch.empty(3 * max(132 * 128, 16 * cmax), dtype=torch.float32, device=dev)  # split-vocabulary statistics
+            lbuf = torch.empty((cmax, ld), dtype=torch.bfloat16, device=dev)
+            if need_h or need_w:
+                dbuf = torch.empty((cmax, ld), dtype=torch.bfloat16, device=dev)
+                dbuf[:, V:].zero_()  # K1b writes columns [0, V); the GEMMs read all ld
+                seed = torch.full((1,), -float(loss_scale) / N, dtype=torch.float32, device=dev)
+                d_rows = torch.empty_like(rows) if need_h else None
+                d_weight = torch.empty_like(weight) if need_w else None
+                acc = torch.empty((V, H), dtype=torch.float32, device=dev) if (need_w and len(chunks) > 1) else None
+            for i, (r0, n) in enumerate(chunks):
+                h, y = rows[r0:r0 + n], lab[r0:r0 + n]
+                L.check(lib.aa_linear_logits(
+                    h.data_ptr(), n, H, h.stride(0), weight.data_ptr(), V, weight.stride(0), y.data_ptr(),
+                    logp[r0:r0 + n].data_ptr(), L.AA_F32, stats[0, r0:r0 + n].data_ptr(), stats[1, r0:r0 + n].data_ptr(),
+                    partial.data_ptr(), partial.numel(), L.MODE_F32, sc['status'].data_ptr(), lbuf.data_ptr(), ld, st))
+                if not (need_h or need_w):
+                    continue
+                plan = _dense_plan(1, n, n * ld, ld, n, 0, n, 0, str(dev))
+                _launch_bwd(lbuf[:n, :V], y, plan, stats[0, r0:r0 + n], stats[1, r0:r0 + n], None, None, seed,
+                            dbuf[:n, :V], L.MODE_F32, grad_row_stride=ld)
+                if need_h:
+                    dh = d_rows[r0:r0 + n]
+                    L.check(lib.aa_linear_dhidden(dbuf.data_ptr(), n, ld, weight.data_ptr(), V, H, weight.stride(0),
+                                                  dh.data_ptr(), dh.stride(0), st))
+                if need_w:
+                    last = i == len(chunks) - 1
+                    L.check(lib.aa_linear_dweight(dbuf.data_ptr(), n, ld, h.data_ptr(), H, h.stride(0), V, L.ptr(acc), H,
+                                                  1 if i > 0 else 0, d_weight.data_ptr() if last else None,
+                                                  d_weight.stride(0), st))
+            _ce_loss_launch(logp, lab, N, ignore_index, out, dev)
+        ctx.save_for_backward(d_rows, d_weight)
+        ctx.consumed = False
+        loss = out[0]
+        scaled = loss if loss_scale == 1.0 else loss * float(loss_scale)
+        ctx.mark_non_differentiable(loss)
+        return scaled.clone() if scaled is loss else scaled, loss
+
+    @staticmethod
+    def backward(ctx, g, _unused):
+        if ctx.consumed:
+            raise RuntimeError('the fused lm_head cross-entropy node hands its gradients over once: compute the loss '
+                               'again to run backward twice')
+        ctx.consumed = True
+        d_rows, d_weight = ctx.saved_tensors
+        scale = g.detach().float().reshape(1).contiguous()
+        for t in (d_rows, d_weight):
+            if t is not None:
+                L.check(L.lib().aa_scale_tile(t.data_ptr(), L.dtype_code(t.dtype), t.numel(), scale.data_ptr(), L.AA_F32,
+                                              L.stream_ptr(t.device)))
+        return d_rows, d_weight, None, None, None, None, None
+
+
+def causal_lm_loss_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor, ignore_index: int = -100,
+                               loss_scale: float = 1.0, chunk_rows: int | None = None, valid_rows=None):
+    """causal_lm_loss_scaled(F.linear(hidden, weight), labels, loss_scale, ignore_index) from the last hidden states
+    (B, L, H) bf16 and the lm_head weight (V, H) bf16, H % 64 == 0, without the (B, L, V) logits and gradient tiles:
+    the valid rows (causal_lm_valid_rows; pass its result as `valid_rows` to take the host read earlier) are gathered
+    into a compact (N, H) matrix and go through _LinearCrossEntropyFn in chunks of `chunk_rows`.  Differentiable in
+    hidden and weight; the graph can be backpropagated ONCE.  -> (loss_scale * loss, loss)."""
+    L.require_cuda(hidden, weight, labels)
+    if hidden.dim() != 3 or weight.dim() != 2 or labels.shape != hidden.shape[:2] or weight.size(1) != hidden.size(2):
+        raise ValueError('expected hidden (B, L, H), weight (V, H) and labels (B, L)')
+    if hidden.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16:
+        raise ValueError(f'causal_lm_loss_from_hidden takes bf16 hidden states and head weight, got {hidden.dtype} and '
+                         f'{weight.dtype}: use causal_lm_loss on the logits')
+    B, seq, H = hidden.shape
+    if H % 64:
+        raise ValueError(f'causal_lm_loss_from_hidden needs a hidden size divisible by 64, got {H}: use causal_lm_loss '
+                         'on the logits')
+    if not torch.is_grad_enabled():  # eval under no_grad: a Parameter head would still report needs_input_grad
+        hidden, weight = hidden.detach(), weight.detach()
+    labels = labels.to(torch.int64)
+    idx, _ = causal_lm_valid_rows(labels, ignore_index) if valid_rows is None else valid_rows
+    shift = torch.full((B, seq), int(ignore_index), dtype=torch.int64, device=labels.device)
+    shift[:, :-1] = labels[:, 1:]
+    shift = shift.view(-1)
+    rows = hidden.reshape(B * seq, H).index_select(0, idx)
+    return _LinearCrossEntropyFn.apply(rows, _contiguous_last(weight), shift.index_select(0, idx), shift, int(ignore_index),
+                                       float(loss_scale), chunk_rows)
 
 
 # ---- masked mean ---------------------------------------------------------------------------------

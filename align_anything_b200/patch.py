@@ -13,7 +13,8 @@ swaps, without touching any reference file,
   * the same methods plus cumulative_returns of the text Multi-PPO trainer (trainers/text_to_text/multi_ppo.py:
     the five advantage estimators on K4 / K4r); its actor_step, reward_model_step and split_ptx_micro_batches stay
     the reference's,
-  * SupervisedTrainer.{loss, train_step} of the text / image / audio SFT trainers (cross-entropy from K1),
+  * SupervisedTrainer.{loss, train_step} of the text / image / audio SFT trainers (cross-entropy from K1; the classes
+    also get the `fused_lm_head` / `lm_head_chunk_rows` switches, off),
   * GRPOTrainer.{_get_per_token_logps, train_step} of the text trainer (the PPO and GRPO classes also get the
     `fused_lm_head` / `lm_head_chunk_rows` switches, off), RMTrainer.{loss, train_step} of the text /
     audio / video trainers (the audio and video trainers override `loss` with the text arithmetic, so their own `loss`
@@ -195,6 +196,9 @@ def install(trainers: bool = True, models: bool = True) -> dict[str, list[str]]:
             elif modname in _SFT_TARGETS:
                 _saved.append((cls, 'ignore_index', cls.__dict__.get('ignore_index', None)))
                 setattr(cls, 'ignore_index', -100)
+                for attr in ('fused_lm_head', 'lm_head_chunk_rows'):  # the switch the grafted loss reads
+                    _saved.append((cls, attr, cls.__dict__.get(attr, None)))
+                    setattr(cls, attr, getattr(src, attr))
         for modname, (clsname, src) in _SLICED_TARGETS.items():
             mod = _try_import(modname)
             cls = getattr(mod, clsname, None) if mod is not None else None

@@ -16,6 +16,11 @@ __all__ = ['SupervisedTrainer']
 
 class SupervisedTrainer:
     ignore_index = -100
+    # Opt-in: no (B, L, V) logits tile and no gradient tile.  The model is asked for its last hidden states
+    # (`output_hidden_states=True, logits_to_keep=1`: the lm_head runs on one position only) and the loss comes from
+    # ops.causal_lm_loss_from_hidden over the rows whose next label is not ignored; the gradient is formed in the forward.
+    fused_lm_head = False
+    lm_head_chunk_rows = None
 
     def __init__(self, cfgs, model, tokenizer=None, infer_batch=None) -> None:
         self.cfgs = cfgs
@@ -27,6 +32,15 @@ class SupervisedTrainer:
         """trainers/text_to_text/sft.py:95-98."""
         batch = dict(self.infer_batch(sft_batch))
         labels = batch.pop('labels')
+        if self.fused_lm_head:
+            # refuse a head the fused path would get wrong, then the valid-row index (the step's first host read: the
+            # previous step's read has drained the queue), both before the forward
+            weight = ops.lm_head_weight(getattr(self.model, 'module', self.model))
+            rows = ops.causal_lm_valid_rows(labels, self.ignore_index)
+            out = self.model(**batch, output_hidden_states=True, logits_to_keep=1)
+            loss = ops.causal_lm_loss_from_hidden(out.hidden_states[-1], weight, labels, self.ignore_index,
+                                                  chunk_rows=self.lm_head_chunk_rows, valid_rows=rows)[0]
+            return {'loss': loss}
         logits = self.model(**batch).logits
         return {'loss': ops.causal_lm_loss(logits, labels, self.ignore_index)}
 

@@ -469,6 +469,19 @@ int aa_linear_logprob_fwd(const void *hidden, int64_t n_rows, int32_t H, int64_t
                           void *out, int out_dtype, float *stat_max, float *stat_logsum, float *partial,
                           int64_t partial_floats, int mode, int32_t *status, void *stream);
 
+/* K6s: K6 with a second epilogue on the same accumulator tile -- every logit is rounded to bf16 (nn.Linear's rounding
+ * point, in both modes: the stored tile is bf16) and stored into `logits` (n_rows, ld), ld >= ceil(V / 256) * 256 and a
+ * multiple of 8 (columns >= V are written as +0), while (max, sum-exp, label logit) are folded from the same rounded
+ * values.  Everything else is aa_linear_logprob_fwd: `out` (FAITHFUL: the log-prob rounded to bf16; F32: not rounded),
+ * stat_max / stat_logsum, `partial` and the split-vocabulary merge, NaN and AA_STATUS_LABEL_OOB on an out-of-range
+ * label.  The forward of a loss whose gradient seed is known before any logit exists (the mean cross-entropy: every
+ * valid row's upstream gradient is -loss_scale / n_valid) then runs K1b on the stored tile instead of recomputing it
+ * in the backward (K6b): three GEMM passes over 2 * n_rows * H * V instead of four. */
+int aa_linear_logits(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
+                     const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
+                     void *out, int out_dtype, float *stat_max, float *stat_logsum, float *partial,
+                     int64_t partial_floats, int mode, int32_t *status, void *logits, int64_t ld, void *stream);
+
 /* K6b: K6's pipeline with a store epilogue -- the first of the three backward kernels of the fused lm_head x
  * log-prob path.  Recomputes the logits tile on the tensor cores and writes
  *   dlogits[r, j] = g[r] * ([j == labels[r]] - softmax_j)      (bf16; FAITHFUL: softmax from the rounded log-softmax)
