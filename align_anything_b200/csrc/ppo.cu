@@ -420,9 +420,10 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
       if (on) {
         if (l1 > l2) g1 = round_to(g_rs * (2.f * d1), rp);
         else if (l1 < l2) g2 = in_range ? round_to(g_rs * (2.f * d2), rp) : 0.f;
-        else {
-          g1 = round_to(0.5f * g_rs * (2.f * d1), rp);
-          g2 = in_range ? round_to(0.5f * g_rs * (2.f * d2), rp) : 0.f;
+        else {  // a tie: maximum's backward sends round(grad / 2) down each branch
+          const float half = round_to(0.5f * g_rs, rp);
+          g1 = round_to(half * (2.f * d1), rp);
+          g2 = in_range ? round_to(half * (2.f * d2), rp) : 0.f;
         }
       }
       grad = round_to(round_to(g1, rx) + round_to(g2, rx), rx);

@@ -32,10 +32,15 @@ __device__ __forceinline__ void actor_token(float x, float old, float aux, bool 
   const bool in_range = (ratio >= lo) && (ratio <= hi);
   float gs = 0.f;  // gradient reaching `ratio` through both branches of torch.minimum
   if (on) {
-    if (s1 < s2) gs = round_to(round_to(g_rs * aux, rp), rx);
-    else if (s1 == s2)
-      gs = in_range ? round_to(round_to(g_rs * aux, rp), rx)
-                    : round_to(round_to(0.5f * g_rs * aux, rp), rx);
+    if (s1 < s2) {
+      gs = round_to(round_to(g_rs * aux, rp), rx);
+    } else if (s1 == s2) {
+      // a tie: minimum's backward sends round(grad / 2) down each branch; through the clamp only in range, and the
+      // ratio's gradient is the sum of the two (rounded at each step: the halves differ from g_rs * aux / 2 once they
+      // are fp16 subnormals)
+      const float half = round_to(round_to(round_to(0.5f * g_rs, rp) * aux, rp), rx);
+      gs = in_range ? round_to(half + half, rx) : half;
+    }
     // s1 > s2: the clipped branch wins and clamp's backward is zero outside the range
   }
   grad = round_to(gs * ratio, rx);  // ExpBackward: grad * result
