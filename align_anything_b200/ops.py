@@ -12,7 +12,6 @@ plumbing only; all arithmetic on the path runs in the hand-written sm_90a kernel
 from __future__ import annotations
 
 import functools
-import os
 from typing import Sequence
 
 import torch
@@ -27,21 +26,21 @@ __all__ = [
     'causal_lm_loss_from_hidden', 'causal_lm_valid_rows',
 ]
 
-_REROUTE_TO_BASE = os.environ.get('AA_B200_REROUTE_BASE', '1') != '0'
-_K6B = os.environ.get('AA_B200_K6B', '1') != '0'  # 0: lm_head path with gradient through chunked cuBLAS + K1 / K1b instead of the tensor-core kernels
-_K6 = os.environ.get('AA_B200_K6', '1') != '0'  # 0: no-grad lm_head scoring through chunked cuBLAS + K1 instead of K6
-_ZERO_SPANS = os.environ.get('AA_B200_ZERO_SPANS', '1') != '0'  # 0: K1b zero-fills every unscored tile row itself
-_FUSED_ACTOR = os.environ.get('AA_B200_FUSED_ACTOR', '1') != '0'  # 0: the PPO actor node runs K1 -> K5 -> K1b instead of the single-pass K1f
-# fp16 logits keep the two-pass path by default: under fp16 training the incoming scalar is the loss scale (2^16 ...), and the
+# Path knobs: plain module attributes, read at call time and never from the environment.  Every path is chosen from the
+# input; these exist so that the tests, smoke() and bench.py can drive the other form of a node and compare the two.
+_K6B = True  # False: lm_head path with gradient through chunked cuBLAS + K1 / K1b instead of the tensor-core kernels
+_ZERO_SPANS = True  # False: K1b zero-fills every unscored tile row itself
+_FUSED_ACTOR = True  # False: the PPO actor node runs K1 -> K5 -> K1b instead of the single-pass K1f
+_FUSED_GRPO = True  # False: the GRPO loss runs K1 -> loss kernel -> K1b instead of the single-pass K1f
+_FUSED_CE = True  # False: causal_lm_loss runs K1 -> mean NLL -> K1b instead of the single-pass K1f
+# fp16 logits keep the two-pass path: under fp16 training the incoming scalar is the loss scale (2^16 ...), and the
 # two-pass backward folds it into the per-row gradient BEFORE the tile is rounded to fp16; a tile born unscaled would lose its
 # small entries to fp16 underflow -- exactly what loss scaling is there to prevent.  bf16 / fp32 have the exponent range.
-_FUSED_F16 = os.environ.get('AA_B200_FUSED_F16', '0') == '1'
+_FUSED_F16 = False
 # K1f keeps ONE row per SM in flight (that is what makes its second pass an L2 hit), so its per-row costs -- two block
 # reductions, the boundary thread, ring fill / drain -- weigh more the shorter the row is, and a short-vocabulary row
 # (32064 tokens) is faster on the two-pass path.  Rows below this many bytes keep K1 -> loss kernel -> K1b.
-_FUSED_MIN_ROW_BYTES = int(os.environ.get('AA_B200_FUSED_MIN_ROW_BYTES', str(192 * 1024)))
-_FUSED_GRPO = os.environ.get('AA_B200_FUSED_GRPO', '1') != '0'  # 0: the GRPO loss runs K1 -> loss kernel -> K1b instead of the single-pass K1f
-_FUSED_CE = os.environ.get('AA_B200_FUSED_CE', '1') != '0'  # 0: causal_lm_loss runs K1 -> mean NLL -> K1b instead of the single-pass K1f
+_FUSED_MIN_ROW_BYTES = 192 * 1024
 
 
 def _mode_code(mode: str | None, dtype: torch.dtype) -> int:
@@ -110,12 +109,32 @@ def _raise_status_bits(v: int) -> int:
     return v
 
 
-def _single_pass_ok(logits: torch.Tensor) -> bool:
-    """Whether the single-pass nodes (K1f) take this tile: not fp16 (the tile is written for an upstream gradient of 1 and
-    scaled afterwards, see _FUSED_F16) and rows long enough for K1f to win (see _FUSED_MIN_ROW_BYTES)."""
+def _single_pass_ok(logits: torch.Tensor, enabled: bool = True, needs_grad: bool = True) -> bool:
+    """Whether a single-pass node (K1f) takes this tile: the node's knob is on (`enabled`), a gradient tile is wanted
+    (K1f's second pass writes it; without one K1 alone reads the rows once), the logits are not fp16 (the tile is
+    written for an upstream gradient of 1 and scaled afterwards, see _FUSED_F16) and the rows are long enough for K1f
+    to win (see _FUSED_MIN_ROW_BYTES).  The public wrappers decide with it and hand the answer to their node."""
+    if not (enabled and needs_grad):
+        return False
     if logits.dtype == torch.float16 and not _FUSED_F16:
         return False
     return logits.size(-1) * logits.element_size() >= _FUSED_MIN_ROW_BYTES
+
+
+def _hand_over_once(ctx, g, *grads):
+    """Backward of a node whose forward already wrote its gradients: multiply them in place by the incoming scalar `g`
+    (aa_scale_tile, fp32 scalar; the kernel leaves at once when it is 1) and return them.  A second backward through
+    the same graph would scale the handed-over tensors again, so it raises."""
+    if getattr(ctx, 'consumed', False):
+        raise RuntimeError('a single-pass loss node hands its gradient over once: compute the loss again to run backward '
+                           'twice')
+    ctx.consumed = True
+    scale = g.detach().float().reshape(1).contiguous()
+    for t in grads:
+        if t is not None:
+            L.check(L.lib().aa_scale_tile(t.data_ptr(), L.dtype_code(t.dtype), t.numel(), scale.data_ptr(), L.AA_F32,
+                                          L.stream_ptr(t.device)))
+    return grads
 
 
 # ---- row plans -----------------------------------------------------------------------------------
@@ -336,12 +355,17 @@ def _launch_bwd(logits, labels, plan: RowPlan, stat_max, stat_logsum, grad_rows,
         L.ptr(scratch), mode_code, L.stream_ptr(dev)))
 
 
+def _rows_from(logits: torch.Tensor, first_row: int) -> torch.Tensor:
+    return logits if first_row == 0 else logits.view(-1, logits.size(-1))[first_row:]
+
+
 class _LogProbFn(torch.autograd.Function):
     """K1 forward / K1b backward.  `logits` is the tensor the gradient tile is shaped after; the plan
-    addresses rows inside it."""
+    addresses rows inside it, starting at row `first_row` of `logits` viewed as (rows, V) (nonzero only for
+    the contiguous base of a rerouted view, see _try_reroute)."""
 
     @staticmethod
-    def forward(ctx, logits, labels, plan: RowPlan, mode_code: int):
+    def forward(ctx, logits, labels, plan: RowPlan, mode_code: int, first_row: int = 0):
         out_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         n_out = 1
         for d in plan.out_shape:
@@ -353,23 +377,22 @@ class _LogProbFn(torch.autograd.Function):
         if need_grad:
             stats = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=logits.device)
             stat_max, stat_logsum = stats[0], stats[1]
-        _launch_fwd(logits, labels, plan, out, stat_max, stat_logsum)
+        _launch_fwd(_rows_from(logits, first_row), labels, plan, out, stat_max, stat_logsum)
         if need_grad:
             ctx.save_for_backward(logits, labels, stats)
-            ctx.plan = plan
-            ctx.mode_code = mode_code
+            ctx.plan, ctx.mode_code, ctx.first_row = plan, mode_code, first_row
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
         logits, labels, stats = ctx.saved_tensors
-        plan = ctx.plan
         grad_out = grad_out.contiguous()
         if grad_out.dtype not in (torch.float32, torch.bfloat16, torch.float16):
             grad_out = grad_out.float()
         grad = torch.empty(logits.shape, dtype=logits.dtype, device=logits.device)
-        _launch_bwd(logits, labels, plan, stats[0], stats[1], grad_out, None, None, grad, ctx.mode_code)
-        return grad, None, None, None
+        _launch_bwd(_rows_from(logits, ctx.first_row), labels, ctx.plan, stats[0], stats[1], grad_out, None, None, grad,
+                    ctx.mode_code)
+        return grad, None, None, None, None
 
 
 def _contiguous_last(t: torch.Tensor) -> torch.Tensor:
@@ -380,7 +403,7 @@ def _try_reroute(logits: torch.Tensor):
     """If `logits` is a row-aligned view of a contiguous base (e.g. `full[:, :-1]`,
     `full[idx][-R:]`), address the BASE instead so the backward writes the base's gradient tile
     directly (zero rows included) and autograd's slice-backward never materialises a padded copy."""
-    if not (_REROUTE_TO_BASE and logits._is_view()):
+    if not logits._is_view():
         return None
     base = logits._base
     V = logits.size(-1)
@@ -424,7 +447,7 @@ def gather_log_probabilities(logits: torch.Tensor, labels: torch.Tensor, mode: s
         # logits offsets in the plan are relative to the view's first row (row0 of the base); tile rows are
         # rows of the base, whose shape the gradient takes
         plan = _dense_plan(B, rows, sb_rows * V, V, lab_sb, row0, sb_rows, n_tile, dev)
-        out = _LogProbViewFn.apply(base, row0, labels, plan, mode_code)
+        out = _LogProbFn.apply(base, labels, plan, mode_code, row0)
     else:
         sb = logits.stride(0) if B > 1 else rows * logits.stride(1)
         plan = _dense_plan(B, rows, sb, logits.stride(1), lab_sb, 0, rows, B * rows, dev)
@@ -565,6 +588,12 @@ class _LinearLogProbK6Fn(torch.autograd.Function):
         return d_hidden, d_weight, None, None, None
 
 
+def _wgmma_head(hidden: torch.Tensor, weight: torch.Tensor) -> bool:
+    """Whether the tensor-core lm_head kernels (K6, K6b, aa_linear_dhidden / dweight) take these operands: bf16 hidden
+    states and weight, a hidden size divisible by 64.  Other operands go through library GEMMs around K1 / K1b."""
+    return hidden.dtype == weight.dtype == torch.bfloat16 and hidden.size(-1) % 64 == 0
+
+
 def linear_token_log_probs(hidden: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor,
                            chunk_rows: int | None = None, mode: str | None = None) -> torch.Tensor:
     """gather_log_probabilities(F.linear(hidden, weight), labels) for hidden (N, H), weight (V, H), labels (N,)
@@ -578,7 +607,7 @@ def linear_token_log_probs(hidden: torch.Tensor, weight: torch.Tensor, labels: t
     if hidden.size(0) == 0:
         return hidden.new_zeros((0,))
     labels = labels.to(torch.int64).contiguous()
-    if _K6B and hidden.dtype == torch.bfloat16 and hidden.size(1) % 64 == 0:
+    if _K6B and _wgmma_head(hidden, weight):
         if chunk_rows is None:  # ~2 GB of d(logits) per chunk: few read-modify-write passes over the fp32 d(weight)
             chunk_rows = max(128, (2 << 30) // ((V + 255) // 256 * 256 * 2) // 128 * 128)
         return _LinearLogProbK6Fn.apply(hidden.contiguous(), weight.contiguous(), labels, int(chunk_rows),
@@ -665,7 +694,7 @@ def _tails_from_hidden(hidden, weight, labels_padded, lens, counts, first_pos, l
     rows = hidden.reshape(n * seq, H).index_select(0, src)
     lab = labels_padded[:, lab_shift:lab_shift + W].reshape(-1).index_select(0, dst)
     needs_grad = torch.is_grad_enabled() and (hidden.requires_grad or weight.requires_grad)
-    if not needs_grad and _K6 and hidden.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16 and H % 64 == 0:
+    if not needs_grad and _wgmma_head(hidden, weight):
         lp = fused_linear_token_log_probs(rows, weight, lab, mode)  # K6: one tensor-core kernel, no logits at all
     else:
         lp = linear_token_log_probs(rows, weight, lab, chunk_rows, mode)
@@ -715,35 +744,6 @@ def dense_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, inpu
         raise ValueError(f'start = {start} lies outside [0, {seq - 1}] for sequences of {seq}')
     W = seq - 1 - start
     return _tails_from_hidden(hidden, weight, input_ids, (W,) * B, [W] * B, [start] * B, start + 1, chunk_rows, mode)
-
-
-class _LogProbViewFn(torch.autograd.Function):
-    """Same as _LogProbFn but the differentiable input is the contiguous BASE tensor of the view the caller
-    passed; the scored rows start at row `first_row` of the base viewed as (rows, V)."""
-
-    @staticmethod
-    def forward(ctx, base, first_row: int, labels, plan: RowPlan, mode_code: int):
-        V = base.size(-1)
-        view = base.view(-1, V)[first_row:]
-        out_dtype = base.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
-        out = torch.empty(plan.out_shape, dtype=out_dtype, device=base.device)
-        stats = torch.empty((2, plan.n_rows), dtype=torch.float32, device=base.device)
-        _launch_fwd(view, labels, plan, out, stats[0], stats[1])
-        ctx.save_for_backward(base, labels, stats)
-        ctx.plan, ctx.mode_code, ctx.first_row = plan, mode_code, first_row
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        base, labels, stats = ctx.saved_tensors
-        V = base.size(-1)
-        view = base.view(-1, V)[ctx.first_row:]
-        grad_out = grad_out.contiguous()
-        if grad_out.dtype not in (torch.float32, torch.bfloat16, torch.float16):
-            grad_out = grad_out.float()
-        grad = torch.empty(base.shape, dtype=base.dtype, device=base.device)
-        _launch_bwd(view, labels, ctx.plan, stats[0], stats[1], grad_out, None, None, grad, ctx.mode_code)
-        return grad, None, None, None, None
 
 
 # ---- DPO -----------------------------------------------------------------------------------------
@@ -1100,20 +1100,12 @@ class _GrpoFusedFn(torch.autograd.Function):
                                  mode_code, loss.data_ptr(), None, 0, row_end.data_ptr(), scratch.data_ptr(),
                                  sc['counter'][5:7].data_ptr(), L.stream_ptr(dev)))
         ctx.save_for_backward(grad)
-        ctx.consumed = False
         ctx.mark_non_differentiable(lp, row_end)
         return loss[0], lp, row_end
 
     @staticmethod
     def backward(ctx, g, _lp, _re):
-        (grad,) = ctx.saved_tensors
-        if ctx.consumed:
-            raise RuntimeError('the single-pass GRPO node hands its gradient tile over once: set AA_B200_FUSED_GRPO=0 to '
-                               'run backward twice through the same graph')
-        ctx.consumed = True
-        scale = g.detach().float().reshape(1).contiguous()
-        L.check(L.lib().aa_scale_tile(grad.data_ptr(), L.dtype_code(grad.dtype), grad.numel(), scale.data_ptr(), L.AA_F32,
-                                      L.stream_ptr(grad.device)))
+        (grad,) = _hand_over_once(ctx, g, *ctx.saved_tensors)
         return grad, None, None, None, None, None, None, None, None
 
 
@@ -1127,7 +1119,7 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
     L.require_cuda(logits, input_ids, ref_per_token_logps, advantages)
     K = int(logits_to_keep)
     tokens = input_ids[:, -K:]
-    if not (_FUSED_GRPO and _single_pass_ok(logits) and torch.is_grad_enabled() and logits.requires_grad):
+    if not _single_pass_ok(logits, _FUSED_GRPO, torch.is_grad_enabled() and logits.requires_grad):
         lp = tail_token_log_probs(logits, input_ids, K, mode=mode)
         loss, row_end = grpo_loss(lp, ref_per_token_logps, advantages, tokens, eos_token_id, beta, mode=mode)
         return loss, lp.detach(), row_end
@@ -1253,18 +1245,18 @@ class _CausalLMLossFn(torch.autograd.Function):
     With a gradient (default, K1f): ONE pass over the valid rows produces the fp32 log-probs AND the gradient tile
     (every valid row's upstream gradient is the same -loss_scale / n_valid, counted on the device before the pass;
     each row is streamed twice by one CTA, the second time out of L2); backward hands the tile over, multiplied in
-    place only if the incoming scalar is not 1.  AA_B200_FUSED_CE=0 / no gradient: K1 in fp32 mode over every
-    position (ignored labels cost no traffic), mean-NLL epilogue; backward: one K1b launch with the scalar
-    -loss_scale / n_valid as upstream gradient.  -> (loss_scale * loss, loss)."""
+    place only if the incoming scalar is not 1.  `single_pass` False (see _single_pass_ok) / no gradient: K1 in fp32
+    mode over every position (ignored labels cost no traffic), mean-NLL epilogue; backward: one K1b launch with the
+    scalar -loss_scale / n_valid as upstream gradient.  -> (loss_scale * loss, loss)."""
 
     @staticmethod
-    def forward(ctx, logits, shift_labels, ignore_index, loss_scale):
+    def forward(ctx, logits, shift_labels, ignore_index, loss_scale, single_pass):
         B, seq, V = logits.shape
         dev = logits.device
         plan = _dense_plan(B, seq, logits.stride(0) if B > 1 else seq * logits.stride(1), logits.stride(1), seq, 0, seq,
                            B * seq, str(dev))
         need_grad = ctx.needs_input_grad[0]
-        ctx.fused = bool(_FUSED_CE and need_grad and _single_pass_ok(logits))
+        ctx.fused = bool(single_pass)
         sc = _device_scratch(dev)
         out = torch.empty(3, dtype=torch.float32, device=dev)  # [loss, -1 / n_valid, -loss_scale / n_valid]
         if ctx.fused:
@@ -1287,7 +1279,6 @@ class _CausalLMLossFn(torch.autograd.Function):
                                     sc['counter'][4:5].data_ptr(), L.stream_ptr(dev)))
         if ctx.fused:
             ctx.save_for_backward(grad)
-            ctx.consumed = False
         elif need_grad:
             ctx.save_for_backward(logits, shift_labels, stats, out)
             ctx.plan, ctx.ignore_index = plan, int(ignore_index)
@@ -1300,21 +1291,14 @@ class _CausalLMLossFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g, _unused):
         if ctx.fused:
-            (grad,) = ctx.saved_tensors
-            if ctx.consumed:
-                raise RuntimeError('the single-pass cross-entropy node hands its gradient tile over once: set '
-                                   'AA_B200_FUSED_CE=0 to run backward twice through the same graph')
-            ctx.consumed = True
-            scale = g.detach().float().reshape(1).contiguous()
-            L.check(L.lib().aa_scale_tile(grad.data_ptr(), L.dtype_code(grad.dtype), grad.numel(), scale.data_ptr(),
-                                          L.AA_F32, L.stream_ptr(grad.device)))
-            return grad, None, None, None
+            (grad,) = _hand_over_once(ctx, g, *ctx.saved_tensors)
+            return grad, None, None, None, None
         logits, shift_labels, stats, out = ctx.saved_tensors
         grad = torch.empty(logits.shape, dtype=logits.dtype, device=logits.device)
         scale = (out[1] * (g.float() * ctx.loss_scale)).reshape(1).contiguous()
         _launch_bwd(logits, shift_labels, ctx.plan, stats[0], stats[1], None, None, scale, grad, L.MODE_F32,
                     ignore_index=ctx.ignore_index)
-        return grad, None, None, None
+        return grad, None, None, None, None
 
 
 def _shifted_labels(logits: torch.Tensor, labels: torch.Tensor, ignore_index: int):
@@ -1336,7 +1320,8 @@ def causal_lm_loss(logits: torch.Tensor, labels: torch.Tensor, ignore_index: int
     (trainers/text_to_text/sft.py:95-98) and of PPOTrainer.ptx_step (trainers/text_to_text/ppo.py:400-408).
     logits (B, L, V) in the model dtype, labels (B, L) -> fp32 scalar, differentiable in logits."""
     logits, shift = _shifted_labels(logits, labels, ignore_index)
-    return _CausalLMLossFn.apply(logits, shift, int(ignore_index), 1.0)[0]
+    single_pass = _single_pass_ok(logits, _FUSED_CE, torch.is_grad_enabled() and logits.requires_grad)
+    return _CausalLMLossFn.apply(logits, shift, int(ignore_index), 1.0, single_pass)[0]
 
 
 def causal_lm_loss_scaled(logits: torch.Tensor, labels: torch.Tensor, loss_scale: float, ignore_index: int = -100):
@@ -1344,7 +1329,8 @@ def causal_lm_loss_scaled(logits: torch.Tensor, labels: torch.Tensor, loss_scale
     `loss_scale` (ptx_step's `ptx_coeff * ptx_loss`, trainers/text_to_text/ppo.py:405), so no pass over the tile is spent
     on the multiplication; log the second."""
     logits, shift = _shifted_labels(logits, labels, ignore_index)
-    return _CausalLMLossFn.apply(logits, shift, int(ignore_index), float(loss_scale))
+    single_pass = _single_pass_ok(logits, _FUSED_CE, torch.is_grad_enabled() and logits.requires_grad)
+    return _CausalLMLossFn.apply(logits, shift, int(ignore_index), float(loss_scale), single_pass)
 
 
 # ---- causal-LM cross-entropy from the last hidden states (fused lm_head SFT) ---------------------------------------
@@ -1448,7 +1434,6 @@ class _LinearCrossEntropyFn(torch.autograd.Function):
                                                   d_weight.stride(0), st))
             _ce_loss_launch(logp, lab, N, ignore_index, out, dev)
         ctx.save_for_backward(d_rows, d_weight)
-        ctx.consumed = False
         loss = out[0]
         scaled = loss if loss_scale == 1.0 else loss * float(loss_scale)
         ctx.mark_non_differentiable(loss)
@@ -1456,16 +1441,7 @@ class _LinearCrossEntropyFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g, _unused):
-        if ctx.consumed:
-            raise RuntimeError('the fused lm_head cross-entropy node hands its gradients over once: compute the loss '
-                               'again to run backward twice')
-        ctx.consumed = True
-        d_rows, d_weight = ctx.saved_tensors
-        scale = g.detach().float().reshape(1).contiguous()
-        for t in (d_rows, d_weight):
-            if t is not None:
-                L.check(L.lib().aa_scale_tile(t.data_ptr(), L.dtype_code(t.dtype), t.numel(), scale.data_ptr(), L.AA_F32,
-                                              L.stream_ptr(t.device)))
+        d_rows, d_weight = _hand_over_once(ctx, g, *ctx.saved_tensors)
         return d_rows, d_weight, None, None, None, None, None
 
 
@@ -1820,16 +1796,17 @@ class _TailActorLossFn(torch.autograd.Function):
     token's own log-prob; each row is streamed twice by the same CTA and the second pass comes out of L2.  K5 then reduces
     the loss value from the log-probs; backward hands the tile over (aa_scale_tile multiplies it by the incoming scalar
     on the device iff that is not 1).
-    AA_B200_FUSED_ACTOR=0 (and rows without gradient): forward = K1 over the response tails + K5; backward = K1b taking
-    K5's d loss / d log-probs as its per-row upstream gradient and the incoming scalar as a device scale."""
+    `single_pass` False (see _single_pass_ok), or a plan K1f does not take: forward = K1 over the response tails + K5;
+    backward = K1b taking K5's d loss / d log-probs as its per-row upstream gradient and the incoming scalar as a device
+    scale."""
 
     @staticmethod
-    def forward(ctx, logits, ids, plan, old, aux, mask, clip, mode_code):
+    def forward(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, single_pass):
         out_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         dev = logits.device
         lp = torch.zeros(plan.out_shape, dtype=out_dtype, device=dev)
-        ctx.fused = bool(_FUSED_ACTOR and _single_pass_ok(logits) and ctx.needs_input_grad[0] and plan.n_tile_rows > 0 and plan.n_seg > 0
-                         and plan.n_tile_rows % plan.n_seg == 0 and len(plan.out_shape) == 2)
+        ctx.fused = bool(single_pass and plan.n_tile_rows > 0 and plan.n_seg > 0 and plan.n_tile_rows % plan.n_seg == 0
+                         and len(plan.out_shape) == 2)
         if ctx.fused:
             grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
             scratch = torch.empty(plan.n_tile_rows * 6, dtype=torch.int64, device=dev)  # 48 bytes per tile row
@@ -1842,7 +1819,6 @@ class _TailActorLossFn(torch.autograd.Function):
                 scratch.data_ptr(), _device_scratch(dev)['status'].data_ptr(), L.stream_ptr(dev)))
             loss, cast, _, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True)
             ctx.save_for_backward(grad)
-            ctx.consumed = False
         else:
             stats = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=dev)
             _launch_fwd(logits, ids, plan, lp, stats[0], stats[1])
@@ -1854,23 +1830,17 @@ class _TailActorLossFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_loss, _lp, _l):
+        if ctx.fused:
+            (grad,) = _hand_over_once(ctx, g_loss, *ctx.saved_tensors)
+            return grad, None, None, None, None, None, None, None, None
         scale = g_loss.detach().reshape(1)
         if scale.dtype not in (torch.float32, torch.bfloat16, torch.float16):
             scale = scale.float()
         scale = scale.contiguous()
-        if ctx.fused:
-            (grad,) = ctx.saved_tensors
-            if ctx.consumed:
-                raise RuntimeError('the single-pass actor node hands its gradient tile over once: set '
-                                   'AA_B200_FUSED_ACTOR=0 to run backward twice through the same graph')
-            ctx.consumed = True
-            L.check(L.lib().aa_scale_tile(grad.data_ptr(), L.dtype_code(grad.dtype), grad.numel(), scale.data_ptr(),
-                                          L.dtype_code(scale.dtype), L.stream_ptr(grad.device)))
-            return grad, None, None, None, None, None, None, None
         logits, ids, stats, grad_lp = ctx.saved_tensors
         grad = torch.empty(logits.shape, dtype=logits.dtype, device=logits.device)
         _launch_bwd(logits, ids, ctx.plan, stats[0], stats[1], grad_lp, None, scale, grad, ctx.mode_code)
-        return grad, None, None, None, None, None, None, None
+        return grad, None, None, None, None, None, None, None, None
 
 
 class _TailCriticLossFn(torch.autograd.Function):
@@ -1953,7 +1923,8 @@ def tail_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, lens, old_log
         aux = aux.float()
     m = _contiguous_last(mask.to(torch.bool))
     plan = device_tail_plan(lens, K, logits.stride(0), logits.stride(1), ids.stride(0), ids.size(1), 0, -1, lens.bound)
-    return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code)
+    single_pass = _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad)
+    return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass)
 
 
 @functools.lru_cache(maxsize=64)
@@ -1983,7 +1954,7 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
         raise ValueError(f'start = {start} leaves no scored position in a sequence of {Lq}')
     if not (tuple(old_log_probs.shape) == tuple(advantages.shape) == tuple(mask.shape) == (B, W)):
         raise ValueError('old_log_probs, advantages and mask must all be (B, L - 1 - start)')
-    if not (_FUSED_ACTOR and _single_pass_ok(logits) and torch.is_grad_enabled() and logits.requires_grad):
+    if not _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad):
         # short rows, fp16, no gradient: the composed ops (K1 over the response rows -> K5; backward K1b)
         lp = gather_log_probabilities(logits[:, start:-1], input_ids[:, start + 1:], mode=mode)
         loss = actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, mode=mode)
@@ -1999,7 +1970,7 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
         aux = aux.float()
     m = _contiguous_last(mask.to(torch.bool))
     plan = _dense_actor_plan(B, Lq, start, logits.stride(0), logits.stride(1), ids.stride(0), str(logits.device))
-    return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code)
+    return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, True)
 
 
 def tail_critic_loss(scores: torch.Tensor, lens, old_values, returns, mask, clip_range_value: float,
@@ -2123,9 +2094,6 @@ def response_tail_log_probs(logits: torch.Tensor, input_ids: torch.Tensor, lens,
     logits, ids = _contiguous_last(logits), input_ids.contiguous()
     plan = device_tail_plan(lens, K, logits.stride(0), logits.stride(1), ids.stride(0), ids.size(1), 0, -1, lens.bound)
     return _LogProbFn.apply(logits, ids, plan, _mode_code(mode, logits.dtype))
-
-
-_DUAL_K1 = os.environ.get('AA_B200_DUAL_K1', '1') != '0'  # actor + reference rollout scoring in ONE K1 launch (bit-identical, ~1% of the PPO step)
 
 
 def response_tail_log_probs_pair(logits_a: torch.Tensor, logits_b: torch.Tensor, input_ids: torch.Tensor, lens,

@@ -114,7 +114,7 @@ class PPOTrainer(_TextPPOTrainer):
         reward_batch = self.reward_model_step(actor_batch)
         ids = actor_batch['input_ids']
         lens = ops.as_device_lens(response_lens, ids.device)
-        if ops._DUAL_K1 and not self.fused_lm_head:  # EXPERIMENTAL: both models' tiles through ONE K1 launch
+        if not self.fused_lm_head:  # both models' tiles through ONE K1 launch
             log_probs, ref_log_probs = ops.response_tail_log_probs_pair(
                 self._actor_logits(self.actor_model, actor_batch, lens),
                 self._actor_logits(self.actor_reference_model, actor_batch, lens), ids, lens, mode=self.mode)

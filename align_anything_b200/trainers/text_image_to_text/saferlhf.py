@@ -120,14 +120,14 @@ class SafeRLHFVTrainer(_MMPPOTrainer):
                                                       sequence_mask)
         else:
             logits = self._actor_logits(self.actor_model, batch, lens, use_cache=False)
-            if ops._FUSED_ACTOR and ops._single_pass_ok(logits) and new_size == lens.bound == old_log_probs.size(-1):
+            if new_size == lens.bound == old_log_probs.size(-1):
                 # actor_loss_fn_with_cost (:432-451) is the clipped-ratio loss on the Lagrangian mix of the two advantages:
-                # the same single-pass actor node as the PPO trainers (K1f: log-probs, d loss / d log-prob, gradient tile)
+                # the same actor node as the PPO trainers, which picks the single-pass K1f or K1 -> K5 -> K1b itself
                 multiplier = self.log_lambda.exp().item()
                 advantages = (reward_advantages - multiplier * cost_advantages) / (1.0 + multiplier)
                 actor_loss, _, _ = ops.tail_actor_loss(logits, input_ids, lens, old_log_probs, advantages, sequence_mask,
                                                        self.clip_range_ratio, mode=self.mode)
-            else:  # short rows / fp16: K1 over the response tails -> K5; backward K1b
+            else:  # widths off the response bound (widened or truncated above): K1 over the tails -> K5; backward K1b
                 log_probs = ops.response_tail_log_probs(logits, input_ids, lens, mode=self.mode)
                 actor_loss = self.actor_loss_fn_with_cost(log_probs, old_log_probs, reward_advantages, cost_advantages,
                                                           sequence_mask)

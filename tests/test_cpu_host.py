@@ -538,17 +538,18 @@ def test_k1f_interleaved_work_list_is_a_permutation():
 
 def test_single_pass_routing(monkeypatch):
     """ops._single_pass_ok: K1f's tile is written for an upstream gradient of 1, so fp16 logits (loss scaling) stay on the
-    two-pass path unless AA_B200_FUSED_F16=1, and so do rows shorter than AA_B200_FUSED_MIN_ROW_BYTES (192 KB by default:
-    K1f measured 0.83x of the two-pass path at V = 32064 bf16, 1.15x at 128256, 1.25x at 152064)."""
+    two-pass path unless ops._FUSED_F16 is set, and so do rows shorter than ops._FUSED_MIN_ROW_BYTES (192 KB by default:
+    K1f measured 0.83x of the two-pass path at V = 32064 bf16, 1.15x at 128256, 1.25x at 152064), a node whose knob is
+    off, and logits that need no gradient."""
     from align_anything_b200 import ops
 
     def tile(V, dtype):
         return torch.empty((1, 1, V), dtype=dtype)
 
-    assert ops._FUSED_MIN_ROW_BYTES == 192 * 1024 or 'AA_B200_FUSED_MIN_ROW_BYTES' in os.environ
-    monkeypatch.setattr(ops, '_FUSED_MIN_ROW_BYTES', 192 * 1024)
-    monkeypatch.setattr(ops, '_FUSED_F16', False)
+    assert ops._FUSED_MIN_ROW_BYTES == 192 * 1024 and not ops._FUSED_F16
     assert ops._single_pass_ok(tile(152064, torch.bfloat16)) and ops._single_pass_ok(tile(128257, torch.bfloat16))
+    assert not ops._single_pass_ok(tile(152064, torch.bfloat16), enabled=False)
+    assert not ops._single_pass_ok(tile(152064, torch.bfloat16), needs_grad=False)
     assert not ops._single_pass_ok(tile(32064, torch.bfloat16)) and not ops._single_pass_ok(tile(65536, torch.bfloat16))
     assert ops._single_pass_ok(tile(65536, torch.float32))            # 256 KB rows
     assert not ops._single_pass_ok(tile(152064, torch.float16))       # fp16: loss scaling

@@ -45,19 +45,27 @@ class _FakeLib:
         return b''
 
 
-@pytest.fixture
-def dry(monkeypatch):
+def _install_dry(setattr_):
+    """Swap the stand-in library in through `setattr_` (monkeypatch.setattr, or the builtin in a subprocess)."""
     from align_anything_b200 import _lib, ops
 
     lib = _FakeLib(_lib._SIGS)
-    monkeypatch.setattr(_lib, 'lib', lambda: lib)
-    monkeypatch.setattr(_lib, 'require_cuda', lambda *t: None)
-    monkeypatch.setattr(_lib, 'stream_ptr', lambda device=None: 0)
-    monkeypatch.setattr(torch, 'empty', torch.zeros)  # outputs the kernels would have written: zeros (status word = 0)
-    monkeypatch.setattr(ops, '_scratch', {})
-    monkeypatch.setattr(ops, '_FUSED_MIN_ROW_BYTES', 0)  # the toy vocabularies here would take the two-pass path: drive K1f's calls
-    monkeypatch.setattr(ops, '_device_scratch', lambda device: ops._scratch.setdefault('cpu', {
+    setattr_(_lib, 'lib', lambda: lib)
+    setattr_(_lib, 'require_cuda', lambda *t: None)
+    setattr_(_lib, 'stream_ptr', lambda device=None: 0)
+    setattr_(torch, 'empty', torch.zeros)  # outputs the kernels would have written: zeros (status word = 0)
+    setattr_(ops, '_scratch', {})
+    setattr_(ops, '_device_scratch', lambda device: ops._scratch.setdefault('cpu', {
         'status': torch.zeros(1, dtype=torch.int32), 'counter': torch.zeros(8, dtype=torch.int32)}))
+    return lib
+
+
+@pytest.fixture
+def dry(monkeypatch):
+    from align_anything_b200 import ops
+
+    lib = _install_dry(monkeypatch.setattr)
+    monkeypatch.setattr(ops, '_FUSED_MIN_ROW_BYTES', 0)  # the toy vocabularies here would take the two-pass path: drive K1f's calls
     ops._lens_tensor.cache_clear()
     ops._tail_plan.cache_clear()
     ops._dense_plan.cache_clear()
@@ -218,8 +226,7 @@ def test_sibling_trainers_dry_run(dry):
     assert 'aa_logprob_grpo_fused' in dry.calls and 'aa_grpo_loss' in dry.calls  # the single-pass GRPO node
 
 
-def test_saferlhf_rollout_and_rl_step_dry_run(dry):
-    """Safe RLHF-V: actor_step -> score_rollout (reward + cost) -> rl_step, scalar-only dict with the 16 + 5 keys."""
+def _saferlhf_trainer():
     import copy
 
     from align_anything_b200.trainers.text_image_to_text.saferlhf import SafeRLHFVTrainer
@@ -240,6 +247,12 @@ def test_saferlhf_rollout_and_rl_step_dry_run(dry):
 
     t.cost_model_step = cost_model_step
     t.set_train = lambda mode=True: None
+    return t
+
+
+def test_saferlhf_rollout_and_rl_step_dry_run(dry):
+    """Safe RLHF-V: actor_step -> score_rollout (reward + cost) -> rl_step, scalar-only dict with the 16 + 5 keys."""
+    t = _saferlhf_trainer()
     inference, training = t.rollout(t.prompt_only_dataloader[0])
     assert len(inference) == len(training) == 1 and {'cost', 'cost_values', 'response_lens', 'response_mask'} <= set(training[0])
     out = t.rl_step(inference[0], training[0])
@@ -249,7 +262,7 @@ def test_saferlhf_rollout_and_rl_step_dry_run(dry):
 
 
 def test_short_rows_take_the_two_pass_calls(dry, monkeypatch):
-    """With the default AA_B200_FUSED_MIN_ROW_BYTES the toy vocabulary (97 tokens) is far too short for K1f: the text PPO
+    """With the default ops._FUSED_MIN_ROW_BYTES the toy vocabulary (97 tokens) is far too short for K1f: the text PPO
     rl_step must then call K1 -> K5 -> K1b (aa_logprob_fwd, aa_ppo_actor_loss, aa_logprob_bwd) and never the single-pass entry."""
     from align_anything_b200 import ops, patch
 
@@ -264,3 +277,67 @@ def test_short_rows_take_the_two_pass_calls(dry, monkeypatch):
             patch.uninstall()
     assert 'aa_logprob_actor_fused' not in dry.calls
     assert {'aa_logprob_fwd', 'aa_ppo_actor_loss', 'aa_logprob_bwd'} <= set(dry.calls)
+
+
+@pytest.mark.parametrize('min_row_bytes', [0, 192 * 1024])
+def test_saferlhf_actor_node_picks_its_path(dry, monkeypatch, min_row_bytes):
+    """SafeRLHF-V's rl_step hands the Lagrangian-mixed advantages to ops.tail_actor_loss and lets ops pick the path:
+    the single-pass K1f once the rows are long enough, K1 -> K5 -> K1b on the toy vocabulary's 194-byte rows at the
+    default threshold."""
+    from align_anything_b200 import ops
+
+    monkeypatch.setattr(ops, '_FUSED_MIN_ROW_BYTES', min_row_bytes)
+    t = _saferlhf_trainer()
+    inference, training = t.rollout(t.prompt_only_dataloader[0])
+    dry.calls.clear()
+    t.rl_step(inference[0], training[0])
+    if min_row_bytes == 0:
+        assert 'aa_logprob_actor_fused' in dry.calls and 'aa_logprob_bwd' not in dry.calls
+    else:
+        assert 'aa_logprob_actor_fused' not in dry.calls
+        assert {'aa_logprob_fwd', 'aa_ppo_actor_loss', 'aa_logprob_bwd'} <= set(dry.calls)
+
+
+_RETIRED_SWITCHES = {  # environment variables that once chose between duplicate paths, at their non-default values
+    'AA_B200_REROUTE_BASE': '0', 'AA_B200_K6': '0', 'AA_B200_K6B': '0', 'AA_B200_ZERO_SPANS': '0',
+    'AA_B200_FUSED_ACTOR': '0', 'AA_B200_FUSED_F16': '1', 'AA_B200_FUSED_MIN_ROW_BYTES': '0',
+    'AA_B200_FUSED_GRPO': '0', 'AA_B200_FUSED_CE': '0', 'AA_B200_DUAL_K1': '0',
+}
+
+_ENV_WORKER = r'''
+import sys
+sys.path[:0] = sys.argv[1:]
+import torch
+import test_cpu_plumbing as T
+from align_anything_b200 import ops
+knobs = (ops._K6B, ops._ZERO_SPANS, ops._FUSED_ACTOR, ops._FUSED_GRPO, ops._FUSED_CE, ops._FUSED_F16, ops._FUSED_MIN_ROW_BYTES)
+assert knobs == (True, True, True, True, True, False, 192 * 1024), knobs
+lib = T._install_dry(setattr)
+B, K, V = 2, 6, 98304  # 192 KB bf16 rows: long enough for the single-pass nodes
+gen = torch.Generator().manual_seed(0)
+logits = torch.randn(B, K, V, generator=gen).bfloat16().requires_grad_(True)
+ids = torch.randint(0, V, (B, K + 2), generator=gen)
+W = 3
+loss, _, _ = ops.tail_actor_loss(logits, ids, [W, 2], torch.zeros(B, W), torch.randn(B, W, generator=gen),
+                                 torch.ones(B, W, dtype=torch.bool), 0.2)
+loss.backward()
+assert 'aa_logprob_actor_fused' in lib.calls and 'aa_logprob_fwd' not in lib.calls, lib.calls
+lib.calls.clear()
+ops.causal_lm_loss(logits, torch.randint(0, V, (B, K), generator=gen)).backward()
+assert 'aa_logprob_ce_fused' in lib.calls and 'aa_logprob_fwd' not in lib.calls, lib.calls
+print('ok')
+'''
+
+
+def test_retired_switches_do_not_change_paths(tmp_path):
+    """The paths are chosen from the input alone: with every retired switch set, ops still starts from its defaults and
+    a long-row tile still reaches the single-pass actor and cross-entropy entry points."""
+    import os
+    import subprocess
+
+    tests = os.path.dirname(os.path.abspath(__file__))
+    script = tmp_path / 'worker.py'
+    script.write_text(_ENV_WORKER)
+    r = subprocess.run([sys.executable, str(script), os.path.dirname(tests), tests], env=dict(os.environ, **_RETIRED_SWITCHES),
+                       capture_output=True, text=True, timeout=300)
+    assert r.returncode == 0 and r.stdout.strip().endswith('ok'), r.stdout + r.stderr
