@@ -240,9 +240,10 @@ __global__ void __launch_bounds__(THREADS)
     out[B + i] = valid ? sh_div : 0;
     out[2 * B + i] = sh_ec;
     out[3 * B + i] = sh_er;
-    if (status) {
+    // only a valid pair raises: the reference skips an identical pair before it reads either mask row
+    if (status && valid) {
       if (sh_ec < 0 || sh_er < 0) atomicOr(status, AA_STATUS_EMPTY_MASK);
-      else if (valid && (sh_div > sh_ec || sh_div > sh_er)) atomicOr(status, AA_STATUS_DIVERGE_RANGE);  // the asserts
+      else if (sh_div > sh_ec || sh_div > sh_er) atomicOr(status, AA_STATUS_DIVERGE_RANGE);  // the asserts
     }
   }
 }

@@ -73,20 +73,24 @@ __global__ void __launch_bounds__(THREADS)
   }
 }
 
-// pad_sequence of per-sample tails (adjoint = 0):  out[b, k] = k < R_b ? src[b, W - R_b + k] : 0,  out (B, Rmax)
-// its adjoint, the gradient scatter (adjoint = 1):  out[b, j] = j >= W - R_b ? src[b, j - (W - R_b)] : 0,  out (B, W)
+// The tail rule (shared with the critic's tail load in ppo.cu and tail_plan_kernel below): R_b = clamp(lens[b], 0, W)
+// and the gathered span is row columns [W - R_b, W - R_b + n_b) with n_b = min(R_b, Rmax).
+// pad_sequence of per-sample tails (adjoint = 0):  out[b, k] = k < n_b ? src[b, W - R_b + k] : 0,  out (B, Rmax)
+// its exact transpose, the gradient scatter (adjoint = 1):
+//   out[b, j] = W - R_b <= j < W - R_b + n_b ? src[b, j - (W - R_b)] : 0,  out (B, W)
+// Neither direction touches a column outside row b of its operands, for any int32 length.
 template <typename U>
 __global__ void __launch_bounds__(256)
     tail_rows_kernel(const U *__restrict__ src, int64_t src_stride, const int32_t *__restrict__ lens, int W, int Rmax,
                      U *__restrict__ out, int64_t out_stride, int adjoint) {
   const int b = blockIdx.y;
   const int c = blockIdx.x * 256 + threadIdx.x;
-  const int R = lens[b];
-  const int off = W - R;
+  const int R = min(max(lens[b], 0), W);
+  const int off = W - R, n = min(R, Rmax);
   if (!adjoint) {
-    if (c < Rmax) out[b * out_stride + c] = (c < R) ? src[b * src_stride + off + c] : U(0);
+    if (c < Rmax) out[b * out_stride + c] = (c < n) ? src[b * src_stride + off + c] : U(0);
   } else {
-    if (c < W) out[b * out_stride + c] = (c >= off) ? src[b * src_stride + (c - off)] : U(0);
+    if (c < W) out[b * out_stride + c] = (c >= off && c < off + n) ? src[b * src_stride + (c - off)] : U(0);
   }
 }
 

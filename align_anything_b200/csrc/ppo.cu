@@ -377,8 +377,8 @@ struct LossParams {
   float *row_mean;      // optional: masked row mean of x
   float *row_scratch;   // [B] per-row masked means of the objective
   uint32_t *counter;
-  const int32_t *x_lens;  // optional: x[b, t] = t < lens[b] ? src[b, x_width - lens[b] + t] : 0  (the pad_sequence of
-  int x_width;            // per-sample tails of text_image_to_text/ppo.py:318-330 folded into the load)
+  const int32_t *x_lens;  // optional: x[b, t] = t < R_b ? src[b, x_width - R_b + t] : 0, R_b = clamp(lens[b], 0, x_width)
+  int x_width;            // (the pad_sequence of per-sample tails of text_image_to_text/ppo.py:318-330 folded into the load)
 };
 
 template <int THREADS, bool ACTOR>
@@ -457,7 +457,9 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
 
 // Gradient of the critic loss w.r.t. the RAW scores: the adjoint of `scores.squeeze(-1)[:, :-1]` followed by the
 // pad_sequence of per-sample tails (text_image_to_text/ppo.py:318-330), times the upstream scalar -- one launch writes
-// the whole (B, out_width) tile, zeros included:  out[b, t] = src_width - R_b <= t < src_width ? g * grad[b, t - (src_width - R_b)] : 0
+// the whole (B, out_width) tile, zeros included.  The exact transpose of the critic's tail load (x_lens above): with
+// R_b = clamp(lens[b], 0, src_width) and n_b = min(R_b, W),
+//   out[b, t] = src_width - R_b <= t < src_width - R_b + n_b ? g * grad[b, t - (src_width - R_b)] : 0
 template <typename T>
 __global__ void __launch_bounds__(256)
     tail_scatter_scaled_kernel(const T *__restrict__ grad, int64_t grad_stride, const int32_t *__restrict__ lens, int W,
@@ -466,10 +468,10 @@ __global__ void __launch_bounds__(256)
   const int b = blockIdx.y;
   const int t = blockIdx.x * 256 + threadIdx.x;
   if (t >= out_width) return;
-  const int R = min(max(lens[b], 0), min(W, src_width));
-  const int off = src_width - R;
+  const int R = min(max(lens[b], 0), src_width);
+  const int off = src_width - R, n = min(R, W);
   float v = 0.f;
-  if (t >= off && t < src_width) {
+  if (t >= off && t < off + n) {
     v = Traits<T>::to_float(grad[b * grad_stride + (t - off)]);
     if (scale) v = v * load_as_float(scale, 0, scale_dtype);  // fp32 product, one rounding (ATen's mul of a 16-bit tensor)
   }

@@ -196,7 +196,9 @@ int aa_dpo_loss(const void *policy_lp, const void *ref_lp, int lp_dtype, int32_t
  * Pair bookkeeping and slice sums of SimPO / ORPO / KTO (SURVEY.md 8f row 2).
  * aa_pair_slices: trainers/text_to_text/simpo.py:61-77 (orpo.py:61-77, kto.py:111-125): identical-pair test, last
  *   attended index of both rows, first index where the id rows differ -> out int32 [4][n_pairs] =
- *   valid, diverge_index, end_better, end_worse (bit-exact; 4 host syncs per pair in the reference).
+ *   valid, diverge_index, end_better, end_worse (bit-exact; 4 host syncs per pair in the reference).  Only a valid
+ *   pair sets AA_STATUS_EMPTY_MASK / AA_STATUS_DIVERGE_RANGE: the reference skips an identical pair before it reads
+ *   the masks.
  * aa_slice_sums: sums[r] = sum(lp[r, diverge : end + 1]) (simpo.py:78-79; Python slice semantics on the (2B, W)
  *   zero-padded log-prob rows), fp32 accumulate, rounded to the lp dtype in FAITHFUL mode; fp32 [2 * n_pairs] out.
  * The O(B) scalar formulas on top (log-ratio, log-sigmoid, odds ratio ...) are elementwise ATen ops on B-vectors in
@@ -317,8 +319,8 @@ int aa_ppo_returns(const void *rewards, int rew_dtype, int64_t rew_row_stride, c
  *   grad      : (B, Wm) d loss / d new_log_probs (resp. new values), input dtype, or NULL
  *   value_tail_lens / value_src_width (critic, optional): `values` is then the RAW (B, value_src_width) tensor
  *               `scores.squeeze(-1)[:, :-1]` and the kernel reads values[b, t] = t < R_b ? raw[b, value_src_width - R_b + t] : 0
- *               (the pad_sequence of per-sample tails of text_image_to_text/ppo.py:318-330 folded into the load);
- *               aa_tail_scatter_scaled is its adjoint.
+ *               with R_b = clamp(value_tail_lens[b], 0, value_src_width) (the pad_sequence of per-sample tails of
+ *               text_image_to_text/ppo.py:318-330 folded into the load); aa_tail_scatter_scaled is its exact transpose.
  *   row_mean  : optional fp32 [B], masked row mean of `new` values (critic: reward_value metric)
  *   counter   : device uint32 scratch (zero before first use; self-cleaning)
  * ------------------------------------------------------------------------------------- */
@@ -336,7 +338,8 @@ int aa_ppo_critic_loss(const void *values, int64_t val_stride, const void *old_v
                        int32_t value_src_width, void *stream);
 
 /* Adjoint of the tail gather above times an upstream scalar, one launch for the whole (B, out_width) tile (zeros
- * included): out[b, t] = src_width - R_b <= t < src_width ? scale * grad[b, t - (src_width - R_b)] : 0.  grad (B, W) and out
+ * included).  With the same R_b = clamp(lens[b], 0, src_width) and n_b = min(R_b, W):
+ * out[b, t] = src_width - R_b <= t < src_width - R_b + n_b ? scale * grad[b, t - (src_width - R_b)] : 0.  grad (B, W) and out
  * share `dtype`; scale: optional device scalar of scale_dtype (fp32 product, rounded once).  Replaces the autograd of
  * `scores.squeeze(-1)[:, :-1]` + per-sample slicing + pad_sequence (SliceBackward / CatBackward / a zero-filled tile). */
 int aa_tail_scatter_scaled(const void *grad, int dtype, int64_t grad_row_stride, const int32_t *lens, int32_t B, int32_t W,
@@ -546,9 +549,13 @@ int aa_tail_plan_build(const int32_t *response_lens, int32_t B, int32_t seq, int
 
 /* pad_sequence([x[b][-R_b:] for b], batch_first=True) -- trainers/text_image_to_text/ppo.py:233-249 (rollout) and
  * :318-330 (rl_step: critic values), a Python loop + pad_sequence in the reference -- and its adjoint.
- *   adjoint = 0:  src (B, W), out (B, Rmax):  out[b, k] = k < R_b ? src[b, W - R_b + k] : 0
- *   adjoint = 1:  src (B, Rmax), out (B, W):  out[b, j] = j >= W - R_b ? src[b, j - (W - R_b)] : 0   (gradient)
- * src / out hold `dtype` elements (bit copies); lens (B,) int32 on the device, 0 <= R_b <= Rmax <= W. */
+ * One tail rule, the one the critic's tail load and aa_tail_plan_build use: R_b = clamp(lens[b], 0, W), and the tail is
+ * columns [W - R_b, W - R_b + n_b) of the width-W row, n_b = min(R_b, Rmax).
+ *   adjoint = 0:  src (B, W), out (B, Rmax):  out[b, k] = k < n_b ? src[b, W - R_b + k] : 0
+ *   adjoint = 1:  src (B, Rmax), out (B, W):  out[b, j] = W - R_b <= j < W - R_b + n_b ? src[b, j - (W - R_b)] : 0
+ *                 (the gradient: the exact transpose of adjoint = 0)
+ * src / out hold `dtype` elements (bit copies); lens (B,) int32 on the device, Rmax <= W.  Lengths in [0, Rmax] are the
+ * intended use; any other int32 length follows the rule above, and no access leaves row b of src or out. */
 int aa_tail_rows(const void *src, int dtype, int64_t src_row_stride, const int32_t *lens, int32_t B, int32_t W,
                  int32_t Rmax, void *out, int64_t out_row_stride, int32_t adjoint, void *stream);
 

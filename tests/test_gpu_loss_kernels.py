@@ -43,10 +43,11 @@ gpu = pytest.mark.gpu
 BF, F16, F32, F64 = torch.bfloat16, torch.float16, torch.float32, torch.float64
 CODE = {BF: Lb.AA_BF16, F16: Lb.AA_F16, F32: Lb.AA_F32}
 FAITHFUL, F32MODE = Lb.MODE_FAITHFUL, Lb.MODE_F32
-# bit patterns: POISON is a NaN in bf16 / f16 (0x7FA5), fp32 (0x7FA5A5A5) and fp64; SENTINEL is finite
-POISON = {2: 0x7FA5, 4: 0x7FA5A5A5, 8: 0x7FA5A5A5A5A5A5A5}
-SENTINEL = {2: 0x3C5A, 4: 0x3C5A5A5A, 8: 0x3C5A5A5A5A5A5A5A}
-INT = {2: torch.int16, 4: torch.int32, 8: torch.int64}
+# bit patterns: POISON is a NaN in bf16 / f16 (0x7FA5), fp32 (0x7FA5A5A5) and fp64; SENTINEL is finite (bytes: neither
+# pattern is 0 or 1, so a byte mask output shows both a skipped and a stray write)
+POISON = {1: 0xA5, 2: 0x7FA5, 4: 0x7FA5A5A5, 8: 0x7FA5A5A5A5A5A5A5}
+SENTINEL = {1: 0x5A, 2: 0x3C5A, 4: 0x3C5A5A5A, 8: 0x3C5A5A5A5A5A5A5A}
+INT = {1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}
 EXACT = 2 ** 24
 U = 2.0 ** -24
 SEED = 4321
@@ -194,15 +195,16 @@ class Guarded:
             assert bool(un[~written].all()), f'{what}: {int((~un[~written]).sum())} elements written outside the contract'
 
 
-def fenced(values, stride=None, pad=None):
-    """`values` (rows, cols) placed between fence rows (>= 256 bytes on each side) in an allocation of row stride
-    `stride` >= cols; fence rows and pad columns hold `pad` (NaN for floats).  Returns the (rows, cols) view."""
+def fenced(values, stride=None, pad=None, reach=0):
+    """`values` (rows, cols) placed between fence rows (>= 256 bytes and >= `reach` elements on each side) in an
+    allocation of row stride `stride` >= cols; fence rows and pad columns hold `pad` (NaN for floats).  Returns the
+    (rows, cols) view."""
     rows, cols = values.shape
     stride = cols if stride is None else stride
     if pad is None:
         pad = float('nan') if values.is_floating_point() else -7
     esz = values.element_size()
-    extra = max(2, -(-256 // max(stride * esz, 1)))
+    extra = max(2, -(-max(256, reach * esz) // max(stride * esz, 1)))
     buf = torch.full((rows + 2 * extra, max(stride, 1)), pad, dtype=values.dtype, device=DEV)
     buf[extra:extra + rows, :cols] = values.to(DEV)
     return buf[extra:extra + rows, :cols]
