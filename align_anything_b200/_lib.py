@@ -42,6 +42,8 @@ _SIGS = {
     'aa_logprob_set_tuning_bwd': (c_int, [c_int, c_int]),
     'aa_logprob_fwd': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int64, c_int32, c_int32, c_int64, _P, _P, _P, _P,
                                _P, c_int, _P, _P, _P, _P]),
+    'aa_logprob_fwd_entropy': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int64, c_int32, c_int32, c_int64, _P, _P, _P,
+                                       _P, _P, c_int, _P, _P, _P, _P, c_int64, _P]),
     'aa_logprob_bwd': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int64, c_int32, c_int32, c_int64, _P, _P, _P, _P,
                                _P, _P, _P, _P, c_int, _P, _P, c_int, _P, c_int64, c_int64, _P, c_int64, _P, c_int, _P]),
     'aa_zero_rows': (c_int, [_P, c_int, c_int64, c_int32, c_int64, _P, c_int32, _P]),
@@ -50,6 +52,8 @@ _SIGS = {
     'aa_linear_dweight': (c_int, [_P, c_int64, c_int64, _P, c_int32, c_int64, c_int32, _P, c_int64, c_int32, _P, c_int64, _P]),
     'aa_linear_logprob_fwd': (c_int, [_P, c_int64, c_int32, c_int64, _P, c_int32, c_int64, _P, _P, c_int, _P, _P, _P, c_int64,
                                       c_int, _P, _P]),
+    'aa_linear_logprob_fwd_entropy': (c_int, [_P, c_int64, c_int32, c_int64, _P, c_int32, c_int64, _P, _P, c_int, _P, _P,
+                                              _P, c_int64, c_int, _P, _P, _P]),
     'aa_linear_logits': (c_int, [_P, c_int64, c_int32, c_int64, _P, c_int32, c_int64, _P, _P, c_int, _P, _P, _P, c_int64,
                                  c_int, _P, _P, c_int64, _P]),
     'aa_strip_pad_tail': (c_int, [_P, c_int32, c_int32, c_int64, c_int64, c_int, _P, _P, c_int64, _P, _P]),
@@ -80,6 +84,9 @@ _SIGS = {
                                     c_float, _P, c_int64, _P, _P, _P, _P]),
     'aa_logprob_grpo_fused': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P, c_int, _P, c_int64,
                                       _P, _P, c_int64, c_int64, c_int32, c_float, c_int, _P, c_int64, _P, _P, _P, _P, _P, _P]),
+    'aa_logprob_grpo_fused_entropy': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P, c_int,
+                                              _P, c_int64, _P, _P, c_int64, c_int64, c_int32, c_float, c_int, _P, c_int64, _P,
+                                              _P, _P, _P, _P, _P, _P]),
     'aa_scale_tile': (c_int, [_P, c_int, c_int64, _P, c_int, _P]),
     'aa_tail_scatter_scaled': (c_int, [_P, c_int, c_int64, _P, c_int32, c_int32, c_int32, _P, c_int, _P, c_int64, c_int32, _P]),
     'aa_group_advantages': (c_int, [_P, c_int32, c_int32, _P, _P]),

@@ -38,7 +38,8 @@ struct Params {
   int rot_groups;                 // CTAs start their sweep (m_tile % rot_groups) * rot_step tiles into the range
   int rot_step;
   int group_tiles, m_tiles;       // linear block id -> (row-tile group, split, row tile in group); see the host code
-  float *partial;                 // v_splits > 1: (row, split) -> {max, sum, label logit}
+  float *partial;                 // v_splits > 1: (row, split) -> {max, sum, label logit[, entropy sum t]}
+  float *entropy;                 // ENT kernels: fp32 entropy per row
 };
 
 // the tile store of K6b (d(logits)) and K6s (the logits): the upstream gradient per row (K6b) and the padded bf16 buffer
@@ -66,13 +67,25 @@ __device__ __forceinline__ void lse_merge(float &m, float &s, float m_o, float s
   m = mn;
 }
 
+// the same with the entropy sum t = sum e^{x - m} (x - m) (logprob_math.cuh: t' = alpha (t + (m - m') s)); the (m, s)
+// arithmetic is lse_merge's, so the statistics do not depend on whether the entropy is on
+__device__ __forceinline__ float ent_part(float t, float s, float m, float mn) {
+  return m == -INFINITY ? 0.f : (m == mn ? t : ex2_approx((m - mn) * kLog2e) * fmaf(m - mn, s, t));
+}
+__device__ __forceinline__ void lse_merge_ent(float &m, float &s, float &t, float m_o, float s_o, float t_o) {
+  const float mn = fmaxf(m, m_o);
+  if (mn == -INFINITY) return;
+  t = ent_part(t, s, m, mn) + ent_part(t_o, s_o, m_o, mn);
+  lse_merge(m, s, m_o, s_o);
+}
+
 // K6, K6b and K6s are ONE kernel: same TMA producer, same wgmma main loop; they differ in what the consumer
 // warpgroups do with a finished 128 x 256 logits tile (Epi) -- fold it into the running (max, sum-exp, label logit) of
 // the row, turn it into d(logits) with the statistics K6 saved and store it as bf16, or (K6s) fold it AND store the
 // bf16-rounded logits, so that the logits of a loss whose gradient seed is known in the forward cost one GEMM pass.
 // Each consumer thread holds 2 rows x 64 columns of the tile (wgmma.cuh, frag_row / frag_col); the 4 threads of a quad
 // share a row, so the per-row statistics are per-thread partials merged across the quad once, at the end.
-template <Epi EPI>
+template <Epi EPI, bool ENT = false>
 __global__ void __launch_bounds__(THREADS, 1)
     linear_logprob_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                           const Params p, const GradParams gp) {
@@ -161,6 +174,7 @@ __global__ void __launch_bounds__(THREADS, 1)
 #pragma unroll
     for (int r = 0; r < 2; ++r) lab[r] = (label[r] >= 0 && label[r] < p.V) ? static_cast<int>(label[r]) : -BN;
     float m[2] = {-INFINITY, -INFINITY}, s[2] = {0.f, 0.f}, x_label[2] = {-INFINITY, -INFINITY};
+    float ent_t[2] = {0.f, 0.f};  // ENT: running sum e^{x - m} (x - m) of the values the statistics fold
     for (int nt = 0; nt < n_tiles; ++nt) {
       consume_tile<0, 0>(acc, tiles, full, empty, k_blocks, it, w);
       const int col_base = (t0 + (nt + rot) % n_tiles) * BN;
@@ -187,10 +201,13 @@ __global__ void __launch_bounds__(THREADS, 1)
         for (int i = 2 * r; i < ACC; i += 4) cmax = fmaxf(cmax, fmaxf(acc[i], acc[i + 1]));
         if (EPI == Epi::Logits || p.faithful) cmax = bf16_round(cmax);
         if (cmax > m[r]) {  // m == -inf implies s == 0
+          if constexpr (ENT) {
+            if (m[r] != -INFINITY) ent_t[r] = ex2_approx((m[r] - cmax) * kLog2e) * fmaf(m[r] - cmax, s[r], ent_t[r]);
+          }
           s[r] *= ex2_approx((m[r] - cmax) * kLog2e);
           m[r] = cmax;
         }
-        float add = 0.f;
+        float add = 0.f, tadd = 0.f;
 #pragma unroll
         for (int i = 2 * r; i < ACC; i += 4) {
           float x0 = acc[i], x1 = acc[i + 1];
@@ -203,9 +220,18 @@ __global__ void __launch_bounds__(THREADS, 1)
           } else {
             if (p.faithful) round_bf16_pair(x0, x1);
           }
-          add += ex2_approx((x0 - m[r]) * kLog2e) + ex2_approx((x1 - m[r]) * kLog2e);
+          if constexpr (ENT) {
+            // pad columns of the last tile are -inf: their (x - m) is clamped so that the term is 0 * finite
+            const float d0 = x0 - m[r], d1 = x1 - m[r];
+            const float e0 = ex2_approx(d0 * kLog2e), e1 = ex2_approx(d1 * kLog2e);
+            add += e0 + e1;
+            tadd = fmaf(e0, fmaxf(d0, -3.0e38f), fmaf(e1, fmaxf(d1, -3.0e38f), tadd));
+          } else {
+            add += ex2_approx((x0 - m[r]) * kLog2e) + ex2_approx((x1 - m[r]) * kLog2e);
+          }
         }
         s[r] += add;
+        if constexpr (ENT) ent_t[r] += tadd;
       }
     }
 #pragma unroll
@@ -215,14 +241,19 @@ __global__ void __launch_bounds__(THREADS, 1)
       for (int o = 1; o <= 2; o <<= 1) {
         const float m_o = __shfl_xor_sync(0xffffffffu, m[r], o), s_o = __shfl_xor_sync(0xffffffffu, s[r], o);
         x_label[r] = fmaxf(x_label[r], __shfl_xor_sync(0xffffffffu, x_label[r], o));
-        lse_merge(m[r], s[r], m_o, s_o);
+        if constexpr (ENT) {
+          lse_merge_ent(m[r], s[r], ent_t[r], m_o, s_o, __shfl_xor_sync(0xffffffffu, ent_t[r], o));
+        } else {
+          lse_merge(m[r], s[r], m_o, s_o);
+        }
       }
       if ((t & 3) != 0 || !live[r]) continue;
       if (p.v_splits > 1) {
-        float *dst = p.partial + (row[r] * p.v_splits + split) * 3;
+        float *dst = p.partial + (row[r] * p.v_splits + split) * (ENT ? 4 : 3);
         dst[0] = m[r];
         dst[1] = s[r];
         dst[2] = x_label[r];
+        if constexpr (ENT) dst[3] = ent_t[r];
       } else {
         const float logsum = logf(s[r]);
         float lp = (x_label[r] - m[r]) - logsum;
@@ -231,6 +262,7 @@ __global__ void __launch_bounds__(THREADS, 1)
         store_from_float(p.out, row[r], p.out_dtype, lp);
         if (p.stat_max) p.stat_max[row[r]] = m[r];
         if (p.stat_logsum) p.stat_logsum[row[r]] = logsum;
+        if constexpr (ENT) p.entropy[row[r]] = logsum - ent_t[r] / s[r];
       }
     }
   } else {
@@ -269,18 +301,25 @@ __global__ void __launch_bounds__(THREADS, 1)
   }
 }
 
-// v_splits > 1: merge the per-split (max, sum, label logit) of each row
+// v_splits > 1: merge the per-split (max, sum, label logit[, entropy sum]) of each row
+template <bool ENT = false>
 __global__ void linear_logprob_merge_kernel(const Params p) {
+  constexpr int F = ENT ? 4 : 3;  // floats per (row, split)
   const int64_t row = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (row >= p.n_rows) return;
-  const float *src = p.partial + row * p.v_splits * 3;
+  const float *src = p.partial + row * p.v_splits * F;
   float m = -INFINITY, x_label = -INFINITY;
   for (int i = 0; i < p.v_splits; ++i) {
-    m = fmaxf(m, src[3 * i]);
-    x_label = fmaxf(x_label, src[3 * i + 2]);  // exactly one split holds the label column
+    m = fmaxf(m, src[F * i]);
+    x_label = fmaxf(x_label, src[F * i + 2]);  // exactly one split holds the label column
   }
   float s = 0.f;
-  for (int i = 0; i < p.v_splits; ++i) s += src[3 * i + 1] * ex2_approx((src[3 * i] - m) * kLog2e);
+  for (int i = 0; i < p.v_splits; ++i) s += src[F * i + 1] * ex2_approx((src[F * i] - m) * kLog2e);
+  if constexpr (ENT) {  // t = sum_i alpha_i (t_i + (m_i - m) s_i), alpha_i = e^{m_i - m}
+    float t = 0.f;
+    for (int i = 0; i < p.v_splits; ++i) t += ent_part(src[F * i + 3], src[F * i + 1], src[F * i], m);
+    p.entropy[row] = logf(s) - t / s;
+  }
   const int64_t label = __ldg(p.labels + row);
   const float logsum = logf(s);
   float lp = (x_label - m) - logsum;
@@ -306,7 +345,7 @@ struct Schedule {
   int64_t splits, group, n_groups, units;
   int tps;
 };
-static Schedule make_schedule(int64_t n_rows, int V, bool may_split, int64_t partial_floats) {
+static Schedule make_schedule(int64_t n_rows, int V, bool may_split, int64_t partial_floats, int per_split = 3) {
   const int rows_per_unit = BM;
   const int S = sm_count();
   Schedule sc;
@@ -335,7 +374,7 @@ static Schedule make_schedule(int64_t n_rows, int V, bool may_split, int64_t par
     }
     if (sc.splits > all_tiles) sc.splits = all_tiles;
     if (sc.splits < 1) sc.splits = 1;
-    while (partial_floats >= 0 && sc.splits > 1 && n_rows * sc.splits * 3 > partial_floats) --sc.splits;
+    while (partial_floats >= 0 && sc.splits > 1 && n_rows * sc.splits * per_split > partial_floats) --sc.splits;
     if (sc.group > sc.units) sc.group = sc.units;
     if (sc.group < 1) sc.group = 1;
   }
@@ -345,7 +384,7 @@ static Schedule make_schedule(int64_t n_rows, int V, bool may_split, int64_t par
   return sc;
 }
 
-template <Epi EPI>
+template <Epi EPI, bool ENT = false>
 static int launch(const void *hidden, int64_t n_rows, int H, int64_t hidden_row_stride, const void *weight, int V,
                   int64_t weight_row_stride, Params p, const GradParams &gp, const Schedule &sc, cudaStream_t st,
                   const char *who) {
@@ -359,7 +398,7 @@ static int launch(const void *hidden, int64_t n_rows, int H, int64_t hidden_row_
   p.group_tiles = static_cast<int>(sc.group);
   p.m_tiles = static_cast<int>(sc.units);
   const unsigned units = static_cast<unsigned>(sc.n_groups * sc.group * sc.splits);
-  auto kern = linear_logprob_kernel<EPI>;
+  auto kern = linear_logprob_kernel<EPI, ENT>;
   static std::atomic<bool> configured{false};  // once per process (idempotent; a race sets it twice, harmlessly)
   if (!configured.load(std::memory_order_relaxed)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
@@ -374,11 +413,11 @@ static int launch(const void *hidden, int64_t n_rows, int H, int64_t hidden_row_
 }
 
 // K6 / K6s: argument checks, the launch and (split vocabulary) the merge of the per-split statistics
-template <Epi EPI>
+template <Epi EPI, bool ENT = false>
 static int forward(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride, const void *weight,
                    int32_t V, int64_t weight_row_stride, const int64_t *labels, void *out, int out_dtype,
                    float *stat_max, float *stat_logsum, float *partial, int64_t partial_floats, int mode,
-                   int32_t *status, const GradParams &gp, void *stream, const char *who) {
+                   int32_t *status, const GradParams &gp, void *stream, const char *who, float *entropy = nullptr) {
   AA_REQUIRE(n_rows >= 0 && H > 0 && V > 0, AA_ERR_ARG, "%s: bad sizes", who);
   if (n_rows == 0) return AA_OK;
   AA_REQUIRE(hidden && weight && labels && out, AA_ERR_ARG, "%s: null pointer", who);
@@ -389,15 +428,15 @@ static int forward(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden
   AA_REQUIRE(out_dtype == AA_BF16 || out_dtype == AA_F32, AA_ERR_DTYPE, "%s: out must be bf16 or f32", who);
   AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "%s: bad mode", who);
   AA_REQUIRE(n_rows < (int64_t(1) << 31) - BM, AA_ERR_UNSUPPORTED, "%s: too many rows", who);
-  const Schedule sc = make_schedule(n_rows, V, partial != nullptr, partial_floats);
+  const Schedule sc = make_schedule(n_rows, V, partial != nullptr, partial_floats, ENT ? 4 : 3);
   Params p{labels, n_rows, V, H, out, out_dtype, stat_max, stat_logsum, mode == AA_MODE_FAITHFUL ? 1 : 0, status,
-           1, 1, 1, 1, 1, 1, partial};
+           1, 1, 1, 1, 1, 1, partial, entropy};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = launch<EPI>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, p, gp, sc, st, who);
+  int rc = launch<EPI, ENT>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, p, gp, sc, st, who);
   p.v_splits = static_cast<int>(sc.splits);  // the merge kernel reads the split count
   const int64_t splits = sc.splits;
   if (rc || splits == 1) return rc;
-  linear_logprob_merge_kernel<<<static_cast<unsigned>((n_rows + 255) / 256), 256, 0, st>>>(p);
+  linear_logprob_merge_kernel<ENT><<<static_cast<unsigned>((n_rows + 255) / 256), 256, 0, st>>>(p);
   return check_launch(EPI == Epi::Logits ? "aa_linear_logits(merge)" : "aa_linear_logprob_fwd(merge)");
 }
 }  // namespace k6
@@ -412,6 +451,18 @@ extern "C" int aa_linear_logprob_fwd(const void *hidden, int64_t n_rows, int32_t
   return k6::forward<k6::Epi::Lse>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, labels, out,
                                    out_dtype, stat_max, stat_logsum, partial, partial_floats, mode, status,
                                    k6::GradParams{nullptr, AA_F32, nullptr, 0}, stream, "aa_linear_logprob_fwd");
+}
+
+extern "C" int aa_linear_logprob_fwd_entropy(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
+                                             const void *weight, int32_t V, int64_t weight_row_stride,
+                                             const int64_t *labels, void *out, int out_dtype, float *stat_max,
+                                             float *stat_logsum, float *partial, int64_t partial_floats, int mode,
+                                             int32_t *status, float *entropy, void *stream) {
+  AA_REQUIRE(n_rows == 0 || entropy, AA_ERR_ARG, "aa_linear_logprob_fwd_entropy: null entropy");
+  return k6::forward<k6::Epi::Lse, true>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, labels, out,
+                                         out_dtype, stat_max, stat_logsum, partial, partial_floats, mode, status,
+                                         k6::GradParams{nullptr, AA_F32, nullptr, 0}, stream,
+                                         "aa_linear_logprob_fwd_entropy", entropy);
 }
 
 extern "C" int aa_linear_logits(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
@@ -452,7 +503,7 @@ extern "C" int aa_linear_dlogits(const void *hidden, int64_t n_rows, int32_t H, 
   AA_REQUIRE(n_rows < (int64_t(1) << 31) - k6::BM, AA_ERR_UNSUPPORTED, "aa_linear_dlogits: too many rows");
   const k6::Schedule sc = k6::make_schedule(n_rows, V, true, -1);
   k6::Params p{labels, n_rows, V, H, nullptr, AA_BF16, const_cast<float *>(stat_max), const_cast<float *>(stat_logsum),
-               mode == AA_MODE_FAITHFUL ? 1 : 0, nullptr, 1, 1, 1, 1, 1, 1, nullptr};
+               mode == AA_MODE_FAITHFUL ? 1 : 0, nullptr, 1, 1, 1, 1, 1, 1, nullptr, nullptr};
   k6::GradParams gp{grad_rows, grad_rows_dtype, static_cast<__nv_bfloat16 *>(dlogits), ld};
   return k6::launch<k6::Epi::DLogits>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, p, gp, sc,
                           static_cast<cudaStream_t>(stream), "aa_linear_dlogits");

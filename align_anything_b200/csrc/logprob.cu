@@ -32,6 +32,9 @@ struct FwdParams {
   float *stat_logsum;
   int32_t *status;
   float log2e;  // = kLog2e, passed at run time so that ptxas keeps the packed FMUL2 (no immediate form)
+  // entropy kernels only (ENT = true): fp32 entropy of the row at its out position, for out positions < n_entropy
+  float *entropy;
+  int64_t n_entropy;
 };
 
 struct BwdParams {
@@ -63,10 +66,11 @@ __host__ __device__ __forceinline__ int64_t bwd_work_rows(const BwdParams &p) {
 }
 
 // ---- K1 forward, LDG: direct vectorised loads (rows of 128 KB and more, see launch_fwd) -------------
-template <typename T, int THREADS, int UNROLL>
+template <typename T, int THREADS, int UNROLL, bool ENT = false>
 __global__ void __launch_bounds__(THREADS) logprob_fwd_kernel(const FwdParams p) {
   constexpr int E = Traits<T>::kVec;
   __shared__ float sh_m[32], sh_s[32];
+  __shared__ float sh_t[ENT ? 32 : 1];
   const int tid = threadIdx.x;
   const T *__restrict__ logits = reinterpret_cast<const T *>(p.logits);
   const int V = p.V;
@@ -84,6 +88,10 @@ __global__ void __launch_bounds__(THREADS) logprob_fwd_kernel(const FwdParams p)
     if (p.use_ignore && y == p.ignore_index) {  // ignored position (cross-entropy ignore_index): no traffic
       if (tid == 0) {
         store_from_float(p.out, __ldg(p.map.seg_out_off + seg) + j, p.out_dtype, 0.f);
+        if constexpr (ENT) {
+          const int64_t o = __ldg(p.map.seg_out_off + seg) + j;
+          if (o < p.n_entropy) p.entropy[o] = 0.f;
+        }
         if (p.stat_max) {
           p.stat_max[row] = 0.f;
           p.stat_logsum[row] = 0.f;
@@ -104,16 +112,16 @@ __global__ void __launch_bounds__(THREADS) logprob_fwd_kernel(const FwdParams p)
     const int tail0 = head + nvec * E;
     const uint4 *body = reinterpret_cast<const uint4 *>(x + head);
 
-    float m = -INFINITY, s = 0.f;
-    if (tid < head) lse_push(m, s, Traits<T>::to_float(x[tid]));
-    if (tid < V - tail0) lse_push(m, s, Traits<T>::to_float(x[tail0 + tid]));
+    float m = -INFINITY, s = 0.f, t = 0.f;
+    if (tid < head) lse_push_t<ENT>(m, s, t, Traits<T>::to_float(x[tid]));
+    if (tid < V - tail0) lse_push_t<ENT>(m, s, t, Traits<T>::to_float(x[tail0 + tid]));
 
     int k = tid;
     for (; k + (UNROLL - 1) * THREADS < nvec; k += UNROLL * THREADS) {
       uint4 v[UNROLL];
 #pragma unroll
       for (int u = 0; u < UNROLL; ++u) v[u] = ldg_stream(body + k + u * THREADS);
-      fold_batch<T, UNROLL>(v, m, s, L2);
+      fold_batch_t<T, UNROLL, ENT>(v, m, s, t, L2);
     }
     if (k < nvec) {  // last, partial batch: missing vectors are replaced by -inf (exp -> 0), one fold instead of
                      // up to UNROLL-1 single-vector folds (each of which pays its own max / rescale)
@@ -121,10 +129,10 @@ __global__ void __launch_bounds__(THREADS) logprob_fwd_kernel(const FwdParams p)
 #pragma unroll
       for (int u = 0; u < UNROLL; ++u)
         v[u] = (k + u * THREADS < nvec) ? ldg_stream(body + k + u * THREADS) : bulk::neg_inf_vec<T>();
-      fold_batch<T, UNROLL>(v, m, s, L2);
+      fold_batch_t<T, UNROLL, ENT>(v, m, s, t, L2);
     }
 
-    block_lse<THREADS>(m, s, sh_m, sh_s);
+    block_lse_t<THREADS, ENT>(m, s, t, sh_m, sh_s, sh_t);
     if (tid == 0) {
       const float logsum = logf(s);
       float lp = (xy - m) - logsum;  // same association as ATen's `x - max - log(sum)`
@@ -133,6 +141,10 @@ __global__ void __launch_bounds__(THREADS) logprob_fwd_kernel(const FwdParams p)
         if (p.status) atomicOr(p.status, AA_STATUS_LABEL_OOB);
       }
       store_from_float(p.out, __ldg(p.map.seg_out_off + seg) + j, p.out_dtype, lp);
+      if constexpr (ENT) {
+        const int64_t o = __ldg(p.map.seg_out_off + seg) + j;
+        if (o < p.n_entropy) p.entropy[o] = entropy_of(logsum, s, t);
+      }
       if (p.stat_max) {
         p.stat_max[row] = m;
         p.stat_logsum[row] = logsum;
@@ -169,7 +181,7 @@ constexpr size_t fwd_ring_smem() {
          2 * kFwdDescs * sizeof(uint64_t) + kFwdDescs * sizeof(FwdRowDesc);
 }
 
-template <typename T, int CONSUMERS, int STAGES, int UNROLL>
+template <typename T, int CONSUMERS, int STAGES, int UNROLL, bool ENT = false>
 __global__ void __launch_bounds__(CONSUMERS + 32) logprob_fwd_ring_kernel(const FwdParams p) {
   constexpr int E = Traits<T>::kVec;
   constexpr int NW = CONSUMERS / kWarp;
@@ -182,6 +194,7 @@ __global__ void __launch_bounds__(CONSUMERS + 32) logprob_fwd_ring_kernel(const 
   uint64_t *dempty = dfull + kFwdDescs;
   FwdRowDesc *desc = reinterpret_cast<FwdRowDesc *>(dempty + kFwdDescs);
   __shared__ float sh_m[2][NW], sh_s[2][NW], sh_xy[2];
+  __shared__ float sh_t[2][ENT ? NW : 1];
   const int tid = threadIdx.x;
   const int V = p.V;
   if (tid == 0) {
@@ -219,6 +232,9 @@ __global__ void __launch_bounds__(CONSUMERS + 32) logprob_fwd_ring_kernel(const 
       const int64_t y = __ldg(p.labels + label_off + j);
       if (p.use_ignore && y == p.ignore_index) {  // ignored position (cross-entropy ignore_index): no traffic
         store_from_float(p.out, out_off + j, p.out_dtype, 0.f);
+        if constexpr (ENT) {
+          if (out_off + j < p.n_entropy) p.entropy[out_off + j] = 0.f;
+        }
         if (p.stat_max) {
           p.stat_max[row] = 0.f;
           p.stat_logsum[row] = 0.f;
@@ -279,7 +295,7 @@ __global__ void __launch_bounds__(CONSUMERS + 32) logprob_fwd_ring_kernel(const 
     const float tx = tid < V - tail0 ? Traits<T>::to_float(x[tail0 + tid]) : -INFINITY;
     const float xy_peel = (tid == 0 && d.y >= 0 && yb < 0) ? Traits<T>::to_float(x[d.y]) : 0.f;
 
-    float m = -INFINITY, s = 0.f;
+    float m = -INFINITY, s = 0.f, t = 0.f;
     for (int v0 = 0; v0 < nvec; v0 += STAGE_VECS) {
       const int n = min(STAGE_VECS, nvec - v0);
       bulk::mbar_wait(full + stage, phase);
@@ -305,38 +321,30 @@ __global__ void __launch_bounds__(CONSUMERS + 32) logprob_fwd_ring_kernel(const 
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
       if (lane == 0) bulk::mbar_arrive(empty + stage);  // this warp's reads of the stage are done
-      fold_batch<T, UNROLL>(v, m, s, L2);
+      fold_batch_t<T, UNROLL, ENT>(v, m, s, t, L2);
       if (++stage == STAGES) {
         stage = 0;
         phase ^= 1u;
       }
     }
-    lse_push(m, s, hx);
-    lse_push(m, s, tx);
+    lse_push_t<ENT>(m, s, t, hx);
+    lse_push_t<ENT>(m, s, t, tx);
 
     // merge the partials of the CONSUMERS threads.  Named barrier 1 leaves the producer out; the scratch is
     // double-buffered by row parity, so warp 0 reading this row's partials cannot race the next row's writes
     // (those come after the next row's barrier, which warp 0 reaches only when it is done here).
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      float m2 = __shfl_xor_sync(0xffffffffu, m, o);
-      float s2 = __shfl_xor_sync(0xffffffffu, s, o);
-      lse_merge(m, s, m2, s2);
-    }
+    warp_lse_t<ENT>(m, s, t);
     if (lane == 0) {
       sh_m[par][wid] = m;
       sh_s[par][wid] = s;
+      if constexpr (ENT) sh_t[par][wid] = t;
     }
     asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
     if (wid == 0) {
       m = lane < NW ? sh_m[par][lane] : -INFINITY;
       s = lane < NW ? sh_s[par][lane] : 0.f;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        float m2 = __shfl_xor_sync(0xffffffffu, m, o);
-        float s2 = __shfl_xor_sync(0xffffffffu, s, o);
-        lse_merge(m, s, m2, s2);
-      }
+      if constexpr (ENT) t = lane < NW ? sh_t[par][lane] : 0.f;
+      warp_lse_t<ENT>(m, s, t);
       if (tid == 0) {
         const float logsum = logf(s);
         const float xy = yb >= 0 ? sh_xy[par] : xy_peel;
@@ -346,6 +354,9 @@ __global__ void __launch_bounds__(CONSUMERS + 32) logprob_fwd_ring_kernel(const 
           if (p.status) atomicOr(p.status, AA_STATUS_LABEL_OOB);
         }
         store_from_float(p.out, d.out_idx, p.out_dtype, lp);
+        if constexpr (ENT) {
+          if (d.out_idx < p.n_entropy) p.entropy[d.out_idx] = entropy_of(logsum, s, t);
+        }
         if (p.stat_max) {
           p.stat_max[d.row] = m;
           p.stat_logsum[d.row] = logsum;
@@ -723,10 +734,10 @@ static int fwd_grid(K kern, int threads, size_t smem, std::atomic<int> &resident
   return 0;
 }
 
-template <typename T>
+template <typename T, bool ENT>
 static int launch_fwd_ldg(const FwdParams &p, cudaStream_t st) {
   constexpr int THREADS = 512, UNROLL = 4;
-  auto kern = logprob_fwd_kernel<T, THREADS, UNROLL>;
+  auto kern = logprob_fwd_kernel<T, THREADS, UNROLL, ENT>;
   static std::atomic<int> resident{0};
   unsigned grid = 0;
   int rc = fwd_grid(kern, THREADS, 0, resident, p.n_rows, grid);
@@ -735,11 +746,11 @@ static int launch_fwd_ldg(const FwdParams &p, cudaStream_t st) {
   return check_launch("aa_logprob_fwd(ldg)");
 }
 
-template <typename T>
+template <typename T, bool ENT>
 static int launch_fwd_ring(const FwdParams &p, cudaStream_t st) {
   constexpr int CONSUMERS = 256, STAGES = 4, UNROLL = 4;  // 4 stages x 16 KB; 3 CTAs per SM are resident
   constexpr size_t smem = fwd_ring_smem<CONSUMERS, STAGES, UNROLL>();
-  auto kern = logprob_fwd_ring_kernel<T, CONSUMERS, STAGES, UNROLL>;
+  auto kern = logprob_fwd_ring_kernel<T, CONSUMERS, STAGES, UNROLL, ENT>;
   static std::atomic<int> resident{0};
   unsigned grid = 0;
   int rc = fwd_grid(kern, CONSUMERS + 32, smem, resident, p.n_rows, grid);
@@ -754,12 +765,12 @@ static int launch_fwd_ring(const FwdParams &p, cudaStream_t st) {
 // against 0.62 ms).  Tuning variant 1 forces the ring, variant 2 the LDG kernel.
 constexpr int64_t kFwdLdgMinRowBytes = 128 * 1024;
 
-template <typename T>
+template <typename T, bool ENT = false>
 static int launch_fwd(const FwdParams &p, cudaStream_t st) {
   const int variant = fwd_variant();
   if (variant == 2 || (variant != 1 && static_cast<int64_t>(p.V) * sizeof(T) >= kFwdLdgMinRowBytes))
-    return launch_fwd_ldg<T>(p, st);
-  return launch_fwd_ring<T>(p, st);
+    return launch_fwd_ldg<T, ENT>(p, st);
+  return launch_fwd_ring<T, ENT>(p, st);
 }
 
 template <typename T, int THREADS, int UNROLL, bool FAITHFUL>
@@ -838,6 +849,43 @@ extern "C" int aa_logprob_set_tuning_bwd(int variant, int ctas_per_sm) {
   return AA_OK;
 }
 
+static int logprob_fwd(const char *who, const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                       const int64_t *labels, int64_t ignore_index, int32_t use_ignore, int32_t n_segments,
+                       int64_t n_rows, const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                       const int64_t *seg_out_off, const int64_t *seg_cum, void *out, int out_dtype, float *stat_max,
+                       float *stat_logsum, int32_t *status, float *entropy, int64_t n_entropy, void *stream) {
+  AA_REQUIRE(V > 0 && n_segments >= 0 && n_rows >= 0, AA_ERR_ARG, "%s: bad sizes", who);
+  if (n_rows == 0 || n_segments == 0) return AA_OK;
+  AA_REQUIRE(logits && labels && out && seg_logit_off && seg_label_off && seg_out_off && seg_cum,
+             AA_ERR_ARG, "%s: null pointer", who);
+  AA_REQUIRE((stat_max == nullptr) == (stat_logsum == nullptr), AA_ERR_ARG,
+             "%s: stat_max and stat_logsum go together", who);
+  AA_REQUIRE(out_dtype == AA_BF16 || out_dtype == AA_F16 || out_dtype == AA_F32, AA_ERR_DTYPE,
+             "%s: bad out_dtype %d", who, out_dtype);
+  const int esz = dtype_size(logits_dtype);
+  AA_REQUIRE(reinterpret_cast<uintptr_t>(logits) % esz == 0, AA_ERR_ALIGN,
+             "%s: logits not element-aligned", who);
+  FwdParams p{logits, row_stride, V, labels, ignore_index, use_ignore,
+              RowMap{seg_logit_off, seg_label_off, seg_out_off, seg_cum, n_segments},
+              n_rows, out, out_dtype, stat_max, stat_logsum, status, kLog2e, entropy, n_entropy};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (entropy) {
+    switch (logits_dtype) {
+      case AA_BF16: return launch_fwd<__nv_bfloat16, true>(p, st);
+      case AA_F16: return launch_fwd<__half, true>(p, st);
+      case AA_F32: return launch_fwd<float, true>(p, st);
+    }
+  } else {
+    switch (logits_dtype) {
+      case AA_BF16: return launch_fwd<__nv_bfloat16>(p, st);
+      case AA_F16: return launch_fwd<__half>(p, st);
+      case AA_F32: return launch_fwd<float>(p, st);
+    }
+  }
+  set_error("%s: unsupported logits dtype %d", who, logits_dtype);
+  return AA_ERR_DTYPE;
+}
+
 extern "C" int aa_logprob_fwd(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
                               const int64_t *labels, int64_t ignore_index, int32_t use_ignore,
                               int32_t n_segments, int64_t n_rows,
@@ -845,28 +893,22 @@ extern "C" int aa_logprob_fwd(const void *logits, int logits_dtype, int64_t row_
                               const int64_t *seg_out_off, const int64_t *seg_cum, void *out,
                               int out_dtype, float *stat_max, float *stat_logsum, int32_t *status,
                               void *stream) {
-  AA_REQUIRE(V > 0 && n_segments >= 0 && n_rows >= 0, AA_ERR_ARG, "aa_logprob_fwd: bad sizes");
-  if (n_rows == 0 || n_segments == 0) return AA_OK;
-  AA_REQUIRE(logits && labels && out && seg_logit_off && seg_label_off && seg_out_off && seg_cum,
-             AA_ERR_ARG, "aa_logprob_fwd: null pointer");
-  AA_REQUIRE((stat_max == nullptr) == (stat_logsum == nullptr), AA_ERR_ARG,
-             "aa_logprob_fwd: stat_max and stat_logsum go together");
-  AA_REQUIRE(out_dtype == AA_BF16 || out_dtype == AA_F16 || out_dtype == AA_F32, AA_ERR_DTYPE,
-             "aa_logprob_fwd: bad out_dtype %d", out_dtype);
-  const int esz = dtype_size(logits_dtype);
-  AA_REQUIRE(reinterpret_cast<uintptr_t>(logits) % esz == 0, AA_ERR_ALIGN,
-             "aa_logprob_fwd: logits not element-aligned");
-  FwdParams p{logits, row_stride, V, labels, ignore_index, use_ignore,
-              RowMap{seg_logit_off, seg_label_off, seg_out_off, seg_cum, n_segments},
-              n_rows, out, out_dtype, stat_max, stat_logsum, status, kLog2e};
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  switch (logits_dtype) {
-    case AA_BF16: return launch_fwd<__nv_bfloat16>(p, st);
-    case AA_F16: return launch_fwd<__half>(p, st);
-    case AA_F32: return launch_fwd<float>(p, st);
-  }
-  set_error("aa_logprob_fwd: unsupported logits dtype %d", logits_dtype);
-  return AA_ERR_DTYPE;
+  return logprob_fwd("aa_logprob_fwd", logits, logits_dtype, row_stride, V, labels, ignore_index, use_ignore,
+                     n_segments, n_rows, seg_logit_off, seg_label_off, seg_out_off, seg_cum, out, out_dtype, stat_max,
+                     stat_logsum, status, nullptr, 0, stream);
+}
+
+extern "C" int aa_logprob_fwd_entropy(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                      const int64_t *labels, int64_t ignore_index, int32_t use_ignore,
+                                      int32_t n_segments, int64_t n_rows,
+                                      const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                                      const int64_t *seg_out_off, const int64_t *seg_cum, void *out,
+                                      int out_dtype, float *stat_max, float *stat_logsum, int32_t *status,
+                                      float *entropy, int64_t n_entropy, void *stream) {
+  AA_REQUIRE(entropy && n_entropy >= 0, AA_ERR_ARG, "aa_logprob_fwd_entropy: null entropy");
+  return logprob_fwd("aa_logprob_fwd_entropy", logits, logits_dtype, row_stride, V, labels, ignore_index, use_ignore,
+                     n_segments, n_rows, seg_logit_off, seg_label_off, seg_out_off, seg_cum, out, out_dtype, stat_max,
+                     stat_logsum, status, entropy, n_entropy, stream);
 }
 
 extern "C" int aa_zero_rows(void *tile, int dtype, int64_t row_stride, int32_t V, int64_t n_tile_rows,

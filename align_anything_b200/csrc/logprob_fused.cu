@@ -67,6 +67,7 @@ struct FusedActorParams {
   const float *ce_coeff;
   const int32_t *row_end;
   const float *total;
+  float *entropy;  // ENT kernels: fp32 entropy of every scored row at its log-prob's position (phase A)
 };
 
 // One record per gradient-tile row, in the order the persistent kernel walks them.  The scored rows are bound by
@@ -191,7 +192,7 @@ __device__ __forceinline__ uint4 vec_grad_pk(const uint4 &v, const GradConsts &k
   }
 }
 
-template <typename T, int CONSUMERS, int STAGES, int UNROLL, int LAG, bool FAITHFUL>
+template <typename T, int CONSUMERS, int STAGES, int UNROLL, int LAG, bool FAITHFUL, bool ENT = false>
 __global__ void __launch_bounds__(CONSUMERS + 32)
     logprob_actor_fused_kernel(const FusedActorParams p, const FusedRec *__restrict__ rec, int64_t n_work) {
   constexpr int E = Traits<T>::kVec;
@@ -206,6 +207,7 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
   uint64_t *st_dst = done + STAGES;  // destination of the chunk held by each stage (phase B), 0 for phase A
   uint32_t *st_bytes = reinterpret_cast<uint32_t *>(st_dst + STAGES);
   __shared__ float sh_m[32], sh_s[32], sh_b[4];
+  __shared__ float sh_t[ENT ? 32 : 1];
   const int tid = threadIdx.x;
   const int V = p.V;
   const T *__restrict__ logits = reinterpret_cast<const T *>(p.logits);
@@ -337,10 +339,10 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
     if (tid == 0) xy = (y >= 0) ? Traits<T>::to_float(x[y]) : NAN;  // label column, issued before the streaming loop
 
     // ---- phase A: (max, sum exp) of the row ----
-    float m = -INFINITY, s = 0.f;
+    float m = -INFINITY, s = 0.f, t = 0.f;
     if (same_phase) {
-      if (tid < head) lse_push(m, s, Traits<T>::to_float(x[tid]));
-      if (tid < V - tail0) lse_push(m, s, Traits<T>::to_float(x[tail0 + tid]));
+      if (tid < head) lse_push_t<ENT>(m, s, t, Traits<T>::to_float(x[tid]));
+      if (tid < V - tail0) lse_push_t<ENT>(m, s, t, Traits<T>::to_float(x[tail0 + tid]));
       // two stages per fold: the running-max rescale (one MUFU, a compare and a select) is paid per 4 vectors
       for (int v0 = 0; v0 < nvec; v0 += 2 * STAGE_VECS) {
         const int n0 = min(STAGE_VECS, nvec - v0);
@@ -380,7 +382,7 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
           bulk::mbar_arrive(done + st0);
           if (n1 > 0) bulk::mbar_arrive(done + st1);
         }
-        fold_batch<T, 2 * UNROLL>(v, m, s, L2);
+        fold_batch_t<T, 2 * UNROLL, ENT>(v, m, s, t, L2);
         stage = st1;
         phase = ph1;
         if (n1 > 0 && ++stage == STAGES) {
@@ -389,29 +391,21 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
         }
       }
     } else {  // logits view and gradient tile disagree on the 16-byte phase of this row: element loops, no staging
-      for (int e = tid; e < V; e += CONSUMERS) lse_push(m, s, Traits<T>::to_float(x[e]));
+      for (int e = tid; e < V; e += CONSUMERS) lse_push_t<ENT>(m, s, t, Traits<T>::to_float(x[e]));
     }
     // merge the partials of the CONSUMERS threads (named barrier 1: the producer warp is not part of it)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float m2 = __shfl_xor_sync(0xffffffffu, m, o);
-      const float s2 = __shfl_xor_sync(0xffffffffu, s, o);
-      lse_merge(m, s, m2, s2);
-    }
+    warp_lse_t<ENT>(m, s, t);
     if (lane == 0) {
       sh_m[wid] = m;
       sh_s[wid] = s;
+      if constexpr (ENT) sh_t[wid] = t;
     }
     asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
     if (wid == 0) {
       m = lane < NW ? sh_m[lane] : -INFINITY;
       s = lane < NW ? sh_s[lane] : 0.f;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float m2 = __shfl_xor_sync(0xffffffffu, m, o);
-        const float s2 = __shfl_xor_sync(0xffffffffu, s, o);
-        lse_merge(m, s, m2, s2);
-      }
+      if constexpr (ENT) t = lane < NW ? sh_t[lane] : 0.f;
+      warp_lse_t<ENT>(m, s, t);
       if (lane == 0) {
         // ---- boundary: log-prob -> d loss / d log-prob of this token ----
         const float logsum = logf(s);
@@ -421,6 +415,7 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
           if (p.status) atomicOr(p.status, AA_STATUS_LABEL_OOB);
         }
         store_from_float(p.out, out_idx, p.out_dtype, lp);
+        if constexpr (ENT) p.entropy[out_idx] = entropy_of(logsum, s, t);
         if (p.stat_max) {
           p.stat_max[flat] = m;
           p.stat_logsum[flat] = logsum;
@@ -544,13 +539,13 @@ __global__ void __launch_bounds__(256) scale_tile_kernel(T *__restrict__ tile, i
 // two passes, inside the 50 MB L2, so the second pass is an L2 hit; with two rows in flight per SM part of it misses.
 // The kernel is bound by the MUFU / conversion pipe and instruction issue (two exp per logit + the bf16 pack) rather
 // than by HBM.
-template <typename T>
+template <typename T, bool ENT = false>
 static int launch_fused_kernel(const FusedActorParams &p, int mode, FusedRec *rec, int64_t n_work, cudaStream_t st) {
   constexpr int CONSUMERS = 992, STAGES = 6, UNROLL = 2, LAG = 4;
   constexpr size_t smem = static_cast<size_t>(STAGES + 1) * CONSUMERS * UNROLL * 16 + STAGES * (8 + 8 + 8 + 4) + 16;
   const bool faithful = (mode == AA_MODE_FAITHFUL) && sizeof(T) == 2;
-  auto kf = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, true>;
-  auto kn = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, false>;
+  auto kf = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, true, ENT>;
+  auto kn = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, false, ENT>;
   static std::atomic<bool> configured{false};  // the attribute is idempotent: a race sets it twice, harmlessly
   if (!configured.load(std::memory_order_relaxed)) {
     cudaError_t e = cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -578,6 +573,14 @@ static int launch_fused_kernel(const FusedActorParams &p, int mode, FusedRec *re
 
 static int launch_fused(const FusedActorParams &p, int logits_dtype, int mode, FusedRec *rec, int64_t n_work,
                         cudaStream_t st) {
+  if (p.entropy) {
+    switch (logits_dtype) {
+      case AA_BF16: return launch_fused_kernel<__nv_bfloat16, true>(p, mode, rec, n_work, st);
+      case AA_F16: return launch_fused_kernel<__half, true>(p, mode, rec, n_work, st);
+      case AA_F32: return launch_fused_kernel<float, true>(p, mode, rec, n_work, st);
+    }
+    return AA_ERR_DTYPE;
+  }
   switch (logits_dtype) {
     case AA_BF16: return launch_fused_kernel<__nv_bfloat16>(p, mode, rec, n_work, st);
     case AA_F16: return launch_fused_kernel<__half>(p, mode, rec, n_work, st);
@@ -689,7 +692,9 @@ extern "C" int aa_logprob_ce_fused(const void *logits, int logits_dtype, int64_t
   return launch_fused(p, logits_dtype, AA_MODE_F32, static_cast<FusedRec *>(row_scratch), n_tile_rows, st);
 }
 
-extern "C" int aa_logprob_grpo_fused(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+// aa_logprob_grpo_fused{,_entropy}: entropy == nullptr runs the plain kernels
+static int logprob_grpo_fused(float *entropy, const char *who, const void *logits, int logits_dtype, int64_t row_stride,
+                                    int32_t V,
                                     const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
                                     const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
                                     const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
@@ -698,15 +703,15 @@ extern "C" int aa_logprob_grpo_fused(const void *logits, int logits_dtype, int64
                                     float beta, int mode, void *grad_logits, int64_t grad_row_stride, void *row_scratch,
                                     int32_t *row_end, float *total, uint32_t *counter, int32_t *status, void *stream) {
   AA_REQUIRE(V > 0 && n_segments > 0 && K > 0 && n_tile_rows > 0 && n_tile_rows % n_segments == 0, AA_ERR_ARG,
-             "aa_logprob_grpo_fused: bad sizes (the gradient tile holds n_tile_rows / n_segments rows per sample)");
+             "%s: bad sizes (the gradient tile holds n_tile_rows / n_segments rows per sample)", who);
   AA_REQUIRE(logits && labels && seg_logit_off && seg_label_off && seg_out_off && seg_cum && seg_tile_row && log_probs &&
                  ref_log_probs && advantages && completion_tokens && grad_logits && row_scratch && row_end && total && counter,
-             AA_ERR_ARG, "aa_logprob_grpo_fused: null pointer");
-  AA_REQUIRE(fdtype_ok(logits_dtype) && fdtype_ok(lp_dtype), AA_ERR_DTYPE, "aa_logprob_grpo_fused: bad dtype");
-  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_logprob_grpo_fused: bad mode");
+             AA_ERR_ARG, "%s: null pointer", who);
+  AA_REQUIRE(fdtype_ok(logits_dtype) && fdtype_ok(lp_dtype), AA_ERR_DTYPE, "%s: bad dtype", who);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "%s: bad mode", who);
   AA_REQUIRE((reinterpret_cast<uintptr_t>(row_scratch) & 15) == 0, AA_ERR_ALIGN,
-             "aa_logprob_grpo_fused: row_scratch must be 16-byte aligned");
-  AA_REQUIRE(n_tile_rows < (1ll << 31), AA_ERR_ARG, "aa_logprob_grpo_fused: tile too large");
+             "%s: row_scratch must be 16-byte aligned", who);
+  AA_REQUIRE(n_tile_rows < (1ll << 31), AA_ERR_ARG, "%s: tile too large", who);
   const bool f = (mode == AA_MODE_FAITHFUL);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   grpo_mask_kernel<128><<<n_segments, 128, 0, st>>>(completion_tokens, tok_stride, n_segments, K, eos_id, row_end, total, counter);
@@ -724,7 +729,39 @@ extern "C" int aa_logprob_grpo_fused(const void *logits, int logits_dtype, int64
   p.rp = f ? lp_dtype : AA_F32;
   p.row_end = row_end;
   p.total = total;
+  p.entropy = entropy;
   return launch_fused(p, logits_dtype, mode, static_cast<FusedRec *>(row_scratch), n_tile_rows, st);
+}
+
+extern "C" int aa_logprob_grpo_fused(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                    const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                    const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
+                                    const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
+                                    const void *ref_log_probs, int64_t ref_stride, const float *advantages,
+                                    const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t K,
+                                    float beta, int mode, void *grad_logits, int64_t grad_row_stride, void *row_scratch,
+                                    int32_t *row_end, float *total, uint32_t *counter, int32_t *status, void *stream) {
+  return logprob_grpo_fused(nullptr, "aa_logprob_grpo_fused", logits, logits_dtype, row_stride, V, labels, n_segments,
+                            seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row, n_tile_rows, log_probs,
+                            lp_dtype, ref_log_probs, ref_stride, advantages, completion_tokens, tok_stride, eos_id, K, beta,
+                            mode, grad_logits, grad_row_stride, row_scratch, row_end, total, counter, status, stream);
+}
+
+extern "C" int aa_logprob_grpo_fused_entropy(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                            const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                            const int64_t *seg_label_off, const int64_t *seg_out_off,
+                                            const int64_t *seg_cum, const int64_t *seg_tile_row, int64_t n_tile_rows,
+                                            void *log_probs, int lp_dtype, const void *ref_log_probs, int64_t ref_stride,
+                                            const float *advantages, const int64_t *completion_tokens, int64_t tok_stride,
+                                            int64_t eos_id, int32_t K, float beta, int mode, void *grad_logits,
+                                            int64_t grad_row_stride, void *row_scratch, int32_t *row_end, float *total,
+                                            uint32_t *counter, int32_t *status, float *entropy, void *stream) {
+  AA_REQUIRE(entropy, AA_ERR_ARG, "aa_logprob_grpo_fused_entropy: null entropy");
+  return logprob_grpo_fused(entropy, "aa_logprob_grpo_fused_entropy", logits, logits_dtype, row_stride, V, labels,
+                            n_segments, seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row, n_tile_rows,
+                            log_probs, lp_dtype, ref_log_probs, ref_stride, advantages, completion_tokens, tok_stride,
+                            eos_id, K, beta, mode, grad_logits, grad_row_stride, row_scratch, row_end, total, counter,
+                            status, stream);
 }
 
 extern "C" int aa_scale_tile(void *tile, int dtype, int64_t n, const void *scale, int scale_dtype, void *stream) {

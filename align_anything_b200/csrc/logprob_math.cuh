@@ -87,6 +87,109 @@ __device__ __forceinline__ void fold_batch(const uint4 (&v)[N], float &m, float 
   m = mn;
 }
 
+// ---- entropy: a third running sum next to (m, s) ----------------------------------------------------
+// t = sum_j e^{x_j - m} (x_j - m) over the elements folded so far; the row's entropy is H = log s - t / s.  When the
+// running maximum moves from m to m' (alpha = e^{m - m'}) the partial becomes t' = alpha (t + (m - m') s), the rule the
+// fold, the thread merges and K6's split merge share.  A -inf logit adds 0 (the limit of p log p), an all -inf row has
+// s = 0 and gets NaN.  The ENT = false forms below are the plain (m, s) code: t is dead and compiled away.
+__device__ __forceinline__ float ent_rescale(float t, float s, float m_old, float m_new) {
+  if (m_old == m_new) return t;
+  if (m_old == -INFINITY) return 0.f;  // s == t == 0
+  return lse_rescale(m_old, m_new) * fmaf(m_old - m_new, s, t);
+}
+
+template <bool ENT>
+__device__ __forceinline__ void lse_merge_t(float &m, float &s, float &t, float m2, float s2, float t2) {
+  if constexpr (ENT) {
+    const float mn = fmaxf(m, m2);
+    t = ent_rescale(t, s, m, mn) + ent_rescale(t2, s2, m2, mn);
+    s = s * lse_rescale(m, mn) + s2 * lse_rescale(m2, mn);  // lse_merge's expression
+    m = mn;
+  } else {
+    lse_merge(m, s, m2, s2);
+  }
+}
+
+template <bool ENT>
+__device__ __forceinline__ void lse_push_t(float &m, float &s, float &t, float x) {
+  if constexpr (ENT) {
+    if (x == -INFINITY) return;
+    lse_merge_t<true>(m, s, t, x, 1.f, 0.f);
+  } else {
+    lse_push(m, s, x);
+  }
+}
+
+// log s - t / s (fp32, never rounded)
+__device__ __forceinline__ float entropy_of(float logsum, float s, float t) { return logsum - t / s; }
+
+// vec_expsum plus tacc += e * (x - mref); the (x - mref) of a -inf logit is clamped so that its term is 0 * finite
+template <typename T>
+__device__ __forceinline__ void vec_expsum_ent(const uint4 &v, f32x2 mref2, f32x2 L2, f32x2 &acc0, f32x2 &acc1,
+                                               f32x2 &tac0, f32x2 &tac1) {
+  const f32x2 lim = f2_splat(-3.0e38f);
+  auto term = [&](float lo, float hi, f32x2 &acc, f32x2 &tac) {
+    const f32x2 d = f2_sub(f2_pack(lo, hi), mref2);
+    const f32x2 e = f2_ex2(f2_mul(d, L2));
+    acc = f2_add(acc, e);
+    tac = f2_fma(e, make_float2(fmaxf(d.x, lim.x), fmaxf(d.y, lim.y)), tac);
+  };
+  if constexpr (sizeof(T) == 4) {
+    term(__uint_as_float(v.x), __uint_as_float(v.y), acc0, tac0);
+    term(__uint_as_float(v.z), __uint_as_float(v.w), acc1, tac1);
+  } else {
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      float lo, hi;
+      unpack2<T>(w[i], lo, hi);
+      if (i & 1)
+        term(lo, hi, acc1, tac1);
+      else
+        term(lo, hi, acc0, tac0);
+    }
+  }
+}
+
+// fold_batch, with the entropy sum when ENT
+template <typename T, int N, bool ENT>
+__device__ __forceinline__ void fold_batch_t(const uint4 (&v)[N], float &m, float &s, float &t, f32x2 L2) {
+  if constexpr (ENT) {
+    float bm = vec_max<T>(v[0]);
+#pragma unroll
+    for (int u = 1; u < N; ++u) bm = fmaxf(bm, vec_max<T>(v[u]));
+    const float mn = fmaxf(m, bm);
+    const float mref = (mn == -INFINITY) ? 0.f : mn;
+    const f32x2 mref2 = f2_splat(mref);
+    f32x2 acc0 = f2_pack(s * lse_rescale(m, mn), 0.f), acc1 = f2_pack(0.f, 0.f);
+    f32x2 tac0 = f2_pack(ent_rescale(t, s, m, mn), 0.f), tac1 = f2_pack(0.f, 0.f);
+#pragma unroll
+    for (int u = 0; u < N; ++u) vec_expsum_ent<T>(v[u], mref2, L2, acc0, acc1, tac0, tac1);
+    float a0, a1, a2, a3;
+    f2_unpack(acc0, a0, a1);
+    f2_unpack(acc1, a2, a3);
+    s = (a0 + a1) + (a2 + a3);
+    f2_unpack(tac0, a0, a1);
+    f2_unpack(tac1, a2, a3);
+    t = (a0 + a1) + (a2 + a3);
+    m = mn;
+  } else {
+    fold_batch<T, N>(v, m, s, L2);
+  }
+}
+
+// warp-level merge of (m, s[, t]) over all 32 lanes
+template <bool ENT>
+__device__ __forceinline__ void warp_lse_t(float &m, float &s, float &t) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, m, o);
+    const float s2 = __shfl_xor_sync(0xffffffffu, s, o);
+    const float t2 = ENT ? __shfl_xor_sync(0xffffffffu, t, o) : 0.f;
+    lse_merge_t<ENT>(m, s, t, m2, s2, t2);
+  }
+}
+
 template <int THREADS>
 __device__ __forceinline__ void block_lse(float &m, float &s, float *sh_m, float *sh_s) {
   constexpr int NW = THREADS / kWarp;
@@ -111,6 +214,30 @@ __device__ __forceinline__ void block_lse(float &m, float &s, float *sh_m, float
       float s2 = __shfl_xor_sync(0xffffffffu, s, o);
       lse_merge(m, s, m2, s2);
     }
+  }
+}
+
+// block_lse, with the entropy sum when ENT (sh_t: 32 floats, unused otherwise)
+template <int THREADS, bool ENT>
+__device__ __forceinline__ void block_lse_t(float &m, float &s, float &t, float *sh_m, float *sh_s, float *sh_t) {
+  if constexpr (ENT) {
+    constexpr int NW = THREADS / kWarp;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    warp_lse_t<true>(m, s, t);
+    if (lane == 0) {
+      sh_m[wid] = m;
+      sh_s[wid] = s;
+      sh_t[wid] = t;
+    }
+    __syncthreads();
+    if (wid == 0) {
+      m = lane < NW ? sh_m[lane] : -INFINITY;
+      s = lane < NW ? sh_s[lane] : 0.f;
+      t = lane < NW ? sh_t[lane] : 0.f;
+      warp_lse_t<true>(m, s, t);
+    }
+  } else {
+    block_lse<THREADS>(m, s, sh_m, sh_s);
   }
 }
 

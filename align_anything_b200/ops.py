@@ -23,7 +23,8 @@ __all__ = [
     'dpo_fused_loss', 'score_head', 'score_end', 'kl_rewards_and_gae', 'gae_from_rewards', 'estimator_returns', 'actor_loss', 'critic_loss',
     'move_padding_left', 'count_nonpad', 'strip_pad_tail', 'ppo_pack_metrics', 'check_status', 'raise_for_status', 'status_lane', 'causal_lm_loss', 'rm_pair_loss', 'cost_pair_loss','group_advantages', 'grpo_loss', 'tail_token_log_probs', 'pair_slices', 'slice_sums', 'tail_rows', 'linear_token_log_probs',
     'sequence_log_probs_from_hidden', 'fused_linear_token_log_probs', 'tail_log_probs_from_hidden', 'dense_log_probs_from_hidden', 'tail_actor_loss', 'tail_critic_loss', 'lm_head_weight',
-    'causal_lm_loss_from_hidden', 'causal_lm_valid_rows',
+    'causal_lm_loss_from_hidden', 'causal_lm_valid_rows', 'gather_log_probabilities_with_entropy',
+    'response_tail_log_probs_pair_with_entropy',
 ]
 
 # Path knobs: plain module attributes, read at call time and never from the environment.  Every path is chosen from the
@@ -313,15 +314,20 @@ def _tail_plan(lens: tuple, L_seq: int, sb: int, sl: int, lab_stride: int, lab_s
 
 
 # ---- K1 / K1b autograd ---------------------------------------------------------------------------
-def _launch_fwd(logits, labels, plan: RowPlan, out, stat_max, stat_logsum, ignore_index=None):
+def _launch_fwd(logits, labels, plan: RowPlan, out, stat_max, stat_logsum, ignore_index=None, entropy=None):
+    """K1; with `entropy` (fp32, indexed like `out`, zero-initialised) the entropy variant, which writes the entropy of
+    every scored row whose out position lies inside `entropy` and leaves every other output bit-identical."""
     dev = logits.device
     sc = _device_scratch(dev)
     p = plan.ptrs()
-    L.check(L.lib().aa_logprob_fwd(
-        logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), labels.data_ptr(),
-        0 if ignore_index is None else int(ignore_index), 0 if ignore_index is None else 1,
-        plan.n_seg, plan.n_rows, p[0], p[1], p[2], p[3], out.data_ptr(), L.dtype_code(out.dtype),
-        L.ptr(stat_max), L.ptr(stat_logsum), sc['status'].data_ptr(), L.stream_ptr(dev)))
+    args = (logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), labels.data_ptr(),
+            0 if ignore_index is None else int(ignore_index), 0 if ignore_index is None else 1,
+            plan.n_seg, plan.n_rows, p[0], p[1], p[2], p[3], out.data_ptr(), L.dtype_code(out.dtype),
+            L.ptr(stat_max), L.ptr(stat_logsum), sc['status'].data_ptr())
+    if entropy is None:
+        L.check(L.lib().aa_logprob_fwd(*args, L.stream_ptr(dev)))
+    else:
+        L.check(L.lib().aa_logprob_fwd_entropy(*args, entropy.data_ptr(), entropy.numel(), L.stream_ptr(dev)))
 
 
 def _launch_bwd(logits, labels, plan: RowPlan, stat_max, stat_logsum, grad_rows, grad_seg, grad_scale,
@@ -362,10 +368,11 @@ def _rows_from(logits: torch.Tensor, first_row: int) -> torch.Tensor:
 class _LogProbFn(torch.autograd.Function):
     """K1 forward / K1b backward.  `logits` is the tensor the gradient tile is shaped after; the plan
     addresses rows inside it, starting at row `first_row` of `logits` viewed as (rows, V) (nonzero only for
-    the contiguous base of a rerouted view, see _try_reroute)."""
+    the contiguous base of a rerouted view, see _try_reroute).  `entropy` (optional, fp32, plan.out_shape, zeros): the
+    forward also writes each scored row's entropy there (a metric: no gradient flows through it)."""
 
     @staticmethod
-    def forward(ctx, logits, labels, plan: RowPlan, mode_code: int, first_row: int = 0):
+    def forward(ctx, logits, labels, plan: RowPlan, mode_code: int, first_row: int = 0, entropy=None):
         out_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         n_out = 1
         for d in plan.out_shape:
@@ -377,7 +384,7 @@ class _LogProbFn(torch.autograd.Function):
         if need_grad:
             stats = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=logits.device)
             stat_max, stat_logsum = stats[0], stats[1]
-        _launch_fwd(_rows_from(logits, first_row), labels, plan, out, stat_max, stat_logsum)
+        _launch_fwd(_rows_from(logits, first_row), labels, plan, out, stat_max, stat_logsum, entropy=entropy)
         if need_grad:
             ctx.save_for_backward(logits, labels, stats)
             ctx.plan, ctx.mode_code, ctx.first_row = plan, mode_code, first_row
@@ -392,7 +399,14 @@ class _LogProbFn(torch.autograd.Function):
         grad = torch.empty(logits.shape, dtype=logits.dtype, device=logits.device)
         _launch_bwd(_rows_from(logits, ctx.first_row), labels, ctx.plan, stats[0], stats[1], grad_out, None, None, grad,
                     ctx.mode_code)
-        return grad, None, None, None, None
+        return grad, None, None, None, None, None
+
+
+def _log_probs_and_entropy(logits, labels, plan, mode_code: int, first_row: int = 0):
+    """_LogProbFn with the entropy variant of K1: -> (log-probs, fp32 entropy of the same shape, 0 where unscored)."""
+    entropy = torch.zeros(plan.out_shape, dtype=torch.float32, device=logits.device)
+    out = _LogProbFn.apply(logits, labels, plan, mode_code, first_row, entropy)
+    return out, entropy
 
 
 def _contiguous_last(t: torch.Tensor) -> torch.Tensor:
@@ -421,6 +435,18 @@ def gather_log_probabilities(logits: torch.Tensor, labels: torch.Tensor, mode: s
     """Drop-in for utils/tools.py:402-413: log_softmax(logits, -1) gathered at `labels`, without ever
     writing the (B, L, V) log-prob tile.  logits (B, L, V) or (L, V), any batch/row strides (the
     callers pass `[:, :-1]` views); differentiable in `logits` (K1b)."""
+    return _gather(logits, labels, mode, False)
+
+
+def gather_log_probabilities_with_entropy(logits: torch.Tensor, labels: torch.Tensor, mode: str | None = None):
+    """gather_log_probabilities plus the policy entropy of every row, -(softmax(x) * log_softmax(x)).sum(-1) of the fp32
+    upcast logits, from the same K1 pass (one more FMA per logit; no extra read of the tile).  -> (log_probs, entropy):
+    log_probs bit-identical to gather_log_probabilities (and as differentiable), entropy fp32 in both modes, never
+    requiring grad.  A -inf logit contributes 0 (the limit of p log p); a row of -inf only gets NaN."""
+    return _gather(logits, labels, mode, True)
+
+
+def _gather(logits, labels, mode, with_entropy: bool):
     L.require_cuda(logits, labels)
     squeeze = logits.dim() == 2
     if squeeze:
@@ -437,7 +463,10 @@ def gather_log_probabilities(logits: torch.Tensor, labels: torch.Tensor, mode: s
     if B == 0 or rows == 0:
         out_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         out = logits.new_zeros((B, rows), dtype=out_dtype)
-        return out.squeeze(0) if squeeze else out
+        ent = logits.new_zeros((B, rows), dtype=torch.float32)
+        if squeeze:
+            out, ent = out.squeeze(0), ent.squeeze(0)
+        return (out, ent) if with_entropy else out
     routed = _try_reroute(logits) if (logits.requires_grad and torch.is_grad_enabled()) else None
     lab_sb = labels.stride(0) if B > 1 else rows
     if routed is not None:
@@ -447,12 +476,16 @@ def gather_log_probabilities(logits: torch.Tensor, labels: torch.Tensor, mode: s
         # logits offsets in the plan are relative to the view's first row (row0 of the base); tile rows are
         # rows of the base, whose shape the gradient takes
         plan = _dense_plan(B, rows, sb_rows * V, V, lab_sb, row0, sb_rows, n_tile, dev)
-        out = _LogProbFn.apply(base, labels, plan, mode_code, row0)
+        tile, first_row = base, row0
     else:
         sb = logits.stride(0) if B > 1 else rows * logits.stride(1)
         plan = _dense_plan(B, rows, sb, logits.stride(1), lab_sb, 0, rows, B * rows, dev)
-        out = _LogProbFn.apply(logits, labels, plan, mode_code)
-    return out.squeeze(0) if squeeze else out
+        tile, first_row = logits, 0
+    if not with_entropy:
+        out = _LogProbFn.apply(tile, labels, plan, mode_code, first_row)
+        return out.squeeze(0) if squeeze else out
+    out, ent = _log_probs_and_entropy(tile, labels, plan, mode_code, first_row)
+    return (out.squeeze(0), ent.squeeze(0)) if squeeze else (out, ent)
 
 
 # ---- lm_head x log-prob without the (rows, V) tile (SURVEY.md 8f rank 1, first step) ------------------------
@@ -489,7 +522,7 @@ class _LinearLogProbFn(torch.autograd.Function):
     buffers, the padded weight and an fp32 d(weight) accumulator instead of two (rows, V) tiles."""
 
     @staticmethod
-    def forward(ctx, hidden, weight, labels, chunk: int, mode_code: int):
+    def forward(ctx, hidden, weight, labels, chunk: int, mode_code: int, entropy=None):
         N, V = hidden.size(0), weight.size(0)
         dev = hidden.device
         out_dtype = hidden.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
@@ -503,7 +536,8 @@ class _LinearLogProbFn(torch.autograd.Function):
             torch.matmul(hidden[r0:r0 + n], w_pad.t(), out=buf[:n])  # the dtype rounding point of nn.Linear
             plan = _dense_plan(1, n, n * Vp, Vp, n, 0, n, 0, str(dev))
             _launch_fwd(buf[:n, :V], labels[r0:r0 + n], plan, out[r0:r0 + n],
-                        stats[0, r0:r0 + n] if need_grad else None, stats[1, r0:r0 + n] if need_grad else None)
+                        stats[0, r0:r0 + n] if need_grad else None, stats[1, r0:r0 + n] if need_grad else None,
+                        entropy=None if entropy is None else entropy[r0:r0 + n])
         if need_grad:
             ctx.save_for_backward(hidden, weight, labels, stats)
             ctx.chunk, ctx.mode_code = chunk, mode_code
@@ -533,7 +567,7 @@ class _LinearLogProbFn(torch.autograd.Function):
                 torch.matmul(dbuf[:n], w_pad, out=d_hidden[r0:r0 + n])
             if need_w:  # fp32 accumulation across chunks, one rounding at the end (like a single GEMM)
                 d_weight.add_(_mm_f32(dbuf[:n].t(), hidden[r0:r0 + n]))
-        return d_hidden, (d_weight[:V].to(weight.dtype) if need_w else None), None, None, None
+        return d_hidden, (d_weight[:V].to(weight.dtype) if need_w else None), None, None, None, None
 
 
 class _LinearLogProbK6Fn(torch.autograd.Function):
@@ -544,9 +578,8 @@ class _LinearLogProbK6Fn(torch.autograd.Function):
     library GEMM, no padded / transposed copy of the weight."""
 
     @staticmethod
-    def forward(ctx, hidden, weight, labels, chunk: int, mode_code: int):
-        out, stats = fused_linear_token_log_probs(hidden, weight, labels, 'faithful' if mode_code == L.MODE_FAITHFUL else 'f32',
-                                                  return_stats=True)
+    def forward(ctx, hidden, weight, labels, chunk: int, mode_code: int, entropy=None):
+        out, stats = _k6_forward(hidden, weight, labels, mode_code, True, entropy)
         ctx.save_for_backward(hidden, weight, labels, stats)
         ctx.chunk, ctx.mode_code = chunk, mode_code
         return out
@@ -585,7 +618,7 @@ class _LinearLogProbK6Fn(torch.autograd.Function):
                 last = i == n_chunks - 1
                 L.check(lib.aa_linear_dweight(dbuf.data_ptr(), n, ld, h.data_ptr(), H, h.stride(0), V, L.ptr(acc), H,
                                               1 if i > 0 else 0, d_weight.data_ptr() if last else None, d_weight.stride(0), st))
-        return d_hidden, d_weight, None, None, None
+        return d_hidden, d_weight, None, None, None, None
 
 
 def _wgmma_head(hidden: torch.Tensor, weight: torch.Tensor) -> bool:
@@ -595,9 +628,11 @@ def _wgmma_head(hidden: torch.Tensor, weight: torch.Tensor) -> bool:
 
 
 def linear_token_log_probs(hidden: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor,
-                           chunk_rows: int | None = None, mode: str | None = None) -> torch.Tensor:
+                           chunk_rows: int | None = None, mode: str | None = None, return_entropy: bool = False):
     """gather_log_probabilities(F.linear(hidden, weight), labels) for hidden (N, H), weight (V, H), labels (N,)
-    without materialising the (N, V) logits / gradient tiles.  Differentiable in hidden and weight."""
+    without materialising the (N, V) logits / gradient tiles.  Differentiable in hidden and weight.  return_entropy:
+    -> (log_probs, entropy), the fp32 entropy of every row from the forward pass that computes the log-probs (K6's
+    entropy variant, or K1's on the library-GEMM path): no extra GEMM pass, no gradient."""
     L.require_cuda(hidden, weight, labels)
     if hidden.dim() != 2 or weight.dim() != 2 or hidden.size(1) != weight.size(1) or labels.shape != hidden.shape[:1]:
         raise ValueError('expected hidden (N, H), weight (V, H), labels (N,)')
@@ -605,24 +640,30 @@ def linear_token_log_probs(hidden: torch.Tensor, weight: torch.Tensor, labels: t
         raise ValueError('hidden and weight must share a dtype')
     V = weight.size(0)
     if hidden.size(0) == 0:
-        return hidden.new_zeros((0,))
+        return (hidden.new_zeros((0,)), hidden.new_zeros((0,), dtype=torch.float32)) if return_entropy else hidden.new_zeros((0,))
     labels = labels.to(torch.int64).contiguous()
+    entropy = torch.zeros(hidden.size(0), dtype=torch.float32, device=hidden.device) if return_entropy else None
     if _K6B and _wgmma_head(hidden, weight):
         if chunk_rows is None:  # ~2 GB of d(logits) per chunk: few read-modify-write passes over the fp32 d(weight)
             chunk_rows = max(128, (2 << 30) // ((V + 255) // 256 * 256 * 2) // 128 * 128)
-        return _LinearLogProbK6Fn.apply(hidden.contiguous(), weight.contiguous(), labels, int(chunk_rows),
-                                        _mode_code(mode, hidden.dtype))
-    # f16 / f32 operands or H % 64 != 0: library GEMMs (cuBLAS) around K1 / K1b -- not the product's hot configuration
-    if chunk_rows is None:  # ~256 MB of logits per chunk
-        chunk_rows = max(128, (256 << 20) // (V * hidden.element_size()) // 128 * 128)
-    return _LinearLogProbFn.apply(hidden.contiguous(), weight.contiguous(), labels, int(chunk_rows),
-                                  _mode_code(mode, hidden.dtype))
+        fn = _LinearLogProbK6Fn
+    else:
+        # f16 / f32 operands or H % 64 != 0: library GEMMs (cuBLAS) around K1 / K1b -- not the product's hot configuration
+        if chunk_rows is None:  # ~256 MB of logits per chunk
+            chunk_rows = max(128, (256 << 20) // (V * hidden.element_size()) // 128 * 128)
+        fn = _LinearLogProbFn
+    args = (hidden.contiguous(), weight.contiguous(), labels, int(chunk_rows), _mode_code(mode, hidden.dtype))
+    if not return_entropy:
+        return fn.apply(*args)
+    return fn.apply(*args, entropy), entropy
 
 
 def fused_linear_token_log_probs(hidden: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor,
-                                 mode: str | None = None, return_stats: bool = False):
+                                 mode: str | None = None, return_stats: bool = False, return_entropy: bool = False):
     """K6 (wgmma): log_softmax(hidden @ weight.T)[label] per row in ONE kernel, no logits tile, for rows that
-    carry NO gradient (reference model / rollout scoring).  hidden (N, H) bf16, weight (V, H) bf16, H % 64 == 0."""
+    carry NO gradient (reference model / rollout scoring).  hidden (N, H) bf16, weight (V, H) bf16, H % 64 == 0.
+    return_stats adds the (2, N) (max, logsum); return_entropy adds the fp32 entropy per row (K6's entropy variant, the
+    same log-probs and statistics bit for bit), in that order."""
     L.require_cuda(hidden, weight, labels)
     if hidden.dim() != 2 or weight.dim() != 2 or hidden.size(1) != weight.size(1) or labels.shape != hidden.shape[:1]:
         raise ValueError('expected hidden (N, H), weight (V, H), labels (N,)')
@@ -630,18 +671,30 @@ def fused_linear_token_log_probs(hidden: torch.Tensor, weight: torch.Tensor, lab
         raise ValueError('K6 takes bf16 operands')
     hidden, weight = _contiguous_last(hidden.detach()), _contiguous_last(weight.detach())
     labels = labels.to(torch.int64).contiguous()
+    entropy = torch.empty(hidden.size(0), dtype=torch.float32, device=hidden.device) if return_entropy else None
+    out, stats = _k6_forward(hidden, weight, labels, _mode_code(mode, hidden.dtype), return_stats, entropy)
+    return (out,) + ((stats,) if return_stats else ()) + ((entropy,) if return_entropy else ()) \
+        if (return_stats or return_entropy) else out
+
+
+def _k6_forward(hidden, weight, labels, mode_code: int, return_stats: bool, entropy=None):
+    """One K6 launch (+ the split merge) on contiguous bf16 operands and int64 labels -> (out, stats or None); with
+    `entropy` (fp32 (N,)) the entropy variant, which also fills it."""
     N, V = hidden.size(0), weight.size(0)
-    mode_code = _mode_code(mode, hidden.dtype)
     out = torch.empty(N, dtype=torch.bfloat16 if mode_code == L.MODE_FAITHFUL else torch.float32, device=hidden.device)
     stats = torch.empty((2, max(N, 1)), dtype=torch.float32, device=hidden.device) if return_stats else None
     sc = _device_scratch(hidden.device)
-    partial = torch.empty(3 * max(132 * 128, 16 * N), dtype=torch.float32, device=hidden.device)  # split-vocabulary statistics
-    L.check(L.lib().aa_linear_logprob_fwd(
-        hidden.data_ptr(), N, hidden.size(1), hidden.stride(0), weight.data_ptr(), V, weight.stride(0), labels.data_ptr(),
-        out.data_ptr(), L.dtype_code(out.dtype), L.ptr(stats[0]) if return_stats else None,
-        L.ptr(stats[1]) if return_stats else None, partial.data_ptr(), partial.numel(), mode_code,
-        sc['status'].data_ptr(), L.stream_ptr(hidden.device)))
-    return (out, stats) if return_stats else out
+    per_split = 3 if entropy is None else 4  # floats per (row, vocabulary split) of the merge scratch
+    partial = torch.empty(per_split * max(132 * 128, 16 * N), dtype=torch.float32, device=hidden.device)
+    args = (hidden.data_ptr(), N, hidden.size(1), hidden.stride(0), weight.data_ptr(), V, weight.stride(0), labels.data_ptr(),
+            out.data_ptr(), L.dtype_code(out.dtype), L.ptr(stats[0]) if return_stats else None,
+            L.ptr(stats[1]) if return_stats else None, partial.data_ptr(), partial.numel(), mode_code,
+            sc['status'].data_ptr())
+    if entropy is None:
+        L.check(L.lib().aa_linear_logprob_fwd(*args, L.stream_ptr(hidden.device)))
+    else:
+        L.check(L.lib().aa_linear_logprob_fwd_entropy(*args, entropy.data_ptr(), L.stream_ptr(hidden.device)))
+    return out, stats
 
 
 def lm_head_weight(module) -> torch.Tensor:
@@ -680,25 +733,36 @@ def _tail_indices(counts: tuple, first_pos: tuple, seq: int, W: int, device_str:
             torch.tensor(dst, dtype=torch.int64).to(dev, non_blocking=True))
 
 
-def _tails_from_hidden(hidden, weight, labels_padded, lens, counts, first_pos, lab_shift, chunk_rows, mode):
+def _tails_from_hidden(hidden, weight, labels_padded, lens, counts, first_pos, lab_shift, chunk_rows, mode,
+                       return_entropy: bool = False):
     """Sample i scores counts[i] rows: hidden position first_pos[i] + k against labels_padded[i, lab_shift + k].
     The scored rows are gathered into a compact (rows, H) matrix: K6 when nothing needs a gradient, else K6 + K6b + the
-    two backward GEMMs (linear_token_log_probs).  Returns (n, max(counts)) right-padded with 0."""
+    two backward GEMMs (linear_token_log_probs).  Returns (n, max(counts)) right-padded with 0; return_entropy: and the
+    fp32 entropy of the same rows, laid out alike, from the same forward kernel."""
     n, seq, H = hidden.shape
     W = max(max(counts), 0)
     out_dtype = hidden.dtype if _mode_code(mode, hidden.dtype) == L.MODE_FAITHFUL else torch.float32
     if W == 0:
-        return hidden.new_zeros((n, 0), dtype=out_dtype)
+        out = hidden.new_zeros((n, 0), dtype=out_dtype)
+        return (out, hidden.new_zeros((n, 0), dtype=torch.float32)) if return_entropy else out
     dev = hidden.device
     src, dst = _tail_indices(tuple(int(c) for c in counts), tuple(int(f) for f in first_pos), seq, W, str(dev))
     rows = hidden.reshape(n * seq, H).index_select(0, src)
     lab = labels_padded[:, lab_shift:lab_shift + W].reshape(-1).index_select(0, dst)
     needs_grad = torch.is_grad_enabled() and (hidden.requires_grad or weight.requires_grad)
-    if not needs_grad and _wgmma_head(hidden, weight):
-        lp = fused_linear_token_log_probs(rows, weight, lab, mode)  # K6: one tensor-core kernel, no logits at all
+    ent = None
+    if not needs_grad and _wgmma_head(hidden, weight):  # K6: one tensor-core kernel, no logits at all
+        lp = fused_linear_token_log_probs(rows, weight, lab, mode, return_entropy=return_entropy)
+        if return_entropy:
+            lp, ent = lp
+    elif return_entropy:
+        lp, ent = linear_token_log_probs(rows, weight, lab, chunk_rows, mode, return_entropy=True)
     else:
         lp = linear_token_log_probs(rows, weight, lab, chunk_rows, mode)
-    return torch.zeros(n * W, dtype=lp.dtype, device=dev).index_copy(0, dst, lp).view(n, W)
+    out = torch.zeros(n * W, dtype=lp.dtype, device=dev).index_copy(0, dst, lp).view(n, W)
+    if not return_entropy:
+        return out
+    return out, torch.zeros(n * W, dtype=torch.float32, device=dev).index_copy(0, dst, ent).view(n, W)
 
 
 def sequence_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, input_ids: torch.Tensor,
@@ -717,24 +781,27 @@ def sequence_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, i
 
 def tail_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, input_ids: torch.Tensor,
                                response_lens: Sequence[int], chunk_rows: int | None = None,
-                               mode: str | None = None) -> torch.Tensor:
+                               mode: str | None = None, return_entropy: bool = False):
     """The multimodal PPO scoring rows (trainers/text_image_to_text/ppo.py:233-246, 296-309): sample b scores
     `logits[b, :-1][-R_b:]` against `input_ids[b, 1:][-R_b:]`, here from the last hidden states (B, L, H) and the
-    lm_head weight -- hidden position L - 1 - R_b + k predicts token L - R_b + k."""
+    lm_head weight -- hidden position L - 1 - R_b + k predicts token L - R_b + k.  return_entropy: -> (log_probs,
+    entropy), the fp32 policy entropy of the same rows (0 in the padding) from the same forward kernel."""
     L.require_cuda(hidden, weight, input_ids)
     lens = tuple(int(r) for r in response_lens)
     seq = hidden.size(1)
     labels = strip_pad_tail(input_ids, lens, 0, strip=False)  # (B, max R): input_ids[b, -R_b:]
-    return _tails_from_hidden(hidden, weight, labels, lens, list(lens), [seq - 1 - r for r in lens], 0, chunk_rows, mode)
+    return _tails_from_hidden(hidden, weight, labels, lens, list(lens), [seq - 1 - r for r in lens], 0, chunk_rows, mode,
+                              return_entropy)
 
 
 def dense_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, input_ids: torch.Tensor, start: int,
-                                chunk_rows: int | None = None, mode: str | None = None) -> torch.Tensor:
+                                chunk_rows: int | None = None, mode: str | None = None, return_entropy: bool = False):
     """`gather_log_probabilities(F.linear(hidden, weight)[:, :-1], input_ids[:, 1:])[:, start:]` from the last hidden
     states (B, L, H) and the lm_head weight (V, H), without the (B, L, V) logits tile: every sample scores the same rows,
     hidden positions [start, L - 1) against tokens [start + 1, L).  The text PPO rollout (start = 0), its rl_step
     (start = prompt_idx) and GRPO (start = L - 1 - logits_to_keep) all read this.  Without a gradient the rows go to K6;
-    with one to linear_token_log_probs.  -> (B, L - 1 - start), the dtype gather_log_probabilities returns."""
+    with one to linear_token_log_probs.  -> (B, L - 1 - start), the dtype gather_log_probabilities returns;
+    return_entropy: (log_probs, fp32 entropy (B, L - 1 - start)) from the same forward kernel (no gradient)."""
     L.require_cuda(hidden, weight, input_ids)
     if hidden.dim() != 3 or input_ids.shape != hidden.shape[:2]:
         raise ValueError('expected hidden (B, L, H) and input_ids (B, L)')
@@ -743,7 +810,8 @@ def dense_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, inpu
     if not 0 <= start <= seq - 1:
         raise ValueError(f'start = {start} lies outside [0, {seq - 1}] for sequences of {seq}')
     W = seq - 1 - start
-    return _tails_from_hidden(hidden, weight, input_ids, (W,) * B, [W] * B, [start] * B, start + 1, chunk_rows, mode)
+    return _tails_from_hidden(hidden, weight, input_ids, (W,) * B, [W] * B, [start] * B, start + 1, chunk_rows, mode,
+                              return_entropy)
 
 
 # ---- DPO -----------------------------------------------------------------------------------------
@@ -1054,9 +1122,11 @@ def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, 
     return _GrpoLossFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype))
 
 
-def tail_token_log_probs(logits: torch.Tensor, input_ids: torch.Tensor, logits_to_keep: int, mode: str | None = None):
+def tail_token_log_probs(logits: torch.Tensor, input_ids: torch.Tensor, logits_to_keep: int, mode: str | None = None,
+                         return_entropy: bool = False):
     """GRPOTrainer._get_per_token_logps after the model forward (trainers/text_to_text/grpo.py:205-210):
-    log-probs of input_ids[:, -K:] under logits[:, :-1][:, -K:], one K1 launch, (B, K)."""
+    log-probs of input_ids[:, -K:] under logits[:, :-1][:, -K:], one K1 launch, (B, K).  return_entropy: and the fp32
+    entropy (B, K) of the same rows from that launch."""
     L.require_cuda(logits, input_ids)
     B, seq, _ = logits.shape
     K = int(logits_to_keep)
@@ -1066,6 +1136,8 @@ def tail_token_log_probs(logits: torch.Tensor, input_ids: torch.Tensor, logits_t
     lens = (K,) * B
     labels = strip_pad_tail(input_ids, lens, 0, strip=False)
     plan = _tail_plan(lens, seq, logits.stride(0), logits.stride(1), K, 0, -1, None, str(logits.device))
+    if return_entropy:
+        return _log_probs_and_entropy(logits, labels, plan, _mode_code(mode, logits.dtype))
     return _LogProbFn.apply(logits, labels, plan, _mode_code(mode, logits.dtype))
 
 
@@ -1076,7 +1148,7 @@ class _GrpoFusedFn(torch.autograd.Function):
     value from the log-probs that pass wrote."""
 
     @staticmethod
-    def forward(ctx, logits, labels, plan, ref_lp, adv, tokens, eos_id, beta, mode_code):
+    def forward(ctx, logits, labels, plan, ref_lp, adv, tokens, eos_id, beta, mode_code, entropy=None):
         dev = logits.device
         B, K = plan.out_shape
         lp_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
@@ -1089,12 +1161,15 @@ class _GrpoFusedFn(torch.autograd.Function):
         sc = _device_scratch(dev)
         p = plan.ptrs()
         lib = L.lib()
-        L.check(lib.aa_logprob_grpo_fused(
-            logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), labels.data_ptr(), plan.n_seg,
-            p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp_dtype), ref_lp.data_ptr(),
-            ref_lp.stride(0), adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), K, float(beta), mode_code,
-            grad.data_ptr(), logits.size(-1), rows.data_ptr(), row_end.data_ptr(), scratch.data_ptr(),
-            sc['counter'][5:6].data_ptr(), sc['status'].data_ptr(), L.stream_ptr(dev)))
+        args = (logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), labels.data_ptr(),
+                plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp_dtype),
+                ref_lp.data_ptr(), ref_lp.stride(0), adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), K,
+                float(beta), mode_code, grad.data_ptr(), logits.size(-1), rows.data_ptr(), row_end.data_ptr(),
+                scratch.data_ptr(), sc['counter'][5:6].data_ptr(), sc['status'].data_ptr())
+        if entropy is None:
+            L.check(lib.aa_logprob_grpo_fused(*args, L.stream_ptr(dev)))
+        else:  # the same launch with the entropy of every completion row from its (max, sum-exp) pass
+            L.check(lib.aa_logprob_grpo_fused_entropy(*args, entropy.data_ptr(), L.stream_ptr(dev)))
         L.check(lib.aa_grpo_loss(lp.data_ptr(), lp.stride(0), ref_lp.data_ptr(), ref_lp.stride(0), L.dtype_code(lp_dtype),
                                  adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), B, K, float(beta),
                                  mode_code, loss.data_ptr(), None, 0, row_end.data_ptr(), scratch.data_ptr(),
@@ -1106,23 +1181,28 @@ class _GrpoFusedFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g, _lp, _re):
         (grad,) = _hand_over_once(ctx, g, *ctx.saved_tensors)
-        return grad, None, None, None, None, None, None, None, None
+        return grad, None, None, None, None, None, None, None, None, None
 
 
 def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_to_keep: int,
                           ref_per_token_logps: torch.Tensor, advantages: torch.Tensor, eos_token_id: int, beta: float,
-                          mode: str | None = None):
+                          mode: str | None = None, return_entropy: bool = False):
     """`_get_per_token_logps` of the policy + the loss of GRPOTrainer.train_step (trainers/text_to_text/grpo.py:205-210,
     290-312) from the policy's logits; the reference model's per-token log-probs must already be there.
     -> (loss fp32 scalar, policy per-token log-probs (B, K), counted tokens per row).  With a gradient: one pass over the
-    completion rows (see _GrpoFusedFn); otherwise tail_token_log_probs + grpo_loss."""
+    completion rows (see _GrpoFusedFn); otherwise tail_token_log_probs + grpo_loss.  return_entropy appends the fp32
+    policy entropy (B, K) of the completion rows, from the same pass (K1f's phase A, or K1's entropy variant); the
+    other outputs are bit-identical."""
     L.require_cuda(logits, input_ids, ref_per_token_logps, advantages)
     K = int(logits_to_keep)
     tokens = input_ids[:, -K:]
     if not _single_pass_ok(logits, _FUSED_GRPO, torch.is_grad_enabled() and logits.requires_grad):
-        lp = tail_token_log_probs(logits, input_ids, K, mode=mode)
+        if return_entropy:
+            lp, ent = tail_token_log_probs(logits, input_ids, K, mode=mode, return_entropy=True)
+        else:
+            lp = tail_token_log_probs(logits, input_ids, K, mode=mode)
         loss, row_end = grpo_loss(lp, ref_per_token_logps, advantages, tokens, eos_token_id, beta, mode=mode)
-        return loss, lp.detach(), row_end
+        return (loss, lp.detach(), row_end, ent) if return_entropy else (loss, lp.detach(), row_end)
     B, seq, _ = logits.shape
     if not 0 < K < seq:
         raise ValueError('logits_to_keep must lie in (0, L)')
@@ -1139,7 +1219,10 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
     if adv.numel() != B:
         raise ValueError('one advantage per sequence expected')
     tok = _contiguous_last(tokens.to(torch.int64))
-    return _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code)
+    if not return_entropy:
+        return _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code)
+    ent = torch.zeros((B, K), dtype=torch.float32, device=logits.device)
+    return _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code, ent) + (ent,)
 
 
 # ---- reward-model pairwise loss -----------------------------------------------------------------------
@@ -2101,6 +2184,18 @@ def response_tail_log_probs_pair(logits_a: torch.Tensor, logits_b: torch.Tensor,
     """response_tail_log_probs of TWO logits tensors of identical shape / dtype / strides against the same labels (the
     rollout's actor and reference model, text_image_to_text/ppo.py:229-246) in ONE K1 launch: the second tensor is
     addressed relative to the first one's base pointer.  No gradient.  -> (log_probs_a, log_probs_b), each (B, W)."""
+    return _tail_pair(logits_a, logits_b, input_ids, lens, mode, False)
+
+
+def response_tail_log_probs_pair_with_entropy(logits_a: torch.Tensor, logits_b: torch.Tensor, input_ids: torch.Tensor,
+                                              lens, mode: str | None = None):
+    """response_tail_log_probs_pair plus the fp32 policy entropy of the FIRST tensor's scored rows (the actor's), from
+    the same single launch (K1's entropy variant; the second copy's rows skip the store).  -> (log_probs_a, log_probs_b,
+    entropy_a), each (B, W); the log-probs are bit-identical to response_tail_log_probs_pair's."""
+    return _tail_pair(logits_a, logits_b, input_ids, lens, mode, True)
+
+
+def _tail_pair(logits_a, logits_b, input_ids, lens, mode, with_entropy: bool):
     L.require_cuda(logits_a, logits_b, input_ids)
     lens = as_device_lens(lens, logits_a.device)
     a, b = _contiguous_last(logits_a.detach()), _contiguous_last(logits_b.detach())
@@ -2117,8 +2212,12 @@ def response_tail_log_probs_pair(logits_a: torch.Tensor, logits_b: torch.Tensor,
                             delta // a.element_size())
     mode_code = _mode_code(mode, a.dtype)
     out = torch.zeros(plan.out_shape, dtype=a.dtype if mode_code == L.MODE_FAITHFUL else torch.float32, device=a.device)
-    _launch_fwd(a, ids, plan, out, None, None)
-    return out[0], out[1]
+    if not with_entropy:
+        _launch_fwd(a, ids, plan, out, None, None)
+        return out[0], out[1]
+    entropy = torch.zeros(plan.out_shape[1:], dtype=torch.float32, device=a.device)  # room for the first copy only
+    _launch_fwd(a, ids, plan, out, None, None, entropy=entropy)
+    return out[0], out[1], entropy
 
 
 def count_nonpad(ids: torch.Tensor, pad_id: int) -> torch.Tensor:

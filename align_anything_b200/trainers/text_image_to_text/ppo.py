@@ -15,7 +15,7 @@ import torch
 
 from ... import ops
 from ...utils.multi_process import all_reduce_packed, fused_allreduce
-from ..text_to_text.ppo import METRIC_KEYS
+from ..text_to_text.ppo import METRIC_KEYS, with_entropy_lane
 from ..text_to_text.ppo import PPOTrainer as _TextPPOTrainer
 
 __all__ = ['PPOTrainer', 'move_padding_left']
@@ -47,14 +47,16 @@ class PPOTrainer(_TextPPOTrainer):
     # loops over micro-batches of per_device_train_batch_size (text_audio_to_text/ppo.py:217-277)
     micro_batched_rollout = False
 
-    def _tail_log_probs(self, model, batch, lens, input_ids, **kw):
-        """(B, W) log-probs of the response tails, right-padded with 0 (W = lens.bound)."""
+    def _tail_log_probs(self, model, batch, lens, input_ids, return_entropy=False, **kw):
+        """(B, W) log-probs of the response tails, right-padded with 0 (W = lens.bound); return_entropy (fused_lm_head
+        only): and the fp32 policy entropy of the same rows, from the same kernel."""
         lens = ops.as_device_lens(lens, input_ids.device)
         if self.fused_lm_head:
             out = model(**batch, output_hidden_states=True, logits_to_keep=1, **kw)
             module = getattr(model, 'module', model)
             return ops.tail_log_probs_from_hidden(out.hidden_states[-1], ops.lm_head_weight(module), input_ids,
-                                                  lens.tolist(), chunk_rows=self.lm_head_chunk_rows, mode=self.mode)
+                                                  lens.tolist(), chunk_rows=self.lm_head_chunk_rows, mode=self.mode,
+                                                  return_entropy=return_entropy)
         logits = self._actor_logits(model, batch, lens, **kw)
         return ops.response_tail_log_probs(logits, input_ids, lens, mode=self.mode)
 
@@ -114,12 +116,18 @@ class PPOTrainer(_TextPPOTrainer):
         reward_batch = self.reward_model_step(actor_batch)
         ids = actor_batch['input_ids']
         lens = ops.as_device_lens(response_lens, ids.device)
+        entropy = None
         if not self.fused_lm_head:  # both models' tiles through ONE K1 launch
-            log_probs, ref_log_probs = ops.response_tail_log_probs_pair(
-                self._actor_logits(self.actor_model, actor_batch, lens),
-                self._actor_logits(self.actor_reference_model, actor_batch, lens), ids, lens, mode=self.mode)
+            pair = ops.response_tail_log_probs_pair_with_entropy if self.log_entropy else ops.response_tail_log_probs_pair
+            scored = pair(self._actor_logits(self.actor_model, actor_batch, lens),
+                          self._actor_logits(self.actor_reference_model, actor_batch, lens), ids, lens, mode=self.mode)
+            log_probs, ref_log_probs = scored[:2]
+            if self.log_entropy:
+                entropy = scored[2]
         else:
-            log_probs = self._tail_log_probs(self.actor_model, actor_batch, lens, ids)
+            log_probs = self._tail_log_probs(self.actor_model, actor_batch, lens, ids, return_entropy=self.log_entropy)
+            if self.log_entropy:
+                log_probs, entropy = log_probs
             ref_log_probs = self._tail_log_probs(self.actor_reference_model, actor_batch, lens, ids)
         training = {
             'response_lens': lens,  # ops.DeviceLens: list-like for reference code, device tensor for ours
@@ -129,6 +137,8 @@ class PPOTrainer(_TextPPOTrainer):
             'reward_values': _tail_values(reward_batch['reward_values'], lens),
             'response_mask': (log_probs != 0),
         }
+        if entropy is not None:
+            training['entropy'] = entropy  # (B, W) fp32, the actor's response tails, aligned with log_probs
         inference = dict(actor_batch)
         inference['input_ids'] = reward_batch['input_ids']
         return inference, training
@@ -168,14 +178,18 @@ class PPOTrainer(_TextPPOTrainer):
         self.reward_critic_model.step()
 
         with torch.no_grad():
-            fused = fused_allreduce(row_stats.device)
+            fused = fused_allreduce(row_stats.device) if not self.log_entropy else None  # see the text rl_step
             stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss32, critic_loss32,
                                          coll=fused.next((9, 10)) if fused is not None else None)
+            if self.log_entropy:
+                stats = with_entropy_lane(stats, training_batch['entropy'], sequence_mask)
             if fused is None:
                 stats = all_reduce_packed(stats, max_lanes=(9, 10))
             v = stats.tolist()  # the ONE host sync of rollout scoring + rl_step
         ops.raise_for_status(v[10], stats.device)  # lane 10 = device status word (MAX over ranks): raise like the reference
         out = dict(zip(METRIC_KEYS, v[:10]))
+        if self.log_entropy:
+            out['train/entropy'] = v[11]
         out['train/actor_lr'] = self.actor_model.optimizer.param_groups[0]['lr']
         out['train/reward_critic_lr'] = self.reward_critic_model.optimizer.param_groups[0]['lr']
         self.last_rl_tensors = {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns}

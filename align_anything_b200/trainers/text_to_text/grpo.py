@@ -23,6 +23,9 @@ class GRPOTrainer:
     # two backward GEMMs (ops.dense_log_probs_from_hidden), then the GRPO loss kernel (ops.grpo_loss).
     fused_lm_head = False
     lm_head_chunk_rows = None
+    # Opt-in: `train/entropy`, the policy entropy of the completions (token mean over the completion mask, as the loss),
+    # from the policy pass of the step (K1f's phase A, or K6 with fused_lm_head), in the step's one packed collective
+    log_entropy = False
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, tokenizer=None, *, beta=None,
                  num_generations=None) -> None:
@@ -35,13 +38,14 @@ class GRPOTrainer:
         self.num_generations = num_generations if num_generations is not None else getattr(tc, 'num_generations', 4)
 
     # -- trainers/text_to_text/grpo.py:199-210 ---------------------------------------------------
-    def _get_per_token_logps(self, model, input_ids, attention_mask, logits_to_keep):
+    def _get_per_token_logps(self, model, input_ids, attention_mask, logits_to_keep, return_entropy=False):
         """Log-probs of the last `logits_to_keep` tokens: one K1 launch on the model's logits (the reference
-        slices, log-softmaxes the whole (B, K, V) tile and gathers).  With fused_lm_head: from the hidden states."""
+        slices, log-softmaxes the whole (B, K, V) tile and gathers).  With fused_lm_head: from the hidden states
+        (return_entropy: and the fp32 entropy of the same rows, from the same kernel)."""
         if self.fused_lm_head:
             return hidden_log_probs(model, {'input_ids': input_ids, 'attention_mask': attention_mask}, input_ids,
                                     input_ids.size(1) - 1 - logits_to_keep, lm_head_of(model), self.lm_head_chunk_rows,
-                                    self.mode)
+                                    self.mode, return_entropy=return_entropy)
         logits = model(input_ids=input_ids, attention_mask=attention_mask).logits
         return ops.tail_token_log_probs(logits, input_ids, logits_to_keep, mode=self.mode)
 
@@ -58,23 +62,38 @@ class GRPOTrainer:
         with torch.no_grad():
             ref_per_token_logps = self._get_per_token_logps(self.actor_reference_model, sequences, attention_mask,
                                                             logits_to_keep)
+        entropy = None
         if self.fused_lm_head:  # the composed path: K1f needs a logits tile
-            per_token_logps = self._get_per_token_logps(self.actor_model, sequences, attention_mask, logits_to_keep)
-            loss, _ = ops.grpo_loss(per_token_logps, ref_per_token_logps, advantages, sequences[:, -logits_to_keep:],
-                                    self.tokenizer.eos_token_id, self.beta, mode=self.mode)
+            per_token_logps = self._get_per_token_logps(self.actor_model, sequences, attention_mask, logits_to_keep,
+                                                        return_entropy=self.log_entropy)
+            if self.log_entropy:
+                per_token_logps, entropy = per_token_logps
+            loss, row_end = ops.grpo_loss(per_token_logps, ref_per_token_logps, advantages,
+                                          sequences[:, -logits_to_keep:], self.tokenizer.eos_token_id, self.beta,
+                                          mode=self.mode)
         else:
             logits = self.actor_model(input_ids=sequences, attention_mask=attention_mask).logits
-            loss, _, _ = ops.grpo_loss_from_logits(logits, sequences, logits_to_keep, ref_per_token_logps, advantages,
-                                                   self.tokenizer.eos_token_id, self.beta, mode=self.mode)
+            scored = ops.grpo_loss_from_logits(logits, sequences, logits_to_keep, ref_per_token_logps, advantages,
+                                               self.tokenizer.eos_token_id, self.beta, mode=self.mode,
+                                               return_entropy=self.log_entropy)
+            loss, row_end = scored[0], scored[2]
+            if self.log_entropy:
+                entropy = scored[3]
         self.actor_model.zero_grad()
         self.actor_model.backward(loss)
         self.actor_model.step()
         with torch.no_grad():
-            stats = torch.cat([torch.stack([loss.detach().float(), rewards.float().mean()]), ops.status_lane(loss.device)])
+            lanes = [torch.stack([loss.detach().float(), rewards.float().mean()]), ops.status_lane(loss.device)]
+            if self.log_entropy:  # token mean over the completion mask (tokens up to and including the first eos)
+                mask = torch.arange(logits_to_keep, device=row_end.device) < row_end.unsqueeze(1)
+                lanes.append(((entropy * mask).sum() / mask.sum()).reshape(1))
             # ONE collective, ONE sync (reference: 2 + 2); lane 2 = device status word, MAX over ranks
-            loss_val, avg_reward, status = all_reduce_packed(stats, max_lanes=(2,)).tolist()
-        ops.raise_for_status(status, loss.device)
-        return {'train/loss': loss_val, 'train/reward': avg_reward}
+            v = all_reduce_packed(torch.cat(lanes), max_lanes=(2,)).tolist()
+        ops.raise_for_status(v[2], loss.device)
+        out = {'train/loss': v[0], 'train/reward': v[1]}
+        if self.log_entropy:
+            out['train/entropy'] = v[3]
+        return out
 
     def train_step(self, prompt_batch: dict) -> dict[str, float]:
         """trainers/text_to_text/grpo.py:258-318; generate_completions / compute_rewards come from the reference."""

@@ -22,7 +22,7 @@ import torch
 
 from ... import ops
 from ...utils.multi_process import all_reduce_packed, fused_allreduce
-from .ppo import METRIC_KEYS, actor_loss_node, lm_head_of
+from .ppo import METRIC_KEYS, actor_loss_node, lm_head_of, with_entropy_lane
 from .ppo import PPOTrainer as _TextPPOTrainer
 
 __all__ = ['PPOTrainer']
@@ -125,14 +125,18 @@ class PPOTrainer(_TextPPOTrainer):
         self.reward_critic_model.step()
 
         with torch.no_grad():
-            fused = fused_allreduce(row_stats.device)
+            fused = fused_allreduce(row_stats.device) if not self.log_entropy else None  # see the text rl_step
             stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss32, reward_critic_loss,
                                          coll=fused.next((9, 10)) if fused is not None else None)
+            if self.log_entropy:
+                stats = with_entropy_lane(stats, training_batch['entropy'][:, start:], sequence_mask[:, start:])
             if fused is None:
                 stats = all_reduce_packed(stats, max_lanes=(9, 10))  # ONE collective (reference: 10 + barrier)
             v = stats.tolist()  # ONE host sync (reference: 12 .item())
         ops.raise_for_status(v[10], stats.device)
         out = dict(zip(METRIC_KEYS, v[:10]))
+        if self.log_entropy:
+            out['train/entropy'] = v[11]
         out['train/actor_lr'] = self.actor_model.optimizer.param_groups[0]['lr']
         out['train/reward_critic_lr'] = self.reward_critic_model.optimizer.param_groups[0]['lr']
         self.last_rl_tensors = {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns}

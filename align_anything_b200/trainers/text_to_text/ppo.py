@@ -32,12 +32,21 @@ def lm_head_of(model) -> torch.Tensor:
     return ops.lm_head_weight(getattr(model, 'module', model))
 
 
-def hidden_log_probs(model, batch, input_ids, start, weight, chunk_rows, mode, **kw) -> torch.Tensor:
+def hidden_log_probs(model, batch, input_ids, start, weight, chunk_rows, mode, return_entropy=False, **kw):
     """`gather_log_probabilities(model(**batch).logits[:, :-1], input_ids[:, 1:])[:, start:]` from the model's last
-    hidden states: the lm_head runs on one position inside the model and on the scored rows in ops, no logits tile."""
+    hidden states: the lm_head runs on one position inside the model and on the scored rows in ops, no logits tile.
+    return_entropy: -> (log_probs, fp32 policy entropy of the same rows) from the same kernel."""
     out = model(**batch, output_hidden_states=True, logits_to_keep=1, **kw)
     return ops.dense_log_probs_from_hidden(out.hidden_states[-1], weight, input_ids, start, chunk_rows=chunk_rows,
-                                           mode=mode)
+                                           mode=mode, return_entropy=return_entropy)
+
+
+def with_entropy_lane(stats: torch.Tensor, entropy: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
+    """ppo_pack_metrics' vector with its spare last lane (always 0) set to the rollout policy's entropy, reduced like
+    train/kl_divergence: summed over each row's masked tokens, averaged over rows (and, by the step's one packed
+    all-reduce, over ranks), so the two read side by side.  Two tiny launches, no host sync."""
+    ent = (entropy * mask).sum(dim=-1).mean()
+    return torch.cat([stats[:11], ent.reshape(1)])
 
 
 def actor_loss_node(tr, inference_batch, input_ids, start, head, old_log_probs, advantages, sequence_mask):
@@ -66,6 +75,9 @@ class PPOTrainer:
     # backward GEMMs and then K5 (ops.dense_log_probs_from_hidden -> ops.actor_loss).  ptx_step keeps its logits.
     fused_lm_head = False
     lm_head_chunk_rows = None
+    # Opt-in: `train/entropy`, the policy entropy of the rollout, taken from the pass that scores its log-probs (K1's
+    # or K6's entropy variant: one more FMA per logit, no extra read) and reduced in the step's one packed collective
+    log_entropy = False
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, reward_model=None,
                  reward_critic_model=None, tokenizer=None, reward_tokenizer=None, *, kl_coeff=0.02,
@@ -176,15 +188,21 @@ class PPOTrainer:
             heads = (lm_head_of(self.actor_model), lm_head_of(self.actor_reference_model))
         reward_batch = self.reward_model_step(actor_batch)
         ids = actor_batch['input_ids']
+        entropy = None
         if self.fused_lm_head:  # every position, prompt and pad included: the width the tile path stores
             log_probs = hidden_log_probs(self.actor_model, actor_batch, ids, 0, heads[0], self.lm_head_chunk_rows,
-                                         self.mode)
+                                         self.mode, return_entropy=self.log_entropy)
+            if self.log_entropy:
+                log_probs, entropy = log_probs
             ref_log_probs = hidden_log_probs(self.actor_reference_model, actor_batch, ids, 0, heads[1],
                                              self.lm_head_chunk_rows, self.mode)
         else:
             logits = self.actor_model(**actor_batch).logits
             ref_logits = self.actor_reference_model(**actor_batch).logits
-            log_probs = ops.gather_log_probabilities(logits[:, :-1], ids[:, 1:], mode=self.mode)
+            if self.log_entropy:
+                log_probs, entropy = ops.gather_log_probabilities_with_entropy(logits[:, :-1], ids[:, 1:], mode=self.mode)
+            else:
+                log_probs = ops.gather_log_probabilities(logits[:, :-1], ids[:, 1:], mode=self.mode)
             ref_log_probs = ops.gather_log_probabilities(ref_logits[:, :-1], ids[:, 1:], mode=self.mode)
         training = {
             'prompt_idx': prompt_len - 1,
@@ -193,6 +211,8 @@ class PPOTrainer:
             'reward': reward_batch['reward'],
             'reward_values': reward_batch['reward_values'],
         }
+        if entropy is not None:
+            training['entropy'] = entropy  # (B, L - 1) fp32, the actor's, aligned with log_probs
         inference = {'input_ids': reward_batch['input_ids'], 'attention_mask': actor_batch['attention_mask']}
         return inference, training
 
@@ -240,14 +260,20 @@ class PPOTrainer:
         self.reward_critic_model.step()
 
         with torch.no_grad():
-            fused = fused_allreduce(row_stats.device)
+            # with log_entropy the entropy lane is filled in before the one packed all-reduce, so the NVLink reduction
+            # fused into ppo_pack_metrics (which reduces the vector as it writes it) gives way to all_reduce_packed
+            fused = fused_allreduce(row_stats.device) if not self.log_entropy else None
             stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss32, reward_critic_loss,
                                          coll=fused.next((9, 10)) if fused is not None else None)
+            if self.log_entropy:
+                stats = with_entropy_lane(stats, training_batch['entropy'][:, start:], sequence_mask[:, start:])
             if fused is None:
                 stats = all_reduce_packed(stats, max_lanes=(9, 10))  # ONE collective (reference: 10 + barrier)
             v = stats.tolist()  # ONE host sync (reference: 12 .item())
         ops.raise_for_status(v[10], stats.device)  # lane 10 = device status word (MAX over ranks): raise like the reference
         out = dict(zip(METRIC_KEYS, v[:10]))
+        if self.log_entropy:
+            out['train/entropy'] = v[11]
         out['train/actor_lr'] = self.actor_model.optimizer.param_groups[0]['lr']
         out['train/reward_critic_lr'] = self.reward_critic_model.optimizer.param_groups[0]['lr']
         # the per-token tensors stay OUT of the returned dict: the reference hands it to Logger.log -> add_scalar /

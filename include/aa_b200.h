@@ -108,6 +108,21 @@ int aa_logprob_fwd(const void *logits, int logits_dtype, int64_t row_stride, int
                    void *out, int out_dtype, float *stat_max, float *stat_logsum,
                    int32_t *status, void *stream);
 
+/* K1 with the policy entropy of every scored row: aa_logprob_fwd's arguments (same outputs, bit for bit) plus
+ *   entropy   : fp32, H = -sum_j p_j log p_j of the row's fp32-upcast logits, written at the row's OUT position
+ *               (never rounded to out_dtype).  Only rows whose out position is < n_entropy are written: with a two-copy
+ *               plan (aa_tail_plan_build, copies = 2) n_entropy = copy_out_delta keeps the entropy of the first copy
+ *               and the buffer needs no room for the second.  Ignored rows (use_ignore) get 0; rows the plan does not
+ *               score are not written (the caller zero-initialises); an all -inf row gets NaN; a -inf logit adds 0.
+ * One more FMA (and a clamp) per logit on top of the online (max, sum-exp): t = sum_j e^{x_j - m} (x_j - m), H = log s - t / s. */
+int aa_logprob_fwd_entropy(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                           const int64_t *labels, int64_t ignore_index, int32_t use_ignore,
+                           int32_t n_segments, int64_t n_rows,
+                           const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                           const int64_t *seg_out_off, const int64_t *seg_cum,
+                           void *out, int out_dtype, float *stat_max, float *stat_logsum,
+                           int32_t *status, float *entropy, int64_t n_entropy, void *stream);
+
 /* ---------------------------------------------------------------------------------------
  * K1b  d(log-prob)/d(logits): autograd of the two ops above (ATen _log_softmax_backward_data
  * + gather backward) in ONE pass: grad[j] = g * ([j == label] - softmax_j), written in the
@@ -400,6 +415,17 @@ int aa_logprob_grpo_fused(const void *logits, int logits_dtype, int64_t row_stri
                           const float *advantages, const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id,
                           int32_t K, float beta, int mode, void *grad_logits, int64_t grad_row_stride, void *row_scratch,
                           int32_t *row_end, float *total, uint32_t *counter, int32_t *status, void *stream);
+/* The same launch with the entropy of every scored row (fp32, aa_logprob_fwd_entropy's definition) written to entropy,
+ * laid out like log_probs ((n_segments, K), zero-initialised by the caller), from the (max, sum-exp) pass (phase A).
+ * log_probs, the gradient tile and everything else are bit-identical to aa_logprob_grpo_fused. */
+int aa_logprob_grpo_fused_entropy(const void *logits, int logits_dtype, int64_t row_stride, int32_t V, const int64_t *labels,
+                                  int32_t n_segments, const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                                  const int64_t *seg_out_off, const int64_t *seg_cum, const int64_t *seg_tile_row,
+                                  int64_t n_tile_rows, void *log_probs, int lp_dtype, const void *ref_log_probs,
+                                  int64_t ref_stride, const float *advantages, const int64_t *completion_tokens,
+                                  int64_t tok_stride, int64_t eos_id, int32_t K, float beta, int mode, void *grad_logits,
+                                  int64_t grad_row_stride, void *row_scratch, int32_t *row_end, float *total,
+                                  uint32_t *counter, int32_t *status, float *entropy, void *stream);
 
 /* tile[0..n) *= *scale unless *scale == 1 (checked on the device: the usual `loss.backward()` costs one empty launch).
  * Contiguous tile; scale: device scalar of scale_dtype.  The autograd backward of the K1f node. */
@@ -471,6 +497,16 @@ int aa_linear_logprob_fwd(const void *hidden, int64_t n_rows, int32_t H, int64_t
                           const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
                           void *out, int out_dtype, float *stat_max, float *stat_logsum, float *partial,
                           int64_t partial_floats, int mode, int32_t *status, void *stream);
+
+/* K6 with the entropy of every row: entropy fp32 [n_rows], H = -sum_j p_j log p_j over the logits the statistics fold
+ * (bf16-rounded in FAITHFUL mode, the fp32 accumulators in F32 mode), never rounded.  The (max, sum-exp, entropy sum)
+ * merge across the quad and across vocabulary splits uses t' = alpha (t + (m - m') s); `partial` then holds FOUR floats
+ * per (row, split): 4 * 132 * 128 always suffices on a 132-SM H100 (with fewer floats the split count is lowered as for
+ * K6).  out, stat_max and stat_logsum are bit-identical to aa_linear_logprob_fwd. */
+int aa_linear_logprob_fwd_entropy(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
+                                  const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
+                                  void *out, int out_dtype, float *stat_max, float *stat_logsum, float *partial,
+                                  int64_t partial_floats, int mode, int32_t *status, float *entropy, void *stream);
 
 /* K6s: K6 with a second epilogue on the same accumulator tile -- every logit is rounded to bf16 (nn.Linear's rounding
  * point, in both modes: the stored tile is bf16) and stored into `logits` (n_rows, ld), ld >= ceil(V / 256) * 256 and a
