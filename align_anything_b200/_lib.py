@@ -46,8 +46,13 @@ _SIGS = {
                                        _P, _P, c_int, _P, _P, _P, _P, c_int64, _P]),
     'aa_logprob_bwd': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int64, c_int32, c_int32, c_int64, _P, _P, _P, _P,
                                _P, _P, _P, _P, c_int, _P, _P, c_int, _P, c_int64, c_int64, _P, c_int64, _P, c_int, _P]),
+    'aa_logprob_bwd_entropy': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int64, c_int32, c_int32, c_int64, _P, _P, _P,
+                                       _P, _P, _P, _P, _P, c_int, _P, _P, c_int, _P, _P, c_int, _P, c_int64, c_int64, _P,
+                                       c_int64, _P, c_int, _P]),
     'aa_zero_rows': (c_int, [_P, c_int, c_int64, c_int32, c_int64, _P, c_int32, _P]),
     'aa_linear_dlogits': (c_int, [_P, c_int64, c_int32, c_int64, _P, c_int32, c_int64, _P, _P, _P, _P, c_int, _P, c_int64, c_int, _P]),
+    'aa_linear_dlogits_entropy': (c_int, [_P, c_int64, c_int32, c_int64, _P, c_int32, c_int64, _P, _P, _P, _P, c_int, _P,
+                                          _P, c_int, _P, c_int64, c_int, _P]),
     'aa_linear_dhidden': (c_int, [_P, c_int64, c_int64, _P, c_int32, c_int32, c_int64, _P, c_int64, _P]),
     'aa_linear_dweight': (c_int, [_P, c_int64, c_int64, _P, c_int32, c_int64, c_int32, _P, c_int64, c_int32, _P, c_int64, _P]),
     'aa_linear_logprob_fwd': (c_int, [_P, c_int64, c_int32, c_int64, _P, c_int32, c_int64, _P, _P, c_int, _P, _P, _P, c_int64,
@@ -80,6 +85,9 @@ _SIGS = {
     'aa_logprob_actor_fused': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P, c_int, _P, _P,
                                        _P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int32, c_float, c_int, _P, c_int64, _P,
                                        _P, _P]),
+    'aa_logprob_actor_fused_entropy': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P,
+                                               c_int, _P, _P, _P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int32,
+                                               c_float, c_int, _P, c_int64, _P, _P, c_float, _P, _P]),
     'aa_logprob_ce_fused': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int64, c_int64, c_int32, _P, _P, _P, _P, _P, c_int64, _P,
                                     c_float, _P, c_int64, _P, _P, _P, _P]),
     'aa_logprob_grpo_fused': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P, c_int, _P, c_int64,
@@ -87,6 +95,9 @@ _SIGS = {
     'aa_logprob_grpo_fused_entropy': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P, c_int,
                                               _P, c_int64, _P, _P, c_int64, c_int64, c_int32, c_float, c_int, _P, c_int64, _P,
                                               _P, _P, _P, _P, _P, _P]),
+    'aa_logprob_grpo_fused_entropy_grad': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64,
+                                                   _P, c_int, _P, c_int64, _P, _P, c_int64, c_int64, c_int32, c_float,
+                                                   c_int, _P, c_int64, _P, _P, _P, _P, _P, _P, c_float, _P]),
     'aa_scale_tile': (c_int, [_P, c_int, c_int64, _P, c_int, _P]),
     'aa_tail_scatter_scaled': (c_int, [_P, c_int, c_int64, _P, c_int32, c_int32, c_int32, _P, c_int, _P, c_int64, c_int32, _P]),
     'aa_group_advantages': (c_int, [_P, c_int32, c_int32, _P, _P]),

@@ -48,6 +48,10 @@ struct GradParams {
   int grad_rows_dtype;
   __nv_bfloat16 *dlogits; // (n_rows, ld) bf16, ld >= ceil(V / 256) * 256, multiple of 8
   int64_t ld;
+  // K6b's entropy-gradient kernel (ENT): the upstream gradient of each row's entropy (dtype grad_entropy_dtype); the
+  // entropy itself is read from Params::entropy (K6's entropy variant wrote it)
+  const void *grad_entropy;
+  int grad_entropy_dtype;
 };
 
 // what the consumer warpgroups do with a finished 128 x 256 logits tile
@@ -269,7 +273,10 @@ __global__ void __launch_bounds__(THREADS, 1)
     // ------------------------------- K6b epilogue: d(logits) tile store ----------------
     // d(logits)[row, col] = g * ([col == label] - p),  p = exp(round_bf16((x - max) - logsum)) in FAITHFUL mode
     // (what ATen's backward sees: it re-reads the rounded log-softmax), written as bf16 into the padded buffer
-    float m[2], logsum[2], g[2];
+    // ENT: a row whose entropy has the upstream gradient g_H gets - g_H p (l + H) added in fp32 before the bf16 store,
+    // with the p and l of the line above (logprob_math.cuh, vec_grad_ent); rows with g_H == 0 keep the plain bits
+    // (a select, not a branch: the accumulators must not be read in divergent code)
+    float m[2], logsum[2], g[2], h[2] = {0.f, 0.f}, ngh[2] = {0.f, 0.f};
     __nv_bfloat16 *drow[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -277,6 +284,10 @@ __global__ void __launch_bounds__(THREADS, 1)
       logsum[r] = live[r] ? __ldg(p.stat_logsum + row[r]) : 0.f;
       g[r] = live[r] ? load_as_float(gp.grad_rows, row[r], gp.grad_rows_dtype) : 0.f;
       drow[r] = gp.dlogits + (live[r] ? row[r] : 0) * gp.ld;
+      if constexpr (ENT) {
+        h[r] = live[r] ? __ldg(p.entropy + row[r]) : 0.f;
+        ngh[r] = live[r] ? -load_as_float(gp.grad_entropy, row[r], gp.grad_entropy_dtype) : 0.f;
+      }
     }
     for (int nt = 0; nt < n_tiles; ++nt) {
       consume_tile<0, 0>(acc, tiles, full, empty, k_blocks, it, w);
@@ -289,10 +300,17 @@ __global__ void __launch_bounds__(THREADS, 1)
         if (p.faithful) round_bf16_pair(xs[0], xs[1]);
         float ls[2] = {(xs[0] - m[r]) - logsum[r], (xs[1] - m[r]) - logsum[r]};
         if (p.faithful) round_bf16_pair(ls[0], ls[1]);
-        float d0 = ex2_approx(ls[0] * kLog2e) * -g[r];  // -(p * g), every column but the label's
-        float d1 = ex2_approx(ls[1] * kLog2e) * -g[r];
+        const float e0 = ex2_approx(ls[0] * kLog2e), e1 = ex2_approx(ls[1] * kLog2e);
+        float d0 = e0 * -g[r];  // -(p * g), every column but the label's
+        float d1 = e1 * -g[r];
         if (label[r] == col) d0 = __fadd_rn(d0, g[r]);  // g - p * g, the same two roundings
         if (label[r] == col + 1) d1 = __fadd_rn(d1, g[r]);
+        if constexpr (ENT) {
+          const float c0 = fmaf(e0 * (fmaxf(ls[0], -3.0e38f) + h[r]), ngh[r], d0);
+          const float c1 = fmaf(e1 * (fmaxf(ls[1], -3.0e38f) + h[r]), ngh[r], d1);
+          d0 = ngh[r] != 0.f ? c0 : d0;
+          d1 = ngh[r] != 0.f ? c1 : d1;
+        }
         if (col >= p.V) d0 = 0.f;  // last vocabulary tile: pad columns of the buffer stay zero
         if (col + 1 >= p.V) d1 = 0.f;
         if (live[r]) *reinterpret_cast<uint32_t *>(drow[r] + col) = pack2<__nv_bfloat16>(d0, d1);
@@ -450,7 +468,7 @@ extern "C" int aa_linear_logprob_fwd(const void *hidden, int64_t n_rows, int32_t
                                      int64_t partial_floats, int mode, int32_t *status, void *stream) {
   return k6::forward<k6::Epi::Lse>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, labels, out,
                                    out_dtype, stat_max, stat_logsum, partial, partial_floats, mode, status,
-                                   k6::GradParams{nullptr, AA_F32, nullptr, 0}, stream, "aa_linear_logprob_fwd");
+                                   k6::GradParams{nullptr, AA_F32, nullptr, 0, nullptr, AA_F32}, stream, "aa_linear_logprob_fwd");
 }
 
 extern "C" int aa_linear_logprob_fwd_entropy(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
@@ -461,7 +479,7 @@ extern "C" int aa_linear_logprob_fwd_entropy(const void *hidden, int64_t n_rows,
   AA_REQUIRE(n_rows == 0 || entropy, AA_ERR_ARG, "aa_linear_logprob_fwd_entropy: null entropy");
   return k6::forward<k6::Epi::Lse, true>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, labels, out,
                                          out_dtype, stat_max, stat_logsum, partial, partial_floats, mode, status,
-                                         k6::GradParams{nullptr, AA_F32, nullptr, 0}, stream,
+                                         k6::GradParams{nullptr, AA_F32, nullptr, 0, nullptr, AA_F32}, stream,
                                          "aa_linear_logprob_fwd_entropy", entropy);
 }
 
@@ -478,33 +496,62 @@ extern "C" int aa_linear_logits(const void *hidden, int64_t n_rows, int32_t H, i
   }
   return k6::forward<k6::Epi::Logits>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, labels, out,
                                       out_dtype, stat_max, stat_logsum, partial, partial_floats, mode, status,
-                                      k6::GradParams{nullptr, AA_F32, static_cast<__nv_bfloat16 *>(logits), ld}, stream,
+                                      k6::GradParams{nullptr, AA_F32, static_cast<__nv_bfloat16 *>(logits), ld, nullptr, AA_F32}, stream,
                                       "aa_linear_logits");
+}
+
+// aa_linear_dlogits{,_entropy}: entropy == nullptr runs the plain kernel
+static int linear_dlogits(const char *who, const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
+                          const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
+                          const float *stat_max, const float *stat_logsum, const void *grad_rows, int grad_rows_dtype,
+                          const float *entropy, const void *grad_entropy, int grad_entropy_dtype, void *dlogits,
+                          int64_t ld, int mode, void *stream) {
+  AA_REQUIRE(n_rows >= 0 && H > 0 && V > 0, AA_ERR_ARG, "%s: bad sizes", who);
+  if (n_rows == 0) return AA_OK;
+  AA_REQUIRE(hidden && weight && labels && stat_max && stat_logsum && grad_rows && dlogits, AA_ERR_ARG,
+             "%s: null pointer", who);
+  AA_REQUIRE(H % k6::BK == 0, AA_ERR_UNSUPPORTED, "%s: H=%d must be a multiple of %d", who, H, k6::BK);
+  const int all_tiles = (V + k6::BN - 1) / k6::BN;
+  AA_REQUIRE(ld >= static_cast<int64_t>(all_tiles) * k6::BN && ld % 8 == 0 && (reinterpret_cast<uintptr_t>(dlogits) & 15) == 0,
+             AA_ERR_ALIGN, "%s: ld must be >= ceil(V / 256) * 256, a multiple of 8, buffer 16-byte aligned", who);
+  AA_REQUIRE((reinterpret_cast<uintptr_t>(hidden) & 15) == 0 && (reinterpret_cast<uintptr_t>(weight) & 15) == 0 &&
+                 hidden_row_stride % 8 == 0 && weight_row_stride % 8 == 0 && hidden_row_stride >= H && weight_row_stride >= H,
+             AA_ERR_ALIGN, "%s: operands must be 16-byte aligned with 16-byte row strides", who);
+  AA_REQUIRE(grad_rows_dtype == AA_BF16 || grad_rows_dtype == AA_F16 || grad_rows_dtype == AA_F32, AA_ERR_DTYPE,
+             "%s: bad grad dtype", who);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "%s: bad mode", who);
+  AA_REQUIRE(n_rows < (int64_t(1) << 31) - k6::BM, AA_ERR_UNSUPPORTED, "%s: too many rows", who);
+  const k6::Schedule sc = k6::make_schedule(n_rows, V, true, -1);
+  k6::Params p{labels, n_rows, V, H, nullptr, AA_BF16, const_cast<float *>(stat_max), const_cast<float *>(stat_logsum),
+               mode == AA_MODE_FAITHFUL ? 1 : 0, nullptr, 1, 1, 1, 1, 1, 1, nullptr, const_cast<float *>(entropy)};
+  k6::GradParams gp{grad_rows, grad_rows_dtype, static_cast<__nv_bfloat16 *>(dlogits), ld, grad_entropy,
+                    grad_entropy_dtype};
+  if (entropy)
+    return k6::launch<k6::Epi::DLogits, true>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, p, gp,
+                                              sc, static_cast<cudaStream_t>(stream), who);
+  return k6::launch<k6::Epi::DLogits>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, p, gp, sc,
+                          static_cast<cudaStream_t>(stream), who);
 }
 
 extern "C" int aa_linear_dlogits(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
                                  const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
                                  const float *stat_max, const float *stat_logsum, const void *grad_rows,
                                  int grad_rows_dtype, void *dlogits, int64_t ld, int mode, void *stream) {
-  AA_REQUIRE(n_rows >= 0 && H > 0 && V > 0, AA_ERR_ARG, "aa_linear_dlogits: bad sizes");
-  if (n_rows == 0) return AA_OK;
-  AA_REQUIRE(hidden && weight && labels && stat_max && stat_logsum && grad_rows && dlogits, AA_ERR_ARG,
-             "aa_linear_dlogits: null pointer");
-  AA_REQUIRE(H % k6::BK == 0, AA_ERR_UNSUPPORTED, "aa_linear_dlogits: H=%d must be a multiple of %d", H, k6::BK);
-  const int all_tiles = (V + k6::BN - 1) / k6::BN;
-  AA_REQUIRE(ld >= static_cast<int64_t>(all_tiles) * k6::BN && ld % 8 == 0 && (reinterpret_cast<uintptr_t>(dlogits) & 15) == 0,
-             AA_ERR_ALIGN, "aa_linear_dlogits: ld must be >= ceil(V / 256) * 256, a multiple of 8, buffer 16-byte aligned");
-  AA_REQUIRE((reinterpret_cast<uintptr_t>(hidden) & 15) == 0 && (reinterpret_cast<uintptr_t>(weight) & 15) == 0 &&
-                 hidden_row_stride % 8 == 0 && weight_row_stride % 8 == 0 && hidden_row_stride >= H && weight_row_stride >= H,
-             AA_ERR_ALIGN, "aa_linear_dlogits: operands must be 16-byte aligned with 16-byte row strides");
-  AA_REQUIRE(grad_rows_dtype == AA_BF16 || grad_rows_dtype == AA_F16 || grad_rows_dtype == AA_F32, AA_ERR_DTYPE,
-             "aa_linear_dlogits: bad grad dtype");
-  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_linear_dlogits: bad mode");
-  AA_REQUIRE(n_rows < (int64_t(1) << 31) - k6::BM, AA_ERR_UNSUPPORTED, "aa_linear_dlogits: too many rows");
-  const k6::Schedule sc = k6::make_schedule(n_rows, V, true, -1);
-  k6::Params p{labels, n_rows, V, H, nullptr, AA_BF16, const_cast<float *>(stat_max), const_cast<float *>(stat_logsum),
-               mode == AA_MODE_FAITHFUL ? 1 : 0, nullptr, 1, 1, 1, 1, 1, 1, nullptr, nullptr};
-  k6::GradParams gp{grad_rows, grad_rows_dtype, static_cast<__nv_bfloat16 *>(dlogits), ld};
-  return k6::launch<k6::Epi::DLogits>(hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, p, gp, sc,
-                          static_cast<cudaStream_t>(stream), "aa_linear_dlogits");
+  return linear_dlogits("aa_linear_dlogits", hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride, labels,
+                        stat_max, stat_logsum, grad_rows, grad_rows_dtype, nullptr, nullptr, AA_F32, dlogits, ld, mode,
+                        stream);
+}
+
+extern "C" int aa_linear_dlogits_entropy(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
+                                         const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
+                                         const float *stat_max, const float *stat_logsum, const void *grad_rows,
+                                         int grad_rows_dtype, const float *entropy, const void *grad_entropy,
+                                         int grad_entropy_dtype, void *dlogits, int64_t ld, int mode, void *stream) {
+  AA_REQUIRE(n_rows == 0 || (entropy && grad_entropy), AA_ERR_ARG,
+             "aa_linear_dlogits_entropy: entropy and grad_entropy are required");
+  AA_REQUIRE(grad_entropy_dtype == AA_BF16 || grad_entropy_dtype == AA_F16 || grad_entropy_dtype == AA_F32, AA_ERR_DTYPE,
+             "aa_linear_dlogits_entropy: bad grad_entropy dtype");
+  return linear_dlogits("aa_linear_dlogits_entropy", hidden, n_rows, H, hidden_row_stride, weight, V, weight_row_stride,
+                        labels, stat_max, stat_logsum, grad_rows, grad_rows_dtype, n_rows ? entropy : nullptr,
+                        grad_entropy, grad_entropy_dtype, dlogits, ld, mode, stream);
 }

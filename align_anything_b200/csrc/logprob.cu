@@ -60,6 +60,11 @@ struct BwdParams {
   float zero;  // +0.0f supplied at run time (see f2_round_bf16 in common.cuh)
   const int64_t *extra_zero_rows;  // n_tile_rows == 0 only: tile rows to zero-fill after the scored rows
   int64_t n_extra;
+  // entropy-gradient kernels only (ENT = true): the forward's fp32 entropy and its upstream gradient, both indexed like
+  // grad_rows (grad_entropy in dtype grad_entropy_dtype); grad_scale multiplies g_H as it multiplies g
+  const float *entropy;
+  const void *grad_entropy;
+  int grad_entropy_dtype;
 };
 __host__ __device__ __forceinline__ int64_t bwd_work_rows(const BwdParams &p) {
   return p.n_tile_rows > 0 ? p.n_tile_rows : p.n_rows + p.n_extra;
@@ -493,7 +498,15 @@ struct __align__(16) RowRec {
   float m, logsum, g;
   int32_t y;       // label column; -1: out of range (no one-hot term); -2: zero-fill the row
 };
+// the entropy-gradient kernels' record: RowRec, then the row's entropy and its upstream gradient
+struct __align__(16) RowRecEnt {
+  RowRec r;
+  float H, gH;
+  int32_t pad[2];
+};
+static_assert(sizeof(RowRec) == 32 && sizeof(RowRecEnt) == 48, "records are read as 16-byte vectors");
 
+template <bool ENT = false>
 __global__ void bwd_row_prep_kernel(const BwdParams p, RowRec *__restrict__ rec) {
   const bool tile_mode = p.n_tile_rows > 0;
   const int64_t n_work = bwd_work_rows(p);
@@ -529,15 +542,25 @@ __global__ void bwd_row_prep_kernel(const BwdParams p, RowRec *__restrict__ rec)
     r.g_row = __ldg(p.seg_tile_row + seg) + j;
     scored = true;
   }
+  float H = 0.f, gH = 0.f;
   if (scored) {
     const int64_t flat = __ldg(p.map.seg_cum + seg) + j;
     float g = 1.f;
     if (p.grad_rows) g *= load_as_float(p.grad_rows, __ldg(p.map.seg_out_off + seg) + j, p.grad_rows_dtype);
     if (p.grad_seg) g *= __ldg(p.grad_seg + seg);
     if (p.grad_scale) g *= load_as_float(p.grad_scale, 0, p.grad_scale_dtype);
+    if constexpr (ENT) {
+      const int64_t o = __ldg(p.map.seg_out_off + seg) + j;
+      gH = load_as_float(p.grad_entropy, o, p.grad_entropy_dtype);
+      if (p.grad_scale) gH *= load_as_float(p.grad_scale, 0, p.grad_scale_dtype);
+      H = __ldg(p.entropy + o);
+    }
     const int64_t y = __ldg(p.labels + __ldg(p.map.seg_label_off + seg) + j);
-    if (p.use_ignore && y == p.ignore_index) g = 0.f;
-    if (g != 0.f) {  // g == 0 (masked / prompt / ignored rows): plain zero row
+    if (p.use_ignore && y == p.ignore_index) {
+      g = 0.f;
+      if constexpr (ENT) gH = 0.f;
+    }
+    if (g != 0.f || (ENT && gH != 0.f)) {  // g == 0 (masked / prompt / ignored rows): plain zero row
       r.x_off = __ldg(p.map.seg_logit_off + seg) + j * p.row_stride;
       r.m = __ldg(p.stat_max + flat);
       r.logsum = __ldg(p.stat_logsum + flat);
@@ -545,7 +568,10 @@ __global__ void bwd_row_prep_kernel(const BwdParams p, RowRec *__restrict__ rec)
       r.y = (y >= 0 && y < p.V) ? static_cast<int32_t>(y) : -1;
     }
   }
-  rec[slot] = r;
+  if constexpr (ENT)
+    reinterpret_cast<RowRecEnt *>(rec)[slot] = RowRecEnt{r, H, gH, {0, 0}};
+  else
+    rec[slot] = r;
 }
 
 // A pure copy with the one-CTA-per-row access structure of the LDG kernel above stays below what the copy
@@ -559,12 +585,14 @@ __global__ void bwd_row_prep_kernel(const BwdParams p, RowRec *__restrict__ rec)
 //   8 consumer warps: LDS.128 -> grad math (f32x2, Veltkamp rounding) -> STS.128 in place, one-hot label
 //                   patched in registers, fence.proxy.async, arrive(done).
 // Rows whose logits and gradient addresses disagree modulo 16 fall back to an element loop.
-template <typename T, int CONSUMERS, int STAGES, int UNROLL, int LAG, bool FAITHFUL>
+// ENT: the records are RowRecEnt and rows with g_H != 0 get the entropy correction (vec_grad_ent).
+template <typename T, int CONSUMERS, int STAGES, int UNROLL, int LAG, bool FAITHFUL, bool ENT = false>
 __global__ void __launch_bounds__(CONSUMERS + 32)
     logprob_bwd_tma_kernel(const T *__restrict__ logits, T *__restrict__ grad, int64_t grad_row_stride, int V,
                            const RowRec *__restrict__ rec, int64_t n_work, float zero) {
   constexpr int E = Traits<T>::kVec;
   constexpr int STAGE_VECS = CONSUMERS * UNROLL;
+  constexpr int kRecVecs = (ENT ? sizeof(RowRecEnt) : sizeof(RowRec)) / 16;
   static_assert(LAG >= 1 && LAG < STAGES, "LAG must leave at least one free stage");
   extern __shared__ __align__(128) uint8_t smem_raw[];
   uint4 *ring = reinterpret_cast<uint4 *>(smem_raw);
@@ -600,8 +628,9 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
       ++retired;
     };
     for (int64_t r = blockIdx.x; r < n_work; r += gridDim.x) {
-      const int4 r0 = __ldg(reinterpret_cast<const int4 *>(rec + r));
-      const int4 r1 = __ldg(reinterpret_cast<const int4 *>(rec + r) + 1);
+      const int4 *rv = reinterpret_cast<const int4 *>(rec) + r * kRecVecs;
+      const int4 r0 = __ldg(rv);
+      const int4 r1 = __ldg(rv + 1);
       const int64_t x_off = (static_cast<int64_t>(static_cast<uint32_t>(r0.y)) << 32) | static_cast<uint32_t>(r0.x);
       const int64_t g_row = (static_cast<int64_t>(static_cast<uint32_t>(r0.w)) << 32) | static_cast<uint32_t>(r0.z);
       const int y = r1.w;
@@ -648,10 +677,18 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
   // ------------------------------ consumer warps ------------------------------
   int64_t it = 0;
   for (int64_t r = blockIdx.x; r < n_work; r += gridDim.x) {
-    const int4 r0 = __ldg(reinterpret_cast<const int4 *>(rec + r));
-    const int4 r1 = __ldg(reinterpret_cast<const int4 *>(rec + r) + 1);
+    const int4 *rv = reinterpret_cast<const int4 *>(rec) + r * kRecVecs;
+    const int4 r0 = __ldg(rv);
+    const int4 r1 = __ldg(rv + 1);
     const int y = r1.w;
     if (y == -2) continue;
+    float H = 0.f, gH = 0.f;
+    if constexpr (ENT) {
+      const int4 r2 = __ldg(rv + 2);
+      H = __int_as_float(r2.x);
+      gH = __int_as_float(r2.y);
+    }
+    const bool ent = ENT && gH != 0.f;  // rows without an entropy gradient run the plain code
     const int64_t x_off = (static_cast<int64_t>(static_cast<uint32_t>(r0.y)) << 32) | static_cast<uint32_t>(r0.x);
     const int64_t g_row = (static_cast<int64_t>(static_cast<uint32_t>(r0.w)) << 32) | static_cast<uint32_t>(r0.z);
     const float m = __int_as_float(r1.x), logsum = __int_as_float(r1.y), g = __int_as_float(r1.z);
@@ -661,20 +698,24 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
     const float c_f32 = -lse * kLog2e;
     const float neg_g = FAITHFUL ? -g : -g * ex2_approx(fmaf(-lse, kLog2e, -c_f32));
     const GradConsts gk = make_grad_consts(m, logsum, c_f32, neg_g, zero);
+    // -g_H, with the F32 mode's offset residual folded in as for -g
+    const float ngh = !ENT ? 0.f : FAITHFUL ? -gH : -gH * ex2_approx(fmaf(-lse, kLog2e, -c_f32));
+    const EntConsts ek{f2_splat(H), f2_splat(ngh)};
+    // element c of the row; ENT = false is grad_of itself
+#define AA_K1B_ELEM(c)                                                                                        \
+  (ENT ? grad_of_ent<T, FAITHFUL>(Traits<T>::to_float(x[c]), m, logsum, c_f32, neg_g, g, (c) == y, ent, ngh, H) \
+       : grad_of<T, FAITHFUL>(Traits<T>::to_float(x[c]), m, logsum, c_f32, neg_g, g, (c) == y))
     if (((reinterpret_cast<uintptr_t>(x) ^ reinterpret_cast<uintptr_t>(g_out)) & 15) != 0) {
-      for (int e = tid; e < V; e += CONSUMERS)
-        g_out[e] = Traits<T>::from_float(grad_of<T, FAITHFUL>(Traits<T>::to_float(x[e]), m, logsum, c_f32, neg_g, g, e == y));
+      for (int e = tid; e < V; e += CONSUMERS) g_out[e] = Traits<T>::from_float(AA_K1B_ELEM(e));
       continue;
     }
     const int mis = static_cast<int>((reinterpret_cast<uintptr_t>(g_out) & 15) / sizeof(T));
     const int head = mis ? min(E - mis, V) : 0;
     const int nvec = (V - head) / E;
     const int tail0 = head + nvec * E;
-    if (tid < head)
-      g_out[tid] = Traits<T>::from_float(grad_of<T, FAITHFUL>(Traits<T>::to_float(x[tid]), m, logsum, c_f32, neg_g, g, tid == y));
-    if (tid < V - tail0)
-      g_out[tail0 + tid] = Traits<T>::from_float(
-          grad_of<T, FAITHFUL>(Traits<T>::to_float(x[tail0 + tid]), m, logsum, c_f32, neg_g, g, tail0 + tid == y));
+    if (tid < head) g_out[tid] = Traits<T>::from_float(AA_K1B_ELEM(tid));
+    if (tid < V - tail0) g_out[tail0 + tid] = Traits<T>::from_float(AA_K1B_ELEM(tail0 + tid));
+#undef AA_K1B_ELEM
     const int yv = (y >= head && y < tail0) ? (y - head) / E : -1;  // body vector holding the label column
     for (int v0 = 0; v0 < nvec; v0 += STAGE_VECS) {
       const int n = min(STAGE_VECS, nvec - v0);
@@ -686,8 +727,9 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
         const int k = tid + u * CONSUMERS;
         if (k < n) {
           const uint4 in = buf[k];
-          uint4 o = vec_grad<T, FAITHFUL>(in, gk);
-          if (v0 + k == yv) patch_label<T, FAITHFUL>(o, in, (y - head) - (v0 + k) * E, m, logsum, c_f32, neg_g, g);
+          uint4 o = ent ? vec_grad_ent<T, FAITHFUL, false>(in, gk, ek) : vec_grad<T, FAITHFUL>(in, gk);
+          if (v0 + k == yv)
+            patch_label<T, FAITHFUL, ENT>(o, in, (y - head) - (v0 + k) * E, m, logsum, c_f32, neg_g, g, ent, ngh, H);
           buf[k] = o;
         }
       }
@@ -783,17 +825,17 @@ static int launch_bwd_shape(const BwdParams &p, int per_sm, cudaStream_t st) {
 }
 
 // TMA-staged backward: 256 consumers, 4 stages x 8 KB, lag 3, 3 CTAs/SM.
-template <typename T>
+template <typename T, bool ENT = false>
 static int launch_bwd_tma(const BwdParams &p, int mode, RowRec *rec, cudaStream_t st) {
   constexpr int CONSUMERS = 256, STAGES = 4, UNROLL = 2, LAG = 3;
   const int64_t n_work = bwd_work_rows(p);
-  bwd_row_prep_kernel<<<static_cast<unsigned>((n_work + 255) / 256), 256, 0, st>>>(p, rec);
+  bwd_row_prep_kernel<ENT><<<static_cast<unsigned>((n_work + 255) / 256), 256, 0, st>>>(p, rec);
   int rc = check_launch("aa_logprob_bwd(prep)");
   if (rc) return rc;
   constexpr size_t smem = static_cast<size_t>(STAGES + 1) * CONSUMERS * UNROLL * 16 + STAGES * (8 + 8 + 8 + 4) + 16;
   const bool faithful = (mode == AA_MODE_FAITHFUL) && sizeof(T) == 2;
-  auto kf = logprob_bwd_tma_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, true>;
-  auto kn = logprob_bwd_tma_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, false>;
+  auto kf = logprob_bwd_tma_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, true, ENT>;
+  auto kn = logprob_bwd_tma_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, false, ENT>;
   static std::atomic<bool> configured{false};  // the attribute is idempotent: a race sets it twice, harmlessly
   if (!configured.load(std::memory_order_relaxed)) {
     cudaError_t e = cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -949,35 +991,48 @@ extern "C" int aa_zero_rows(void *tile, int dtype, int64_t row_stride, int32_t V
   return AA_OK;
 }
 
-extern "C" int aa_logprob_bwd(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
-                              const int64_t *labels, int64_t ignore_index, int32_t use_ignore,
-                              int32_t n_segments, int64_t n_rows,
-                              const int64_t *seg_logit_off, const int64_t *seg_label_off,
-                              const int64_t *seg_out_off, const int64_t *seg_cum,
-                              const int64_t *seg_tile_row, const float *stat_max,
-                              const float *stat_logsum, const void *grad_rows, int grad_rows_dtype,
-                              const float *grad_seg, const void *grad_scale, int grad_scale_dtype, void *grad_logits,
-                              int64_t grad_row_stride, int64_t n_tile_rows, const int64_t *extra_zero_rows,
-                              int64_t n_extra_zero_rows, void *row_scratch, int mode, void *stream) {
+// aa_logprob_bwd{,_entropy}: entropy == nullptr runs the plain kernels
+static int logprob_bwd(const char *who, const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                       const int64_t *labels, int64_t ignore_index, int32_t use_ignore, int32_t n_segments,
+                       int64_t n_rows, const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                       const int64_t *seg_out_off, const int64_t *seg_cum, const int64_t *seg_tile_row,
+                       const float *stat_max, const float *stat_logsum, const void *grad_rows, int grad_rows_dtype,
+                       const float *grad_seg, const void *grad_scale, int grad_scale_dtype, void *grad_logits,
+                       int64_t grad_row_stride, int64_t n_tile_rows, const int64_t *extra_zero_rows,
+                       int64_t n_extra_zero_rows, const float *entropy, const void *grad_entropy,
+                       int grad_entropy_dtype, void *row_scratch, int mode, void *stream) {
   AA_REQUIRE(V > 0 && n_segments >= 0 && n_rows >= 0 && n_tile_rows >= 0 && n_extra_zero_rows >= 0, AA_ERR_ARG,
-             "aa_logprob_bwd: bad sizes");
+             "%s: bad sizes", who);
   AA_REQUIRE(n_extra_zero_rows == 0 || (n_tile_rows == 0 && extra_zero_rows), AA_ERR_ARG,
-             "aa_logprob_bwd: extra_zero_rows needs n_tile_rows == 0 and a device row list");
+             "%s: extra_zero_rows needs n_tile_rows == 0 and a device row list", who);
   if (n_segments == 0) n_rows = 0;
   if (n_tile_rows == 0 && n_rows == 0 && n_extra_zero_rows == 0) return AA_OK;
-  AA_REQUIRE(grad_logits, AA_ERR_ARG, "aa_logprob_bwd: null grad_logits");
+  AA_REQUIRE(grad_logits, AA_ERR_ARG, "%s: null grad_logits", who);
   if (n_segments > 0)
     AA_REQUIRE(logits && labels && seg_logit_off && seg_label_off && seg_out_off && seg_cum &&
                    seg_tile_row && stat_max && stat_logsum,
-               AA_ERR_ARG, "aa_logprob_bwd: null pointer");
-  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_logprob_bwd: bad mode");
+               AA_ERR_ARG, "%s: null pointer", who);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "%s: bad mode", who);
   AA_REQUIRE(!grad_scale || grad_scale_dtype == AA_BF16 || grad_scale_dtype == AA_F16 || grad_scale_dtype == AA_F32,
-             AA_ERR_DTYPE, "aa_logprob_bwd: bad grad_scale dtype");
+             AA_ERR_DTYPE, "%s: bad grad_scale dtype", who);
   BwdParams p{logits, row_stride, V, labels, ignore_index, use_ignore,
               RowMap{seg_logit_off, seg_label_off, seg_out_off, seg_cum, n_segments},
               n_rows, seg_tile_row, stat_max, stat_logsum, grad_rows, grad_rows_dtype, grad_seg,
-              grad_scale, grad_scale_dtype, grad_logits, grad_row_stride, n_tile_rows, 0.0f, extra_zero_rows, n_extra_zero_rows};
+              grad_scale, grad_scale_dtype, grad_logits, grad_row_stride, n_tile_rows, 0.0f, extra_zero_rows, n_extra_zero_rows,
+              entropy, grad_entropy, grad_entropy_dtype};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (entropy) {  // the TMA-staged kernel only (the caller checked row_scratch)
+    AA_REQUIRE((reinterpret_cast<uintptr_t>(row_scratch) & 15) == 0, AA_ERR_ALIGN,
+               "%s: row_scratch must be 16-byte aligned", who);
+    RowRec *rec = static_cast<RowRec *>(row_scratch);
+    switch (logits_dtype) {
+      case AA_BF16: return launch_bwd_tma<__nv_bfloat16, true>(p, mode, rec, st);
+      case AA_F16: return launch_bwd_tma<__half, true>(p, mode, rec, st);
+      case AA_F32: return launch_bwd_tma<float, true>(p, mode, rec, st);
+    }
+    set_error("%s: unsupported logits dtype %d", who, logits_dtype);
+    return AA_ERR_DTYPE;
+  }
   if (row_scratch && bwd_variant() != 3) {  // TMA-staged backward (the default); tuning variant 3 takes the LDG kernel
     AA_REQUIRE((reinterpret_cast<uintptr_t>(row_scratch) & 15) == 0, AA_ERR_ALIGN,
                "aa_logprob_bwd: row_scratch must be 16-byte aligned");
@@ -993,6 +1048,46 @@ extern "C" int aa_logprob_bwd(const void *logits, int logits_dtype, int64_t row_
     case AA_F16: return launch_bwd<__half>(p, mode, st);
     case AA_F32: return launch_bwd<float>(p, mode, st);
   }
-  set_error("aa_logprob_bwd: unsupported logits dtype %d", logits_dtype);
+  set_error("%s: unsupported logits dtype %d", who, logits_dtype);
   return AA_ERR_DTYPE;
+}
+
+extern "C" int aa_logprob_bwd(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                              const int64_t *labels, int64_t ignore_index, int32_t use_ignore,
+                              int32_t n_segments, int64_t n_rows,
+                              const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                              const int64_t *seg_out_off, const int64_t *seg_cum,
+                              const int64_t *seg_tile_row, const float *stat_max,
+                              const float *stat_logsum, const void *grad_rows, int grad_rows_dtype,
+                              const float *grad_seg, const void *grad_scale, int grad_scale_dtype, void *grad_logits,
+                              int64_t grad_row_stride, int64_t n_tile_rows, const int64_t *extra_zero_rows,
+                              int64_t n_extra_zero_rows, void *row_scratch, int mode, void *stream) {
+  return logprob_bwd("aa_logprob_bwd", logits, logits_dtype, row_stride, V, labels, ignore_index, use_ignore, n_segments,
+                     n_rows, seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row, stat_max, stat_logsum,
+                     grad_rows, grad_rows_dtype, grad_seg, grad_scale, grad_scale_dtype, grad_logits, grad_row_stride,
+                     n_tile_rows, extra_zero_rows, n_extra_zero_rows, nullptr, nullptr, AA_F32, row_scratch, mode,
+                     stream);
+}
+
+extern "C" int aa_logprob_bwd_entropy(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                      const int64_t *labels, int64_t ignore_index, int32_t use_ignore,
+                                      int32_t n_segments, int64_t n_rows,
+                                      const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                                      const int64_t *seg_out_off, const int64_t *seg_cum,
+                                      const int64_t *seg_tile_row, const float *stat_max,
+                                      const float *stat_logsum, const void *grad_rows, int grad_rows_dtype,
+                                      const float *grad_seg, const void *grad_scale, int grad_scale_dtype,
+                                      const float *entropy, const void *grad_entropy, int grad_entropy_dtype,
+                                      void *grad_logits, int64_t grad_row_stride, int64_t n_tile_rows,
+                                      const int64_t *extra_zero_rows, int64_t n_extra_zero_rows, void *row_scratch,
+                                      int mode, void *stream) {
+  AA_REQUIRE(entropy && grad_entropy && row_scratch, AA_ERR_ARG,
+             "aa_logprob_bwd_entropy: entropy, grad_entropy and row_scratch (48 bytes per work row) are required");
+  AA_REQUIRE(grad_entropy_dtype == AA_BF16 || grad_entropy_dtype == AA_F16 || grad_entropy_dtype == AA_F32,
+             AA_ERR_DTYPE, "aa_logprob_bwd_entropy: bad grad_entropy dtype");
+  return logprob_bwd("aa_logprob_bwd_entropy", logits, logits_dtype, row_stride, V, labels, ignore_index, use_ignore,
+                     n_segments, n_rows, seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row, stat_max,
+                     stat_logsum, grad_rows, grad_rows_dtype, grad_seg, grad_scale, grad_scale_dtype, grad_logits,
+                     grad_row_stride, n_tile_rows, extra_zero_rows, n_extra_zero_rows, entropy, grad_entropy,
+                     grad_entropy_dtype, row_scratch, mode, stream);
 }

@@ -68,6 +68,11 @@ struct FusedActorParams {
   const int32_t *row_end;
   const float *total;
   float *entropy;  // ENT kernels: fp32 entropy of every scored row at its log-prob's position (phase A)
+  // EGRAD kernels (entropy bonus, loss - ent_coeff * mean entropy): the row's g_H = d loss / d H is
+  // kind 0: ent_seg[segment] (= -ent_coeff / (n_seg * mask count), the masked mean's coefficient, written by the prep
+  // kernel) for masked-in tokens; kind 2: -ent_coeff * g_rs (= -ent_coeff / counted tokens) for counted tokens
+  float ent_coeff;
+  float *ent_seg;
 };
 
 // One record per gradient-tile row, in the order the persistent kernel walks them.  The scored rows are bound by
@@ -87,6 +92,7 @@ struct __align__(16) FusedRec {
 static_assert(sizeof(FusedRec) == 48, "FusedRec is read as three 16-byte vectors");
 
 // grid (ceil(seq / 256), n_seg): block (c, seg) resolves tile rows [256 c, 256 c + 256) of sample `seg`.
+template <bool EGRAD = false>
 __global__ void __launch_bounds__(256) fused_actor_prep_kernel(const FusedActorParams p, FusedRec *__restrict__ rec) {
   __shared__ float scratch[33];
   const int seg = blockIdx.y, tid = threadIdx.x;
@@ -95,6 +101,9 @@ __global__ void __launch_bounds__(256) fused_actor_prep_kernel(const FusedActorP
   if (p.kind == 0) {
     for (int t = tid; t < p.W; t += 256) cnt += p.mask[seg * p.mask_stride + t] ? 1.f : 0.f;
     cnt = block_sum<256>(cnt, scratch);
+    if constexpr (EGRAD) {
+      if (blockIdx.x == 0 && tid == 0) p.ent_seg[seg] = -p.ent_coeff / (static_cast<float>(p.map.n_seg) * cnt);
+    }
   }
   if (k >= p.seq) return;
   const int64_t work = static_cast<int64_t>(seg) * p.seq + k;
@@ -192,7 +201,8 @@ __device__ __forceinline__ uint4 vec_grad_pk(const uint4 &v, const GradConsts &k
   }
 }
 
-template <typename T, int CONSUMERS, int STAGES, int UNROLL, int LAG, bool FAITHFUL, bool ENT = false>
+// EGRAD (implies ENT): phase B adds the entropy's gradient (logprob_math.cuh, vec_grad_ent) to rows with g_H != 0.
+template <typename T, int CONSUMERS, int STAGES, int UNROLL, int LAG, bool FAITHFUL, bool ENT = false, bool EGRAD = false>
 __global__ void __launch_bounds__(CONSUMERS + 32)
     logprob_actor_fused_kernel(const FusedActorParams p, const FusedRec *__restrict__ rec, int64_t n_work) {
   constexpr int E = Traits<T>::kVec;
@@ -206,7 +216,8 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
   uint64_t *done = full + STAGES;
   uint64_t *st_dst = done + STAGES;  // destination of the chunk held by each stage (phase B), 0 for phase A
   uint32_t *st_bytes = reinterpret_cast<uint32_t *>(st_dst + STAGES);
-  __shared__ float sh_m[32], sh_s[32], sh_b[4];
+  static_assert(ENT || !EGRAD, "the entropy gradient needs the entropy");
+  __shared__ float sh_m[32], sh_s[32], sh_b[EGRAD ? 8 : 4];
   __shared__ float sh_t[ENT ? 32 : 1];
   const int tid = threadIdx.x;
   const int V = p.V;
@@ -426,6 +437,12 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
         sh_b[0] = m;
         sh_b[1] = logsum;
         sh_b[2] = g;
+        if constexpr (EGRAD) {
+          float gH = 0.f;
+          if (on) gH = (p.kind == 0) ? __ldg(p.ent_seg + g_row / p.seq) : -p.ent_coeff * g_rs;
+          sh_b[3] = entropy_of(logsum, s, t);
+          sh_b[4] = gH;
+        }
       }
     }
     asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
@@ -436,26 +453,31 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
     }
     m = sh_b[0];
     const float logsum = sh_b[1], g = sh_b[2];
+    float H = 0.f, gH = 0.f;
+    if constexpr (EGRAD) {
+      H = sh_b[3];
+      gH = sh_b[4];
+    }
+    const bool ent = EGRAD && gH != 0.f;  // rows without an entropy gradient run the plain code
 
     // ---- phase B: g * (onehot - softmax), the row comes from L2 ----
     const float lse = m + logsum;
     const float c_f32 = -lse * kLog2e;
     const float neg_g = FAITHFUL ? -g : -g * ex2_approx(fmaf(-lse, kLog2e, -c_f32));
     const GradConsts gk = make_grad_consts(m, logsum, c_f32, neg_g, p.zero);
-    const bool dead = (g == 0.f);  // clipped token: 0 * softmax, written as +0 like K1b's zero rows
+    const float ngh = !EGRAD ? 0.f : FAITHFUL ? -gH : -gH * ex2_approx(fmaf(-lse, kLog2e, -c_f32));
+    const EntConsts ek{f2_splat(H), f2_splat(ngh)};
+    const bool dead = (g == 0.f) && !ent;  // clipped token: 0 * softmax, written as +0 like K1b's zero rows
+#define AA_K1F_ELEM(c)                                                                                        \
+  (EGRAD ? grad_of_ent<T, FAITHFUL>(Traits<T>::to_float(x[c]), m, logsum, c_f32, neg_g, g, (c) == y, ent, ngh, H) \
+         : grad_of<T, FAITHFUL>(Traits<T>::to_float(x[c]), m, logsum, c_f32, neg_g, g, (c) == y))
     if (!same_phase) {
-      for (int e = tid; e < V; e += CONSUMERS)
-        g_out[e] = Traits<T>::from_float(
-            dead ? 0.f : grad_of<T, FAITHFUL>(Traits<T>::to_float(x[e]), m, logsum, c_f32, neg_g, g, e == y));
+      for (int e = tid; e < V; e += CONSUMERS) g_out[e] = Traits<T>::from_float(dead ? 0.f : AA_K1F_ELEM(e));
       continue;
     }
-    if (tid < head)
-      g_out[tid] = Traits<T>::from_float(
-          dead ? 0.f : grad_of<T, FAITHFUL>(Traits<T>::to_float(x[tid]), m, logsum, c_f32, neg_g, g, tid == y));
-    if (tid < V - tail0)
-      g_out[tail0 + tid] = Traits<T>::from_float(
-          dead ? 0.f
-               : grad_of<T, FAITHFUL>(Traits<T>::to_float(x[tail0 + tid]), m, logsum, c_f32, neg_g, g, tail0 + tid == y));
+    if (tid < head) g_out[tid] = Traits<T>::from_float(dead ? 0.f : AA_K1F_ELEM(tid));
+    if (tid < V - tail0) g_out[tail0 + tid] = Traits<T>::from_float(dead ? 0.f : AA_K1F_ELEM(tail0 + tid));
+#undef AA_K1F_ELEM
     const int yv = (y >= head && y < tail0) ? (y - head) / E : -1;  // body vector holding the label column
     for (int v0 = 0; v0 < nvec; v0 += STAGE_VECS) {
       const int n = min(STAGE_VECS, nvec - v0);
@@ -470,8 +492,9 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
             buf[k] = make_uint4(0, 0, 0, 0);
           } else {
             const uint4 in = buf[k];
-            uint4 o = vec_grad_pk<T, FAITHFUL>(in, gk);
-            if (v0 + k == yv) patch_label<T, FAITHFUL>(o, in, (y - head) - (v0 + k) * E, m, logsum, c_f32, neg_g, g);
+            uint4 o = ent ? vec_grad_ent<T, FAITHFUL, true>(in, gk, ek) : vec_grad_pk<T, FAITHFUL>(in, gk);
+            if (v0 + k == yv)
+              patch_label<T, FAITHFUL, EGRAD>(o, in, (y - head) - (v0 + k) * E, m, logsum, c_f32, neg_g, g, ent, ngh, H);
             buf[k] = o;
           }
         }
@@ -539,13 +562,13 @@ __global__ void __launch_bounds__(256) scale_tile_kernel(T *__restrict__ tile, i
 // two passes, inside the 50 MB L2, so the second pass is an L2 hit; with two rows in flight per SM part of it misses.
 // The kernel is bound by the MUFU / conversion pipe and instruction issue (two exp per logit + the bf16 pack) rather
 // than by HBM.
-template <typename T, bool ENT = false>
+template <typename T, bool ENT = false, bool EGRAD = false>
 static int launch_fused_kernel(const FusedActorParams &p, int mode, FusedRec *rec, int64_t n_work, cudaStream_t st) {
   constexpr int CONSUMERS = 992, STAGES = 6, UNROLL = 2, LAG = 4;
   constexpr size_t smem = static_cast<size_t>(STAGES + 1) * CONSUMERS * UNROLL * 16 + STAGES * (8 + 8 + 8 + 4) + 16;
   const bool faithful = (mode == AA_MODE_FAITHFUL) && sizeof(T) == 2;
-  auto kf = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, true, ENT>;
-  auto kn = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, false, ENT>;
+  auto kf = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, true, ENT, EGRAD>;
+  auto kn = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, false, ENT, EGRAD>;
   static std::atomic<bool> configured{false};  // the attribute is idempotent: a race sets it twice, harmlessly
   if (!configured.load(std::memory_order_relaxed)) {
     cudaError_t e = cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -561,7 +584,7 @@ static int launch_fused_kernel(const FusedActorParams &p, int mode, FusedRec *re
   FusedActorParams q = p;
   q.interleave = static_cast<int>(grid);
   const dim3 pgrid((q.seq + 255) / 256, q.map.n_seg);
-  fused_actor_prep_kernel<<<pgrid, 256, 0, st>>>(q, rec);
+  fused_actor_prep_kernel<EGRAD><<<pgrid, 256, 0, st>>>(q, rec);
   int rc = check_launch("aa_logprob_actor_fused(prep)");
   if (rc) return rc;
   if (faithful)
@@ -571,8 +594,17 @@ static int launch_fused_kernel(const FusedActorParams &p, int mode, FusedRec *re
   return check_launch("aa_logprob_actor_fused");
 }
 
+// egrad: the entropy-bonus kernels (p.entropy set)
 static int launch_fused(const FusedActorParams &p, int logits_dtype, int mode, FusedRec *rec, int64_t n_work,
-                        cudaStream_t st) {
+                        cudaStream_t st, bool egrad = false) {
+  if (egrad) {
+    switch (logits_dtype) {
+      case AA_BF16: return launch_fused_kernel<__nv_bfloat16, true, true>(p, mode, rec, n_work, st);
+      case AA_F16: return launch_fused_kernel<__half, true, true>(p, mode, rec, n_work, st);
+      case AA_F32: return launch_fused_kernel<float, true, true>(p, mode, rec, n_work, st);
+    }
+    return AA_ERR_DTYPE;
+  }
   if (p.entropy) {
     switch (logits_dtype) {
       case AA_BF16: return launch_fused_kernel<__nv_bfloat16, true>(p, mode, rec, n_work, st);
@@ -620,28 +652,30 @@ static inline int promote_dt(int a, int b) { return (a == b) ? a : AA_F32; }
 
 using namespace aa;
 
-extern "C" int aa_logprob_actor_fused(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
-                                      const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
-                                      const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
-                                      const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
-                                      float *stat_max, float *stat_logsum, const void *old_log_probs, int64_t old_stride,
-                                      const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
-                                      int64_t mask_stride, int32_t W, float clip_range_ratio, int mode, void *grad_logits,
-                                      int64_t grad_row_stride, void *row_scratch, int32_t *status, void *stream) {
+// aa_logprob_actor_fused{,_entropy}: entropy == nullptr runs the plain kernels
+static int logprob_actor_fused(const char *who, float *entropy, float entropy_coeff, const void *logits, int logits_dtype,
+                               int64_t row_stride, int32_t V, const int64_t *labels, int32_t n_segments,
+                               const int64_t *seg_logit_off, const int64_t *seg_label_off, const int64_t *seg_out_off,
+                               const int64_t *seg_cum, const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs,
+                               int lp_dtype, float *stat_max, float *stat_logsum, const void *old_log_probs,
+                               int64_t old_stride, const void *advantages, int64_t adv_stride, int adv_dtype,
+                               const uint8_t *mask, int64_t mask_stride, int32_t W, float clip_range_ratio, int mode,
+                               void *grad_logits, int64_t grad_row_stride, void *row_scratch, int32_t *status,
+                               void *stream) {
   AA_REQUIRE(V > 0 && n_segments > 0 && W > 0 && n_tile_rows > 0 && n_tile_rows % n_segments == 0, AA_ERR_ARG,
-             "aa_logprob_actor_fused: bad sizes (the gradient tile holds n_tile_rows / n_segments rows per sample)");
+             "%s: bad sizes (the gradient tile holds n_tile_rows / n_segments rows per sample)", who);
   AA_REQUIRE(logits && labels && seg_logit_off && seg_label_off && seg_out_off && seg_cum && seg_tile_row && log_probs &&
                  old_log_probs && advantages && mask && grad_logits && row_scratch,
-             AA_ERR_ARG, "aa_logprob_actor_fused: null pointer");
+             AA_ERR_ARG, "%s: null pointer", who);
   AA_REQUIRE((stat_max == nullptr) == (stat_logsum == nullptr), AA_ERR_ARG,
-             "aa_logprob_actor_fused: stat_max and stat_logsum go together");
+             "%s: stat_max and stat_logsum go together", who);
   AA_REQUIRE(fdtype_ok(logits_dtype) && fdtype_ok(lp_dtype) && fdtype_ok(adv_dtype), AA_ERR_DTYPE,
-             "aa_logprob_actor_fused: bad dtype");
-  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_logprob_actor_fused: bad mode");
+             "%s: bad dtype", who);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "%s: bad mode", who);
   AA_REQUIRE((reinterpret_cast<uintptr_t>(row_scratch) & 15) == 0, AA_ERR_ALIGN,
-             "aa_logprob_actor_fused: row_scratch must be 16-byte aligned");
+             "%s: row_scratch must be 16-byte aligned", who);
   AA_REQUIRE(n_tile_rows / n_segments < (1ll << 31) && n_tile_rows < (1ll << 31), AA_ERR_ARG,
-             "aa_logprob_actor_fused: tile too large");
+             "%s: tile too large", who);
   const bool f = (mode == AA_MODE_FAITHFUL);
   FusedActorParams p = fused_params(logits, row_stride, V, labels, n_segments, seg_logit_off, seg_label_off, seg_out_off,
                                     seg_cum, seg_tile_row, n_tile_rows, log_probs, lp_dtype, grad_logits,
@@ -660,8 +694,47 @@ extern "C" int aa_logprob_actor_fused(const void *logits, int logits_dtype, int6
   p.clip = clip_range_ratio;
   p.rx = f ? lp_dtype : AA_F32;
   p.rp = f ? promote_dt(lp_dtype, adv_dtype) : AA_F32;
-  return launch_fused(p, logits_dtype, mode, static_cast<FusedRec *>(row_scratch), n_tile_rows,
-                      static_cast<cudaStream_t>(stream));
+  FusedRec *rec = static_cast<FusedRec *>(row_scratch);
+  if (entropy) {
+    p.entropy = entropy;
+    p.ent_coeff = entropy_coeff;
+    p.ent_seg = reinterpret_cast<float *>(rec + n_tile_rows);
+  }
+  return launch_fused(p, logits_dtype, mode, rec, n_tile_rows, static_cast<cudaStream_t>(stream), entropy != nullptr);
+}
+
+extern "C" int aa_logprob_actor_fused(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                      const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                      const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
+                                      const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
+                                      float *stat_max, float *stat_logsum, const void *old_log_probs, int64_t old_stride,
+                                      const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
+                                      int64_t mask_stride, int32_t W, float clip_range_ratio, int mode, void *grad_logits,
+                                      int64_t grad_row_stride, void *row_scratch, int32_t *status, void *stream) {
+  return logprob_actor_fused("aa_logprob_actor_fused", nullptr, 0.f, logits, logits_dtype, row_stride, V, labels, n_segments, seg_logit_off,
+                             seg_label_off, seg_out_off, seg_cum, seg_tile_row, n_tile_rows, log_probs, lp_dtype,
+                             stat_max, stat_logsum, old_log_probs, old_stride, advantages, adv_stride, adv_dtype, mask,
+                             mask_stride, W, clip_range_ratio, mode, grad_logits, grad_row_stride, row_scratch, status,
+                             stream);
+}
+
+extern "C" int aa_logprob_actor_fused_entropy(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                              const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                              const int64_t *seg_label_off, const int64_t *seg_out_off,
+                                              const int64_t *seg_cum, const int64_t *seg_tile_row, int64_t n_tile_rows,
+                                              void *log_probs, int lp_dtype, float *stat_max, float *stat_logsum,
+                                              const void *old_log_probs, int64_t old_stride, const void *advantages,
+                                              int64_t adv_stride, int adv_dtype, const uint8_t *mask,
+                                              int64_t mask_stride, int32_t W, float clip_range_ratio, int mode,
+                                              void *grad_logits, int64_t grad_row_stride, void *row_scratch,
+                                              int32_t *status, float entropy_coeff, float *entropy, void *stream) {
+  AA_REQUIRE(entropy, AA_ERR_ARG, "aa_logprob_actor_fused_entropy: null entropy");
+  AA_REQUIRE(entropy_coeff == entropy_coeff, AA_ERR_ARG, "aa_logprob_actor_fused_entropy: entropy_coeff is NaN");
+  return logprob_actor_fused("aa_logprob_actor_fused_entropy", entropy, entropy_coeff, logits, logits_dtype, row_stride, V, labels, n_segments,
+                             seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row, n_tile_rows, log_probs,
+                             lp_dtype, stat_max, stat_logsum, old_log_probs, old_stride, advantages, adv_stride,
+                             adv_dtype, mask, mask_stride, W, clip_range_ratio, mode, grad_logits, grad_row_stride,
+                             row_scratch, status, stream);
 }
 
 extern "C" int aa_logprob_ce_fused(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
@@ -693,8 +766,8 @@ extern "C" int aa_logprob_ce_fused(const void *logits, int logits_dtype, int64_t
 }
 
 // aa_logprob_grpo_fused{,_entropy}: entropy == nullptr runs the plain kernels
-static int logprob_grpo_fused(float *entropy, const char *who, const void *logits, int logits_dtype, int64_t row_stride,
-                                    int32_t V,
+static int logprob_grpo_fused(float *entropy, float entropy_coeff, bool egrad, const char *who, const void *logits,
+                              int logits_dtype, int64_t row_stride, int32_t V,
                                     const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
                                     const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
                                     const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
@@ -730,7 +803,8 @@ static int logprob_grpo_fused(float *entropy, const char *who, const void *logit
   p.row_end = row_end;
   p.total = total;
   p.entropy = entropy;
-  return launch_fused(p, logits_dtype, mode, static_cast<FusedRec *>(row_scratch), n_tile_rows, st);
+  p.ent_coeff = entropy_coeff;
+  return launch_fused(p, logits_dtype, mode, static_cast<FusedRec *>(row_scratch), n_tile_rows, st, egrad);
 }
 
 extern "C" int aa_logprob_grpo_fused(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
@@ -741,7 +815,7 @@ extern "C" int aa_logprob_grpo_fused(const void *logits, int logits_dtype, int64
                                     const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t K,
                                     float beta, int mode, void *grad_logits, int64_t grad_row_stride, void *row_scratch,
                                     int32_t *row_end, float *total, uint32_t *counter, int32_t *status, void *stream) {
-  return logprob_grpo_fused(nullptr, "aa_logprob_grpo_fused", logits, logits_dtype, row_stride, V, labels, n_segments,
+  return logprob_grpo_fused(nullptr, 0.f, false, "aa_logprob_grpo_fused", logits, logits_dtype, row_stride, V, labels, n_segments,
                             seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row, n_tile_rows, log_probs,
                             lp_dtype, ref_log_probs, ref_stride, advantages, completion_tokens, tok_stride, eos_id, K, beta,
                             mode, grad_logits, grad_row_stride, row_scratch, row_end, total, counter, status, stream);
@@ -757,11 +831,31 @@ extern "C" int aa_logprob_grpo_fused_entropy(const void *logits, int logits_dtyp
                                             int64_t grad_row_stride, void *row_scratch, int32_t *row_end, float *total,
                                             uint32_t *counter, int32_t *status, float *entropy, void *stream) {
   AA_REQUIRE(entropy, AA_ERR_ARG, "aa_logprob_grpo_fused_entropy: null entropy");
-  return logprob_grpo_fused(entropy, "aa_logprob_grpo_fused_entropy", logits, logits_dtype, row_stride, V, labels,
-                            n_segments, seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row, n_tile_rows,
-                            log_probs, lp_dtype, ref_log_probs, ref_stride, advantages, completion_tokens, tok_stride,
-                            eos_id, K, beta, mode, grad_logits, grad_row_stride, row_scratch, row_end, total, counter,
-                            status, stream);
+  return logprob_grpo_fused(entropy, 0.f, false, "aa_logprob_grpo_fused_entropy", logits, logits_dtype, row_stride, V,
+                            labels, n_segments, seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row,
+                            n_tile_rows, log_probs, lp_dtype, ref_log_probs, ref_stride, advantages, completion_tokens,
+                            tok_stride, eos_id, K, beta, mode, grad_logits, grad_row_stride, row_scratch, row_end, total,
+                            counter, status, stream);
+}
+
+extern "C" int aa_logprob_grpo_fused_entropy_grad(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                                 const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                                 const int64_t *seg_label_off, const int64_t *seg_out_off,
+                                                 const int64_t *seg_cum, const int64_t *seg_tile_row, int64_t n_tile_rows,
+                                                 void *log_probs, int lp_dtype, const void *ref_log_probs,
+                                                 int64_t ref_stride, const float *advantages,
+                                                 const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id,
+                                                 int32_t K, float beta, int mode, void *grad_logits,
+                                                 int64_t grad_row_stride, void *row_scratch, int32_t *row_end,
+                                                 float *total, uint32_t *counter, int32_t *status, float *entropy,
+                                                 float entropy_coeff, void *stream) {
+  AA_REQUIRE(entropy, AA_ERR_ARG, "aa_logprob_grpo_fused_entropy_grad: null entropy");
+  AA_REQUIRE(entropy_coeff == entropy_coeff, AA_ERR_ARG, "aa_logprob_grpo_fused_entropy_grad: entropy_coeff is NaN");
+  return logprob_grpo_fused(entropy, entropy_coeff, true, "aa_logprob_grpo_fused_entropy_grad", logits, logits_dtype,
+                            row_stride, V, labels, n_segments, seg_logit_off, seg_label_off, seg_out_off, seg_cum,
+                            seg_tile_row, n_tile_rows, log_probs, lp_dtype, ref_log_probs, ref_stride, advantages,
+                            completion_tokens, tok_stride, eos_id, K, beta, mode, grad_logits, grad_row_stride,
+                            row_scratch, row_end, total, counter, status, stream);
 }
 
 extern "C" int aa_scale_tile(void *tile, int dtype, int64_t n, const void *scale, int scale_dtype, void *stream) {

@@ -363,6 +363,92 @@ __device__ __forceinline__ float grad_of(float x, float m, float logsum, float c
   return neg_g * pr;
 }
 
+// ---- entropy bonus: the entropy's gradient added to the gradient tile ---------------------------------------
+// With l_k = x_k - m - logsum and p_k = e^{l_k}, dH/dx_k = -p_k (l_k + H), so a row whose entropy has the upstream
+// gradient g_H gets  tile_k = [log-prob term] - g_H p_k (l_k + H).  p_k and l_k are the ones the log-prob term uses
+// (FAITHFUL: the rounded log-softmax), the correction is fp32 and added before the tile's one rounding.  A -inf logit's
+// l_k is clamped as in the entropy forward, so its term is e * finite = 0 before the coefficient multiplies it.
+// Callers take these forms only for rows with g_H != 0: every other row runs the plain code and keeps its bits.
+struct EntConsts {
+  f32x2 h2, ngh2;  // H, -g_H (times the offset residual in F32 mode, like GradConsts::ng2)
+};
+
+template <typename T, bool FAITHFUL, bool PK>
+__device__ __forceinline__ f32x2 pair_grad_ent(f32x2 x2, const GradConsts &k, const EntConsts &ek) {
+  f32x2 lp = f2_sub(f2_sub(x2, k.m2), k.ls2), t;
+  if (FAITHFUL) {
+    if constexpr (PK && sizeof(T) == 2) {  // vec_grad_pk's rounding (logprob_fused.cu): one F2FP per pair, -inf stays -inf
+      float lo, hi;
+      f2_unpack(lp, lo, hi);
+      unpack2<T>(pack2<T>(lo, hi), lo, hi);
+      lp = f2_pack(lo, hi);
+    } else {
+      lp = (Traits<T>::kCode == AA_BF16) ? f2_round_bf16(lp, k.zero2) : f2_round_f16(lp, k.zero2);
+    }
+    t = f2_mul(lp, f2_splat(kLog2e));
+  } else {
+    t = f2_fma(x2, f2_splat(kLog2e), k.c2);
+  }
+  const f32x2 e = f2_ex2(t);
+  const f32x2 d = f2_add(make_float2(fmaxf(lp.x, -3.0e38f), fmaxf(lp.y, -3.0e38f)), ek.h2);
+  return f2_fma(f2_mul(e, d), ek.ngh2, f2_mul(e, k.ng2));
+}
+
+template <typename T, bool FAITHFUL, bool PK>
+__device__ __forceinline__ uint4 vec_grad_ent(const uint4 &v, const GradConsts &k, const EntConsts &ek) {
+  if constexpr (sizeof(T) == 4) {
+    float a, b, c, d;
+    f2_unpack(pair_grad_ent<T, FAITHFUL, PK>(f2_pack(__uint_as_float(v.x), __uint_as_float(v.y)), k, ek), a, b);
+    f2_unpack(pair_grad_ent<T, FAITHFUL, PK>(f2_pack(__uint_as_float(v.z), __uint_as_float(v.w)), k, ek), c, d);
+    return make_uint4(__float_as_uint(a), __float_as_uint(b), __float_as_uint(c), __float_as_uint(d));
+  } else {
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      uint32_t wi = w[i];
+      if (FAITHFUL && !PK) {  // vec_grad's clamp: the Veltkamp split must not see -inf
+        if constexpr (Traits<T>::kCode == AA_BF16) {
+          const __nv_bfloat162 lim = __float2bfloat162_rn(-1e30f);
+          __nv_bfloat162 h = __hmax2(*reinterpret_cast<__nv_bfloat162 *>(&wi), lim);
+          wi = *reinterpret_cast<uint32_t *>(&h);
+        } else {
+          const __half2 lim = __float2half2_rn(-65504.f);
+          __half2 h = __hmax2(*reinterpret_cast<__half2 *>(&wi), lim);
+          wi = *reinterpret_cast<uint32_t *>(&h);
+        }
+      }
+      float lo, hi;
+      unpack2<T>(wi, lo, hi);
+      f2_unpack(pair_grad_ent<T, FAITHFUL, PK>(f2_pack(lo, hi), k, ek), lo, hi);
+      o[i] = pack2<T>(lo, hi);
+    }
+    return make_uint4(o[0], o[1], o[2], o[3]);
+  }
+}
+
+// the correction for one element (head / tail peel, element loops, the label column)
+template <typename T, bool FAITHFUL>
+__device__ __forceinline__ float ent_corr(float x, float m, float logsum, float c_f32, float ngh, float H) {
+  float lp = (x - m) - logsum, e;
+  if (FAITHFUL) {
+    lp = Traits<T>::round(lp);
+    e = ex2_approx(lp * kLog2e);
+  } else {
+    e = ex2_approx(fmaf(x, kLog2e, c_f32));
+  }
+  return (e * (fmaxf(lp, -3.0e38f) + H)) * ngh;
+}
+
+// grad_of, plus the entropy correction when `ent` (a row with g_H != 0)
+template <typename T, bool FAITHFUL>
+__device__ __forceinline__ float grad_of_ent(float x, float m, float logsum, float c_f32, float neg_g, float g,
+                                             bool is_label, bool ent, float ngh, float H) {
+  float v = grad_of<T, FAITHFUL>(x, m, logsum, c_f32, neg_g, g, is_label);
+  if (ent) v += ent_corr<T, FAITHFUL>(x, m, logsum, c_f32, ngh, H);
+  return v;
+}
+
 __device__ __forceinline__ uint32_t get_word(const uint4 &v, int i) {
   return i == 0 ? v.x : (i == 1 ? v.y : (i == 2 ? v.z : v.w));
 }
@@ -372,18 +458,22 @@ __device__ __forceinline__ void set_word(uint4 &v, int i, uint32_t w) {
 
 // Rewrite element k of the output vector with the one-hot (label) gradient; register-only
 // (no dynamically indexed local arrays).
-template <typename T, bool FAITHFUL>
+// ENT: the entropy correction is added when `ent` (see grad_of_ent); the ENT = false form is the plain code.
+template <typename T, bool FAITHFUL, bool ENT = false>
 __device__ __forceinline__ void patch_label(uint4 &o, const uint4 &in, int k, float m, float logsum, float c_f32,
-                                            float neg_g, float g) {
+                                            float neg_g, float g, bool ent = false, float ngh = 0.f, float H = 0.f) {
   if constexpr (sizeof(T) == 4) {
     const float x = __uint_as_float(get_word(in, k));
-    set_word(o, k, __float_as_uint(grad_of<T, FAITHFUL>(x, m, logsum, c_f32, neg_g, g, true)));
+    const float gv = ENT ? grad_of_ent<T, FAITHFUL>(x, m, logsum, c_f32, neg_g, g, true, ent, ngh, H)
+                         : grad_of<T, FAITHFUL>(x, m, logsum, c_f32, neg_g, g, true);
+    set_word(o, k, __float_as_uint(gv));
   } else {
     const int w = k >> 1;
     const bool hi_half = (k & 1) != 0;
     float lo, hi;
     unpack2<T>(get_word(in, w), lo, hi);
-    const float gv = grad_of<T, FAITHFUL>(hi_half ? hi : lo, m, logsum, c_f32, neg_g, g, true);
+    const float gv = ENT ? grad_of_ent<T, FAITHFUL>(hi_half ? hi : lo, m, logsum, c_f32, neg_g, g, true, ent, ngh, H)
+                         : grad_of<T, FAITHFUL>(hi_half ? hi : lo, m, logsum, c_f32, neg_g, g, true);
     const uint32_t bits = pack2<T>(gv, gv) & 0xffffu;
     const uint32_t ow = get_word(o, w);
     set_word(o, w, hi_half ? ((ow & 0x0000ffffu) | (bits << 16)) : ((ow & 0xffff0000u) | bits));

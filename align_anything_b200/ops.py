@@ -331,7 +331,10 @@ def _launch_fwd(logits, labels, plan: RowPlan, out, stat_max, stat_logsum, ignor
 
 
 def _launch_bwd(logits, labels, plan: RowPlan, stat_max, stat_logsum, grad_rows, grad_seg, grad_scale,
-                grad_logits, mode_code, scratch=None, ignore_index=None, grad_row_stride=None):
+                grad_logits, mode_code, scratch=None, ignore_index=None, grad_row_stride=None, entropy=None,
+                grad_entropy=None):
+    """K1b; with `entropy` (the forward's fp32 entropy) and `grad_entropy` (its upstream gradient, indexed like
+    grad_rows) the entropy-gradient variant, which adds d H / d logits times g_H to every row with g_H != 0."""
     dev = logits.device
     p = plan.ptrs()
     V = logits.size(-1)
@@ -348,17 +351,21 @@ def _launch_bwd(logits, labels, plan: RowPlan, stat_max, stat_logsum, grad_rows,
                                          plan.n_tile_rows, ctypes.cast(plan.zero_spans, ctypes.c_void_p),
                                          plan.n_zero_spans, L.stream_ptr(dev)))
         n_tile_rows, extra, n_extra = 0, plan.extra_zero_rows, plan.n_extra
-    if scratch is None:  # 32 bytes per work row: the RowRec table of the TMA-staged K1b
+    if scratch is None:  # 32 (entropy variant: 48) bytes per work row: the row records of the TMA-staged K1b
         n_work = n_tile_rows if n_tile_rows > 0 else plan.n_rows + n_extra
-        scratch = torch.empty(max(n_work, 1) * 4, dtype=torch.int64, device=dev)
-    L.check(L.lib().aa_logprob_bwd(
-        logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), labels.data_ptr(),
-        0 if ignore_index is None else int(ignore_index), 0 if ignore_index is None else 1,
-        plan.n_seg, plan.n_rows, p[0], p[1], p[2], p[3], p[4], stat_max.data_ptr(), stat_logsum.data_ptr(),
-        L.ptr(grad_rows), L.dtype_code(grad_rows.dtype) if grad_rows is not None else L.AA_F32,
-        L.ptr(grad_seg), L.ptr(grad_scale), L.dtype_code(grad_scale.dtype) if grad_scale is not None else L.AA_F32,
-        grad_logits.data_ptr(), grad_row_stride, n_tile_rows, L.ptr(extra), n_extra,
-        L.ptr(scratch), mode_code, L.stream_ptr(dev)))
+        scratch = torch.empty(max(n_work, 1) * (4 if entropy is None else 6), dtype=torch.int64, device=dev)
+    head = (logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), labels.data_ptr(),
+            0 if ignore_index is None else int(ignore_index), 0 if ignore_index is None else 1,
+            plan.n_seg, plan.n_rows, p[0], p[1], p[2], p[3], p[4], stat_max.data_ptr(), stat_logsum.data_ptr(),
+            L.ptr(grad_rows), L.dtype_code(grad_rows.dtype) if grad_rows is not None else L.AA_F32,
+            L.ptr(grad_seg), L.ptr(grad_scale), L.dtype_code(grad_scale.dtype) if grad_scale is not None else L.AA_F32)
+    tail = (grad_logits.data_ptr(), grad_row_stride, n_tile_rows, L.ptr(extra), n_extra, L.ptr(scratch), mode_code,
+            L.stream_ptr(dev))
+    if entropy is None:
+        L.check(L.lib().aa_logprob_bwd(*head, *tail))
+    else:
+        L.check(L.lib().aa_logprob_bwd_entropy(*head, entropy.data_ptr(), grad_entropy.data_ptr(),
+                                               L.dtype_code(grad_entropy.dtype), *tail))
 
 
 def _rows_from(logits: torch.Tensor, first_row: int) -> torch.Tensor:
@@ -369,10 +376,17 @@ class _LogProbFn(torch.autograd.Function):
     """K1 forward / K1b backward.  `logits` is the tensor the gradient tile is shaped after; the plan
     addresses rows inside it, starting at row `first_row` of `logits` viewed as (rows, V) (nonzero only for
     the contiguous base of a rerouted view, see _try_reroute).  `entropy` (optional, fp32, plan.out_shape, zeros): the
-    forward also writes each scored row's entropy there (a metric: no gradient flows through it)."""
+    forward also writes each scored row's entropy there (a metric: no gradient flows through it).  `entropy_grad`: the
+    node makes the entropy itself and returns (log-probs, entropy), both differentiable; the backward is K1b's entropy
+    variant, or the plain K1b when the graph never used the entropy."""
 
     @staticmethod
-    def forward(ctx, logits, labels, plan: RowPlan, mode_code: int, first_row: int = 0, entropy=None):
+    def forward(ctx, logits, labels, plan: RowPlan, mode_code: int, first_row: int = 0, entropy=None,
+                entropy_grad: bool = False):
+        ctx.entropy_grad = entropy_grad
+        if entropy_grad:
+            ctx.set_materialize_grads(False)
+            entropy = torch.zeros(plan.out_shape, dtype=torch.float32, device=logits.device)
         out_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         n_out = 1
         for d in plan.out_shape:
@@ -386,24 +400,33 @@ class _LogProbFn(torch.autograd.Function):
             stat_max, stat_logsum = stats[0], stats[1]
         _launch_fwd(_rows_from(logits, first_row), labels, plan, out, stat_max, stat_logsum, entropy=entropy)
         if need_grad:
-            ctx.save_for_backward(logits, labels, stats)
+            ctx.save_for_backward(logits, labels, stats, entropy if entropy_grad else None)
             ctx.plan, ctx.mode_code, ctx.first_row = plan, mode_code, first_row
-        return out
+        return (out, entropy) if entropy_grad else out
 
     @staticmethod
-    def backward(ctx, grad_out):
-        logits, labels, stats = ctx.saved_tensors
+    def backward(ctx, grad_out, grad_entropy=None):
+        logits, labels, stats, entropy = ctx.saved_tensors
+        if grad_out is None:  # only the entropy reached the loss
+            grad_out = torch.zeros(ctx.plan.out_shape, dtype=torch.float32, device=logits.device)
         grad_out = grad_out.contiguous()
         if grad_out.dtype not in (torch.float32, torch.bfloat16, torch.float16):
             grad_out = grad_out.float()
+        if grad_entropy is not None:
+            grad_entropy = grad_entropy.float().contiguous()
+        else:
+            entropy = None
         grad = torch.empty(logits.shape, dtype=logits.dtype, device=logits.device)
         _launch_bwd(_rows_from(logits, ctx.first_row), labels, ctx.plan, stats[0], stats[1], grad_out, None, None, grad,
-                    ctx.mode_code)
-        return grad, None, None, None, None, None
+                    ctx.mode_code, entropy=entropy, grad_entropy=grad_entropy)
+        return grad, None, None, None, None, None, None
 
 
-def _log_probs_and_entropy(logits, labels, plan, mode_code: int, first_row: int = 0):
-    """_LogProbFn with the entropy variant of K1: -> (log-probs, fp32 entropy of the same shape, 0 where unscored)."""
+def _log_probs_and_entropy(logits, labels, plan, mode_code: int, first_row: int = 0, entropy_grad: bool = False):
+    """_LogProbFn with the entropy variant of K1: -> (log-probs, fp32 entropy of the same shape, 0 where unscored).
+    entropy_grad: the entropy is differentiable too (see _LogProbFn)."""
+    if entropy_grad:
+        return _LogProbFn.apply(logits, labels, plan, mode_code, first_row, None, True)
     entropy = torch.zeros(plan.out_shape, dtype=torch.float32, device=logits.device)
     out = _LogProbFn.apply(logits, labels, plan, mode_code, first_row, entropy)
     return out, entropy
@@ -438,15 +461,19 @@ def gather_log_probabilities(logits: torch.Tensor, labels: torch.Tensor, mode: s
     return _gather(logits, labels, mode, False)
 
 
-def gather_log_probabilities_with_entropy(logits: torch.Tensor, labels: torch.Tensor, mode: str | None = None):
+def gather_log_probabilities_with_entropy(logits: torch.Tensor, labels: torch.Tensor, mode: str | None = None,
+                                          entropy_grad: bool = False):
     """gather_log_probabilities plus the policy entropy of every row, -(softmax(x) * log_softmax(x)).sum(-1) of the fp32
     upcast logits, from the same K1 pass (one more FMA per logit; no extra read of the tile).  -> (log_probs, entropy):
-    log_probs bit-identical to gather_log_probabilities (and as differentiable), entropy fp32 in both modes, never
-    requiring grad.  A -inf logit contributes 0 (the limit of p log p); a row of -inf only gets NaN."""
-    return _gather(logits, labels, mode, True)
+    log_probs bit-identical to gather_log_probabilities (and as differentiable), entropy fp32 in both modes.  A -inf
+    logit contributes 0 (the limit of p log p); a row of -inf only gets NaN.  By default the entropy never requires
+    grad; entropy_grad=True makes it differentiable in `logits` (an entropy bonus): its gradient enters the same K1b
+    launch as the log-probs' (-g_H p_k (l_k + H) per logit), and a graph that leaves the entropy unused runs the plain
+    K1b."""
+    return _gather(logits, labels, mode, True, entropy_grad)
 
 
-def _gather(logits, labels, mode, with_entropy: bool):
+def _gather(logits, labels, mode, with_entropy: bool, entropy_grad: bool = False):
     L.require_cuda(logits, labels)
     squeeze = logits.dim() == 2
     if squeeze:
@@ -484,7 +511,8 @@ def _gather(logits, labels, mode, with_entropy: bool):
     if not with_entropy:
         out = _LogProbFn.apply(tile, labels, plan, mode_code, first_row)
         return out.squeeze(0) if squeeze else out
-    out, ent = _log_probs_and_entropy(tile, labels, plan, mode_code, first_row)
+    out, ent = _log_probs_and_entropy(tile, labels, plan, mode_code, first_row,
+                                      entropy_grad and logits.requires_grad and torch.is_grad_enabled())
     return (out.squeeze(0), ent.squeeze(0)) if squeeze else (out, ent)
 
 
@@ -522,9 +550,12 @@ class _LinearLogProbFn(torch.autograd.Function):
     buffers, the padded weight and an fp32 d(weight) accumulator instead of two (rows, V) tiles."""
 
     @staticmethod
-    def forward(ctx, hidden, weight, labels, chunk: int, mode_code: int, entropy=None):
+    def forward(ctx, hidden, weight, labels, chunk: int, mode_code: int, entropy=None, entropy_grad: bool = False):
         N, V = hidden.size(0), weight.size(0)
         dev = hidden.device
+        ctx.set_materialize_grads(False)
+        if entropy_grad:  # the node owns a differentiable entropy (see _LogProbFn)
+            entropy = torch.zeros(N, dtype=torch.float32, device=dev)
         out_dtype = hidden.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         out = torch.empty(N, dtype=out_dtype, device=dev)
         need_grad = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
@@ -539,18 +570,16 @@ class _LinearLogProbFn(torch.autograd.Function):
                         stats[0, r0:r0 + n] if need_grad else None, stats[1, r0:r0 + n] if need_grad else None,
                         entropy=None if entropy is None else entropy[r0:r0 + n])
         if need_grad:
-            ctx.save_for_backward(hidden, weight, labels, stats)
+            ctx.save_for_backward(hidden, weight, labels, stats, entropy if entropy_grad else None)
             ctx.chunk, ctx.mode_code = chunk, mode_code
-        return out
+        return (out, entropy) if entropy_grad else out
 
     @staticmethod
-    def backward(ctx, grad_out):
-        hidden, weight, labels, stats = ctx.saved_tensors
+    def backward(ctx, grad_out, grad_entropy=None):
+        hidden, weight, labels, stats, entropy = ctx.saved_tensors
         N, V, chunk = hidden.size(0), weight.size(0), ctx.chunk
         dev = hidden.device
-        grad_out = grad_out.contiguous()
-        if grad_out.dtype not in (torch.float32, torch.bfloat16, torch.float16):
-            grad_out = grad_out.float()
+        grad_out, entropy, grad_entropy = _lm_head_grads(grad_out, entropy, grad_entropy, N, dev)
         need_h, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         w_pad, Vp = _pad_vocab(weight)
         d_hidden = torch.empty_like(hidden) if need_h else None
@@ -562,12 +591,27 @@ class _LinearLogProbFn(torch.autograd.Function):
             torch.matmul(hidden[r0:r0 + n], w_pad.t(), out=buf[:n])
             plan = _dense_plan(1, n, n * Vp, Vp, n, 0, n, 0, str(dev))
             _launch_bwd(buf[:n, :V], labels[r0:r0 + n], plan, stats[0, r0:r0 + n], stats[1, r0:r0 + n],
-                        grad_out[r0:r0 + n], None, None, dbuf[:n, :V], ctx.mode_code, grad_row_stride=Vp)
+                        grad_out[r0:r0 + n], None, None, dbuf[:n, :V], ctx.mode_code, grad_row_stride=Vp,
+                        entropy=None if entropy is None else entropy[r0:r0 + n],
+                        grad_entropy=None if entropy is None else grad_entropy[r0:r0 + n])
             if need_h:
                 torch.matmul(dbuf[:n], w_pad, out=d_hidden[r0:r0 + n])
             if need_w:  # fp32 accumulation across chunks, one rounding at the end (like a single GEMM)
                 d_weight.add_(_mm_f32(dbuf[:n].t(), hidden[r0:r0 + n]))
-        return d_hidden, (d_weight[:V].to(weight.dtype) if need_w else None), None, None, None, None
+        return d_hidden, (d_weight[:V].to(weight.dtype) if need_w else None), None, None, None, None, None
+
+
+def _lm_head_grads(grad_out, entropy, grad_entropy, N, dev):
+    """The upstream gradients of an lm_head node: the log-probs' (zeros when only the entropy reached the loss) and,
+    when the entropy is differentiable and was used, the entropy with its fp32 gradient; otherwise (None, None)."""
+    if grad_out is None:
+        grad_out = torch.zeros(N, dtype=torch.float32, device=dev)
+    grad_out = grad_out.contiguous()
+    if grad_out.dtype not in (torch.float32, torch.bfloat16, torch.float16):
+        grad_out = grad_out.float()
+    if entropy is None or grad_entropy is None:
+        return grad_out, None, None
+    return grad_out, entropy, grad_entropy.float().contiguous()
 
 
 class _LinearLogProbK6Fn(torch.autograd.Function):
@@ -578,20 +622,21 @@ class _LinearLogProbK6Fn(torch.autograd.Function):
     library GEMM, no padded / transposed copy of the weight."""
 
     @staticmethod
-    def forward(ctx, hidden, weight, labels, chunk: int, mode_code: int, entropy=None):
+    def forward(ctx, hidden, weight, labels, chunk: int, mode_code: int, entropy=None, entropy_grad: bool = False):
+        ctx.set_materialize_grads(False)
+        if entropy_grad:  # the node owns a differentiable entropy; its gradient enters K6b's epilogue
+            entropy = torch.zeros(hidden.size(0), dtype=torch.float32, device=hidden.device)
         out, stats = _k6_forward(hidden, weight, labels, mode_code, True, entropy)
-        ctx.save_for_backward(hidden, weight, labels, stats)
+        ctx.save_for_backward(hidden, weight, labels, stats, entropy if entropy_grad else None)
         ctx.chunk, ctx.mode_code = chunk, mode_code
-        return out
+        return (out, entropy) if entropy_grad else out
 
     @staticmethod
-    def backward(ctx, grad_out):
-        hidden, weight, labels, stats = ctx.saved_tensors
+    def backward(ctx, grad_out, grad_entropy=None):
+        hidden, weight, labels, stats, entropy = ctx.saved_tensors
         N, (V, H), chunk = hidden.size(0), weight.shape, ctx.chunk
         dev = hidden.device
-        grad_out = grad_out.contiguous()
-        if grad_out.dtype not in (torch.float32, torch.bfloat16, torch.float16):
-            grad_out = grad_out.float()
+        grad_out, entropy, grad_entropy = _lm_head_grads(grad_out, entropy, grad_entropy, N, dev)
         ld = (V + 255) // 256 * 256
         need_h, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         d_hidden = torch.empty_like(hidden) if need_h else None
@@ -606,10 +651,15 @@ class _LinearLogProbK6Fn(torch.autograd.Function):
         for i, r0 in enumerate(range(0, N, chunk)):
             n = min(chunk, N - r0)
             h = hidden[r0:r0 + n]
-            L.check(lib.aa_linear_dlogits(
-                h.data_ptr(), n, H, h.stride(0), weight.data_ptr(), V, weight.stride(0), labels[r0:r0 + n].data_ptr(),
-                stats[0, r0:r0 + n].data_ptr(), stats[1, r0:r0 + n].data_ptr(), grad_out[r0:r0 + n].data_ptr(),
-                L.dtype_code(grad_out.dtype), dbuf.data_ptr(), ld, ctx.mode_code, st))
+            head = (h.data_ptr(), n, H, h.stride(0), weight.data_ptr(), V, weight.stride(0), labels[r0:r0 + n].data_ptr(),
+                    stats[0, r0:r0 + n].data_ptr(), stats[1, r0:r0 + n].data_ptr(), grad_out[r0:r0 + n].data_ptr(),
+                    L.dtype_code(grad_out.dtype))
+            if entropy is None:
+                L.check(lib.aa_linear_dlogits(*head, dbuf.data_ptr(), ld, ctx.mode_code, st))
+            else:
+                L.check(lib.aa_linear_dlogits_entropy(*head, entropy[r0:r0 + n].data_ptr(),
+                                                      grad_entropy[r0:r0 + n].data_ptr(), L.AA_F32, dbuf.data_ptr(),
+                                                      ld, ctx.mode_code, st))
             if need_h:
                 dh = d_hidden[r0:r0 + n]
                 L.check(lib.aa_linear_dhidden(dbuf.data_ptr(), n, ld, weight.data_ptr(), V, H, weight.stride(0),
@@ -618,7 +668,7 @@ class _LinearLogProbK6Fn(torch.autograd.Function):
                 last = i == n_chunks - 1
                 L.check(lib.aa_linear_dweight(dbuf.data_ptr(), n, ld, h.data_ptr(), H, h.stride(0), V, L.ptr(acc), H,
                                               1 if i > 0 else 0, d_weight.data_ptr() if last else None, d_weight.stride(0), st))
-        return d_hidden, d_weight, None, None, None, None
+        return d_hidden, d_weight, None, None, None, None, None
 
 
 def _wgmma_head(hidden: torch.Tensor, weight: torch.Tensor) -> bool:
@@ -628,11 +678,14 @@ def _wgmma_head(hidden: torch.Tensor, weight: torch.Tensor) -> bool:
 
 
 def linear_token_log_probs(hidden: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor,
-                           chunk_rows: int | None = None, mode: str | None = None, return_entropy: bool = False):
+                           chunk_rows: int | None = None, mode: str | None = None, return_entropy: bool = False,
+                           entropy_grad: bool = False):
     """gather_log_probabilities(F.linear(hidden, weight), labels) for hidden (N, H), weight (V, H), labels (N,)
     without materialising the (N, V) logits / gradient tiles.  Differentiable in hidden and weight.  return_entropy:
     -> (log_probs, entropy), the fp32 entropy of every row from the forward pass that computes the log-probs (K6's
-    entropy variant, or K1's on the library-GEMM path): no extra GEMM pass, no gradient."""
+    entropy variant, or K1's on the library-GEMM path): no extra GEMM pass, and by default no gradient.  entropy_grad
+    (with return_entropy): the entropy is differentiable in hidden and weight too; its gradient enters the d(logits)
+    buffer in K6b's epilogue (K1b's entropy variant on the library-GEMM path), so the backward runs the same GEMMs."""
     L.require_cuda(hidden, weight, labels)
     if hidden.dim() != 2 or weight.dim() != 2 or hidden.size(1) != weight.size(1) or labels.shape != hidden.shape[:1]:
         raise ValueError('expected hidden (N, H), weight (V, H), labels (N,)')
@@ -655,6 +708,8 @@ def linear_token_log_probs(hidden: torch.Tensor, weight: torch.Tensor, labels: t
     args = (hidden.contiguous(), weight.contiguous(), labels, int(chunk_rows), _mode_code(mode, hidden.dtype))
     if not return_entropy:
         return fn.apply(*args)
+    if entropy_grad and torch.is_grad_enabled() and (hidden.requires_grad or weight.requires_grad):
+        return fn.apply(*args, None, True)
     return fn.apply(*args, entropy), entropy
 
 
@@ -734,7 +789,7 @@ def _tail_indices(counts: tuple, first_pos: tuple, seq: int, W: int, device_str:
 
 
 def _tails_from_hidden(hidden, weight, labels_padded, lens, counts, first_pos, lab_shift, chunk_rows, mode,
-                       return_entropy: bool = False):
+                       return_entropy: bool = False, entropy_grad: bool = False):
     """Sample i scores counts[i] rows: hidden position first_pos[i] + k against labels_padded[i, lab_shift + k].
     The scored rows are gathered into a compact (rows, H) matrix: K6 when nothing needs a gradient, else K6 + K6b + the
     two backward GEMMs (linear_token_log_probs).  Returns (n, max(counts)) right-padded with 0; return_entropy: and the
@@ -756,7 +811,8 @@ def _tails_from_hidden(hidden, weight, labels_padded, lens, counts, first_pos, l
         if return_entropy:
             lp, ent = lp
     elif return_entropy:
-        lp, ent = linear_token_log_probs(rows, weight, lab, chunk_rows, mode, return_entropy=True)
+        lp, ent = linear_token_log_probs(rows, weight, lab, chunk_rows, mode, return_entropy=True,
+                                         entropy_grad=entropy_grad)
     else:
         lp = linear_token_log_probs(rows, weight, lab, chunk_rows, mode)
     out = torch.zeros(n * W, dtype=lp.dtype, device=dev).index_copy(0, dst, lp).view(n, W)
@@ -781,27 +837,30 @@ def sequence_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, i
 
 def tail_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, input_ids: torch.Tensor,
                                response_lens: Sequence[int], chunk_rows: int | None = None,
-                               mode: str | None = None, return_entropy: bool = False):
+                               mode: str | None = None, return_entropy: bool = False, entropy_grad: bool = False):
     """The multimodal PPO scoring rows (trainers/text_image_to_text/ppo.py:233-246, 296-309): sample b scores
     `logits[b, :-1][-R_b:]` against `input_ids[b, 1:][-R_b:]`, here from the last hidden states (B, L, H) and the
     lm_head weight -- hidden position L - 1 - R_b + k predicts token L - R_b + k.  return_entropy: -> (log_probs,
-    entropy), the fp32 policy entropy of the same rows (0 in the padding) from the same forward kernel."""
+    entropy), the fp32 policy entropy of the same rows (0 in the padding) from the same forward kernel; entropy_grad:
+    differentiable too (see linear_token_log_probs)."""
     L.require_cuda(hidden, weight, input_ids)
     lens = tuple(int(r) for r in response_lens)
     seq = hidden.size(1)
     labels = strip_pad_tail(input_ids, lens, 0, strip=False)  # (B, max R): input_ids[b, -R_b:]
     return _tails_from_hidden(hidden, weight, labels, lens, list(lens), [seq - 1 - r for r in lens], 0, chunk_rows, mode,
-                              return_entropy)
+                              return_entropy, entropy_grad)
 
 
 def dense_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, input_ids: torch.Tensor, start: int,
-                                chunk_rows: int | None = None, mode: str | None = None, return_entropy: bool = False):
+                                chunk_rows: int | None = None, mode: str | None = None, return_entropy: bool = False,
+                                entropy_grad: bool = False):
     """`gather_log_probabilities(F.linear(hidden, weight)[:, :-1], input_ids[:, 1:])[:, start:]` from the last hidden
     states (B, L, H) and the lm_head weight (V, H), without the (B, L, V) logits tile: every sample scores the same rows,
     hidden positions [start, L - 1) against tokens [start + 1, L).  The text PPO rollout (start = 0), its rl_step
     (start = prompt_idx) and GRPO (start = L - 1 - logits_to_keep) all read this.  Without a gradient the rows go to K6;
     with one to linear_token_log_probs.  -> (B, L - 1 - start), the dtype gather_log_probabilities returns;
-    return_entropy: (log_probs, fp32 entropy (B, L - 1 - start)) from the same forward kernel (no gradient)."""
+    return_entropy: (log_probs, fp32 entropy (B, L - 1 - start)) from the same forward kernel (no gradient unless
+    entropy_grad, see linear_token_log_probs)."""
     L.require_cuda(hidden, weight, input_ids)
     if hidden.dim() != 3 or input_ids.shape != hidden.shape[:2]:
         raise ValueError('expected hidden (B, L, H) and input_ids (B, L)')
@@ -811,7 +870,7 @@ def dense_log_probs_from_hidden(hidden: torch.Tensor, weight: torch.Tensor, inpu
         raise ValueError(f'start = {start} lies outside [0, {seq - 1}] for sequences of {seq}')
     W = seq - 1 - start
     return _tails_from_hidden(hidden, weight, input_ids, (W,) * B, [W] * B, [start] * B, start + 1, chunk_rows, mode,
-                              return_entropy)
+                              return_entropy, entropy_grad)
 
 
 # ---- DPO -----------------------------------------------------------------------------------------
@@ -1123,10 +1182,10 @@ def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, 
 
 
 def tail_token_log_probs(logits: torch.Tensor, input_ids: torch.Tensor, logits_to_keep: int, mode: str | None = None,
-                         return_entropy: bool = False):
+                         return_entropy: bool = False, entropy_grad: bool = False):
     """GRPOTrainer._get_per_token_logps after the model forward (trainers/text_to_text/grpo.py:205-210):
     log-probs of input_ids[:, -K:] under logits[:, :-1][:, -K:], one K1 launch, (B, K).  return_entropy: and the fp32
-    entropy (B, K) of the same rows from that launch."""
+    entropy (B, K) of the same rows from that launch; entropy_grad: differentiable too (see _LogProbFn)."""
     L.require_cuda(logits, input_ids)
     B, seq, _ = logits.shape
     K = int(logits_to_keep)
@@ -1137,7 +1196,8 @@ def tail_token_log_probs(logits: torch.Tensor, input_ids: torch.Tensor, logits_t
     labels = strip_pad_tail(input_ids, lens, 0, strip=False)
     plan = _tail_plan(lens, seq, logits.stride(0), logits.stride(1), K, 0, -1, None, str(logits.device))
     if return_entropy:
-        return _log_probs_and_entropy(logits, labels, plan, _mode_code(mode, logits.dtype))
+        return _log_probs_and_entropy(logits, labels, plan, _mode_code(mode, logits.dtype), 0,
+                                      entropy_grad and logits.requires_grad and torch.is_grad_enabled())
     return _LogProbFn.apply(logits, labels, plan, _mode_code(mode, logits.dtype))
 
 
@@ -1148,7 +1208,8 @@ class _GrpoFusedFn(torch.autograd.Function):
     value from the log-probs that pass wrote."""
 
     @staticmethod
-    def forward(ctx, logits, labels, plan, ref_lp, adv, tokens, eos_id, beta, mode_code, entropy=None):
+    def forward(ctx, logits, labels, plan, ref_lp, adv, tokens, eos_id, beta, mode_code, entropy=None,
+                entropy_coeff=0.0):
         dev = logits.device
         B, K = plan.out_shape
         lp_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
@@ -1168,35 +1229,59 @@ class _GrpoFusedFn(torch.autograd.Function):
                 scratch.data_ptr(), sc['counter'][5:6].data_ptr(), sc['status'].data_ptr())
         if entropy is None:
             L.check(lib.aa_logprob_grpo_fused(*args, L.stream_ptr(dev)))
-        else:  # the same launch with the entropy of every completion row from its (max, sum-exp) pass
+        elif entropy_coeff == 0.0:  # the same launch with the entropy of every completion row from its (max, sum-exp) pass
             L.check(lib.aa_logprob_grpo_fused_entropy(*args, entropy.data_ptr(), L.stream_ptr(dev)))
+        else:  # ... and the entropy bonus's gradient in the tile
+            L.check(lib.aa_logprob_grpo_fused_entropy_grad(*args, entropy.data_ptr(), float(entropy_coeff),
+                                                           L.stream_ptr(dev)))
         L.check(lib.aa_grpo_loss(lp.data_ptr(), lp.stride(0), ref_lp.data_ptr(), ref_lp.stride(0), L.dtype_code(lp_dtype),
                                  adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), B, K, float(beta),
                                  mode_code, loss.data_ptr(), None, 0, row_end.data_ptr(), scratch.data_ptr(),
                                  sc['counter'][5:7].data_ptr(), L.stream_ptr(dev)))
         ctx.save_for_backward(grad)
-        ctx.mark_non_differentiable(lp, row_end)
-        return loss[0], lp, row_end
+        if entropy_coeff == 0.0:
+            ctx.mark_non_differentiable(lp, row_end)
+            return loss[0], lp, row_end
+        h_mean = _completion_mean(entropy, row_end)
+        plain = loss[0].clone()
+        ctx.mark_non_differentiable(lp, row_end, h_mean, plain)  # one call: a second one would replace the first
+        return loss[0] - entropy_coeff * h_mean, lp, row_end, h_mean, plain
 
     @staticmethod
-    def backward(ctx, g, _lp, _re):
+    def backward(ctx, g, *_unused):
         (grad,) = _hand_over_once(ctx, g, *ctx.saved_tensors)
-        return grad, None, None, None, None, None, None, None, None, None
+        return grad, None, None, None, None, None, None, None, None, None, None
+
+
+def _completion_mean(x: torch.Tensor, row_end: torch.Tensor) -> torch.Tensor:
+    """GRPO's token mean of x (B, K) over the completion mask (tokens up to and including the first eos)."""
+    mask = torch.arange(x.size(1), device=x.device) < row_end.unsqueeze(1)
+    return (x * mask).sum() / mask.sum()
 
 
 def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_to_keep: int,
                           ref_per_token_logps: torch.Tensor, advantages: torch.Tensor, eos_token_id: int, beta: float,
-                          mode: str | None = None, return_entropy: bool = False):
+                          mode: str | None = None, return_entropy: bool = False, entropy_coeff: float = 0.0):
     """`_get_per_token_logps` of the policy + the loss of GRPOTrainer.train_step (trainers/text_to_text/grpo.py:205-210,
     290-312) from the policy's logits; the reference model's per-token log-probs must already be there.
     -> (loss fp32 scalar, policy per-token log-probs (B, K), counted tokens per row).  With a gradient: one pass over the
     completion rows (see _GrpoFusedFn); otherwise tail_token_log_probs + grpo_loss.  return_entropy appends the fp32
     policy entropy (B, K) of the completion rows, from the same pass (K1f's phase A, or K1's entropy variant); the
-    other outputs are bit-identical."""
+    other outputs are bit-identical.  entropy_coeff != 0 (entropy bonus): the loss is
+    loss - entropy_coeff * (H * mask).sum() / mask.sum()  over the completion mask, and the detached entropy mean and
+    the detached GRPO loss without the bonus follow row_end (before the entropy when return_entropy); the single pass is K1f's entropy-gradient variant, the
+    composed path K1's entropy variant -> grpo_loss -> K1b's entropy variant."""
     L.require_cuda(logits, input_ids, ref_per_token_logps, advantages)
     K = int(logits_to_keep)
     tokens = input_ids[:, -K:]
+    coeff = float(entropy_coeff)
     if not _single_pass_ok(logits, _FUSED_GRPO, torch.is_grad_enabled() and logits.requires_grad):
+        if coeff != 0.0:
+            lp, ent = tail_token_log_probs(logits, input_ids, K, mode=mode, return_entropy=True, entropy_grad=True)
+            loss, row_end = grpo_loss(lp, ref_per_token_logps, advantages, tokens, eos_token_id, beta, mode=mode)
+            h_mean = _completion_mean(ent, row_end)
+            out = (loss - coeff * h_mean, lp.detach(), row_end, h_mean.detach(), loss.detach())
+            return out + (ent.detach(),) if return_entropy else out
         if return_entropy:
             lp, ent = tail_token_log_probs(logits, input_ids, K, mode=mode, return_entropy=True)
         else:
@@ -1219,10 +1304,14 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
     if adv.numel() != B:
         raise ValueError('one advantage per sequence expected')
     tok = _contiguous_last(tokens.to(torch.int64))
-    if not return_entropy:
+    if not return_entropy and coeff == 0.0:
         return _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code)
     ent = torch.zeros((B, K), dtype=torch.float32, device=logits.device)
-    return _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code, ent) + (ent,)
+    if coeff == 0.0:
+        return _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code,
+                                  ent) + (ent,)
+    out = _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code, ent, coeff)
+    return out + (ent,) if return_entropy else out
 
 
 # ---- reward-model pairwise loss -----------------------------------------------------------------------
@@ -1881,15 +1970,23 @@ class _TailActorLossFn(torch.autograd.Function):
     on the device iff that is not 1).
     `single_pass` False (see _single_pass_ok), or a plan K1f does not take: forward = K1 over the response tails + K5;
     backward = K1b taking K5's d loss / d log-probs as its per-row upstream gradient and the incoming scalar as a device
-    scale."""
+    scale.
+    entropy_coeff != 0 (entropy bonus): the node's loss is  actor_loss - entropy_coeff * masked_mean(H, mask)  and a
+    fourth output, the detached masked-mean entropy, follows; the third stays the actor loss without the bonus.  K1f's
+    entropy-gradient variant (aa_logprob_actor_fused_entropy), or K1's entropy variant + K5 + masked_mean and, in the
+    backward, K1b's entropy variant with g_H = -entropy_coeff * mask / (B * mask count of the row)."""
 
     @staticmethod
-    def forward(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, single_pass):
+    def forward(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, single_pass, entropy_coeff=0.0):
         out_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         dev = logits.device
         lp = torch.zeros(plan.out_shape, dtype=out_dtype, device=dev)
         ctx.fused = bool(single_pass and plan.n_tile_rows > 0 and plan.n_seg > 0 and plan.n_tile_rows % plan.n_seg == 0
                          and len(plan.out_shape) == 2)
+        if entropy_coeff != 0.0:
+            return _TailActorLossFn._forward_bonus(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, lp,
+                                                   float(entropy_coeff))
+        ctx.bonus = False
         if ctx.fused:
             grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
             scratch = torch.empty(plan.n_tile_rows * 6, dtype=torch.int64, device=dev)  # 48 bytes per tile row
@@ -1912,18 +2009,54 @@ class _TailActorLossFn(torch.autograd.Function):
         return cast, lp, loss
 
     @staticmethod
-    def backward(ctx, g_loss, _lp, _l):
+    def _forward_bonus(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, lp, coeff):
+        dev = logits.device
+        ctx.bonus = True
+        ent = torch.zeros(plan.out_shape, dtype=torch.float32, device=dev)
+        if ctx.fused:
+            grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
+            # 48 bytes per tile row (the row records) + 4 per segment (the rows' g_H coefficients)
+            scratch = torch.empty(plan.n_tile_rows * 6 + (plan.n_seg + 1) // 2, dtype=torch.int64, device=dev)
+            p = plan.ptrs()
+            L.check(L.lib().aa_logprob_actor_fused_entropy(
+                logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), ids.data_ptr(),
+                plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp.dtype),
+                None, None, old.data_ptr(), old.stride(0), aux.data_ptr(), aux.stride(0), L.dtype_code(aux.dtype),
+                mask.data_ptr(), mask.stride(0), lp.size(1), float(clip), mode_code, grad.data_ptr(), logits.size(-1),
+                scratch.data_ptr(), _device_scratch(dev)['status'].data_ptr(), coeff, ent.data_ptr(), L.stream_ptr(dev)))
+            loss, _, _, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True)
+            ctx.save_for_backward(grad)
+        else:
+            stats = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=dev)
+            _launch_fwd(logits, ids, plan, lp, stats[0], stats[1], entropy=ent)
+            loss, _, grad_lp, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True)
+            # d (-coeff * masked_mean(H, mask)) / d H, as _MaskedMeanFn's backward forms it
+            # (0, not 0 * -inf, for a sample without masked-in tokens: K1f forms g_H for masked-in tokens only)
+            g_h = torch.where(mask, -coeff / (mask.size(0) * mask.sum(dim=-1, keepdim=True).float()), 0.0)
+            ctx.save_for_backward(logits, ids, stats, grad_lp, ent, g_h)
+            ctx.plan, ctx.mode_code = plan, mode_code
+        h_mean = masked_mean(ent, mask)
+        reg = loss[0] - coeff * h_mean
+        ctx.mark_non_differentiable(lp, loss, h_mean)
+        return reg, lp, loss, h_mean
+
+    @staticmethod
+    def backward(ctx, g_loss, *_unused):
         if ctx.fused:
             (grad,) = _hand_over_once(ctx, g_loss, *ctx.saved_tensors)
-            return grad, None, None, None, None, None, None, None, None
+            return grad, None, None, None, None, None, None, None, None, None
         scale = g_loss.detach().reshape(1)
         if scale.dtype not in (torch.float32, torch.bfloat16, torch.float16):
             scale = scale.float()
         scale = scale.contiguous()
-        logits, ids, stats, grad_lp = ctx.saved_tensors
+        if ctx.bonus:
+            logits, ids, stats, grad_lp, ent, g_h = ctx.saved_tensors
+        else:
+            (logits, ids, stats, grad_lp), ent, g_h = ctx.saved_tensors, None, None
         grad = torch.empty(logits.shape, dtype=logits.dtype, device=logits.device)
-        _launch_bwd(logits, ids, ctx.plan, stats[0], stats[1], grad_lp, None, scale, grad, ctx.mode_code)
-        return grad, None, None, None, None, None, None, None, None
+        _launch_bwd(logits, ids, ctx.plan, stats[0], stats[1], grad_lp, None, scale, grad, ctx.mode_code, entropy=ent,
+                    grad_entropy=g_h)
+        return grad, None, None, None, None, None, None, None, None, None
 
 
 class _TailCriticLossFn(torch.autograd.Function):
@@ -1987,9 +2120,11 @@ def critic_loss(values, old_values, returns, mask, clip_range_value: float, mode
 
 
 def tail_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, lens, old_log_probs, advantages, mask,
-                    clip_range_ratio: float, mode: str | None = None):
+                    clip_range_ratio: float, mode: str | None = None, entropy_coeff: float = 0.0):
     """response_tail_log_probs + actor_loss as one autograd node (see _TailActorLossFn).
-    -> (actor loss, new log-probs (B, W), the loss as fp32[2] for ppo_pack_metrics)."""
+    -> (actor loss, new log-probs (B, W), the loss as fp32[2] for ppo_pack_metrics).  entropy_coeff != 0: the first
+    output is  actor_loss - entropy_coeff * masked_mean(H, mask)  (fp32), the third stays the actor loss without the
+    bonus, and the detached masked-mean entropy follows as a fourth."""
     L.require_cuda(logits, input_ids, old_log_probs, advantages, mask)
     lens = as_device_lens(lens, logits.device)
     B, K, _ = logits.shape
@@ -2007,6 +2142,9 @@ def tail_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, lens, old_log
     m = _contiguous_last(mask.to(torch.bool))
     plan = device_tail_plan(lens, K, logits.stride(0), logits.stride(1), ids.stride(0), ids.size(1), 0, -1, lens.bound)
     single_pass = _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad)
+    if entropy_coeff != 0.0:
+        return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass,
+                                      float(entropy_coeff))
     return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass)
 
 
@@ -2020,13 +2158,17 @@ def _dense_actor_plan(B: int, L: int, start: int, sb: int, sl: int, lab_sb: int,
 
 
 def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, old_log_probs, advantages, mask,
-                     clip_range_ratio: float, mode: str | None = None):
+                     clip_range_ratio: float, mode: str | None = None, entropy_coeff: float = 0.0):
     """The actor half of the text rl_step (trainers/text_to_text/ppo.py:336-349) as one autograd node:
     `gather_log_probabilities(logits[:, :-1], ids[:, 1:])[:, start:]` -> `actor_loss_fn` -> backward up to d logits.
     Only the rows `[start, L - 1)` are read (the reference scores every position and slices afterwards); with a
     gradient and rows long enough (see _single_pass_ok) the node is the single-pass K1f (see _TailActorLossFn), otherwise the
     composed ops gather_log_probabilities -> actor_loss.  old_log_probs / advantages / mask: (B, L - 1 - start).
-    -> (actor loss, new log-probs (B, L - 1 - start), the loss for ppo_pack_metrics: fp32[2] buffer or the 0-dim loss)."""
+    -> (actor loss, new log-probs (B, L - 1 - start), the loss for ppo_pack_metrics: fp32[2] buffer or the 0-dim loss).
+    entropy_coeff != 0 (entropy bonus): the first output is  actor_loss - entropy_coeff * masked_mean(H, mask)  (fp32),
+    the third stays the actor loss without the bonus and the detached masked-mean entropy follows as a fourth; the
+    single pass is K1f's entropy-gradient variant, the composed path K1's entropy variant -> K5 + masked_mean -> K1b's
+    entropy variant."""
     L.require_cuda(logits, input_ids, old_log_probs, advantages, mask)
     if logits.dim() != 3 or input_ids.shape != logits.shape[:2]:
         raise ValueError('expected logits (B, L, V) and input_ids (B, L)')
@@ -2039,6 +2181,12 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
         raise ValueError('old_log_probs, advantages and mask must all be (B, L - 1 - start)')
     if not _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad):
         # short rows, fp16, no gradient: the composed ops (K1 over the response rows -> K5; backward K1b)
+        if entropy_coeff != 0.0:
+            lp, ent = gather_log_probabilities_with_entropy(logits[:, start:-1], input_ids[:, start + 1:], mode=mode,
+                                                            entropy_grad=True)
+            loss = actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, mode=mode)
+            h_mean = masked_mean(ent, mask)
+            return loss - float(entropy_coeff) * h_mean, lp.detach(), loss, h_mean.detach()
         lp = gather_log_probabilities(logits[:, start:-1], input_ids[:, start + 1:], mode=mode)
         loss = actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, mode=mode)
         return loss, lp.detach(), loss
@@ -2053,6 +2201,9 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
         aux = aux.float()
     m = _contiguous_last(mask.to(torch.bool))
     plan = _dense_actor_plan(B, Lq, start, logits.stride(0), logits.stride(1), ids.stride(0), str(logits.device))
+    if entropy_coeff != 0.0:
+        return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, True,
+                                      float(entropy_coeff))
     return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, True)
 
 

@@ -15,7 +15,7 @@ import torch
 
 from ... import ops
 from ...utils.multi_process import all_reduce_packed, fused_allreduce
-from ..text_to_text.ppo import METRIC_KEYS, with_entropy_lane
+from ..text_to_text.ppo import METRIC_KEYS, entropy_coeff_of, with_bonus_lane, with_entropy_lane
 from ..text_to_text.ppo import PPOTrainer as _TextPPOTrainer
 
 __all__ = ['PPOTrainer', 'move_padding_left']
@@ -47,16 +47,16 @@ class PPOTrainer(_TextPPOTrainer):
     # loops over micro-batches of per_device_train_batch_size (text_audio_to_text/ppo.py:217-277)
     micro_batched_rollout = False
 
-    def _tail_log_probs(self, model, batch, lens, input_ids, return_entropy=False, **kw):
+    def _tail_log_probs(self, model, batch, lens, input_ids, return_entropy=False, entropy_grad=False, **kw):
         """(B, W) log-probs of the response tails, right-padded with 0 (W = lens.bound); return_entropy (fused_lm_head
-        only): and the fp32 policy entropy of the same rows, from the same kernel."""
+        only): and the fp32 policy entropy of the same rows, from the same kernel (differentiable with entropy_grad)."""
         lens = ops.as_device_lens(lens, input_ids.device)
         if self.fused_lm_head:
             out = model(**batch, output_hidden_states=True, logits_to_keep=1, **kw)
             module = getattr(model, 'module', model)
             return ops.tail_log_probs_from_hidden(out.hidden_states[-1], ops.lm_head_weight(module), input_ids,
                                                   lens.tolist(), chunk_rows=self.lm_head_chunk_rows, mode=self.mode,
-                                                  return_entropy=return_entropy)
+                                                  return_entropy=return_entropy, entropy_grad=entropy_grad)
         logits = self._actor_logits(model, batch, lens, **kw)
         return ops.response_tail_log_probs(logits, input_ids, lens, mode=self.mode)
 
@@ -159,14 +159,30 @@ class PPOTrainer(_TextPPOTrainer):
 
         # actor: K1 over the response tails + K5 as ONE autograd node; its backward is K1b alone (:296-316)
         batch = self.infer_batch(inference_batch)
-        if self.fused_lm_head:
+        coeff = entropy_coeff_of(self)  # entropy bonus over the response tails (the actor loss's rows and mask)
+        entropy_mean = None
+        if self.fused_lm_head and coeff != 0.0:  # K6's entropy variant; K6b adds the entropy's gradient in its epilogue
+            log_probs, ent = self._tail_log_probs(self.actor_model, batch, lens, input_ids, return_entropy=True,
+                                                  entropy_grad=True, use_cache=False)
+            actor_loss32 = ops.actor_loss(log_probs, old_log_probs, reward_advantages, sequence_mask,
+                                          self.clip_range_ratio, mode=self.mode)
+            entropy_mean = ops.masked_mean(ent, sequence_mask)
+            actor_loss = actor_loss32 - coeff * entropy_mean
+            entropy_mean = entropy_mean.detach()
+        elif self.fused_lm_head:
             log_probs = self._tail_log_probs(self.actor_model, batch, lens, input_ids, use_cache=False)
             actor_loss = actor_loss32 = ops.actor_loss(log_probs, old_log_probs, reward_advantages, sequence_mask,
                                                        self.clip_range_ratio, mode=self.mode)
         else:
             logits = self._actor_logits(self.actor_model, batch, lens, use_cache=False)
-            actor_loss, _, actor_loss32 = ops.tail_actor_loss(logits, input_ids, lens, old_log_probs, reward_advantages,
-                                                              sequence_mask, self.clip_range_ratio, mode=self.mode)
+            if coeff != 0.0:
+                actor_loss, _, actor_loss32, entropy_mean = ops.tail_actor_loss(
+                    logits, input_ids, lens, old_log_probs, reward_advantages, sequence_mask, self.clip_range_ratio,
+                    mode=self.mode, entropy_coeff=coeff)
+            else:
+                actor_loss, _, actor_loss32 = ops.tail_actor_loss(logits, input_ids, lens, old_log_probs,
+                                                                  reward_advantages, sequence_mask,
+                                                                  self.clip_range_ratio, mode=self.mode)
         self.actor_model.backward(actor_loss)
         self.actor_model.step()
 
@@ -178,11 +194,14 @@ class PPOTrainer(_TextPPOTrainer):
         self.reward_critic_model.step()
 
         with torch.no_grad():
-            fused = fused_allreduce(row_stats.device) if not self.log_entropy else None  # see the text rl_step
+            # see the text rl_step
+            fused = fused_allreduce(row_stats.device) if not (self.log_entropy or entropy_mean is not None) else None
             stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss32, critic_loss32,
                                          coll=fused.next((9, 10)) if fused is not None else None)
             if self.log_entropy:
                 stats = with_entropy_lane(stats, training_batch['entropy'], sequence_mask)
+            if entropy_mean is not None:
+                stats = with_bonus_lane(stats, entropy_mean)
             if fused is None:
                 stats = all_reduce_packed(stats, max_lanes=(9, 10))
             v = stats.tolist()  # the ONE host sync of rollout scoring + rl_step
@@ -190,6 +209,8 @@ class PPOTrainer(_TextPPOTrainer):
         out = dict(zip(METRIC_KEYS, v[:10]))
         if self.log_entropy:
             out['train/entropy'] = v[11]
+        if entropy_mean is not None:
+            out['train/actor_entropy'] = v[12]
         out['train/actor_lr'] = self.actor_model.optimizer.param_groups[0]['lr']
         out['train/reward_critic_lr'] = self.reward_critic_model.optimizer.param_groups[0]['lr']
         self.last_rl_tensors = {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns}

@@ -32,13 +32,15 @@ def lm_head_of(model) -> torch.Tensor:
     return ops.lm_head_weight(getattr(model, 'module', model))
 
 
-def hidden_log_probs(model, batch, input_ids, start, weight, chunk_rows, mode, return_entropy=False, **kw):
+def hidden_log_probs(model, batch, input_ids, start, weight, chunk_rows, mode, return_entropy=False, entropy_grad=False,
+                     **kw):
     """`gather_log_probabilities(model(**batch).logits[:, :-1], input_ids[:, 1:])[:, start:]` from the model's last
     hidden states: the lm_head runs on one position inside the model and on the scored rows in ops, no logits tile.
-    return_entropy: -> (log_probs, fp32 policy entropy of the same rows) from the same kernel."""
+    return_entropy: -> (log_probs, fp32 policy entropy of the same rows) from the same kernel (differentiable with
+    entropy_grad: its gradient enters K6b's epilogue)."""
     out = model(**batch, output_hidden_states=True, logits_to_keep=1, **kw)
     return ops.dense_log_probs_from_hidden(out.hidden_states[-1], weight, input_ids, start, chunk_rows=chunk_rows,
-                                           mode=mode, return_entropy=return_entropy)
+                                           mode=mode, return_entropy=return_entropy, entropy_grad=entropy_grad)
 
 
 def with_entropy_lane(stats: torch.Tensor, entropy: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
@@ -49,23 +51,52 @@ def with_entropy_lane(stats: torch.Tensor, entropy: torch.Tensor, mask: torch.Te
     return torch.cat([stats[:11], ent.reshape(1)])
 
 
+def entropy_coeff_of(tr) -> float:
+    """The entropy-bonus coefficient in effect: `cfgs.train_cfgs.entropy_coeff` when the config sets it (a yaml recipe),
+    otherwise the class switch `entropy_coeff`."""
+    tc = getattr(getattr(tr, 'cfgs', None), 'train_cfgs', None)
+    v = getattr(tc, 'entropy_coeff', None) if tc is not None else None
+    return float(tr.entropy_coeff if v is None else v)
+
+
+def with_bonus_lane(stats: torch.Tensor, entropy_mean: torch.Tensor) -> torch.Tensor:
+    """The packed metric vector with one more lane: the masked-mean policy entropy the bonus regularises (AVG-reduced
+    by the step's one packed all-reduce)."""
+    return torch.cat([stats, entropy_mean.detach().float().reshape(1)])
+
+
 def actor_loss_node(tr, inference_batch, input_ids, start, head, old_log_probs, advantages, sequence_mask):
-    """The actor loss of the text rl_step over the rows `[start:]` -> (loss, the loss for ppo_pack_metrics).  `head`:
-    the lm_head weight when `tr.fused_lm_head` is on, else None.  A function rather than a method, so that the grafted
-    rl_step of the reference's classes finds it without being grafted itself."""
+    """The actor loss of the text rl_step over the rows `[start:]` -> (loss, the loss for ppo_pack_metrics, the
+    masked-mean entropy or None).  `head`: the lm_head weight when `tr.fused_lm_head` is on, else None.  With an entropy
+    bonus (entropy_coeff_of(tr) != 0) the loss is  actor_loss - c * masked_mean(H, mask)  over the same rows and mask,
+    the second output stays the actor loss without it.  A function rather than a method, so that the grafted rl_step
+    of the reference's classes finds it without being grafted itself."""
+    coeff = entropy_coeff_of(tr)
+    if head is not None and coeff != 0.0:  # K6's entropy variant; K6b adds the entropy's gradient in its epilogue
+        log_probs, ent = hidden_log_probs(tr.actor_model, inference_batch, input_ids, start, head, tr.lm_head_chunk_rows,
+                                          tr.mode, return_entropy=True, entropy_grad=True, use_cache=False)
+        loss = ops.actor_loss(log_probs, old_log_probs[:, start:], advantages, sequence_mask[:, start:],
+                              tr.clip_range_ratio, mode=tr.mode)
+        h_mean = ops.masked_mean(ent, sequence_mask[:, start:])
+        return loss - coeff * h_mean, loss, h_mean.detach()
     if head is not None:  # K6 + K6b + backward GEMMs for the log-probs, then K5
         log_probs = hidden_log_probs(tr.actor_model, inference_batch, input_ids, start, head, tr.lm_head_chunk_rows,
                                      tr.mode, use_cache=False)
         loss = ops.actor_loss(log_probs, old_log_probs[:, start:], advantages, sequence_mask[:, start:],
                               tr.clip_range_ratio, mode=tr.mode)
-        return loss, loss
+        return loss, loss, None
     logits = tr.actor_model(**inference_batch, use_cache=False).logits
     # the reference scores every position and then slices `[:, start:]` (:338-346); only those rows are ever used, so
     # only they are read here.  One autograd node (K1f): log-probs, d loss / d log-prob and the gradient tile in a
     # single pass over the response rows; the prompt rows of the tile are written as zeros by the same kernel.
+    if coeff != 0.0:
+        loss, _, loss32, h_mean = ops.dense_actor_loss(logits, input_ids, start, old_log_probs[:, start:], advantages,
+                                                       sequence_mask[:, start:], tr.clip_range_ratio, mode=tr.mode,
+                                                       entropy_coeff=coeff)
+        return loss, loss32, h_mean
     loss, _, loss32 = ops.dense_actor_loss(logits, input_ids, start, old_log_probs[:, start:], advantages,
                                            sequence_mask[:, start:], tr.clip_range_ratio, mode=tr.mode)
-    return loss, loss32
+    return loss, loss32, None
 
 
 class PPOTrainer:
@@ -78,6 +109,11 @@ class PPOTrainer:
     # Opt-in: `train/entropy`, the policy entropy of the rollout, taken from the pass that scores its log-probs (K1's
     # or K6's entropy variant: one more FMA per logit, no extra read) and reduced in the step's one packed collective
     log_entropy = False
+    # Entropy bonus: the actor minimises  actor_loss - entropy_coeff * masked_mean(H, mask)  (H: the policy entropy of
+    # rl_step's own pass, its gradient written by the log-prob kernels).  `cfgs.train_cfgs.entropy_coeff` overrides it
+    # when set; 0 leaves the step unchanged.  train/actor_loss stays the loss without the bonus, train/actor_entropy
+    # carries the entropy term.
+    entropy_coeff = 0.0
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, reward_model=None,
                  reward_critic_model=None, tokenizer=None, reward_tokenizer=None, *, kl_coeff=0.02,
@@ -246,8 +282,8 @@ class PPOTrainer:
             reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, start, self.kl_coeff,
             self.clip_range_score, self.gamma, self.gae_lambda, mode=self.mode)
 
-        actor_loss, actor_loss32 = actor_loss_node(self, inference_batch, input_ids, start, head, old_log_probs,
-                                                   reward_advantages, sequence_mask)
+        actor_loss, actor_loss32, entropy_mean = actor_loss_node(self, inference_batch, input_ids, start, head,
+                                                                 old_log_probs, reward_advantages, sequence_mask)
         self.actor_model.backward(actor_loss)
         self.actor_model.step()
 
@@ -262,11 +298,14 @@ class PPOTrainer:
         with torch.no_grad():
             # with log_entropy the entropy lane is filled in before the one packed all-reduce, so the NVLink reduction
             # fused into ppo_pack_metrics (which reduces the vector as it writes it) gives way to all_reduce_packed
-            fused = fused_allreduce(row_stats.device) if not self.log_entropy else None
+            # (so does the entropy bonus's lane)
+            fused = fused_allreduce(row_stats.device) if not (self.log_entropy or entropy_mean is not None) else None
             stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss32, reward_critic_loss,
                                          coll=fused.next((9, 10)) if fused is not None else None)
             if self.log_entropy:
                 stats = with_entropy_lane(stats, training_batch['entropy'][:, start:], sequence_mask[:, start:])
+            if entropy_mean is not None:
+                stats = with_bonus_lane(stats, entropy_mean)
             if fused is None:
                 stats = all_reduce_packed(stats, max_lanes=(9, 10))  # ONE collective (reference: 10 + barrier)
             v = stats.tolist()  # ONE host sync (reference: 12 .item())
@@ -274,6 +313,8 @@ class PPOTrainer:
         out = dict(zip(METRIC_KEYS, v[:10]))
         if self.log_entropy:
             out['train/entropy'] = v[11]
+        if entropy_mean is not None:
+            out['train/actor_entropy'] = v[12]
         out['train/actor_lr'] = self.actor_model.optimizer.param_groups[0]['lr']
         out['train/reward_critic_lr'] = self.reward_critic_model.optimizer.param_groups[0]['lr']
         # the per-token tensors stay OUT of the returned dict: the reference hands it to Logger.log -> add_scalar /

@@ -162,6 +162,28 @@ int aa_logprob_bwd(const void *logits, int logits_dtype, int64_t row_stride, int
                    const int64_t *extra_zero_rows, int64_t n_extra_zero_rows,
                    void *row_scratch, int mode, void *stream);
 
+/* aa_logprob_bwd with the gradient of the rows' entropy added (entropy bonus): the tile element becomes
+ *   g * (onehot_y - p_k)  -  g_H * p_k * (l_k + H),   l_k = x_k - max - logsum, p_k = e^{l_k}
+ * with p_k and l_k as the log-prob term uses them (FAITHFUL: the rounded log-softmax), the correction in fp32 before the
+ * tile's one rounding, and 0 for a -inf logit.  entropy: the fp32 H of aa_logprob_fwd_entropy; grad_entropy: g_H in
+ * grad_entropy_dtype; both indexed like grad_rows.  grad_scale multiplies g_H too, grad_seg does not.  A row with
+ * g_H == 0 is bit-identical to aa_logprob_bwd's.  row_scratch is required: 48 bytes per work row, 16-byte aligned.
+ * This entry always runs the TMA-staged kernel: the LDG row kernel (aa_logprob_set_tuning_bwd variant 3) has no
+ * entropy variant, and the tuning does not apply here. */
+int aa_logprob_bwd_entropy(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                           const int64_t *labels, int64_t ignore_index, int32_t use_ignore,
+                           int32_t n_segments, int64_t n_rows,
+                           const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                           const int64_t *seg_out_off, const int64_t *seg_cum,
+                           const int64_t *seg_tile_row,
+                           const float *stat_max, const float *stat_logsum,
+                           const void *grad_rows, int grad_rows_dtype, const float *grad_seg,
+                           const void *grad_scale, int grad_scale_dtype,
+                           const float *entropy, const void *grad_entropy, int grad_entropy_dtype,
+                           void *grad_logits, int64_t grad_row_stride, int64_t n_tile_rows,
+                           const int64_t *extra_zero_rows, int64_t n_extra_zero_rows,
+                           void *row_scratch, int mode, void *stream);
+
 /* Zero-fill row spans of an (n_tile_rows, V) tile with the copy engine.  spans_host: n_spans pairs
  * (first_row, n_rows) in HOST memory (read during the call); rows are row_stride elements apart.
  * Used for the prompt / padding rows of the gradient tile, BEFORE aa_logprob_bwd on the same stream:
@@ -385,6 +407,20 @@ int aa_logprob_actor_fused(const void *logits, int logits_dtype, int64_t row_str
                            const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
                            int64_t mask_stride, int32_t W, float clip_range_ratio, int mode, void *grad_logits,
                            int64_t grad_row_stride, void *row_scratch, int32_t *status, void *stream);
+/* aa_logprob_actor_fused for the regularised objective  actor_loss - entropy_coeff * masked_mean(H, mask): the
+ * entropy of every scored row is written to `entropy` (fp32, laid out like log_probs, zero-initialised by the caller)
+ * and the gradient tile carries the entropy's gradient (aa_logprob_bwd_entropy's formula) with
+ * g_H = -entropy_coeff * mask / (n_segments * mask count of the row).  log_probs, stat_* and the rows with g_H == 0
+ * are bit-identical to aa_logprob_actor_fused.  row_scratch: 48 bytes per tile row plus 4 bytes per segment. */
+int aa_logprob_actor_fused_entropy(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                   const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                   const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
+                                   const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
+                                   float *stat_max, float *stat_logsum, const void *old_log_probs, int64_t old_stride,
+                                   const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
+                                   int64_t mask_stride, int32_t W, float clip_range_ratio, int mode, void *grad_logits,
+                                   int64_t grad_row_stride, void *row_scratch, int32_t *status, float entropy_coeff,
+                                   float *entropy, void *stream);
 
 /* The same single pass for the mean cross-entropy behind `outputs.loss` (trainers/text_to_text/sft.py:95-98
  * `SupervisedTrainer.loss`, ppo.py:400-408 `ptx_step`; transformers' ForCausalLMLoss): every row whose label !=
@@ -426,6 +462,18 @@ int aa_logprob_grpo_fused_entropy(const void *logits, int logits_dtype, int64_t 
                                   int64_t tok_stride, int64_t eos_id, int32_t K, float beta, int mode, void *grad_logits,
                                   int64_t grad_row_stride, void *row_scratch, int32_t *row_end, float *total,
                                   uint32_t *counter, int32_t *status, float *entropy, void *stream);
+/* aa_logprob_grpo_fused_entropy for  loss - entropy_coeff * (H * mask).sum() / mask.sum()  over the completion mask:
+ * the tile also carries the entropy's gradient (aa_logprob_bwd_entropy's formula) with g_H = -entropy_coeff / total for
+ * counted tokens.  log_probs, row_end, total and the rows with g_H == 0 are bit-identical to aa_logprob_grpo_fused. */
+int aa_logprob_grpo_fused_entropy_grad(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                       const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                       const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
+                                       const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
+                                       const void *ref_log_probs, int64_t ref_stride, const float *advantages,
+                                       const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t K,
+                                       float beta, int mode, void *grad_logits, int64_t grad_row_stride,
+                                       void *row_scratch, int32_t *row_end, float *total, uint32_t *counter,
+                                       int32_t *status, float *entropy, float entropy_coeff, void *stream);
 
 /* tile[0..n) *= *scale unless *scale == 1 (checked on the device: the usual `loss.backward()` costs one empty launch).
  * Contiguous tile; scale: device scalar of scale_dtype.  The autograd backward of the K1f node. */
@@ -531,6 +579,15 @@ int aa_linear_dlogits(const void *hidden, int64_t n_rows, int32_t H, int64_t hid
                       const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
                       const float *stat_max, const float *stat_logsum, const void *grad_rows,
                       int grad_rows_dtype, void *dlogits, int64_t ld, int mode, void *stream);
+/* aa_linear_dlogits with the gradient of each row's entropy added in the epilogue (entropy bonus):
+ *   d(logits)[row, k] += -g_H * p_k * (l_k + H)   with the p_k and l_k of the line above, in fp32 before the bf16 store,
+ * 0 for a -inf logit.  entropy: the fp32 H of aa_linear_logprob_fwd_entropy; grad_entropy: g_H per row
+ * (grad_entropy_dtype).  Rows with g_H == 0 are bit-identical to aa_linear_dlogits's. */
+int aa_linear_dlogits_entropy(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
+                              const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
+                              const float *stat_max, const float *stat_logsum, const void *grad_rows,
+                              int grad_rows_dtype, const float *entropy, const void *grad_entropy,
+                              int grad_entropy_dtype, void *dlogits, int64_t ld, int mode, void *stream);
 
 /* The two GEMMs that finish that backward: the autograd of the model's nn.Linear lm_head (callers
  * trainers/text_to_text/dpo.py:128, ppo.py:338) given the d(logits) buffer of aa_linear_dlogits.  Same wgmma / TMA
