@@ -53,6 +53,10 @@ struct FusedActorParams {
   int W;
   float clip;
   int rx, rp;
+  // kind 0 objective (aa_logprob_actor_fused_obj; otherwise clip_hi = clip, dual = 0, agg = seq-mean-token-mean): clip
+  // range [1 - clip, 1 + clip_hi], dual-clip factor (0 = off) with `dual * adv` rounded to ra, loss aggregation
+  float clip_hi, dual;
+  int ra, agg;
   void *grad;
   int64_t grad_row_stride;
   int32_t *status;
@@ -69,8 +73,8 @@ struct FusedActorParams {
   const float *total;
   float *entropy;  // ENT kernels: fp32 entropy of every scored row at its log-prob's position (phase A)
   // EGRAD kernels (entropy bonus, loss - ent_coeff * mean entropy): the row's g_H = d loss / d H is
-  // kind 0: ent_seg[segment] (= -ent_coeff / (n_seg * mask count), the masked mean's coefficient, written by the prep
-  // kernel) for masked-in tokens; kind 2: -ent_coeff * g_rs (= -ent_coeff / counted tokens) for counted tokens
+  // kind 0: ent_seg[segment] (= -ent_coeff / (n_seg * mask count), the masked mean's coefficient, or -ent_coeff / total
+  // mask count under token-mean, written by the prep kernel) for masked-in tokens; kind 2: -ent_coeff * g_rs (= -ent_coeff / counted tokens) for counted tokens
   float ent_coeff;
   float *ent_seg;
 };
@@ -98,11 +102,15 @@ __global__ void __launch_bounds__(256) fused_actor_prep_kernel(const FusedActorP
   const int seg = blockIdx.y, tid = threadIdx.x;
   const int k = blockIdx.x * 256 + tid;
   float cnt = 0.f;
+  const bool token_mean = p.kind == 0 && p.agg == AA_AGG_TOKEN_MEAN;
   if (p.kind == 0) {
-    for (int t = tid; t < p.W; t += 256) cnt += p.mask[seg * p.mask_stride + t] ? 1.f : 0.f;
+    // token-mean: the mask count of the whole micro-batch (every block counts it; no host sync, no extra launch)
+    for (int k = token_mean ? 0 : seg; k < (token_mean ? p.map.n_seg : seg + 1); ++k)
+      for (int t = tid; t < p.W; t += 256) cnt += p.mask[k * p.mask_stride + t] ? 1.f : 0.f;
     cnt = block_sum<256>(cnt, scratch);
     if constexpr (EGRAD) {
-      if (blockIdx.x == 0 && tid == 0) p.ent_seg[seg] = -p.ent_coeff / (static_cast<float>(p.map.n_seg) * cnt);
+      if (blockIdx.x == 0 && tid == 0)
+        p.ent_seg[seg] = -p.ent_coeff / (token_mean ? cnt : static_cast<float>(p.map.n_seg) * cnt);
     }
   }
   if (k >= p.seq) return;
@@ -134,7 +142,7 @@ __global__ void __launch_bounds__(256) fused_actor_prep_kernel(const FusedActorP
       if (p.kind == 0) {
         r.old = load_as_float(p.old, seg * p.old_stride + j, p.out_dtype);
         r.adv = load_as_float(p.adv, seg * p.adv_stride + j, p.adv_dtype);
-        r.g_rs = actor_row_coeff(cnt, p.map.n_seg, p.rp);
+        r.g_rs = token_mean ? actor_token_mean_coeff(cnt, p.rp) : actor_row_coeff(cnt, p.map.n_seg, p.rp);
         r.on = p.mask[seg * p.mask_stride + j] ? 1 : 0;
       } else if (p.kind == 2) {
         r.old = load_as_float(p.old, seg * p.old_stride + j, p.out_dtype);
@@ -432,7 +440,10 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
           p.stat_logsum[flat] = logsum;
         }
         float obj, g = g_rs;  // cross-entropy: the same -loss_scale / n_valid for every scored row
-        if (p.kind == 0) actor_token(round_to(lp, p.out_dtype), old, adv, on, g_rs, p.clip, p.rx, p.rp, obj, g);
+        int why;
+        if (p.kind == 0)
+          actor_token(round_to(lp, p.out_dtype), old, adv, on, g_rs, p.clip, p.clip_hi, p.dual, p.rx, p.rp, p.ra, obj, g,
+                      why);
         if (p.kind == 2) grpo_token(round_to(lp, p.out_dtype), old, adv, on, g_rs, p.clip, p.rx, obj, g);
         sh_b[0] = m;
         sh_b[1] = logsum;
@@ -659,9 +670,9 @@ static int logprob_actor_fused(const char *who, float *entropy, float entropy_co
                                const int64_t *seg_cum, const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs,
                                int lp_dtype, float *stat_max, float *stat_logsum, const void *old_log_probs,
                                int64_t old_stride, const void *advantages, int64_t adv_stride, int adv_dtype,
-                               const uint8_t *mask, int64_t mask_stride, int32_t W, float clip_range_ratio, int mode,
-                               void *grad_logits, int64_t grad_row_stride, void *row_scratch, int32_t *status,
-                               void *stream) {
+                               const uint8_t *mask, int64_t mask_stride, int32_t W, float clip_low, float clip_high,
+                               float dual_clip, int loss_agg, int mode, void *grad_logits, int64_t grad_row_stride,
+                               void *row_scratch, int32_t *status, void *stream) {
   AA_REQUIRE(V > 0 && n_segments > 0 && W > 0 && n_tile_rows > 0 && n_tile_rows % n_segments == 0, AA_ERR_ARG,
              "%s: bad sizes (the gradient tile holds n_tile_rows / n_segments rows per sample)", who);
   AA_REQUIRE(logits && labels && seg_logit_off && seg_label_off && seg_out_off && seg_cum && seg_tile_row && log_probs &&
@@ -691,9 +702,13 @@ static int logprob_actor_fused(const char *who, float *entropy, float entropy_co
   p.mask = mask;
   p.mask_stride = mask_stride;
   p.W = W;
-  p.clip = clip_range_ratio;
+  p.clip = clip_low;
+  p.clip_hi = clip_high;
+  p.dual = dual_clip;
+  p.agg = loss_agg;
   p.rx = f ? lp_dtype : AA_F32;
   p.rp = f ? promote_dt(lp_dtype, adv_dtype) : AA_F32;
+  p.ra = f ? adv_dtype : AA_F32;
   FusedRec *rec = static_cast<FusedRec *>(row_scratch);
   if (entropy) {
     p.entropy = entropy;
@@ -714,8 +729,8 @@ extern "C" int aa_logprob_actor_fused(const void *logits, int logits_dtype, int6
   return logprob_actor_fused("aa_logprob_actor_fused", nullptr, 0.f, logits, logits_dtype, row_stride, V, labels, n_segments, seg_logit_off,
                              seg_label_off, seg_out_off, seg_cum, seg_tile_row, n_tile_rows, log_probs, lp_dtype,
                              stat_max, stat_logsum, old_log_probs, old_stride, advantages, adv_stride, adv_dtype, mask,
-                             mask_stride, W, clip_range_ratio, mode, grad_logits, grad_row_stride, row_scratch, status,
-                             stream);
+                             mask_stride, W, clip_range_ratio, clip_range_ratio, 0.f, AA_AGG_SEQ_MEAN_TOKEN_MEAN, mode,
+                             grad_logits, grad_row_stride, row_scratch, status, stream);
 }
 
 extern "C" int aa_logprob_actor_fused_entropy(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
@@ -733,8 +748,29 @@ extern "C" int aa_logprob_actor_fused_entropy(const void *logits, int logits_dty
   return logprob_actor_fused("aa_logprob_actor_fused_entropy", entropy, entropy_coeff, logits, logits_dtype, row_stride, V, labels, n_segments,
                              seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row, n_tile_rows, log_probs,
                              lp_dtype, stat_max, stat_logsum, old_log_probs, old_stride, advantages, adv_stride,
-                             adv_dtype, mask, mask_stride, W, clip_range_ratio, mode, grad_logits, grad_row_stride,
-                             row_scratch, status, stream);
+                             adv_dtype, mask, mask_stride, W, clip_range_ratio, clip_range_ratio, 0.f,
+                             AA_AGG_SEQ_MEAN_TOKEN_MEAN, mode, grad_logits, grad_row_stride, row_scratch, status, stream);
+}
+
+extern "C" int aa_logprob_actor_fused_obj(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                          const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                          const int64_t *seg_label_off, const int64_t *seg_out_off,
+                                          const int64_t *seg_cum, const int64_t *seg_tile_row, int64_t n_tile_rows,
+                                          void *log_probs, int lp_dtype, float *stat_max, float *stat_logsum,
+                                          const void *old_log_probs, int64_t old_stride, const void *advantages,
+                                          int64_t adv_stride, int adv_dtype, const uint8_t *mask, int64_t mask_stride,
+                                          int32_t W, float clip_low, float clip_high, float dual_clip, int loss_agg,
+                                          int mode, void *grad_logits, int64_t grad_row_stride, void *row_scratch,
+                                          int32_t *status, float entropy_coeff, float *entropy, void *stream) {
+  AA_REQUIRE(actor_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
+             "aa_logprob_actor_fused_obj: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a "
+             "known loss_agg; got %g %g %g %d)", clip_low, clip_high, dual_clip, loss_agg);
+  AA_REQUIRE(entropy_coeff == entropy_coeff, AA_ERR_ARG, "aa_logprob_actor_fused_obj: entropy_coeff is NaN");
+  return logprob_actor_fused("aa_logprob_actor_fused_obj", entropy, entropy_coeff, logits, logits_dtype, row_stride, V,
+                             labels, n_segments, seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row,
+                             n_tile_rows, log_probs, lp_dtype, stat_max, stat_logsum, old_log_probs, old_stride,
+                             advantages, adv_stride, adv_dtype, mask, mask_stride, W, clip_low, clip_high, dual_clip,
+                             loss_agg, mode, grad_logits, grad_row_stride, row_scratch, status, stream);
 }
 
 extern "C" int aa_logprob_ce_fused(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,

@@ -379,6 +379,11 @@ struct LossParams {
   uint32_t *counter;
   const int32_t *x_lens;  // optional: x[b, t] = t < R_b ? src[b, x_width - R_b + t] : 0, R_b = clamp(lens[b], 0, x_width)
   int x_width;            // (the pad_sequence of per-sample tails of text_image_to_text/ppo.py:318-330 folded into the load)
+  // actor objective (aa_ppo_actor_loss_obj; aa_ppo_actor_loss: clip_hi = clip, dual = 0, agg = seq-mean-token-mean):
+  // clip range [1 - clip, 1 + clip_hi], dual-clip factor (0 = off), `dual * adv` rounded to r_a, loss aggregation
+  float clip_hi, dual;
+  int r_a, agg;
+  float *clip_frac;  // optional fp32[2]: clipped fraction, dual-clip fraction (row_scratch then holds 4 * B floats)
 };
 
 template <int THREADS, bool ACTOR>
@@ -394,12 +399,20 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
   float cnt = 0.f;
   for (int t = tid; t < Wm; t += THREADS) cnt += mrow[t] ? 1.f : 0.f;
   cnt = block_sum<THREADS>(cnt, scratch);
+  const bool token_mean = ACTOR && p.agg == AA_AGG_TOKEN_MEAN;
+  float total = 0.f;  // token-mean: the micro-batch's masked-in token count (every block counts the whole mask)
+  if (token_mean) {
+    for (int k = 0; k < p.B; ++k)
+      for (int t = tid; t < Wm; t += THREADS) total += p.mask[k * p.mask_stride + t] ? 1.f : 0.f;
+    total = block_sum<THREADS>(total, scratch);
+  }
 
-  // upstream coefficient of d loss / d (row sum):  actor: -(1/B)/cnt ; critic: 0.5*(1/B)/cnt
-  const float g_rs = ACTOR ? actor_row_coeff(cnt, p.B, rp)
+  // upstream coefficient of d loss / d (row sum):  actor: -(1/B)/cnt (token-mean: -1/total) ; critic: 0.5*(1/B)/cnt
+  const float g_rs = ACTOR ? (token_mean ? actor_token_mean_coeff(total, rp) : actor_row_coeff(cnt, p.B, rp))
                            : round_to(round_to(round_to(0.5f, rp) / static_cast<float>(p.B), rp) / cnt, rp);
 
   float row_sum = 0.f, x_sum = 0.f;
+  float n_clip = 0.f, n_dual = 0.f, n_neg = 0.f;  // clip-fraction counters of the row's masked-in tokens
   for (int t = tid; t < Wm; t += THREADS) {
     const bool on = mrow[t] != 0;
     const float x = (t < x_rows) ? load_as_float(p.x, xo + x_shift + t, p.x_dtype) : 0.f;
@@ -407,7 +420,13 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
     const float aux = load_as_float(p.aux, ao + t, p.aux_dtype);
     float obj, grad;
     if (ACTOR) {
-      actor_token(x, old, aux, on, g_rs, p.clip, rx, rp, obj, grad);
+      int why;
+      actor_token(x, old, aux, on, g_rs, p.clip, p.clip_hi, p.dual, rx, rp, p.r_a, obj, grad, why);
+      if (on) {
+        n_clip += (why & 1) ? 1.f : 0.f;
+        n_dual += (why & 2) ? 1.f : 0.f;
+        n_neg += (aux < 0.f) ? 1.f : 0.f;
+      }
     } else {
       const float lo = round_to(old - p.clip, rx), hi = round_to(old + p.clip, rx);
       const float vc = fminf(fmaxf(x, lo), hi);
@@ -434,19 +453,50 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
     }
     if (p.grad) store_from_float(p.grad, b * p.grad_stride + t, p.x_dtype, on ? grad : 0.f);
   }
-  row_sum = round_to(block_sum<THREADS>(row_sum, scratch), rp);
+  row_sum = block_sum<THREADS>(row_sum, scratch);
   x_sum = block_sum<THREADS>(x_sum, scratch);
+  const bool fracs = ACTOR && p.clip_frac;
+  if (fracs) {
+    n_clip = block_sum<THREADS>(n_clip, scratch);
+    n_dual = block_sum<THREADS>(n_dual, scratch);
+    n_neg = block_sum<THREADS>(n_neg, scratch);
+  }
   if (tid == 0) {
-    p.row_scratch[b] = round_to(row_sum / cnt, rp);
+    // seq-mean-token-mean: the row's masked mean in the promoted dtype; token-mean: the row's fp32 sum (rounded once,
+    // after the cross-row sum, as ATen's sum over the whole tensor does)
+    p.row_scratch[b] = token_mean ? row_sum : round_to(round_to(row_sum, rp) / cnt, rp);
     if (p.row_mean) p.row_mean[b] = x_sum / cnt;
+    if (fracs) {  // the counters reduced like the loss: per-row fractions (seq-mean) or raw counts (token-mean)
+      const float d = token_mean ? 1.f : cnt;
+      p.row_scratch[p.B + b] = n_clip / d;
+      p.row_scratch[2 * p.B + b] = n_dual / d;
+      p.row_scratch[3 * p.B + b] = n_neg / d;
+    }
   }
   if (!last_block_arrives(p.counter, gridDim.x)) return;
   const volatile float *rows = p.row_scratch;
   float acc = 0.f;
   for (int k = tid; k < p.B; k += THREADS) acc += rows[k];
   acc = block_sum<THREADS>(acc, scratch);
+  if (fracs) {
+    float fc = 0.f, fd = 0.f, fn = 0.f;
+    for (int k = tid; k < p.B; k += THREADS) {
+      fc += rows[p.B + k];
+      fd += rows[2 * p.B + k];
+      fn += rows[3 * p.B + k];
+    }
+    fc = block_sum<THREADS>(fc, scratch);
+    fd = block_sum<THREADS>(fd, scratch);
+    fn = block_sum<THREADS>(fn, scratch);
+    if (tid == 0) {
+      // clipped: the masked mean of the indicator; dual: the share of negative-advantage tokens where c * adv wins
+      // (the ratio of the two indicators' masked means; 0 without such tokens)
+      p.clip_frac[0] = fc / (token_mean ? total : static_cast<float>(p.B));
+      p.clip_frac[1] = fn > 0.f ? fd / fn : 0.f;
+    }
+  }
   if (tid == 0) {
-    const float mm = round_to(acc / static_cast<float>(p.B), rp);
+    const float mm = token_mean ? round_to(round_to(acc, rp) / total, rp) : round_to(acc / static_cast<float>(p.B), rp);
     const float loss = ACTOR ? -mm : round_to(0.5f * mm, rp);
     p.loss[0] = loss;
     // the same value as a 16-bit scalar in the first two bytes of loss[1]: the caller views it as the 0-dim bf16 / f16
@@ -726,21 +776,47 @@ extern "C" int aa_ppo_returns(const void *rewards, int rew_dtype, int64_t rew_ro
 
 static int promote(int a, int b) { return (a == b) ? a : AA_F32; }
 
+static int ppo_actor_loss(const char *who, const void *log_probs, int64_t lp_stride, const void *old_log_probs,
+                          int64_t old_stride, int lp_dtype, const void *advantages, int64_t adv_stride, int adv_dtype,
+                          const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t Wm, float clip_low,
+                          float clip_high, float dual_clip, int loss_agg, int mode, float *loss, void *grad,
+                          int64_t grad_stride, float *clip_frac, float *row_scratch, uint32_t *counter, void *stream) {
+  AA_REQUIRE(B > 0 && Wm > 0, AA_ERR_ARG, "%s: bad sizes", who);
+  AA_REQUIRE(log_probs && old_log_probs && advantages && mask && loss && row_scratch && counter, AA_ERR_ARG,
+             "%s: null pointer", who);
+  AA_REQUIRE(dtype_ok(lp_dtype) && dtype_ok(adv_dtype), AA_ERR_DTYPE, "%s: bad dtype", who);
+  const bool f = (mode == AA_MODE_FAITHFUL);
+  LossParams p{log_probs, lp_stride, old_log_probs, old_stride, lp_dtype, advantages, adv_stride, adv_dtype,
+               mask, mask_stride, B, Wm, clip_low, f ? lp_dtype : AA_F32,
+               f ? promote(lp_dtype, adv_dtype) : AA_F32, loss, grad, grad_stride, nullptr, row_scratch, counter, nullptr, 0,
+               clip_high, dual_clip, f ? adv_dtype : AA_F32, loss_agg, clip_frac};
+  ppo_loss_kernel<128, true><<<B, 128, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch(who);
+}
+
 extern "C" int aa_ppo_actor_loss(const void *log_probs, int64_t lp_stride, const void *old_log_probs,
                                  int64_t old_stride, int lp_dtype, const void *advantages, int64_t adv_stride,
                                  int adv_dtype, const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t Wm,
                                  float clip_range_ratio, int mode, float *loss, void *grad, int64_t grad_stride,
                                  float *row_scratch, uint32_t *counter, void *stream) {
-  AA_REQUIRE(B > 0 && Wm > 0, AA_ERR_ARG, "aa_ppo_actor_loss: bad sizes");
-  AA_REQUIRE(log_probs && old_log_probs && advantages && mask && loss && row_scratch && counter, AA_ERR_ARG,
-             "aa_ppo_actor_loss: null pointer");
-  AA_REQUIRE(dtype_ok(lp_dtype) && dtype_ok(adv_dtype), AA_ERR_DTYPE, "aa_ppo_actor_loss: bad dtype");
-  const bool f = (mode == AA_MODE_FAITHFUL);
-  LossParams p{log_probs, lp_stride, old_log_probs, old_stride, lp_dtype, advantages, adv_stride, adv_dtype,
-               mask, mask_stride, B, Wm, clip_range_ratio, f ? lp_dtype : AA_F32,
-               f ? promote(lp_dtype, adv_dtype) : AA_F32, loss, grad, grad_stride, nullptr, row_scratch, counter, nullptr, 0};
-  ppo_loss_kernel<128, true><<<B, 128, 0, static_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("aa_ppo_actor_loss");
+  return ppo_actor_loss("aa_ppo_actor_loss", log_probs, lp_stride, old_log_probs, old_stride, lp_dtype, advantages,
+                        adv_stride, adv_dtype, mask, mask_stride, B, Wm, clip_range_ratio, clip_range_ratio, 0.f,
+                        AA_AGG_SEQ_MEAN_TOKEN_MEAN, mode, loss, grad, grad_stride, nullptr, row_scratch, counter, stream);
+}
+
+extern "C" int aa_ppo_actor_loss_obj(const void *log_probs, int64_t lp_stride, const void *old_log_probs,
+                                     int64_t old_stride, int lp_dtype, const void *advantages, int64_t adv_stride,
+                                     int adv_dtype, const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t Wm,
+                                     float clip_low, float clip_high, float dual_clip, int loss_agg, int mode,
+                                     float *loss, void *grad, int64_t grad_stride, float *clip_frac, float *row_scratch,
+                                     uint32_t *counter, void *stream) {
+  AA_REQUIRE(actor_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
+             "aa_ppo_actor_loss_obj: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a known "
+             "loss_agg; got %g %g %g %d)", clip_low, clip_high, dual_clip, loss_agg);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_ppo_actor_loss_obj: bad mode");
+  return ppo_actor_loss("aa_ppo_actor_loss_obj", log_probs, lp_stride, old_log_probs, old_stride, lp_dtype, advantages,
+                        adv_stride, adv_dtype, mask, mask_stride, B, Wm, clip_low, clip_high, dual_clip, loss_agg, mode,
+                        loss, grad, grad_stride, clip_frac, row_scratch, counter, stream);
 }
 
 extern "C" int aa_ppo_critic_loss(const void *values, int64_t val_stride, const void *old_values,

@@ -16,29 +16,58 @@ __device__ __forceinline__ float actor_row_coeff(float cnt, int B, int rp) {
   return round_to(g_q / cnt, rp);
 }
 
+// upstream coefficient under token-mean aggregation, -(s * mask).sum() / mask.sum():  -1 / total (DivBackward's
+// rounding), total = the micro-batch's masked-in token count
+__device__ __forceinline__ float actor_token_mean_coeff(float total, int rp) { return round_to(-1.f / total, rp); }
+
+// the argument check of the objective entry points (ops.ActorObjective checks the same on the host)
+inline bool actor_objective_ok(float clip_low, float clip_high, float dual_clip, int loss_agg) {
+  return clip_low >= 0.f && clip_low < 1.f && clip_high >= 0.f && (dual_clip == 0.f || dual_clip > 1.f) &&
+         (loss_agg == AA_AGG_SEQ_MEAN_TOKEN_MEAN || loss_agg == AA_AGG_TOKEN_MEAN);
+}
+
 // One token of the clipped-ratio objective.  x / old: new / old log-prob (dtype code rx), aux: advantage,
-// on: the mask bit, g_rs: actor_row_coeff of the token's row.
+// on: the mask bit, g_rs: d loss / d (the token's objective) for a masked-in token (actor_row_coeff or
+// actor_token_mean_coeff).  eps_lo / eps_hi: the clip range [1 - eps_lo, 1 + eps_hi]; dual: the dual-clip factor c
+// (0 = off), ra: the rounding code of `c * adv` (the advantages' dtype).
 //   obj  = min(adv * ratio, adv * clip(ratio))     (the NEGATED loss term; NaN-propagating like torch.minimum)
+//          dual-clip, adv < 0:  max(obj, c * adv)  (torch.where(adv < 0, torch.maximum(obj, c * adv), obj))
 //   grad = d loss / d x                            (0 when the mask is off)
-__device__ __forceinline__ void actor_token(float x, float old, float aux, bool on, float g_rs, float clip, int rx,
-                                            int rp, float &obj, float &grad) {
-  const float lo = round_to(1.f - clip, rx), hi = round_to(1.f + clip, rx);
+//   why  = bit 0: the clipped branch is strictly smaller; bit 1: c * adv wins (the clip-fraction counters)
+__device__ __forceinline__ void actor_token(float x, float old, float aux, bool on, float g_rs, float eps_lo,
+                                            float eps_hi, float dual, int rx, int rp, int ra, float &obj, float &grad,
+                                            int &why) {
+  const float lo = round_to(1.f - eps_lo, rx), hi = round_to(1.f + eps_hi, rx);
   const float ratio = round_to(expf(round_to(x - old, rx)), rx);
   const float s1 = round_to(aux * ratio, rp);
   const float clipped = fminf(fmaxf(ratio, lo), hi);
   const float s2 = round_to(aux * clipped, rp);
   obj = fminf(s1, s2);
   if (s1 != s1 || s2 != s2) obj = NAN;
+  why = (s2 < s1) ? 1 : 0;
+  float g = g_rs;  // gradient reaching min(s1, s2)
+  if (dual != 0.f && aux < 0.f) {
+    // maximum's backward: all to the larger input, round(grad / 2) to each on a tie; the c * adv branch does not
+    // reach the ratio
+    const float ca = round_to(dual * aux, ra);
+    if (obj < ca) {
+      g = 0.f;
+      why |= 2;
+    } else if (obj == ca) {
+      g = round_to(0.5f * g_rs, rp);
+    }
+    if (obj == obj) obj = fmaxf(obj, ca);
+  }
   const bool in_range = (ratio >= lo) && (ratio <= hi);
   float gs = 0.f;  // gradient reaching `ratio` through both branches of torch.minimum
   if (on) {
     if (s1 < s2) {
-      gs = round_to(round_to(g_rs * aux, rp), rx);
+      gs = round_to(round_to(g * aux, rp), rx);
     } else if (s1 == s2) {
       // a tie: minimum's backward sends round(grad / 2) down each branch; through the clamp only in range, and the
-      // ratio's gradient is the sum of the two (rounded at each step: the halves differ from g_rs * aux / 2 once they
+      // ratio's gradient is the sum of the two (rounded at each step: the halves differ from g * aux / 2 once they
       // are fp16 subnormals)
-      const float half = round_to(round_to(round_to(0.5f * g_rs, rp) * aux, rp), rx);
+      const float half = round_to(round_to(round_to(0.5f * g, rp) * aux, rp), rx);
       gs = in_range ? round_to(half + half, rx) : half;
     }
     // s1 > s2: the clipped branch wins and clamp's backward is zero outside the range

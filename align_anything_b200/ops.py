@@ -11,7 +11,9 @@ plumbing only; all arithmetic on the path runs in the hand-written sm_90a kernel
 """
 from __future__ import annotations
 
+import dataclasses
 import functools
+import math
 from typing import Sequence
 
 import torch
@@ -24,7 +26,7 @@ __all__ = [
     'move_padding_left', 'count_nonpad', 'strip_pad_tail', 'ppo_pack_metrics', 'check_status', 'raise_for_status', 'status_lane', 'causal_lm_loss', 'rm_pair_loss', 'cost_pair_loss','group_advantages', 'grpo_loss', 'tail_token_log_probs', 'pair_slices', 'slice_sums', 'tail_rows', 'linear_token_log_probs',
     'sequence_log_probs_from_hidden', 'fused_linear_token_log_probs', 'tail_log_probs_from_hidden', 'dense_log_probs_from_hidden', 'tail_actor_loss', 'tail_critic_loss', 'lm_head_weight',
     'causal_lm_loss_from_hidden', 'causal_lm_valid_rows', 'gather_log_probabilities_with_entropy',
-    'response_tail_log_probs_pair_with_entropy',
+    'response_tail_log_probs_pair_with_entropy', 'ActorObjective', 'token_mean',
 ]
 
 # Path knobs: plain module attributes, read at call time and never from the environment.  Every path is chosen from the
@@ -1915,9 +1917,77 @@ def estimator_returns(rewards, sequence_mask, start: int, estimator: str, n_samp
     return adv, ret
 
 
-def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=None):
+LOSS_AGG_MODES = {'seq-mean-token-mean': 0, 'token-mean': 1}  # include/aa_b200.h AA_AGG_*
+
+
+@dataclasses.dataclass(frozen=True)
+class ActorObjective:
+    """The PPO actor's clipped-ratio objective (the reference's actor_loss_fn, trainers/text_to_text/ppo.py:291-307,
+    when every field is at its default):
+
+        ratio = exp(lp - old_lp) ;  s = min(A * ratio, A * clamp(ratio, 1 - clip_range_ratio_low, 1 + clip_range_ratio_high))
+        dual-clip:  s = where(A < 0, max(s, dual_clip_ratio * A), s)
+        loss = -masked_mean(s, mask)                (loss_agg_mode 'seq-mean-token-mean': mean of per-sample means)
+             = -(s * mask).sum() / mask.sum()       ('token-mean': mean over the micro-batch's response tokens)
+
+    clip_range_ratio_low / _high: None takes the trainer's clip_range_ratio (clip-higher: high > low); dual_clip_ratio:
+    None = off, otherwise c > 1.  The fields are checked here, on the host, before anything is launched."""
+
+    clip_range_ratio_low: float | None = None
+    clip_range_ratio_high: float | None = None
+    dual_clip_ratio: float | None = None
+    loss_agg_mode: str = 'seq-mean-token-mean'
+
+    def __post_init__(self):
+        lo, hi, c = self.clip_range_ratio_low, self.clip_range_ratio_high, self.dual_clip_ratio
+        if lo is not None and not (0.0 <= float(lo) < 1.0):
+            raise ValueError(f'clip_range_ratio_low must be in [0, 1), got {lo!r}')
+        if hi is not None and not (float(hi) >= 0.0):
+            raise ValueError(f'clip_range_ratio_high must be >= 0, got {hi!r}')
+        if c is not None and not (float(c) > 1.0 and math.isfinite(float(c))):
+            raise ValueError(f'dual_clip_ratio must be None (off) or a finite value > 1, got {c!r}')
+        if self.loss_agg_mode not in LOSS_AGG_MODES:
+            raise ValueError(f'loss_agg_mode must be one of {sorted(LOSS_AGG_MODES)}, got {self.loss_agg_mode!r}')
+
+    @property
+    def is_default(self) -> bool:
+        """The reference's objective: the kernels run today's launches."""
+        return (self.clip_range_ratio_low is None and self.clip_range_ratio_high is None and self.dual_clip_ratio is None
+                and self.loss_agg_mode == 'seq-mean-token-mean')
+
+    @property
+    def token_mean(self) -> bool:
+        return self.loss_agg_mode == 'token-mean'
+
+    def args(self, clip_range_ratio: float) -> tuple[float, float, float, int]:
+        """-> (clip_low, clip_high, dual_clip (0 = off), loss_agg code) of the C entry points."""
+        lo = float(clip_range_ratio if self.clip_range_ratio_low is None else self.clip_range_ratio_low)
+        hi = float(clip_range_ratio if self.clip_range_ratio_high is None else self.clip_range_ratio_high)
+        if not (0.0 <= lo < 1.0 and hi >= 0.0):
+            raise ValueError(f'clip range [1 - {lo}, 1 + {hi}]: need 0 <= low < 1 and high >= 0')
+        return lo, hi, float(self.dual_clip_ratio or 0.0), LOSS_AGG_MODES[self.loss_agg_mode]
+
+
+def _objective(objective: ActorObjective | None) -> ActorObjective | None:
+    """None for the reference's objective (today's launches), else the objective."""
+    if objective is None:
+        return None
+    if not isinstance(objective, ActorObjective):
+        raise TypeError(f'objective must be an ops.ActorObjective, got {type(objective).__name__}')
+    return None if objective.is_default else objective
+
+
+def token_mean(x: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
+    """(x * mask).sum() / mask.sum() over the whole (B, W) tensor -> fp32 scalar (NaN without a masked-in token): the
+    masked_mean kernel on the tensor as one row, differentiable in x."""
+    return masked_mean(x.reshape(1, -1), mask.reshape(1, -1))
+
+
+def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=None, obj=None, clip_frac=None):
     """K5: -> (loss fp32[2], loss as a 0-dim tensor of the promoted dtype (a view, no launch), grad (B, Wm), row_mean).
-    x_tail = (DeviceLens, src_width): `x` is the raw (B, src_width) tensor and the kernel reads the per-sample tails."""
+    x_tail = (DeviceLens, src_width): `x` is the raw (B, src_width) tensor and the kernel reads the per-sample tails.
+    Actor only: obj = ActorObjective.args(...) (None: the reference's objective), clip_frac = an fp32[2] tensor the
+    kernel fills with the clip fractions (aa_ppo_actor_loss_obj)."""
     B, Wm = old.shape
     dev = x.device
     loss = torch.empty(2, dtype=torch.float32, device=dev)
@@ -1926,7 +1996,15 @@ def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=Non
     row_mean = torch.empty(B, dtype=torch.float32, device=dev)
     sc = _device_scratch(dev)
     lib = L.lib()
-    if actor:
+    if actor and (obj is not None or clip_frac is not None):
+        lo, hi, dual, agg = obj if obj is not None else (clip, clip, 0.0, 0)
+        rows = torch.empty(4 * B, dtype=torch.float32, device=dev)
+        L.check(lib.aa_ppo_actor_loss_obj(
+            x.data_ptr(), x.stride(0), old.data_ptr(), old.stride(0), L.dtype_code(x.dtype), aux.data_ptr(),
+            aux.stride(0), L.dtype_code(aux.dtype), mask.data_ptr(), mask.stride(0), B, Wm, float(lo), float(hi),
+            float(dual), int(agg), mode_code, loss.data_ptr(), grad.data_ptr(), grad.stride(0), L.ptr(clip_frac),
+            rows.data_ptr(), sc['counter'][2:3].data_ptr(), L.stream_ptr(dev)))
+    elif actor:
         L.check(lib.aa_ppo_actor_loss(
             x.data_ptr(), x.stride(0), old.data_ptr(), old.stride(0), L.dtype_code(x.dtype), aux.data_ptr(),
             aux.stride(0), L.dtype_code(aux.dtype), mask.data_ptr(), mask.stride(0), B, Wm, float(clip),
@@ -1948,8 +2026,9 @@ class _PpoLossFn(torch.autograd.Function):
     """K5: forward computes the loss AND d loss / d x in the same launch; backward scales it."""
 
     @staticmethod
-    def forward(ctx, x, old, aux, mask, clip, mode_code, actor: bool):
-        loss, cast, grad, row_mean = _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor)
+    def forward(ctx, x, old, aux, mask, clip, mode_code, actor: bool, obj=None, clip_frac=None):
+        loss, cast, grad, row_mean = _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor, obj=obj,
+                                                      clip_frac=clip_frac)
         ctx.save_for_backward(grad)
         ctx.mark_non_differentiable(row_mean, loss)
         return cast, row_mean, loss
@@ -1957,7 +2036,7 @@ class _PpoLossFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_loss, _g, _l):
         (grad,) = ctx.saved_tensors
-        return (grad.float() * g_loss.float()).to(grad.dtype), None, None, None, None, None, None
+        return (grad.float() * g_loss.float()).to(grad.dtype), None, None, None, None, None, None, None, None
 
 
 class _TailActorLossFn(torch.autograd.Function):
@@ -1974,15 +2053,22 @@ class _TailActorLossFn(torch.autograd.Function):
     entropy_coeff != 0 (entropy bonus): the node's loss is  actor_loss - entropy_coeff * masked_mean(H, mask)  and a
     fourth output, the detached masked-mean entropy, follows; the third stays the actor loss without the bonus.  K1f's
     entropy-gradient variant (aa_logprob_actor_fused_entropy), or K1's entropy variant + K5 + masked_mean and, in the
-    backward, K1b's entropy variant with g_H = -entropy_coeff * mask / (B * mask count of the row)."""
+    backward, K1b's entropy variant with g_H = -entropy_coeff * mask / (B * mask count of the row).
+    objective (a non-default ActorObjective): K1f's objective entry point (aa_logprob_actor_fused_obj) and K5's
+    (aa_ppo_actor_loss_obj); under token-mean the entropy term is a token mean too.  clip_frac: an fp32[2] tensor K5
+    fills with the clip fractions."""
 
     @staticmethod
-    def forward(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, single_pass, entropy_coeff=0.0):
+    def forward(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, single_pass, entropy_coeff=0.0, objective=None,
+                clip_frac=None):
         out_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         dev = logits.device
         lp = torch.zeros(plan.out_shape, dtype=out_dtype, device=dev)
         ctx.fused = bool(single_pass and plan.n_tile_rows > 0 and plan.n_seg > 0 and plan.n_tile_rows % plan.n_seg == 0
                          and len(plan.out_shape) == 2)
+        if objective is not None or clip_frac is not None:
+            return _TailActorLossFn._forward_objective(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, lp,
+                                                       float(entropy_coeff), objective, clip_frac)
         if entropy_coeff != 0.0:
             return _TailActorLossFn._forward_bonus(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, lp,
                                                    float(entropy_coeff))
@@ -2007,6 +2093,63 @@ class _TailActorLossFn(torch.autograd.Function):
             ctx.plan, ctx.mode_code = plan, mode_code
         ctx.mark_non_differentiable(lp, loss)
         return cast, lp, loss
+
+    @staticmethod
+    def _forward_objective(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, lp, coeff, objective, clip_frac):
+        """The node under an ActorObjective (None: the reference's objective, reached with clip_frac only)."""
+        dev = logits.device
+        obj = objective.args(clip) if objective is not None else None
+        tm = objective is not None and objective.token_mean
+        ctx.bonus = coeff != 0.0
+        ent = torch.zeros(plan.out_shape, dtype=torch.float32, device=dev) if ctx.bonus else None
+        if ctx.fused and obj is None:  # today's K1f launch (plain or entropy-bonus form)
+            grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
+            scratch = torch.empty(plan.n_tile_rows * 6 + (plan.n_seg + 1) // 2, dtype=torch.int64, device=dev)
+            p = plan.ptrs()
+            args = (logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), ids.data_ptr(),
+                    plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp.dtype),
+                    None, None, old.data_ptr(), old.stride(0), aux.data_ptr(), aux.stride(0), L.dtype_code(aux.dtype),
+                    mask.data_ptr(), mask.stride(0), lp.size(1), float(clip), mode_code, grad.data_ptr(),
+                    logits.size(-1), scratch.data_ptr(), _device_scratch(dev)['status'].data_ptr())
+            if ctx.bonus:
+                L.check(L.lib().aa_logprob_actor_fused_entropy(*args, coeff, ent.data_ptr(), L.stream_ptr(dev)))
+            else:
+                L.check(L.lib().aa_logprob_actor_fused(*args, L.stream_ptr(dev)))
+            ctx.save_for_backward(grad)
+        elif ctx.fused:
+            grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
+            # 48 bytes per tile row (the row records) + 4 per segment (the rows' g_H coefficients)
+            scratch = torch.empty(plan.n_tile_rows * 6 + (plan.n_seg + 1) // 2, dtype=torch.int64, device=dev)
+            p = plan.ptrs()
+            L.check(L.lib().aa_logprob_actor_fused_obj(
+                logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), ids.data_ptr(),
+                plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp.dtype),
+                None, None, old.data_ptr(), old.stride(0), aux.data_ptr(), aux.stride(0), L.dtype_code(aux.dtype),
+                mask.data_ptr(), mask.stride(0), lp.size(1), obj[0], obj[1], obj[2], obj[3], mode_code, grad.data_ptr(),
+                logits.size(-1), scratch.data_ptr(), _device_scratch(dev)['status'].data_ptr(), coeff, L.ptr(ent),
+                L.stream_ptr(dev)))
+            ctx.save_for_backward(grad)
+        else:
+            stats = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=dev)
+            _launch_fwd(logits, ids, plan, lp, stats[0], stats[1], entropy=ent)
+        loss, cast, grad_lp, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True, obj=obj, clip_frac=clip_frac)
+        if not ctx.fused:
+            if ctx.bonus:
+                # d (-coeff * mean(H)) / d H on masked-in tokens (0 elsewhere, as K1f forms it): the masked mean's
+                # coefficient, or -coeff / (masked-in tokens of the micro-batch) under token-mean
+                den = mask.sum().float() if tm else mask.size(0) * mask.sum(dim=-1, keepdim=True).float()
+                g_h = torch.where(mask, -coeff / den, 0.0)
+                ctx.save_for_backward(logits, ids, stats, grad_lp, ent, g_h)
+            else:
+                ctx.save_for_backward(logits, ids, stats, grad_lp)
+            ctx.plan, ctx.mode_code = plan, mode_code
+        if not ctx.bonus:
+            ctx.mark_non_differentiable(lp, loss)
+            return cast, lp, loss
+        h_mean = token_mean(ent, mask) if tm else masked_mean(ent, mask)
+        reg = loss[0] - coeff * h_mean
+        ctx.mark_non_differentiable(lp, loss, h_mean)
+        return reg, lp, loss, h_mean
 
     @staticmethod
     def _forward_bonus(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, lp, coeff):
@@ -2044,7 +2187,7 @@ class _TailActorLossFn(torch.autograd.Function):
     def backward(ctx, g_loss, *_unused):
         if ctx.fused:
             (grad,) = _hand_over_once(ctx, g_loss, *ctx.saved_tensors)
-            return grad, None, None, None, None, None, None, None, None, None
+            return grad, None, None, None, None, None, None, None, None, None, None, None
         scale = g_loss.detach().reshape(1)
         if scale.dtype not in (torch.float32, torch.bfloat16, torch.float16):
             scale = scale.float()
@@ -2056,7 +2199,7 @@ class _TailActorLossFn(torch.autograd.Function):
         grad = torch.empty(logits.shape, dtype=logits.dtype, device=logits.device)
         _launch_bwd(logits, ids, ctx.plan, stats[0], stats[1], grad_lp, None, scale, grad, ctx.mode_code, entropy=ent,
                     grad_entropy=g_h)
-        return grad, None, None, None, None, None, None, None, None, None
+        return grad, None, None, None, None, None, None, None, None, None, None, None
 
 
 class _TailCriticLossFn(torch.autograd.Function):
@@ -2104,11 +2247,20 @@ def _loss_inputs(x, old, aux, mask):
     return x, old, aux, mask
 
 
-def actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio: float, mode: str | None = None):
-    """PPOTrainer.actor_loss_fn (trainers/text_to_text/ppo.py:291-307), differentiable in log_probs."""
+def actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio: float, mode: str | None = None,
+               objective: ActorObjective | None = None, return_clip_fraction: bool = False):
+    """PPOTrainer.actor_loss_fn (trainers/text_to_text/ppo.py:291-307), differentiable in log_probs.
+    objective: an ActorObjective (None: the reference's).  return_clip_fraction: -> (loss, fp32[2] device tensor: the
+    clipped fraction and the dual-clip fraction, aggregated like the loss; see aa_ppo_actor_loss_obj)."""
+    objective = _objective(objective)
     x, old, aux, m = _loss_inputs(log_probs, old_log_probs, advantages, mask)
-    loss, _, _ = _PpoLossFn.apply(x, old, aux, m, clip_range_ratio, _mode_code(mode, x.dtype), True)
-    return loss
+    obj = objective.args(clip_range_ratio) if objective is not None else None
+    if obj is None and not return_clip_fraction:
+        loss, _, _ = _PpoLossFn.apply(x, old, aux, m, clip_range_ratio, _mode_code(mode, x.dtype), True)
+        return loss
+    cf = torch.zeros(2, dtype=torch.float32, device=x.device) if return_clip_fraction else None
+    loss, _, _ = _PpoLossFn.apply(x, old, aux, m, clip_range_ratio, _mode_code(mode, x.dtype), True, obj, cf)
+    return (loss, cf) if return_clip_fraction else loss
 
 
 def critic_loss(values, old_values, returns, mask, clip_range_value: float, mode: str | None = None,
@@ -2120,11 +2272,15 @@ def critic_loss(values, old_values, returns, mask, clip_range_value: float, mode
 
 
 def tail_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, lens, old_log_probs, advantages, mask,
-                    clip_range_ratio: float, mode: str | None = None, entropy_coeff: float = 0.0):
+                    clip_range_ratio: float, mode: str | None = None, entropy_coeff: float = 0.0,
+                    objective: ActorObjective | None = None, return_clip_fraction: bool = False):
     """response_tail_log_probs + actor_loss as one autograd node (see _TailActorLossFn).
     -> (actor loss, new log-probs (B, W), the loss as fp32[2] for ppo_pack_metrics).  entropy_coeff != 0: the first
     output is  actor_loss - entropy_coeff * masked_mean(H, mask)  (fp32), the third stays the actor loss without the
-    bonus, and the detached masked-mean entropy follows as a fourth."""
+    bonus, and the detached masked-mean entropy follows as a fourth.  objective: an ActorObjective (None: the
+    reference's; under token-mean the entropy term is a token mean too).  return_clip_fraction: the fp32[2] clip
+    fractions (see actor_loss) follow as the last output."""
+    objective = _objective(objective)
     L.require_cuda(logits, input_ids, old_log_probs, advantages, mask)
     lens = as_device_lens(lens, logits.device)
     B, K, _ = logits.shape
@@ -2142,6 +2298,13 @@ def tail_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, lens, old_log
     m = _contiguous_last(mask.to(torch.bool))
     plan = device_tail_plan(lens, K, logits.stride(0), logits.stride(1), ids.stride(0), ids.size(1), 0, -1, lens.bound)
     single_pass = _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad)
+    if objective is not None or return_clip_fraction:
+        if objective is not None:
+            objective.args(clip_range_ratio)  # a bad clip range fails here, before any launch
+        cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
+        out = _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass,
+                                     float(entropy_coeff), objective, cf)
+        return (*out, cf) if return_clip_fraction else out
     if entropy_coeff != 0.0:
         return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass,
                                       float(entropy_coeff))
@@ -2158,7 +2321,8 @@ def _dense_actor_plan(B: int, L: int, start: int, sb: int, sl: int, lab_sb: int,
 
 
 def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, old_log_probs, advantages, mask,
-                     clip_range_ratio: float, mode: str | None = None, entropy_coeff: float = 0.0):
+                     clip_range_ratio: float, mode: str | None = None, entropy_coeff: float = 0.0,
+                     objective: ActorObjective | None = None, return_clip_fraction: bool = False):
     """The actor half of the text rl_step (trainers/text_to_text/ppo.py:336-349) as one autograd node:
     `gather_log_probabilities(logits[:, :-1], ids[:, 1:])[:, start:]` -> `actor_loss_fn` -> backward up to d logits.
     Only the rows `[start, L - 1)` are read (the reference scores every position and slices afterwards); with a
@@ -2168,7 +2332,8 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
     entropy_coeff != 0 (entropy bonus): the first output is  actor_loss - entropy_coeff * masked_mean(H, mask)  (fp32),
     the third stays the actor loss without the bonus and the detached masked-mean entropy follows as a fourth; the
     single pass is K1f's entropy-gradient variant, the composed path K1's entropy variant -> K5 + masked_mean -> K1b's
-    entropy variant."""
+    entropy variant.  objective / return_clip_fraction: as tail_actor_loss (the clip fractions are the last output)."""
+    objective = _objective(objective)
     L.require_cuda(logits, input_ids, old_log_probs, advantages, mask)
     if logits.dim() != 3 or input_ids.shape != logits.shape[:2]:
         raise ValueError('expected logits (B, L, V) and input_ids (B, L)')
@@ -2179,6 +2344,27 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
         raise ValueError(f'start = {start} leaves no scored position in a sequence of {Lq}')
     if not (tuple(old_log_probs.shape) == tuple(advantages.shape) == tuple(mask.shape) == (B, W)):
         raise ValueError('old_log_probs, advantages and mask must all be (B, L - 1 - start)')
+    if objective is not None:
+        objective.args(clip_range_ratio)  # a bad clip range fails here, before any launch
+    extended = objective is not None or return_clip_fraction
+    if not _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad) and extended:
+        # the composed ops below with the objective: K5 takes it, K1 / K1b are unchanged
+        kw = dict(mode=mode, objective=objective, return_clip_fraction=return_clip_fraction)
+        cf = ()
+        if entropy_coeff != 0.0:
+            lp, ent = gather_log_probabilities_with_entropy(logits[:, start:-1], input_ids[:, start + 1:], mode=mode,
+                                                            entropy_grad=True)
+            loss = actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, **kw)
+            if return_clip_fraction:
+                loss, cf = loss[0], (loss[1],)
+            m = mask.to(torch.bool)
+            h_mean = token_mean(ent, m) if objective is not None and objective.token_mean else masked_mean(ent, m)
+            return (loss - float(entropy_coeff) * h_mean, lp.detach(), loss, h_mean.detach(), *cf)
+        lp = gather_log_probabilities(logits[:, start:-1], input_ids[:, start + 1:], mode=mode)
+        loss = actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, **kw)
+        if return_clip_fraction:
+            loss, cf = loss[0], (loss[1],)
+        return (loss, lp.detach(), loss, *cf)
     if not _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad):
         # short rows, fp16, no gradient: the composed ops (K1 over the response rows -> K5; backward K1b)
         if entropy_coeff != 0.0:
@@ -2201,6 +2387,11 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
         aux = aux.float()
     m = _contiguous_last(mask.to(torch.bool))
     plan = _dense_actor_plan(B, Lq, start, logits.stride(0), logits.stride(1), ids.stride(0), str(logits.device))
+    if extended:
+        cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
+        out = _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, True,
+                                     float(entropy_coeff), objective, cf)
+        return (*out, cf) if return_clip_fraction else out
     if entropy_coeff != 0.0:
         return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, True,
                                       float(entropy_coeff))

@@ -15,7 +15,8 @@ import torch
 
 from ... import ops
 from ...utils.multi_process import all_reduce_packed, fused_allreduce
-from ..text_to_text.ppo import METRIC_KEYS, entropy_coeff_of, with_bonus_lane, with_entropy_lane
+from ..text_to_text.ppo import (METRIC_KEYS, clip_metrics, entropy_coeff_of, objective_kwargs, with_bonus_lane,
+                                with_clip_lanes, with_entropy_lane)
 from ..text_to_text.ppo import PPOTrainer as _TextPPOTrainer
 
 __all__ = ['PPOTrainer', 'move_padding_left']
@@ -160,29 +161,35 @@ class PPOTrainer(_TextPPOTrainer):
         # actor: K1 over the response tails + K5 as ONE autograd node; its backward is K1b alone (:296-316)
         batch = self.infer_batch(inference_batch)
         coeff = entropy_coeff_of(self)  # entropy bonus over the response tails (the actor loss's rows and mask)
-        entropy_mean = None
-        if self.fused_lm_head and coeff != 0.0:  # K6's entropy variant; K6b adds the entropy's gradient in its epilogue
-            log_probs, ent = self._tail_log_probs(self.actor_model, batch, lens, input_ids, return_entropy=True,
-                                                  entropy_grad=True, use_cache=False)
-            actor_loss32 = ops.actor_loss(log_probs, old_log_probs, reward_advantages, sequence_mask,
-                                          self.clip_range_ratio, mode=self.mode)
-            entropy_mean = ops.masked_mean(ent, sequence_mask)
-            actor_loss = actor_loss32 - coeff * entropy_mean
-            entropy_mean = entropy_mean.detach()
-        elif self.fused_lm_head:
-            log_probs = self._tail_log_probs(self.actor_model, batch, lens, input_ids, use_cache=False)
+        kw = objective_kwargs(self)  # the actor objective switches (empty: the reference's objective)
+        entropy_mean = clip_frac = None
+        if self.fused_lm_head:
+            # with a bonus K6's entropy variant; K6b adds the entropy's gradient in its epilogue
+            log_probs = self._tail_log_probs(self.actor_model, batch, lens, input_ids, return_entropy=coeff != 0.0,
+                                             entropy_grad=coeff != 0.0, use_cache=False)
+            if coeff != 0.0:
+                log_probs, ent = log_probs
             actor_loss = actor_loss32 = ops.actor_loss(log_probs, old_log_probs, reward_advantages, sequence_mask,
-                                                       self.clip_range_ratio, mode=self.mode)
+                                                       self.clip_range_ratio, mode=self.mode, **kw)
+            if kw.get('return_clip_fraction'):
+                actor_loss32, clip_frac = actor_loss32
+                actor_loss = actor_loss32
+            if coeff != 0.0:
+                token = 'objective' in kw and kw['objective'].token_mean
+                entropy_mean = (ops.token_mean if token else ops.masked_mean)(ent, sequence_mask)
+                actor_loss = actor_loss32 - coeff * entropy_mean
+                entropy_mean = entropy_mean.detach()
         else:
             logits = self._actor_logits(self.actor_model, batch, lens, use_cache=False)
             if coeff != 0.0:
-                actor_loss, _, actor_loss32, entropy_mean = ops.tail_actor_loss(
-                    logits, input_ids, lens, old_log_probs, reward_advantages, sequence_mask, self.clip_range_ratio,
-                    mode=self.mode, entropy_coeff=coeff)
-            else:
-                actor_loss, _, actor_loss32 = ops.tail_actor_loss(logits, input_ids, lens, old_log_probs,
-                                                                  reward_advantages, sequence_mask,
-                                                                  self.clip_range_ratio, mode=self.mode)
+                kw['entropy_coeff'] = coeff
+            out = ops.tail_actor_loss(logits, input_ids, lens, old_log_probs, reward_advantages, sequence_mask,
+                                      self.clip_range_ratio, mode=self.mode, **kw)
+            if kw.get('return_clip_fraction'):
+                out, clip_frac = out[:-1], out[-1]
+            actor_loss, actor_loss32 = out[0], out[2]
+            if coeff != 0.0:
+                entropy_mean = out[3]
         self.actor_model.backward(actor_loss)
         self.actor_model.step()
 
@@ -195,13 +202,17 @@ class PPOTrainer(_TextPPOTrainer):
 
         with torch.no_grad():
             # see the text rl_step
-            fused = fused_allreduce(row_stats.device) if not (self.log_entropy or entropy_mean is not None) else None
+            extra = self.log_entropy or entropy_mean is not None or clip_frac is not None
+            fused = fused_allreduce(row_stats.device) if not extra else None
             stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss32, critic_loss32,
                                          coll=fused.next((9, 10)) if fused is not None else None)
             if self.log_entropy:
                 stats = with_entropy_lane(stats, training_batch['entropy'], sequence_mask)
             if entropy_mean is not None:
                 stats = with_bonus_lane(stats, entropy_mean)
+            clip_lane = stats.numel()
+            if clip_frac is not None:
+                stats = with_clip_lanes(stats, clip_frac, self)
             if fused is None:
                 stats = all_reduce_packed(stats, max_lanes=(9, 10))
             v = stats.tolist()  # the ONE host sync of rollout scoring + rl_step
@@ -211,6 +222,8 @@ class PPOTrainer(_TextPPOTrainer):
             out['train/entropy'] = v[11]
         if entropy_mean is not None:
             out['train/actor_entropy'] = v[12]
+        if clip_frac is not None:
+            clip_metrics(out, v, clip_lane, self)
         out['train/actor_lr'] = self.actor_model.optimizer.param_groups[0]['lr']
         out['train/reward_critic_lr'] = self.reward_critic_model.optimizer.param_groups[0]['lr']
         self.last_rl_tensors = {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns}

@@ -22,7 +22,8 @@ import torch
 
 from ... import ops
 from ...utils.multi_process import all_reduce_packed, fused_allreduce
-from .ppo import METRIC_KEYS, actor_loss_node, lm_head_of, with_bonus_lane, with_entropy_lane
+from .ppo import (METRIC_KEYS, actor_loss_node, clip_metrics, lm_head_of, with_bonus_lane, with_clip_lanes,
+                  with_entropy_lane)
 from .ppo import PPOTrainer as _TextPPOTrainer
 
 __all__ = ['PPOTrainer']
@@ -111,8 +112,8 @@ class PPOTrainer(_TextPPOTrainer):
             old_rewards, sequence_mask, start, self.advantage_estimator, self.n_samples_per_prompt, self.gamma,
             mode=self.mode, row_stats=row_stats)
 
-        actor_loss, actor_loss32, entropy_mean = actor_loss_node(self, inference_batch, input_ids, start, head,
-                                                                 old_log_probs, reward_advantages, sequence_mask)
+        actor_loss, actor_loss32, entropy_mean, clip_frac = actor_loss_node(
+            self, inference_batch, input_ids, start, head, old_log_probs, reward_advantages, sequence_mask)
         self.actor_model.backward(actor_loss)
         self.actor_model.step()
 
@@ -126,13 +127,17 @@ class PPOTrainer(_TextPPOTrainer):
 
         with torch.no_grad():
             # see the text rl_step
-            fused = fused_allreduce(row_stats.device) if not (self.log_entropy or entropy_mean is not None) else None
+            extra = self.log_entropy or entropy_mean is not None or clip_frac is not None
+            fused = fused_allreduce(row_stats.device) if not extra else None
             stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss32, reward_critic_loss,
                                          coll=fused.next((9, 10)) if fused is not None else None)
             if self.log_entropy:
                 stats = with_entropy_lane(stats, training_batch['entropy'][:, start:], sequence_mask[:, start:])
             if entropy_mean is not None:
                 stats = with_bonus_lane(stats, entropy_mean)
+            clip_lane = stats.numel()
+            if clip_frac is not None:
+                stats = with_clip_lanes(stats, clip_frac, self)
             if fused is None:
                 stats = all_reduce_packed(stats, max_lanes=(9, 10))  # ONE collective (reference: 10 + barrier)
             v = stats.tolist()  # ONE host sync (reference: 12 .item())
@@ -142,6 +147,8 @@ class PPOTrainer(_TextPPOTrainer):
             out['train/entropy'] = v[11]
         if entropy_mean is not None:
             out['train/actor_entropy'] = v[12]
+        if clip_frac is not None:
+            clip_metrics(out, v, clip_lane, self)
         out['train/actor_lr'] = self.actor_model.optimizer.param_groups[0]['lr']
         out['train/reward_critic_lr'] = self.reward_critic_model.optimizer.param_groups[0]['lr']
         self.last_rl_tensors = {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns}

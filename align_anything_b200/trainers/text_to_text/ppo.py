@@ -51,12 +51,46 @@ def with_entropy_lane(stats: torch.Tensor, entropy: torch.Tensor, mask: torch.Te
     return torch.cat([stats[:11], ent.reshape(1)])
 
 
-def entropy_coeff_of(tr) -> float:
-    """The entropy-bonus coefficient in effect: `cfgs.train_cfgs.entropy_coeff` when the config sets it (a yaml recipe),
-    otherwise the class switch `entropy_coeff`."""
+def switch_of(tr, name: str):
+    """A trainer switch in effect: `cfgs.train_cfgs.<name>` when the config sets it (a yaml recipe), otherwise the
+    class attribute `<name>`."""
     tc = getattr(getattr(tr, 'cfgs', None), 'train_cfgs', None)
-    v = getattr(tc, 'entropy_coeff', None) if tc is not None else None
-    return float(tr.entropy_coeff if v is None else v)
+    v = getattr(tc, name, None) if tc is not None else None
+    return getattr(tr, name, None) if v is None else v
+
+
+def entropy_coeff_of(tr) -> float:
+    """The entropy-bonus coefficient in effect (switch_of `entropy_coeff`)."""
+    return float(switch_of(tr, 'entropy_coeff'))
+
+
+OBJECTIVE_KEYS = ('clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode')
+
+
+def actor_objective_of(tr) -> ops.ActorObjective | None:
+    """The actor objective in effect (switch_of each of OBJECTIVE_KEYS), or None when every key is unset: the
+    reference's objective and today's launches.  A bad value raises ValueError here, before anything runs."""
+    fields = {k: switch_of(tr, k) for k in OBJECTIVE_KEYS}
+    fields = {k: v for k, v in fields.items() if v is not None}
+    return ops.ActorObjective(**fields) if fields else None
+
+
+def _dual_clip_on(tr) -> bool:
+    obj = actor_objective_of(tr)
+    return obj is not None and obj.dual_clip_ratio is not None
+
+
+def with_clip_lanes(stats: torch.Tensor, clip_frac: torch.Tensor, tr) -> torch.Tensor:
+    """The packed metric vector with the clip fraction (and the dual-clip fraction when dual-clip is on) appended as
+    AVG lanes of the step's one packed all-reduce."""
+    return torch.cat([stats, clip_frac[:2 if _dual_clip_on(tr) else 1]])
+
+
+def clip_metrics(out: dict, v: list, lane: int, tr) -> None:
+    """train/actor_clip_fraction (+ train/actor_dual_clip_fraction) from the lanes with_clip_lanes appended at `lane`."""
+    out['train/actor_clip_fraction'] = v[lane]
+    if _dual_clip_on(tr):
+        out['train/actor_dual_clip_fraction'] = v[lane + 1]
 
 
 def with_bonus_lane(stats: torch.Tensor, entropy_mean: torch.Tensor) -> torch.Tensor:
@@ -65,38 +99,54 @@ def with_bonus_lane(stats: torch.Tensor, entropy_mean: torch.Tensor) -> torch.Te
     return torch.cat([stats, entropy_mean.detach().float().reshape(1)])
 
 
+def objective_kwargs(tr) -> dict:
+    """The ops keywords of the actor objective switches: empty when they are all at their defaults (today's call)."""
+    kw = {}
+    objective = actor_objective_of(tr)
+    if objective is not None:
+        kw['objective'] = objective
+    if tr.log_clip_fraction:
+        kw['return_clip_fraction'] = True
+    return kw
+
+
 def actor_loss_node(tr, inference_batch, input_ids, start, head, old_log_probs, advantages, sequence_mask):
     """The actor loss of the text rl_step over the rows `[start:]` -> (loss, the loss for ppo_pack_metrics, the
-    masked-mean entropy or None).  `head`: the lm_head weight when `tr.fused_lm_head` is on, else None.  With an entropy
-    bonus (entropy_coeff_of(tr) != 0) the loss is  actor_loss - c * masked_mean(H, mask)  over the same rows and mask,
-    the second output stays the actor loss without it.  A function rather than a method, so that the grafted rl_step
-    of the reference's classes finds it without being grafted itself."""
+    masked-mean entropy or None, the fp32[2] clip fractions or None).  `head`: the lm_head weight when
+    `tr.fused_lm_head` is on, else None.  With an entropy bonus (entropy_coeff_of(tr) != 0) the loss is
+    actor_loss - c * masked_mean(H, mask)  over the same rows and mask (a token mean under loss_agg_mode 'token-mean'),
+    the second output stays the actor loss without it.  The actor objective switches (actor_objective_of) reach K5 and
+    K1f; `tr.log_clip_fraction` asks K5 for the clip fractions.  A function rather than a method, so that the grafted
+    rl_step of the reference's classes finds it without being grafted itself."""
     coeff = entropy_coeff_of(tr)
-    if head is not None and coeff != 0.0:  # K6's entropy variant; K6b adds the entropy's gradient in its epilogue
-        log_probs, ent = hidden_log_probs(tr.actor_model, inference_batch, input_ids, start, head, tr.lm_head_chunk_rows,
-                                          tr.mode, return_entropy=True, entropy_grad=True, use_cache=False)
-        loss = ops.actor_loss(log_probs, old_log_probs[:, start:], advantages, sequence_mask[:, start:],
-                              tr.clip_range_ratio, mode=tr.mode)
-        h_mean = ops.masked_mean(ent, sequence_mask[:, start:])
-        return loss - coeff * h_mean, loss, h_mean.detach()
+    kw = objective_kwargs(tr)
+    cf = None
     if head is not None:  # K6 + K6b + backward GEMMs for the log-probs, then K5
+        # with a bonus K6's entropy variant; K6b adds the entropy's gradient in its epilogue
         log_probs = hidden_log_probs(tr.actor_model, inference_batch, input_ids, start, head, tr.lm_head_chunk_rows,
-                                     tr.mode, use_cache=False)
+                                     tr.mode, return_entropy=coeff != 0.0, entropy_grad=coeff != 0.0, use_cache=False)
+        if coeff != 0.0:
+            log_probs, ent = log_probs
         loss = ops.actor_loss(log_probs, old_log_probs[:, start:], advantages, sequence_mask[:, start:],
-                              tr.clip_range_ratio, mode=tr.mode)
-        return loss, loss, None
+                              tr.clip_range_ratio, mode=tr.mode, **kw)
+        if kw.get('return_clip_fraction'):
+            loss, cf = loss
+        if coeff == 0.0:
+            return loss, loss, None, cf
+        token = 'objective' in kw and kw['objective'].token_mean
+        h_mean = (ops.token_mean if token else ops.masked_mean)(ent, sequence_mask[:, start:])
+        return loss - coeff * h_mean, loss, h_mean.detach(), cf
     logits = tr.actor_model(**inference_batch, use_cache=False).logits
     # the reference scores every position and then slices `[:, start:]` (:338-346); only those rows are ever used, so
     # only they are read here.  One autograd node (K1f): log-probs, d loss / d log-prob and the gradient tile in a
     # single pass over the response rows; the prompt rows of the tile are written as zeros by the same kernel.
     if coeff != 0.0:
-        loss, _, loss32, h_mean = ops.dense_actor_loss(logits, input_ids, start, old_log_probs[:, start:], advantages,
-                                                       sequence_mask[:, start:], tr.clip_range_ratio, mode=tr.mode,
-                                                       entropy_coeff=coeff)
-        return loss, loss32, h_mean
-    loss, _, loss32 = ops.dense_actor_loss(logits, input_ids, start, old_log_probs[:, start:], advantages,
-                                           sequence_mask[:, start:], tr.clip_range_ratio, mode=tr.mode)
-    return loss, loss32, None
+        kw['entropy_coeff'] = coeff
+    out = ops.dense_actor_loss(logits, input_ids, start, old_log_probs[:, start:], advantages, sequence_mask[:, start:],
+                               tr.clip_range_ratio, mode=tr.mode, **kw)
+    if kw.get('return_clip_fraction'):
+        out, cf = out[:-1], out[-1]
+    return out[0], out[2], (out[3] if coeff != 0.0 else None), cf
 
 
 class PPOTrainer:
@@ -114,6 +164,17 @@ class PPOTrainer:
     # when set; 0 leaves the step unchanged.  train/actor_loss stays the loss without the bonus, train/actor_entropy
     # carries the entropy term.
     entropy_coeff = 0.0
+    # The actor objective (ops.ActorObjective): clip-higher (clip_range_ratio_low / _high; None = clip_range_ratio),
+    # dual-clip (dual_clip_ratio c > 1, None = off) and loss_agg_mode ('seq-mean-token-mean', the reference's
+    # masked_mean, or 'token-mean').  `cfgs.train_cfgs.<key>` overrides each when set; all None is the reference's
+    # objective and today's launches.
+    clip_range_ratio_low = None
+    clip_range_ratio_high = None
+    dual_clip_ratio = None
+    loss_agg_mode = None
+    # Opt-in: train/actor_clip_fraction (and train/actor_dual_clip_fraction with dual-clip) from K5, reduced in the
+    # step's one packed all-reduce
+    log_clip_fraction = False
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, reward_model=None,
                  reward_critic_model=None, tokenizer=None, reward_tokenizer=None, *, kl_coeff=0.02,
@@ -282,8 +343,8 @@ class PPOTrainer:
             reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, start, self.kl_coeff,
             self.clip_range_score, self.gamma, self.gae_lambda, mode=self.mode)
 
-        actor_loss, actor_loss32, entropy_mean = actor_loss_node(self, inference_batch, input_ids, start, head,
-                                                                 old_log_probs, reward_advantages, sequence_mask)
+        actor_loss, actor_loss32, entropy_mean, clip_frac = actor_loss_node(
+            self, inference_batch, input_ids, start, head, old_log_probs, reward_advantages, sequence_mask)
         self.actor_model.backward(actor_loss)
         self.actor_model.step()
 
@@ -299,13 +360,17 @@ class PPOTrainer:
             # with log_entropy the entropy lane is filled in before the one packed all-reduce, so the NVLink reduction
             # fused into ppo_pack_metrics (which reduces the vector as it writes it) gives way to all_reduce_packed
             # (so does the entropy bonus's lane)
-            fused = fused_allreduce(row_stats.device) if not (self.log_entropy or entropy_mean is not None) else None
+            extra = self.log_entropy or entropy_mean is not None or clip_frac is not None
+            fused = fused_allreduce(row_stats.device) if not extra else None
             stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss32, reward_critic_loss,
                                          coll=fused.next((9, 10)) if fused is not None else None)
             if self.log_entropy:
                 stats = with_entropy_lane(stats, training_batch['entropy'][:, start:], sequence_mask[:, start:])
             if entropy_mean is not None:
                 stats = with_bonus_lane(stats, entropy_mean)
+            clip_lane = stats.numel()
+            if clip_frac is not None:
+                stats = with_clip_lanes(stats, clip_frac, self)
             if fused is None:
                 stats = all_reduce_packed(stats, max_lanes=(9, 10))  # ONE collective (reference: 10 + barrier)
             v = stats.tolist()  # ONE host sync (reference: 12 .item())
@@ -315,6 +380,8 @@ class PPOTrainer:
             out['train/entropy'] = v[11]
         if entropy_mean is not None:
             out['train/actor_entropy'] = v[12]
+        if clip_frac is not None:
+            clip_metrics(out, v, clip_lane, self)
         out['train/actor_lr'] = self.actor_model.optimizer.param_groups[0]['lr']
         out['train/reward_critic_lr'] = self.reward_critic_model.optimizer.param_groups[0]['lr']
         # the per-token tensors stay OUT of the returned dict: the reference hands it to Logger.log -> add_scalar /

@@ -367,6 +367,25 @@ int aa_ppo_actor_loss(const void *log_probs, int64_t lp_stride, const void *old_
                       float clip_range_ratio, int mode, float *loss, void *grad, int64_t grad_stride,
                       float *row_scratch, uint32_t *counter, void *stream);
 
+/* aa_ppo_actor_loss with the objective's options (ops.ActorObjective):
+ *   clip_low / clip_high : the ratio is clamped to [1 - clip_low, 1 + clip_high] (clip-higher: clip_high > clip_low);
+ *                          0 <= clip_low < 1, clip_high >= 0
+ *   dual_clip            : 0 (off) or c > 1: for adv < 0 the objective is max(min(s1, s2), c * adv)
+ *   loss_agg             : AA_AGG_SEQ_MEAN_TOKEN_MEAN (the reference's masked_mean) or AA_AGG_TOKEN_MEAN
+ *                          (-(s * mask).sum() / mask.sum() over the whole micro-batch)
+ *   clip_frac            : optional fp32[2]: [0] the masked-in share of tokens whose clipped branch is strictly smaller,
+ *                          [1] the share of masked-in adv < 0 tokens where c * adv wins (0 without such tokens), both
+ *                          aggregated like the loss
+ *   row_scratch          : fp32 [4 * B]
+ * With clip_low == clip_high == clip_range_ratio, dual_clip 0 and AA_AGG_SEQ_MEAN_TOKEN_MEAN the loss and gradient
+ * are bit-identical to aa_ppo_actor_loss.  Arguments are checked before any CUDA call. */
+enum { AA_AGG_SEQ_MEAN_TOKEN_MEAN = 0, AA_AGG_TOKEN_MEAN = 1 };
+int aa_ppo_actor_loss_obj(const void *log_probs, int64_t lp_stride, const void *old_log_probs, int64_t old_stride,
+                          int lp_dtype, const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
+                          int64_t mask_stride, int32_t B, int32_t Wm, float clip_low, float clip_high, float dual_clip,
+                          int loss_agg, int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac,
+                          float *row_scratch, uint32_t *counter, void *stream);
+
 int aa_ppo_critic_loss(const void *values, int64_t val_stride, const void *old_values,
                        int64_t old_stride, int val_dtype, const void *returns, int64_t ret_stride,
                        int ret_dtype, const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t Wm,
@@ -421,6 +440,21 @@ int aa_logprob_actor_fused_entropy(const void *logits, int logits_dtype, int64_t
                                    int64_t mask_stride, int32_t W, float clip_range_ratio, int mode, void *grad_logits,
                                    int64_t grad_row_stride, void *row_scratch, int32_t *status, float entropy_coeff,
                                    float *entropy, void *stream);
+/* aa_logprob_actor_fused / _entropy with the objective of aa_ppo_actor_loss_obj (clip_low, clip_high, dual_clip,
+ * loss_agg: same meaning and checks).  entropy == NULL: the plain kernel; otherwise the entropy-bonus kernel of
+ * aa_logprob_actor_fused_entropy, whose g_H under AA_AGG_TOKEN_MEAN is -entropy_coeff / (masked-in tokens of the
+ * micro-batch) on every masked-in token.  Under AA_AGG_TOKEN_MEAN every row's coefficient is -1 / that count.  With the
+ * default objective the outputs are bit-identical to aa_logprob_actor_fused / _entropy.  row_scratch: 48 bytes per
+ * tile row plus 4 bytes per segment. */
+int aa_logprob_actor_fused_obj(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                               const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                               const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
+                               const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
+                               float *stat_max, float *stat_logsum, const void *old_log_probs, int64_t old_stride,
+                               const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
+                               int64_t mask_stride, int32_t W, float clip_low, float clip_high, float dual_clip,
+                               int loss_agg, int mode, void *grad_logits, int64_t grad_row_stride, void *row_scratch,
+                               int32_t *status, float entropy_coeff, float *entropy, void *stream);
 
 /* The same single pass for the mean cross-entropy behind `outputs.loss` (trainers/text_to_text/sft.py:95-98
  * `SupervisedTrainer.loss`, ppo.py:400-408 `ptx_step`; transformers' ForCausalLMLoss): every row whose label !=
