@@ -407,9 +407,11 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
     total = block_sum<THREADS>(total, scratch);
   }
 
-  // upstream coefficient of d loss / d (row sum):  actor: -(1/B)/cnt (token-mean: -1/total) ; critic: 0.5*(1/B)/cnt
+  // upstream coefficient of d loss / d (row sum):  actor: -(1/B)/cnt (token-mean: -1/total) ; critic: 0.5*(1/B)/cnt.
+  // Every count divides as the reference's int64 `mask.sum()` does: cast to the promoted dtype first (ppo_math.cuh)
+  const float cnt_p = round_to(cnt, rp), total_p = round_to(total, rp);
   const float g_rs = ACTOR ? (token_mean ? actor_token_mean_coeff(total, rp) : actor_row_coeff(cnt, p.B, rp))
-                           : round_to(round_to(round_to(0.5f, rp) / static_cast<float>(p.B), rp) / cnt, rp);
+                           : round_to(round_to(round_to(0.5f, rp) / static_cast<float>(p.B), rp) / cnt_p, rp);
 
   float row_sum = 0.f, x_sum = 0.f;
   float n_clip = 0.f, n_dual = 0.f, n_neg = 0.f;  // clip-fraction counters of the row's masked-in tokens
@@ -464,7 +466,7 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
   if (tid == 0) {
     // seq-mean-token-mean: the row's masked mean in the promoted dtype; token-mean: the row's fp32 sum (rounded once,
     // after the cross-row sum, as ATen's sum over the whole tensor does)
-    p.row_scratch[b] = token_mean ? row_sum : round_to(round_to(row_sum, rp) / cnt, rp);
+    p.row_scratch[b] = token_mean ? row_sum : round_to(round_to(row_sum, rp) / cnt_p, rp);
     if (p.row_mean) p.row_mean[b] = x_sum / cnt;
     if (fracs) {  // the counters reduced like the loss: per-row fractions (seq-mean) or raw counts (token-mean)
       const float d = token_mean ? 1.f : cnt;
@@ -496,7 +498,7 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
     }
   }
   if (tid == 0) {
-    const float mm = token_mean ? round_to(round_to(acc, rp) / total, rp) : round_to(acc / static_cast<float>(p.B), rp);
+    const float mm = token_mean ? round_to(round_to(acc, rp) / total_p, rp) : round_to(acc / static_cast<float>(p.B), rp);
     const float loss = ACTOR ? -mm : round_to(0.5f * mm, rp);
     p.loss[0] = loss;
     // the same value as a 16-bit scalar in the first two bytes of loss[1]: the caller views it as the 0-dim bf16 / f16

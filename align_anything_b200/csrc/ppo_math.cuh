@@ -10,15 +10,18 @@
 namespace aa {
 
 // upstream coefficient of d loss / d (row sum of the masked objective): -(1/B)/cnt, rounded where the eager ops round
-// (`rp` = promoted dtype of log-probs and advantages)
+// (`rp` = promoted dtype of log-probs and advantages).  The count is the int64 `mask.sum(-1)`, which ATen casts to `rp`
+// before it divides (a bf16 row of 257 tokens is divided by 256), in the forward and in DivBackward alike.
 __device__ __forceinline__ float actor_row_coeff(float cnt, int B, int rp) {
   const float g_q = round_to(-1.f / static_cast<float>(B), rp);
-  return round_to(g_q / cnt, rp);
+  return round_to(g_q / round_to(cnt, rp), rp);
 }
 
 // upstream coefficient under token-mean aggregation, -(s * mask).sum() / mask.sum():  -1 / total (DivBackward's
-// rounding), total = the micro-batch's masked-in token count
-__device__ __forceinline__ float actor_token_mean_coeff(float total, int rp) { return round_to(-1.f / total, rp); }
+// rounding), total = the micro-batch's masked-in token count, cast to `rp` by ATen CUDA like the row count above
+__device__ __forceinline__ float actor_token_mean_coeff(float total, int rp) {
+  return round_to(-1.f / round_to(total, rp), rp);
+}
 
 // the argument check of the objective entry points (ops.ActorObjective checks the same on the host)
 inline bool actor_objective_ok(float clip_low, float clip_high, float dual_clip, int loss_agg) {
