@@ -66,7 +66,12 @@ struct FusedActorParams {
   // *ce_coeff = -loss_scale / n_valid (written by ce_coeff_kernel); old / adv / mask are unused
   // kind 2 (GRPO, aa_logprob_grpo_fused): old = reference log-probs, adv = ONE fp32 advantage per segment, clip = beta,
   // a token counts while j < row_end[segment], 1 / *total is d loss / d per-token loss (grpo_mask_kernel wrote both)
+  // kind 3 (GRPO's clipped objective, aa_logprob_grpo_fused_obj): kind 2's fields, W = K, the clip range
+  // [1 - clip_lo, 1 + clip_hi], dual (0 = off) and agg (grpo_agg_coeff gives g_rs); old_pol: the rollout-time policy
+  // log-probs at the log-prob's own index (out_idx), or nullptr for the pass's own log-probs (ratio 1)
   int kind;
+  const void *old_pol;
+  float clip_lo;
   int64_t ignore_index;
   const float *ce_coeff;
   const int32_t *row_end;
@@ -144,11 +149,13 @@ __global__ void __launch_bounds__(256) fused_actor_prep_kernel(const FusedActorP
         r.adv = load_as_float(p.adv, seg * p.adv_stride + j, p.adv_dtype);
         r.g_rs = token_mean ? actor_token_mean_coeff(cnt, p.rp) : actor_row_coeff(cnt, p.map.n_seg, p.rp);
         r.on = p.mask[seg * p.mask_stride + j] ? 1 : 0;
-      } else if (p.kind == 2) {
+      } else if (p.kind >= 2) {
+        const int end = __ldg(p.row_end + seg);
         r.old = load_as_float(p.old, seg * p.old_stride + j, p.out_dtype);
         r.adv = reinterpret_cast<const float *>(p.adv)[seg];
-        r.g_rs = 1.f / __ldg(p.total);
-        r.on = (j < __ldg(p.row_end + seg)) ? 1 : 0;
+        r.g_rs = (p.kind == 2) ? 1.f / __ldg(p.total)
+                               : grpo_agg_coeff(p.agg, __ldg(p.total), static_cast<float>(end), p.map.n_seg, p.W);
+        r.on = (j < end) ? 1 : 0;
       } else {
         r.g_rs = __ldg(p.ce_coeff);
         r.on = 1;
@@ -445,12 +452,20 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
           actor_token(round_to(lp, p.out_dtype), old, adv, on, g_rs, p.clip, p.clip_hi, p.dual, p.rx, p.rp, p.ra, obj, g,
                       why);
         if (p.kind == 2) grpo_token(round_to(lp, p.out_dtype), old, adv, on, g_rs, p.clip, p.rx, obj, g);
+        if (p.kind == 3) {
+          const float lpr = round_to(lp, p.out_dtype);
+          const float po = p.old_pol ? load_as_float(p.old_pol, out_idx, p.out_dtype) : lpr;
+          grpo_obj_token(lpr, po, old, adv, on, g_rs, p.clip, p.clip_lo, p.clip_hi, p.dual, p.rx, obj, g, why);
+        }
         sh_b[0] = m;
         sh_b[1] = logsum;
         sh_b[2] = g;
         if constexpr (EGRAD) {
           float gH = 0.f;
-          if (on) gH = (p.kind == 0) ? __ldg(p.ent_seg + g_row / p.seq) : -p.ent_coeff * g_rs;
+          // GRPO: a token mean over the completion mask under every aggregation (kind 3's g_rs is the loss's)
+          if (on)
+            gH = (p.kind == 0) ? __ldg(p.ent_seg + g_row / p.seq)
+                               : -p.ent_coeff * ((p.kind == 2) ? g_rs : 1.f / __ldg(p.total));
           sh_b[3] = entropy_of(logsum, s, t);
           sh_b[4] = gH;
         }
@@ -801,7 +816,14 @@ extern "C" int aa_logprob_ce_fused(const void *logits, int logits_dtype, int64_t
   return launch_fused(p, logits_dtype, AA_MODE_F32, static_cast<FusedRec *>(row_scratch), n_tile_rows, st);
 }
 
-// aa_logprob_grpo_fused{,_entropy}: entropy == nullptr runs the plain kernels
+// the objective of aa_logprob_grpo_fused_obj (kind 3)
+struct GrpoObjective {
+  const void *old_pol;
+  float clip_lo, clip_hi, dual;
+  int agg;
+};
+
+// aa_logprob_grpo_fused{,_entropy,_obj}: entropy == nullptr runs the plain kernels; obj == nullptr: kind 2
 static int logprob_grpo_fused(float *entropy, float entropy_coeff, bool egrad, const char *who, const void *logits,
                               int logits_dtype, int64_t row_stride, int32_t V,
                                     const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
@@ -810,7 +832,8 @@ static int logprob_grpo_fused(float *entropy, float entropy_coeff, bool egrad, c
                                     const void *ref_log_probs, int64_t ref_stride, const float *advantages,
                                     const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t K,
                                     float beta, int mode, void *grad_logits, int64_t grad_row_stride, void *row_scratch,
-                                    int32_t *row_end, float *total, uint32_t *counter, int32_t *status, void *stream) {
+                                    int32_t *row_end, float *total, uint32_t *counter, int32_t *status, void *stream,
+                                    const GrpoObjective *obj = nullptr) {
   AA_REQUIRE(V > 0 && n_segments > 0 && K > 0 && n_tile_rows > 0 && n_tile_rows % n_segments == 0, AA_ERR_ARG,
              "%s: bad sizes (the gradient tile holds n_tile_rows / n_segments rows per sample)", who);
   AA_REQUIRE(logits && labels && seg_logit_off && seg_label_off && seg_out_off && seg_cum && seg_tile_row && log_probs &&
@@ -840,6 +863,15 @@ static int logprob_grpo_fused(float *entropy, float entropy_coeff, bool egrad, c
   p.total = total;
   p.entropy = entropy;
   p.ent_coeff = entropy_coeff;
+  if (obj) {
+    p.kind = 3;
+    p.W = K;
+    p.old_pol = obj->old_pol;
+    p.clip_lo = obj->clip_lo;
+    p.clip_hi = obj->clip_hi;
+    p.dual = obj->dual;
+    p.agg = obj->agg;
+  }
   return launch_fused(p, logits_dtype, mode, static_cast<FusedRec *>(row_scratch), n_tile_rows, st, egrad);
 }
 
@@ -892,6 +924,30 @@ extern "C" int aa_logprob_grpo_fused_entropy_grad(const void *logits, int logits
                             seg_tile_row, n_tile_rows, log_probs, lp_dtype, ref_log_probs, ref_stride, advantages,
                             completion_tokens, tok_stride, eos_id, K, beta, mode, grad_logits, grad_row_stride,
                             row_scratch, row_end, total, counter, status, stream);
+}
+
+extern "C" int aa_logprob_grpo_fused_obj(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                         const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                         const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
+                                         const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
+                                         const void *ref_log_probs, int64_t ref_stride, const void *old_log_probs,
+                                         const float *advantages, const int64_t *completion_tokens, int64_t tok_stride,
+                                         int64_t eos_id, int32_t K, float beta, float clip_low, float clip_high,
+                                         float dual_clip, int loss_agg, int mode, void *grad_logits,
+                                         int64_t grad_row_stride, void *row_scratch, int32_t *row_end, float *total,
+                                         uint32_t *counter, int32_t *status, float *entropy, float entropy_coeff,
+                                         void *stream) {
+  AA_REQUIRE(grpo_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
+             "aa_logprob_grpo_fused_obj: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a "
+             "known loss_agg; got %g %g %g %d)", clip_low, clip_high, dual_clip, loss_agg);
+  AA_REQUIRE(entropy_coeff == entropy_coeff, AA_ERR_ARG, "aa_logprob_grpo_fused_obj: entropy_coeff is NaN");
+  AA_REQUIRE(entropy || entropy_coeff == 0.f, AA_ERR_ARG, "aa_logprob_grpo_fused_obj: entropy_coeff needs entropy");
+  GrpoObjective obj{old_log_probs, clip_low, clip_high, dual_clip, loss_agg};
+  return logprob_grpo_fused(entropy, entropy_coeff, entropy && entropy_coeff != 0.f, "aa_logprob_grpo_fused_obj",
+                            logits, logits_dtype, row_stride, V, labels, n_segments, seg_logit_off, seg_label_off,
+                            seg_out_off, seg_cum, seg_tile_row, n_tile_rows, log_probs, lp_dtype, ref_log_probs,
+                            ref_stride, advantages, completion_tokens, tok_stride, eos_id, K, beta, mode, grad_logits,
+                            grad_row_stride, row_scratch, row_end, total, counter, status, stream, &obj);
 }
 
 extern "C" int aa_scale_tile(void *tile, int dtype, int64_t n, const void *scale, int scale_dtype, void *stream) {

@@ -623,6 +623,97 @@ __global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoParams p) 
   if (tid == 0) p.loss[0] = acc / cnt;
 }
 
+// Dr. GRPO's advantages: r - group mean (the mean of group_advantages_kernel), no std scaling
+__global__ void __launch_bounds__(32)
+    group_centered_kernel(const float *__restrict__ rewards, int n_groups, int G, float *__restrict__ adv) {
+  const int g = blockIdx.x, lane = threadIdx.x;
+  if (g >= n_groups) return;
+  float s = 0.f;
+  for (int i = lane; i < G; i += kWarp) s += rewards[g * G + i];
+  const float mean = warp_sum(s) / static_cast<float>(G);
+  for (int i = lane; i < G; i += kWarp) adv[g * G + i] = rewards[g * G + i] - mean;
+}
+
+struct GrpoObjParams {
+  GrpoParams base;
+  const void *old;  // rollout-time policy log-probs, or nullptr: the log-probs themselves (ratio 1)
+  int64_t old_stride;
+  float clip_lo, clip_hi, dual;
+  int agg;
+  float *clip_frac;  // optional fp32[2]; row_scratch then holds 4 * B floats
+};
+
+// aa_grpo_loss_obj: GRPO's clipped objective (grpo_obj_token) under one of the three aggregations
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS) grpo_loss_obj_kernel(const GrpoObjParams q) {
+  __shared__ float scratch[33];
+  const GrpoParams &p = q.base;
+  const int b = blockIdx.x, tid = threadIdx.x, r = p.r_lp;
+  const int end = p.row_end[b];
+  const float total = p.total[0];
+  const float A = p.adv[b];
+  const float g_t = grpo_agg_coeff(q.agg, total, static_cast<float>(end), p.B, p.K);
+  float row = 0.f, n_clip = 0.f, n_dual = 0.f;
+  for (int t = tid; t < p.K; t += THREADS) {
+    const bool on = t < end;
+    const float lp = load_as_float(p.lp, b * p.lp_stride + t, p.dtype);
+    const float rf = load_as_float(p.ref_lp, b * p.ref_stride + t, p.dtype);
+    const float old = q.old ? load_as_float(q.old, b * q.old_stride + t, p.dtype) : lp;
+    float ptl, g;
+    int why;
+    grpo_obj_token(lp, old, rf, A, on, g_t, p.beta, q.clip_lo, q.clip_hi, q.dual, r, ptl, g, why);
+    if (on) {
+      row += ptl;
+      n_clip += (why & 1) ? 1.f : 0.f;
+      n_dual += (why & 2) ? 1.f : 0.f;
+    }
+    if (p.grad) store_from_float(p.grad, b * p.grad_stride + t, p.dtype, g);
+  }
+  row = block_sum<THREADS>(row, scratch);
+  const bool fracs = q.clip_frac != nullptr;
+  if (fracs) {
+    n_clip = block_sum<THREADS>(n_clip, scratch);
+    n_dual = block_sum<THREADS>(n_dual, scratch);
+  }
+  const bool seq_mean = q.agg == AA_AGG_SEQ_MEAN_TOKEN_MEAN;
+  if (tid == 0) {
+    // seq-mean-token-mean: the row's token mean (the fp32 row sum over its count); otherwise the fp32 row sum
+    p.row_scratch[b] = seq_mean ? row / static_cast<float>(end) : row;
+    if (fracs) {  // per-row fractions (seq-mean-token-mean) or raw counts; the negative-advantage tokens are the row's
+      const float d = seq_mean ? static_cast<float>(end) : 1.f;
+      p.row_scratch[p.B + b] = n_clip / d;
+      p.row_scratch[2 * p.B + b] = n_dual / d;
+      p.row_scratch[3 * p.B + b] = (A < 0.f) ? static_cast<float>(end) / d : 0.f;
+    }
+  }
+  if (!last_block_arrives(p.counter, gridDim.x)) return;
+  const volatile float *rows = p.row_scratch;
+  float acc = 0.f;
+  for (int k = tid; k < p.B; k += THREADS) acc += rows[k];
+  acc = block_sum<THREADS>(acc, scratch);
+  if (fracs) {
+    float fc = 0.f, fd = 0.f, fn = 0.f;
+    for (int k = tid; k < p.B; k += THREADS) {
+      fc += rows[p.B + k];
+      fd += rows[2 * p.B + k];
+      fn += rows[3 * p.B + k];
+    }
+    fc = block_sum<THREADS>(fc, scratch);
+    fd = block_sum<THREADS>(fd, scratch);
+    fn = block_sum<THREADS>(fn, scratch);
+    if (tid == 0) {
+      q.clip_frac[0] = fc / (seq_mean ? static_cast<float>(p.B) : total);
+      q.clip_frac[1] = fn > 0.f ? fd / fn : 0.f;
+    }
+  }
+  if (tid == 0) {
+    if (q.agg == AA_AGG_SEQ_MEAN_TOKEN_SUM_NORM)
+      p.loss[0] = acc / (static_cast<float>(p.B) * static_cast<float>(p.K));
+    else
+      p.loss[0] = seq_mean ? acc / static_cast<float>(p.B) : acc / total;
+  }
+}
+
 // mean NLL over non-ignored rows (deterministic two-level reduction; last block finalises)
 template <int THREADS>
 __global__ void __launch_bounds__(THREADS)
@@ -900,6 +991,41 @@ extern "C" int aa_grpo_loss(const void *log_probs, int64_t lp_stride, const void
                (mode == AA_MODE_FAITHFUL) ? lp_dtype : AA_F32, loss, grad, grad_stride, scratch + 1, counter + 1};
   grpo_loss_kernel<128><<<B, 128, 0, st>>>(p);
   return check_launch("aa_grpo_loss");
+}
+
+extern "C" int aa_group_advantages_centered(const float *rewards, int32_t n_groups, int32_t group_size,
+                                            float *advantages, void *stream) {
+  AA_REQUIRE(rewards && advantages && n_groups > 0 && group_size > 0, AA_ERR_ARG,
+             "aa_group_advantages_centered: bad arguments");
+  group_centered_kernel<<<n_groups, 32, 0, static_cast<cudaStream_t>(stream)>>>(rewards, n_groups, group_size,
+                                                                                advantages);
+  return check_launch("aa_group_advantages_centered");
+}
+
+extern "C" int aa_grpo_loss_obj(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
+                                const void *old_log_probs, int64_t old_stride, int lp_dtype, const float *advantages,
+                                const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B,
+                                int32_t K, float beta, float clip_low, float clip_high, float dual_clip, int loss_agg,
+                                int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac,
+                                int32_t *row_end, float *scratch, uint32_t *counter, void *stream) {
+  AA_REQUIRE(B > 0 && K > 0 && log_probs && ref_log_probs && advantages && completion_tokens && loss && row_end &&
+                 scratch && counter,
+             AA_ERR_ARG, "aa_grpo_loss_obj: bad arguments");
+  AA_REQUIRE(dtype_ok(lp_dtype), AA_ERR_DTYPE, "aa_grpo_loss_obj: bad dtype");
+  AA_REQUIRE(grpo_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
+             "aa_grpo_loss_obj: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a known "
+             "loss_agg; got %g %g %g %d)", clip_low, clip_high, dual_clip, loss_agg);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_grpo_loss_obj: bad mode");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  grpo_mask_kernel<128><<<B, 128, 0, st>>>(completion_tokens, tok_stride, B, K, eos_id, row_end, scratch, counter);
+  int rc = check_launch("aa_grpo_loss_obj(mask)");
+  if (rc) return rc;
+  GrpoObjParams q{GrpoParams{log_probs, ref_log_probs, lp_dtype, lp_stride, ref_stride, advantages, row_end, scratch, B,
+                             K, beta, (mode == AA_MODE_FAITHFUL) ? lp_dtype : AA_F32, loss, grad, grad_stride,
+                             scratch + 1, counter + 1},
+                  old_log_probs, old_stride, clip_low, clip_high, dual_clip, loss_agg, clip_frac};
+  grpo_loss_obj_kernel<128><<<B, 128, 0, st>>>(q);
+  return check_launch("aa_grpo_loss_obj");
 }
 
 extern "C" int aa_nll_mean(const void *logp, int dtype, const int64_t *labels, int64_t n, int64_t ignore_index,

@@ -103,6 +103,48 @@ __device__ __forceinline__ void grpo_token(float lp, float rf, float A, bool on,
   }
 }
 
+// the argument check of the GRPO objective entry points: the actor objective's ranges, and GRPO's third aggregation
+// (ops.GrpoObjective checks the same on the host)
+inline bool grpo_objective_ok(float clip_low, float clip_high, float dual_clip, int loss_agg) {
+  return actor_objective_ok(clip_low, clip_high, dual_clip, AA_AGG_TOKEN_MEAN) &&
+         (loss_agg == AA_AGG_TOKEN_MEAN || loss_agg == AA_AGG_SEQ_MEAN_TOKEN_MEAN ||
+          loss_agg == AA_AGG_SEQ_MEAN_TOKEN_SUM_NORM);
+}
+
+// d loss / d per-token loss of a counted token under each GRPO aggregation, as the eager ops round it (fp32: the
+// per-token loss is fp32 because the advantages are):  token-mean  1 / total ;  seq-mean-token-mean  (1 / B) / cnt_b
+// (MeanBackward, then DivBackward by the row's count) ;  seq-mean-token-sum-norm  1 / (B * K)
+__device__ __forceinline__ float grpo_agg_coeff(int agg, float total, float cnt, int B, int K) {
+  if (agg == AA_AGG_SEQ_MEAN_TOKEN_MEAN) return (1.f / static_cast<float>(B)) / cnt;
+  if (agg == AA_AGG_SEQ_MEAN_TOKEN_SUM_NORM) return 1.f / (static_cast<float>(B) * static_cast<float>(K));
+  return 1.f / total;
+}
+
+// One token of GRPO's clipped objective (DeepSeekMath's GRPO with clip-higher and dual-clip):
+//   -(s - beta * KL),  s = the clipped-ratio objective of actor_token with r = exp(lp - old), old = the rollout-time
+// policy log-prob, and the k3 KL of grpo_token.  g_t: d loss / d per-token loss (grpo_agg_coeff).  The advantage is
+// fp32, so s and the per-token loss are fp32 (actor_token's promoted and `c * A` roundings are fp32); `r` rounds what
+// has the log-prob dtype.  The gradient reaching lp through the ratio takes c1's place in grpo_token's accumulation
+// order (the ratio is created after the KL, as the reference creates its exp(lp - lp.detach()) term).
+//   why: actor_token's clip-fraction bits
+__device__ __forceinline__ void grpo_obj_token(float lp, float old, float rf, float A, bool on, float g_t, float beta,
+                                               float eps_lo, float eps_hi, float dual, int r, float &ptl, float &grad,
+                                               int &why) {
+  float s, ga;
+  actor_token(lp, old, A, on, -g_t, eps_lo, eps_hi, dual, r, AA_F32, AA_F32, s, ga, why);
+  const float d = round_to(rf - lp, r);
+  const float e = round_to(expf(d), r);
+  const float kl = round_to(round_to(e - d, r) - 1.f, r);
+  const float bk = round_to(beta * kl, r);
+  ptl = -(s - bk);
+  grad = 0.f;
+  if (on) {
+    const float g_kl = round_to(round_to(g_t, r) * beta, r);
+    const float c2 = -round_to(g_kl * e, r);
+    grad = round_to(round_to(ga + g_kl, r) + c2, r);
+  }
+}
+
 // pass 1: first eos per row (-> row_end[b] = number of counted tokens) and the global token count
 template <int THREADS>
 __global__ void __launch_bounds__(THREADS)

@@ -1128,16 +1128,16 @@ def slice_sums(sequence_log_probs: torch.Tensor, slices: torch.Tensor, mode: str
 
 
 # ---- GRPO ---------------------------------------------------------------------------------------------
-def group_advantages(rewards: torch.Tensor, num_generations: int) -> torch.Tensor:
+def group_advantages(rewards: torch.Tensor, num_generations: int, scale: bool = True) -> torch.Tensor:
     """trainers/text_to_text/grpo.py:268-274: rewards (B * G,) fp32 -> advantages (B * G, 1),
-    (r - group mean) / (unbiased group std + 1e-4)."""
+    (r - group mean) / (unbiased group std + 1e-4).  scale=False (Dr. GRPO): r - group mean."""
     L.require_cuda(rewards)
     r = rewards.detach().float().contiguous().view(-1)
     if r.numel() % num_generations:
         raise ValueError('rewards must hold B * num_generations values')
     adv = torch.empty_like(r)
-    L.check(L.lib().aa_group_advantages(r.data_ptr(), r.numel() // num_generations, int(num_generations), adv.data_ptr(),
-                                        L.stream_ptr(r.device)))
+    fn = L.lib().aa_group_advantages if scale else L.lib().aa_group_advantages_centered
+    L.check(fn(r.data_ptr(), r.numel() // num_generations, int(num_generations), adv.data_ptr(), L.stream_ptr(r.device)))
     return adv.view(-1, 1)
 
 
@@ -1165,12 +1165,71 @@ class _GrpoLossFn(torch.autograd.Function):
         return (grad.float() * g.float()).to(grad.dtype), None, None, None, None, None, None
 
 
+class _GrpoLossObjFn(torch.autograd.Function):
+    """aa_grpo_loss_obj: GRPO's clipped objective; forward writes the loss and d loss / d lp in one launch."""
+
+    @staticmethod
+    def forward(ctx, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, clip_frac):
+        B, K = lp.shape
+        dev = lp.device
+        loss = torch.empty(1, dtype=torch.float32, device=dev)
+        grad = torch.empty((B, K), dtype=lp.dtype, device=dev)
+        row_end = torch.empty(B, dtype=torch.int32, device=dev)
+        scratch = torch.empty(1 + 4 * B, dtype=torch.float32, device=dev)
+        _grpo_loss_obj_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac,
+                              row_end, scratch)
+        ctx.save_for_backward(grad)
+        ctx.mark_non_differentiable(row_end)
+        return loss[0], row_end
+
+    @staticmethod
+    def backward(ctx, g, _):
+        (grad,) = ctx.saved_tensors
+        return (grad.float() * g.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None
+
+
+def _grpo_loss_obj_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
+                          scratch):
+    """aa_grpo_loss_obj; obj = GrpoObjective.args(), old: the old log-probs or None (the log-probs themselves)."""
+    B, K = lp.shape
+    lo, hi, dual, agg = obj
+    L.check(L.lib().aa_grpo_loss_obj(
+        lp.data_ptr(), lp.stride(0), ref_lp.data_ptr(), ref_lp.stride(0), L.ptr(old), old.stride(0) if old is not None else 0,
+        L.dtype_code(lp.dtype), adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), B, K, float(beta),
+        float(lo), float(hi), float(dual), int(agg), mode_code, loss.data_ptr(), L.ptr(grad),
+        grad.stride(0) if grad is not None else 0, L.ptr(clip_frac), row_end.data_ptr(), scratch.data_ptr(),
+        _device_scratch(lp.device)['counter'][5:7].data_ptr(), L.stream_ptr(lp.device)))
+
+
+def _grpo_objective(objective) -> GrpoObjective | None:
+    if objective is None:
+        return None
+    if not isinstance(objective, GrpoObjective):
+        raise TypeError(f'objective must be an ops.GrpoObjective, got {type(objective).__name__}')
+    return objective
+
+
+def _old_log_probs(old, shape, dtype):
+    """The rollout-time policy log-probs for the objective kernels: detached, contiguous, in the log-probs' dtype."""
+    if old is None:
+        return None
+    if tuple(old.shape) != tuple(shape):
+        raise ValueError(f'old_per_token_logps must be {tuple(shape)}, got {tuple(old.shape)}')
+    return _contiguous_last(old.detach().to(dtype)).contiguous()
+
+
 def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, advantages: torch.Tensor,
-              completion_tokens: torch.Tensor, eos_token_id: int, beta: float, mode: str | None = None):
+              completion_tokens: torch.Tensor, eos_token_id: int, beta: float, mode: str | None = None, *,
+              objective: GrpoObjective | None = None, old_per_token_logps: torch.Tensor | None = None,
+              return_clip_fraction: bool = False):
     """The loss of GRPOTrainer.train_step (trainers/text_to_text/grpo.py:290-312): per-token k3 KL, per-token loss
     -(exp(lp - lp.detach()) * A - beta * KL), completion mask up to the first eos, token mean -> fp32 scalar,
-    differentiable in per_token_logps.  Returns (loss, counted_tokens_per_row)."""
+    differentiable in per_token_logps.  Returns (loss, counted_tokens_per_row).
+    objective (ops.GrpoObjective) / old_per_token_logps (the rollout-time policy log-probs, (B, K)): GRPO's clipped
+    objective (aa_grpo_loss_obj) with ratio exp(lp - old); without old_per_token_logps the ratio is 1.  None / default
+    fields and no old log-probs: today's launch.  return_clip_fraction appends the fp32[2] clip fractions."""
     L.require_cuda(per_token_logps, ref_per_token_logps, advantages, completion_tokens)
+    obj = _grpo_objective(objective)
     if per_token_logps.dim() != 2 or per_token_logps.shape != ref_per_token_logps.shape or \
             completion_tokens.shape != per_token_logps.shape:
         raise ValueError('per-token log-probs and completion tokens must all be (B, K)')
@@ -1179,8 +1238,14 @@ def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, 
     adv = advantages.detach().float().contiguous().view(-1)
     if adv.numel() != lp.size(0):
         raise ValueError('one advantage per sequence expected')
+    old = _old_log_probs(old_per_token_logps, lp.shape, lp.dtype)
     tok = _contiguous_last(completion_tokens.to(torch.int64))
-    return _GrpoLossFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype))
+    if (obj is None or obj.is_default) and old is None and not return_clip_fraction:
+        return _GrpoLossFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype))
+    args = (obj or GrpoObjective()).args()
+    cf = torch.zeros(2, dtype=torch.float32, device=lp.device) if return_clip_fraction else None
+    out = _GrpoLossObjFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype), args, old, cf)
+    return out + (cf,) if return_clip_fraction else out
 
 
 def tail_token_log_probs(logits: torch.Tensor, input_ids: torch.Tensor, logits_to_keep: int, mode: str | None = None,
@@ -1211,7 +1276,9 @@ class _GrpoFusedFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, logits, labels, plan, ref_lp, adv, tokens, eos_id, beta, mode_code, entropy=None,
-                entropy_coeff=0.0):
+                entropy_coeff=0.0, obj=None, old=None, clip_frac=None):
+        """obj: GrpoObjective.args() for aa_logprob_grpo_fused_obj + aa_grpo_loss_obj (old: the old log-probs or None,
+        clip_frac: an fp32[2] tensor for the clip fractions or None); None: today's launches."""
         dev = logits.device
         B, K = plan.out_shape
         lp_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
@@ -1229,17 +1296,30 @@ class _GrpoFusedFn(torch.autograd.Function):
                 ref_lp.data_ptr(), ref_lp.stride(0), adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), K,
                 float(beta), mode_code, grad.data_ptr(), logits.size(-1), rows.data_ptr(), row_end.data_ptr(),
                 scratch.data_ptr(), sc['counter'][5:6].data_ptr(), sc['status'].data_ptr())
-        if entropy is None:
+        if obj is not None:
+            o = (logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), labels.data_ptr(),
+                 plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp_dtype),
+                 ref_lp.data_ptr(), ref_lp.stride(0), L.ptr(old), adv.data_ptr(), tokens.data_ptr(), tokens.stride(0),
+                 int(eos_id), K, float(beta), float(obj[0]), float(obj[1]), float(obj[2]), int(obj[3]), mode_code,
+                 grad.data_ptr(), logits.size(-1), rows.data_ptr(), row_end.data_ptr(), scratch.data_ptr(),
+                 sc['counter'][5:6].data_ptr(), sc['status'].data_ptr(), L.ptr(entropy), float(entropy_coeff))
+            L.check(lib.aa_logprob_grpo_fused_obj(*o, L.stream_ptr(dev)))
+            scratch = torch.empty(1 + 4 * B, dtype=torch.float32, device=dev)
+            _grpo_loss_obj_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, None, clip_frac,
+                                  row_end, scratch)
+        elif entropy is None:
             L.check(lib.aa_logprob_grpo_fused(*args, L.stream_ptr(dev)))
         elif entropy_coeff == 0.0:  # the same launch with the entropy of every completion row from its (max, sum-exp) pass
             L.check(lib.aa_logprob_grpo_fused_entropy(*args, entropy.data_ptr(), L.stream_ptr(dev)))
         else:  # ... and the entropy bonus's gradient in the tile
             L.check(lib.aa_logprob_grpo_fused_entropy_grad(*args, entropy.data_ptr(), float(entropy_coeff),
                                                            L.stream_ptr(dev)))
-        L.check(lib.aa_grpo_loss(lp.data_ptr(), lp.stride(0), ref_lp.data_ptr(), ref_lp.stride(0), L.dtype_code(lp_dtype),
-                                 adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), B, K, float(beta),
-                                 mode_code, loss.data_ptr(), None, 0, row_end.data_ptr(), scratch.data_ptr(),
-                                 sc['counter'][5:7].data_ptr(), L.stream_ptr(dev)))
+        if obj is None:
+            L.check(lib.aa_grpo_loss(lp.data_ptr(), lp.stride(0), ref_lp.data_ptr(), ref_lp.stride(0),
+                                     L.dtype_code(lp_dtype), adv.data_ptr(), tokens.data_ptr(), tokens.stride(0),
+                                     int(eos_id), B, K, float(beta), mode_code, loss.data_ptr(), None, 0,
+                                     row_end.data_ptr(), scratch.data_ptr(), sc['counter'][5:7].data_ptr(),
+                                     L.stream_ptr(dev)))
         ctx.save_for_backward(grad)
         if entropy_coeff == 0.0:
             ctx.mark_non_differentiable(lp, row_end)
@@ -1252,7 +1332,7 @@ class _GrpoFusedFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g, *_unused):
         (grad,) = _hand_over_once(ctx, g, *ctx.saved_tensors)
-        return grad, None, None, None, None, None, None, None, None, None, None
+        return grad, None, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 def _completion_mean(x: torch.Tensor, row_end: torch.Tensor) -> torch.Tensor:
@@ -1263,7 +1343,9 @@ def _completion_mean(x: torch.Tensor, row_end: torch.Tensor) -> torch.Tensor:
 
 def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_to_keep: int,
                           ref_per_token_logps: torch.Tensor, advantages: torch.Tensor, eos_token_id: int, beta: float,
-                          mode: str | None = None, return_entropy: bool = False, entropy_coeff: float = 0.0):
+                          mode: str | None = None, return_entropy: bool = False, entropy_coeff: float = 0.0, *,
+                          objective: GrpoObjective | None = None, old_per_token_logps: torch.Tensor | None = None,
+                          return_clip_fraction: bool = False):
     """`_get_per_token_logps` of the policy + the loss of GRPOTrainer.train_step (trainers/text_to_text/grpo.py:205-210,
     290-312) from the policy's logits; the reference model's per-token log-probs must already be there.
     -> (loss fp32 scalar, policy per-token log-probs (B, K), counted tokens per row).  With a gradient: one pass over the
@@ -1272,8 +1354,16 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
     other outputs are bit-identical.  entropy_coeff != 0 (entropy bonus): the loss is
     loss - entropy_coeff * (H * mask).sum() / mask.sum()  over the completion mask, and the detached entropy mean and
     the detached GRPO loss without the bonus follow row_end (before the entropy when return_entropy); the single pass is K1f's entropy-gradient variant, the
-    composed path K1's entropy variant -> grpo_loss -> K1b's entropy variant."""
+    composed path K1's entropy variant -> grpo_loss -> K1b's entropy variant.
+    objective / old_per_token_logps: GRPO's clipped objective as in grpo_loss (K1f's objective entry point, or K1 ->
+    aa_grpo_loss_obj -> K1b); the entropy bonus stays a token mean over the completion mask.  return_clip_fraction
+    appends the fp32[2] clip fractions last.  None / default fields and no old log-probs: today's launches."""
     L.require_cuda(logits, input_ids, ref_per_token_logps, advantages)
+    obj = _grpo_objective(objective)
+    if (obj is not None and not obj.is_default) or old_per_token_logps is not None or return_clip_fraction:
+        return _grpo_objective_from_logits(logits, input_ids, int(logits_to_keep), ref_per_token_logps, advantages,
+                                           eos_token_id, beta, mode, return_entropy, float(entropy_coeff),
+                                           obj or GrpoObjective(), old_per_token_logps, return_clip_fraction)
     K = int(logits_to_keep)
     tokens = input_ids[:, -K:]
     coeff = float(entropy_coeff)
@@ -1314,6 +1404,53 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
                                   ent) + (ent,)
     out = _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code, ent, coeff)
     return out + (ent,) if return_entropy else out
+
+
+def _grpo_objective_from_logits(logits, input_ids, K, ref_per_token_logps, advantages, eos_token_id, beta, mode,
+                                return_entropy, coeff, obj, old, return_cf):
+    """grpo_loss_from_logits under GRPO's clipped objective (the same outputs, then the clip fractions)."""
+    tokens = input_ids[:, -K:]
+    if not _single_pass_ok(logits, _FUSED_GRPO, torch.is_grad_enabled() and logits.requires_grad):
+        ent = None
+        if return_entropy or coeff != 0.0:
+            lp, ent = tail_token_log_probs(logits, input_ids, K, mode=mode, return_entropy=True,
+                                           entropy_grad=coeff != 0.0)
+        else:
+            lp = tail_token_log_probs(logits, input_ids, K, mode=mode)
+        scored = grpo_loss(lp, ref_per_token_logps, advantages, tokens, eos_token_id, beta, mode=mode, objective=obj,
+                           old_per_token_logps=old, return_clip_fraction=return_cf)
+        loss, row_end = scored[0], scored[1]
+        out = (loss, lp.detach(), row_end)
+        if coeff != 0.0:
+            h_mean = _completion_mean(ent, row_end)
+            out = (loss - coeff * h_mean, lp.detach(), row_end, h_mean.detach(), loss.detach())
+        if return_entropy:
+            out += (ent.detach(),)
+        return out + (scored[2],) if return_cf else out
+    B, seq, _ = logits.shape
+    if not 0 < K < seq:
+        raise ValueError('logits_to_keep must lie in (0, L)')
+    if tuple(ref_per_token_logps.shape) != (B, K):
+        raise ValueError('ref_per_token_logps must be (B, logits_to_keep)')
+    logits = _contiguous_last(logits)
+    mode_code = _mode_code(mode, logits.dtype)
+    lp_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
+    lens = (K,) * B
+    labels = strip_pad_tail(input_ids, lens, 0, strip=False)
+    plan = _tail_plan(lens, seq, logits.stride(0), logits.stride(1), K, 0, -1, None, str(logits.device))
+    rlp = _contiguous_last(ref_per_token_logps.detach().to(lp_dtype))
+    adv = advantages.detach().float().contiguous().view(-1)
+    if adv.numel() != B:
+        raise ValueError('one advantage per sequence expected')
+    old = _old_log_probs(old, (B, K), lp_dtype)
+    tok = _contiguous_last(tokens.to(torch.int64))
+    ent = torch.zeros((B, K), dtype=torch.float32, device=logits.device) if return_entropy or coeff != 0.0 else None
+    cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_cf else None
+    out = _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code, ent, coeff,
+                             obj.args(), old, cf)
+    if return_entropy:
+        out += (ent,)
+    return out + (cf,) if return_cf else out
 
 
 # ---- reward-model pairwise loss -----------------------------------------------------------------------
@@ -1937,6 +2074,7 @@ class ActorObjective:
     clip_range_ratio_high: float | None = None
     dual_clip_ratio: float | None = None
     loss_agg_mode: str = 'seq-mean-token-mean'
+    _MODES = LOSS_AGG_MODES  # the aggregations this objective takes (a class attribute, not a field)
 
     def __post_init__(self):
         lo, hi, c = self.clip_range_ratio_low, self.clip_range_ratio_high, self.dual_clip_ratio
@@ -1946,8 +2084,8 @@ class ActorObjective:
             raise ValueError(f'clip_range_ratio_high must be >= 0, got {hi!r}')
         if c is not None and not (float(c) > 1.0 and math.isfinite(float(c))):
             raise ValueError(f'dual_clip_ratio must be None (off) or a finite value > 1, got {c!r}')
-        if self.loss_agg_mode not in LOSS_AGG_MODES:
-            raise ValueError(f'loss_agg_mode must be one of {sorted(LOSS_AGG_MODES)}, got {self.loss_agg_mode!r}')
+        if self.loss_agg_mode not in self._MODES:
+            raise ValueError(f'loss_agg_mode must be one of {sorted(self._MODES)}, got {self.loss_agg_mode!r}')
 
     @property
     def is_default(self) -> bool:
@@ -1965,7 +2103,43 @@ class ActorObjective:
         hi = float(clip_range_ratio if self.clip_range_ratio_high is None else self.clip_range_ratio_high)
         if not (0.0 <= lo < 1.0 and hi >= 0.0):
             raise ValueError(f'clip range [1 - {lo}, 1 + {hi}]: need 0 <= low < 1 and high >= 0')
-        return lo, hi, float(self.dual_clip_ratio or 0.0), LOSS_AGG_MODES[self.loss_agg_mode]
+        return lo, hi, float(self.dual_clip_ratio or 0.0), self._MODES[self.loss_agg_mode]
+
+
+# include/aa_b200.h AA_AGG_*: GRPO also takes Dr. GRPO's constant normaliser
+GRPO_LOSS_AGG_MODES = {**LOSS_AGG_MODES, 'seq-mean-token-sum-norm': 2}
+
+
+@dataclasses.dataclass(frozen=True)
+class GrpoObjective(ActorObjective):
+    """GRPO's clipped objective (DeepSeekMath's GRPO over several updates per rollout, with DAPO's clip-higher and
+    Dr. GRPO's aggregation), the fields and checks of ActorObjective with GRPO's defaults:
+
+        ratio = exp(lp - old_lp) ;  s = min(A * ratio, A * clamp(ratio, 1 - low, 1 + high))
+        dual-clip:  s = where(A < 0, max(s, dual_clip_ratio * A), s) ;  per-token loss = -(s - beta * KL_k3)
+        loss = (ptl * mask).sum() / mask.sum()                      ('token-mean', the default: the reference's loss)
+             = ((ptl * mask).sum(-1) / mask.sum(-1)).mean()         ('seq-mean-token-mean')
+             = (ptl * mask).sum() / (B * K)                         ('seq-mean-token-sum-norm', K = logits_to_keep)
+
+    clip_range_ratio: the ε of both bounds when clip_range_ratio_low / _high are None.  With old_lp = lp (the first
+    update of a rollout) the ratio is 1 and nothing is clipped.  Checked on the host when constructed."""
+
+    loss_agg_mode: str = 'token-mean'
+    clip_range_ratio: float = 0.2
+    _MODES = GRPO_LOSS_AGG_MODES
+
+    def __post_init__(self):
+        super().__post_init__()
+        self.args()  # the clip range with clip_range_ratio filled in
+
+    @property
+    def is_default(self) -> bool:
+        """The reference's loss when the ratio is 1: the kernels run today's launches."""
+        return (self.clip_range_ratio_low is None and self.clip_range_ratio_high is None and self.dual_clip_ratio is None
+                and self.loss_agg_mode == 'token-mean')
+
+    def args(self, clip_range_ratio: float | None = None) -> tuple[float, float, float, int]:
+        return super().args(self.clip_range_ratio if clip_range_ratio is None else clip_range_ratio)
 
 
 def _objective(objective: ActorObjective | None) -> ActorObjective | None:

@@ -16,7 +16,10 @@ swaps, without touching any reference file,
   * SupervisedTrainer.{loss, train_step} of the text / image / audio SFT trainers (cross-entropy from K1; the classes
     also get the `fused_lm_head` / `lm_head_chunk_rows` switches, off),
   * GRPOTrainer.{_get_per_token_logps, train_step} of the text trainer (the PPO and GRPO classes also get the
-    `fused_lm_head` / `lm_head_chunk_rows` / `log_entropy` / `entropy_coeff` switches, off; the PPO classes also the actor-objective switches), RMTrainer.{loss, train_step} of the text /
+    `fused_lm_head` / `lm_head_chunk_rows` / `log_entropy` / `entropy_coeff` switches, off; the PPO classes also the
+    actor-objective switches; the GRPO class also the GRPO-objective switches `num_iterations`, `clip_range_ratio`,
+    `clip_range_ratio_low`, `clip_range_ratio_high`, `dual_clip_ratio`, `loss_agg_mode`, `scale_rewards` and
+    `log_clip_fraction`, at the reference's single-update loss), RMTrainer.{loss, train_step} of the text /
     audio / video trainers (the audio and video trainers override `loss` with the text arithmetic, so their own `loss`
     is replaced too; the image trainers inherit both) and CMTrainer.{loss, train_step} of the text cost-model
     trainer (Safe RLHF's signed cost loss in one launch; the image cost-model trainer inherits both),
@@ -192,7 +195,9 @@ def install(trainers: bool = True, models: bool = True) -> dict[str, list[str]]:
                             _saved.append((cls, attr, cls.__dict__.get(attr, None)))
                             setattr(cls, attr, getattr(src, attr))
                 else:  # the switches the grafted step_from_rollout / _get_per_token_logps read
-                    for attr in ('fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff'):
+                    for attr in ('fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'num_iterations',
+                                 'clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio',
+                                 'loss_agg_mode', 'scale_rewards', 'log_clip_fraction'):
                         _saved.append((cls, attr, cls.__dict__.get(attr, None)))
                         setattr(cls, attr, getattr(src, attr))
             elif modname in _SFT_TARGETS:

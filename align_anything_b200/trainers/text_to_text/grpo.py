@@ -11,9 +11,36 @@ import torch
 
 from ... import ops
 from ...utils.multi_process import all_reduce_packed
-from .ppo import entropy_coeff_of, hidden_log_probs, lm_head_of
+from .ppo import entropy_coeff_of, hidden_log_probs, lm_head_of, switch_of
 
 __all__ = ['GRPOTrainer']
+
+GRPO_OBJECTIVE_KEYS = ('clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio',
+                       'loss_agg_mode')
+
+
+def num_iterations_of(tr) -> int:
+    """The updates per rollout in effect (switch_of `num_iterations`).  The reference sizes its LR schedule by
+    `train_cfgs.update_iters`, so a different `num_iterations` > 1 is refused here, before anything runs."""
+    mu = switch_of(tr, 'num_iterations')
+    if isinstance(mu, bool) or int(mu) != mu or int(mu) < 1:
+        raise ValueError(f'num_iterations must be an integer >= 1, got {mu!r}')
+    mu = int(mu)
+    tc = getattr(getattr(tr, 'cfgs', None), 'train_cfgs', None)
+    ui = getattr(tc, 'update_iters', None) if tc is not None else None
+    if mu > 1 and ui is not None and int(ui) != mu:
+        raise ValueError(f'num_iterations={mu} differs from train_cfgs.update_iters={ui}, which sizes the LR schedule')
+    return mu
+
+
+def grpo_objective_of(tr) -> ops.GrpoObjective | None:
+    """The GRPO objective in effect (switch_of each of GRPO_OBJECTIVE_KEYS), or None for the reference's loss and
+    today's launches: one update per rollout and every objective field at its default.  A bad value raises
+    ValueError here, before anything runs."""
+    fields = {k: switch_of(tr, k) for k in GRPO_OBJECTIVE_KEYS}
+    fields = {k: v for k, v in fields.items() if v is not None}
+    obj = ops.GrpoObjective(**fields)
+    return None if obj.is_default and num_iterations_of(tr) == 1 else obj
 
 
 class GRPOTrainer:
@@ -30,6 +57,23 @@ class GRPOTrainer:
     # mask (H: the step's own policy pass).  `cfgs.train_cfgs.entropy_coeff` overrides it when set; 0 leaves the step
     # unchanged.  train/loss stays GRPO's loss, train/actor_entropy carries the entropy term.
     entropy_coeff = 0.0
+    # GRPO's objective (ops.GrpoObjective).  num_iterations = mu updates per rollout (DeepSeekMath's GRPO; TRL's
+    # `num_iterations`): the advantages and the reference log-probs are computed once, the first update's detached
+    # log-probs are the old log-probs of the ratio exp(lp - old) for updates 2..mu.  The ratio is clipped to
+    # [1 - clip_range_ratio_low, 1 + clip_range_ratio_high] (None: clip_range_ratio); dual_clip_ratio c > 1 (None =
+    # off); loss_agg_mode 'token-mean' (the reference's), 'seq-mean-token-mean' or 'seq-mean-token-sum-norm' (Dr. GRPO,
+    # with scale_rewards False: advantages r - group mean).  `cfgs.train_cfgs.<key>` overrides each when set; the
+    # defaults are the reference's single-update step and today's launches.
+    num_iterations = 1
+    clip_range_ratio = 0.2
+    clip_range_ratio_low = None
+    clip_range_ratio_high = None
+    dual_clip_ratio = None
+    loss_agg_mode = 'token-mean'
+    scale_rewards = True
+    # Opt-in: train/actor_clip_fraction (and train/actor_dual_clip_fraction with dual-clip), the mean over the updates,
+    # in the step's one packed all-reduce
+    log_clip_fraction = False
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, tokenizer=None, *, beta=None,
                  num_generations=None) -> None:
@@ -56,64 +100,66 @@ class GRPOTrainer:
 
     # -- the arithmetic of train_step, trainers/text_to_text/grpo.py:268-318 ---------------------------
     def step_from_rollout(self, sequences: torch.Tensor, prompt_length: int, rewards: torch.Tensor) -> dict[str, Any]:
+        mu = num_iterations_of(self)
+        objective = grpo_objective_of(self)
+        log_cf = bool(switch_of(self, 'log_clip_fraction'))
         if self.fused_lm_head:  # refuse a head the fused path would get wrong before anything runs
             for model in (self.actor_reference_model, self.actor_model):
                 lm_head_of(model)
-        advantages = ops.group_advantages(rewards, self.num_generations)  # (B * G, 1)
+        advantages = ops.group_advantages(rewards, self.num_generations,
+                                          **({} if switch_of(self, 'scale_rewards') else {'scale': False}))  # (B * G, 1)
         attention_mask = (sequences != self.tokenizer.pad_token_id).long()
         logits_to_keep = sequences.size(1) - prompt_length
         # the frozen reference model is scored FIRST (the reference scores it second, :284-288): with its per-token
-        # log-probs at hand the policy's log-probs, the loss and d loss / d logits come out of ONE pass over the policy tile
+        # log-probs at hand the policy's log-probs, the loss and d loss / d logits come out of ONE pass over the policy
+        # tile.  It is scored once per rollout, however many updates follow.
         with torch.no_grad():
             ref_per_token_logps = self._get_per_token_logps(self.actor_reference_model, sequences, attention_mask,
                                                             logits_to_keep)
-        entropy = None
-        coeff = entropy_coeff_of(self)
-        entropy_mean = plain = None  # with the bonus: its entropy term and GRPO's loss without it
-        if self.fused_lm_head:  # the composed path: K1f needs a logits tile
-            want_entropy = self.log_entropy or coeff != 0.0
-            per_token_logps = self._get_per_token_logps(self.actor_model, sequences, attention_mask, logits_to_keep,
-                                                        return_entropy=want_entropy, entropy_grad=coeff != 0.0)
-            if want_entropy:
-                per_token_logps, entropy = per_token_logps
-            loss, row_end = ops.grpo_loss(per_token_logps, ref_per_token_logps, advantages,
-                                          sequences[:, -logits_to_keep:], self.tokenizer.eos_token_id, self.beta,
-                                          mode=self.mode)
-            if coeff != 0.0:  # K6b adds the entropy's gradient in its epilogue
-                entropy_mean = ops._completion_mean(entropy, row_end)
-                plain, loss = loss, loss - coeff * entropy_mean
-                entropy, entropy_mean = entropy.detach(), entropy_mean.detach()
-        else:
-            logits = self.actor_model(input_ids=sequences, attention_mask=attention_mask).logits
-            scored = ops.grpo_loss_from_logits(logits, sequences, logits_to_keep, ref_per_token_logps, advantages,
-                                               self.tokenizer.eos_token_id, self.beta, mode=self.mode,
-                                               return_entropy=self.log_entropy,
-                                               **({'entropy_coeff': coeff} if coeff != 0.0 else {}))
-            loss, row_end = scored[0], scored[2]
-            if coeff != 0.0:
-                entropy_mean, plain = scored[3], scored[4]
-            if self.log_entropy:
-                entropy = scored[-1]
-        self.actor_model.zero_grad()
-        self.actor_model.backward(loss)
-        self.actor_model.step()
+        kw = {}
+        if objective is not None:
+            kw['objective'] = objective
+        if log_cf:
+            kw['return_clip_fraction'] = True
+        old = None  # updates 2..mu: the first update's log-probs
+        plains, entropies, entropy_means, fracs = [], [], [], []
+        for _ in range(mu):
+            if old is not None:
+                kw['old_per_token_logps'] = old
+            loss, plain, entropy, entropy_mean, cf, lp, row_end = policy_update(
+                self, sequences, attention_mask, logits_to_keep, ref_per_token_logps, advantages, kw)
+            if old is None and mu > 1:
+                old = lp
+            plains.append(plain)
+            entropies.append(entropy)
+            entropy_means.append(entropy_mean)
+            fracs.append(cf)
         with torch.no_grad():
-            # train/loss is GRPO's loss, without the bonus
-            plain = (loss if plain is None else plain).detach().float()
-            lanes = [torch.stack([plain, rewards.float().mean()]), ops.status_lane(loss.device)]
+            # train/loss is GRPO's loss without the bonus, the mean over the updates
+            lanes = [torch.stack([_mean(plains), rewards.float().mean()]), ops.status_lane(loss.device)]
             if self.log_entropy:  # token mean over the completion mask (tokens up to and including the first eos)
                 mask = torch.arange(logits_to_keep, device=row_end.device) < row_end.unsqueeze(1)
-                lanes.append(((entropy * mask).sum() / mask.sum()).reshape(1))
-            if entropy_mean is not None:
-                lanes.append(entropy_mean.reshape(1))
-            # ONE collective, ONE sync (reference: 2 + 2); lane 2 = device status word, MAX over ranks
+                lanes.append(_mean([((e * mask).sum() / mask.sum()).reshape(1) for e in entropies]))
+            if entropy_means[0] is not None:
+                lanes.append(_mean([m.reshape(1) for m in entropy_means]))
+            dual = objective is not None and objective.dual_clip_ratio is not None
+            if log_cf:  # AVG lanes: the clip fraction (and the dual-clip fraction)
+                lanes.append(_mean(fracs)[:2 if dual else 1])
+            # ONE collective, ONE sync per rollout (reference: 2 + 2 per update); lane 2 = device status word, MAX
             v = all_reduce_packed(torch.cat(lanes), max_lanes=(2,)).tolist()
         ops.raise_for_status(v[2], loss.device)
         out = {'train/loss': v[0], 'train/reward': v[1]}
+        i = 3
         if self.log_entropy:
-            out['train/entropy'] = v[3]
-        if entropy_mean is not None:
-            out['train/actor_entropy'] = v[-1]
+            out['train/entropy'] = v[i]
+            i += 1
+        if entropy_means[0] is not None:
+            out['train/actor_entropy'] = v[i]
+            i += 1
+        if log_cf:
+            out['train/actor_clip_fraction'] = v[i]
+            if dual:
+                out['train/actor_dual_clip_fraction'] = v[i + 1]
         return out
 
     def train_step(self, prompt_batch: dict) -> dict[str, float]:
@@ -125,3 +171,53 @@ class GRPOTrainer:
         self.actor_model.train()
         rewards = self.compute_rewards(sequences, prompt_length)
         return self.step_from_rollout(sequences, prompt_length, rewards)
+
+
+def _mean(xs):
+    """The mean over the updates (one update: the value itself, bit for bit)."""
+    return xs[0] if len(xs) == 1 else torch.stack(xs).mean(0)
+
+
+def policy_update(tr, sequences, attention_mask, logits_to_keep, ref_per_token_logps, advantages, kw):
+    """One policy pass, backward and optimizer step of the trainer `tr` on the rollout -> (loss, GRPO's loss without
+    the bonus (fp32, detached), entropy or None, entropy term or None, clip fractions or None, detached log-probs,
+    row_end).  A function rather than a method, so that the grafted step_from_rollout of the reference's class finds
+    it without being grafted itself."""
+    entropy = cf = None
+    coeff = entropy_coeff_of(tr)
+    entropy_mean = plain = None  # with the bonus: its entropy term and GRPO's loss without it
+    if tr.fused_lm_head:  # the composed path: K1f needs a logits tile
+        want_entropy = tr.log_entropy or coeff != 0.0
+        per_token_logps = tr._get_per_token_logps(tr.actor_model, sequences, attention_mask, logits_to_keep,
+                                                    return_entropy=want_entropy, entropy_grad=coeff != 0.0)
+        if want_entropy:
+            per_token_logps, entropy = per_token_logps
+        scored = ops.grpo_loss(per_token_logps, ref_per_token_logps, advantages,
+                               sequences[:, -logits_to_keep:], tr.tokenizer.eos_token_id, tr.beta,
+                               mode=tr.mode, **kw)
+        loss, row_end = scored[0], scored[1]
+        if kw.get('return_clip_fraction'):
+            cf = scored[2]
+        lp = per_token_logps.detach()
+        if coeff != 0.0:  # K6b adds the entropy's gradient in its epilogue
+            entropy_mean = ops._completion_mean(entropy, row_end)
+            plain, loss = loss, loss - coeff * entropy_mean
+            entropy, entropy_mean = entropy.detach(), entropy_mean.detach()
+    else:
+        logits = tr.actor_model(input_ids=sequences, attention_mask=attention_mask).logits
+        scored = ops.grpo_loss_from_logits(logits, sequences, logits_to_keep, ref_per_token_logps, advantages,
+                                           tr.tokenizer.eos_token_id, tr.beta, mode=tr.mode,
+                                           return_entropy=tr.log_entropy,
+                                           **({'entropy_coeff': coeff} if coeff != 0.0 else {}), **kw)
+        if kw.get('return_clip_fraction'):
+            scored, cf = scored[:-1], scored[-1]
+        loss, lp, row_end = scored[0], scored[1], scored[2]
+        if coeff != 0.0:
+            entropy_mean, plain = scored[3], scored[4]
+        if tr.log_entropy:
+            entropy = scored[-1]
+    tr.actor_model.zero_grad()
+    tr.actor_model.backward(loss)
+    tr.actor_model.step()
+    plain = (loss if plain is None else plain).detach().float()
+    return loss, plain, entropy, entropy_mean, cf, lp, row_end

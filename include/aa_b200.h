@@ -8,6 +8,7 @@
  * function(s) whose arithmetic it replaces (file:line relative to the reference's
  * align_anything/ directory); the Python mirror in align_anything_b200/ keeps the
  * reference's names and signatures and calls these through ctypes (INTEGRATION.md).
+ * 54 entry points, ABI version 3.
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
@@ -379,7 +380,8 @@ int aa_ppo_actor_loss(const void *log_probs, int64_t lp_stride, const void *old_
  *   row_scratch          : fp32 [4 * B]
  * With clip_low == clip_high == clip_range_ratio, dual_clip 0 and AA_AGG_SEQ_MEAN_TOKEN_MEAN the loss and gradient
  * are bit-identical to aa_ppo_actor_loss.  Arguments are checked before any CUDA call. */
-enum { AA_AGG_SEQ_MEAN_TOKEN_MEAN = 0, AA_AGG_TOKEN_MEAN = 1 };
+/* AA_AGG_SEQ_MEAN_TOKEN_SUM_NORM (Dr. GRPO: sum(loss * mask) / (B * K)) is taken by the GRPO objective entry points only. */
+enum { AA_AGG_SEQ_MEAN_TOKEN_MEAN = 0, AA_AGG_TOKEN_MEAN = 1, AA_AGG_SEQ_MEAN_TOKEN_SUM_NORM = 2 };
 int aa_ppo_actor_loss_obj(const void *log_probs, int64_t lp_stride, const void *old_log_probs, int64_t old_stride,
                           int lp_dtype, const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
                           int64_t mask_stride, int32_t B, int32_t Wm, float clip_low, float clip_high, float dual_clip,
@@ -508,6 +510,22 @@ int aa_logprob_grpo_fused_entropy_grad(const void *logits, int logits_dtype, int
                                        float beta, int mode, void *grad_logits, int64_t grad_row_stride,
                                        void *row_scratch, int32_t *row_end, float *total, uint32_t *counter,
                                        int32_t *status, float *entropy, float entropy_coeff, void *stream);
+/* aa_logprob_grpo_fused with GRPO's clipped objective (aa_grpo_loss_obj's per-token loss and aggregation; clip_low,
+ * clip_high, dual_clip, loss_agg: same meaning and checks).  old_log_probs: NULL (the ratio is exp(lp - lp) = 1: the
+ * first update of a rollout) or the rollout-time policy log-probs (lp_dtype, laid out exactly like log_probs: read at
+ * the log-prob's own index).  entropy == NULL: the plain kernel; otherwise entropy is written as by
+ * aa_logprob_grpo_fused_entropy and, with entropy_coeff != 0, the tile carries the bonus's gradient with
+ * g_H = -entropy_coeff / total (a token mean over the completion mask under every aggregation).  The loss VALUE and the
+ * clip fractions are aa_grpo_loss_obj on `log_probs`. */
+int aa_logprob_grpo_fused_obj(const void *logits, int logits_dtype, int64_t row_stride, int32_t V, const int64_t *labels,
+                              int32_t n_segments, const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                              const int64_t *seg_out_off, const int64_t *seg_cum, const int64_t *seg_tile_row,
+                              int64_t n_tile_rows, void *log_probs, int lp_dtype, const void *ref_log_probs,
+                              int64_t ref_stride, const void *old_log_probs, const float *advantages,
+                              const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t K, float beta,
+                              float clip_low, float clip_high, float dual_clip, int loss_agg, int mode, void *grad_logits,
+                              int64_t grad_row_stride, void *row_scratch, int32_t *row_end, float *total,
+                              uint32_t *counter, int32_t *status, float *entropy, float entropy_coeff, void *stream);
 
 /* tile[0..n) *= *scale unless *scale == 1 (checked on the device: the usual `loss.backward()` costs one empty launch).
  * Contiguous tile; scale: device scalar of scale_dtype.  The autograd backward of the K1f node. */
@@ -537,6 +555,25 @@ int aa_grpo_loss(const void *log_probs, int64_t lp_stride, const void *ref_log_p
                  const float *advantages, const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id,
                  int32_t B, int32_t K, float beta, int mode, float *loss, void *grad, int64_t grad_stride,
                  int32_t *row_end, float *scratch, uint32_t *counter, void *stream);
+/* Dr. GRPO's advantages: r - group mean, no std scaling (the group mean as aa_group_advantages computes it). */
+int aa_group_advantages_centered(const float *rewards, int32_t n_groups, int32_t group_size, float *advantages,
+                                 void *stream);
+/* aa_grpo_loss with GRPO's clipped objective.  With r = exp(lp - old):
+ *   s = min(A * r, A * clamp(r, 1 - clip_low, 1 + clip_high)); dual_clip c > 1 (0 = off): s = max(s, c * A) where A < 0;
+ *   per-token loss = -(s - beta * KL)  (the KL of aa_grpo_loss);
+ *   loss_agg: AA_AGG_TOKEN_MEAN  sum(loss * mask) / sum(mask)  (aa_grpo_loss's aggregation),
+ *             AA_AGG_SEQ_MEAN_TOKEN_MEAN  the mean over rows of each row's token mean,
+ *             AA_AGG_SEQ_MEAN_TOKEN_SUM_NORM  sum(loss * mask) / (B * K).
+ *   old_log_probs: lp_dtype with row stride old_stride, or NULL for the log-probs themselves (r == 1).
+ *   clip_frac: optional fp32[2] as aa_ppo_actor_loss_obj's (seq-mean-token-mean: mean of the row fractions; the other
+ *              two aggregations: token fractions over the completion mask).
+ * Arguments are checked before any CUDA call; scratch: fp32 [1 + 4 * B]; counter: uint32 [2], zeroed once. */
+int aa_grpo_loss_obj(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
+                     const void *old_log_probs, int64_t old_stride, int lp_dtype, const float *advantages,
+                     const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B, int32_t K,
+                     float beta, float clip_low, float clip_high, float dual_clip, int loss_agg, int mode, float *loss,
+                     void *grad, int64_t grad_stride, float *clip_frac, int32_t *row_end, float *scratch,
+                     uint32_t *counter, void *stream);
 
 /* masked_mean (utils/tools.py:460-467): mean over rows of masked row means -> out[0];
  * mask == NULL: plain mean. */
