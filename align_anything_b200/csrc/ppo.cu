@@ -593,36 +593,6 @@ struct GrpoParams {
   uint32_t *counter;
 };
 
-template <int THREADS>
-__global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoParams p) {
-  __shared__ float scratch[33];
-  const int b = blockIdx.x, tid = threadIdx.x, r = p.r_lp;
-  const int end = p.row_end[b];
-  const float cnt = p.total[0];
-  const float A = p.adv[b];
-  const float g_t = 1.f / cnt;  // d loss / d per_token_loss on counted tokens (fp32, like the reference)
-  float row = 0.f;
-  for (int t = tid; t < p.K; t += THREADS) {
-    const bool on = t < end;
-    const float lp = load_as_float(p.lp, b * p.lp_stride + t, p.dtype);
-    const float rf = load_as_float(p.ref_lp, b * p.ref_stride + t, p.dtype);
-    float ptl, g;
-    grpo_token(lp, rf, A, on, g_t, p.beta, r, ptl, g);
-    if (on) row += ptl;
-    if (p.grad) {
-      store_from_float(p.grad, b * p.grad_stride + t, p.dtype, g);
-    }
-  }
-  row = block_sum<THREADS>(row, scratch);
-  if (tid == 0) p.row_scratch[b] = row;
-  if (!last_block_arrives(p.counter, gridDim.x)) return;
-  const volatile float *rows = p.row_scratch;
-  float acc = 0.f;
-  for (int k = tid; k < p.B; k += THREADS) acc += rows[k];
-  acc = block_sum<THREADS>(acc, scratch);
-  if (tid == 0) p.loss[0] = acc / cnt;
-}
-
 // Dr. GRPO's advantages: r - group mean (the mean of group_advantages_kernel), no std scaling
 __global__ void __launch_bounds__(32)
     group_centered_kernel(const float *__restrict__ rewards, int n_groups, int G, float *__restrict__ adv) {
@@ -643,9 +613,12 @@ struct GrpoObjParams {
   float *clip_frac;  // optional fp32[2]; row_scratch then holds 4 * B floats
 };
 
-// aa_grpo_loss_obj: GRPO's clipped objective (grpo_obj_token) under one of the three aggregations
-template <int THREADS>
-__global__ void __launch_bounds__(THREADS) grpo_loss_obj_kernel(const GrpoObjParams q) {
+// GRPO's loss and d loss / d lp, one block per row, the last block to arrive reduces the rows.  OBJECTIVE: the clipped
+// objective (grpo_obj_token) under one of the three aggregations (aa_grpo_loss_obj); otherwise the reference's loss
+// (grpo_token, aa_grpo_loss), which passes agg = token-mean, old = clip_frac = nullptr: g_t = 1 / total, the row
+// partial is the fp32 row sum and the loss acc / total, as the reference computes them
+template <int THREADS, bool OBJECTIVE>
+__global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoObjParams q) {
   __shared__ float scratch[33];
   const GrpoParams &p = q.base;
   const int b = blockIdx.x, tid = threadIdx.x, r = p.r_lp;
@@ -658,10 +631,14 @@ __global__ void __launch_bounds__(THREADS) grpo_loss_obj_kernel(const GrpoObjPar
     const bool on = t < end;
     const float lp = load_as_float(p.lp, b * p.lp_stride + t, p.dtype);
     const float rf = load_as_float(p.ref_lp, b * p.ref_stride + t, p.dtype);
-    const float old = q.old ? load_as_float(q.old, b * q.old_stride + t, p.dtype) : lp;
     float ptl, g;
-    int why;
-    grpo_obj_token(lp, old, rf, A, on, g_t, p.beta, q.clip_lo, q.clip_hi, q.dual, r, ptl, g, why);
+    int why = 0;
+    if constexpr (OBJECTIVE) {
+      const float old = q.old ? load_as_float(q.old, b * q.old_stride + t, p.dtype) : lp;
+      grpo_obj_token(lp, old, rf, A, on, g_t, p.beta, q.clip_lo, q.clip_hi, q.dual, r, ptl, g, why);
+    } else {
+      grpo_token(lp, rf, A, on, g_t, p.beta, r, ptl, g);
+    }
     if (on) {
       row += ptl;
       n_clip += (why & 1) ? 1.f : 0.f;
@@ -974,23 +951,48 @@ extern "C" int aa_group_advantages(const float *rewards, int32_t n_groups, int32
   return check_launch("aa_group_advantages");
 }
 
+// aa_grpo_loss (objective false: the reference's loss, any mode) and aa_grpo_loss_obj: the checks, the completion mask
+// (row_end, and the token count in scratch[0]) and the loss kernel over scratch + 1
+static int grpo_loss(bool objective, const void *log_probs, int64_t lp_stride, const void *ref_log_probs,
+                     int64_t ref_stride, const void *old_log_probs, int64_t old_stride, int lp_dtype,
+                     const float *advantages, const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id,
+                     int32_t B, int32_t K, float beta, float clip_low, float clip_high, float dual_clip, int loss_agg,
+                     int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac, int32_t *row_end,
+                     float *scratch, uint32_t *counter, void *stream) {
+  const char *who = objective ? "aa_grpo_loss_obj" : "aa_grpo_loss";
+  AA_REQUIRE(B > 0 && K > 0 && log_probs && ref_log_probs && advantages && completion_tokens && loss && row_end &&
+                 scratch && counter,
+             AA_ERR_ARG, "%s: bad arguments", who);
+  AA_REQUIRE(dtype_ok(lp_dtype), AA_ERR_DTYPE, "%s: bad dtype", who);
+  if (objective) {
+    AA_REQUIRE(grpo_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
+               "%s: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a known loss_agg; got "
+               "%g %g %g %d)", who, clip_low, clip_high, dual_clip, loss_agg);
+    AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "%s: bad mode", who);
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  grpo_mask_kernel<128><<<B, 128, 0, st>>>(completion_tokens, tok_stride, B, K, eos_id, row_end, scratch, counter);
+  int rc = check_launch(objective ? "aa_grpo_loss_obj(mask)" : "aa_grpo_loss(mask)");
+  if (rc) return rc;
+  GrpoObjParams q{GrpoParams{log_probs, ref_log_probs, lp_dtype, lp_stride, ref_stride, advantages, row_end, scratch, B,
+                             K, beta, (mode == AA_MODE_FAITHFUL) ? lp_dtype : AA_F32, loss, grad, grad_stride,
+                             scratch + 1, counter + 1},
+                  old_log_probs, old_stride, clip_low, clip_high, dual_clip, loss_agg, clip_frac};
+  if (objective)
+    grpo_loss_kernel<128, true><<<B, 128, 0, st>>>(q);
+  else
+    grpo_loss_kernel<128, false><<<B, 128, 0, st>>>(q);
+  return check_launch(who);
+}
+
 extern "C" int aa_grpo_loss(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
                             int lp_dtype, const float *advantages, const int64_t *completion_tokens,
                             int64_t tok_stride, int64_t eos_id, int32_t B, int32_t K, float beta, int mode,
                             float *loss, void *grad, int64_t grad_stride, int32_t *row_end, float *scratch,
                             uint32_t *counter, void *stream) {
-  AA_REQUIRE(B > 0 && K > 0 && log_probs && ref_log_probs && advantages && completion_tokens && loss && row_end &&
-                 scratch && counter,
-             AA_ERR_ARG, "aa_grpo_loss: bad arguments");
-  AA_REQUIRE(dtype_ok(lp_dtype), AA_ERR_DTYPE, "aa_grpo_loss: bad dtype");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  grpo_mask_kernel<128><<<B, 128, 0, st>>>(completion_tokens, tok_stride, B, K, eos_id, row_end, scratch, counter);
-  int rc = check_launch("aa_grpo_loss(mask)");
-  if (rc) return rc;
-  GrpoParams p{log_probs, ref_log_probs, lp_dtype, lp_stride, ref_stride, advantages, row_end, scratch, B, K, beta,
-               (mode == AA_MODE_FAITHFUL) ? lp_dtype : AA_F32, loss, grad, grad_stride, scratch + 1, counter + 1};
-  grpo_loss_kernel<128><<<B, 128, 0, st>>>(p);
-  return check_launch("aa_grpo_loss");
+  return grpo_loss(false, log_probs, lp_stride, ref_log_probs, ref_stride, nullptr, 0, lp_dtype, advantages,
+                   completion_tokens, tok_stride, eos_id, B, K, beta, 0.f, 0.f, 0.f, AA_AGG_TOKEN_MEAN, mode, loss, grad,
+                   grad_stride, nullptr, row_end, scratch, counter, stream);
 }
 
 extern "C" int aa_group_advantages_centered(const float *rewards, int32_t n_groups, int32_t group_size,
@@ -1008,24 +1010,9 @@ extern "C" int aa_grpo_loss_obj(const void *log_probs, int64_t lp_stride, const 
                                 int32_t K, float beta, float clip_low, float clip_high, float dual_clip, int loss_agg,
                                 int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac,
                                 int32_t *row_end, float *scratch, uint32_t *counter, void *stream) {
-  AA_REQUIRE(B > 0 && K > 0 && log_probs && ref_log_probs && advantages && completion_tokens && loss && row_end &&
-                 scratch && counter,
-             AA_ERR_ARG, "aa_grpo_loss_obj: bad arguments");
-  AA_REQUIRE(dtype_ok(lp_dtype), AA_ERR_DTYPE, "aa_grpo_loss_obj: bad dtype");
-  AA_REQUIRE(grpo_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
-             "aa_grpo_loss_obj: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a known "
-             "loss_agg; got %g %g %g %d)", clip_low, clip_high, dual_clip, loss_agg);
-  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_grpo_loss_obj: bad mode");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  grpo_mask_kernel<128><<<B, 128, 0, st>>>(completion_tokens, tok_stride, B, K, eos_id, row_end, scratch, counter);
-  int rc = check_launch("aa_grpo_loss_obj(mask)");
-  if (rc) return rc;
-  GrpoObjParams q{GrpoParams{log_probs, ref_log_probs, lp_dtype, lp_stride, ref_stride, advantages, row_end, scratch, B,
-                             K, beta, (mode == AA_MODE_FAITHFUL) ? lp_dtype : AA_F32, loss, grad, grad_stride,
-                             scratch + 1, counter + 1},
-                  old_log_probs, old_stride, clip_low, clip_high, dual_clip, loss_agg, clip_frac};
-  grpo_loss_obj_kernel<128><<<B, 128, 0, st>>>(q);
-  return check_launch("aa_grpo_loss_obj");
+  return grpo_loss(true, log_probs, lp_stride, ref_log_probs, ref_stride, old_log_probs, old_stride, lp_dtype, advantages,
+                   completion_tokens, tok_stride, eos_id, B, K, beta, clip_low, clip_high, dual_clip, loss_agg, mode, loss,
+                   grad, grad_stride, clip_frac, row_end, scratch, counter, stream);
 }
 
 extern "C" int aa_nll_mean(const void *logp, int dtype, const int64_t *labels, int64_t n, int64_t ignore_index,

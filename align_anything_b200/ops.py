@@ -1142,42 +1142,17 @@ def group_advantages(rewards: torch.Tensor, num_generations: int, scale: bool = 
 
 
 class _GrpoLossFn(torch.autograd.Function):
+    """GRPO's loss over per-token log-probs: the forward writes the loss and d loss / d lp in one launch
+    (_grpo_loss_launch); obj / old / clip_frac select and feed the clipped objective."""
+
     @staticmethod
-    def forward(ctx, lp, ref_lp, adv, tokens, eos_id, beta, mode_code):
+    def forward(ctx, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj=None, old=None, clip_frac=None):
         B, K = lp.shape
         dev = lp.device
         loss = torch.empty(1, dtype=torch.float32, device=dev)
         grad = torch.empty((B, K), dtype=lp.dtype, device=dev)
         row_end = torch.empty(B, dtype=torch.int32, device=dev)
-        scratch = torch.empty(B + 1, dtype=torch.float32, device=dev)
-        sc = _device_scratch(dev)
-        L.check(L.lib().aa_grpo_loss(lp.data_ptr(), lp.stride(0), ref_lp.data_ptr(), ref_lp.stride(0), L.dtype_code(lp.dtype),
-                                     adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), B, K, float(beta),
-                                     mode_code, loss.data_ptr(), grad.data_ptr(), grad.stride(0), row_end.data_ptr(),
-                                     scratch.data_ptr(), sc['counter'][5:7].data_ptr(), L.stream_ptr(dev)))
-        ctx.save_for_backward(grad)
-        ctx.mark_non_differentiable(row_end)
-        return loss[0], row_end
-
-    @staticmethod
-    def backward(ctx, g, _):
-        (grad,) = ctx.saved_tensors
-        return (grad.float() * g.float()).to(grad.dtype), None, None, None, None, None, None
-
-
-class _GrpoLossObjFn(torch.autograd.Function):
-    """aa_grpo_loss_obj: GRPO's clipped objective; forward writes the loss and d loss / d lp in one launch."""
-
-    @staticmethod
-    def forward(ctx, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, clip_frac):
-        B, K = lp.shape
-        dev = lp.device
-        loss = torch.empty(1, dtype=torch.float32, device=dev)
-        grad = torch.empty((B, K), dtype=lp.dtype, device=dev)
-        row_end = torch.empty(B, dtype=torch.int32, device=dev)
-        scratch = torch.empty(1 + 4 * B, dtype=torch.float32, device=dev)
-        _grpo_loss_obj_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac,
-                              row_end, scratch)
+        _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end)
         ctx.save_for_backward(grad)
         ctx.mark_non_differentiable(row_end)
         return loss[0], row_end
@@ -1188,25 +1163,35 @@ class _GrpoLossObjFn(torch.autograd.Function):
         return (grad.float() * g.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None
 
 
-def _grpo_loss_obj_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
-                          scratch):
-    """aa_grpo_loss_obj; obj = GrpoObjective.args(), old: the old log-probs or None (the log-probs themselves)."""
+def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
+                      scratch=None):
+    """GRPO's loss kernel, writing loss, row_end and (unless None) grad.  obj None: the reference loss (aa_grpo_loss);
+    otherwise obj = GrpoObjective.args() for aa_grpo_loss_obj, old = the old log-probs (None: the log-probs
+    themselves, ratio 1) and clip_frac = an fp32[2] tensor for the clip fractions or None.  scratch (fp32): the token
+    count and the row sums, B + 1 values, and under the objective the rows' clip counts too, 1 + 4 B; None allocates it."""
     B, K = lp.shape
-    lo, hi, dual, agg = obj
-    L.check(L.lib().aa_grpo_loss_obj(
-        lp.data_ptr(), lp.stride(0), ref_lp.data_ptr(), ref_lp.stride(0), L.ptr(old), old.stride(0) if old is not None else 0,
-        L.dtype_code(lp.dtype), adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), B, K, float(beta),
-        float(lo), float(hi), float(dual), int(agg), mode_code, loss.data_ptr(), L.ptr(grad),
-        grad.stride(0) if grad is not None else 0, L.ptr(clip_frac), row_end.data_ptr(), scratch.data_ptr(),
-        _device_scratch(lp.device)['counter'][5:7].data_ptr(), L.stream_ptr(lp.device)))
+    dev = lp.device
+    if scratch is None:
+        scratch = torch.empty(B + 1 if obj is None else 1 + 4 * B, dtype=torch.float32, device=dev)
+    lib = L.lib()
+    lps = (lp.data_ptr(), lp.stride(0), ref_lp.data_ptr(), ref_lp.stride(0))
+    rows = (L.dtype_code(lp.dtype), adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), B, K, float(beta))
+    out = (loss.data_ptr(), L.ptr(grad), grad.stride(0) if grad is not None else 0)
+    tail = (row_end.data_ptr(), scratch.data_ptr(), _device_scratch(dev)['counter'][5:7].data_ptr(), L.stream_ptr(dev))
+    if obj is None:
+        L.check(lib.aa_grpo_loss(*lps, *rows, mode_code, *out, *tail))
+    else:
+        L.check(lib.aa_grpo_loss_obj(*lps, L.ptr(old), old.stride(0) if old is not None else 0, *rows, *obj, mode_code,
+                                     *out, L.ptr(clip_frac), *tail))
 
 
-def _grpo_objective(objective) -> GrpoObjective | None:
-    if objective is None:
+def _grpo_objective_args(objective, old, return_clip_fraction: bool):
+    """The one rule for GRPO's reference loss -- no objective or one with default fields, no old log-probs and no clip
+    fractions: None, and the nodes run today's launches.  Otherwise GrpoObjective.args() for the objective kernels
+    (a default objective still gives its clip_range_ratio)."""
+    if _objective(objective, GrpoObjective) is None and old is None and not return_clip_fraction:
         return None
-    if not isinstance(objective, GrpoObjective):
-        raise TypeError(f'objective must be an ops.GrpoObjective, got {type(objective).__name__}')
-    return objective
+    return (objective or GrpoObjective()).args()
 
 
 def _old_log_probs(old, shape, dtype):
@@ -1229,7 +1214,7 @@ def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, 
     objective (aa_grpo_loss_obj) with ratio exp(lp - old); without old_per_token_logps the ratio is 1.  None / default
     fields and no old log-probs: today's launch.  return_clip_fraction appends the fp32[2] clip fractions."""
     L.require_cuda(per_token_logps, ref_per_token_logps, advantages, completion_tokens)
-    obj = _grpo_objective(objective)
+    obj = _grpo_objective_args(objective, old_per_token_logps, return_clip_fraction)
     if per_token_logps.dim() != 2 or per_token_logps.shape != ref_per_token_logps.shape or \
             completion_tokens.shape != per_token_logps.shape:
         raise ValueError('per-token log-probs and completion tokens must all be (B, K)')
@@ -1240,11 +1225,8 @@ def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, 
         raise ValueError('one advantage per sequence expected')
     old = _old_log_probs(old_per_token_logps, lp.shape, lp.dtype)
     tok = _contiguous_last(completion_tokens.to(torch.int64))
-    if (obj is None or obj.is_default) and old is None and not return_clip_fraction:
-        return _GrpoLossFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype))
-    args = (obj or GrpoObjective()).args()
     cf = torch.zeros(2, dtype=torch.float32, device=lp.device) if return_clip_fraction else None
-    out = _GrpoLossObjFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype), args, old, cf)
+    out = _GrpoLossFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype), obj, old, cf)
     return out + (cf,) if return_clip_fraction else out
 
 
@@ -1286,40 +1268,12 @@ class _GrpoFusedFn(torch.autograd.Function):
         grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
         rows = torch.empty(plan.n_tile_rows * 6, dtype=torch.int64, device=dev)  # 48 bytes per tile row
         row_end = torch.empty(B, dtype=torch.int32, device=dev)
-        scratch = torch.empty(B + 1, dtype=torch.float32, device=dev)
+        scratch = torch.empty(B + 1, dtype=torch.float32, device=dev)  # K1f's token count; aa_grpo_loss's scratch too
         loss = torch.empty(1, dtype=torch.float32, device=dev)
-        sc = _device_scratch(dev)
-        p = plan.ptrs()
-        lib = L.lib()
-        args = (logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), labels.data_ptr(),
-                plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp_dtype),
-                ref_lp.data_ptr(), ref_lp.stride(0), adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), K,
-                float(beta), mode_code, grad.data_ptr(), logits.size(-1), rows.data_ptr(), row_end.data_ptr(),
-                scratch.data_ptr(), sc['counter'][5:6].data_ptr(), sc['status'].data_ptr())
-        if obj is not None:
-            o = (logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), labels.data_ptr(),
-                 plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp_dtype),
-                 ref_lp.data_ptr(), ref_lp.stride(0), L.ptr(old), adv.data_ptr(), tokens.data_ptr(), tokens.stride(0),
-                 int(eos_id), K, float(beta), float(obj[0]), float(obj[1]), float(obj[2]), int(obj[3]), mode_code,
-                 grad.data_ptr(), logits.size(-1), rows.data_ptr(), row_end.data_ptr(), scratch.data_ptr(),
-                 sc['counter'][5:6].data_ptr(), sc['status'].data_ptr(), L.ptr(entropy), float(entropy_coeff))
-            L.check(lib.aa_logprob_grpo_fused_obj(*o, L.stream_ptr(dev)))
-            scratch = torch.empty(1 + 4 * B, dtype=torch.float32, device=dev)
-            _grpo_loss_obj_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, None, clip_frac,
-                                  row_end, scratch)
-        elif entropy is None:
-            L.check(lib.aa_logprob_grpo_fused(*args, L.stream_ptr(dev)))
-        elif entropy_coeff == 0.0:  # the same launch with the entropy of every completion row from its (max, sum-exp) pass
-            L.check(lib.aa_logprob_grpo_fused_entropy(*args, entropy.data_ptr(), L.stream_ptr(dev)))
-        else:  # ... and the entropy bonus's gradient in the tile
-            L.check(lib.aa_logprob_grpo_fused_entropy_grad(*args, entropy.data_ptr(), float(entropy_coeff),
-                                                           L.stream_ptr(dev)))
-        if obj is None:
-            L.check(lib.aa_grpo_loss(lp.data_ptr(), lp.stride(0), ref_lp.data_ptr(), ref_lp.stride(0),
-                                     L.dtype_code(lp_dtype), adv.data_ptr(), tokens.data_ptr(), tokens.stride(0),
-                                     int(eos_id), B, K, float(beta), mode_code, loss.data_ptr(), None, 0,
-                                     row_end.data_ptr(), scratch.data_ptr(), sc['counter'][5:7].data_ptr(),
-                                     L.stream_ptr(dev)))
+        _k1f_grpo_launch(logits, labels, plan, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, grad, rows, row_end,
+                         scratch, entropy, entropy_coeff, obj, old)
+        _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, None, clip_frac, row_end,
+                          scratch if obj is None else None)
         ctx.save_for_backward(grad)
         if entropy_coeff == 0.0:
             ctx.mark_non_differentiable(lp, row_end)
@@ -1333,6 +1287,34 @@ class _GrpoFusedFn(torch.autograd.Function):
     def backward(ctx, g, *_unused):
         (grad,) = _hand_over_once(ctx, g, *ctx.saved_tensors)
         return grad, None, None, None, None, None, None, None, None, None, None, None, None, None
+
+
+def _k1f_grpo_launch(logits, labels, plan, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, grad, rows, row_end,
+                     total, entropy, entropy_coeff, obj, old):
+    """K1f over GRPO's completion rows (`rows`: its int64 row records, 6 per tile row), writing lp, row_end, the token
+    count `total[0]`, the gradient tile `grad` and (unless None) the fp32 entropy.  obj: GrpoObjective.args() for the objective entry point (aa_logprob_grpo_fused_obj, old: the old
+    log-probs or None); None: the reference loss, plain, with the entropy, or with the entropy bonus's gradient."""
+    dev = logits.device
+    K = plan.out_shape[1]
+    sc = _device_scratch(dev)
+    p = plan.ptrs()
+    lib = L.lib()
+    head = (logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), labels.data_ptr(),
+            plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp.dtype),
+            ref_lp.data_ptr(), ref_lp.stride(0))
+    mid = (adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), K, float(beta))
+    tail = (mode_code, grad.data_ptr(), logits.size(-1), rows.data_ptr(), row_end.data_ptr(), total.data_ptr(),
+            sc['counter'][5:6].data_ptr(), sc['status'].data_ptr())
+    if obj is not None:
+        L.check(lib.aa_logprob_grpo_fused_obj(*head, L.ptr(old), *mid, *obj, *tail, L.ptr(entropy),
+                                              float(entropy_coeff), L.stream_ptr(dev)))
+    elif entropy is None:
+        L.check(lib.aa_logprob_grpo_fused(*head, *mid, *tail, L.stream_ptr(dev)))
+    elif entropy_coeff == 0.0:  # the same launch with the entropy of every completion row from its (max, sum-exp) pass
+        L.check(lib.aa_logprob_grpo_fused_entropy(*head, *mid, *tail, entropy.data_ptr(), L.stream_ptr(dev)))
+    else:  # ... and the entropy bonus's gradient in the tile
+        L.check(lib.aa_logprob_grpo_fused_entropy_grad(*head, *mid, *tail, entropy.data_ptr(), float(entropy_coeff),
+                                                       L.stream_ptr(dev)))
 
 
 def _completion_mean(x: torch.Tensor, row_end: torch.Tensor) -> torch.Tensor:
@@ -1359,57 +1341,10 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
     aa_grpo_loss_obj -> K1b); the entropy bonus stays a token mean over the completion mask.  return_clip_fraction
     appends the fp32[2] clip fractions last.  None / default fields and no old log-probs: today's launches."""
     L.require_cuda(logits, input_ids, ref_per_token_logps, advantages)
-    obj = _grpo_objective(objective)
-    if (obj is not None and not obj.is_default) or old_per_token_logps is not None or return_clip_fraction:
-        return _grpo_objective_from_logits(logits, input_ids, int(logits_to_keep), ref_per_token_logps, advantages,
-                                           eos_token_id, beta, mode, return_entropy, float(entropy_coeff),
-                                           obj or GrpoObjective(), old_per_token_logps, return_clip_fraction)
+    obj = _grpo_objective_args(objective, old_per_token_logps, return_clip_fraction)
     K = int(logits_to_keep)
     tokens = input_ids[:, -K:]
     coeff = float(entropy_coeff)
-    if not _single_pass_ok(logits, _FUSED_GRPO, torch.is_grad_enabled() and logits.requires_grad):
-        if coeff != 0.0:
-            lp, ent = tail_token_log_probs(logits, input_ids, K, mode=mode, return_entropy=True, entropy_grad=True)
-            loss, row_end = grpo_loss(lp, ref_per_token_logps, advantages, tokens, eos_token_id, beta, mode=mode)
-            h_mean = _completion_mean(ent, row_end)
-            out = (loss - coeff * h_mean, lp.detach(), row_end, h_mean.detach(), loss.detach())
-            return out + (ent.detach(),) if return_entropy else out
-        if return_entropy:
-            lp, ent = tail_token_log_probs(logits, input_ids, K, mode=mode, return_entropy=True)
-        else:
-            lp = tail_token_log_probs(logits, input_ids, K, mode=mode)
-        loss, row_end = grpo_loss(lp, ref_per_token_logps, advantages, tokens, eos_token_id, beta, mode=mode)
-        return (loss, lp.detach(), row_end, ent) if return_entropy else (loss, lp.detach(), row_end)
-    B, seq, _ = logits.shape
-    if not 0 < K < seq:
-        raise ValueError('logits_to_keep must lie in (0, L)')
-    if tuple(ref_per_token_logps.shape) != (B, K):
-        raise ValueError('ref_per_token_logps must be (B, logits_to_keep)')
-    logits = _contiguous_last(logits)
-    mode_code = _mode_code(mode, logits.dtype)
-    lp_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
-    lens = (K,) * B
-    labels = strip_pad_tail(input_ids, lens, 0, strip=False)
-    plan = _tail_plan(lens, seq, logits.stride(0), logits.stride(1), K, 0, -1, None, str(logits.device))
-    rlp = _contiguous_last(ref_per_token_logps.detach().to(lp_dtype))
-    adv = advantages.detach().float().contiguous().view(-1)
-    if adv.numel() != B:
-        raise ValueError('one advantage per sequence expected')
-    tok = _contiguous_last(tokens.to(torch.int64))
-    if not return_entropy and coeff == 0.0:
-        return _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code)
-    ent = torch.zeros((B, K), dtype=torch.float32, device=logits.device)
-    if coeff == 0.0:
-        return _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code,
-                                  ent) + (ent,)
-    out = _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code, ent, coeff)
-    return out + (ent,) if return_entropy else out
-
-
-def _grpo_objective_from_logits(logits, input_ids, K, ref_per_token_logps, advantages, eos_token_id, beta, mode,
-                                return_entropy, coeff, obj, old, return_cf):
-    """grpo_loss_from_logits under GRPO's clipped objective (the same outputs, then the clip fractions)."""
-    tokens = input_ids[:, -K:]
     if not _single_pass_ok(logits, _FUSED_GRPO, torch.is_grad_enabled() and logits.requires_grad):
         ent = None
         if return_entropy or coeff != 0.0:
@@ -1417,8 +1352,9 @@ def _grpo_objective_from_logits(logits, input_ids, K, ref_per_token_logps, advan
                                            entropy_grad=coeff != 0.0)
         else:
             lp = tail_token_log_probs(logits, input_ids, K, mode=mode)
-        scored = grpo_loss(lp, ref_per_token_logps, advantages, tokens, eos_token_id, beta, mode=mode, objective=obj,
-                           old_per_token_logps=old, return_clip_fraction=return_cf)
+        scored = grpo_loss(lp, ref_per_token_logps, advantages, tokens, eos_token_id, beta, mode=mode,
+                           objective=objective, old_per_token_logps=old_per_token_logps,
+                           return_clip_fraction=return_clip_fraction)
         loss, row_end = scored[0], scored[1]
         out = (loss, lp.detach(), row_end)
         if coeff != 0.0:
@@ -1426,7 +1362,7 @@ def _grpo_objective_from_logits(logits, input_ids, K, ref_per_token_logps, advan
             out = (loss - coeff * h_mean, lp.detach(), row_end, h_mean.detach(), loss.detach())
         if return_entropy:
             out += (ent.detach(),)
-        return out + (scored[2],) if return_cf else out
+        return out + (scored[2],) if return_clip_fraction else out
     B, seq, _ = logits.shape
     if not 0 < K < seq:
         raise ValueError('logits_to_keep must lie in (0, L)')
@@ -1442,15 +1378,15 @@ def _grpo_objective_from_logits(logits, input_ids, K, ref_per_token_logps, advan
     adv = advantages.detach().float().contiguous().view(-1)
     if adv.numel() != B:
         raise ValueError('one advantage per sequence expected')
-    old = _old_log_probs(old, (B, K), lp_dtype)
+    old = _old_log_probs(old_per_token_logps, (B, K), lp_dtype)
     tok = _contiguous_last(tokens.to(torch.int64))
     ent = torch.zeros((B, K), dtype=torch.float32, device=logits.device) if return_entropy or coeff != 0.0 else None
-    cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_cf else None
+    cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
     out = _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code, ent, coeff,
-                             obj.args(), old, cf)
+                             obj, old, cf)
     if return_entropy:
         out += (ent,)
-    return out + (cf,) if return_cf else out
+    return out + (cf,) if return_clip_fraction else out
 
 
 # ---- reward-model pairwise loss -----------------------------------------------------------------------
@@ -2142,12 +2078,13 @@ class GrpoObjective(ActorObjective):
         return super().args(self.clip_range_ratio if clip_range_ratio is None else clip_range_ratio)
 
 
-def _objective(objective: ActorObjective | None) -> ActorObjective | None:
-    """None for the reference's objective (today's launches), else the objective."""
+def _objective(objective: ActorObjective | None, cls: type = ActorObjective) -> ActorObjective | None:
+    """None for the reference's objective (None, or every field at its default: today's launches), else the objective,
+    which must be a `cls`."""
     if objective is None:
         return None
-    if not isinstance(objective, ActorObjective):
-        raise TypeError(f'objective must be an ops.ActorObjective, got {type(objective).__name__}')
+    if not isinstance(objective, cls):
+        raise TypeError(f'objective must be an ops.{cls.__name__}, got {type(objective).__name__}')
     return None if objective.is_default else objective
 
 
@@ -2213,6 +2150,30 @@ class _PpoLossFn(torch.autograd.Function):
         return (grad.float() * g_loss.float()).to(grad.dtype), None, None, None, None, None, None, None, None
 
 
+def _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, grad, obj, coeff, ent):
+    """K1f over the actor's scored rows, writing lp and the gradient tile `grad`.  obj: ActorObjective.args(...) for
+    the objective entry point (aa_logprob_actor_fused_obj), None for the reference's objective -- with an entropy
+    bonus (`ent`, the fp32 entropy out) the entropy-gradient entry point, otherwise the plain one."""
+    dev = logits.device
+    # 48 bytes per tile row (the row records); the entropy-gradient and objective forms add 4 per segment (the rows'
+    # g_H coefficients)
+    extra = (plan.n_seg + 1) // 2 if obj is not None or ent is not None else 0
+    scratch = torch.empty(plan.n_tile_rows * 6 + extra, dtype=torch.int64, device=dev)
+    p = plan.ptrs()
+    lib = L.lib()
+    head = (logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), ids.data_ptr(),
+            plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp.dtype), None,
+            None, old.data_ptr(), old.stride(0), aux.data_ptr(), aux.stride(0), L.dtype_code(aux.dtype),
+            mask.data_ptr(), mask.stride(0), lp.size(1))
+    tail = (mode_code, grad.data_ptr(), logits.size(-1), scratch.data_ptr(), _device_scratch(dev)['status'].data_ptr())
+    if obj is not None:
+        L.check(lib.aa_logprob_actor_fused_obj(*head, *obj, *tail, coeff, L.ptr(ent), L.stream_ptr(dev)))
+    elif ent is not None:
+        L.check(lib.aa_logprob_actor_fused_entropy(*head, float(clip), *tail, coeff, ent.data_ptr(), L.stream_ptr(dev)))
+    else:
+        L.check(lib.aa_logprob_actor_fused(*head, float(clip), *tail, L.stream_ptr(dev)))
+
+
 class _TailActorLossFn(torch.autograd.Function):
     """The actor half of the multimodal rl_step as ONE autograd node (trainers/text_image_to_text/ppo.py:298-316).
 
@@ -2237,80 +2198,27 @@ class _TailActorLossFn(torch.autograd.Function):
                 clip_frac=None):
         out_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         dev = logits.device
+        coeff = float(entropy_coeff)
+        obj = objective.args(clip) if objective is not None else None
         lp = torch.zeros(plan.out_shape, dtype=out_dtype, device=dev)
         ctx.fused = bool(single_pass and plan.n_tile_rows > 0 and plan.n_seg > 0 and plan.n_tile_rows % plan.n_seg == 0
                          and len(plan.out_shape) == 2)
-        if objective is not None or clip_frac is not None:
-            return _TailActorLossFn._forward_objective(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, lp,
-                                                       float(entropy_coeff), objective, clip_frac)
-        if entropy_coeff != 0.0:
-            return _TailActorLossFn._forward_bonus(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, lp,
-                                                   float(entropy_coeff))
-        ctx.bonus = False
-        if ctx.fused:
-            grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
-            scratch = torch.empty(plan.n_tile_rows * 6, dtype=torch.int64, device=dev)  # 48 bytes per tile row
-            p = plan.ptrs()
-            L.check(L.lib().aa_logprob_actor_fused(
-                logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), ids.data_ptr(),
-                plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp.dtype),
-                None, None, old.data_ptr(), old.stride(0), aux.data_ptr(), aux.stride(0), L.dtype_code(aux.dtype),
-                mask.data_ptr(), mask.stride(0), lp.size(1), float(clip), mode_code, grad.data_ptr(), logits.size(-1),
-                scratch.data_ptr(), _device_scratch(dev)['status'].data_ptr(), L.stream_ptr(dev)))
-            loss, cast, _, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True)
-            ctx.save_for_backward(grad)
-        else:
-            stats = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=dev)
-            _launch_fwd(logits, ids, plan, lp, stats[0], stats[1])
-            loss, cast, grad, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True)
-            ctx.save_for_backward(logits, ids, stats, grad)
-            ctx.plan, ctx.mode_code = plan, mode_code
-        ctx.mark_non_differentiable(lp, loss)
-        return cast, lp, loss
-
-    @staticmethod
-    def _forward_objective(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, lp, coeff, objective, clip_frac):
-        """The node under an ActorObjective (None: the reference's objective, reached with clip_frac only)."""
-        dev = logits.device
-        obj = objective.args(clip) if objective is not None else None
-        tm = objective is not None and objective.token_mean
         ctx.bonus = coeff != 0.0
         ent = torch.zeros(plan.out_shape, dtype=torch.float32, device=dev) if ctx.bonus else None
-        if ctx.fused and obj is None:  # today's K1f launch (plain or entropy-bonus form)
+        if ctx.fused:
             grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
-            scratch = torch.empty(plan.n_tile_rows * 6 + (plan.n_seg + 1) // 2, dtype=torch.int64, device=dev)
-            p = plan.ptrs()
-            args = (logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), ids.data_ptr(),
-                    plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp.dtype),
-                    None, None, old.data_ptr(), old.stride(0), aux.data_ptr(), aux.stride(0), L.dtype_code(aux.dtype),
-                    mask.data_ptr(), mask.stride(0), lp.size(1), float(clip), mode_code, grad.data_ptr(),
-                    logits.size(-1), scratch.data_ptr(), _device_scratch(dev)['status'].data_ptr())
-            if ctx.bonus:
-                L.check(L.lib().aa_logprob_actor_fused_entropy(*args, coeff, ent.data_ptr(), L.stream_ptr(dev)))
-            else:
-                L.check(L.lib().aa_logprob_actor_fused(*args, L.stream_ptr(dev)))
-            ctx.save_for_backward(grad)
-        elif ctx.fused:
-            grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
-            # 48 bytes per tile row (the row records) + 4 per segment (the rows' g_H coefficients)
-            scratch = torch.empty(plan.n_tile_rows * 6 + (plan.n_seg + 1) // 2, dtype=torch.int64, device=dev)
-            p = plan.ptrs()
-            L.check(L.lib().aa_logprob_actor_fused_obj(
-                logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), ids.data_ptr(),
-                plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp.dtype),
-                None, None, old.data_ptr(), old.stride(0), aux.data_ptr(), aux.stride(0), L.dtype_code(aux.dtype),
-                mask.data_ptr(), mask.stride(0), lp.size(1), obj[0], obj[1], obj[2], obj[3], mode_code, grad.data_ptr(),
-                logits.size(-1), scratch.data_ptr(), _device_scratch(dev)['status'].data_ptr(), coeff, L.ptr(ent),
-                L.stream_ptr(dev)))
+            _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, grad, obj, coeff, ent)
             ctx.save_for_backward(grad)
         else:
             stats = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=dev)
             _launch_fwd(logits, ids, plan, lp, stats[0], stats[1], entropy=ent)
         loss, cast, grad_lp, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True, obj=obj, clip_frac=clip_frac)
+        tm = objective is not None and objective.token_mean
         if not ctx.fused:
             if ctx.bonus:
-                # d (-coeff * mean(H)) / d H on masked-in tokens (0 elsewhere, as K1f forms it): the masked mean's
-                # coefficient, or -coeff / (masked-in tokens of the micro-batch) under token-mean
+                # d (-coeff * mean(H)) / d H on masked-in tokens (0, not 0 * -inf, elsewhere: K1f forms g_H for
+                # masked-in tokens only): the masked mean's coefficient as _MaskedMeanFn's backward forms it, or
+                # -coeff / (masked-in tokens of the micro-batch) under token-mean
                 den = mask.sum().float() if tm else mask.size(0) * mask.sum(dim=-1, keepdim=True).float()
                 g_h = torch.where(mask, -coeff / den, 0.0)
                 ctx.save_for_backward(logits, ids, stats, grad_lp, ent, g_h)
@@ -2321,38 +2229,6 @@ class _TailActorLossFn(torch.autograd.Function):
             ctx.mark_non_differentiable(lp, loss)
             return cast, lp, loss
         h_mean = token_mean(ent, mask) if tm else masked_mean(ent, mask)
-        reg = loss[0] - coeff * h_mean
-        ctx.mark_non_differentiable(lp, loss, h_mean)
-        return reg, lp, loss, h_mean
-
-    @staticmethod
-    def _forward_bonus(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, lp, coeff):
-        dev = logits.device
-        ctx.bonus = True
-        ent = torch.zeros(plan.out_shape, dtype=torch.float32, device=dev)
-        if ctx.fused:
-            grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
-            # 48 bytes per tile row (the row records) + 4 per segment (the rows' g_H coefficients)
-            scratch = torch.empty(plan.n_tile_rows * 6 + (plan.n_seg + 1) // 2, dtype=torch.int64, device=dev)
-            p = plan.ptrs()
-            L.check(L.lib().aa_logprob_actor_fused_entropy(
-                logits.data_ptr(), L.dtype_code(logits.dtype), logits.stride(-2), logits.size(-1), ids.data_ptr(),
-                plan.n_seg, p[0], p[1], p[2], p[3], p[4], plan.n_tile_rows, lp.data_ptr(), L.dtype_code(lp.dtype),
-                None, None, old.data_ptr(), old.stride(0), aux.data_ptr(), aux.stride(0), L.dtype_code(aux.dtype),
-                mask.data_ptr(), mask.stride(0), lp.size(1), float(clip), mode_code, grad.data_ptr(), logits.size(-1),
-                scratch.data_ptr(), _device_scratch(dev)['status'].data_ptr(), coeff, ent.data_ptr(), L.stream_ptr(dev)))
-            loss, _, _, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True)
-            ctx.save_for_backward(grad)
-        else:
-            stats = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=dev)
-            _launch_fwd(logits, ids, plan, lp, stats[0], stats[1], entropy=ent)
-            loss, _, grad_lp, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True)
-            # d (-coeff * masked_mean(H, mask)) / d H, as _MaskedMeanFn's backward forms it
-            # (0, not 0 * -inf, for a sample without masked-in tokens: K1f forms g_H for masked-in tokens only)
-            g_h = torch.where(mask, -coeff / (mask.size(0) * mask.sum(dim=-1, keepdim=True).float()), 0.0)
-            ctx.save_for_backward(logits, ids, stats, grad_lp, ent, g_h)
-            ctx.plan, ctx.mode_code = plan, mode_code
-        h_mean = masked_mean(ent, mask)
         reg = loss[0] - coeff * h_mean
         ctx.mark_non_differentiable(lp, loss, h_mean)
         return reg, lp, loss, h_mean
@@ -2408,17 +2284,22 @@ class _TailCriticLossFn(torch.autograd.Function):
         return out.view(ctx.shape), None, None, None, None, None, None, None
 
 
+def _k5_operands(old, aux, mask, dtype):
+    """K5's detached operands beside the differentiated input: old in that input's dtype `dtype`, aux (advantages or
+    returns) in a dtype the kernel reads, mask as bool; each contiguous along the last dimension."""
+    old = _contiguous_last(old.detach().to(dtype))
+    aux = _contiguous_last(aux.detach())
+    if aux.dtype not in (torch.float32, torch.bfloat16, torch.float16):
+        aux = aux.float()
+    return old, aux, _contiguous_last(mask.to(torch.bool))
+
+
 def _loss_inputs(x, old, aux, mask):
     L.require_cuda(x, old, aux, mask)
     if not (x.shape == old.shape == aux.shape == mask.shape) or x.dim() != 2:
         raise ValueError('loss inputs must all be (B, W)')
     x = _contiguous_last(x)
-    old = _contiguous_last(old.detach().to(x.dtype))
-    aux = _contiguous_last(aux.detach())
-    if aux.dtype not in (torch.float32, torch.bfloat16, torch.float16):
-        aux = aux.float()
-    mask = _contiguous_last(mask.to(torch.bool))
-    return x, old, aux, mask
+    return (x, *_k5_operands(old, aux, mask, x.dtype))
 
 
 def actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio: float, mode: str | None = None,
@@ -2429,9 +2310,6 @@ def actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio: flo
     objective = _objective(objective)
     x, old, aux, m = _loss_inputs(log_probs, old_log_probs, advantages, mask)
     obj = objective.args(clip_range_ratio) if objective is not None else None
-    if obj is None and not return_clip_fraction:
-        loss, _, _ = _PpoLossFn.apply(x, old, aux, m, clip_range_ratio, _mode_code(mode, x.dtype), True)
-        return loss
     cf = torch.zeros(2, dtype=torch.float32, device=x.device) if return_clip_fraction else None
     loss, _, _ = _PpoLossFn.apply(x, old, aux, m, clip_range_ratio, _mode_code(mode, x.dtype), True, obj, cf)
     return (loss, cf) if return_clip_fraction else loss
@@ -2464,25 +2342,16 @@ def tail_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, lens, old_log
         raise ValueError('old_log_probs, advantages and mask must all be (B, W), W = the bound of the response lengths')
     logits, ids = _contiguous_last(logits), input_ids.contiguous()
     mode_code = _mode_code(mode, logits.dtype)
-    lp_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
-    old = _contiguous_last(old_log_probs.detach().to(lp_dtype))
-    aux = _contiguous_last(advantages.detach())
-    if aux.dtype not in (torch.float32, torch.bfloat16, torch.float16):
-        aux = aux.float()
-    m = _contiguous_last(mask.to(torch.bool))
+    old, aux, m = _k5_operands(old_log_probs, advantages, mask,
+                               logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32)
     plan = device_tail_plan(lens, K, logits.stride(0), logits.stride(1), ids.stride(0), ids.size(1), 0, -1, lens.bound)
     single_pass = _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad)
-    if objective is not None or return_clip_fraction:
-        if objective is not None:
-            objective.args(clip_range_ratio)  # a bad clip range fails here, before any launch
-        cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
-        out = _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass,
-                                     float(entropy_coeff), objective, cf)
-        return (*out, cf) if return_clip_fraction else out
-    if entropy_coeff != 0.0:
-        return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass,
-                                      float(entropy_coeff))
-    return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass)
+    if objective is not None:
+        objective.args(clip_range_ratio)  # a bad clip range fails here, before the node launches anything
+    cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
+    out = _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass,
+                                 float(entropy_coeff), objective, cf)
+    return (*out, cf) if return_clip_fraction else out
 
 
 @functools.lru_cache(maxsize=64)
@@ -2520,56 +2389,35 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
         raise ValueError('old_log_probs, advantages and mask must all be (B, L - 1 - start)')
     if objective is not None:
         objective.args(clip_range_ratio)  # a bad clip range fails here, before any launch
-    extended = objective is not None or return_clip_fraction
-    if not _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad) and extended:
-        # the composed ops below with the objective: K5 takes it, K1 / K1b are unchanged
-        kw = dict(mode=mode, objective=objective, return_clip_fraction=return_clip_fraction)
-        cf = ()
+    if not _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad):
+        # short rows, fp16, no gradient: the composed ops (K1 over the response rows -> K5, which takes the objective;
+        # backward K1b)
+        rows, labels = logits[:, start:-1], input_ids[:, start + 1:]
         if entropy_coeff != 0.0:
-            lp, ent = gather_log_probabilities_with_entropy(logits[:, start:-1], input_ids[:, start + 1:], mode=mode,
-                                                            entropy_grad=True)
-            loss = actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, **kw)
-            if return_clip_fraction:
-                loss, cf = loss[0], (loss[1],)
-            m = mask.to(torch.bool)
-            h_mean = token_mean(ent, m) if objective is not None and objective.token_mean else masked_mean(ent, m)
-            return (loss - float(entropy_coeff) * h_mean, lp.detach(), loss, h_mean.detach(), *cf)
-        lp = gather_log_probabilities(logits[:, start:-1], input_ids[:, start + 1:], mode=mode)
-        loss = actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, **kw)
+            lp, ent = gather_log_probabilities_with_entropy(rows, labels, mode=mode, entropy_grad=True)
+        else:
+            lp = gather_log_probabilities(rows, labels, mode=mode)
+        loss = actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, mode=mode, objective=objective,
+                          return_clip_fraction=return_clip_fraction)
+        cf = ()
         if return_clip_fraction:
             loss, cf = loss[0], (loss[1],)
-        return (loss, lp.detach(), loss, *cf)
-    if not _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad):
-        # short rows, fp16, no gradient: the composed ops (K1 over the response rows -> K5; backward K1b)
-        if entropy_coeff != 0.0:
-            lp, ent = gather_log_probabilities_with_entropy(logits[:, start:-1], input_ids[:, start + 1:], mode=mode,
-                                                            entropy_grad=True)
-            loss = actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, mode=mode)
-            h_mean = masked_mean(ent, mask)
-            return loss - float(entropy_coeff) * h_mean, lp.detach(), loss, h_mean.detach()
-        lp = gather_log_probabilities(logits[:, start:-1], input_ids[:, start + 1:], mode=mode)
-        loss = actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, mode=mode)
-        return loss, lp.detach(), loss
+        if entropy_coeff == 0.0:
+            return (loss, lp.detach(), loss, *cf)
+        m = mask.to(torch.bool)
+        h_mean = token_mean(ent, m) if objective is not None and objective.token_mean else masked_mean(ent, m)
+        return (loss - float(entropy_coeff) * h_mean, lp.detach(), loss, h_mean.detach(), *cf)
     logits, ids = _contiguous_last(logits), input_ids.contiguous()
     if B > 1 and (logits.stride(0) != Lq * logits.stride(1)):
         logits = logits.contiguous()  # the gradient tile is shaped after the logits: rows must be uniformly strided
     mode_code = _mode_code(mode, logits.dtype)
-    lp_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
-    old = _contiguous_last(old_log_probs.detach().to(lp_dtype))
-    aux = _contiguous_last(advantages.detach())
-    if aux.dtype not in (torch.float32, torch.bfloat16, torch.float16):
-        aux = aux.float()
-    m = _contiguous_last(mask.to(torch.bool))
+    old, aux, m = _k5_operands(old_log_probs, advantages, mask,
+                               logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32)
     plan = _dense_actor_plan(B, Lq, start, logits.stride(0), logits.stride(1), ids.stride(0), str(logits.device))
-    if extended:
-        cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
-        out = _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, True,
-                                     float(entropy_coeff), objective, cf)
-        return (*out, cf) if return_clip_fraction else out
-    if entropy_coeff != 0.0:
-        return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, True,
-                                      float(entropy_coeff))
-    return _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, True)
+    cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
+    out = _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, True,
+                                 float(entropy_coeff), objective, cf)
+    return (*out, cf) if return_clip_fraction else out
 
 
 def tail_critic_loss(scores: torch.Tensor, lens, old_values, returns, mask, clip_range_value: float,
@@ -2584,11 +2432,7 @@ def tail_critic_loss(scores: torch.Tensor, lens, old_values, returns, mask, clip
     if lens.bound > scores.size(1) - 1:
         raise ValueError('the scores tensor is too short for the response lengths')
     x = scores if scores.dtype in (torch.float32, torch.bfloat16, torch.float16) else scores.float()
-    old = _contiguous_last(old_values.detach().to(x.dtype))
-    aux = _contiguous_last(returns.detach())
-    if aux.dtype not in (torch.float32, torch.bfloat16, torch.float16):
-        aux = aux.float()
-    m = _contiguous_last(mask.to(torch.bool))
+    old, aux, m = _k5_operands(old_values, returns, mask, x.dtype)
     return _TailCriticLossFn.apply(x, lens.dev, lens.bound, old, aux, m, clip_range_value, _mode_code(mode, x.dtype))
 
 
