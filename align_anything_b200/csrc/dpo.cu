@@ -83,6 +83,15 @@ struct DpoParams {
   const int32_t *status;  // optional: device status word, copied into stats[7] (MAX lane of the step's all-reduce)
 };
 
+// K2 with the objective options (DESIGN section 4.5).  A type of its own, so that the reference loss's
+// instantiation keeps its parameter block, and its code, as they were.
+struct DpoObjParams : DpoParams {
+  int loss_type;          // AA_DPO_*
+  float eps;              // label_smoothing
+  float alpha;            // rpo_alpha: 0 = no NLL term
+  const int32_t *counts;  // optional: scored rows per sample (R_i - 1), [2 * n_pairs]
+};
+
 template <int THREADS>
 __device__ __forceinline__ float row_sum(const void *base, int dt, int64_t off, int width, float *scratch) {
   float acc = 0.f;
@@ -101,8 +110,182 @@ __device__ __forceinline__ float dlog_sigmoid(float z) {
   return (neg ? 1.f : 0.f) - (neg ? 1.f : -1.f) * (e / (1.f + e));
 }
 
+// ---- K2 objective options (DESIGN section 4.5) ----------------------------------------------
+// Each loss restates tests/dpo_objective_port.py op for op: FAITHFUL rounds (rd) wherever the port's eager op on a
+// 0-dim tensor of the log-prob dtype rounds, and every product is __fmul_rn so that no rounding point is contracted
+// away.  The forward keeps two floats per pair (s0, s1) from which the last block, once it knows 1 / n_kept, runs the
+// port's autograd chain.  a = pc - rc, b = pr - rr (IPO: each sum divided by its row count first).
+struct DpoPairFwd {
+  float loss, s0, s1;
+};
+
+__device__ __forceinline__ float sigmoid_f(float z) { return 1.f / (1.f + expf(-z)); }
+
+__device__ __forceinline__ DpoPairFwd dpo_obj_forward(int type, float a, float b, float beta, float eps, int rd) {
+  const float c = static_cast<float>(0.5 / static_cast<double>(beta));  // 1 / (2 beta)
+  DpoPairFwd f{0.f, 0.f, 0.f};
+  switch (type) {
+    case AA_DPO_SIGMOID:
+    case AA_DPO_ROBUST: {
+      const float z = round_to(__fmul_rn(beta, round_to(a - b, rd)), rd);
+      const float t1 = round_to(log_sigmoid(z), rd);
+      f.loss = -t1;
+      if (eps != 0.f) {
+        const float m1 = round_to(__fmul_rn(-t1, 1.f - eps), rd);
+        const float m2 = round_to(__fmul_rn(round_to(log_sigmoid(-z), rd), eps), rd);
+        f.loss = type == AA_DPO_SIGMOID ? round_to(m1 - m2, rd)
+                                        : round_to(__fmul_rn(round_to(m1 + m2, rd), 1.f / (1.f - 2.f * eps)), rd);
+      }
+      f.s0 = z;
+      break;
+    }
+    case AA_DPO_HINGE: {
+      const float u = round_to(1.f - round_to(__fmul_rn(beta, round_to(a - b, rd)), rd), rd);
+      f.loss = (u > 0.f || u != u) ? u : 0.f;
+      f.s0 = f.loss;
+      break;
+    }
+    case AA_DPO_IPO: {
+      const float d = round_to(round_to(a - b, rd) - c, rd);
+      f.loss = round_to(__fmul_rn(d, d), rd);
+      f.s0 = d;
+      break;
+    }
+    case AA_DPO_SPPO_HARD: {
+      const float d1 = round_to(a - c, rd), d2 = round_to(b + c, rd);
+      f.loss = round_to(round_to(__fmul_rn(d1, d1), rd) + round_to(__fmul_rn(d2, d2), rd), rd);
+      f.s0 = d1;
+      f.s1 = d2;
+      break;
+    }
+    case AA_DPO_NCA_PAIR: {
+      const float za = round_to(__fmul_rn(beta, a), rd), zb = round_to(__fmul_rn(beta, b), rd);
+      const float t1 = round_to(log_sigmoid(za), rd), t2 = round_to(log_sigmoid(-za), rd);
+      const float t3 = round_to(log_sigmoid(-zb), rd);
+      f.loss = round_to(round_to(-t1 - __fmul_rn(0.5f, t2), rd) - __fmul_rn(0.5f, t3), rd);
+      f.s0 = za;
+      f.s1 = zb;
+      break;
+    }
+    case AA_DPO_APO_ZERO: {
+      const float sa = round_to(sigmoid_f(round_to(__fmul_rn(beta, a), rd)), rd);
+      const float sb = round_to(sigmoid_f(round_to(__fmul_rn(beta, b), rd)), rd);
+      f.loss = round_to(round_to(1.f - sa, rd) + sb, rd);
+      f.s0 = sa;
+      f.s1 = sb;
+      break;
+    }
+    default: {  // AA_DPO_APO_DOWN
+      const float sa = round_to(sigmoid_f(round_to(__fmul_rn(beta, a), rd)), rd);
+      const float sh = round_to(sigmoid_f(round_to(__fmul_rn(beta, round_to(a - b, rd)), rd)), rd);
+      f.loss = round_to(sa + round_to(1.f - sh, rd), rd);
+      f.s0 = sa;
+      f.s1 = sh;
+      break;
+    }
+  }
+  return f;
+}
+
+// sigmoid_backward(g, s) = g * (1 - s) * s, evaluated by ATen CUDA in the tensor's dtype: a rounding after each op
+__device__ __forceinline__ float dsigmoid(float g, float s, int rd) {
+  return round_to(__fmul_rn(round_to(__fmul_rn(g, round_to(1.f - s, rd)), rd), s), rd);
+}
+
+// d (gl * loss) / d (chosen sum, rejected sum) from the forward's (s0, s1); gl = d mean / d loss_i.  inv_nc / inv_nr:
+// 1 / row count (IPO only).
+__device__ __forceinline__ float2 dpo_obj_backward(int type, float gl, float s0, float s1, float beta, float eps,
+                                                   float inv_nc, float inv_nr, int rd) {
+  switch (type) {
+    case AA_DPO_SIGMOID:
+    case AA_DPO_ROBUST: {
+      float gz;
+      if (eps == 0.f) {
+        gz = round_to(__fmul_rn(-gl, dlog_sigmoid(s0)), rd);
+      } else {
+        const float g0 = type == AA_DPO_ROBUST ? round_to(__fmul_rn(gl, 1.f / (1.f - 2.f * eps)), rd) : gl;
+        const float dt1 = -round_to(__fmul_rn(g0, 1.f - eps), rd);
+        const float dt2 = round_to(__fmul_rn(type == AA_DPO_ROBUST ? g0 : -g0, eps), rd);
+        gz = round_to(round_to(__fmul_rn(dt1, dlog_sigmoid(s0)), rd) - round_to(__fmul_rn(dt2, dlog_sigmoid(-s0)), rd),
+                      rd);
+      }
+      const float gh = round_to(__fmul_rn(gz, beta), rd);
+      return make_float2(gh, -gh);
+    }
+    case AA_DPO_HINGE: {  // ReluBackward: no gradient where the result is <= 0
+      const float gh = round_to(__fmul_rn(s0 > 0.f || s0 != s0 ? -gl : 0.f, beta), rd);
+      return make_float2(gh, -gh);
+    }
+    case AA_DPO_IPO: {
+      const float gd = round_to(__fmul_rn(gl, 2.f * s0), rd);
+      return make_float2(round_to(__fmul_rn(gd, inv_nc), rd), round_to(__fmul_rn(-gd, inv_nr), rd));
+    }
+    case AA_DPO_SPPO_HARD:
+      return make_float2(round_to(__fmul_rn(gl, 2.f * s0), rd), round_to(__fmul_rn(gl, 2.f * s1), rd));
+    case AA_DPO_NCA_PAIR: {
+      const float hg = __fmul_rn(-gl, 0.5f);
+      const float gza = round_to(round_to(__fmul_rn(-gl, dlog_sigmoid(s0)), rd) -
+                                     round_to(__fmul_rn(hg, dlog_sigmoid(-s0)), rd), rd);
+      const float gzb = -round_to(__fmul_rn(hg, dlog_sigmoid(-s1)), rd);
+      return make_float2(round_to(__fmul_rn(gza, beta), rd), round_to(__fmul_rn(gzb, beta), rd));
+    }
+    case AA_DPO_APO_ZERO:
+      return make_float2(round_to(__fmul_rn(dsigmoid(-gl, s0, rd), beta), rd),
+                         round_to(__fmul_rn(dsigmoid(gl, s1, rd), beta), rd));
+    default: {  // AA_DPO_APO_DOWN
+      const float gh = round_to(__fmul_rn(dsigmoid(-gl, s1, rd), beta), rd);
+      const float ga = round_to(__fmul_rn(dsigmoid(gl, s0, rd), beta), rd);
+      return make_float2(round_to(ga + gh, rd), -gh);
+    }
+  }
+}
+
+// The last block of the objective variant, after the metric means: the RPO NLL term (alpha > 0), then the seeds.
+// per_pair[3] holds each pair's chosen sum and grad_seg the forward's (s0, s1) until they are replaced here.
 template <int THREADS>
-__global__ void __launch_bounds__(THREADS) dpo_loss_kernel(const DpoParams p) {
+__device__ __forceinline__ void dpo_obj_finish(const DpoObjParams &p, float sum_loss_over_n, float inv_n, float *scratch) {
+  const int B = p.n_pairs, rd = p.round_dt, tid = threadIdx.x;
+  volatile float *v_g = p.per_pair + 3 * B, *v_seg = p.grad_seg;
+  const volatile float *v_valid = p.per_pair + 4 * B;
+  float g_nll = 0.f;
+  if (p.alpha > 0.f) {  // NLL = -(sum of the kept chosen sums) / (their scored rows): the token mean, as in RPO
+    float s_pc = 0.f, s_cnt = 0.f;
+    for (int k = tid; k < B; k += THREADS) {
+      if (v_valid[k] != 0.f) {
+        s_pc += v_g[k];
+        s_cnt += static_cast<float>(p.counts[k]);
+      }
+    }
+    s_pc = block_sum<THREADS>(s_pc, scratch);
+    s_cnt = block_sum<THREADS>(s_cnt, scratch);
+    const float inv_cnt = 1.f / s_cnt;  // x / int: x * (1 / n)
+    const float nll = -round_to(__fmul_rn(round_to(s_pc, rd), inv_cnt), rd);
+    g_nll = round_to(__fmul_rn(-round_to(p.alpha, rd), inv_cnt), rd);  // Add -> Mul(alpha) -> Neg -> Div -> Sum
+    if (tid == 0) {
+      p.stats[0] = round_to(round_to(sum_loss_over_n, rd) + round_to(__fmul_rn(nll, p.alpha), rd), rd);
+      p.stats[8] = nll;
+    }
+  }
+  const float gl = round_to(inv_n, rd);  // MeanBackward
+  for (int k = tid; k < B; k += THREADS) {
+    float gc = 0.f, gr = -0.f;  // a skipped pair: the seeds aa_dpo_loss writes (+0, -0)
+    if (v_valid[k] != 0.f) {
+      const bool ipo = p.loss_type == AA_DPO_IPO;
+      const float2 g = dpo_obj_backward(p.loss_type, gl, v_seg[k], v_seg[B + k], p.beta, p.eps,
+                                        ipo ? 1.f / static_cast<float>(p.counts[k]) : 0.f,
+                                        ipo ? 1.f / static_cast<float>(p.counts[B + k]) : 0.f, rd);
+      gc = p.alpha > 0.f ? round_to(g.x + g_nll, rd) : g.x;
+      gr = g.y;
+    }
+    v_g[k] = gc;
+    v_seg[k] = gc;
+    v_seg[B + k] = gr;
+  }
+}
+
+template <int THREADS, class Params>
+__global__ void __launch_bounds__(THREADS) dpo_loss_kernel(const Params p) {
+  constexpr bool OBJ = std::is_same<Params, DpoObjParams>::value;
   __shared__ float scratch[33];
   __shared__ int same_flag;
   const int i = blockIdx.x, tid = threadIdx.x;
@@ -113,8 +296,11 @@ __global__ void __launch_bounds__(THREADS) dpo_loss_kernel(const DpoParams p) {
 
   const float pc = round_to(row_sum<THREADS>(p.policy_lp, p.lp_dtype, int64_t(i) * p.row_stride, p.width, scratch), rd);
   const float pr = round_to(row_sum<THREADS>(p.policy_lp, p.lp_dtype, int64_t(B + i) * p.row_stride, p.width, scratch), rd);
-  const float rc = round_to(row_sum<THREADS>(p.ref_lp, p.lp_dtype, int64_t(i) * p.row_stride, p.width, scratch), rd);
-  const float rr = round_to(row_sum<THREADS>(p.ref_lp, p.lp_dtype, int64_t(B + i) * p.row_stride, p.width, scratch), rd);
+  float rc = 0.f, rr = 0.f;  // reference-free (OBJ with ref_lp == NULL): the reference sums are 0
+  if (!OBJ || p.ref_lp) {
+    rc = round_to(row_sum<THREADS>(p.ref_lp, p.lp_dtype, int64_t(i) * p.row_stride, p.width, scratch), rd);
+    rr = round_to(row_sum<THREADS>(p.ref_lp, p.lp_dtype, int64_t(B + i) * p.row_stride, p.width, scratch), rd);
+  }
 
   bool valid = true;
   if (p.ids) {  // text_audio_to_text/dpo.py:138: skip when chosen ids == rejected ids
@@ -132,11 +318,27 @@ __global__ void __launch_bounds__(THREADS) dpo_loss_kernel(const DpoParams p) {
   if (tid == 0) {
     const float ratio_c = round_to(pc - rc, rd);
     const float ratio_r = round_to(pr - rr, rd);
-    const float z = round_to(p.beta * round_to(ratio_c - ratio_r, rd), rd);
-    loss_i[i] = -round_to(log_sigmoid(z), rd);
-    better_i[i] = round_to(p.beta * ratio_c, rd);
-    worse_i[i] = round_to(p.beta * ratio_r, rd);
-    g_i[i] = z;  // converted to the gradient coefficient by the last block
+    if constexpr (OBJ) {
+      float a = ratio_c, b = ratio_r;
+      if (p.loss_type == AA_DPO_IPO) {  // the four sums divided by their row counts first (x / int: x * (1 / n))
+        const float inv_c = 1.f / static_cast<float>(p.counts[i]), inv_r = 1.f / static_cast<float>(p.counts[B + i]);
+        a = round_to(round_to(__fmul_rn(pc, inv_c), rd) - round_to(__fmul_rn(rc, inv_c), rd), rd);
+        b = round_to(round_to(__fmul_rn(pr, inv_r), rd) - round_to(__fmul_rn(rr, inv_r), rd), rd);
+      }
+      const DpoPairFwd f = dpo_obj_forward(p.loss_type, a, b, p.beta, p.eps, rd);
+      loss_i[i] = f.loss;
+      better_i[i] = round_to(p.beta * ratio_c, rd);  // the metrics keep the summed ratios for every loss type
+      worse_i[i] = round_to(p.beta * ratio_r, rd);
+      g_i[i] = pc;  // the chosen sum, for the NLL term; the last block overwrites it with the chosen seed
+      p.grad_seg[i] = f.s0;  // the backward's operands, until the last block turns them into the seeds
+      p.grad_seg[B + i] = f.s1;
+    } else {
+      const float z = round_to(p.beta * round_to(ratio_c - ratio_r, rd), rd);
+      loss_i[i] = -round_to(log_sigmoid(z), rd);
+      better_i[i] = round_to(p.beta * ratio_c, rd);
+      worse_i[i] = round_to(p.beta * ratio_r, rd);
+      g_i[i] = z;  // converted to the gradient coefficient by the last block
+    }
     valid_i[i] = valid ? 1.f : 0.f;
   }
 
@@ -177,6 +379,10 @@ __global__ void __launch_bounds__(THREADS) dpo_loss_kernel(const DpoParams p) {
     p.stats[6] = n;
     // the sticky status word rides in the free lane: the trainers read it with the metrics (no extra sync) and raise
     p.stats[7] = p.status ? static_cast<float>(*reinterpret_cast<const volatile int32_t *>(p.status)) : 0.f;
+  }
+  if constexpr (OBJ) {
+    dpo_obj_finish<THREADS>(p, s_loss * inv_n, inv_n, scratch);
+    return;
   }
   if (p.coll.world > 1 && p.stats_global) {
     // the packed-metric all-reduce of train_step (trainers/text_to_text/dpo.py:222-227), done by this very
@@ -456,6 +662,37 @@ extern "C" int aa_dpo_loss(const void *policy_lp, const void *ref_lp, int lp_dty
     p.coll = CollParams{reinterpret_cast<float *const *>(coll->peer_bufs), coll->rank, coll->world, coll->epoch,
                         coll->max_lanes};
   }
-  dpo_loss_kernel<128><<<n_pairs, 128, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  dpo_loss_kernel<128, DpoParams><<<n_pairs, 128, 0, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("aa_dpo_loss");
+}
+
+extern "C" int aa_dpo_loss_obj(const void *policy_lp, const void *ref_lp, int lp_dtype, int32_t n_pairs,
+                               int32_t width, int64_t lp_row_stride, float scale_coeff, int mode, int loss_type,
+                               float label_smoothing, float rpo_alpha, const int32_t *counts,
+                               const int64_t *input_ids, int32_t L, int64_t ids_row_stride, float *per_pair,
+                               float *grad_seg, float *stats, uint32_t *counter, const int32_t *status,
+                               void *stream) {
+  AA_REQUIRE(n_pairs > 0 && width >= 0, AA_ERR_ARG, "aa_dpo_loss_obj: bad sizes");
+  AA_REQUIRE(policy_lp && per_pair && grad_seg && stats && counter, AA_ERR_ARG, "aa_dpo_loss_obj: null pointer");
+  AA_REQUIRE(lp_dtype == AA_BF16 || lp_dtype == AA_F16 || lp_dtype == AA_F32, AA_ERR_DTYPE,
+             "aa_dpo_loss_obj: bad dtype %d", lp_dtype);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_dpo_loss_obj: bad mode %d", mode);
+  AA_REQUIRE(loss_type >= AA_DPO_SIGMOID && loss_type <= AA_DPO_APO_DOWN, AA_ERR_ARG,
+             "aa_dpo_loss_obj: bad objective: loss_type %d", loss_type);
+  const bool smoothable = loss_type == AA_DPO_SIGMOID || loss_type == AA_DPO_ROBUST;
+  AA_REQUIRE(label_smoothing >= 0.f && label_smoothing < 0.5f && (smoothable || label_smoothing == 0.f), AA_ERR_ARG,
+             "aa_dpo_loss_obj: bad objective: label_smoothing %g with loss_type %d", label_smoothing, loss_type);
+  AA_REQUIRE(rpo_alpha >= 0.f && isfinite(rpo_alpha), AA_ERR_ARG, "aa_dpo_loss_obj: bad objective: rpo_alpha %g",
+             rpo_alpha);
+  AA_REQUIRE((loss_type != AA_DPO_IPO && loss_type != AA_DPO_SPPO_HARD) || (scale_coeff > 0.f && isfinite(scale_coeff)),
+             AA_ERR_ARG, "aa_dpo_loss_obj: bad objective: loss_type %d needs scale_coeff > 0, got %g", loss_type,
+             scale_coeff);
+  AA_REQUIRE(counts || (loss_type != AA_DPO_IPO && rpo_alpha == 0.f), AA_ERR_ARG,
+             "aa_dpo_loss_obj: loss_type %d with rpo_alpha %g needs the row counts", loss_type, rpo_alpha);
+  DpoObjParams p{{policy_lp, ref_lp, lp_dtype, n_pairs, width, lp_row_stride, scale_coeff,
+                  mode == AA_MODE_FAITHFUL ? lp_dtype : AA_F32, input_ids, L, ids_row_stride, per_pair, grad_seg,
+                  stats, counter, nullptr, CollParams{nullptr, 0, 1, 0u, 0u}, status},
+                 loss_type, label_smoothing, rpo_alpha, counts};
+  dpo_loss_kernel<128, DpoObjParams><<<n_pairs, 128, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("aa_dpo_loss_obj");
 }

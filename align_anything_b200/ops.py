@@ -26,7 +26,7 @@ __all__ = [
     'move_padding_left', 'count_nonpad', 'strip_pad_tail', 'ppo_pack_metrics', 'check_status', 'raise_for_status', 'status_lane', 'causal_lm_loss', 'rm_pair_loss', 'cost_pair_loss','group_advantages', 'grpo_loss', 'tail_token_log_probs', 'pair_slices', 'slice_sums', 'tail_rows', 'linear_token_log_probs',
     'sequence_log_probs_from_hidden', 'fused_linear_token_log_probs', 'tail_log_probs_from_hidden', 'dense_log_probs_from_hidden', 'tail_actor_loss', 'tail_critic_loss', 'lm_head_weight',
     'causal_lm_loss_from_hidden', 'causal_lm_valid_rows', 'gather_log_probabilities_with_entropy',
-    'response_tail_log_probs_pair_with_entropy', 'ActorObjective', 'token_mean',
+    'response_tail_log_probs_pair_with_entropy', 'ActorObjective', 'token_mean', 'DpoObjective',
 ]
 
 # Path knobs: plain module attributes, read at call time and never from the environment.  Every path is chosen from the
@@ -923,26 +923,105 @@ def sequence_log_probs(logits: torch.Tensor, input_ids: torch.Tensor, response_l
     return _LogProbFn.apply(logits, labels, plan, _mode_code(mode, logits.dtype))
 
 
-def _dpo_launch(policy_lp, ref_lp, scale_coeff, mode_code, input_ids, want_grad_seg, coll=None):
+DPO_LOSS_TYPES = {'sigmoid': 0, 'robust': 1, 'hinge': 2, 'ipo': 3, 'sppo_hard': 4, 'nca_pair': 5, 'apo_zero': 6,
+                  'apo_down': 7}  # include/aa_b200.h AA_DPO_*
+
+
+@dataclasses.dataclass(frozen=True)
+class DpoObjective:
+    """The DPO objective options of TRL's DPOConfig (the reference's loss, trainers/text_to_text/dpo.py:166-203, when
+    every field is at its default).  With a = pc - rc and b = pr - rr the policy-minus-reference log-prob sums of the
+    chosen and rejected rows, h = a - b, z = beta * h and eps = label_smoothing, the per-pair loss is
+
+        sigmoid    -(1 - eps) logsigmoid(z) - eps logsigmoid(-z)            (eps > 0: conservative DPO)
+        robust     (-(1 - eps) logsigmoid(z) + eps logsigmoid(-z)) / (1 - 2 eps)
+        hinge      relu(1 - z)
+        ipo        (h - 1 / (2 beta))^2, each of pc, pr, rc, rr divided by its row's scored-token count first
+        sppo_hard  (a - 1 / (2 beta))^2 + (b + 1 / (2 beta))^2
+        nca_pair   -logsigmoid(beta a) - logsigmoid(-beta a) / 2 - logsigmoid(-beta b) / 2
+        apo_zero   (1 - sigmoid(beta a)) + sigmoid(beta b)
+        apo_down   sigmoid(beta a) + (1 - sigmoid(beta h))
+
+    The loss is the mean over the kept pairs; rpo_alpha > 0 adds rpo_alpha * NLL, NLL = -sum(pc) / sum(R_c - 1) over
+    the kept pairs' chosen rows (RPO), reported as train/nll_loss.  reference_free: rc = rr = 0 and no reference model
+    runs.  The metrics keep the reference's definitions for every loss type.  Checked here, before anything runs."""
+
+    loss_type: str = 'sigmoid'
+    label_smoothing: float = 0.0
+    rpo_alpha: float = 0.0
+    reference_free: bool = False
+
+    def __post_init__(self):
+        if self.loss_type not in DPO_LOSS_TYPES:
+            raise ValueError(f'loss_type must be one of {sorted(DPO_LOSS_TYPES)}, got {self.loss_type!r}')
+        eps, alpha = float(self.label_smoothing), float(self.rpo_alpha)
+        if not 0.0 <= eps < 0.5:
+            raise ValueError(f'label_smoothing must lie in [0, 0.5), got {self.label_smoothing!r}')
+        if eps > 0.0 and self.loss_type not in ('sigmoid', 'robust'):
+            raise ValueError(f"label_smoothing applies to loss_type 'sigmoid' and 'robust' only, not {self.loss_type!r}")
+        if not (alpha >= 0.0 and math.isfinite(alpha)):
+            raise ValueError(f'rpo_alpha must be a finite value >= 0, got {self.rpo_alpha!r}')
+        if not isinstance(self.reference_free, bool):
+            raise ValueError(f'reference_free must be a bool, got {self.reference_free!r}')
+
+    @property
+    def is_default(self) -> bool:
+        """The reference's objective: K2 runs today's launch."""
+        return (self.loss_type == 'sigmoid' and float(self.label_smoothing) == 0.0 and float(self.rpo_alpha) == 0.0
+                and not self.reference_free)
+
+    @property
+    def needs_counts(self) -> bool:
+        return self.loss_type == 'ipo' or float(self.rpo_alpha) > 0.0
+
+
+def _dpo_counts(obj: DpoObjective | None, response_lens, device):
+    """int32 [2B] scored rows per sample (R_i - 1) when the objective divides by them, else None; a count it would
+    divide by that is 0 raises here."""
+    if obj is None or not obj.needs_counts:
+        return None
+    if response_lens is None:
+        raise ValueError(f'loss_type={obj.loss_type!r} with rpo_alpha={obj.rpo_alpha} needs response_lens')
+    counts = tuple(int(r) - 1 for r in response_lens)
+    B = len(counts) // 2
+    if obj.loss_type == 'ipo' and min(counts) < 1:
+        raise ValueError(f'ipo divides each log-prob sum by its row count R_i - 1: a response of length 1 has none '
+                         f'(response_lens {tuple(response_lens)})')
+    if float(obj.rpo_alpha) > 0.0 and sum(counts[:B]) < 1:
+        raise ValueError('rpo_alpha > 0 takes the token mean of the chosen responses: they score no token')
+    return _lens_tensor(counts, str(device))
+
+
+def _dpo_launch(policy_lp, ref_lp, scale_coeff, mode_code, input_ids, want_grad_seg, coll=None, obj=None, counts=None):
     """coll: an `_lib.AaColl` descriptor (utils.multi_process.FusedPackedAllReduce.next()) -> K2's last block
-    also all-reduces the stats over NVLink; the reduced vector comes back as a 4th result."""
+    also all-reduces the stats over NVLink; the reduced vector comes back as a 4th result.  obj: a non-default
+    DpoObjective -> aa_dpo_loss_obj (ref_lp None when reference-free; stats gets a 9th lane, the NLL, with rpo_alpha)."""
     import ctypes
 
     dev = policy_lp.device
     n2, W = policy_lp.shape
     B = n2 // 2
     per_pair = torch.empty((5, B), dtype=torch.float32, device=dev)
-    stats = torch.empty(8, dtype=torch.float32, device=dev)
-    grad_seg = torch.empty(n2, dtype=torch.float32, device=dev) if want_grad_seg else None
+    stats = torch.empty(9 if obj is not None and float(obj.rpo_alpha) > 0.0 else 8, dtype=torch.float32, device=dev)
+    grad_seg = torch.empty(n2, dtype=torch.float32, device=dev) if want_grad_seg or obj is not None else None
     sc = _device_scratch(dev)
     ids = None
     if input_ids is not None:
         ids = _contiguous_last(input_ids)
+    ids_args = (L.ptr(ids), ids.size(1) if ids is not None else 0, ids.stride(0) if ids is not None else 0)
+    if obj is not None:
+        if coll is not None:
+            raise ValueError('the DPO objective options have no in-kernel collective: all-reduce the stats instead')
+        L.check(L.lib().aa_dpo_loss_obj(
+            policy_lp.data_ptr(), L.ptr(ref_lp), L.dtype_code(policy_lp.dtype), B, W, policy_lp.stride(0),
+            float(scale_coeff), mode_code, DPO_LOSS_TYPES[obj.loss_type], float(obj.label_smoothing),
+            float(obj.rpo_alpha), L.ptr(counts), *ids_args, per_pair.data_ptr(), grad_seg.data_ptr(), stats.data_ptr(),
+            sc['counter'][0:1].data_ptr(), sc['status'].data_ptr(), L.stream_ptr(dev)))
+        return per_pair, stats, grad_seg
     stats_global = torch.empty(8, dtype=torch.float32, device=dev) if coll is not None else None
     L.check(L.lib().aa_dpo_loss(
         policy_lp.data_ptr(), ref_lp.data_ptr(), L.dtype_code(policy_lp.dtype), B, W, policy_lp.stride(0),
-        float(scale_coeff), mode_code, L.ptr(ids), ids.size(1) if ids is not None else 0,
-        ids.stride(0) if ids is not None else 0, per_pair.data_ptr(), L.ptr(grad_seg), stats.data_ptr(),
+        float(scale_coeff), mode_code, *ids_args, per_pair.data_ptr(), L.ptr(grad_seg), stats.data_ptr(),
         sc['counter'][0:1].data_ptr(), ctypes.byref(coll) if coll is not None else None, L.ptr(stats_global),
         sc['status'].data_ptr(), L.stream_ptr(dev)))
     if coll is not None:
@@ -968,8 +1047,9 @@ def _dpo_dict(per_pair, stats, out_dtype, skip_identical):
 
 class _DpoFromLpFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, policy_lp, ref_lp, scale_coeff, mode_code, input_ids):
-        per_pair, stats, grad_seg = _dpo_launch(policy_lp, ref_lp, scale_coeff, mode_code, input_ids, True)
+    def forward(ctx, policy_lp, ref_lp, scale_coeff, mode_code, input_ids, obj=None, counts=None):
+        per_pair, stats, grad_seg = _dpo_launch(policy_lp, ref_lp, scale_coeff, mode_code, input_ids, True, obj=obj,
+                                                counts=counts)
         ctx.save_for_backward(grad_seg)
         ctx.lp_shape, ctx.lp_dtype = policy_lp.shape, policy_lp.dtype
         ctx.mark_non_differentiable(per_pair, stats)
@@ -980,40 +1060,61 @@ class _DpoFromLpFn(torch.autograd.Function):
     def backward(ctx, g_loss, _g1, _g2):
         (grad_seg,) = ctx.saved_tensors
         g = (grad_seg * g_loss.float()).to(ctx.lp_dtype)
-        return g.unsqueeze(1).expand(ctx.lp_shape), None, None, None, None
+        return g.unsqueeze(1).expand(ctx.lp_shape), None, None, None, None, None, None
 
 
-def dpo_loss_from_log_probs(policy_lp: torch.Tensor, ref_lp: torch.Tensor, scale_coeff: float,
+def _dpo_outputs(loss, per_pair, stats, out_dtype, skip_identical_pairs, obj):
+    out = {'loss': loss}
+    out.update(_dpo_dict(per_pair, stats, out_dtype, skip_identical_pairs))
+    if obj is not None and float(obj.rpo_alpha) > 0.0:
+        out['nll_loss'] = stats[8]
+    out['_stats'] = stats
+    return out
+
+
+def dpo_loss_from_log_probs(policy_lp: torch.Tensor, ref_lp: torch.Tensor | None, scale_coeff: float,
                             input_ids: torch.Tensor | None = None, skip_identical_pairs: bool = False,
-                            mode: str | None = None) -> dict[str, torch.Tensor]:
+                            mode: str | None = None, objective: DpoObjective | None = None,
+                            response_lens: Sequence[int] | None = None) -> dict[str, torch.Tensor]:
     """trainers/text_to_text/dpo.py:150-203 given the two (2B, W) log-prob tensors: ONE launch for
     the 4 sums per pair, the log-sigmoid loss and the five metrics (K2).  `skip_identical_pairs`:
     text_audio_to_text/dpo.py:134-139.  Extra key '_stats' = packed fp32[8] local means for
-    the all-reduce (utils.multi_process.all_reduce_packed)."""
+    the all-reduce (utils.multi_process.all_reduce_packed).  objective: a DpoObjective (ref_lp may be None when it is
+    reference-free); response_lens (R_i per row) give the row counts that ipo and rpo_alpha divide by.  With rpo_alpha
+    the dict also has 'nll_loss' and '_stats' a 9th lane."""
+    obj = _objective(objective, DpoObjective)
+    if obj is not None and obj.reference_free:
+        ref_lp = None
+    elif ref_lp is None:
+        raise ValueError('ref_lp is None: only a reference_free objective runs without the reference log-probs')
     L.require_cuda(policy_lp, ref_lp)
-    if policy_lp.shape != ref_lp.shape or policy_lp.dim() != 2 or policy_lp.size(0) % 2:
+    if policy_lp.dim() != 2 or policy_lp.size(0) % 2 or (ref_lp is not None and policy_lp.shape != ref_lp.shape):
         raise ValueError('policy / reference log-probs must both be (2B, W)')
+    if response_lens is not None and len(response_lens) != policy_lp.size(0):
+        raise ValueError('need one response_len per row of the log-probs')
     policy_lp = policy_lp if policy_lp.stride(1) == 1 or policy_lp.size(1) <= 1 else policy_lp.contiguous()
-    ref_lp = ref_lp.to(policy_lp.dtype).contiguous()
-    if policy_lp.stride(0) != ref_lp.stride(0):
-        policy_lp = policy_lp.contiguous()
+    if ref_lp is not None:
+        ref_lp = ref_lp.to(policy_lp.dtype).contiguous()
+        if policy_lp.stride(0) != ref_lp.stride(0):
+            policy_lp = policy_lp.contiguous()
+        ref_lp = ref_lp.detach()
     mode_code = _mode_code(mode, policy_lp.dtype)
     ids = input_ids if skip_identical_pairs else None
-    loss, per_pair, stats = _DpoFromLpFn.apply(policy_lp, ref_lp.detach(), scale_coeff, mode_code, ids)
+    counts = _dpo_counts(obj, response_lens, policy_lp.device)
+    loss, per_pair, stats = _DpoFromLpFn.apply(policy_lp, ref_lp, scale_coeff, mode_code, ids, obj, counts)
     out_dtype = policy_lp.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
-    out = {'loss': loss}
-    out.update(_dpo_dict(per_pair, stats, out_dtype, skip_identical_pairs))
-    out['_stats'] = stats
+    out = _dpo_outputs(loss, per_pair, stats, out_dtype, skip_identical_pairs, obj)
     out['_per_pair'] = per_pair
     return out
 
 
 class _DpoFusedFn(torch.autograd.Function):
-    """policy logits (grad) + reference logits (no grad) -> DPO loss.  Forward: K1 x2, K2.  Backward:
-    ONE K1b launch taking the per-sample coefficient straight from K2 (no per-row gradient tensor)."""
+    """policy logits (grad) + reference logits (no grad) -> DPO loss.  Forward: K1 x2 (x1 reference-free), K2.
+    Backward: ONE K1b launch taking the per-sample coefficient straight from K2 (no per-row gradient tensor)."""
 
     @staticmethod
-    def forward(ctx, policy_logits, ref_logits, labels, plan, scale_coeff, mode_code, ids, coll=None):
+    def forward(ctx, policy_logits, ref_logits, labels, plan, scale_coeff, mode_code, ids, coll=None, obj=None,
+                counts=None):
         dev = policy_logits.device
         out_dtype = policy_logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         lp = torch.zeros((2,) + plan.out_shape, dtype=out_dtype, device=dev)
@@ -1021,8 +1122,10 @@ class _DpoFusedFn(torch.autograd.Function):
         stats_rows = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=dev) if need_grad else None
         _launch_fwd(policy_logits, labels, plan, lp[0], stats_rows[0] if need_grad else None,
                     stats_rows[1] if need_grad else None)
-        _launch_fwd(ref_logits, labels, plan, lp[1], None, None)
-        res = _dpo_launch(lp[0], lp[1], scale_coeff, mode_code, ids, True, coll)
+        if ref_logits is not None:
+            _launch_fwd(ref_logits, labels, plan, lp[1], None, None)
+        res = _dpo_launch(lp[0], lp[1] if ref_logits is not None else None, scale_coeff, mode_code, ids, True, coll,
+                          obj, counts)
         per_pair, stats, grad_seg = res[0], res[1], res[2]
         stats_global = res[3] if coll is not None else stats
         if need_grad:
@@ -1038,36 +1141,43 @@ class _DpoFusedFn(torch.autograd.Function):
         scale = g_loss.detach().to(torch.float32).reshape(1).contiguous()
         _launch_bwd(logits, labels, ctx.plan, stats_rows[0], stats_rows[1], None, grad_seg, scale, grad,
                     ctx.mode_code)
-        return grad, None, None, None, None, None, None, None
+        return grad, None, None, None, None, None, None, None, None, None
 
 
-def dpo_fused_loss(policy_logits: torch.Tensor, ref_logits: torch.Tensor, input_ids: torch.Tensor,
+def dpo_fused_loss(policy_logits: torch.Tensor, ref_logits: torch.Tensor | None, input_ids: torch.Tensor,
                    response_lens: Sequence[int], pad_id: int, scale_coeff: float, strip: bool = True,
-                   skip_identical_pairs: bool = False, mode: str | None = None, coll=None) -> dict[str, torch.Tensor]:
+                   skip_identical_pairs: bool = False, mode: str | None = None, coll=None,
+                   objective: DpoObjective | None = None) -> dict[str, torch.Tensor]:
     """The whole of DPOTrainer.loss after the two model forwards (trainers/text_to_text/dpo.py:144-203):
-    5 launches forward (label extraction, K1 policy, K1 reference, K2), 1 launch backward (K1b)."""
+    5 launches forward (label extraction, K1 policy, K1 reference, K2), 1 launch backward (K1b).  objective: a
+    DpoObjective; reference-free, ref_logits may be None and is not read (no reference K1)."""
+    obj = _objective(objective, DpoObjective)
+    if obj is not None and obj.reference_free:
+        ref_logits = None
+    elif ref_logits is None:
+        raise ValueError('ref_logits is None: only a reference_free objective runs without the reference model')
     L.require_cuda(policy_logits, ref_logits, input_ids)
-    if policy_logits.shape != ref_logits.shape or policy_logits.dim() != 3:
+    if policy_logits.dim() != 3 or (ref_logits is not None and policy_logits.shape != ref_logits.shape):
         raise ValueError('policy / reference logits must both be (2B, L, V)')
     if policy_logits.size(0) % 2 or policy_logits.size(0) != len(response_lens):
         raise ValueError('need 2B rows (chosen first, rejected second) and one response_len per row')
     lens = tuple(int(r) for r in response_lens)
     labels = strip_pad_tail(input_ids, lens, pad_id, strip)
     policy_logits = _contiguous_last(policy_logits)
-    ref_logits = ref_logits.detach()
-    if ref_logits.stride() != policy_logits.stride() or ref_logits.dtype != policy_logits.dtype:
-        ref_logits = ref_logits.to(policy_logits.dtype).contiguous()
-        if ref_logits.stride() != policy_logits.stride():
-            policy_logits = policy_logits.contiguous()
+    if ref_logits is not None:
+        ref_logits = ref_logits.detach()
+        if ref_logits.stride() != policy_logits.stride() or ref_logits.dtype != policy_logits.dtype:
+            ref_logits = ref_logits.to(policy_logits.dtype).contiguous()
+            if ref_logits.stride() != policy_logits.stride():
+                policy_logits = policy_logits.contiguous()
     plan = _dpo_plan(policy_logits, lens, labels.stride(0))
     mode_code = _mode_code(mode, policy_logits.dtype)
     ids = input_ids if skip_identical_pairs else None
+    counts = _dpo_counts(obj, lens, policy_logits.device)
     loss, per_pair, stats, lp, stats_global = _DpoFusedFn.apply(policy_logits, ref_logits, labels, plan, scale_coeff,
-                                                               mode_code, ids, coll)
+                                                               mode_code, ids, coll, obj, counts)
     out_dtype = policy_logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
-    out = {'loss': loss}
-    out.update(_dpo_dict(per_pair, stats, out_dtype, skip_identical_pairs))
-    out['_stats'] = stats
+    out = _dpo_outputs(loss, per_pair, stats, out_dtype, skip_identical_pairs, obj)
     if coll is not None:
         out['_stats_global'] = stats_global  # already averaged over the ranks by K2 itself (NVLink peer memory)
     out['_per_pair'] = per_pair

@@ -5,7 +5,9 @@
 swaps, without touching any reference file,
   * align_anything.utils.tools.{gather_log_probabilities, masked_mean, move_padding_left}
     (and the names re-imported by the trainer modules),
-  * DPOTrainer.{compute_log_probs, loss, train_step} of the text / image / audio / video trainers,
+  * DPOTrainer.{compute_log_probs, loss, train_step} of the text / image / audio / video trainers (the classes also
+    get the objective switches `loss_type`, `label_smoothing`, `rpo_alpha` and `reference_free`, unset: the
+    reference's loss),
   * PPOTrainer.{rollout, actor_loss_fn, critic_loss_fn, add_kl_divergence_regularization,
     get_advantages_and_returns, rl_step, ptx_step} of the text / image / audio / video trainers, and the
     multimodal trainers' actor_step (its post-generate bookkeeping); `reward_model_step` and the text trainer's
@@ -172,7 +174,8 @@ def install(trainers: bool = True, models: bool = True) -> dict[str, list[str]]:
                     setattr(cls, m, fn)
                     done.setdefault(modname, []).append(f'{cls.__name__}.{m}')
             if modname in _DPO_TARGETS:  # class attributes the grafted methods read
-                for attr in ('strip_pad_tokens', 'skip_identical_pairs', 'mode', 'fused_lm_head', 'lm_head_chunk_rows'):
+                for attr in ('strip_pad_tokens', 'skip_identical_pairs', 'mode', 'fused_lm_head', 'lm_head_chunk_rows',
+                             'loss_type', 'label_smoothing', 'rpo_alpha', 'reference_free'):
                     _saved.append((cls, attr, cls.__dict__.get(attr, None)))
                     setattr(cls, attr, getattr(src, attr))
             elif modname in _PPO_TARGETS or modname in _GRPO_TARGETS:

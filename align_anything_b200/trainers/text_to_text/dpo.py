@@ -15,11 +15,21 @@ import torch
 
 from ... import ops
 from ...utils.multi_process import all_reduce_packed, fused_allreduce
+from .ppo import switch_of
 
 __all__ = ['DPOTrainer', 'strip_pad']
 
 METRIC_KEYS = ('train/loss', 'train/reward', 'train/better_sample_reward', 'train/worse_sample_reward',
                'train/reward_accuracy', 'train/reward_margin')
+DPO_OBJECTIVE_KEYS = ('loss_type', 'label_smoothing', 'rpo_alpha', 'reference_free')
+
+
+def dpo_objective_of(tr) -> ops.DpoObjective | None:
+    """The DPO objective in effect (switch_of each of DPO_OBJECTIVE_KEYS), or None when every key is unset: the
+    reference's loss and today's launches.  A bad value raises ValueError here, before anything runs."""
+    fields = {k: switch_of(tr, k) for k in DPO_OBJECTIVE_KEYS}
+    fields = {k: v for k, v in fields.items() if v is not None}
+    return ops.DpoObjective(**fields) if fields else None
 
 
 def strip_pad(seq: torch.Tensor, pad_token_id: int):
@@ -39,6 +49,14 @@ class DPOTrainer:
     # the scored rows go through ops.sequence_log_probs_from_hidden (chunked lm_head GEMM + K1 / K1b).
     fused_lm_head = False
     lm_head_chunk_rows = None
+    # The objective (ops.DpoObjective, TRL's DPOConfig names): loss_type ('sigmoid', 'robust', 'hinge', 'ipo',
+    # 'sppo_hard', 'nca_pair', 'apo_zero', 'apo_down'), label_smoothing (cDPO / robust), rpo_alpha (RPO's NLL term on
+    # the chosen responses, logged as train/nll_loss) and reference_free (no reference model forward).  None: the
+    # reference's loss; `cfgs.train_cfgs.<name>` overrides each when set.
+    loss_type = None
+    label_smoothing = None
+    rpo_alpha = None
+    reference_free = None
 
     def __init__(self, cfgs, model, reference_model, tokenizer, infer_batch=None) -> None:
         self.cfgs = cfgs
@@ -68,19 +86,27 @@ class DPOTrainer:
 
     # -- trainers/text_to_text/dpo.py:144-203 --------------------------------------------------
     def loss(self, batch) -> dict[str, torch.Tensor]:
+        obj = dpo_objective_of(self)
+        ref_free = obj is not None and obj.reference_free
+        lens = batch['meta_info']['response_lens']
         if self.fused_lm_head:
             policy_lp = self.compute_log_probs(self.model.module, batch)
-            with torch.no_grad():
-                ref_lp = self.compute_log_probs(self.reference_model.module, batch)
+            ref_lp = None
+            if not ref_free:
+                with torch.no_grad():
+                    ref_lp = self.compute_log_probs(self.reference_model.module, batch)
             return ops.dpo_loss_from_log_probs(policy_lp, ref_lp, float(self.cfgs.train_cfgs.scale_coeff), batch['input_ids'],
-                                               skip_identical_pairs=self.skip_identical_pairs, mode=self.mode)
+                                               skip_identical_pairs=self.skip_identical_pairs, mode=self.mode,
+                                               objective=obj, response_lens=lens)
         policy_logits = self.model.module(**self.infer_batch(batch)).logits
-        with torch.no_grad():
-            ref_logits = self.reference_model.module(**self.infer_batch(batch)).logits
+        ref_logits = None
+        if not ref_free:
+            with torch.no_grad():
+                ref_logits = self.reference_model.module(**self.infer_batch(batch)).logits
         out = ops.dpo_fused_loss(
-            policy_logits, ref_logits, batch['input_ids'], batch['meta_info']['response_lens'],
+            policy_logits, ref_logits, batch['input_ids'], lens,
             self.tokenizer.pad_token_id, float(self.cfgs.train_cfgs.scale_coeff),
-            strip=self.strip_pad_tokens, skip_identical_pairs=self.skip_identical_pairs, mode=self.mode)
+            strip=self.strip_pad_tokens, skip_identical_pairs=self.skip_identical_pairs, mode=self.mode, objective=obj)
         # inside train_step on several GPUs the packed metrics are all-reduced over NVLink peer memory by a one-warp
         # kernel on a side stream, launched HERE so that its wait for the slowest rank overlaps the backward (K1b);
         # every rank runs the same number of steps; a bare loss() call never enters a collective
@@ -108,5 +134,7 @@ class DPOTrainer:
         # at those points, we raise here -- same exception class, no extra sync, every rank together
         ops.raise_for_status(values[7], stats.device)
         out = dict(zip(METRIC_KEYS, values[:6]))
+        if len(values) > 8:  # rpo_alpha > 0: the NLL term's lane
+            out['train/nll_loss'] = values[8]
         out['train/lr'] = self.model.optimizer.param_groups[0]['lr']
         return out

@@ -8,7 +8,7 @@
  * function(s) whose arithmetic it replaces (file:line relative to the reference's
  * align_anything/ directory); the Python mirror in align_anything_b200/ keeps the
  * reference's names and signatures and calls these through ctypes (INTEGRATION.md).
- * 54 entry points, ABI version 3.
+ * 55 entry points, ABI version 3.
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
@@ -229,6 +229,45 @@ int aa_dpo_loss(const void *policy_lp, const void *ref_lp, int lp_dtype, int32_t
                 const int64_t *input_ids, int32_t L, int64_t ids_row_stride,
                 float *per_pair, float *grad_seg, float *stats, uint32_t *counter,
                 const aa_coll *coll, float *stats_global, const int32_t *status, void *stream);
+
+/* ---------------------------------------------------------------------------------------
+ * K2 with the objective options of TRL's DPOConfig (DESIGN.md section 4.5): loss_type, label_smoothing
+ * (cDPO / robust DPO), rpo_alpha (RPO's NLL term) and reference-free DPO.  With a = pc - rc, b = pr - rr (the
+ * policy / reference log-prob sums of the chosen / rejected rows), h = a - b, z = scale_coeff * h:
+ *   AA_DPO_SIGMOID    -(1-e) logsig(z) - e logsig(-z)            (e = label_smoothing; e = 0: aa_dpo_loss's loss)
+ *   AA_DPO_ROBUST     (-(1-e) logsig(z) + e logsig(-z)) / (1 - 2e)
+ *   AA_DPO_HINGE      relu(1 - z)
+ *   AA_DPO_IPO        (h - 1/(2 beta))^2, each of the four sums divided by its row's counts[] entry first
+ *   AA_DPO_SPPO_HARD  (a - 1/(2 beta))^2 + (b + 1/(2 beta))^2
+ *   AA_DPO_NCA_PAIR   -logsig(beta a) - logsig(-beta a) / 2 - logsig(-beta b) / 2
+ *   AA_DPO_APO_ZERO   (1 - sigmoid(beta a)) + sigmoid(beta b)
+ *   AA_DPO_APO_DOWN   sigmoid(beta a) + (1 - sigmoid(beta h))
+ * loss = mean over kept pairs; rpo_alpha > 0 adds rpo_alpha * NLL, NLL = -sum(pc) / sum(counts of those chosen rows)
+ * over the kept pairs, and stats has a 9th lane = NLL.  ref_lp == NULL: reference-free (rc = rr = 0, nothing read).
+ *   counts   : int32 [2*n_pairs] scored rows per sample (R_i - 1); needed by AA_DPO_IPO and rpo_alpha > 0.
+ *   per_pair : as aa_dpo_loss, g_i = d loss / d chosen sum_i.
+ *   grad_seg : required, fp32 [2*n_pairs] = (d loss / d chosen sum ..., d loss / d rejected sum ...) for
+ *              aa_logprob_bwd; the rejected seeds are no longer -g_i.
+ *   stats    : fp32 [8] as aa_dpo_loss (stats[0] = the loss with the NLL term), [9] when rpo_alpha > 0.
+ * Metrics keep aa_dpo_loss's definitions (from the summed ratios) for every loss type.  No collective: the caller
+ * all-reduces stats.  label_smoothing must lie in [0, 0.5) and be 0 unless the type is SIGMOID or ROBUST;
+ * rpo_alpha >= 0; IPO and SPPO_HARD need scale_coeff > 0.
+ * ------------------------------------------------------------------------------------- */
+enum {
+  AA_DPO_SIGMOID = 0,
+  AA_DPO_ROBUST = 1,
+  AA_DPO_HINGE = 2,
+  AA_DPO_IPO = 3,
+  AA_DPO_SPPO_HARD = 4,
+  AA_DPO_NCA_PAIR = 5,
+  AA_DPO_APO_ZERO = 6,
+  AA_DPO_APO_DOWN = 7
+};
+int aa_dpo_loss_obj(const void *policy_lp, const void *ref_lp, int lp_dtype, int32_t n_pairs, int32_t width,
+                    int64_t lp_row_stride, float scale_coeff, int mode, int loss_type, float label_smoothing,
+                    float rpo_alpha, const int32_t *counts, const int64_t *input_ids, int32_t L,
+                    int64_t ids_row_stride, float *per_pair, float *grad_seg, float *stats, uint32_t *counter,
+                    const int32_t *status, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * Pair bookkeeping and slice sums of SimPO / ORPO / KTO (SURVEY.md 8f row 2).
