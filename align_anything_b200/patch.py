@@ -173,42 +173,19 @@ def install(trainers: bool = True, models: bool = True) -> dict[str, list[str]]:
                     _saved.append((cls, m, cls.__dict__.get(m, None)))
                     setattr(cls, m, fn)
                     done.setdefault(modname, []).append(f'{cls.__name__}.{m}')
-            if modname in _DPO_TARGETS:  # class attributes the grafted methods read
-                for attr in ('strip_pad_tokens', 'skip_identical_pairs', 'mode', 'fused_lm_head', 'lm_head_chunk_rows',
-                             'loss_type', 'label_smoothing', 'rpo_alpha', 'reference_free'):
-                    _saved.append((cls, attr, cls.__dict__.get(attr, None)))
-                    setattr(cls, attr, getattr(src, attr))
-            elif modname in _PPO_TARGETS or modname in _GRPO_TARGETS:
-                _saved.append((cls, 'mode', cls.__dict__.get('mode', None)))
-                setattr(cls, 'mode', None)
-                if modname in _PPO_TARGETS:  # helpers the grafted rl_step calls + the H100-side entry points
-                    helpers = ('_actor_logits', '_tail_log_probs', 'score_rollout', 'postprocess_generation')
-                    if src not in (_TextPPO, _MultiPPO):  # multimodal: the post-generate bookkeeping of actor_step is ours too
-                        helpers += ('actor_step',)
-                    for m in helpers:
-                        fn = next((b.__dict__[m] for b in src.__mro__ if m in b.__dict__), None)
-                        if fn is not None:
-                            _saved.append((cls, m, cls.__dict__.get(m, None)))
-                            setattr(cls, m, fn)
-                            done.setdefault(modname, []).append(f'{cls.__name__}.{m}')
-                    for attr in ('tail_logits', 'fused_lm_head', 'lm_head_chunk_rows', 'micro_batched_rollout', 'log_entropy',
-                                 'entropy_coeff', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio',
-                                 'loss_agg_mode', 'log_clip_fraction'):
-                        if hasattr(src, attr):
-                            _saved.append((cls, attr, cls.__dict__.get(attr, None)))
-                            setattr(cls, attr, getattr(src, attr))
-                else:  # the switches the grafted step_from_rollout / _get_per_token_logps read
-                    for attr in ('fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'num_iterations',
-                                 'clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio',
-                                 'loss_agg_mode', 'scale_rewards', 'log_clip_fraction'):
-                        _saved.append((cls, attr, cls.__dict__.get(attr, None)))
-                        setattr(cls, attr, getattr(src, attr))
-            elif modname in _SFT_TARGETS:
-                _saved.append((cls, 'ignore_index', cls.__dict__.get('ignore_index', None)))
-                setattr(cls, 'ignore_index', -100)
-                for attr in ('fused_lm_head', 'lm_head_chunk_rows'):  # the switch the grafted loss reads
-                    _saved.append((cls, attr, cls.__dict__.get(attr, None)))
-                    setattr(cls, attr, getattr(src, attr))
+            if modname in _PPO_TARGETS:  # helpers the grafted rl_step calls + the H100-side entry points
+                helpers = ('_actor_logits', '_tail_log_probs', 'score_rollout', 'postprocess_generation')
+                if src not in (_TextPPO, _MultiPPO):  # multimodal: the post-generate bookkeeping of actor_step is ours too
+                    helpers += ('actor_step',)
+                for m in helpers:
+                    fn = next((b.__dict__[m] for b in src.__mro__ if m in b.__dict__), None)
+                    if fn is not None:
+                        _saved.append((cls, m, cls.__dict__.get(m, None)))
+                        setattr(cls, m, fn)
+                        done.setdefault(modname, []).append(f'{cls.__name__}.{m}')
+            for attr in src.SWITCHES:  # the class attributes the grafted methods read
+                _saved.append((cls, attr, cls.__dict__.get(attr, None)))
+                setattr(cls, attr, getattr(src, attr))
         for modname, (clsname, src) in _SLICED_TARGETS.items():
             mod = _try_import(modname)
             cls = getattr(mod, clsname, None) if mod is not None else None

@@ -14,10 +14,8 @@ from typing import Any
 import torch
 
 from ... import ops
-from ...utils.multi_process import all_reduce_packed, fused_allreduce
-from ..text_to_text.ppo import (METRIC_KEYS, clip_metrics, entropy_coeff_of, objective_kwargs, with_bonus_lane,
-                                with_clip_lanes, with_entropy_lane)
 from ..text_to_text.ppo import PPOTrainer as _TextPPOTrainer
+from ..text_to_text.ppo import actor_loss_node, ppo_metrics
 
 __all__ = ['PPOTrainer', 'move_padding_left']
 
@@ -47,6 +45,7 @@ class PPOTrainer(_TextPPOTrainer):
     # text+image / text+video: the whole prompt batch is generated and scored at once (:206-269); the audio trainer
     # loops over micro-batches of per_device_train_batch_size (text_audio_to_text/ppo.py:217-277)
     micro_batched_rollout = False
+    SWITCHES = _TextPPOTrainer.SWITCHES + ('tail_logits', 'micro_batched_rollout')
 
     def _tail_log_probs(self, model, batch, lens, input_ids, return_entropy=False, entropy_grad=False, **kw):
         """(B, W) log-probs of the response tails, right-padded with 0 (W = lens.bound); return_entropy (fused_lm_head
@@ -159,37 +158,9 @@ class PPOTrainer(_TextPPOTrainer):
             self.clip_range_score, self.gamma, self.gae_lambda, mode=self.mode)
 
         # actor: K1 over the response tails + K5 as ONE autograd node; its backward is K1b alone (:296-316)
-        batch = self.infer_batch(inference_batch)
-        coeff = entropy_coeff_of(self)  # entropy bonus over the response tails (the actor loss's rows and mask)
-        kw = objective_kwargs(self)  # the actor objective switches (empty: the reference's objective)
-        entropy_mean = clip_frac = None
-        if self.fused_lm_head:
-            # with a bonus K6's entropy variant; K6b adds the entropy's gradient in its epilogue
-            log_probs = self._tail_log_probs(self.actor_model, batch, lens, input_ids, return_entropy=coeff != 0.0,
-                                             entropy_grad=coeff != 0.0, use_cache=False)
-            if coeff != 0.0:
-                log_probs, ent = log_probs
-            actor_loss = actor_loss32 = ops.actor_loss(log_probs, old_log_probs, reward_advantages, sequence_mask,
-                                                       self.clip_range_ratio, mode=self.mode, **kw)
-            if kw.get('return_clip_fraction'):
-                actor_loss32, clip_frac = actor_loss32
-                actor_loss = actor_loss32
-            if coeff != 0.0:
-                token = 'objective' in kw and kw['objective'].token_mean
-                entropy_mean = (ops.token_mean if token else ops.masked_mean)(ent, sequence_mask)
-                actor_loss = actor_loss32 - coeff * entropy_mean
-                entropy_mean = entropy_mean.detach()
-        else:
-            logits = self._actor_logits(self.actor_model, batch, lens, use_cache=False)
-            if coeff != 0.0:
-                kw['entropy_coeff'] = coeff
-            out = ops.tail_actor_loss(logits, input_ids, lens, old_log_probs, reward_advantages, sequence_mask,
-                                      self.clip_range_ratio, mode=self.mode, **kw)
-            if kw.get('return_clip_fraction'):
-                out, clip_frac = out[:-1], out[-1]
-            actor_loss, actor_loss32 = out[0], out[2]
-            if coeff != 0.0:
-                entropy_mean = out[3]
+        actor_loss, actor_loss32, entropy_mean, clip_frac = actor_loss_node(
+            self, self.infer_batch(inference_batch), input_ids, old_log_probs, reward_advantages, sequence_mask,
+            lens=lens)
         self.actor_model.backward(actor_loss)
         self.actor_model.step()
 
@@ -200,31 +171,8 @@ class PPOTrainer(_TextPPOTrainer):
         self.reward_critic_model.backward(reward_critic_loss)
         self.reward_critic_model.step()
 
-        with torch.no_grad():
-            # see the text rl_step
-            extra = self.log_entropy or entropy_mean is not None or clip_frac is not None
-            fused = fused_allreduce(row_stats.device) if not extra else None
-            stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss32, critic_loss32,
-                                         coll=fused.next((9, 10)) if fused is not None else None)
-            if self.log_entropy:
-                stats = with_entropy_lane(stats, training_batch['entropy'], sequence_mask)
-            if entropy_mean is not None:
-                stats = with_bonus_lane(stats, entropy_mean)
-            clip_lane = stats.numel()
-            if clip_frac is not None:
-                stats = with_clip_lanes(stats, clip_frac, self)
-            if fused is None:
-                stats = all_reduce_packed(stats, max_lanes=(9, 10))
-            v = stats.tolist()  # the ONE host sync of rollout scoring + rl_step
-        ops.raise_for_status(v[10], stats.device)  # lane 10 = device status word (MAX over ranks): raise like the reference
-        out = dict(zip(METRIC_KEYS, v[:10]))
-        if self.log_entropy:
-            out['train/entropy'] = v[11]
-        if entropy_mean is not None:
-            out['train/actor_entropy'] = v[12]
-        if clip_frac is not None:
-            clip_metrics(out, v, clip_lane, self)
-        out['train/actor_lr'] = self.actor_model.optimizer.param_groups[0]['lr']
-        out['train/reward_critic_lr'] = self.reward_critic_model.optimizer.param_groups[0]['lr']
-        self.last_rl_tensors = {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns}
-        return out
+        return ppo_metrics(
+            self, row_stats, reward, value_row_mean, actor_loss32, critic_loss32,
+            {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns},
+            entropy=training_batch['entropy'] if self.log_entropy else None, mask=sequence_mask,
+            entropy_mean=entropy_mean, clip_frac=clip_frac)

@@ -57,6 +57,9 @@ class DPOTrainer:
     label_smoothing = None
     rpo_alpha = None
     reference_free = None
+    # the class attributes above that the grafted methods read: patch.install() copies them onto the reference's classes
+    SWITCHES = ('strip_pad_tokens', 'skip_identical_pairs', 'mode', 'fused_lm_head', 'lm_head_chunk_rows', 'loss_type',
+                'label_smoothing', 'rpo_alpha', 'reference_free')
 
     def __init__(self, cfgs, model, reference_model, tokenizer, infer_batch=None) -> None:
         self.cfgs = cfgs

@@ -74,6 +74,10 @@ class GRPOTrainer:
     # Opt-in: train/actor_clip_fraction (and train/actor_dual_clip_fraction with dual-clip), the mean over the updates,
     # in the step's one packed all-reduce
     log_clip_fraction = False
+    # the class attributes above that the grafted methods read: patch.install() copies them onto the reference's class
+    SWITCHES = ('mode', 'fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'num_iterations',
+                'clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode',
+                'scale_rewards', 'log_clip_fraction')
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, tokenizer=None, *, beta=None,
                  num_generations=None) -> None:
@@ -135,32 +139,23 @@ class GRPOTrainer:
             entropy_means.append(entropy_mean)
             fracs.append(cf)
         with torch.no_grad():
-            # train/loss is GRPO's loss without the bonus, the mean over the updates
-            lanes = [torch.stack([_mean(plains), rewards.float().mean()]), ops.status_lane(loss.device)]
+            # train/loss is GRPO's loss without the bonus, the mean over the updates; lane 2 = device status word, MAX
+            packed = [torch.stack([_mean(plains), rewards.float().mean()]), ops.status_lane(loss.device)]
+            lanes = {}  # the optional AVG lanes after those three, read back under their keys
             if self.log_entropy:  # token mean over the completion mask (tokens up to and including the first eos)
                 mask = torch.arange(logits_to_keep, device=row_end.device) < row_end.unsqueeze(1)
-                lanes.append(_mean([((e * mask).sum() / mask.sum()).reshape(1) for e in entropies]))
+                lanes['train/entropy'] = _mean([((e * mask).sum() / mask.sum()).reshape(1) for e in entropies])
             if entropy_means[0] is not None:
-                lanes.append(_mean([m.reshape(1) for m in entropy_means]))
-            dual = objective is not None and objective.dual_clip_ratio is not None
-            if log_cf:  # AVG lanes: the clip fraction (and the dual-clip fraction)
-                lanes.append(_mean(fracs)[:2 if dual else 1])
-            # ONE collective, ONE sync per rollout (reference: 2 + 2 per update); lane 2 = device status word, MAX
-            v = all_reduce_packed(torch.cat(lanes), max_lanes=(2,)).tolist()
+                lanes['train/actor_entropy'] = _mean([m.reshape(1) for m in entropy_means])
+            if log_cf:  # the clip fraction (and the dual-clip fraction)
+                cf = _mean(fracs)
+                lanes['train/actor_clip_fraction'] = cf[:1]
+                if objective is not None and objective.dual_clip_ratio is not None:
+                    lanes['train/actor_dual_clip_fraction'] = cf[1:2]
+            # ONE collective, ONE sync per rollout (reference: 2 + 2 per update)
+            v = all_reduce_packed(torch.cat([*packed, *lanes.values()]), max_lanes=(2,)).tolist()
         ops.raise_for_status(v[2], loss.device)
-        out = {'train/loss': v[0], 'train/reward': v[1]}
-        i = 3
-        if self.log_entropy:
-            out['train/entropy'] = v[i]
-            i += 1
-        if entropy_means[0] is not None:
-            out['train/actor_entropy'] = v[i]
-            i += 1
-        if log_cf:
-            out['train/actor_clip_fraction'] = v[i]
-            if dual:
-                out['train/actor_dual_clip_fraction'] = v[i + 1]
-        return out
+        return {'train/loss': v[0], 'train/reward': v[1], **dict(zip(lanes, v[3:]))}
 
     def train_step(self, prompt_batch: dict) -> dict[str, float]:
         """trainers/text_to_text/grpo.py:258-318; generate_completions / compute_rewards come from the reference."""

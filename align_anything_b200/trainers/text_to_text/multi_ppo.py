@@ -10,7 +10,7 @@ where the reference loops over every response position.  The group estimators ke
 flattened (B, W) token rewards (SURVEY.md H9).
 
 `fused_lm_head` (inherited from the text trainer) covers all five estimators: rollout scoring is the text trainer's
-score_rollout, and both rl_step branches take the actor node of the text trainer (actor_loss_node).
+score_rollout, and rl_step is the text trainer's, with K4r's advantages and returns for the four non-GAE estimators.
 
 Reads, besides what the text trainer reads, `self.advantage_estimator` and `self.n_samples_per_prompt`.
 """
@@ -21,9 +21,6 @@ from typing import Any
 import torch
 
 from ... import ops
-from ...utils.multi_process import all_reduce_packed, fused_allreduce
-from .ppo import (METRIC_KEYS, actor_loss_node, clip_metrics, lm_head_of, with_bonus_lane, with_clip_lanes,
-                  with_entropy_lane)
 from .ppo import PPOTrainer as _TextPPOTrainer
 
 __all__ = ['PPOTrainer']
@@ -92,64 +89,11 @@ class PPOTrainer(_TextPPOTrainer):
 
     # ---- multi_ppo.py:330-419 ---------------------------------------------------------------
     def rl_step(self, inference_batch, training_batch) -> dict[str, Any]:
-        if self.advantage_estimator == 'gae':  # textually the text trainer's rl_step
-            return _TextPPOTrainer.rl_step(self, inference_batch, training_batch)
-        old_log_probs = training_batch['log_probs']
-        ref_log_probs = training_batch['ref_log_probs']
-        reward = training_batch['reward']
-        old_reward_values = training_batch['reward_values']
-        start = training_batch['prompt_idx']
-        input_ids = inference_batch['input_ids']
-        sequence_mask = inference_batch['attention_mask'][:, 1:]
-        head = lm_head_of(self.actor_model) if self.fused_lm_head else None  # refusals before any launch
+        """The text trainer's rl_step.  Past 'gae', K4r's outputs replace K4's GAE ones: the estimator's advantages and
+        returns, with their row means written into lanes 3 / 4 of row_stats."""
+        def returns(old_rewards, sequence_mask, start, row_stats):
+            return ops.estimator_returns(old_rewards, sequence_mask, start, self.advantage_estimator,
+                                         self.n_samples_per_prompt, self.gamma, mode=self.mode, row_stats=row_stats)
 
-        # K4 gives the KL-shaped rewards, the metric row sums and the status word (its GAE output is not used); K4r
-        # then writes the estimator's advantages / returns and their row means into lanes 3 / 4 of row_stats
-        old_rewards, _, _, row_stats = ops.kl_rewards_and_gae(
-            reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, start, self.kl_coeff,
-            self.clip_range_score, self.gamma, self.gae_lambda, mode=self.mode)
-        reward_advantages, reward_returns = ops.estimator_returns(
-            old_rewards, sequence_mask, start, self.advantage_estimator, self.n_samples_per_prompt, self.gamma,
-            mode=self.mode, row_stats=row_stats)
-
-        actor_loss, actor_loss32, entropy_mean, clip_frac = actor_loss_node(
-            self, inference_batch, input_ids, start, head, old_log_probs, reward_advantages, sequence_mask)
-        self.actor_model.backward(actor_loss)
-        self.actor_model.step()
-
-        reward_values = self.reward_critic_model(**inference_batch).scores
-        reward_values = reward_values.squeeze(dim=-1)[:, :-1]
-        reward_critic_loss, value_row_mean = ops.critic_loss(
-            reward_values[:, start:], old_reward_values[:, start:], reward_returns, sequence_mask[:, start:],
-            self.clip_range_value, mode=self.mode, return_row_mean=True)
-        self.reward_critic_model.backward(reward_critic_loss)
-        self.reward_critic_model.step()
-
-        with torch.no_grad():
-            # see the text rl_step
-            extra = self.log_entropy or entropy_mean is not None or clip_frac is not None
-            fused = fused_allreduce(row_stats.device) if not extra else None
-            stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss32, reward_critic_loss,
-                                         coll=fused.next((9, 10)) if fused is not None else None)
-            if self.log_entropy:
-                stats = with_entropy_lane(stats, training_batch['entropy'][:, start:], sequence_mask[:, start:])
-            if entropy_mean is not None:
-                stats = with_bonus_lane(stats, entropy_mean)
-            clip_lane = stats.numel()
-            if clip_frac is not None:
-                stats = with_clip_lanes(stats, clip_frac, self)
-            if fused is None:
-                stats = all_reduce_packed(stats, max_lanes=(9, 10))  # ONE collective (reference: 10 + barrier)
-            v = stats.tolist()  # ONE host sync (reference: 12 .item())
-        ops.raise_for_status(v[10], stats.device)
-        out = dict(zip(METRIC_KEYS, v[:10]))
-        if self.log_entropy:
-            out['train/entropy'] = v[11]
-        if entropy_mean is not None:
-            out['train/actor_entropy'] = v[12]
-        if clip_frac is not None:
-            clip_metrics(out, v, clip_lane, self)
-        out['train/actor_lr'] = self.actor_model.optimizer.param_groups[0]['lr']
-        out['train/reward_critic_lr'] = self.reward_critic_model.optimizer.param_groups[0]['lr']
-        self.last_rl_tensors = {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns}
-        return out
+        return _TextPPOTrainer.rl_step(self, inference_batch, training_batch,
+                                       returns=None if self.advantage_estimator == 'gae' else returns)

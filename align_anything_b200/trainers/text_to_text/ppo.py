@@ -43,14 +43,6 @@ def hidden_log_probs(model, batch, input_ids, start, weight, chunk_rows, mode, r
                                            mode=mode, return_entropy=return_entropy, entropy_grad=entropy_grad)
 
 
-def with_entropy_lane(stats: torch.Tensor, entropy: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
-    """ppo_pack_metrics' vector with its spare last lane (always 0) set to the rollout policy's entropy, reduced like
-    train/kl_divergence: summed over each row's masked tokens, averaged over rows (and, by the step's one packed
-    all-reduce, over ranks), so the two read side by side.  Two tiny launches, no host sync."""
-    ent = (entropy * mask).sum(dim=-1).mean()
-    return torch.cat([stats[:11], ent.reshape(1)])
-
-
 def switch_of(tr, name: str):
     """A trainer switch in effect: `cfgs.train_cfgs.<name>` when the config sets it (a yaml recipe), otherwise the
     class attribute `<name>`."""
@@ -75,30 +67,6 @@ def actor_objective_of(tr) -> ops.ActorObjective | None:
     return ops.ActorObjective(**fields) if fields else None
 
 
-def _dual_clip_on(tr) -> bool:
-    obj = actor_objective_of(tr)
-    return obj is not None and obj.dual_clip_ratio is not None
-
-
-def with_clip_lanes(stats: torch.Tensor, clip_frac: torch.Tensor, tr) -> torch.Tensor:
-    """The packed metric vector with the clip fraction (and the dual-clip fraction when dual-clip is on) appended as
-    AVG lanes of the step's one packed all-reduce."""
-    return torch.cat([stats, clip_frac[:2 if _dual_clip_on(tr) else 1]])
-
-
-def clip_metrics(out: dict, v: list, lane: int, tr) -> None:
-    """train/actor_clip_fraction (+ train/actor_dual_clip_fraction) from the lanes with_clip_lanes appended at `lane`."""
-    out['train/actor_clip_fraction'] = v[lane]
-    if _dual_clip_on(tr):
-        out['train/actor_dual_clip_fraction'] = v[lane + 1]
-
-
-def with_bonus_lane(stats: torch.Tensor, entropy_mean: torch.Tensor) -> torch.Tensor:
-    """The packed metric vector with one more lane: the masked-mean policy entropy the bonus regularises (AVG-reduced
-    by the step's one packed all-reduce)."""
-    return torch.cat([stats, entropy_mean.detach().float().reshape(1)])
-
-
 def objective_kwargs(tr) -> dict:
     """The ops keywords of the actor objective switches: empty when they are all at their defaults (today's call)."""
     kw = {}
@@ -110,10 +78,11 @@ def objective_kwargs(tr) -> dict:
     return kw
 
 
-def actor_loss_node(tr, inference_batch, input_ids, start, head, old_log_probs, advantages, sequence_mask):
-    """The actor loss of the text rl_step over the rows `[start:]` -> (loss, the loss for ppo_pack_metrics, the
-    masked-mean entropy or None, the fp32[2] clip fractions or None).  `head`: the lm_head weight when
-    `tr.fused_lm_head` is on, else None.  With an entropy bonus (entropy_coeff_of(tr) != 0) the loss is
+def actor_loss_node(tr, batch, input_ids, old_log_probs, advantages, mask, *, start=0, head=None, lens=None):
+    """The actor loss of an rl_step -> (loss, the loss for ppo_pack_metrics, the masked-mean entropy or None, the
+    fp32[2] clip fractions or None).  The rows scored are those of the text layout, `[start:]` of every row, or with
+    `lens` the response tails of the multimodal layout (`old_log_probs`, `advantages` and `mask` already (B, W)).
+    `head`: the lm_head weight of the text layout's fused path.  With an entropy bonus (entropy_coeff_of(tr) != 0) the loss is
     actor_loss - c * masked_mean(H, mask)  over the same rows and mask (a token mean under loss_agg_mode 'token-mean'),
     the second output stays the actor loss without it.  The actor objective switches (actor_objective_of) reach K5 and
     K1f; `tr.log_clip_fraction` asks K5 for the clip fractions.  A function rather than a method, so that the grafted
@@ -121,32 +90,86 @@ def actor_loss_node(tr, inference_batch, input_ids, start, head, old_log_probs, 
     coeff = entropy_coeff_of(tr)
     kw = objective_kwargs(tr)
     cf = None
-    if head is not None:  # K6 + K6b + backward GEMMs for the log-probs, then K5
+    if lens is None:
+        old_log_probs, mask = old_log_probs[:, start:], mask[:, start:]
+    if tr.fused_lm_head:  # K6 + K6b + backward GEMMs for the log-probs, then K5
         # with a bonus K6's entropy variant; K6b adds the entropy's gradient in its epilogue
-        log_probs = hidden_log_probs(tr.actor_model, inference_batch, input_ids, start, head, tr.lm_head_chunk_rows,
-                                     tr.mode, return_entropy=coeff != 0.0, entropy_grad=coeff != 0.0, use_cache=False)
+        ent_kw = {'return_entropy': coeff != 0.0, 'entropy_grad': coeff != 0.0, 'use_cache': False}
+        if lens is None:
+            log_probs = hidden_log_probs(tr.actor_model, batch, input_ids, start, head, tr.lm_head_chunk_rows, tr.mode,
+                                         **ent_kw)
+        else:
+            log_probs = tr._tail_log_probs(tr.actor_model, batch, lens, input_ids, **ent_kw)
         if coeff != 0.0:
             log_probs, ent = log_probs
-        loss = ops.actor_loss(log_probs, old_log_probs[:, start:], advantages, sequence_mask[:, start:],
-                              tr.clip_range_ratio, mode=tr.mode, **kw)
+        loss = ops.actor_loss(log_probs, old_log_probs, advantages, mask, tr.clip_range_ratio, mode=tr.mode, **kw)
         if kw.get('return_clip_fraction'):
             loss, cf = loss
         if coeff == 0.0:
             return loss, loss, None, cf
         token = 'objective' in kw and kw['objective'].token_mean
-        h_mean = (ops.token_mean if token else ops.masked_mean)(ent, sequence_mask[:, start:])
+        h_mean = (ops.token_mean if token else ops.masked_mean)(ent, mask)
         return loss - coeff * h_mean, loss, h_mean.detach(), cf
-    logits = tr.actor_model(**inference_batch, use_cache=False).logits
-    # the reference scores every position and then slices `[:, start:]` (:338-346); only those rows are ever used, so
-    # only they are read here.  One autograd node (K1f): log-probs, d loss / d log-prob and the gradient tile in a
-    # single pass over the response rows; the prompt rows of the tile are written as zeros by the same kernel.
+    # One autograd node (K1f): log-probs, d loss / d log-prob and the gradient tile in a single pass over the scored
+    # rows.  The text layout reads only the rows `[start:]` the reference keeps after scoring every position
+    # (:338-346); the prompt rows of the tile are written as zeros by the same kernel.
     if coeff != 0.0:
         kw['entropy_coeff'] = coeff
-    out = ops.dense_actor_loss(logits, input_ids, start, old_log_probs[:, start:], advantages, sequence_mask[:, start:],
-                               tr.clip_range_ratio, mode=tr.mode, **kw)
+    if lens is None:
+        logits = tr.actor_model(**batch, use_cache=False).logits
+        out = ops.dense_actor_loss(logits, input_ids, start, old_log_probs, advantages, mask, tr.clip_range_ratio,
+                                   mode=tr.mode, **kw)
+    else:
+        logits = tr._actor_logits(tr.actor_model, batch, lens, use_cache=False)
+        out = ops.tail_actor_loss(logits, input_ids, lens, old_log_probs, advantages, mask, tr.clip_range_ratio,
+                                  mode=tr.mode, **kw)
     if kw.get('return_clip_fraction'):
         out, cf = out[:-1], out[-1]
     return out[0], out[2], (out[3] if coeff != 0.0 else None), cf
+
+
+def ppo_metrics(tr, row_stats, reward, value_row_mean, actor_loss, critic_loss, tensors, *, entropy=None, mask=None,
+                entropy_mean=None, clip_frac=None) -> dict[str, Any]:
+    """The metric dict of a PPO rl_step from ONE packed collective and ONE host sync (reference: 10 all-reduces, a
+    barrier and 12 .item()).  ppo_pack_metrics packs the ten metrics of METRIC_KEYS, the device status word (lane 10,
+    MAX-reduced with lane 9) and a spare lane 11 (0).  Optional AVG lanes follow, each read back under its key:
+      * `entropy` (the rollout policy's, with `mask`; both over the scored rows) takes lane 11 as train/entropy, reduced
+        like train/kl_divergence: summed over each row's masked tokens, averaged over rows and ranks;
+      * `entropy_mean`, the entropy term of the bonus (train/actor_entropy);
+      * `clip_frac`, K5's clip fraction (train/actor_clip_fraction) and with dual-clip its dual-clip fraction
+        (train/actor_dual_clip_fraction).
+    Sets `tr.last_rl_tensors = tensors` (per-token tensors stay out of the dict: the reference hands it to Logger.log,
+    which takes scalars only)."""
+    with torch.no_grad():
+        # an optional lane is filled in before the one packed all-reduce, so the NVLink reduction fused into
+        # ppo_pack_metrics (which reduces the vector as it writes it) gives way to all_reduce_packed
+        extra = entropy is not None or entropy_mean is not None or clip_frac is not None
+        fused = fused_allreduce(row_stats.device) if not extra else None
+        stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss, critic_loss,
+                                     coll=fused.next((9, 10)) if fused is not None else None)
+        lanes = {}
+        if entropy is not None:
+            lanes['train/entropy'] = (entropy * mask).sum(dim=-1).mean().reshape(1)
+        if entropy_mean is not None:
+            lanes['train/actor_entropy'] = entropy_mean.detach().float().reshape(1)
+        if clip_frac is not None:
+            lanes['train/actor_clip_fraction'] = clip_frac[:1]
+            objective = actor_objective_of(tr)
+            if objective is not None and objective.dual_clip_ratio is not None:
+                lanes['train/actor_dual_clip_fraction'] = clip_frac[1:2]
+        first = 11 if entropy is not None else 12  # the entropy takes the spare lane 11
+        if lanes:
+            stats = torch.cat([stats[:first], *lanes.values()])
+        if fused is None:
+            stats = all_reduce_packed(stats, max_lanes=(9, 10))
+        v = stats.tolist()
+    ops.raise_for_status(v[10], stats.device)  # the device status word (MAX over ranks): raise like the reference
+    out = dict(zip(METRIC_KEYS, v[:10]))
+    out.update(zip(lanes, v[first:]))
+    out['train/actor_lr'] = tr.actor_model.optimizer.param_groups[0]['lr']
+    out['train/reward_critic_lr'] = tr.reward_critic_model.optimizer.param_groups[0]['lr']
+    tr.last_rl_tensors = tensors
+    return out
 
 
 class PPOTrainer:
@@ -175,6 +198,9 @@ class PPOTrainer:
     # Opt-in: train/actor_clip_fraction (and train/actor_dual_clip_fraction with dual-clip) from K5, reduced in the
     # step's one packed all-reduce
     log_clip_fraction = False
+    # the class attributes above that the grafted methods read: patch.install() copies them onto the reference's classes
+    SWITCHES = ('mode', 'fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'clip_range_ratio_low',
+                'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode', 'log_clip_fraction')
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, reward_model=None,
                  reward_critic_model=None, tokenizer=None, reward_tokenizer=None, *, kl_coeff=0.02,
@@ -329,7 +355,9 @@ class PPOTrainer:
         return {'train/ptx_loss': ptx_loss.item()}
 
     # ---- trainers/text_to_text/ppo.py:309-398 -----------------------------------------------
-    def rl_step(self, inference_batch, training_batch) -> dict[str, Any]:
+    def rl_step(self, inference_batch, training_batch, returns=None) -> dict[str, Any]:
+        """returns: None for K4's GAE advantages and returns, or `returns(old_rewards, sequence_mask, start, row_stats)
+        -> (advantages, returns)`, which also rewrites their metric lanes of row_stats (Multi-PPO's K4r)."""
         old_log_probs = training_batch['log_probs']
         ref_log_probs = training_batch['ref_log_probs']
         reward = training_batch['reward']
@@ -342,9 +370,11 @@ class PPOTrainer:
         old_rewards, reward_advantages, reward_returns, row_stats = ops.kl_rewards_and_gae(
             reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, start, self.kl_coeff,
             self.clip_range_score, self.gamma, self.gae_lambda, mode=self.mode)
+        if returns is not None:
+            reward_advantages, reward_returns = returns(old_rewards, sequence_mask, start, row_stats)
 
         actor_loss, actor_loss32, entropy_mean, clip_frac = actor_loss_node(
-            self, inference_batch, input_ids, start, head, old_log_probs, reward_advantages, sequence_mask)
+            self, inference_batch, input_ids, old_log_probs, reward_advantages, sequence_mask, start=start, head=head)
         self.actor_model.backward(actor_loss)
         self.actor_model.step()
 
@@ -356,35 +386,8 @@ class PPOTrainer:
         self.reward_critic_model.backward(reward_critic_loss)
         self.reward_critic_model.step()
 
-        with torch.no_grad():
-            # with log_entropy the entropy lane is filled in before the one packed all-reduce, so the NVLink reduction
-            # fused into ppo_pack_metrics (which reduces the vector as it writes it) gives way to all_reduce_packed
-            # (so does the entropy bonus's lane)
-            extra = self.log_entropy or entropy_mean is not None or clip_frac is not None
-            fused = fused_allreduce(row_stats.device) if not extra else None
-            stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss32, reward_critic_loss,
-                                         coll=fused.next((9, 10)) if fused is not None else None)
-            if self.log_entropy:
-                stats = with_entropy_lane(stats, training_batch['entropy'][:, start:], sequence_mask[:, start:])
-            if entropy_mean is not None:
-                stats = with_bonus_lane(stats, entropy_mean)
-            clip_lane = stats.numel()
-            if clip_frac is not None:
-                stats = with_clip_lanes(stats, clip_frac, self)
-            if fused is None:
-                stats = all_reduce_packed(stats, max_lanes=(9, 10))  # ONE collective (reference: 10 + barrier)
-            v = stats.tolist()  # ONE host sync (reference: 12 .item())
-        ops.raise_for_status(v[10], stats.device)  # lane 10 = device status word (MAX over ranks): raise like the reference
-        out = dict(zip(METRIC_KEYS, v[:10]))
-        if self.log_entropy:
-            out['train/entropy'] = v[11]
-        if entropy_mean is not None:
-            out['train/actor_entropy'] = v[12]
-        if clip_frac is not None:
-            clip_metrics(out, v, clip_lane, self)
-        out['train/actor_lr'] = self.actor_model.optimizer.param_groups[0]['lr']
-        out['train/reward_critic_lr'] = self.reward_critic_model.optimizer.param_groups[0]['lr']
-        # the per-token tensors stay OUT of the returned dict: the reference hands it to Logger.log -> add_scalar /
-        # wandb.log (utils/logger.py:130-138), which takes scalars only.  Tests read them from this attribute.
-        self.last_rl_tensors = {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns}
-        return out
+        return ppo_metrics(
+            self, row_stats, reward, value_row_mean, actor_loss32, reward_critic_loss,
+            {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns},
+            entropy=training_batch['entropy'][:, start:] if self.log_entropy else None, mask=sequence_mask[:, start:],
+            entropy_mean=entropy_mean, clip_frac=clip_frac)

@@ -15,6 +15,8 @@ __all__ = ['RMTrainer']
 
 
 class RMTrainer:
+    SWITCHES = ()  # the grafted methods read no class attribute of ours
+
     def __init__(self, cfgs, model, tokenizer=None, infer_batch=None) -> None:
         self.cfgs = cfgs
         self.model = model

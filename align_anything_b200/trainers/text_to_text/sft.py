@@ -21,6 +21,8 @@ class SupervisedTrainer:
     # ops.causal_lm_loss_from_hidden over the rows whose next label is not ignored; the gradient is formed in the forward.
     fused_lm_head = False
     lm_head_chunk_rows = None
+    # the class attributes above that the grafted methods read: patch.install() copies them onto the reference's classes
+    SWITCHES = ('ignore_index', 'fused_lm_head', 'lm_head_chunk_rows')
 
     def __init__(self, cfgs, model, tokenizer=None, infer_batch=None) -> None:
         self.cfgs = cfgs
