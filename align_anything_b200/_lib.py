@@ -78,6 +78,9 @@ _SIGS = {
     'aa_ppo_prep': (c_int, [_P, _P, c_int, c_int64, _P, _P, c_int, c_int64, _P, c_int64, c_int32, c_int32,
                             c_int32, c_float, c_float, c_float, c_float, c_int, _P, c_int, _P, _P, c_int, _P,
                             _P, _P]),
+    'aa_ppo_prep_kl': (c_int, [_P, _P, c_int, c_int64, _P, _P, c_int, c_int64, _P, c_int64, c_int32, c_int32,
+                               c_int32, c_float, c_int, c_float, c_float, c_float, c_int, _P, c_int, _P, _P, c_int, _P,
+                               _P, _P]),
     'aa_ppo_returns': (c_int, [_P, c_int, c_int64, _P, c_int64, c_int32, c_int32, c_int32, c_int, c_int32, c_float,
                                c_int, c_int, _P, _P, c_int, _P, _P]),
     'aa_ppo_actor_loss': (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, c_int32,
@@ -108,6 +111,9 @@ _SIGS = {
     'aa_logprob_grpo_fused_obj': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P, c_int,
                                           _P, c_int64, _P, _P, _P, c_int64, c_int64, c_int32, c_float, c_float, c_float,
                                           c_float, c_int, c_int, _P, c_int64, _P, _P, _P, _P, _P, _P, c_float, _P]),
+    'aa_logprob_grpo_fused_kl': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P, c_int,
+                                         _P, c_int64, _P, _P, _P, c_int64, c_int64, c_int32, c_float, c_float, c_float,
+                                         c_float, c_int, c_int, c_int, _P, c_int64, _P, _P, _P, _P, _P, _P, c_float, _P]),
     'aa_scale_tile': (c_int, [_P, c_int, c_int64, _P, c_int, _P]),
     'aa_tail_scatter_scaled': (c_int, [_P, c_int, c_int64, _P, c_int32, c_int32, c_int32, _P, c_int, _P, c_int64, c_int32, _P]),
     'aa_group_advantages': (c_int, [_P, c_int32, c_int32, _P, _P]),
@@ -116,6 +122,9 @@ _SIGS = {
     'aa_group_advantages_centered': (c_int, [_P, c_int32, c_int32, _P, _P]),
     'aa_grpo_loss_obj': (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int, _P, _P, c_int64, c_int64, c_int32, c_int32,
                                  c_float, c_float, c_float, c_float, c_int, c_int, _P, _P, c_int64, _P, _P, _P, _P, _P]),
+    'aa_grpo_loss_kl': (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int, _P, _P, c_int64, c_int64, c_int32, c_int32,
+                                c_float, c_float, c_float, c_float, c_int, c_int, c_int, _P, _P, c_int64, _P, _P, _P, _P,
+                                _P]),
     'aa_nll_mean': (c_int, [_P, c_int, _P, c_int64, c_int64, _P, _P, _P, _P, _P]),
     'aa_masked_mean': (c_int, [_P, c_int, c_int64, _P, c_int64, c_int32, c_int32, _P, _P, _P, _P]),
     'aa_ppo_pack_metrics': (c_int, [_P, _P, _P, _P, _P, c_int32, _P, POINTER(AaColl), _P, _P]),

@@ -72,6 +72,7 @@ struct FusedActorParams {
   int kind;
   const void *old_pol;
   float clip_lo;
+  int kl_est;  // kind 3: the per-token KL's estimator (AA_KL_*; aa_logprob_grpo_fused_obj: AA_KL_K3)
   int64_t ignore_index;
   const float *ce_coeff;
   const int32_t *row_end;
@@ -455,7 +456,8 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
         if (p.kind == 3) {
           const float lpr = round_to(lp, p.out_dtype);
           const float po = p.old_pol ? load_as_float(p.old_pol, out_idx, p.out_dtype) : lpr;
-          grpo_obj_token(lpr, po, old, adv, on, g_rs, p.clip, p.clip_lo, p.clip_hi, p.dual, p.rx, obj, g, why);
+          grpo_obj_token(lpr, po, old, adv, on, g_rs, p.clip, p.clip_lo, p.clip_hi, p.dual, p.kl_est, p.rx, obj, g,
+                         why);
         }
         sh_b[0] = m;
         sh_b[1] = logsum;
@@ -820,7 +822,7 @@ extern "C" int aa_logprob_ce_fused(const void *logits, int logits_dtype, int64_t
 struct GrpoObjective {
   const void *old_pol;
   float clip_lo, clip_hi, dual;
-  int agg;
+  int agg, kl_est;
 };
 
 // aa_logprob_grpo_fused{,_entropy,_obj}: entropy == nullptr runs the plain kernels; obj == nullptr: kind 2
@@ -871,6 +873,7 @@ static int logprob_grpo_fused(float *entropy, float entropy_coeff, bool egrad, c
     p.clip_hi = obj->clip_hi;
     p.dual = obj->dual;
     p.agg = obj->agg;
+    p.kl_est = obj->kl_est;
   }
   return launch_fused(p, logits_dtype, mode, static_cast<FusedRec *>(row_scratch), n_tile_rows, st, egrad);
 }
@@ -926,6 +929,32 @@ extern "C" int aa_logprob_grpo_fused_entropy_grad(const void *logits, int logits
                             row_scratch, row_end, total, counter, status, stream);
 }
 
+// aa_logprob_grpo_fused_obj / _kl: the objective's checks, then kind 3
+static int logprob_grpo_fused_objective(const char *who, const void *logits, int logits_dtype, int64_t row_stride,
+                                        int32_t V, const int64_t *labels, int32_t n_segments,
+                                        const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                                        const int64_t *seg_out_off, const int64_t *seg_cum, const int64_t *seg_tile_row,
+                                        int64_t n_tile_rows, void *log_probs, int lp_dtype, const void *ref_log_probs,
+                                        int64_t ref_stride, const void *old_log_probs, const float *advantages,
+                                        const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t K,
+                                        float beta, float clip_low, float clip_high, float dual_clip, int loss_agg,
+                                        int kl_estimator, int mode, void *grad_logits, int64_t grad_row_stride,
+                                        void *row_scratch, int32_t *row_end, float *total, uint32_t *counter,
+                                        int32_t *status, float *entropy, float entropy_coeff, void *stream) {
+  AA_REQUIRE(grpo_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
+             "%s: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a known loss_agg; got %g "
+             "%g %g %d)", who, clip_low, clip_high, dual_clip, loss_agg);
+  AA_REQUIRE(kl_estimator_ok(kl_estimator), AA_ERR_ARG, "%s: unknown kl_estimator code %d", who, kl_estimator);
+  AA_REQUIRE(entropy_coeff == entropy_coeff, AA_ERR_ARG, "%s: entropy_coeff is NaN", who);
+  AA_REQUIRE(entropy || entropy_coeff == 0.f, AA_ERR_ARG, "%s: entropy_coeff needs entropy", who);
+  GrpoObjective obj{old_log_probs, clip_low, clip_high, dual_clip, loss_agg, kl_estimator};
+  return logprob_grpo_fused(entropy, entropy_coeff, entropy && entropy_coeff != 0.f, who, logits, logits_dtype,
+                            row_stride, V, labels, n_segments, seg_logit_off, seg_label_off, seg_out_off, seg_cum,
+                            seg_tile_row, n_tile_rows, log_probs, lp_dtype, ref_log_probs, ref_stride, advantages,
+                            completion_tokens, tok_stride, eos_id, K, beta, mode, grad_logits, grad_row_stride,
+                            row_scratch, row_end, total, counter, status, stream, &obj);
+}
+
 extern "C" int aa_logprob_grpo_fused_obj(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
                                          const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
                                          const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
@@ -937,17 +966,31 @@ extern "C" int aa_logprob_grpo_fused_obj(const void *logits, int logits_dtype, i
                                          int64_t grad_row_stride, void *row_scratch, int32_t *row_end, float *total,
                                          uint32_t *counter, int32_t *status, float *entropy, float entropy_coeff,
                                          void *stream) {
-  AA_REQUIRE(grpo_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
-             "aa_logprob_grpo_fused_obj: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a "
-             "known loss_agg; got %g %g %g %d)", clip_low, clip_high, dual_clip, loss_agg);
-  AA_REQUIRE(entropy_coeff == entropy_coeff, AA_ERR_ARG, "aa_logprob_grpo_fused_obj: entropy_coeff is NaN");
-  AA_REQUIRE(entropy || entropy_coeff == 0.f, AA_ERR_ARG, "aa_logprob_grpo_fused_obj: entropy_coeff needs entropy");
-  GrpoObjective obj{old_log_probs, clip_low, clip_high, dual_clip, loss_agg};
-  return logprob_grpo_fused(entropy, entropy_coeff, entropy && entropy_coeff != 0.f, "aa_logprob_grpo_fused_obj",
-                            logits, logits_dtype, row_stride, V, labels, n_segments, seg_logit_off, seg_label_off,
-                            seg_out_off, seg_cum, seg_tile_row, n_tile_rows, log_probs, lp_dtype, ref_log_probs,
-                            ref_stride, advantages, completion_tokens, tok_stride, eos_id, K, beta, mode, grad_logits,
-                            grad_row_stride, row_scratch, row_end, total, counter, status, stream, &obj);
+  return logprob_grpo_fused_objective("aa_logprob_grpo_fused_obj", logits, logits_dtype, row_stride, V, labels,
+                                      n_segments, seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row,
+                                      n_tile_rows, log_probs, lp_dtype, ref_log_probs, ref_stride, old_log_probs,
+                                      advantages, completion_tokens, tok_stride, eos_id, K, beta, clip_low, clip_high,
+                                      dual_clip, loss_agg, AA_KL_K3, mode, grad_logits, grad_row_stride, row_scratch,
+                                      row_end, total, counter, status, entropy, entropy_coeff, stream);
+}
+
+extern "C" int aa_logprob_grpo_fused_kl(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                        const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                        const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
+                                        const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
+                                        const void *ref_log_probs, int64_t ref_stride, const void *old_log_probs,
+                                        const float *advantages, const int64_t *completion_tokens, int64_t tok_stride,
+                                        int64_t eos_id, int32_t K, float beta, float clip_low, float clip_high,
+                                        float dual_clip, int loss_agg, int kl_estimator, int mode, void *grad_logits,
+                                        int64_t grad_row_stride, void *row_scratch, int32_t *row_end, float *total,
+                                        uint32_t *counter, int32_t *status, float *entropy, float entropy_coeff,
+                                        void *stream) {
+  return logprob_grpo_fused_objective("aa_logprob_grpo_fused_kl", logits, logits_dtype, row_stride, V, labels,
+                                      n_segments, seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row,
+                                      n_tile_rows, log_probs, lp_dtype, ref_log_probs, ref_stride, old_log_probs,
+                                      advantages, completion_tokens, tok_stride, eos_id, K, beta, clip_low, clip_high,
+                                      dual_clip, loss_agg, kl_estimator, mode, grad_logits, grad_row_stride,
+                                      row_scratch, row_end, total, counter, status, entropy, entropy_coeff, stream);
 }
 
 extern "C" int aa_scale_tile(void *tile, int dtype, int64_t n, const void *scale, int scale_dtype, void *stream) {

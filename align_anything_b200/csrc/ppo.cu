@@ -68,6 +68,7 @@ struct PrepParams {
   int adv_dtype;
   float *row_stats;
   int32_t *status;
+  int kl_est;  // the penalty's KL estimator (AA_KL_*; aa_ppo_prep: AA_KL_K1).  The metric row sums stay k1
 };
 
 // one warp per sample; the row (masked values, shaped rewards) is staged in shared memory so that the
@@ -98,8 +99,11 @@ __global__ void __launch_bounds__(32) ppo_prep_kernel(const PrepParams p) {
     const bool on = mrow[t] != 0;
     float kl = 0.f, r;
     if (p.lp) {
-      kl = round_to(load_as_float(p.lp, lpo + t, p.lp_dtype) - load_as_float(p.ref_lp, lpo + t, p.lp_dtype), p.r_lp);
-      r = round_to(-p.kl_coeff * kl, p.r_lp);
+      const float x = load_as_float(p.lp, lpo + t, p.lp_dtype), rf = load_as_float(p.ref_lp, lpo + t, p.lp_dtype);
+      float aux;
+      kl = round_to(x - rf, p.r_lp);
+      const float pen = (p.kl_est == AA_KL_K1) ? kl : kl_value(x, rf, p.kl_est, p.r_lp, aux);
+      r = round_to(-p.kl_coeff * pen, p.r_lp);
       if (t == end) r = round_to(r + rew_end, p.r_lp);
       r = fminf(fmaxf(r, -clip), clip);
       store_from_float(p.old_rewards, ro + t, p.rew_dtype, r);
@@ -611,6 +615,7 @@ struct GrpoObjParams {
   float clip_lo, clip_hi, dual;
   int agg;
   float *clip_frac;  // optional fp32[2]; row_scratch then holds 4 * B floats
+  int kl_est;        // the per-token KL's estimator (AA_KL_*; aa_grpo_loss_obj: AA_KL_K3)
 };
 
 // GRPO's loss and d loss / d lp, one block per row, the last block to arrive reduces the rows.  OBJECTIVE: the clipped
@@ -635,7 +640,7 @@ __global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoObjParams 
     int why = 0;
     if constexpr (OBJECTIVE) {
       const float old = q.old ? load_as_float(q.old, b * q.old_stride + t, p.dtype) : lp;
-      grpo_obj_token(lp, old, rf, A, on, g_t, p.beta, q.clip_lo, q.clip_hi, q.dual, r, ptl, g, why);
+      grpo_obj_token(lp, old, rf, A, on, g_t, p.beta, q.clip_lo, q.clip_hi, q.dual, q.kl_est, r, ptl, g, why);
     } else {
       grpo_token(lp, rf, A, on, g_t, p.beta, r, ptl, g);
     }
@@ -777,12 +782,11 @@ static bool dtype_ok(int d) { return d == AA_BF16 || d == AA_F16 || d == AA_F32;
 
 using namespace aa;
 
-extern "C" int aa_ppo_prep(const void *log_probs, const void *ref_log_probs, int lp_dtype,
-                           int64_t lp_row_stride, const float *reward, const void *values, int val_dtype,
-                           int64_t val_row_stride, const uint8_t *mask, int64_t mask_row_stride, int32_t B,
-                           int32_t W, int32_t start, float kl_coeff, float clip_range_score, float gamma,
-                           float gae_lambda, int mode, void *old_rewards, int rew_dtype, void *advantages,
-                           void *returns, int adv_dtype, float *row_stats, int32_t *status, void *stream) {
+static int ppo_prep(const void *log_probs, const void *ref_log_probs, int lp_dtype, int64_t lp_row_stride,
+                    const float *reward, const void *values, int val_dtype, int64_t val_row_stride, const uint8_t *mask,
+                    int64_t mask_row_stride, int32_t B, int32_t W, int32_t start, float kl_coeff, int kl_estimator,
+                    float clip_range_score, float gamma, float gae_lambda, int mode, void *old_rewards, int rew_dtype,
+                    void *advantages, void *returns, int adv_dtype, float *row_stats, int32_t *status, void *stream) {
   AA_REQUIRE(B > 0 && W > 0 && start >= 0 && start < W, AA_ERR_ARG, "aa_ppo_prep: bad sizes (B=%d W=%d start=%d)", B, W, start);
   AA_REQUIRE(values && mask && old_rewards && advantages && returns && row_stats, AA_ERR_ARG,
              "aa_ppo_prep: null pointer");
@@ -794,7 +798,7 @@ extern "C" int aa_ppo_prep(const void *log_probs, const void *ref_log_probs, int
   PrepParams p{log_probs, ref_log_probs, lp_dtype, lp_row_stride, reward, values, val_dtype, val_row_stride,
                mask, mask_row_stride, B, W, start, kl_coeff, clip_range_score, gamma, gae_lambda,
                f ? lp_dtype : AA_F32, f ? val_dtype : AA_F32, f ? adv_dtype : AA_F32,
-               old_rewards, rew_dtype, advantages, returns, adv_dtype, row_stats, status};
+               old_rewards, rew_dtype, advantages, returns, adv_dtype, row_stats, status, kl_estimator};
   const size_t smem = static_cast<size_t>(3 * (W + 1)) * sizeof(float);
   if (smem > 48 * 1024) {
     AA_REQUIRE(smem <= 200 * 1024, AA_ERR_UNSUPPORTED, "aa_ppo_prep: W=%d does not fit in shared memory", W);
@@ -806,6 +810,31 @@ extern "C" int aa_ppo_prep(const void *log_probs, const void *ref_log_probs, int
   }
   ppo_prep_kernel<<<B, 32, smem, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("aa_ppo_prep");
+}
+
+extern "C" int aa_ppo_prep(const void *log_probs, const void *ref_log_probs, int lp_dtype,
+                           int64_t lp_row_stride, const float *reward, const void *values, int val_dtype,
+                           int64_t val_row_stride, const uint8_t *mask, int64_t mask_row_stride, int32_t B,
+                           int32_t W, int32_t start, float kl_coeff, float clip_range_score, float gamma,
+                           float gae_lambda, int mode, void *old_rewards, int rew_dtype, void *advantages,
+                           void *returns, int adv_dtype, float *row_stats, int32_t *status, void *stream) {
+  return ppo_prep(log_probs, ref_log_probs, lp_dtype, lp_row_stride, reward, values, val_dtype, val_row_stride, mask,
+                  mask_row_stride, B, W, start, kl_coeff, AA_KL_K1, clip_range_score, gamma, gae_lambda, mode,
+                  old_rewards, rew_dtype, advantages, returns, adv_dtype, row_stats, status, stream);
+}
+
+extern "C" int aa_ppo_prep_kl(const void *log_probs, const void *ref_log_probs, int lp_dtype, int64_t lp_row_stride,
+                              const float *reward, const void *values, int val_dtype, int64_t val_row_stride,
+                              const uint8_t *mask, int64_t mask_row_stride, int32_t B, int32_t W, int32_t start,
+                              float kl_coeff, int kl_estimator, float clip_range_score, float gamma, float gae_lambda,
+                              int mode, void *old_rewards, int rew_dtype, void *advantages, void *returns,
+                              int adv_dtype, float *row_stats, int32_t *status, void *stream) {
+  AA_REQUIRE(kl_estimator_ok(kl_estimator), AA_ERR_ARG, "aa_ppo_prep_kl: unknown kl_estimator code %d", kl_estimator);
+  AA_REQUIRE(isfinite(kl_coeff), AA_ERR_ARG, "aa_ppo_prep_kl: kl_coeff must be finite, got %g", kl_coeff);
+  AA_REQUIRE(log_probs != nullptr, AA_ERR_ARG, "aa_ppo_prep_kl: log_probs is NULL (the GAE-only form is aa_ppo_prep)");
+  return ppo_prep(log_probs, ref_log_probs, lp_dtype, lp_row_stride, reward, values, val_dtype, val_row_stride, mask,
+                  mask_row_stride, B, W, start, kl_coeff, kl_estimator, clip_range_score, gamma, gae_lambda, mode,
+                  old_rewards, rew_dtype, advantages, returns, adv_dtype, row_stats, status, stream);
 }
 
 extern "C" int aa_ppo_returns(const void *rewards, int rew_dtype, int64_t rew_row_stride, const uint8_t *mask,
@@ -953,13 +982,12 @@ extern "C" int aa_group_advantages(const float *rewards, int32_t n_groups, int32
 
 // aa_grpo_loss (objective false: the reference's loss, any mode) and aa_grpo_loss_obj: the checks, the completion mask
 // (row_end, and the token count in scratch[0]) and the loss kernel over scratch + 1
-static int grpo_loss(bool objective, const void *log_probs, int64_t lp_stride, const void *ref_log_probs,
+static int grpo_loss(const char *who, bool objective, const void *log_probs, int64_t lp_stride, const void *ref_log_probs,
                      int64_t ref_stride, const void *old_log_probs, int64_t old_stride, int lp_dtype,
                      const float *advantages, const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id,
                      int32_t B, int32_t K, float beta, float clip_low, float clip_high, float dual_clip, int loss_agg,
-                     int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac, int32_t *row_end,
-                     float *scratch, uint32_t *counter, void *stream) {
-  const char *who = objective ? "aa_grpo_loss_obj" : "aa_grpo_loss";
+                     int kl_estimator, int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac,
+                     int32_t *row_end, float *scratch, uint32_t *counter, void *stream) {
   AA_REQUIRE(B > 0 && K > 0 && log_probs && ref_log_probs && advantages && completion_tokens && loss && row_end &&
                  scratch && counter,
              AA_ERR_ARG, "%s: bad arguments", who);
@@ -969,6 +997,7 @@ static int grpo_loss(bool objective, const void *log_probs, int64_t lp_stride, c
                "%s: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a known loss_agg; got "
                "%g %g %g %d)", who, clip_low, clip_high, dual_clip, loss_agg);
     AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "%s: bad mode", who);
+    AA_REQUIRE(kl_estimator_ok(kl_estimator), AA_ERR_ARG, "%s: unknown kl_estimator code %d", who, kl_estimator);
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   grpo_mask_kernel<128><<<B, 128, 0, st>>>(completion_tokens, tok_stride, B, K, eos_id, row_end, scratch, counter);
@@ -977,7 +1006,7 @@ static int grpo_loss(bool objective, const void *log_probs, int64_t lp_stride, c
   GrpoObjParams q{GrpoParams{log_probs, ref_log_probs, lp_dtype, lp_stride, ref_stride, advantages, row_end, scratch, B,
                              K, beta, (mode == AA_MODE_FAITHFUL) ? lp_dtype : AA_F32, loss, grad, grad_stride,
                              scratch + 1, counter + 1},
-                  old_log_probs, old_stride, clip_low, clip_high, dual_clip, loss_agg, clip_frac};
+                  old_log_probs, old_stride, clip_low, clip_high, dual_clip, loss_agg, clip_frac, kl_estimator};
   if (objective)
     grpo_loss_kernel<128, true><<<B, 128, 0, st>>>(q);
   else
@@ -990,9 +1019,9 @@ extern "C" int aa_grpo_loss(const void *log_probs, int64_t lp_stride, const void
                             int64_t tok_stride, int64_t eos_id, int32_t B, int32_t K, float beta, int mode,
                             float *loss, void *grad, int64_t grad_stride, int32_t *row_end, float *scratch,
                             uint32_t *counter, void *stream) {
-  return grpo_loss(false, log_probs, lp_stride, ref_log_probs, ref_stride, nullptr, 0, lp_dtype, advantages,
-                   completion_tokens, tok_stride, eos_id, B, K, beta, 0.f, 0.f, 0.f, AA_AGG_TOKEN_MEAN, mode, loss, grad,
-                   grad_stride, nullptr, row_end, scratch, counter, stream);
+  return grpo_loss("aa_grpo_loss", false, log_probs, lp_stride, ref_log_probs, ref_stride, nullptr, 0, lp_dtype,
+                   advantages, completion_tokens, tok_stride, eos_id, B, K, beta, 0.f, 0.f, 0.f, AA_AGG_TOKEN_MEAN,
+                   AA_KL_K3, mode, loss, grad, grad_stride, nullptr, row_end, scratch, counter, stream);
 }
 
 extern "C" int aa_group_advantages_centered(const float *rewards, int32_t n_groups, int32_t group_size,
@@ -1010,9 +1039,22 @@ extern "C" int aa_grpo_loss_obj(const void *log_probs, int64_t lp_stride, const 
                                 int32_t K, float beta, float clip_low, float clip_high, float dual_clip, int loss_agg,
                                 int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac,
                                 int32_t *row_end, float *scratch, uint32_t *counter, void *stream) {
-  return grpo_loss(true, log_probs, lp_stride, ref_log_probs, ref_stride, old_log_probs, old_stride, lp_dtype, advantages,
-                   completion_tokens, tok_stride, eos_id, B, K, beta, clip_low, clip_high, dual_clip, loss_agg, mode, loss,
-                   grad, grad_stride, clip_frac, row_end, scratch, counter, stream);
+  return grpo_loss("aa_grpo_loss_obj", true, log_probs, lp_stride, ref_log_probs, ref_stride, old_log_probs, old_stride,
+                   lp_dtype, advantages, completion_tokens, tok_stride, eos_id, B, K, beta, clip_low, clip_high,
+                   dual_clip, loss_agg, AA_KL_K3, mode, loss, grad, grad_stride, clip_frac, row_end, scratch, counter,
+                   stream);
+}
+
+extern "C" int aa_grpo_loss_kl(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
+                               const void *old_log_probs, int64_t old_stride, int lp_dtype, const float *advantages,
+                               const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B,
+                               int32_t K, float beta, float clip_low, float clip_high, float dual_clip, int loss_agg,
+                               int kl_estimator, int mode, float *loss, void *grad, int64_t grad_stride,
+                               float *clip_frac, int32_t *row_end, float *scratch, uint32_t *counter, void *stream) {
+  return grpo_loss("aa_grpo_loss_kl", true, log_probs, lp_stride, ref_log_probs, ref_stride, old_log_probs, old_stride,
+                   lp_dtype, advantages, completion_tokens, tok_stride, eos_id, B, K, beta, clip_low, clip_high,
+                   dual_clip, loss_agg, kl_estimator, mode, loss, grad, grad_stride, clip_frac, row_end, scratch,
+                   counter, stream);
 }
 
 extern "C" int aa_nll_mean(const void *logp, int dtype, const int64_t *labels, int64_t n, int64_t ignore_index,

@@ -79,6 +79,38 @@ __device__ __forceinline__ void actor_token(float x, float old, float aux, bool 
 }
 
 
+// ---- KL estimators (ops.KL_ESTIMATORS; tests/kl_objective_port.py is their specification) ---------------------
+// One token's estimate of KL(policy || reference) from the log-probs lp and rf, each op rounded to `r` as the eager
+// expression rounds it:
+//   AA_KL_K1  lp - rf
+//   AA_KL_K2  0.5 * (lp - rf) ** 2
+//   AA_KL_K3  exp(rf - lp) - (rf - lp) - 1      (the reference GRPO's expression, op for op)
+// aux: what kl_grad needs of the forward (k2: lp - rf; k3: exp(rf - lp)).
+inline bool kl_estimator_ok(int est) { return est == AA_KL_K1 || est == AA_KL_K2 || est == AA_KL_K3; }
+
+__device__ __forceinline__ float kl_value(float lp, float rf, int est, int r, float &aux) {
+  if (est == AA_KL_K3) {
+    const float d = round_to(rf - lp, r);
+    aux = round_to(expf(d), r);
+    return round_to(round_to(aux - d, r) - 1.f, r);
+  }
+  const float d = round_to(lp - rf, r);
+  aux = d;
+  if (est == AA_KL_K1) return d;
+  return round_to(0.5f * round_to(d * d, r), r);  // pow(d, 2) is d * d on ATen CUDA
+}
+
+// d loss / d lp of a token: `acc` (the gradient that reaches lp through the other terms, accumulated first: autograd
+// runs the later-created ratio node before the KL's) plus what g_kl = d loss / d KL sends through the estimator:
+//   k1  acc + g_kl
+//   k2  acc + round(round(0.5 * g_kl) * (2 * d))                    (MulBackward, then PowBackward's grad * (2 * d))
+//   k3  (acc + g_kl) - round(g_kl * e)                              (the linear term first, then ExpBackward)
+__device__ __forceinline__ float kl_grad(float acc, float g_kl, int est, float aux, int r) {
+  if (est == AA_KL_K3) return round_to(round_to(acc + g_kl, r) - round_to(g_kl * aux, r), r);
+  if (est == AA_KL_K1) return round_to(acc + g_kl, r);
+  return round_to(acc + round_to(round_to(0.5f * g_kl, r) * (2.f * aux), r), r);
+}
+
 // ---- GRPO (trainers/text_to_text/grpo.py:290-312) ---------------------------------------------------------
 // One token of  -(exp(lp - lp.detach()) * A - beta * KL),  KL = exp(ref - lp) - (ref - lp) - 1 (k3 estimator), with the
 // reference's rounding points when lp is 16-bit (`r`).  g_t = 1 / (number of counted tokens): d loss / d per-token loss.
@@ -125,24 +157,19 @@ __device__ __forceinline__ float grpo_agg_coeff(int agg, float total, float cnt,
 // policy log-prob, and the k3 KL of grpo_token.  g_t: d loss / d per-token loss (grpo_agg_coeff).  The advantage is
 // fp32, so s and the per-token loss are fp32 (actor_token's promoted and `c * A` roundings are fp32); `r` rounds what
 // has the log-prob dtype.  The gradient reaching lp through the ratio takes c1's place in grpo_token's accumulation
-// order (the ratio is created after the KL, as the reference creates its exp(lp - lp.detach()) term).
+// order (the ratio is created after the KL, as the reference creates its exp(lp - lp.detach()) term).  est: the KL
+// estimator (AA_KL_K3 is the reference's; kl_value / kl_grad).
 //   why: actor_token's clip-fraction bits
 __device__ __forceinline__ void grpo_obj_token(float lp, float old, float rf, float A, bool on, float g_t, float beta,
-                                               float eps_lo, float eps_hi, float dual, int r, float &ptl, float &grad,
-                                               int &why) {
-  float s, ga;
+                                               float eps_lo, float eps_hi, float dual, int est, int r, float &ptl,
+                                               float &grad, int &why) {
+  float s, ga, aux;
   actor_token(lp, old, A, on, -g_t, eps_lo, eps_hi, dual, r, AA_F32, AA_F32, s, ga, why);
-  const float d = round_to(rf - lp, r);
-  const float e = round_to(expf(d), r);
-  const float kl = round_to(round_to(e - d, r) - 1.f, r);
+  const float kl = kl_value(lp, rf, est, r, aux);
   const float bk = round_to(beta * kl, r);
   ptl = -(s - bk);
   grad = 0.f;
-  if (on) {
-    const float g_kl = round_to(round_to(g_t, r) * beta, r);
-    const float c2 = -round_to(g_kl * e, r);
-    grad = round_to(round_to(ga + g_kl, r) + c2, r);
-  }
+  if (on) grad = kl_grad(ga, round_to(round_to(g_t, r) * beta, r), est, aux, r);
 }
 
 // pass 1: first eos per row (-> row_end[b] = number of counted tokens) and the global token count

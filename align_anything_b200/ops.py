@@ -1276,7 +1276,7 @@ class _GrpoLossFn(torch.autograd.Function):
 def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
                       scratch=None):
     """GRPO's loss kernel, writing loss, row_end and (unless None) grad.  obj None: the reference loss (aa_grpo_loss);
-    otherwise obj = GrpoObjective.args() for aa_grpo_loss_obj, old = the old log-probs (None: the log-probs
+    otherwise obj = _grpo_objective_args(...) for aa_grpo_loss_obj (aa_grpo_loss_kl unless the KL is k3), old = the old log-probs (None: the log-probs
     themselves, ratio 1) and clip_frac = an fp32[2] tensor for the clip fractions or None.  scratch (fp32): the token
     count and the row sums, B + 1 values, and under the objective the rows' clip counts too, 1 + 4 B; None allocates it."""
     B, K = lp.shape
@@ -1290,18 +1290,22 @@ def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old
     tail = (row_end.data_ptr(), scratch.data_ptr(), _device_scratch(dev)['counter'][5:7].data_ptr(), L.stream_ptr(dev))
     if obj is None:
         L.check(lib.aa_grpo_loss(*lps, *rows, mode_code, *out, *tail))
+    elif obj[4] == KL_ESTIMATORS['k3']:
+        L.check(lib.aa_grpo_loss_obj(*lps, L.ptr(old), old.stride(0) if old is not None else 0, *rows, *obj[:4],
+                                     mode_code, *out, L.ptr(clip_frac), *tail))
     else:
-        L.check(lib.aa_grpo_loss_obj(*lps, L.ptr(old), old.stride(0) if old is not None else 0, *rows, *obj, mode_code,
-                                     *out, L.ptr(clip_frac), *tail))
+        L.check(lib.aa_grpo_loss_kl(*lps, L.ptr(old), old.stride(0) if old is not None else 0, *rows, *obj, mode_code,
+                                    *out, L.ptr(clip_frac), *tail))
 
 
 def _grpo_objective_args(objective, old, return_clip_fraction: bool):
     """The one rule for GRPO's reference loss -- no objective or one with default fields, no old log-probs and no clip
-    fractions: None, and the nodes run today's launches.  Otherwise GrpoObjective.args() for the objective kernels
-    (a default objective still gives its clip_range_ratio)."""
+    fractions: None, and the nodes run today's launches.  Otherwise GrpoObjective.args() and the KL estimator's code
+    for the objective kernels (a default objective still gives its clip_range_ratio)."""
     if _objective(objective, GrpoObjective) is None and old is None and not return_clip_fraction:
         return None
-    return (objective or GrpoObjective()).args()
+    objective = objective or GrpoObjective()
+    return objective.args() + (KL_ESTIMATORS[objective.kl_estimator],)
 
 
 def _old_log_probs(old, shape, dtype):
@@ -1415,9 +1419,12 @@ def _k1f_grpo_launch(logits, labels, plan, lp, ref_lp, adv, tokens, eos_id, beta
     mid = (adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), K, float(beta))
     tail = (mode_code, grad.data_ptr(), logits.size(-1), rows.data_ptr(), row_end.data_ptr(), total.data_ptr(),
             sc['counter'][5:6].data_ptr(), sc['status'].data_ptr())
-    if obj is not None:
-        L.check(lib.aa_logprob_grpo_fused_obj(*head, L.ptr(old), *mid, *obj, *tail, L.ptr(entropy),
+    if obj is not None and obj[4] == KL_ESTIMATORS['k3']:
+        L.check(lib.aa_logprob_grpo_fused_obj(*head, L.ptr(old), *mid, *obj[:4], *tail, L.ptr(entropy),
                                               float(entropy_coeff), L.stream_ptr(dev)))
+    elif obj is not None:  # another KL estimator: the same kernel with the estimator's code
+        L.check(lib.aa_logprob_grpo_fused_kl(*head, L.ptr(old), *mid, *obj, *tail, L.ptr(entropy),
+                                             float(entropy_coeff), L.stream_ptr(dev)))
     elif entropy is None:
         L.check(lib.aa_logprob_grpo_fused(*head, *mid, *tail, L.stream_ptr(dev)))
     elif entropy_coeff == 0.0:  # the same launch with the entropy of every completion row from its (max, sum-exp) pass
@@ -1974,11 +1981,29 @@ def _promote(a: torch.dtype, b: torch.dtype) -> torch.dtype:
     return a if a == b else torch.float32
 
 
+# the per-token KL estimators of the PPO reward penalty and of GRPO's loss (include/aa_b200.h AA_KL_*), d = lp - ref:
+#   k1  lp - ref ;  k2  0.5 * (lp - ref) ** 2 ;  k3  exp(ref - lp) - (ref - lp) - 1  (eager ops in this order)
+KL_ESTIMATORS = {'k1': 0, 'k2': 1, 'k3': 2}
+
+
+def kl_estimator_code(name: str) -> int:
+    """The AA_KL_* code of an estimator name; anything else is refused here, before a launch."""
+    if name not in KL_ESTIMATORS:
+        raise ValueError(f'kl_estimator must be one of {sorted(KL_ESTIMATORS)}, got {name!r}')
+    return KL_ESTIMATORS[name]
+
+
 def kl_rewards_and_gae(reward, log_probs, ref_log_probs, values, sequence_mask, start: int, kl_coeff: float,
-                       clip_range_score: float, gamma: float, gae_lambda: float, mode: str | None = None):
+                       clip_range_score: float, gamma: float, gae_lambda: float, mode: str | None = None,
+                       kl_estimator: str = 'k1'):
     """add_kl_divergence_regularization (trainers/text_to_text/ppo.py:528-547) +
     get_advantages_and_returns (:487-508) in ONE launch (K4).  Returns
-    (old_rewards (B, W), advantages (B, W-start), returns (B, W-start), row_stats (B, 8) fp32)."""
+    (old_rewards (B, W), advantages (B, W-start), returns (B, W-start), row_stats (B, 8) fp32).
+    kl_estimator ('k1', the reference's, or 'k2' / 'k3', see KL_ESTIMATORS): the estimate the penalty
+    -kl_coeff * KL is formed from (aa_ppo_prep_kl); row_stats[:, 0] stays the k1 row sum behind train/kl_divergence."""
+    est = kl_estimator_code(kl_estimator)
+    if est != KL_ESTIMATORS['k1'] and not math.isfinite(float(kl_coeff)):
+        raise ValueError(f'kl_coeff must be finite, got {kl_coeff!r}')
     L.require_cuda(reward, log_probs, ref_log_probs, values, sequence_mask)
     if log_probs.dim() != 2:
         raise ValueError('log_probs must be (B, W)')
@@ -2008,12 +2033,15 @@ def kl_rewards_and_gae(reward, log_probs, ref_log_probs, values, sequence_mask, 
     ret = torch.empty((B, W - start), dtype=adv_dtype, device=dev)
     row_stats = torch.empty((B, 8), dtype=torch.float32, device=dev)
     sc = _device_scratch(dev)
-    L.check(L.lib().aa_ppo_prep(
-        lp.data_ptr(), rlp.data_ptr(), L.dtype_code(lp.dtype), lp.stride(0), rew.data_ptr(), vals.data_ptr(),
-        L.dtype_code(vals.dtype), vals.stride(0), mask.data_ptr(), mask.stride(0), B, W, int(start),
-        float(kl_coeff), float(clip_range_score), float(gamma), float(gae_lambda), mode_code,
-        old_rewards.data_ptr(), L.dtype_code(rew_dtype), adv.data_ptr(), ret.data_ptr(), L.dtype_code(adv_dtype),
-        row_stats.data_ptr(), sc['status'].data_ptr(), L.stream_ptr(dev)))
+    head = (lp.data_ptr(), rlp.data_ptr(), L.dtype_code(lp.dtype), lp.stride(0), rew.data_ptr(), vals.data_ptr(),
+            L.dtype_code(vals.dtype), vals.stride(0), mask.data_ptr(), mask.stride(0), B, W, int(start), float(kl_coeff))
+    tail = (float(clip_range_score), float(gamma), float(gae_lambda), mode_code, old_rewards.data_ptr(),
+            L.dtype_code(rew_dtype), adv.data_ptr(), ret.data_ptr(), L.dtype_code(adv_dtype), row_stats.data_ptr(),
+            sc['status'].data_ptr(), L.stream_ptr(dev))
+    if est == KL_ESTIMATORS['k1']:
+        L.check(L.lib().aa_ppo_prep(*head, *tail))
+    else:
+        L.check(L.lib().aa_ppo_prep_kl(*head, est, *tail))
     return old_rewards, adv, ret, row_stats
 
 
@@ -2162,27 +2190,30 @@ class GrpoObjective(ActorObjective):
     Dr. GRPO's aggregation), the fields and checks of ActorObjective with GRPO's defaults:
 
         ratio = exp(lp - old_lp) ;  s = min(A * ratio, A * clamp(ratio, 1 - low, 1 + high))
-        dual-clip:  s = where(A < 0, max(s, dual_clip_ratio * A), s) ;  per-token loss = -(s - beta * KL_k3)
+        dual-clip:  s = where(A < 0, max(s, dual_clip_ratio * A), s) ;  per-token loss = -(s - beta * KL)
         loss = (ptl * mask).sum() / mask.sum()                      ('token-mean', the default: the reference's loss)
              = ((ptl * mask).sum(-1) / mask.sum(-1)).mean()         ('seq-mean-token-mean')
              = (ptl * mask).sum() / (B * K)                         ('seq-mean-token-sum-norm', K = logits_to_keep)
 
     clip_range_ratio: the ε of both bounds when clip_range_ratio_low / _high are None.  With old_lp = lp (the first
-    update of a rollout) the ratio is 1 and nothing is clipped.  Checked on the host when constructed."""
+    update of a rollout) the ratio is 1 and nothing is clipped.  kl_estimator: the per-token KL ('k3', the reference's,
+    or 'k1' / 'k2': KL_ESTIMATORS).  Checked on the host when constructed."""
 
     loss_agg_mode: str = 'token-mean'
     clip_range_ratio: float = 0.2
+    kl_estimator: str = 'k3'
     _MODES = GRPO_LOSS_AGG_MODES
 
     def __post_init__(self):
         super().__post_init__()
         self.args()  # the clip range with clip_range_ratio filled in
+        kl_estimator_code(self.kl_estimator)
 
     @property
     def is_default(self) -> bool:
         """The reference's loss when the ratio is 1: the kernels run today's launches."""
         return (self.clip_range_ratio_low is None and self.clip_range_ratio_high is None and self.dual_clip_ratio is None
-                and self.loss_agg_mode == 'token-mean')
+                and self.loss_agg_mode == 'token-mean' and self.kl_estimator == 'k3')
 
     def args(self, clip_range_ratio: float | None = None) -> tuple[float, float, float, int]:
         return super().args(self.clip_range_ratio if clip_range_ratio is None else clip_range_ratio)

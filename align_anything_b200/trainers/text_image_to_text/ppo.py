@@ -15,7 +15,7 @@ import torch
 
 from ... import ops
 from ..text_to_text.ppo import PPOTrainer as _TextPPOTrainer
-from ..text_to_text.ppo import actor_loss_node, ppo_metrics
+from ..text_to_text.ppo import actor_loss_node, kl_rewards, ppo_metrics
 
 __all__ = ['PPOTrainer', 'move_padding_left']
 
@@ -153,9 +153,8 @@ class PPOTrainer(_TextPPOTrainer):
         input_ids = inference_batch['input_ids']
         lens = ops.as_device_lens(training_batch['response_lens'], input_ids.device)
 
-        old_rewards, reward_advantages, reward_returns, row_stats = ops.kl_rewards_and_gae(
-            reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, 0, self.kl_coeff,
-            self.clip_range_score, self.gamma, self.gae_lambda, mode=self.mode)
+        old_rewards, reward_advantages, reward_returns, row_stats = kl_rewards(
+            self, reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, 0)
 
         # actor: K1 over the response tails + K5 as ONE autograd node; its backward is K1b alone (:296-316)
         actor_loss, actor_loss32, entropy_mean, clip_frac = actor_loss_node(

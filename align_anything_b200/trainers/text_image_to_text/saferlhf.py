@@ -18,6 +18,7 @@ from ... import ops
 from ...utils.multi_process import all_reduce_packed
 from .ppo import PPOTrainer as _MMPPOTrainer
 from .ppo import _tail_values
+from ..text_to_text.ppo import switch_of
 
 __all__ = ['SafeRLHFVTrainer']
 
@@ -28,6 +29,16 @@ METRIC_KEYS = (
     'train/cost_critic_loss', 'train/cost', 'train/cost_with_kl_penalty', 'train/cost_advantage', 'train/cost_return',
     'train/cost_value',
 )
+
+
+def refuse_kl_switches(tr) -> None:
+    """Safe RLHF-V keeps the reference's KL: its kl_coeff shapes rewards and costs together (k1, fixed).  The KL
+    switches it inherits from the PPO trainers (all four, kl_horizon included: it only means something with kl_target)
+    raise here, before anything runs, when set to another value."""
+    for name, default in (('kl_estimator', 'k1'), ('kl_target', None), ('kl_horizon', 10000), ('kl_loss_coeff', 0)):
+        v = switch_of(tr, name)
+        if v is not None and v != default:
+            raise ValueError(f'{name}={v!r}: Safe RLHF-V keeps the reference KL penalty (k1, a fixed kl_coeff)')
 
 
 class SafeRLHFVTrainer(_MMPPOTrainer):
@@ -56,6 +67,7 @@ class SafeRLHFVTrainer(_MMPPOTrainer):
 
     # ---- saferlhf.py:453-481 ---------------------------------------------------------------------------
     def add_kl_divergence_regularization_with_cost(self, reward, cost, log_probs, ref_log_probs, sequence_mask):
+        refuse_kl_switches(self)
         zeros = torch.zeros_like(log_probs)
         rewards = ops.kl_rewards_and_gae(reward, log_probs, ref_log_probs, zeros, sequence_mask, 0, self.kl_coeff,
                                          self.clip_range_score, self.gamma, self.gae_lambda, mode=self.mode)[0]
@@ -93,6 +105,7 @@ class SafeRLHFVTrainer(_MMPPOTrainer):
 
     # ---- saferlhf.py:483-675 ---------------------------------------------------------------------------
     def rl_step(self, inference_batch, training_batch) -> dict[str, Any]:
+        refuse_kl_switches(self)
         self._lambda_step()
         lens = ops.as_device_lens(training_batch['response_lens'], training_batch['log_probs'].device)
         old_log_probs = training_batch['log_probs']

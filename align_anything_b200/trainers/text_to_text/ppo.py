@@ -12,6 +12,7 @@ in the reference; the methods below read the same attributes from `self`:
 from __future__ import annotations
 
 import copy
+import math
 from typing import Any
 
 import torch
@@ -54,6 +55,53 @@ def switch_of(tr, name: str):
 def entropy_coeff_of(tr) -> float:
     """The entropy-bonus coefficient in effect (switch_of `entropy_coeff`)."""
     return float(switch_of(tr, 'entropy_coeff'))
+
+
+def kl_estimator_of(tr) -> str:
+    """The KL estimator of the reward penalty in effect (switch_of `kl_estimator`; None: 'k1', the reference's)."""
+    name = switch_of(tr, 'kl_estimator') or 'k1'
+    ops.kl_estimator_code(name)
+    return name
+
+
+def kl_controller_of(tr) -> tuple[float, float] | None:
+    """(kl_target, kl_horizon) of the adaptive KL coefficient in effect, or None when `kl_target` is unset (a fixed
+    kl_coeff, the reference's).  Both, and kl_coeff, must be finite and > 0; anything else raises ValueError here."""
+    target = switch_of(tr, 'kl_target')
+    if target is None:
+        return None
+    horizon = switch_of(tr, 'kl_horizon')
+    for name, v in (('kl_target', target), ('kl_horizon', horizon), ('kl_coeff', tr.kl_coeff)):
+        if isinstance(v, bool) or not isinstance(v, (int, float)) or not (math.isfinite(v) and v > 0):
+            raise ValueError(f'the adaptive KL coefficient needs a finite {name} > 0, got {v!r}')
+    return float(target), float(horizon)
+
+
+def adaptive_kl_coeff(kl_coeff: float, kl: float, n: int, target: float, horizon: float) -> float:
+    """One update of the adaptive KL controller (Ziegler et al. 2019, TRL's AdaptiveKLController):
+    e = clip(kl / target - 1, -0.2, 0.2), kl_coeff * (1 + e * n / horizon); n = samples in the step."""
+    e = min(max(kl / target - 1.0, -0.2), 0.2)
+    return kl_coeff * (1.0 + e * n / horizon)
+
+
+def refuse_kl_loss_term(tr) -> None:
+    """The KL term in the actor loss (`kl_loss_coeff`) is not implemented: K5 and K1f's actor node do not read the
+    reference log-probs.  A non-zero value raises ValueError here, before anything runs, instead of being ignored."""
+    c = switch_of(tr, 'kl_loss_coeff')
+    if c is not None and c != 0:
+        raise ValueError(f'kl_loss_coeff={c!r}: the KL term in the PPO actor loss is not supported; the KL enters '
+                         f'through the reward penalty only (kl_coeff, kl_estimator, kl_target)')
+
+
+def kl_rewards(tr, reward, log_probs, ref_log_probs, values, sequence_mask, start):
+    """K4 of an rl_step under the trainer's KL switches: the KL-shaped rewards, GAE and the metric row sums
+    (ops.kl_rewards_and_gae with kl_estimator_of(tr); checks the KL switches before the launch)."""
+    refuse_kl_loss_term(tr)
+    kl_controller_of(tr)
+    est = kl_estimator_of(tr)
+    return ops.kl_rewards_and_gae(reward, log_probs, ref_log_probs, values, sequence_mask, start, tr.kl_coeff,
+                                  tr.clip_range_score, tr.gamma, tr.gae_lambda, mode=tr.mode,
+                                  **({} if est == 'k1' else {'kl_estimator': est}))
 
 
 OBJECTIVE_KEYS = ('clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode')
@@ -139,7 +187,9 @@ def ppo_metrics(tr, row_stats, reward, value_row_mean, actor_loss, critic_loss, 
       * `clip_frac`, K5's clip fraction (train/actor_clip_fraction) and with dual-clip its dual-clip fraction
         (train/actor_dual_clip_fraction).
     Sets `tr.last_rl_tensors = tensors` (per-token tensors stay out of the dict: the reference hands it to Logger.log,
-    which takes scalars only)."""
+    which takes scalars only).  With `kl_target` set (kl_controller_of) the step's train/kl_coeff goes into the dict and
+    tr.kl_coeff takes the adaptive controller's update from the step's (all-reduced) train/kl_divergence and its
+    sample count over all ranks: every rank computes the same coefficient, from the values already read here."""
     with torch.no_grad():
         # an optional lane is filled in before the one packed all-reduce, so the NVLink reduction fused into
         # ppo_pack_metrics (which reduces the vector as it writes it) gives way to all_reduce_packed
@@ -166,6 +216,13 @@ def ppo_metrics(tr, row_stats, reward, value_row_mean, actor_loss, critic_loss, 
     ops.raise_for_status(v[10], stats.device)  # the device status word (MAX over ranks): raise like the reference
     out = dict(zip(METRIC_KEYS, v[:10]))
     out.update(zip(lanes, v[first:]))
+    controller = kl_controller_of(tr)
+    if controller is not None:
+        ranks = torch.distributed.get_world_size() if torch.distributed.is_available() and \
+            torch.distributed.is_initialized() else 1
+        out['train/kl_coeff'] = float(tr.kl_coeff)
+        tr.kl_coeff = adaptive_kl_coeff(float(tr.kl_coeff), out['train/kl_divergence'], row_stats.size(0) * ranks,
+                                        *controller)
     out['train/actor_lr'] = tr.actor_model.optimizer.param_groups[0]['lr']
     out['train/reward_critic_lr'] = tr.reward_critic_model.optimizer.param_groups[0]['lr']
     tr.last_rl_tensors = tensors
@@ -198,9 +255,20 @@ class PPOTrainer:
     # Opt-in: train/actor_clip_fraction (and train/actor_dual_clip_fraction with dual-clip) from K5, reduced in the
     # step's one packed all-reduce
     log_clip_fraction = False
+    # The KL penalty of the rewards, -kl_coeff * KL per token.  kl_estimator: 'k1' (lp - ref, the reference's; None),
+    # 'k2' (0.5 * (lp - ref) ** 2) or 'k3' (exp(ref - lp) - (ref - lp) - 1); train/kl_divergence stays the k1 sum.
+    # kl_target (None = a fixed kl_coeff): the adaptive KL coefficient of Ziegler et al. (2019), updated after every
+    # rl_step from train/kl_divergence with horizon kl_horizon (adaptive_kl_coeff); train/kl_coeff reports the
+    # coefficient each step used.  `cfgs.train_cfgs.<key>` overrides each when set.  kl_loss_coeff (a KL term in the
+    # actor loss) is not implemented: anything but 0 raises before the step runs (refuse_kl_loss_term).
+    kl_estimator = None
+    kl_target = None
+    kl_horizon = 10000
+    kl_loss_coeff = 0.0
     # the class attributes above that the grafted methods read: patch.install() copies them onto the reference's classes
     SWITCHES = ('mode', 'fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'clip_range_ratio_low',
-                'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode', 'log_clip_fraction')
+                'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode', 'log_clip_fraction', 'kl_estimator',
+                'kl_target', 'kl_horizon', 'kl_loss_coeff')
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, reward_model=None,
                  reward_critic_model=None, tokenizer=None, reward_tokenizer=None, *, kl_coeff=0.02,
@@ -242,9 +310,7 @@ class PPOTrainer:
         """trainers/text_to_text/ppo.py:528-547 (K4; rl_step below fuses it with the GAE scan)."""
         W = log_probs.size(-1)
         dummy = torch.zeros((log_probs.size(0), W), dtype=torch.float32, device=log_probs.device)
-        old_rewards, _, _, _ = ops.kl_rewards_and_gae(
-            reward, log_probs, ref_log_probs, dummy, sequence_mask, W - 1, self.kl_coeff, self.clip_range_score,
-            self.gamma, self.gae_lambda, mode=self.mode)
+        old_rewards, _, _, _ = kl_rewards(self, reward, log_probs, ref_log_probs, dummy, sequence_mask, W - 1)
         return old_rewards
 
     def get_advantages_and_returns(self, values, rewards, sequence_mask, start):
@@ -367,9 +433,8 @@ class PPOTrainer:
         sequence_mask = inference_batch['attention_mask'][:, 1:]
         head = lm_head_of(self.actor_model) if self.fused_lm_head else None  # refusals before any launch
 
-        old_rewards, reward_advantages, reward_returns, row_stats = ops.kl_rewards_and_gae(
-            reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, start, self.kl_coeff,
-            self.clip_range_score, self.gamma, self.gae_lambda, mode=self.mode)
+        old_rewards, reward_advantages, reward_returns, row_stats = kl_rewards(
+            self, reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, start)
         if returns is not None:
             reward_advantages, reward_returns = returns(old_rewards, sequence_mask, start, row_stats)
 

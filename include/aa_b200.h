@@ -8,7 +8,7 @@
  * function(s) whose arithmetic it replaces (file:line relative to the reference's
  * align_anything/ directory); the Python mirror in align_anything_b200/ keeps the
  * reference's names and signatures and calls these through ctypes (INTEGRATION.md).
- * 55 entry points, ABI version 3.
+ * 58 entry points, ABI version 3.
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
@@ -365,6 +365,19 @@ int aa_ppo_prep(const void *log_probs, const void *ref_log_probs, int lp_dtype, 
                 float kl_coeff, float clip_range_score, float gamma, float gae_lambda, int mode,
                 void *old_rewards, int rew_dtype, void *advantages, void *returns, int adv_dtype,
                 float *row_stats, int32_t *status, void *stream);
+/* KL estimators of the per-token penalty (aa_ppo_prep_kl) and of GRPO's per-token loss (aa_grpo_loss_kl,
+ * aa_logprob_grpo_fused_kl), with d = lp - ref:  K1 d ;  K2 0.5 * d^2 ;  K3 exp(-d) + d - 1 (each op rounded as the
+ * eager expression in ops.KL_ESTIMATORS rounds it). */
+enum { AA_KL_K1 = 0, AA_KL_K2 = 1, AA_KL_K3 = 2 };
+/* aa_ppo_prep with the penalty reward -kl_coeff * KL taken by `kl_estimator`; row_stats[b][0] stays the k1 row sum
+ * (the kl_divergence metric).  kl_coeff must be finite.  With AA_KL_K1 the outputs are bit-identical to aa_ppo_prep;
+ * the GAE-only form (NULL log-probs) is aa_ppo_prep's. */
+int aa_ppo_prep_kl(const void *log_probs, const void *ref_log_probs, int lp_dtype, int64_t lp_row_stride,
+                   const float *reward, const void *values, int val_dtype, int64_t val_row_stride,
+                   const uint8_t *mask, int64_t mask_row_stride, int32_t B, int32_t W, int32_t start,
+                   float kl_coeff, int kl_estimator, float clip_range_score, float gamma, float gae_lambda, int mode,
+                   void *old_rewards, int rew_dtype, void *advantages, void *returns, int adv_dtype,
+                   float *row_stats, int32_t *status, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * K4r  Multi-PPO returns, one launch: trainers/text_to_text/multi_ppo.py:510-591
@@ -565,6 +578,18 @@ int aa_logprob_grpo_fused_obj(const void *logits, int logits_dtype, int64_t row_
                               float clip_low, float clip_high, float dual_clip, int loss_agg, int mode, void *grad_logits,
                               int64_t grad_row_stride, void *row_scratch, int32_t *row_end, float *total,
                               uint32_t *counter, int32_t *status, float *entropy, float entropy_coeff, void *stream);
+/* aa_logprob_grpo_fused_obj with the per-token KL taken by `kl_estimator` (AA_KL_*): the loss value and clip fractions
+ * are then aa_grpo_loss_kl's.  With AA_KL_K3 every output is bit-identical to aa_logprob_grpo_fused_obj. */
+int aa_logprob_grpo_fused_kl(const void *logits, int logits_dtype, int64_t row_stride, int32_t V, const int64_t *labels,
+                             int32_t n_segments, const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                             const int64_t *seg_out_off, const int64_t *seg_cum, const int64_t *seg_tile_row,
+                             int64_t n_tile_rows, void *log_probs, int lp_dtype, const void *ref_log_probs,
+                             int64_t ref_stride, const void *old_log_probs, const float *advantages,
+                             const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t K, float beta,
+                             float clip_low, float clip_high, float dual_clip, int loss_agg, int kl_estimator, int mode,
+                             void *grad_logits, int64_t grad_row_stride, void *row_scratch, int32_t *row_end,
+                             float *total, uint32_t *counter, int32_t *status, float *entropy, float entropy_coeff,
+                             void *stream);
 
 /* tile[0..n) *= *scale unless *scale == 1 (checked on the device: the usual `loss.backward()` costs one empty launch).
  * Contiguous tile; scale: device scalar of scale_dtype.  The autograd backward of the K1f node. */
@@ -613,6 +638,14 @@ int aa_grpo_loss_obj(const void *log_probs, int64_t lp_stride, const void *ref_l
                      float beta, float clip_low, float clip_high, float dual_clip, int loss_agg, int mode, float *loss,
                      void *grad, int64_t grad_stride, float *clip_frac, int32_t *row_end, float *scratch,
                      uint32_t *counter, void *stream);
+/* aa_grpo_loss_obj with the per-token KL taken by `kl_estimator` (AA_KL_*, below) instead of k3; with AA_KL_K3 the
+ * outputs are bit-identical to aa_grpo_loss_obj.  An unknown estimator code is refused before any CUDA call. */
+int aa_grpo_loss_kl(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
+                    const void *old_log_probs, int64_t old_stride, int lp_dtype, const float *advantages,
+                    const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B, int32_t K,
+                    float beta, float clip_low, float clip_high, float dual_clip, int loss_agg, int kl_estimator,
+                    int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac, int32_t *row_end,
+                    float *scratch, uint32_t *counter, void *stream);
 
 /* masked_mean (utils/tools.py:460-467): mean over rows of masked row means -> out[0];
  * mask == NULL: plain mean. */
