@@ -87,6 +87,9 @@ _SIGS = {
                                   c_int32, c_float, c_int, _P, _P, c_int64, _P, _P, _P]),
     'aa_ppo_actor_loss_obj': (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, c_int32, c_int32,
                                       c_float, c_float, c_float, c_int, c_int, _P, _P, c_int64, _P, _P, _P, _P]),
+    'aa_ppo_actor_loss_kl': (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, c_int32, c_int32,
+                                     c_float, c_float, c_float, c_int, c_int, _P, c_int64, c_float, c_int, _P, _P, _P,
+                                     c_int64, _P, _P, _P, _P]),
     'aa_ppo_critic_loss': (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, c_int32,
                                    c_int32, c_float, c_int, _P, _P, c_int64, _P, _P, _P, _P, c_int32, _P]),
     'aa_logprob_actor_fused': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P, c_int, _P, _P,
@@ -98,6 +101,10 @@ _SIGS = {
     'aa_logprob_actor_fused_obj': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P, c_int,
                                            _P, _P, _P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int32, c_float, c_float,
                                            c_float, c_int, c_int, _P, c_int64, _P, _P, c_float, _P, _P]),
+    'aa_logprob_actor_fused_kl': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P, c_int,
+                                          _P, _P, _P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int32, c_float, c_float,
+                                          c_float, c_int, c_int, _P, c_int64, _P, _P, c_float, _P, _P, c_float, c_int,
+                                          _P]),
     'aa_logprob_ce_fused': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int64, c_int64, c_int32, _P, _P, _P, _P, _P, c_int64, _P,
                                     c_float, _P, c_int64, _P, _P, _P, _P]),
     'aa_logprob_grpo_fused': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P, c_int, _P, c_int64,

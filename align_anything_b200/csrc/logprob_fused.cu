@@ -72,7 +72,7 @@ struct FusedActorParams {
   int kind;
   const void *old_pol;
   float clip_lo;
-  int kl_est;  // kind 3: the per-token KL's estimator (AA_KL_*; aa_logprob_grpo_fused_obj: AA_KL_K3)
+  int kl_est;  // kind 3: the per-token KL's estimator (AA_KL_*; aa_logprob_grpo_fused_obj: AA_KL_K3); kind 0: the KL term's
   int64_t ignore_index;
   const float *ce_coeff;
   const int32_t *row_end;
@@ -83,6 +83,12 @@ struct FusedActorParams {
   // mask count under token-mean, written by the prep kernel) for masked-in tokens; kind 2: -ent_coeff * g_rs (= -ent_coeff / counted tokens) for counted tokens
   float ent_coeff;
   float *ent_seg;
+  // kind 0 KL loss term (aa_logprob_actor_fused_kl; kl_coeff 0 = off): the KL of the token's log-prob against
+  // ref[out_idx] (the reference log-probs laid out like `out`) by estimator kl_est adds its gradient to the token's;
+  // kl_seg[segment] = d total / d KL of a masked-in token (kl_term_coeff, written by the prep kernel)
+  const void *ref;
+  float kl_coeff;
+  float *kl_seg;
 };
 
 // One record per gradient-tile row, in the order the persistent kernel walks them.  The scored rows are bound by
@@ -118,6 +124,8 @@ __global__ void __launch_bounds__(256) fused_actor_prep_kernel(const FusedActorP
       if (blockIdx.x == 0 && tid == 0)
         p.ent_seg[seg] = -p.ent_coeff / (token_mean ? cnt : static_cast<float>(p.map.n_seg) * cnt);
     }
+    if (p.kl_coeff != 0.f && blockIdx.x == 0 && tid == 0)
+      p.kl_seg[seg] = kl_term_coeff(p.kl_coeff, p.agg, cnt, p.map.n_seg, p.rx);
   }
   if (k >= p.seq) return;
   const int64_t work = static_cast<int64_t>(seg) * p.seq + k;
@@ -449,9 +457,15 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
         }
         float obj, g = g_rs;  // cross-entropy: the same -loss_scale / n_valid for every scored row
         int why;
-        if (p.kind == 0)
-          actor_token(round_to(lp, p.out_dtype), old, adv, on, g_rs, p.clip, p.clip_hi, p.dual, p.rx, p.rp, p.ra, obj, g,
-                      why);
+        if (p.kind == 0) {
+          const float lpr = round_to(lp, p.out_dtype);
+          actor_token(lpr, old, adv, on, g_rs, p.clip, p.clip_hi, p.dual, p.rx, p.rp, p.ra, obj, g, why);
+          if (p.kl_coeff != 0.f && on) {  // the KL term: its gradient is added after the ratio's (as in K5)
+            float kaux;
+            kl_value(lpr, load_as_float(p.ref, out_idx, p.out_dtype), p.kl_est, p.rx, kaux);
+            g = kl_grad(g, __ldg(p.kl_seg + g_row / p.seq), p.kl_est, kaux, p.rx);
+          }
+        }
         if (p.kind == 2) grpo_token(round_to(lp, p.out_dtype), old, adv, on, g_rs, p.clip, p.rx, obj, g);
         if (p.kind == 3) {
           const float lpr = round_to(lp, p.out_dtype);
@@ -680,7 +694,14 @@ static inline int promote_dt(int a, int b) { return (a == b) ? a : AA_F32; }
 
 using namespace aa;
 
-// aa_logprob_actor_fused{,_entropy}: entropy == nullptr runs the plain kernels
+// the KL loss term of aa_logprob_actor_fused_kl
+struct ActorKlTerm {
+  const void *ref;
+  float coeff;
+  int est;
+};
+
+// aa_logprob_actor_fused{,_entropy,_obj,_kl}: entropy == nullptr runs the plain kernels; kl == nullptr: no KL term
 static int logprob_actor_fused(const char *who, float *entropy, float entropy_coeff, const void *logits, int logits_dtype,
                                int64_t row_stride, int32_t V, const int64_t *labels, int32_t n_segments,
                                const int64_t *seg_logit_off, const int64_t *seg_label_off, const int64_t *seg_out_off,
@@ -689,7 +710,7 @@ static int logprob_actor_fused(const char *who, float *entropy, float entropy_co
                                int64_t old_stride, const void *advantages, int64_t adv_stride, int adv_dtype,
                                const uint8_t *mask, int64_t mask_stride, int32_t W, float clip_low, float clip_high,
                                float dual_clip, int loss_agg, int mode, void *grad_logits, int64_t grad_row_stride,
-                               void *row_scratch, int32_t *status, void *stream) {
+                               void *row_scratch, int32_t *status, void *stream, const ActorKlTerm *kl = nullptr) {
   AA_REQUIRE(V > 0 && n_segments > 0 && W > 0 && n_tile_rows > 0 && n_tile_rows % n_segments == 0, AA_ERR_ARG,
              "%s: bad sizes (the gradient tile holds n_tile_rows / n_segments rows per sample)", who);
   AA_REQUIRE(logits && labels && seg_logit_off && seg_label_off && seg_out_off && seg_cum && seg_tile_row && log_probs &&
@@ -731,6 +752,12 @@ static int logprob_actor_fused(const char *who, float *entropy, float entropy_co
     p.entropy = entropy;
     p.ent_coeff = entropy_coeff;
     p.ent_seg = reinterpret_cast<float *>(rec + n_tile_rows);
+  }
+  if (kl) {
+    p.ref = kl->ref;
+    p.kl_coeff = kl->coeff;
+    p.kl_est = kl->est;
+    p.kl_seg = reinterpret_cast<float *>(rec + n_tile_rows) + n_segments;
   }
   return launch_fused(p, logits_dtype, mode, rec, n_tile_rows, static_cast<cudaStream_t>(stream), entropy != nullptr);
 }
@@ -788,6 +815,35 @@ extern "C" int aa_logprob_actor_fused_obj(const void *logits, int logits_dtype, 
                              n_tile_rows, log_probs, lp_dtype, stat_max, stat_logsum, old_log_probs, old_stride,
                              advantages, adv_stride, adv_dtype, mask, mask_stride, W, clip_low, clip_high, dual_clip,
                              loss_agg, mode, grad_logits, grad_row_stride, row_scratch, status, stream);
+}
+
+extern "C" int aa_logprob_actor_fused_kl(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                         const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                         const int64_t *seg_label_off, const int64_t *seg_out_off,
+                                         const int64_t *seg_cum, const int64_t *seg_tile_row, int64_t n_tile_rows,
+                                         void *log_probs, int lp_dtype, float *stat_max, float *stat_logsum,
+                                         const void *old_log_probs, int64_t old_stride, const void *advantages,
+                                         int64_t adv_stride, int adv_dtype, const uint8_t *mask, int64_t mask_stride,
+                                         int32_t W, float clip_low, float clip_high, float dual_clip, int loss_agg,
+                                         int mode, void *grad_logits, int64_t grad_row_stride, void *row_scratch,
+                                         int32_t *status, float entropy_coeff, float *entropy,
+                                         const void *ref_log_probs, float kl_loss_coeff, int kl_estimator,
+                                         void *stream) {
+  AA_REQUIRE(actor_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
+             "aa_logprob_actor_fused_kl: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a "
+             "known loss_agg; got %g %g %g %d)", clip_low, clip_high, dual_clip, loss_agg);
+  AA_REQUIRE(entropy_coeff == entropy_coeff, AA_ERR_ARG, "aa_logprob_actor_fused_kl: entropy_coeff is NaN");
+  AA_REQUIRE(kl_estimator_ok(kl_estimator), AA_ERR_ARG, "aa_logprob_actor_fused_kl: unknown kl_estimator code %d",
+             kl_estimator);
+  AA_REQUIRE(kl_loss_term_ok(kl_loss_coeff), AA_ERR_ARG,
+             "aa_logprob_actor_fused_kl: kl_loss_coeff must be finite and > 0 (got %g)", kl_loss_coeff);
+  AA_REQUIRE(ref_log_probs, AA_ERR_ARG, "aa_logprob_actor_fused_kl: null ref_log_probs");
+  const ActorKlTerm kl{ref_log_probs, kl_loss_coeff, kl_estimator};
+  return logprob_actor_fused("aa_logprob_actor_fused_kl", entropy, entropy_coeff, logits, logits_dtype, row_stride, V,
+                             labels, n_segments, seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row,
+                             n_tile_rows, log_probs, lp_dtype, stat_max, stat_logsum, old_log_probs, old_stride,
+                             advantages, adv_stride, adv_dtype, mask, mask_stride, W, clip_low, clip_high, dual_clip,
+                             loss_agg, mode, grad_logits, grad_row_stride, row_scratch, status, stream, &kl);
 }
 
 extern "C" int aa_logprob_ce_fused(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,

@@ -388,6 +388,13 @@ struct LossParams {
   float clip_hi, dual;
   int r_a, agg;
   float *clip_frac;  // optional fp32[2]: clipped fraction, dual-clip fraction (row_scratch then holds 4 * B floats)
+  // KL loss term (aa_ppo_actor_loss_kl; kl_coeff 0 = off): grad is d (loss + kl_coeff * agg(KL)) / d x, with the KL
+  // of x against `ref` (x's dtype) by estimator kl_est; kl_loss[0] = agg(KL); row_scratch then holds 5 * B floats
+  const void *ref;
+  int64_t ref_stride;
+  float kl_coeff;
+  int kl_est;
+  float *kl_loss;
 };
 
 template <int THREADS, bool ACTOR>
@@ -416,8 +423,10 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
   const float cnt_p = round_to(cnt, rp), total_p = round_to(total, rp);
   const float g_rs = ACTOR ? (token_mean ? actor_token_mean_coeff(total, rp) : actor_row_coeff(cnt, p.B, rp))
                            : round_to(round_to(round_to(0.5f, rp) / static_cast<float>(p.B), rp) / cnt_p, rp);
+  const bool kl_on = ACTOR && p.kl_coeff != 0.f;
+  const float g_kl = kl_on ? kl_term_coeff(p.kl_coeff, p.agg, token_mean ? total : cnt, p.B, rx) : 0.f;
 
-  float row_sum = 0.f, x_sum = 0.f;
+  float row_sum = 0.f, x_sum = 0.f, kl_sum = 0.f;
   float n_clip = 0.f, n_dual = 0.f, n_neg = 0.f;  // clip-fraction counters of the row's masked-in tokens
   for (int t = tid; t < Wm; t += THREADS) {
     const bool on = mrow[t] != 0;
@@ -432,6 +441,11 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
         n_clip += (why & 1) ? 1.f : 0.f;
         n_dual += (why & 2) ? 1.f : 0.f;
         n_neg += (aux < 0.f) ? 1.f : 0.f;
+      }
+      if (kl_on && on) {  // the KL is created before the ratio: its gradient is added after the ratio's
+        float kaux;
+        kl_sum += kl_value(x, load_as_float(p.ref, b * p.ref_stride + t, p.x_dtype), p.kl_est, rx, kaux);
+        grad = kl_grad(grad, g_kl, p.kl_est, kaux, rx);
       }
     } else {
       const float lo = round_to(old - p.clip, rx), hi = round_to(old + p.clip, rx);
@@ -467,10 +481,12 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
     n_dual = block_sum<THREADS>(n_dual, scratch);
     n_neg = block_sum<THREADS>(n_neg, scratch);
   }
+  if (kl_on) kl_sum = block_sum<THREADS>(kl_sum, scratch);
   if (tid == 0) {
     // seq-mean-token-mean: the row's masked mean in the promoted dtype; token-mean: the row's fp32 sum (rounded once,
-    // after the cross-row sum, as ATen's sum over the whole tensor does)
+    // after the cross-row sum, as ATen's sum over the whole tensor does).  The KL's rows alike, in the log-probs' dtype
     p.row_scratch[b] = token_mean ? row_sum : round_to(round_to(row_sum, rp) / cnt_p, rp);
+    if (kl_on) p.row_scratch[4 * p.B + b] = token_mean ? kl_sum : round_to(round_to(kl_sum, rx) / round_to(cnt, rx), rx);
     if (p.row_mean) p.row_mean[b] = x_sum / cnt;
     if (fracs) {  // the counters reduced like the loss: per-row fractions (seq-mean) or raw counts (token-mean)
       const float d = token_mean ? 1.f : cnt;
@@ -500,6 +516,14 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
       p.clip_frac[0] = fc / (token_mean ? total : static_cast<float>(p.B));
       p.clip_frac[1] = fn > 0.f ? fd / fn : 0.f;
     }
+  }
+  if (kl_on) {
+    float ak = 0.f;
+    for (int k = tid; k < p.B; k += THREADS) ak += rows[4 * p.B + k];
+    ak = block_sum<THREADS>(ak, scratch);
+    if (tid == 0)
+      p.kl_loss[0] = token_mean ? round_to(round_to(ak, rx) / round_to(total, rx), rx)
+                                : round_to(ak / static_cast<float>(p.B), rx);
   }
   if (tid == 0) {
     const float mm = token_mean ? round_to(round_to(acc, rp) / total_p, rp) : round_to(acc / static_cast<float>(p.B), rp);
@@ -879,7 +903,9 @@ static int ppo_actor_loss(const char *who, const void *log_probs, int64_t lp_str
                           int64_t old_stride, int lp_dtype, const void *advantages, int64_t adv_stride, int adv_dtype,
                           const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t Wm, float clip_low,
                           float clip_high, float dual_clip, int loss_agg, int mode, float *loss, void *grad,
-                          int64_t grad_stride, float *clip_frac, float *row_scratch, uint32_t *counter, void *stream) {
+                          int64_t grad_stride, float *clip_frac, float *row_scratch, uint32_t *counter, void *stream,
+                          const void *ref = nullptr, int64_t ref_stride = 0, float kl_coeff = 0.f, int kl_est = 0,
+                          float *kl_loss = nullptr) {
   AA_REQUIRE(B > 0 && Wm > 0, AA_ERR_ARG, "%s: bad sizes", who);
   AA_REQUIRE(log_probs && old_log_probs && advantages && mask && loss && row_scratch && counter, AA_ERR_ARG,
              "%s: null pointer", who);
@@ -888,7 +914,8 @@ static int ppo_actor_loss(const char *who, const void *log_probs, int64_t lp_str
   LossParams p{log_probs, lp_stride, old_log_probs, old_stride, lp_dtype, advantages, adv_stride, adv_dtype,
                mask, mask_stride, B, Wm, clip_low, f ? lp_dtype : AA_F32,
                f ? promote(lp_dtype, adv_dtype) : AA_F32, loss, grad, grad_stride, nullptr, row_scratch, counter, nullptr, 0,
-               clip_high, dual_clip, f ? adv_dtype : AA_F32, loss_agg, clip_frac};
+               clip_high, dual_clip, f ? adv_dtype : AA_F32, loss_agg, clip_frac, ref, ref_stride, kl_coeff, kl_est,
+               kl_loss};
   ppo_loss_kernel<128, true><<<B, 128, 0, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch(who);
 }
@@ -916,6 +943,28 @@ extern "C" int aa_ppo_actor_loss_obj(const void *log_probs, int64_t lp_stride, c
   return ppo_actor_loss("aa_ppo_actor_loss_obj", log_probs, lp_stride, old_log_probs, old_stride, lp_dtype, advantages,
                         adv_stride, adv_dtype, mask, mask_stride, B, Wm, clip_low, clip_high, dual_clip, loss_agg, mode,
                         loss, grad, grad_stride, clip_frac, row_scratch, counter, stream);
+}
+
+extern "C" int aa_ppo_actor_loss_kl(const void *log_probs, int64_t lp_stride, const void *old_log_probs,
+                                    int64_t old_stride, int lp_dtype, const void *advantages, int64_t adv_stride,
+                                    int adv_dtype, const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t Wm,
+                                    float clip_low, float clip_high, float dual_clip, int loss_agg, int mode,
+                                    const void *ref_log_probs, int64_t ref_stride, float kl_loss_coeff, int kl_estimator,
+                                    float *loss, float *kl_loss, void *grad, int64_t grad_stride, float *clip_frac,
+                                    float *row_scratch, uint32_t *counter, void *stream) {
+  AA_REQUIRE(actor_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
+             "aa_ppo_actor_loss_kl: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a known "
+             "loss_agg; got %g %g %g %d)", clip_low, clip_high, dual_clip, loss_agg);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_ppo_actor_loss_kl: bad mode");
+  AA_REQUIRE(kl_estimator_ok(kl_estimator), AA_ERR_ARG, "aa_ppo_actor_loss_kl: unknown kl_estimator code %d",
+             kl_estimator);
+  AA_REQUIRE(kl_loss_term_ok(kl_loss_coeff), AA_ERR_ARG,
+             "aa_ppo_actor_loss_kl: kl_loss_coeff must be finite and > 0 (got %g)", kl_loss_coeff);
+  AA_REQUIRE(ref_log_probs && kl_loss, AA_ERR_ARG, "aa_ppo_actor_loss_kl: null ref_log_probs or kl_loss");
+  return ppo_actor_loss("aa_ppo_actor_loss_kl", log_probs, lp_stride, old_log_probs, old_stride, lp_dtype, advantages,
+                        adv_stride, adv_dtype, mask, mask_stride, B, Wm, clip_low, clip_high, dual_clip, loss_agg, mode,
+                        loss, grad, grad_stride, clip_frac, row_scratch, counter, stream, ref_log_probs, ref_stride,
+                        kl_loss_coeff, kl_estimator, kl_loss);
 }
 
 extern "C" int aa_ppo_critic_loss(const void *values, int64_t val_stride, const void *old_values,

@@ -23,6 +23,21 @@ __device__ __forceinline__ float actor_token_mean_coeff(float total, int rp) {
   return round_to(-1.f / round_to(total, rp), rp);
 }
 
+// d total / d KL of a masked-in token for the actor's KL loss term  kl_coeff * agg(KL, mask)  (K5 and K1f's
+// aa_*_kl entry points).  The KL has the log-probs' dtype (rounding code r), and so has every op of its chain:
+//   seq-mean-token-mean  round(round(round(c) * (1/B)) / round(count))   MulBackward by the python scalar c, then
+//                        MeanBackward (ATen CUDA multiplies by the reciprocal of a scalar divisor), then DivBackward
+//                        by the row's int64 mask count cast to r;  count = the row's masked-in tokens
+//   token-mean           round(round(c) / round(count))                  count = the micro-batch's masked-in tokens
+__device__ __forceinline__ float kl_term_coeff(float kl_coeff, int agg, float count, int B, int r) {
+  const float g = round_to(kl_coeff, r);
+  if (agg == AA_AGG_TOKEN_MEAN) return round_to(g / round_to(count, r), r);
+  return round_to(round_to(g * (1.f / static_cast<float>(B)), r) / round_to(count, r), r);
+}
+
+// the argument check of the KL loss term of the actor entry points (the trainers check the same on the host)
+inline bool kl_loss_term_ok(float kl_coeff) { return kl_coeff > 0.f && kl_coeff <= 3.402823466e38f; }
+
 // the argument check of the objective entry points (ops.ActorObjective checks the same on the host)
 inline bool actor_objective_ok(float clip_low, float clip_high, float dual_clip, int loss_agg) {
   return clip_low >= 0.f && clip_low < 1.f && clip_high >= 0.f && (dual_clip == 0.f || dual_clip > 1.f) &&

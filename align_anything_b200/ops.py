@@ -2235,11 +2235,13 @@ def token_mean(x: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
     return masked_mean(x.reshape(1, -1), mask.reshape(1, -1))
 
 
-def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=None, obj=None, clip_frac=None):
+def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=None, obj=None, clip_frac=None, kl=None):
     """K5: -> (loss fp32[2], loss as a 0-dim tensor of the promoted dtype (a view, no launch), grad (B, Wm), row_mean).
     x_tail = (DeviceLens, src_width): `x` is the raw (B, src_width) tensor and the kernel reads the per-sample tails.
     Actor only: obj = ActorObjective.args(...) (None: the reference's objective), clip_frac = an fp32[2] tensor the
-    kernel fills with the clip fractions (aa_ppo_actor_loss_obj)."""
+    kernel fills with the clip fractions (aa_ppo_actor_loss_obj); kl = _KlLossTerm: the KL loss term
+    (aa_ppo_actor_loss_kl: grad is d (loss + coeff * agg(KL)) / d x, kl.out receives agg(KL), `loss` stays the
+    clipped objective)."""
     B, Wm = old.shape
     dev = x.device
     loss = torch.empty(2, dtype=torch.float32, device=dev)
@@ -2248,7 +2250,16 @@ def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=Non
     row_mean = torch.empty(B, dtype=torch.float32, device=dev)
     sc = _device_scratch(dev)
     lib = L.lib()
-    if actor and (obj is not None or clip_frac is not None):
+    if actor and kl is not None:
+        lo, hi, dual, agg = obj if obj is not None else (clip, clip, 0.0, 0)
+        rows = torch.empty(5 * B, dtype=torch.float32, device=dev)
+        L.check(lib.aa_ppo_actor_loss_kl(
+            x.data_ptr(), x.stride(0), old.data_ptr(), old.stride(0), L.dtype_code(x.dtype), aux.data_ptr(),
+            aux.stride(0), L.dtype_code(aux.dtype), mask.data_ptr(), mask.stride(0), B, Wm, float(lo), float(hi),
+            float(dual), int(agg), mode_code, kl.ref.data_ptr(), kl.ref.stride(0), kl.coeff, kl.estimator,
+            loss.data_ptr(), kl.out.data_ptr(), grad.data_ptr(), grad.stride(0), L.ptr(clip_frac), rows.data_ptr(),
+            sc['counter'][2:3].data_ptr(), L.stream_ptr(dev)))
+    elif actor and (obj is not None or clip_frac is not None):
         lo, hi, dual, agg = obj if obj is not None else (clip, clip, 0.0, 0)
         rows = torch.empty(4 * B, dtype=torch.float32, device=dev)
         L.check(lib.aa_ppo_actor_loss_obj(
@@ -2275,30 +2286,32 @@ def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=Non
 
 
 class _PpoLossFn(torch.autograd.Function):
-    """K5: forward computes the loss AND d loss / d x in the same launch; backward scales it."""
+    """K5: forward computes the loss AND d loss / d x in the same launch; backward scales it.  With the KL loss term
+    (kl, actor only) the first output is  loss + kl.coeff * agg(KL)  (fp32) and its gradient is K5's."""
 
     @staticmethod
-    def forward(ctx, x, old, aux, mask, clip, mode_code, actor: bool, obj=None, clip_frac=None):
+    def forward(ctx, x, old, aux, mask, clip, mode_code, actor: bool, obj=None, clip_frac=None, kl=None):
         loss, cast, grad, row_mean = _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor, obj=obj,
-                                                      clip_frac=clip_frac)
+                                                      clip_frac=clip_frac, kl=kl)
         ctx.save_for_backward(grad)
         ctx.mark_non_differentiable(row_mean, loss)
-        return cast, row_mean, loss
+        return (cast if kl is None else kl.regularised(loss[0])), row_mean, loss
 
     @staticmethod
     def backward(ctx, g_loss, _g, _l):
         (grad,) = ctx.saved_tensors
-        return (grad.float() * g_loss.float()).to(grad.dtype), None, None, None, None, None, None, None, None
+        return (grad.float() * g_loss.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None
 
 
-def _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, grad, obj, coeff, ent):
+def _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, grad, obj, coeff, ent, kl=None):
     """K1f over the actor's scored rows, writing lp and the gradient tile `grad`.  obj: ActorObjective.args(...) for
     the objective entry point (aa_logprob_actor_fused_obj), None for the reference's objective -- with an entropy
-    bonus (`ent`, the fp32 entropy out) the entropy-gradient entry point, otherwise the plain one."""
+    bonus (`ent`, the fp32 entropy out) the entropy-gradient entry point, otherwise the plain one.  kl (_KlLossTerm):
+    the KL loss term's entry point (aa_logprob_actor_fused_kl), whatever the objective."""
     dev = logits.device
     # 48 bytes per tile row (the row records); the entropy-gradient and objective forms add 4 per segment (the rows'
-    # g_H coefficients)
-    extra = (plan.n_seg + 1) // 2 if obj is not None or ent is not None else 0
+    # g_H coefficients), the KL form 8 (and the rows' KL coefficients)
+    extra = plan.n_seg if kl is not None else (plan.n_seg + 1) // 2 if obj is not None or ent is not None else 0
     scratch = torch.empty(plan.n_tile_rows * 6 + extra, dtype=torch.int64, device=dev)
     p = plan.ptrs()
     lib = L.lib()
@@ -2307,7 +2320,10 @@ def _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, gr
             None, old.data_ptr(), old.stride(0), aux.data_ptr(), aux.stride(0), L.dtype_code(aux.dtype),
             mask.data_ptr(), mask.stride(0), lp.size(1))
     tail = (mode_code, grad.data_ptr(), logits.size(-1), scratch.data_ptr(), _device_scratch(dev)['status'].data_ptr())
-    if obj is not None:
+    if kl is not None:
+        L.check(lib.aa_logprob_actor_fused_kl(*head, *(obj if obj is not None else (clip, clip, 0.0, 0)), *tail, coeff,
+                                              L.ptr(ent), kl.ref.data_ptr(), kl.coeff, kl.estimator, L.stream_ptr(dev)))
+    elif obj is not None:
         L.check(lib.aa_logprob_actor_fused_obj(*head, *obj, *tail, coeff, L.ptr(ent), L.stream_ptr(dev)))
     elif ent is not None:
         L.check(lib.aa_logprob_actor_fused_entropy(*head, float(clip), *tail, coeff, ent.data_ptr(), L.stream_ptr(dev)))
@@ -2332,11 +2348,13 @@ class _TailActorLossFn(torch.autograd.Function):
     backward, K1b's entropy variant with g_H = -entropy_coeff * mask / (B * mask count of the row).
     objective (a non-default ActorObjective): K1f's objective entry point (aa_logprob_actor_fused_obj) and K5's
     (aa_ppo_actor_loss_obj); under token-mean the entropy term is a token mean too.  clip_frac: an fp32[2] tensor K5
-    fills with the clip fractions."""
+    fills with the clip fractions.  kl (_KlLossTerm): the node's loss gains  + kl.coeff * agg(KL)  (fp32; the third
+    output stays the actor loss without it), K1f's KL entry point (aa_logprob_actor_fused_kl) writes its gradient into
+    the tile, K5's (aa_ppo_actor_loss_kl) the loss value, agg(KL) into kl.out and, for K1b, d total / d log-probs."""
 
     @staticmethod
     def forward(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, single_pass, entropy_coeff=0.0, objective=None,
-                clip_frac=None):
+                clip_frac=None, kl=None):
         out_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         dev = logits.device
         coeff = float(entropy_coeff)
@@ -2348,12 +2366,13 @@ class _TailActorLossFn(torch.autograd.Function):
         ent = torch.zeros(plan.out_shape, dtype=torch.float32, device=dev) if ctx.bonus else None
         if ctx.fused:
             grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
-            _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, grad, obj, coeff, ent)
+            _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, grad, obj, coeff, ent, kl)
             ctx.save_for_backward(grad)
         else:
             stats = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=dev)
             _launch_fwd(logits, ids, plan, lp, stats[0], stats[1], entropy=ent)
-        loss, cast, grad_lp, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True, obj=obj, clip_frac=clip_frac)
+        loss, cast, grad_lp, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True, obj=obj, clip_frac=clip_frac,
+                                                  kl=kl)
         tm = objective is not None and objective.token_mean
         if not ctx.fused:
             if ctx.bonus:
@@ -2368,9 +2387,9 @@ class _TailActorLossFn(torch.autograd.Function):
             ctx.plan, ctx.mode_code = plan, mode_code
         if not ctx.bonus:
             ctx.mark_non_differentiable(lp, loss)
-            return cast, lp, loss
+            return (cast if kl is None else kl.regularised(loss[0])), lp, loss
         h_mean = token_mean(ent, mask) if tm else masked_mean(ent, mask)
-        reg = loss[0] - coeff * h_mean
+        reg = (loss[0] if kl is None else kl.regularised(loss[0])) - coeff * h_mean
         ctx.mark_non_differentiable(lp, loss, h_mean)
         return reg, lp, loss, h_mean
 
@@ -2378,7 +2397,7 @@ class _TailActorLossFn(torch.autograd.Function):
     def backward(ctx, g_loss, *_unused):
         if ctx.fused:
             (grad,) = _hand_over_once(ctx, g_loss, *ctx.saved_tensors)
-            return grad, None, None, None, None, None, None, None, None, None, None, None
+            return grad, None, None, None, None, None, None, None, None, None, None, None, None
         scale = g_loss.detach().reshape(1)
         if scale.dtype not in (torch.float32, torch.bfloat16, torch.float16):
             scale = scale.float()
@@ -2390,7 +2409,7 @@ class _TailActorLossFn(torch.autograd.Function):
         grad = torch.empty(logits.shape, dtype=logits.dtype, device=logits.device)
         _launch_bwd(logits, ids, ctx.plan, stats[0], stats[1], grad_lp, None, scale, grad, ctx.mode_code, entropy=ent,
                     grad_entropy=g_h)
-        return grad, None, None, None, None, None, None, None, None, None, None, None
+        return grad, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 class _TailCriticLossFn(torch.autograd.Function):
@@ -2435,6 +2454,46 @@ def _k5_operands(old, aux, mask, dtype):
     return old, aux, _contiguous_last(mask.to(torch.bool))
 
 
+class _KlLossTerm:
+    """The KL loss term  coeff * agg(KL(lp, ref), mask)  of an actor node: `ref` the reference log-probs, detached, in
+    the dtype the kernels read the log-probs in and contiguous (K1f reads it at each log-prob's own index), `estimator`
+    its AA_KL_* code, `out` the fp32[1] K5 writes agg(KL) into."""
+
+    def __init__(self, ref, coeff: float, estimator: int, out):
+        self.ref, self.coeff, self.estimator, self.out = ref, coeff, estimator, out
+
+    def regularised(self, loss):
+        """loss + coeff * agg(KL), fp32 (one launch)."""
+        return torch.add(loss, self.out[0], alpha=self.coeff)
+
+
+def _kl_loss_args(ref_log_probs, old_log_probs, kl_loss_coeff, kl_loss_estimator) -> tuple[float, int] | None:
+    """None when kl_loss_coeff is 0 (no term: today's calls), otherwise (coefficient, estimator code).  The
+    coefficient must be finite and > 0, the estimator one of KL_ESTIMATORS and ref_log_probs shaped like
+    old_log_probs; anything else raises ValueError."""
+    coeff = float(kl_loss_coeff)
+    if coeff == 0.0:
+        return None
+    if not (math.isfinite(coeff) and coeff > 0.0):
+        raise ValueError(f'kl_loss_coeff must be finite and > 0, got {kl_loss_coeff!r}')
+    est = kl_estimator_code(kl_loss_estimator)
+    if ref_log_probs is None or tuple(ref_log_probs.shape) != tuple(old_log_probs.shape):
+        raise ValueError('a KL loss term (kl_loss_coeff != 0) needs ref_log_probs with the shape of old_log_probs')
+    return coeff, est
+
+
+def _kl_loss_term(ref_log_probs, old_log_probs, kl_loss_coeff, kl_loss_estimator, dtype) -> _KlLossTerm | None:
+    """_kl_loss_args as the term the kernels take: ref_log_probs detached, cast to `dtype` (as _k5_operands casts
+    old_log_probs) and contiguous."""
+    args = _kl_loss_args(ref_log_probs, old_log_probs, kl_loss_coeff, kl_loss_estimator)
+    if args is None:
+        return None
+    coeff, est = args
+    L.require_cuda(ref_log_probs)
+    ref = ref_log_probs.detach().to(dtype).contiguous()
+    return _KlLossTerm(ref, coeff, est, torch.empty(1, dtype=torch.float32, device=ref.device))
+
+
 def _loss_inputs(x, old, aux, mask):
     L.require_cuda(x, old, aux, mask)
     if not (x.shape == old.shape == aux.shape == mask.shape) or x.dim() != 2:
@@ -2444,16 +2503,34 @@ def _loss_inputs(x, old, aux, mask):
 
 
 def actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio: float, mode: str | None = None,
-               objective: ActorObjective | None = None, return_clip_fraction: bool = False):
+               objective: ActorObjective | None = None, return_clip_fraction: bool = False, ref_log_probs=None,
+               kl_loss_coeff: float = 0.0, kl_loss_estimator: str = 'k3'):
     """PPOTrainer.actor_loss_fn (trainers/text_to_text/ppo.py:291-307), differentiable in log_probs.
     objective: an ActorObjective (None: the reference's).  return_clip_fraction: -> (loss, fp32[2] device tensor: the
-    clipped fraction and the dual-clip fraction, aggregated like the loss; see aa_ppo_actor_loss_obj)."""
+    clipped fraction and the dual-clip fraction, aggregated like the loss; see aa_ppo_actor_loss_obj).
+    kl_loss_coeff != 0 (a KL loss term, see _actor_loss): the loss is  actor_loss + kl_loss_coeff * agg(KL)  (fp32)
+    and the detached agg(KL) follows it, before the clip fractions."""
+    loss, _, kl, cf = _actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio, mode, objective,
+                                  return_clip_fraction, ref_log_probs, kl_loss_coeff, kl_loss_estimator)
+    out = (loss,) + ((kl,) if kl is not None else ()) + ((cf,) if return_clip_fraction else ())
+    return out if len(out) > 1 else loss
+
+
+def _actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio, mode, objective, return_clip_fraction,
+                ref_log_probs, kl_loss_coeff, kl_loss_estimator):
+    """actor_loss -> (loss, the actor loss without the KL term for ppo_pack_metrics (the loss itself without the term,
+    K5's fp32[2] with it), the detached agg(KL) or None, clip fractions or None).  The KL loss term: KL(lp, ref) by
+    `kl_loss_estimator` (KL_ESTIMATORS), aggregated over the same mask as the objective (its loss_agg_mode), its
+    gradient added to K5's (aa_ppo_actor_loss_kl)."""
     objective = _objective(objective)
     x, old, aux, m = _loss_inputs(log_probs, old_log_probs, advantages, mask)
+    kl = _kl_loss_term(ref_log_probs, old_log_probs, kl_loss_coeff, kl_loss_estimator, x.dtype)
     obj = objective.args(clip_range_ratio) if objective is not None else None
     cf = torch.zeros(2, dtype=torch.float32, device=x.device) if return_clip_fraction else None
-    loss, _, _ = _PpoLossFn.apply(x, old, aux, m, clip_range_ratio, _mode_code(mode, x.dtype), True, obj, cf)
-    return (loss, cf) if return_clip_fraction else loss
+    loss, _, loss32 = _PpoLossFn.apply(x, old, aux, m, clip_range_ratio, _mode_code(mode, x.dtype), True, obj, cf, kl)
+    if kl is None:
+        return loss, loss, None, cf
+    return loss, loss32, kl.out[0], cf
 
 
 def critic_loss(values, old_values, returns, mask, clip_range_value: float, mode: str | None = None,
@@ -2466,13 +2543,16 @@ def critic_loss(values, old_values, returns, mask, clip_range_value: float, mode
 
 def tail_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, lens, old_log_probs, advantages, mask,
                     clip_range_ratio: float, mode: str | None = None, entropy_coeff: float = 0.0,
-                    objective: ActorObjective | None = None, return_clip_fraction: bool = False):
+                    objective: ActorObjective | None = None, return_clip_fraction: bool = False, ref_log_probs=None,
+                    kl_loss_coeff: float = 0.0, kl_loss_estimator: str = 'k3'):
     """response_tail_log_probs + actor_loss as one autograd node (see _TailActorLossFn).
     -> (actor loss, new log-probs (B, W), the loss as fp32[2] for ppo_pack_metrics).  entropy_coeff != 0: the first
     output is  actor_loss - entropy_coeff * masked_mean(H, mask)  (fp32), the third stays the actor loss without the
     bonus, and the detached masked-mean entropy follows as a fourth.  objective: an ActorObjective (None: the
-    reference's; under token-mean the entropy term is a token mean too).  return_clip_fraction: the fp32[2] clip
-    fractions (see actor_loss) follow as the last output."""
+    reference's; under token-mean the entropy term is a token mean too).  kl_loss_coeff != 0 (a KL loss term, as
+    actor_loss; ref_log_probs (B, W) aligned with old_log_probs): the first output gains  + kl_loss_coeff * agg(KL),
+    the third stays without it and the detached agg(KL) follows the entropy mean (if any).  return_clip_fraction: the
+    fp32[2] clip fractions (see actor_loss) follow as the last output."""
     objective = _objective(objective)
     L.require_cuda(logits, input_ids, old_log_probs, advantages, mask)
     lens = as_device_lens(lens, logits.device)
@@ -2483,16 +2563,17 @@ def tail_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, lens, old_log
         raise ValueError('old_log_probs, advantages and mask must all be (B, W), W = the bound of the response lengths')
     logits, ids = _contiguous_last(logits), input_ids.contiguous()
     mode_code = _mode_code(mode, logits.dtype)
-    old, aux, m = _k5_operands(old_log_probs, advantages, mask,
-                               logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32)
+    lp_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
+    old, aux, m = _k5_operands(old_log_probs, advantages, mask, lp_dtype)
+    kl = _kl_loss_term(ref_log_probs, old_log_probs, kl_loss_coeff, kl_loss_estimator, lp_dtype)
     plan = device_tail_plan(lens, K, logits.stride(0), logits.stride(1), ids.stride(0), ids.size(1), 0, -1, lens.bound)
     single_pass = _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad)
     if objective is not None:
         objective.args(clip_range_ratio)  # a bad clip range fails here, before the node launches anything
     cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
     out = _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass,
-                                 float(entropy_coeff), objective, cf)
-    return (*out, cf) if return_clip_fraction else out
+                                 float(entropy_coeff), objective, cf, kl)
+    return (*out, *((kl.out[0],) if kl is not None else ()), *((cf,) if return_clip_fraction else ()))
 
 
 @functools.lru_cache(maxsize=64)
@@ -2506,7 +2587,8 @@ def _dense_actor_plan(B: int, L: int, start: int, sb: int, sl: int, lab_sb: int,
 
 def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, old_log_probs, advantages, mask,
                      clip_range_ratio: float, mode: str | None = None, entropy_coeff: float = 0.0,
-                     objective: ActorObjective | None = None, return_clip_fraction: bool = False):
+                     objective: ActorObjective | None = None, return_clip_fraction: bool = False, ref_log_probs=None,
+                     kl_loss_coeff: float = 0.0, kl_loss_estimator: str = 'k3'):
     """The actor half of the text rl_step (trainers/text_to_text/ppo.py:336-349) as one autograd node:
     `gather_log_probabilities(logits[:, :-1], ids[:, 1:])[:, start:]` -> `actor_loss_fn` -> backward up to d logits.
     Only the rows `[start, L - 1)` are read (the reference scores every position and slices afterwards); with a
@@ -2516,7 +2598,9 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
     entropy_coeff != 0 (entropy bonus): the first output is  actor_loss - entropy_coeff * masked_mean(H, mask)  (fp32),
     the third stays the actor loss without the bonus and the detached masked-mean entropy follows as a fourth; the
     single pass is K1f's entropy-gradient variant, the composed path K1's entropy variant -> K5 + masked_mean -> K1b's
-    entropy variant.  objective / return_clip_fraction: as tail_actor_loss (the clip fractions are the last output)."""
+    entropy variant.  objective / return_clip_fraction / the KL loss term (ref_log_probs (B, L - 1 - start),
+    kl_loss_coeff, kl_loss_estimator): as tail_actor_loss (agg(KL) after the entropy mean, the clip fractions last);
+    the composed path runs K5's KL entry point, whose gradient K1b carries to the tile."""
     objective = _objective(objective)
     L.require_cuda(logits, input_ids, old_log_probs, advantages, mask)
     if logits.dim() != 3 or input_ids.shape != logits.shape[:2]:
@@ -2534,31 +2618,31 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
         # short rows, fp16, no gradient: the composed ops (K1 over the response rows -> K5, which takes the objective;
         # backward K1b)
         rows, labels = logits[:, start:-1], input_ids[:, start + 1:]
+        _kl_loss_args(ref_log_probs, old_log_probs, kl_loss_coeff, kl_loss_estimator)  # a bad term fails before K1
         if entropy_coeff != 0.0:
             lp, ent = gather_log_probabilities_with_entropy(rows, labels, mode=mode, entropy_grad=True)
         else:
             lp = gather_log_probabilities(rows, labels, mode=mode)
-        loss = actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, mode=mode, objective=objective,
-                          return_clip_fraction=return_clip_fraction)
-        cf = ()
-        if return_clip_fraction:
-            loss, cf = loss[0], (loss[1],)
+        loss, loss32, kl, cf = _actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, mode, objective,
+                                           return_clip_fraction, ref_log_probs, kl_loss_coeff, kl_loss_estimator)
+        tail = ((kl,) if kl is not None else ()) + ((cf,) if return_clip_fraction else ())
         if entropy_coeff == 0.0:
-            return (loss, lp.detach(), loss, *cf)
+            return (loss, lp.detach(), loss32, *tail)
         m = mask.to(torch.bool)
         h_mean = token_mean(ent, m) if objective is not None and objective.token_mean else masked_mean(ent, m)
-        return (loss - float(entropy_coeff) * h_mean, lp.detach(), loss, h_mean.detach(), *cf)
+        return (loss - float(entropy_coeff) * h_mean, lp.detach(), loss32, h_mean.detach(), *tail)
     logits, ids = _contiguous_last(logits), input_ids.contiguous()
     if B > 1 and (logits.stride(0) != Lq * logits.stride(1)):
         logits = logits.contiguous()  # the gradient tile is shaped after the logits: rows must be uniformly strided
     mode_code = _mode_code(mode, logits.dtype)
-    old, aux, m = _k5_operands(old_log_probs, advantages, mask,
-                               logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32)
+    lp_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
+    old, aux, m = _k5_operands(old_log_probs, advantages, mask, lp_dtype)
+    kl = _kl_loss_term(ref_log_probs, old_log_probs, kl_loss_coeff, kl_loss_estimator, lp_dtype)
     plan = _dense_actor_plan(B, Lq, start, logits.stride(0), logits.stride(1), ids.stride(0), str(logits.device))
     cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
     out = _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, True,
-                                 float(entropy_coeff), objective, cf)
-    return (*out, cf) if return_clip_fraction else out
+                                 float(entropy_coeff), objective, cf, kl)
+    return (*out, *((kl.out[0],) if kl is not None else ()), *((cf,) if return_clip_fraction else ()))
 
 
 def tail_critic_loss(scores: torch.Tensor, lens, old_values, returns, mask, clip_range_value: float,

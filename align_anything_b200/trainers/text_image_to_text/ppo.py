@@ -157,9 +157,9 @@ class PPOTrainer(_TextPPOTrainer):
             self, reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, 0)
 
         # actor: K1 over the response tails + K5 as ONE autograd node; its backward is K1b alone (:296-316)
-        actor_loss, actor_loss32, entropy_mean, clip_frac = actor_loss_node(
+        actor_loss, actor_loss32, entropy_mean, clip_frac, kl_loss = actor_loss_node(
             self, self.infer_batch(inference_batch), input_ids, old_log_probs, reward_advantages, sequence_mask,
-            lens=lens)
+            lens=lens, ref_log_probs=ref_log_probs)
         self.actor_model.backward(actor_loss)
         self.actor_model.step()
 
@@ -174,4 +174,4 @@ class PPOTrainer(_TextPPOTrainer):
             self, row_stats, reward, value_row_mean, actor_loss32, critic_loss32,
             {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns},
             entropy=training_batch['entropy'] if self.log_entropy else None, mask=sequence_mask,
-            entropy_mean=entropy_mean, clip_frac=clip_frac)
+            entropy_mean=entropy_mean, clip_frac=clip_frac, kl_loss=kl_loss)

@@ -33,9 +33,10 @@ METRIC_KEYS = (
 
 def refuse_kl_switches(tr) -> None:
     """Safe RLHF-V keeps the reference's KL: its kl_coeff shapes rewards and costs together (k1, fixed).  The KL
-    switches it inherits from the PPO trainers (all four, kl_horizon included: it only means something with kl_target)
+    switches it inherits from the PPO trainers (all five, kl_horizon included: it only means something with kl_target)
     raise here, before anything runs, when set to another value."""
-    for name, default in (('kl_estimator', 'k1'), ('kl_target', None), ('kl_horizon', 10000), ('kl_loss_coeff', 0)):
+    for name, default in (('kl_estimator', 'k1'), ('kl_target', None), ('kl_horizon', 10000), ('kl_loss_coeff', 0),
+                          ('kl_loss_estimator', None)):
         v = switch_of(tr, name)
         if v is not None and v != default:
             raise ValueError(f'{name}={v!r}: Safe RLHF-V keeps the reference KL penalty (k1, a fixed kl_coeff)')

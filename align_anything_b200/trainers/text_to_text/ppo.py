@@ -84,19 +84,28 @@ def adaptive_kl_coeff(kl_coeff: float, kl: float, n: int, target: float, horizon
     return kl_coeff * (1.0 + e * n / horizon)
 
 
-def refuse_kl_loss_term(tr) -> None:
-    """The KL term in the actor loss (`kl_loss_coeff`) is not implemented: K5 and K1f's actor node do not read the
-    reference log-probs.  A non-zero value raises ValueError here, before anything runs, instead of being ignored."""
+def kl_loss_of(tr) -> tuple[float, str] | None:
+    """(kl_loss_coeff, kl_loss_estimator) of the KL term in the actor loss, or None when `kl_loss_estimator` is unset
+    (no term).  The term is on iff the estimator is set (switch_of each): then it must be one of ops.KL_ESTIMATORS and
+    kl_loss_coeff finite and > 0.  A non-zero kl_loss_coeff without an estimator is refused rather than ignored.  Every
+    error raises ValueError here, before anything runs."""
+    est = switch_of(tr, 'kl_loss_estimator')
     c = switch_of(tr, 'kl_loss_coeff')
-    if c is not None and c != 0:
-        raise ValueError(f'kl_loss_coeff={c!r}: the KL term in the PPO actor loss is not supported; the KL enters '
-                         f'through the reward penalty only (kl_coeff, kl_estimator, kl_target)')
+    if est is None:
+        if c is not None and c != 0:
+            raise ValueError(f'kl_loss_coeff={c!r} without kl_loss_estimator: the KL term in the PPO actor loss is '
+                             f'turned on by kl_loss_estimator (k1, k2 or k3)')
+        return None
+    ops.kl_estimator_code(est)
+    if isinstance(c, bool) or not isinstance(c, (int, float)) or not (math.isfinite(c) and c > 0):
+        raise ValueError(f'kl_loss_estimator={est!r} needs a finite kl_loss_coeff > 0, got {c!r}')
+    return float(c), est
 
 
 def kl_rewards(tr, reward, log_probs, ref_log_probs, values, sequence_mask, start):
     """K4 of an rl_step under the trainer's KL switches: the KL-shaped rewards, GAE and the metric row sums
     (ops.kl_rewards_and_gae with kl_estimator_of(tr); checks the KL switches before the launch)."""
-    refuse_kl_loss_term(tr)
+    kl_loss_of(tr)
     kl_controller_of(tr)
     est = kl_estimator_of(tr)
     return ops.kl_rewards_and_gae(reward, log_probs, ref_log_probs, values, sequence_mask, start, tr.kl_coeff,
@@ -126,20 +135,28 @@ def objective_kwargs(tr) -> dict:
     return kw
 
 
-def actor_loss_node(tr, batch, input_ids, old_log_probs, advantages, mask, *, start=0, head=None, lens=None):
+def actor_loss_node(tr, batch, input_ids, old_log_probs, advantages, mask, *, start=0, head=None, lens=None,
+                    ref_log_probs=None):
     """The actor loss of an rl_step -> (loss, the loss for ppo_pack_metrics, the masked-mean entropy or None, the
-    fp32[2] clip fractions or None).  The rows scored are those of the text layout, `[start:]` of every row, or with
-    `lens` the response tails of the multimodal layout (`old_log_probs`, `advantages` and `mask` already (B, W)).
+    fp32[2] clip fractions or None, agg(KL) of the KL loss term or None).  The rows scored are those of the text
+    layout, `[start:]` of every row, or with `lens` the response tails of the multimodal layout (`old_log_probs`,
+    `ref_log_probs`, `advantages` and `mask` already (B, W)).
     `head`: the lm_head weight of the text layout's fused path.  With an entropy bonus (entropy_coeff_of(tr) != 0) the loss is
     actor_loss - c * masked_mean(H, mask)  over the same rows and mask (a token mean under loss_agg_mode 'token-mean'),
     the second output stays the actor loss without it.  The actor objective switches (actor_objective_of) reach K5 and
-    K1f; `tr.log_clip_fraction` asks K5 for the clip fractions.  A function rather than a method, so that the grafted
-    rl_step of the reference's classes finds it without being grafted itself."""
+    K1f; `tr.log_clip_fraction` asks K5 for the clip fractions.  With a KL loss term (kl_loss_of) the loss gains
+    + kl_loss_coeff * agg(KL(lp, ref_log_probs), mask)  aggregated like the objective; the second output stays without
+    it.  A function rather than a method, so that the grafted rl_step of the reference's classes finds it without
+    being grafted itself."""
     coeff = entropy_coeff_of(tr)
     kw = objective_kwargs(tr)
-    cf = None
+    cf = kl = None
     if lens is None:
         old_log_probs, mask = old_log_probs[:, start:], mask[:, start:]
+    term = kl_loss_of(tr)
+    if term is not None:
+        kw.update(ref_log_probs=ref_log_probs if lens is not None else ref_log_probs[:, start:], kl_loss_coeff=term[0],
+                  kl_loss_estimator=term[1])
     if tr.fused_lm_head:  # K6 + K6b + backward GEMMs for the log-probs, then K5
         # with a bonus K6's entropy variant; K6b adds the entropy's gradient in its epilogue
         ent_kw = {'return_entropy': coeff != 0.0, 'entropy_grad': coeff != 0.0, 'use_cache': False}
@@ -150,14 +167,16 @@ def actor_loss_node(tr, batch, input_ids, old_log_probs, advantages, mask, *, st
             log_probs = tr._tail_log_probs(tr.actor_model, batch, lens, input_ids, **ent_kw)
         if coeff != 0.0:
             log_probs, ent = log_probs
-        loss = ops.actor_loss(log_probs, old_log_probs, advantages, mask, tr.clip_range_ratio, mode=tr.mode, **kw)
-        if kw.get('return_clip_fraction'):
-            loss, cf = loss
+        # ops.actor_loss, with the actor loss without the KL term beside the loss
+        loss, loss32, kl, cf = ops._actor_loss(
+            log_probs, old_log_probs, advantages, mask, tr.clip_range_ratio, tr.mode, kw.get('objective'),
+            kw.get('return_clip_fraction', False), kw.get('ref_log_probs'), kw.get('kl_loss_coeff', 0.0),
+            kw.get('kl_loss_estimator', 'k3'))
         if coeff == 0.0:
-            return loss, loss, None, cf
+            return loss, loss32, None, cf, kl
         token = 'objective' in kw and kw['objective'].token_mean
         h_mean = (ops.token_mean if token else ops.masked_mean)(ent, mask)
-        return loss - coeff * h_mean, loss, h_mean.detach(), cf
+        return loss - coeff * h_mean, loss32, h_mean.detach(), cf, kl
     # One autograd node (K1f): log-probs, d loss / d log-prob and the gradient tile in a single pass over the scored
     # rows.  The text layout reads only the rows `[start:]` the reference keeps after scoring every position
     # (:338-346); the prompt rows of the tile are written as zeros by the same kernel.
@@ -173,11 +192,13 @@ def actor_loss_node(tr, batch, input_ids, old_log_probs, advantages, mask, *, st
                                   mode=tr.mode, **kw)
     if kw.get('return_clip_fraction'):
         out, cf = out[:-1], out[-1]
-    return out[0], out[2], (out[3] if coeff != 0.0 else None), cf
+    if term is not None:
+        out, kl = out[:-1], out[-1]
+    return out[0], out[2], (out[3] if coeff != 0.0 else None), cf, kl
 
 
 def ppo_metrics(tr, row_stats, reward, value_row_mean, actor_loss, critic_loss, tensors, *, entropy=None, mask=None,
-                entropy_mean=None, clip_frac=None) -> dict[str, Any]:
+                entropy_mean=None, clip_frac=None, kl_loss=None) -> dict[str, Any]:
     """The metric dict of a PPO rl_step from ONE packed collective and ONE host sync (reference: 10 all-reduces, a
     barrier and 12 .item()).  ppo_pack_metrics packs the ten metrics of METRIC_KEYS, the device status word (lane 10,
     MAX-reduced with lane 9) and a spare lane 11 (0).  Optional AVG lanes follow, each read back under its key:
@@ -185,7 +206,8 @@ def ppo_metrics(tr, row_stats, reward, value_row_mean, actor_loss, critic_loss, 
         like train/kl_divergence: summed over each row's masked tokens, averaged over rows and ranks;
       * `entropy_mean`, the entropy term of the bonus (train/actor_entropy);
       * `clip_frac`, K5's clip fraction (train/actor_clip_fraction) and with dual-clip its dual-clip fraction
-        (train/actor_dual_clip_fraction).
+        (train/actor_dual_clip_fraction);
+      * `kl_loss`, agg(KL) of the KL loss term without its coefficient (train/actor_kl_loss).
     Sets `tr.last_rl_tensors = tensors` (per-token tensors stay out of the dict: the reference hands it to Logger.log,
     which takes scalars only).  With `kl_target` set (kl_controller_of) the step's train/kl_coeff goes into the dict and
     tr.kl_coeff takes the adaptive controller's update from the step's (all-reduced) train/kl_divergence and its
@@ -193,7 +215,7 @@ def ppo_metrics(tr, row_stats, reward, value_row_mean, actor_loss, critic_loss, 
     with torch.no_grad():
         # an optional lane is filled in before the one packed all-reduce, so the NVLink reduction fused into
         # ppo_pack_metrics (which reduces the vector as it writes it) gives way to all_reduce_packed
-        extra = entropy is not None or entropy_mean is not None or clip_frac is not None
+        extra = entropy is not None or entropy_mean is not None or clip_frac is not None or kl_loss is not None
         fused = fused_allreduce(row_stats.device) if not extra else None
         stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss, critic_loss,
                                      coll=fused.next((9, 10)) if fused is not None else None)
@@ -207,6 +229,8 @@ def ppo_metrics(tr, row_stats, reward, value_row_mean, actor_loss, critic_loss, 
             objective = actor_objective_of(tr)
             if objective is not None and objective.dual_clip_ratio is not None:
                 lanes['train/actor_dual_clip_fraction'] = clip_frac[1:2]
+        if kl_loss is not None:
+            lanes['train/actor_kl_loss'] = kl_loss.detach().float().reshape(1)
         first = 11 if entropy is not None else 12  # the entropy takes the spare lane 11
         if lanes:
             stats = torch.cat([stats[:first], *lanes.values()])
@@ -259,16 +283,21 @@ class PPOTrainer:
     # 'k2' (0.5 * (lp - ref) ** 2) or 'k3' (exp(ref - lp) - (ref - lp) - 1); train/kl_divergence stays the k1 sum.
     # kl_target (None = a fixed kl_coeff): the adaptive KL coefficient of Ziegler et al. (2019), updated after every
     # rl_step from train/kl_divergence with horizon kl_horizon (adaptive_kl_coeff); train/kl_coeff reports the
-    # coefficient each step used.  `cfgs.train_cfgs.<key>` overrides each when set.  kl_loss_coeff (a KL term in the
-    # actor loss) is not implemented: anything but 0 raises before the step runs (refuse_kl_loss_term).
+    # coefficient each step used.  `cfgs.train_cfgs.<key>` overrides each when set.
     kl_estimator = None
     kl_target = None
     kl_horizon = 10000
+    # The KL term in the actor loss (verl's use_kl_loss): kl_loss_estimator 'k1' / 'k2' / 'k3' (None = no term) turns
+    # it on, and the actor minimises  actor_loss + kl_loss_coeff * agg(KL(lp, ref), mask)  with the objective's
+    # aggregation.  kl_loss_coeff must then be finite and > 0; without an estimator anything but 0 raises
+    # (kl_loss_of).  Independent of the reward penalty: kl_coeff 0 moves the KL from the reward into the loss.
+    # train/actor_loss stays the clipped objective, train/actor_kl_loss reports agg(KL).
     kl_loss_coeff = 0.0
+    kl_loss_estimator = None
     # the class attributes above that the grafted methods read: patch.install() copies them onto the reference's classes
     SWITCHES = ('mode', 'fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'clip_range_ratio_low',
                 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode', 'log_clip_fraction', 'kl_estimator',
-                'kl_target', 'kl_horizon', 'kl_loss_coeff')
+                'kl_target', 'kl_horizon', 'kl_loss_coeff', 'kl_loss_estimator')
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, reward_model=None,
                  reward_critic_model=None, tokenizer=None, reward_tokenizer=None, *, kl_coeff=0.02,
@@ -438,8 +467,9 @@ class PPOTrainer:
         if returns is not None:
             reward_advantages, reward_returns = returns(old_rewards, sequence_mask, start, row_stats)
 
-        actor_loss, actor_loss32, entropy_mean, clip_frac = actor_loss_node(
-            self, inference_batch, input_ids, old_log_probs, reward_advantages, sequence_mask, start=start, head=head)
+        actor_loss, actor_loss32, entropy_mean, clip_frac, kl_loss = actor_loss_node(
+            self, inference_batch, input_ids, old_log_probs, reward_advantages, sequence_mask, start=start, head=head,
+            ref_log_probs=ref_log_probs)
         self.actor_model.backward(actor_loss)
         self.actor_model.step()
 
@@ -455,4 +485,4 @@ class PPOTrainer:
             self, row_stats, reward, value_row_mean, actor_loss32, reward_critic_loss,
             {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns},
             entropy=training_batch['entropy'][:, start:] if self.log_entropy else None, mask=sequence_mask[:, start:],
-            entropy_mean=entropy_mean, clip_frac=clip_frac)
+            entropy_mean=entropy_mean, clip_frac=clip_frac, kl_loss=kl_loss)

@@ -440,6 +440,22 @@ int aa_ppo_actor_loss_obj(const void *log_probs, int64_t lp_stride, const void *
                           int loss_agg, int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac,
                           float *row_scratch, uint32_t *counter, void *stream);
 
+/* aa_ppo_actor_loss_obj with a KL loss term: the actor minimises  loss + kl_loss_coeff * agg(KL, mask), KL the
+ * per-token estimate (AA_KL_*, kl_estimator) of log_probs against ref_log_probs (lp_dtype, (B, Wm) with row stride
+ * ref_stride), agg the objective's aggregation over the same mask.
+ *   loss      : the clipped objective alone, as aa_ppo_actor_loss_obj writes it
+ *   kl_loss   : fp32 [1], agg(KL) without the coefficient (in the log-probs' dtype's rounding in FAITHFUL mode)
+ *   grad      : d (loss + kl_loss_coeff * agg(KL)) / d log_probs
+ *   row_scratch: fp32 [5 * B]
+ * kl_loss_coeff must be finite and > 0 and ref_log_probs non-NULL; these and the objective's checks run before any
+ * CUDA call. */
+int aa_ppo_actor_loss_kl(const void *log_probs, int64_t lp_stride, const void *old_log_probs, int64_t old_stride,
+                         int lp_dtype, const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
+                         int64_t mask_stride, int32_t B, int32_t Wm, float clip_low, float clip_high, float dual_clip,
+                         int loss_agg, int mode, const void *ref_log_probs, int64_t ref_stride, float kl_loss_coeff,
+                         int kl_estimator, float *loss, float *kl_loss, void *grad, int64_t grad_stride,
+                         float *clip_frac, float *row_scratch, uint32_t *counter, void *stream);
+
 int aa_ppo_critic_loss(const void *values, int64_t val_stride, const void *old_values,
                        int64_t old_stride, int val_dtype, const void *returns, int64_t ret_stride,
                        int ret_dtype, const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t Wm,
@@ -509,6 +525,23 @@ int aa_logprob_actor_fused_obj(const void *logits, int logits_dtype, int64_t row
                                int64_t mask_stride, int32_t W, float clip_low, float clip_high, float dual_clip,
                                int loss_agg, int mode, void *grad_logits, int64_t grad_row_stride, void *row_scratch,
                                int32_t *status, float entropy_coeff, float *entropy, void *stream);
+
+/* aa_logprob_actor_fused_obj with the KL loss term of aa_ppo_actor_loss_kl: the gradient tile carries
+ * d (actor_loss + kl_loss_coeff * agg(KL, mask)) / d logits.  ref_log_probs (lp_dtype) is laid out like log_probs
+ * (contiguous (n_segments, W)) and is read at each log-prob's own index.  log_probs, stat_* and entropy are
+ * bit-identical to aa_logprob_actor_fused_obj; the loss value and agg(KL) are aa_ppo_actor_loss_kl's on log_probs.
+ * row_scratch: 48 bytes per tile row plus 8 bytes per segment.  kl_loss_coeff must be finite and > 0 and
+ * ref_log_probs non-NULL; these and the objective's checks run before any CUDA call. */
+int aa_logprob_actor_fused_kl(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                              const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                              const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
+                              const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
+                              float *stat_max, float *stat_logsum, const void *old_log_probs, int64_t old_stride,
+                              const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
+                              int64_t mask_stride, int32_t W, float clip_low, float clip_high, float dual_clip,
+                              int loss_agg, int mode, void *grad_logits, int64_t grad_row_stride, void *row_scratch,
+                              int32_t *status, float entropy_coeff, float *entropy, const void *ref_log_probs,
+                              float kl_loss_coeff, int kl_estimator, void *stream);
 
 /* The same single pass for the mean cross-entropy behind `outputs.loss` (trainers/text_to_text/sft.py:95-98
  * `SupervisedTrainer.loss`, ppo.py:400-408 `ptx_step`; transformers' ForCausalLMLoss): every row whose label !=
