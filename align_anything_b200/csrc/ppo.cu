@@ -645,9 +645,12 @@ struct GrpoObjParams {
 // GRPO's loss and d loss / d lp, one block per row, the last block to arrive reduces the rows.  OBJECTIVE: the clipped
 // objective (grpo_obj_token) under one of the three aggregations (aa_grpo_loss_obj); otherwise the reference's loss
 // (grpo_token, aa_grpo_loss), which passes agg = token-mean, old = clip_frac = nullptr: g_t = 1 / total, the row
-// partial is the fp32 row sum and the loss acc / total, as the reference computes them
-template <int THREADS, bool OBJECTIVE>
+// partial is the fp32 row sum and the loss acc / total, as the reference computes them.  SEQUENCE (with OBJECTIVE,
+// aa_grpo_loss_seq, old != nullptr): GSPO's sequence-level ratio -- the block first folds its row's summed log-ratio,
+// then every token takes the row's objective and ratio coefficient (grpo_seq_row, grpo_seq_token)
+template <int THREADS, bool OBJECTIVE, bool SEQUENCE = false>
 __global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoObjParams q) {
+  static_assert(OBJECTIVE || !SEQUENCE, "the sequence-level ratio is an option of the clipped objective");
   __shared__ float scratch[33];
   const GrpoParams &p = q.base;
   const int b = blockIdx.x, tid = threadIdx.x, r = p.r_lp;
@@ -656,13 +659,27 @@ __global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoObjParams 
   const float A = p.adv[b];
   const float g_t = grpo_agg_coeff(q.agg, total, static_cast<float>(end), p.B, p.K);
   float row = 0.f, n_clip = 0.f, n_dual = 0.f;
+  float s_seq = 0.f, coef_seq = 0.f;
+  int why_seq = 0;
+  if constexpr (SEQUENCE) {  // the masked-out tokens add (lp - old) * 0: nothing
+    float lr = 0.f;
+    for (int t = tid; t < end; t += THREADS)
+      lr += round_to(load_as_float(p.lp, b * p.lp_stride + t, p.dtype) -
+                         load_as_float(q.old, b * q.old_stride + t, p.dtype),
+                     r);
+    const float S = round_to(block_sum<THREADS>(lr, scratch), r);
+    grpo_seq_row(S, static_cast<float>(end), A, g_t, q.clip_lo, q.clip_hi, q.dual, r, s_seq, coef_seq, why_seq);
+  }
   for (int t = tid; t < p.K; t += THREADS) {
     const bool on = t < end;
     const float lp = load_as_float(p.lp, b * p.lp_stride + t, p.dtype);
     const float rf = load_as_float(p.ref_lp, b * p.ref_stride + t, p.dtype);
     float ptl, g;
     int why = 0;
-    if constexpr (OBJECTIVE) {
+    if constexpr (SEQUENCE) {
+      grpo_seq_token(lp, rf, s_seq, coef_seq, on, g_t, p.beta, q.kl_est, r, ptl, g);
+      why = why_seq;
+    } else if constexpr (OBJECTIVE) {
       const float old = q.old ? load_as_float(q.old, b * q.old_stride + t, p.dtype) : lp;
       grpo_obj_token(lp, old, rf, A, on, g_t, p.beta, q.clip_lo, q.clip_hi, q.dual, q.kl_est, r, ptl, g, why);
     } else {
@@ -1029,18 +1046,21 @@ extern "C" int aa_group_advantages(const float *rewards, int32_t n_groups, int32
   return check_launch("aa_group_advantages");
 }
 
-// aa_grpo_loss (objective false: the reference's loss, any mode) and aa_grpo_loss_obj: the checks, the completion mask
-// (row_end, and the token count in scratch[0]) and the loss kernel over scratch + 1
+// aa_grpo_loss (objective false: the reference's loss, any mode), aa_grpo_loss_obj / _kl and aa_grpo_loss_seq
+// (sequence: GSPO's sequence-level ratio, which needs the old log-probs): the checks, the completion mask (row_end, and
+// the token count in scratch[0]) and the loss kernel over scratch + 1
 static int grpo_loss(const char *who, bool objective, const void *log_probs, int64_t lp_stride, const void *ref_log_probs,
                      int64_t ref_stride, const void *old_log_probs, int64_t old_stride, int lp_dtype,
                      const float *advantages, const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id,
                      int32_t B, int32_t K, float beta, float clip_low, float clip_high, float dual_clip, int loss_agg,
                      int kl_estimator, int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac,
-                     int32_t *row_end, float *scratch, uint32_t *counter, void *stream) {
+                     int32_t *row_end, float *scratch, uint32_t *counter, void *stream, bool sequence = false) {
   AA_REQUIRE(B > 0 && K > 0 && log_probs && ref_log_probs && advantages && completion_tokens && loss && row_end &&
                  scratch && counter,
              AA_ERR_ARG, "%s: bad arguments", who);
   AA_REQUIRE(dtype_ok(lp_dtype), AA_ERR_DTYPE, "%s: bad dtype", who);
+  AA_REQUIRE(!sequence || old_log_probs, AA_ERR_ARG,
+             "%s: the sequence-level ratio needs old_log_probs (without them w = 1: use aa_grpo_loss_kl)", who);
   if (objective) {
     AA_REQUIRE(grpo_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
                "%s: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a known loss_agg; got "
@@ -1056,7 +1076,9 @@ static int grpo_loss(const char *who, bool objective, const void *log_probs, int
                              K, beta, (mode == AA_MODE_FAITHFUL) ? lp_dtype : AA_F32, loss, grad, grad_stride,
                              scratch + 1, counter + 1},
                   old_log_probs, old_stride, clip_low, clip_high, dual_clip, loss_agg, clip_frac, kl_estimator};
-  if (objective)
+  if (sequence)
+    grpo_loss_kernel<128, true, true><<<B, 128, 0, st>>>(q);
+  else if (objective)
     grpo_loss_kernel<128, true><<<B, 128, 0, st>>>(q);
   else
     grpo_loss_kernel<128, false><<<B, 128, 0, st>>>(q);
@@ -1104,6 +1126,18 @@ extern "C" int aa_grpo_loss_kl(const void *log_probs, int64_t lp_stride, const v
                    lp_dtype, advantages, completion_tokens, tok_stride, eos_id, B, K, beta, clip_low, clip_high,
                    dual_clip, loss_agg, kl_estimator, mode, loss, grad, grad_stride, clip_frac, row_end, scratch,
                    counter, stream);
+}
+
+extern "C" int aa_grpo_loss_seq(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
+                                const void *old_log_probs, int64_t old_stride, int lp_dtype, const float *advantages,
+                                const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B,
+                                int32_t K, float beta, float clip_low, float clip_high, float dual_clip, int loss_agg,
+                                int kl_estimator, int mode, float *loss, void *grad, int64_t grad_stride,
+                                float *clip_frac, int32_t *row_end, float *scratch, uint32_t *counter, void *stream) {
+  return grpo_loss("aa_grpo_loss_seq", true, log_probs, lp_stride, ref_log_probs, ref_stride, old_log_probs, old_stride,
+                   lp_dtype, advantages, completion_tokens, tok_stride, eos_id, B, K, beta, clip_low, clip_high,
+                   dual_clip, loss_agg, kl_estimator, mode, loss, grad, grad_stride, clip_frac, row_end, scratch,
+                   counter, stream, true);
 }
 
 extern "C" int aa_nll_mean(const void *logp, int dtype, const int64_t *labels, int64_t n, int64_t ignore_index,

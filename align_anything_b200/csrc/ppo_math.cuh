@@ -44,19 +44,11 @@ inline bool actor_objective_ok(float clip_low, float clip_high, float dual_clip,
          (loss_agg == AA_AGG_SEQ_MEAN_TOKEN_MEAN || loss_agg == AA_AGG_TOKEN_MEAN);
 }
 
-// One token of the clipped-ratio objective.  x / old: new / old log-prob (dtype code rx), aux: advantage,
-// on: the mask bit, g_rs: d loss / d (the token's objective) for a masked-in token (actor_row_coeff or
-// actor_token_mean_coeff).  eps_lo / eps_hi: the clip range [1 - eps_lo, 1 + eps_hi]; dual: the dual-clip factor c
-// (0 = off), ra: the rounding code of `c * adv` (the advantages' dtype).
-//   obj  = min(adv * ratio, adv * clip(ratio))     (the NEGATED loss term; NaN-propagating like torch.minimum)
-//          dual-clip, adv < 0:  max(obj, c * adv)  (torch.where(adv < 0, torch.maximum(obj, c * adv), obj))
-//   grad = d loss / d x                            (0 when the mask is off)
-//   why  = bit 0: the clipped branch is strictly smaller; bit 1: c * adv wins (the clip-fraction counters)
-__device__ __forceinline__ void actor_token(float x, float old, float aux, bool on, float g_rs, float eps_lo,
-                                            float eps_hi, float dual, int rx, int rp, int ra, float &obj, float &grad,
-                                            int &why) {
-  const float lo = round_to(1.f - eps_lo, rx), hi = round_to(1.f + eps_hi, rx);
-  const float ratio = round_to(expf(round_to(x - old, rx)), rx);
+// The clip / tie / dual-clip arithmetic of actor_token at a given ratio (rounding code rx) and clip bounds lo / hi
+// (already rounded to rx), shared by the token-level ratio (actor_token below) and GRPO's sequence-level
+// ratio (grpo_seq_row).  gs: the gradient reaching `ratio` (0 when `on` is false); obj, why: as actor_token's.
+__device__ __forceinline__ void clipped_ratio(float ratio, float lo, float hi, float aux, bool on, float g_rs,
+                                              float dual, int rx, int rp, int ra, float &obj, float &gs, int &why) {
   const float s1 = round_to(aux * ratio, rp);
   const float clipped = fminf(fmaxf(ratio, lo), hi);
   const float s2 = round_to(aux * clipped, rp);
@@ -77,7 +69,7 @@ __device__ __forceinline__ void actor_token(float x, float old, float aux, bool 
     if (obj == obj) obj = fmaxf(obj, ca);
   }
   const bool in_range = (ratio >= lo) && (ratio <= hi);
-  float gs = 0.f;  // gradient reaching `ratio` through both branches of torch.minimum
+  gs = 0.f;  // gradient reaching `ratio` through both branches of torch.minimum
   if (on) {
     if (s1 < s2) {
       gs = round_to(round_to(g * aux, rp), rx);
@@ -90,9 +82,25 @@ __device__ __forceinline__ void actor_token(float x, float old, float aux, bool 
     }
     // s1 > s2: the clipped branch wins and clamp's backward is zero outside the range
   }
-  grad = round_to(gs * ratio, rx);  // ExpBackward: grad * result
 }
 
+// One token of the clipped-ratio objective.  x / old: new / old log-prob (dtype code rx), aux: advantage,
+// on: the mask bit, g_rs: d loss / d (the token's objective) for a masked-in token (actor_row_coeff or
+// actor_token_mean_coeff).  eps_lo / eps_hi: the clip range [1 - eps_lo, 1 + eps_hi]; dual: the dual-clip factor c
+// (0 = off), ra: the rounding code of `c * adv` (the advantages' dtype).
+//   obj  = min(adv * ratio, adv * clip(ratio))     (the NEGATED loss term; NaN-propagating like torch.minimum)
+//          dual-clip, adv < 0:  max(obj, c * adv)  (torch.where(adv < 0, torch.maximum(obj, c * adv), obj))
+//   grad = d loss / d x                            (0 when the mask is off)
+//   why  = bit 0: the clipped branch is strictly smaller; bit 1: c * adv wins (the clip-fraction counters)
+__device__ __forceinline__ void actor_token(float x, float old, float aux, bool on, float g_rs, float eps_lo,
+                                            float eps_hi, float dual, int rx, int rp, int ra, float &obj, float &grad,
+                                            int &why) {
+  const float lo = round_to(1.f - eps_lo, rx), hi = round_to(1.f + eps_hi, rx);
+  const float ratio = round_to(expf(round_to(x - old, rx)), rx);
+  float gs;
+  clipped_ratio(ratio, lo, hi, aux, on, g_rs, dual, rx, rp, ra, obj, gs, why);
+  grad = round_to(gs * ratio, rx);  // ExpBackward: grad * result
+}
 
 // ---- KL estimators (ops.KL_ESTIMATORS; tests/kl_objective_port.py is their specification) ---------------------
 // One token's estimate of KL(policy || reference) from the log-probs lp and rf, each op rounded to `r` as the eager
@@ -185,6 +193,33 @@ __device__ __forceinline__ void grpo_obj_token(float lp, float old, float rf, fl
   ptl = -(s - bk);
   grad = 0.f;
   if (on) grad = kl_grad(ga, round_to(round_to(g_t, r) * beta, r), est, aux, r);
+}
+
+// GSPO's sequence-level ratio for one row (aa_grpo_loss_seq; tests/gspo_port.py is the specification):
+//   S = round_r(sum_t (lp_t - old_t) * m_t)   the row's summed log-ratio, in the log-prob dtype (`r`)
+//   log_w = S / n,  w = exp(log_w)           fp32 (n = the row's fp32 token count), and so are the clip bounds
+//   s = clipped_ratio(w) with fp32 roundings  the row's objective, shared by its tokens
+// g_t: d loss / d per-token loss of a counted token (grpo_agg_coeff), so d loss / d s = -n * g_t, the sum of the
+// row's per-token coefficients.  coef = d loss / d lp_t through the ratio, the same for every masked-in token:
+// ExpBackward (gs * w), DivBackward by n, cast once to `r` at the backward of the sum.  why: clipped_ratio's bits.
+__device__ __forceinline__ void grpo_seq_row(float S, float n, float A, float g_t, float eps_lo, float eps_hi,
+                                             float dual, int r, float &s, float &coef, int &why) {
+  const float w = expf(S / n);
+  float gs;
+  clipped_ratio(w, 1.f - eps_lo, 1.f + eps_hi, A, true, -(n * g_t), dual, AA_F32, AA_F32, AA_F32, s, gs, why);
+  coef = round_to((gs * w) / n, r);
+}
+
+// One token of GSPO's loss: -(s - beta * KL) with the row's objective s and ratio coefficient coef (grpo_seq_row),
+// and grpo_obj_token's KL and accumulation order (the ratio's gradient first, then the KL's)
+__device__ __forceinline__ void grpo_seq_token(float lp, float rf, float s, float coef, bool on, float g_t, float beta,
+                                               int est, int r, float &ptl, float &grad) {
+  float aux;
+  const float kl = kl_value(lp, rf, est, r, aux);
+  const float bk = round_to(beta * kl, r);
+  ptl = -(s - bk);
+  grad = 0.f;
+  if (on) grad = kl_grad(coef, round_to(round_to(g_t, r) * beta, r), est, aux, r);
 }
 
 // pass 1: first eos per row (-> row_end[b] = number of counted tokens) and the global token count

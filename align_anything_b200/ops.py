@@ -1256,13 +1256,15 @@ class _GrpoLossFn(torch.autograd.Function):
     (_grpo_loss_launch); obj / old / clip_frac select and feed the clipped objective."""
 
     @staticmethod
-    def forward(ctx, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj=None, old=None, clip_frac=None):
+    def forward(ctx, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj=None, old=None, clip_frac=None,
+                sequence=False):
         B, K = lp.shape
         dev = lp.device
         loss = torch.empty(1, dtype=torch.float32, device=dev)
         grad = torch.empty((B, K), dtype=lp.dtype, device=dev)
         row_end = torch.empty(B, dtype=torch.int32, device=dev)
-        _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end)
+        _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
+                          sequence=sequence)
         ctx.save_for_backward(grad)
         ctx.mark_non_differentiable(row_end)
         return loss[0], row_end
@@ -1270,14 +1272,15 @@ class _GrpoLossFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g, _):
         (grad,) = ctx.saved_tensors
-        return (grad.float() * g.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None
+        return (grad.float() * g.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None, None
 
 
 def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
-                      scratch=None):
+                      scratch=None, sequence=False):
     """GRPO's loss kernel, writing loss, row_end and (unless None) grad.  obj None: the reference loss (aa_grpo_loss);
     otherwise obj = _grpo_objective_args(...) for aa_grpo_loss_obj (aa_grpo_loss_kl unless the KL is k3), old = the old log-probs (None: the log-probs
-    themselves, ratio 1) and clip_frac = an fp32[2] tensor for the clip fractions or None.  scratch (fp32): the token
+    themselves, ratio 1) and clip_frac = an fp32[2] tensor for the clip fractions or None.  sequence (see
+    _sequence_level; old is then given): GSPO's sequence-level ratio, aa_grpo_loss_seq.  scratch (fp32): the token
     count and the row sums, B + 1 values, and under the objective the rows' clip counts too, 1 + 4 B; None allocates it."""
     B, K = lp.shape
     dev = lp.device
@@ -1290,6 +1293,9 @@ def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old
     tail = (row_end.data_ptr(), scratch.data_ptr(), _device_scratch(dev)['counter'][5:7].data_ptr(), L.stream_ptr(dev))
     if obj is None:
         L.check(lib.aa_grpo_loss(*lps, *rows, mode_code, *out, *tail))
+    elif sequence:
+        L.check(lib.aa_grpo_loss_seq(*lps, old.data_ptr(), old.stride(0), *rows, *obj, mode_code, *out,
+                                     L.ptr(clip_frac), *tail))
     elif obj[4] == KL_ESTIMATORS['k3']:
         L.check(lib.aa_grpo_loss_obj(*lps, L.ptr(old), old.stride(0) if old is not None else 0, *rows, *obj[:4],
                                      mode_code, *out, L.ptr(clip_frac), *tail))
@@ -1301,11 +1307,21 @@ def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old
 def _grpo_objective_args(objective, old, return_clip_fraction: bool):
     """The one rule for GRPO's reference loss -- no objective or one with default fields, no old log-probs and no clip
     fractions: None, and the nodes run today's launches.  Otherwise GrpoObjective.args() and the KL estimator's code
-    for the objective kernels (a default objective still gives its clip_range_ratio)."""
+    for the objective kernels (a default objective still gives its clip_range_ratio).  A sequence-level objective
+    without old log-probs has w = 1: it is the token-level objective and takes its launches."""
+    if old is None and getattr(objective, 'sequence_level', False):
+        objective = dataclasses.replace(objective, importance_sampling_level='token')
     if _objective(objective, GrpoObjective) is None and old is None and not return_clip_fraction:
         return None
     objective = objective or GrpoObjective()
     return objective.args() + (KL_ESTIMATORS[objective.kl_estimator],)
+
+
+def _sequence_level(objective, old) -> bool:
+    """Whether GSPO's sequence-level ratio runs: a sequence-level objective with old log-probs (updates 2..mu).  Its
+    tokens' gradients need the whole row's log-ratio first, so it runs on the composed path (aa_grpo_loss_seq), never
+    on K1f's single pass."""
+    return old is not None and getattr(objective, 'sequence_level', False)
 
 
 def _old_log_probs(old, shape, dtype):
@@ -1325,8 +1341,9 @@ def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, 
     -(exp(lp - lp.detach()) * A - beta * KL), completion mask up to the first eos, token mean -> fp32 scalar,
     differentiable in per_token_logps.  Returns (loss, counted_tokens_per_row).
     objective (ops.GrpoObjective) / old_per_token_logps (the rollout-time policy log-probs, (B, K)): GRPO's clipped
-    objective (aa_grpo_loss_obj) with ratio exp(lp - old); without old_per_token_logps the ratio is 1.  None / default
-    fields and no old log-probs: today's launch.  return_clip_fraction appends the fp32[2] clip fractions."""
+    objective (aa_grpo_loss_obj) with ratio exp(lp - old); without old_per_token_logps the ratio is 1.  A sequence-level
+    objective with old_per_token_logps: GSPO's one ratio per sequence (aa_grpo_loss_seq).  None / default fields and no
+    old log-probs: today's launch.  return_clip_fraction appends the fp32[2] clip fractions."""
     L.require_cuda(per_token_logps, ref_per_token_logps, advantages, completion_tokens)
     obj = _grpo_objective_args(objective, old_per_token_logps, return_clip_fraction)
     if per_token_logps.dim() != 2 or per_token_logps.shape != ref_per_token_logps.shape or \
@@ -1340,7 +1357,8 @@ def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, 
     old = _old_log_probs(old_per_token_logps, lp.shape, lp.dtype)
     tok = _contiguous_last(completion_tokens.to(torch.int64))
     cf = torch.zeros(2, dtype=torch.float32, device=lp.device) if return_clip_fraction else None
-    out = _GrpoLossFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype), obj, old, cf)
+    out = _GrpoLossFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype), obj, old, cf,
+                            _sequence_level(objective, old))
     return out + (cf,) if return_clip_fraction else out
 
 
@@ -1455,14 +1473,17 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
     the detached GRPO loss without the bonus follow row_end (before the entropy when return_entropy); the single pass is K1f's entropy-gradient variant, the
     composed path K1's entropy variant -> grpo_loss -> K1b's entropy variant.
     objective / old_per_token_logps: GRPO's clipped objective as in grpo_loss (K1f's objective entry point, or K1 ->
-    aa_grpo_loss_obj -> K1b); the entropy bonus stays a token mean over the completion mask.  return_clip_fraction
-    appends the fp32[2] clip fractions last.  None / default fields and no old log-probs: today's launches."""
+    aa_grpo_loss_obj -> K1b); the entropy bonus stays a token mean over the completion mask.  A sequence-level objective
+    with old log-probs always takes the composed path (K1 -> aa_grpo_loss_seq -> K1b, see _sequence_level).
+    return_clip_fraction appends the fp32[2] clip fractions last.  None / default fields and no old log-probs: today's
+    launches."""
     L.require_cuda(logits, input_ids, ref_per_token_logps, advantages)
     obj = _grpo_objective_args(objective, old_per_token_logps, return_clip_fraction)
     K = int(logits_to_keep)
     tokens = input_ids[:, -K:]
     coeff = float(entropy_coeff)
-    if not _single_pass_ok(logits, _FUSED_GRPO, torch.is_grad_enabled() and logits.requires_grad):
+    if _sequence_level(objective, old_per_token_logps) or \
+            not _single_pass_ok(logits, _FUSED_GRPO, torch.is_grad_enabled() and logits.requires_grad):
         ent = None
         if return_entropy or coeff != 0.0:
             lp, ent = tail_token_log_probs(logits, input_ids, K, mode=mode, return_entropy=True,
@@ -2182,6 +2203,8 @@ class ActorObjective:
 
 # include/aa_b200.h AA_AGG_*: GRPO also takes Dr. GRPO's constant normaliser
 GRPO_LOSS_AGG_MODES = {**LOSS_AGG_MODES, 'seq-mean-token-sum-norm': 2}
+# GRPO's importance ratio: per token (aa_grpo_loss_obj / _kl) or per sequence (GSPO, aa_grpo_loss_seq)
+IMPORTANCE_SAMPLING_LEVELS = ('token', 'sequence')
 
 
 @dataclasses.dataclass(frozen=True)
@@ -2197,23 +2220,35 @@ class GrpoObjective(ActorObjective):
 
     clip_range_ratio: the ε of both bounds when clip_range_ratio_low / _high are None.  With old_lp = lp (the first
     update of a rollout) the ratio is 1 and nothing is clipped.  kl_estimator: the per-token KL ('k3', the reference's,
-    or 'k1' / 'k2': KL_ESTIMATORS).  Checked on the host when constructed."""
+    or 'k1' / 'k2': KL_ESTIMATORS).  importance_sampling_level: 'token' (the ratio above) or 'sequence' (GSPO, Zheng et
+    al. 2025; TRL's importance_sampling_level): one fp32 ratio per sequence, w = exp(sum((lp - old) * mask) / n) with
+    n = the sequence's counted tokens, clipped in place of each token's ratio (aa_grpo_loss_seq).  Without old
+    log-probs w is 1 and the token-level launches run.  Checked on the host when constructed."""
 
     loss_agg_mode: str = 'token-mean'
     clip_range_ratio: float = 0.2
     kl_estimator: str = 'k3'
+    importance_sampling_level: str = 'token'
     _MODES = GRPO_LOSS_AGG_MODES
 
     def __post_init__(self):
         super().__post_init__()
         self.args()  # the clip range with clip_range_ratio filled in
         kl_estimator_code(self.kl_estimator)
+        if self.importance_sampling_level not in IMPORTANCE_SAMPLING_LEVELS:
+            raise ValueError(f'importance_sampling_level must be one of {IMPORTANCE_SAMPLING_LEVELS}, got '
+                             f'{self.importance_sampling_level!r}')
 
     @property
     def is_default(self) -> bool:
         """The reference's loss when the ratio is 1: the kernels run today's launches."""
         return (self.clip_range_ratio_low is None and self.clip_range_ratio_high is None and self.dual_clip_ratio is None
-                and self.loss_agg_mode == 'token-mean' and self.kl_estimator == 'k3')
+                and self.loss_agg_mode == 'token-mean' and self.kl_estimator == 'k3'
+                and self.importance_sampling_level == 'token')
+
+    @property
+    def sequence_level(self) -> bool:
+        return self.importance_sampling_level == 'sequence'
 
     def args(self, clip_range_ratio: float | None = None) -> tuple[float, float, float, int]:
         return super().args(self.clip_range_ratio if clip_range_ratio is None else clip_range_ratio)

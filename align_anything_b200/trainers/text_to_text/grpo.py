@@ -16,7 +16,7 @@ from .ppo import entropy_coeff_of, hidden_log_probs, lm_head_of, switch_of
 __all__ = ['GRPOTrainer']
 
 GRPO_OBJECTIVE_KEYS = ('clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio',
-                       'loss_agg_mode', 'kl_estimator')
+                       'loss_agg_mode', 'kl_estimator', 'importance_sampling_level')
 
 
 def num_iterations_of(tr) -> int:
@@ -74,13 +74,18 @@ class GRPOTrainer:
     # The per-token KL of the loss -(s - beta * KL): 'k3' (the reference's exp(ref - lp) - (ref - lp) - 1), 'k1'
     # (lp - ref) or 'k2' (0.5 * (lp - ref) ** 2); ops.KL_ESTIMATORS.  `cfgs.train_cfgs.kl_estimator` overrides it.
     kl_estimator = 'k3'
+    # GRPO's importance ratio: 'token' (exp(lp - old) per token, the default) or 'sequence' (GSPO, Zheng et al. 2025;
+    # TRL's importance_sampling_level): one ratio per completion, exp of the mean of its tokens' log-ratios, clipped in
+    # place of the token ratios.  It acts from update 2 on, so it wants num_iterations > 1; the first update (ratio 1)
+    # runs the token-level launches.  `cfgs.train_cfgs.importance_sampling_level` overrides it.
+    importance_sampling_level = 'token'
     # Opt-in: train/actor_clip_fraction (and train/actor_dual_clip_fraction with dual-clip), the mean over the updates,
     # in the step's one packed all-reduce
     log_clip_fraction = False
     # the class attributes above that the grafted methods read: patch.install() copies them onto the reference's class
     SWITCHES = ('mode', 'fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'num_iterations',
                 'clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode',
-                'scale_rewards', 'log_clip_fraction', 'kl_estimator')
+                'scale_rewards', 'log_clip_fraction', 'kl_estimator', 'importance_sampling_level')
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, tokenizer=None, *, beta=None,
                  num_generations=None) -> None:

@@ -679,6 +679,20 @@ int aa_grpo_loss_kl(const void *log_probs, int64_t lp_stride, const void *ref_lo
                     float beta, float clip_low, float clip_high, float dual_clip, int loss_agg, int kl_estimator,
                     int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac, int32_t *row_end,
                     float *scratch, uint32_t *counter, void *stream);
+/* aa_grpo_loss_kl with GSPO's sequence-level ratio (Zheng et al. 2025; TRL's importance_sampling_level="sequence"):
+ * one ratio per row, w = exp(S / n), with S = sum(((lp - old) * mask)) rounded once to lp_dtype and n the row's token
+ * count; w, the clip bounds and s = min(A * w, A * clamp(w, 1 - clip_low, 1 + clip_high)) (and dual-clip) are fp32 in
+ * both modes.  The per-token KL, the aggregations and the clip fractions are aa_grpo_loss_kl's; every counted token of
+ * a row shares w, so the fractions count clipped sequences (seq-mean-token-mean) or the tokens in them.  Each token's
+ * gradient through the ratio is d loss / d w * w / n, cast once to the gradient's rounding dtype.  old_log_probs is
+ * required (without it w == 1 and the objective is aa_grpo_loss_kl's at ratio 1).  Arguments are checked before any
+ * CUDA call. */
+int aa_grpo_loss_seq(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
+                     const void *old_log_probs, int64_t old_stride, int lp_dtype, const float *advantages,
+                     const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B, int32_t K,
+                     float beta, float clip_low, float clip_high, float dual_clip, int loss_agg, int kl_estimator,
+                     int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac, int32_t *row_end,
+                     float *scratch, uint32_t *counter, void *stream);
 
 /* masked_mean (utils/tools.py:460-467): mean over rows of masked row means -> out[0];
  * mask == NULL: plain mean. */
