@@ -19,6 +19,7 @@ AA_BF16, AA_F16, AA_F32 = 0, 1, 2
 MODE_FAITHFUL, MODE_F32 = 0, 1
 MASK_U8, MASK_I64 = 0, 1
 STATUS_LABEL_OOB, STATUS_SHORT_SEQUENCE, STATUS_EMPTY_MASK, STATUS_DIVERGE_RANGE = 1, 2, 4, 8
+STATUS_WHITEN_COUNT = 16
 
 _DTYPE_CODE = {torch.bfloat16: AA_BF16, torch.float16: AA_F16, torch.float32: AA_F32}
 _CODE_DTYPE = {v: k for k, v in _DTYPE_CODE.items()}
@@ -83,6 +84,9 @@ _SIGS = {
                                _P, _P]),
     'aa_ppo_returns': (c_int, [_P, c_int, c_int64, _P, c_int64, c_int32, c_int32, c_int32, c_int, c_int32, c_float,
                                c_int, c_int, _P, _P, c_int, _P, _P]),
+    'aa_whiten_moments': (c_int, [_P, c_int, c_int64, _P, c_int64, c_int32, c_int32, _P, c_int32, c_int32, _P]),
+    'aa_whiten_reduce': (c_int, [_P, c_int32, _P, _P]),
+    'aa_whiten_apply': (c_int, [_P, c_int, c_int64, _P, c_int64, c_int32, c_int32, _P, _P, _P]),
     'aa_ppo_actor_loss': (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, c_int32,
                                   c_int32, c_float, c_int, _P, _P, c_int64, _P, _P, _P]),
     'aa_ppo_actor_loss_obj': (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, c_int32, c_int32,

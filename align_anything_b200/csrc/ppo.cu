@@ -9,6 +9,7 @@
 // K4r aa_ppo_returns     : Multi-PPO's reinforce / rloo / reinforce_baseline / group_norm returns
 //                          (trainers/text_to_text/multi_ppo.py:510-591) on K4's shaped rewards.
 //     aa_ppo_pack_metrics: the ten local scalars of :360-381 packed for ONE all-reduce.
+//     aa_whiten_moments / aa_whiten_reduce / aa_whiten_apply: masked_whiten of a rollout's advantages.
 //
 // These touch ~10 floats per token: latency-bound, not bandwidth-bound.  The point is launch
 // count (thousands -> five) and zero host syncs; each sample is owned by one warp / CTA.
@@ -817,6 +818,95 @@ __global__ void __launch_bounds__(32) allreduce_packed_kernel(const float *src, 
   p2p_allreduce_packed(coll, src, dst, n);
 }
 
+// ---- advantage whitening over a rollout (TRL's / verl's masked_whiten, shift_mean=True) -----------------------------
+// The statistics are fp64 (n, sum A, sum A^2) triples.  Every sum has a fixed order, so a run reproduces its bits:
+// each thread walks the same elements in the same order, then one fixed tree per block, then the K micro-batch slots
+// in slot order.  There are no floating-point atomics.
+constexpr int kWhitenThreads = 1024;
+
+// Deterministic fp64 block sum (block_sum's fixed tree); result valid in every thread.  `scratch` >= 33 doubles.
+template <int THREADS>
+__device__ __forceinline__ double block_sum_f64(double v, double *scratch) {
+  constexpr int W = THREADS / kWarp;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) scratch[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < kWarp) {
+    double t = threadIdx.x < W ? scratch[threadIdx.x] : 0.0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if (threadIdx.x == 0) scratch[32] = t;
+  }
+  __syncthreads();
+  const double r = scratch[32];
+  __syncthreads();
+  return r;
+}
+
+// One CTA per micro-batch: a micro-batch's (B, W) advantages are a few thousand to a few hundred thousand elements, which
+// one CTA reads in microseconds, so the sums need no cross-CTA combine (no partials, no counter).  The element loads are
+// unconditional and masked by a select, so a masked-out NaN never enters the sums.
+__global__ void __launch_bounds__(kWhitenThreads)
+    whiten_moments_kernel(const void *adv, int dtype, int64_t adv_stride, const uint8_t *__restrict__ mask,
+                          int64_t mask_stride, int B, int W, double *slot) {
+  __shared__ double scratch[33];
+  double n = 0.0, s1 = 0.0, s2 = 0.0;
+  const uint32_t total = static_cast<uint32_t>(B) * static_cast<uint32_t>(W);  // < 2^31 (aa_whiten_moments)
+#pragma unroll 4
+  for (uint32_t i = threadIdx.x; i < total; i += kWhitenThreads) {
+    const uint32_t b = i / static_cast<uint32_t>(W), t = i - b * static_cast<uint32_t>(W);
+    const double a = load_as_float(adv, b * adv_stride + t, dtype);
+    const bool on = mask[b * mask_stride + t] != 0;
+    n += on ? 1.0 : 0.0;
+    s1 += on ? a : 0.0;
+    s2 += on ? a * a : 0.0;
+  }
+  n = block_sum_f64<kWhitenThreads>(n, scratch);
+  s1 = block_sum_f64<kWhitenThreads>(s1, scratch);
+  s2 = block_sum_f64<kWhitenThreads>(s2, scratch);
+  if (threadIdx.x == 0) {
+    slot[0] = n;
+    slot[1] = s1;
+    slot[2] = s2;
+  }
+}
+
+// total[c] = sum over k = 0 .. K-1 of moments[k][c], in slot order (K is the rollout's micro-batch count)
+__global__ void __launch_bounds__(32) whiten_reduce_kernel(const double *__restrict__ moments, int K, double *total) {
+  const int c = threadIdx.x;
+  if (c >= 3) return;
+  double s = 0.0;
+  for (int k = 0; k < K; ++k) s += moments[3 * k + c];
+  total[c] = s;
+}
+
+// A' = (A - mean) * rstd where m, 0 where not m, in place.  mean and rstd = 1 / sqrt(var + 1e-8) (var unbiased, clamped at
+// 0 against the rounding of sum A^2 - mean sum A) are formed in fp64 from the reduced triple and rounded once to fp32;
+// the difference and the product are fp32, rounded once to the advantages' dtype.  n < 2 (masked_var's error) sets
+// AA_STATUS_WHITEN_COUNT and writes nothing.
+__global__ void __launch_bounds__(256)
+    whiten_apply_kernel(void *adv, int dtype, int64_t adv_stride, const uint8_t *__restrict__ mask, int64_t mask_stride,
+                        int W, const double *__restrict__ total, int32_t *status) {
+  const int b = blockIdx.y;
+  const int t = blockIdx.x * 256 + threadIdx.x;
+  const double n = total[0];
+  if (!(n >= 2.0)) {
+    if (b == 0 && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(status, AA_STATUS_WHITEN_COUNT);
+    return;
+  }
+  if (t >= W) return;
+  const double mean64 = total[1] / n;
+  const double m2 = total[2] - total[1] * mean64;
+  const double var = (m2 < 0.0 ? 0.0 : m2) / (n - 1.0);  // (a NaN stays NaN, as in masked_whiten)
+  const float mean = static_cast<float>(mean64);
+  const float rstd = static_cast<float>(1.0 / sqrt(var + 1e-8));
+  const int64_t i = static_cast<int64_t>(b) * adv_stride + t;
+  const bool on = mask[static_cast<int64_t>(b) * mask_stride + t] != 0;
+  const float v = on ? __fmul_rn(__fsub_rn(load_as_float(adv, i, dtype), mean), rstd) : 0.f;
+  store_from_float(adv, i, dtype, v);
+}
+
 static bool dtype_ok(int d) { return d == AA_BF16 || d == AA_F16 || d == AA_F32; }
 
 }  // namespace aa
@@ -1173,6 +1263,40 @@ extern "C" int aa_ppo_pack_metrics(const float *row_stats, const float *reward, 
   ppo_pack_metrics_kernel<<<1, 32, 0, static_cast<cudaStream_t>(stream)>>>(row_stats, reward, value_row_mean,
                                                                             actor_loss, critic_loss, B, stats, c, status);
   return check_launch("aa_ppo_pack_metrics");
+}
+
+extern "C" int aa_whiten_moments(const void *advantages, int adv_dtype, int64_t adv_row_stride, const uint8_t *mask,
+                                 int64_t mask_row_stride, int32_t B, int32_t W, double *moments, int32_t k, int32_t K,
+                                 void *stream) {
+  AA_REQUIRE(advantages && mask && moments, AA_ERR_ARG, "aa_whiten_moments: null pointer");
+  AA_REQUIRE(dtype_ok(adv_dtype), AA_ERR_DTYPE, "aa_whiten_moments: bad dtype %d", adv_dtype);
+  AA_REQUIRE(B > 0 && W > 0 && static_cast<int64_t>(B) * W <= INT32_MAX, AA_ERR_ARG,
+             "aa_whiten_moments: bad sizes (B=%d W=%d)", B, W);
+  AA_REQUIRE(adv_row_stride >= W && mask_row_stride >= W, AA_ERR_ARG, "aa_whiten_moments: row strides must be >= W");
+  AA_REQUIRE(K > 0 && k >= 0 && k < K, AA_ERR_ARG, "aa_whiten_moments: slot k=%d outside [0, K=%d)", k, K);
+  whiten_moments_kernel<<<1, kWhitenThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      advantages, adv_dtype, adv_row_stride, mask, mask_row_stride, B, W, moments + 3 * static_cast<int64_t>(k));
+  return check_launch("aa_whiten_moments");
+}
+
+extern "C" int aa_whiten_reduce(const double *moments, int32_t K, double *total, void *stream) {
+  AA_REQUIRE(moments && total, AA_ERR_ARG, "aa_whiten_reduce: null pointer");
+  AA_REQUIRE(K > 0, AA_ERR_ARG, "aa_whiten_reduce: bad slot count K=%d", K);
+  whiten_reduce_kernel<<<1, 32, 0, static_cast<cudaStream_t>(stream)>>>(moments, K, total);
+  return check_launch("aa_whiten_reduce");
+}
+
+extern "C" int aa_whiten_apply(void *advantages, int adv_dtype, int64_t adv_row_stride, const uint8_t *mask,
+                               int64_t mask_row_stride, int32_t B, int32_t W, const double *total, int32_t *status,
+                               void *stream) {
+  AA_REQUIRE(advantages && mask && total && status, AA_ERR_ARG, "aa_whiten_apply: null pointer");
+  AA_REQUIRE(dtype_ok(adv_dtype), AA_ERR_DTYPE, "aa_whiten_apply: bad dtype %d", adv_dtype);
+  AA_REQUIRE(B > 0 && W > 0 && B <= 65535, AA_ERR_ARG, "aa_whiten_apply: bad sizes (B=%d W=%d)", B, W);
+  AA_REQUIRE(adv_row_stride >= W && mask_row_stride >= W, AA_ERR_ARG, "aa_whiten_apply: row strides must be >= W");
+  const dim3 grid((W + 255) / 256, B);
+  whiten_apply_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(advantages, adv_dtype, adv_row_stride, mask,
+                                                                           mask_row_stride, W, total, status);
+  return check_launch("aa_whiten_apply");
 }
 
 extern "C" int aa_allreduce_packed(const float *src, float *dst, int32_t n, const aa_coll *coll, void *stream) {

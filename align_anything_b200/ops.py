@@ -26,7 +26,7 @@ __all__ = [
     'move_padding_left', 'count_nonpad', 'strip_pad_tail', 'ppo_pack_metrics', 'check_status', 'raise_for_status', 'status_lane', 'causal_lm_loss', 'rm_pair_loss', 'cost_pair_loss','group_advantages', 'grpo_loss', 'tail_token_log_probs', 'pair_slices', 'slice_sums', 'tail_rows', 'linear_token_log_probs',
     'sequence_log_probs_from_hidden', 'fused_linear_token_log_probs', 'tail_log_probs_from_hidden', 'dense_log_probs_from_hidden', 'tail_actor_loss', 'tail_critic_loss', 'lm_head_weight',
     'causal_lm_loss_from_hidden', 'causal_lm_valid_rows', 'gather_log_probabilities_with_entropy',
-    'response_tail_log_probs_pair_with_entropy', 'ActorObjective', 'token_mean', 'DpoObjective',
+    'response_tail_log_probs_pair_with_entropy', 'ActorObjective', 'token_mean', 'DpoObjective', 'whiten_advantages',
 ]
 
 # Path knobs: plain module attributes, read at call time and never from the environment.  Every path is chosen from the
@@ -109,6 +109,9 @@ def _raise_status_bits(v: int) -> int:
         raise IndexError('align_anything_b200: a mask row has no True element (m.nonzero()[-1] would raise)')
     if v & L.STATUS_DIVERGE_RANGE:
         raise AssertionError('diverge index is out of range!')  # trainers/text_to_text/simpo.py:72-73
+    if v & L.STATUS_WHITEN_COUNT:
+        raise ValueError('align_anything_b200: whitening the advantages needs at least 2 masked tokens over the rollout '
+                         '(masked_var would raise)')
     return v
 
 
@@ -2147,6 +2150,55 @@ def estimator_returns(rewards, sequence_mask, start: int, estimator: str, n_samp
         ESTIMATORS[estimator], n, float(gamma), mode_code, int(bool(mask_outputs)), adv.data_ptr(), ret.data_ptr(), L.dtype_code(out_dtype),
         L.ptr(row_stats), L.stream_ptr(dev)))
     return adv, ret
+
+
+def whiten_advantages(advantages: list[torch.Tensor], masks: list[torch.Tensor], group=None) -> list[torch.Tensor]:
+    """TRL's / verl's masked_whiten(A, m, shift_mean=True) over ALL the micro-batches of one rollout, and over every rank
+    of `group` (torch.distributed; None: the default group) when torch.distributed is initialised with more than one:
+        n = sum m,  mean = sum m A / n,  var = sum m (A - mean) ** 2 / (n - 1),
+        A' = (A - mean) * rsqrt(var + 1e-8) where m, 0 where not m.
+    `advantages[k]` is micro-batch k's (B_k, W_k) advantages (bf16 / fp16 / fp32; the widths may differ) and `masks[k]`
+    its mask of the same shape.  The statistics are fp64 and every sum has a fixed order, so the result is
+    deterministic; mean and rstd are rounded once to fp32 and A' once to the advantages' dtype.  The tensors are
+    rewritten in place (a copy first when the last dimension is strided) and returned.
+    Launches: aa_whiten_moments per micro-batch, aa_whiten_reduce, all_reduce(SUM) of the (3,) fp64 triple across
+    ranks, aa_whiten_apply per micro-batch; no host sync.  Fewer than 2 masked tokens in all sets a status bit, raised
+    as ValueError at the next status read (check_status, or a PPO step's metrics), and leaves the advantages unchanged.
+    Bad arguments raise ValueError here, before any launch."""
+    advantages, masks = list(advantages), list(masks)
+    if not advantages or len(advantages) != len(masks):
+        raise ValueError(f'whiten_advantages needs one mask per advantages tensor and at least one of each, got '
+                         f'{len(advantages)} and {len(masks)}')
+    for a, m in zip(advantages, masks):
+        if not (isinstance(a, torch.Tensor) and isinstance(m, torch.Tensor)) or a.dim() != 2 or \
+                tuple(m.shape) != tuple(a.shape) or a.numel() == 0:
+            raise ValueError(f'whiten_advantages: advantages and masks must be matching non-empty (B, W) tensors, got '
+                             f'{tuple(getattr(a, "shape", ()))} and {tuple(getattr(m, "shape", ()))}')
+        if a.dtype not in (torch.bfloat16, torch.float16, torch.float32):
+            raise ValueError(f'whiten_advantages: advantages must be bf16 / fp16 / fp32, got {a.dtype}')
+    try:
+        L.require_cuda(*advantages, *masks)
+    except RuntimeError as e:
+        raise ValueError(f'whiten_advantages: {e}') from None
+    dev = advantages[0].device
+    outs = [a if a.stride(-1) == 1 else a.contiguous() for a in advantages]
+    masks = [_contiguous_last(m.to(torch.bool)) for m in masks]
+    K = len(outs)
+    moments = torch.empty((K, 3), dtype=torch.float64, device=dev)
+    total = torch.empty(3, dtype=torch.float64, device=dev)
+    lib, stream = L.lib(), L.stream_ptr(dev)
+    for k, (a, m) in enumerate(zip(outs, masks)):
+        L.check(lib.aa_whiten_moments(a.data_ptr(), L.dtype_code(a.dtype), a.stride(0), m.data_ptr(), m.stride(0),
+                                      a.size(0), a.size(1), moments.data_ptr(), k, K, stream))
+    L.check(lib.aa_whiten_reduce(moments.data_ptr(), K, total.data_ptr(), stream))
+    dist = torch.distributed
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
+        dist.all_reduce(total, op=dist.ReduceOp.SUM, group=group)
+    status = _device_scratch(dev)['status']
+    for a, m in zip(outs, masks):
+        L.check(lib.aa_whiten_apply(a.data_ptr(), L.dtype_code(a.dtype), a.stride(0), m.data_ptr(), m.stride(0),
+                                    a.size(0), a.size(1), total.data_ptr(), status.data_ptr(), stream))
+    return outs
 
 
 LOSS_AGG_MODES = {'seq-mean-token-mean': 0, 'token-mean': 1}  # include/aa_b200.h AA_AGG_*

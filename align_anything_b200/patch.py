@@ -20,7 +20,8 @@ swaps, without touching any reference file,
   * GRPOTrainer.{_get_per_token_logps, train_step} of the text trainer (the PPO and GRPO classes also get the
     `fused_lm_head` / `lm_head_chunk_rows` / `log_entropy` / `entropy_coeff` switches, off; the PPO classes also the
     actor-objective switches and the KL switches `kl_estimator`, `kl_target`, `kl_horizon`, `kl_loss_coeff` and
-    `kl_loss_estimator`, unset: the reference's penalty and no KL term in the actor loss; the GRPO class also the GRPO-objective switches `num_iterations`, `clip_range_ratio`,
+    `kl_loss_estimator`, unset: the reference's penalty and no KL term in the actor loss, and `whiten_advantages`, off;
+    the GRPO class also the GRPO-objective switches `num_iterations`, `clip_range_ratio`,
     `clip_range_ratio_low`, `clip_range_ratio_high`, `dual_clip_ratio`, `loss_agg_mode`, `scale_rewards`,
     `log_clip_fraction`, `kl_estimator` and `importance_sampling_level`, at the reference's single-update loss), RMTrainer.{loss, train_step} of the text /
     audio / video trainers (the audio and video trainers override `loss` with the text arithmetic, so their own `loss`

@@ -15,7 +15,7 @@ import torch
 
 from ... import ops
 from ..text_to_text.ppo import PPOTrainer as _TextPPOTrainer
-from ..text_to_text.ppo import actor_loss_node, kl_rewards, ppo_metrics
+from ..text_to_text.ppo import actor_loss_node, ppo_metrics, step_advantages, whiten_advantages_of, whiten_rollout
 
 __all__ = ['PPOTrainer', 'move_padding_left']
 
@@ -92,6 +92,7 @@ class PPOTrainer(_TextPPOTrainer):
     # ---- trainers/text_image_to_text/ppo.py:206-269, text_audio_to_text/ppo.py:217-277 --------
     @torch.no_grad()
     def rollout(self, prompt_only_batch):
+        whiten = whiten_advantages_of(self)
         self.set_train(mode=False)
         if self.micro_batched_rollout:
             total = prompt_only_batch['input_ids'].size(0)
@@ -107,6 +108,9 @@ class PPOTrainer(_TextPPOTrainer):
             mini_batch['attention_mask'] = actor_batch['attention_mask']
             inference_batches.append(mini_batch)
             training_batches.append(training)
+        if whiten:  # the tail layout: K4 from column 0, the response mask is the actor loss's
+            whiten_rollout(self, training_batches, [t['response_mask'] for t in training_batches],
+                           [0] * len(training_batches))
         self.set_train()
         return inference_batches, training_batches
 
@@ -153,8 +157,7 @@ class PPOTrainer(_TextPPOTrainer):
         input_ids = inference_batch['input_ids']
         lens = ops.as_device_lens(training_batch['response_lens'], input_ids.device)
 
-        old_rewards, reward_advantages, reward_returns, row_stats = kl_rewards(
-            self, reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, 0)
+        old_rewards, reward_advantages, reward_returns, row_stats = step_advantages(self, training_batch, sequence_mask, 0)
 
         # actor: K1 over the response tails + K5 as ONE autograd node; its backward is K1b alone (:296-316)
         actor_loss, actor_loss32, entropy_mean, clip_frac, kl_loss = actor_loss_node(

@@ -18,7 +18,7 @@ from ... import ops
 from ...utils.multi_process import all_reduce_packed
 from .ppo import PPOTrainer as _MMPPOTrainer
 from .ppo import _tail_values
-from ..text_to_text.ppo import switch_of
+from ..text_to_text.ppo import switch_of, whiten_advantages_of
 
 __all__ = ['SafeRLHFVTrainer']
 
@@ -42,8 +42,21 @@ def refuse_kl_switches(tr) -> None:
             raise ValueError(f'{name}={v!r}: Safe RLHF-V keeps the reference KL penalty (k1, a fixed kl_coeff)')
 
 
+def refuse_whitening(tr) -> None:
+    """Safe RLHF-V mixes its reward and cost advantages with the Lagrange multiplier as the reference does, unwhitened:
+    `whiten_advantages` set to True (or to anything but a bool) raises here, before anything runs."""
+    if whiten_advantages_of(tr):
+        raise ValueError('whiten_advantages=True: Safe RLHF-V keeps the reference\'s unwhitened reward and cost advantages')
+
+
 class SafeRLHFVTrainer(_MMPPOTrainer):
     log_lambda: torch.Tensor  # nn.Parameter in the reference (saferlhf.py:107-110)
+
+    @torch.no_grad()
+    def rollout(self, prompt_only_batch):
+        """The multimodal rollout (saferlhf.py:343-430), refusing whiten_advantages before generation."""
+        refuse_whitening(self)
+        return _MMPPOTrainer.rollout(self, prompt_only_batch)
 
     # ---- saferlhf.py:343-430: the multimodal scoring plus the cost model's end score and the cost critic's values ----
     @torch.no_grad()
@@ -107,6 +120,7 @@ class SafeRLHFVTrainer(_MMPPOTrainer):
     # ---- saferlhf.py:483-675 ---------------------------------------------------------------------------
     def rl_step(self, inference_batch, training_batch) -> dict[str, Any]:
         refuse_kl_switches(self)
+        refuse_whitening(self)
         self._lambda_step()
         lens = ops.as_device_lens(training_batch['response_lens'], training_batch['log_probs'].device)
         old_log_probs = training_batch['log_probs']

@@ -22,10 +22,24 @@ import torch
 
 from ... import ops
 from .ppo import PPOTrainer as _TextPPOTrainer
+from .ppo import whiten_advantages_of, whiten_rollout
 
 __all__ = ['PPOTrainer']
 
 GROUP_ESTIMATORS = ('rloo', 'reinforce_baseline', 'group_norm')
+
+
+def estimator_returns_of(tr):
+    """The `returns` hook of the text trainer's rl_step for the advantage estimator in effect: None for 'gae' (K4's
+    GAE), otherwise K4r's advantages and returns, with their row means written into lanes 3 / 4 of row_stats."""
+    if tr.advantage_estimator == 'gae':
+        return None
+
+    def returns(old_rewards, sequence_mask, start, row_stats):
+        return ops.estimator_returns(old_rewards, sequence_mask, start, tr.advantage_estimator, tr.n_samples_per_prompt,
+                                     tr.gamma, mode=tr.mode, row_stats=row_stats)
+
+    return returns
 
 
 class PPOTrainer(_TextPPOTrainer):
@@ -46,7 +60,10 @@ class PPOTrainer(_TextPPOTrainer):
     @torch.no_grad()
     def rollout(self, prompt_only_batch):
         """The text rollout with every prompt repeated n_samples_per_prompt times (tensors: repeat_interleave on dim 0,
-        anything else: each item repeated) and `action_mask` added to each training batch."""
+        anything else: each item repeated) and `action_mask` added to each training batch.  With whiten_advantages, the
+        estimator's advantages whitened over the rollout (REINFORCE++ for 'reinforce'; the group estimators after their
+        own group statistic)."""
+        whiten = whiten_advantages_of(self)
         self.set_train(mode=False)
         total = prompt_only_batch['input_ids'].size(0)
         micro = int(self.cfgs.train_cfgs.per_device_train_batch_size)
@@ -65,6 +82,9 @@ class PPOTrainer(_TextPPOTrainer):
             mini_batch['attention_mask'] = inference['attention_mask']
             inference_batches.append(mini_batch)
             training_batches.append(training)
+        if whiten:
+            whiten_rollout(self, training_batches, [b['attention_mask'][:, 1:] for b in inference_batches],
+                           [t['prompt_idx'] for t in training_batches], estimator_returns_of(self))
         self.set_train()
         return inference_batches, training_batches
 
@@ -90,10 +110,5 @@ class PPOTrainer(_TextPPOTrainer):
     # ---- multi_ppo.py:330-419 ---------------------------------------------------------------
     def rl_step(self, inference_batch, training_batch) -> dict[str, Any]:
         """The text trainer's rl_step.  Past 'gae', K4r's outputs replace K4's GAE ones: the estimator's advantages and
-        returns, with their row means written into lanes 3 / 4 of row_stats."""
-        def returns(old_rewards, sequence_mask, start, row_stats):
-            return ops.estimator_returns(old_rewards, sequence_mask, start, self.advantage_estimator,
-                                         self.n_samples_per_prompt, self.gamma, mode=self.mode, row_stats=row_stats)
-
-        return _TextPPOTrainer.rl_step(self, inference_batch, training_batch,
-                                       returns=None if self.advantage_estimator == 'gae' else returns)
+        returns, with their row means written into lanes 3 / 4 of row_stats (estimator_returns_of)."""
+        return _TextPPOTrainer.rl_step(self, inference_batch, training_batch, returns=estimator_returns_of(self))

@@ -113,6 +113,56 @@ def kl_rewards(tr, reward, log_probs, ref_log_probs, values, sequence_mask, star
                                   **({} if est == 'k1' else {'kl_estimator': est}))
 
 
+def whiten_advantages_of(tr) -> bool:
+    """Whether rollout() whitens the advantages (switch_of `whiten_advantages`; unset: False).  Anything but a bool
+    raises ValueError."""
+    v = switch_of(tr, 'whiten_advantages')
+    if v is None:
+        return False
+    if not isinstance(v, bool):
+        raise ValueError(f'whiten_advantages must be True or False, got {v!r}')
+    return v
+
+
+# the tensors a whitening rollout() stores in each training batch, in rl_step's order
+ROLLOUT_ADVANTAGE_KEYS = ('old_rewards', 'advantages', 'returns', 'row_stats')
+
+
+def micro_batch_advantages(tr, training_batch, sequence_mask, start, returns=None):
+    """The KL-shaped rewards, advantages, returns and metric row sums of one micro-batch: K4 (kl_rewards) and, with
+    `returns(old_rewards, sequence_mask, start, row_stats) -> (advantages, returns)`, K4r (Multi-PPO's estimators)."""
+    old_rewards, advantages, ret, row_stats = kl_rewards(
+        tr, training_batch['reward'], training_batch['log_probs'], training_batch['ref_log_probs'],
+        training_batch['reward_values'], sequence_mask, start)
+    if returns is not None:
+        advantages, ret = returns(old_rewards, sequence_mask, start, row_stats)
+    return old_rewards, advantages, ret, row_stats
+
+
+def step_advantages(tr, training_batch, sequence_mask, start, returns=None):
+    """rl_step's (old_rewards, advantages, returns, row_stats): micro_batch_advantages, or with whiten_advantages on
+    the tensors rollout() stored (whiten_rollout), with no launch; the KL switches are checked first either way."""
+    if not whiten_advantages_of(tr):
+        return micro_batch_advantages(tr, training_batch, sequence_mask, start, returns)
+    kl_loss_of(tr)
+    kl_controller_of(tr)
+    kl_estimator_of(tr)
+    return tuple(training_batch[k] for k in ROLLOUT_ADVANTAGE_KEYS)
+
+
+def whiten_rollout(tr, training_batches, sequence_masks, starts, returns=None) -> None:
+    """rollout()'s advantages under whiten_advantages: K4 (+ K4r through `returns`) for each micro-batch at the
+    kl_coeff in effect now, then ONE ops.whiten_advantages over the whole rollout with the actor-loss masks
+    `sequence_mask[:, start:]`.  Stores ROLLOUT_ADVANTAGE_KEYS in each training batch for rl_step; row_stats keeps the
+    pre-whitening advantage row means (train/reward_advantage), and the returns stay unwhitened."""
+    for training, mask, start in zip(training_batches, sequence_masks, starts):
+        training.update(zip(ROLLOUT_ADVANTAGE_KEYS, micro_batch_advantages(tr, training, mask, start, returns)))
+    whitened = ops.whiten_advantages([t['advantages'] for t in training_batches],
+                                     [m[:, s:] for m, s in zip(sequence_masks, starts)])
+    for training, adv in zip(training_batches, whitened):
+        training['advantages'] = adv
+
+
 OBJECTIVE_KEYS = ('clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode')
 
 
@@ -294,10 +344,16 @@ class PPOTrainer:
     # train/actor_loss stays the clipped objective, train/actor_kl_loss reports agg(KL).
     kl_loss_coeff = 0.0
     kl_loss_estimator = None
+    # Advantage whitening (TRL's / verl's masked_whiten): rollout() forms every micro-batch's advantages with the
+    # kl_coeff in effect then (K4, and K4r for Multi-PPO's other estimators) and whitens them with ONE mean and std over
+    # the whole rollout's actor-loss mask, on every data-parallel rank (ops.whiten_advantages); rl_step reuses them (all
+    # update_iters).  The returns stay unwhitened, train/reward_advantage stays the pre-whitening row mean.  A bool;
+    # `cfgs.train_cfgs.whiten_advantages` overrides it when set; False leaves rollout and rl_step unchanged.
+    whiten_advantages = False
     # the class attributes above that the grafted methods read: patch.install() copies them onto the reference's classes
     SWITCHES = ('mode', 'fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'clip_range_ratio_low',
                 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode', 'log_clip_fraction', 'kl_estimator',
-                'kl_target', 'kl_horizon', 'kl_loss_coeff', 'kl_loss_estimator')
+                'kl_target', 'kl_horizon', 'kl_loss_coeff', 'kl_loss_estimator', 'whiten_advantages')
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, reward_model=None,
                  reward_critic_model=None, tokenizer=None, reward_tokenizer=None, *, kl_coeff=0.02,
@@ -381,7 +437,8 @@ class PPOTrainer:
     @torch.no_grad()
     def rollout(self, prompt_only_batch):
         """Micro-batched generation + scoring -> (inference_batches, training_batches), the lists the reference's
-        train() loop zips into rl_step (:430-447)."""
+        train() loop zips into rl_step (:430-447); with whiten_advantages, the whitened advantages (whiten_rollout)."""
+        whiten = whiten_advantages_of(self)
         self.set_train(mode=False)
         total = prompt_only_batch['input_ids'].size(0)
         micro = int(self.cfgs.train_cfgs.per_device_train_batch_size)
@@ -394,6 +451,9 @@ class PPOTrainer:
             mini_batch['attention_mask'] = inference['attention_mask']
             inference_batches.append(mini_batch)
             training_batches.append(training)
+        if whiten:
+            whiten_rollout(self, training_batches, [b['attention_mask'][:, 1:] for b in inference_batches],
+                           [t['prompt_idx'] for t in training_batches])
         self.set_train()
         return inference_batches, training_batches
 
@@ -452,7 +512,8 @@ class PPOTrainer:
     # ---- trainers/text_to_text/ppo.py:309-398 -----------------------------------------------
     def rl_step(self, inference_batch, training_batch, returns=None) -> dict[str, Any]:
         """returns: None for K4's GAE advantages and returns, or `returns(old_rewards, sequence_mask, start, row_stats)
-        -> (advantages, returns)`, which also rewrites their metric lanes of row_stats (Multi-PPO's K4r)."""
+        -> (advantages, returns)`, which also rewrites their metric lanes of row_stats (Multi-PPO's K4r).  With
+        whiten_advantages, the rollout's stored tensors instead (step_advantages)."""
         old_log_probs = training_batch['log_probs']
         ref_log_probs = training_batch['ref_log_probs']
         reward = training_batch['reward']
@@ -462,10 +523,8 @@ class PPOTrainer:
         sequence_mask = inference_batch['attention_mask'][:, 1:]
         head = lm_head_of(self.actor_model) if self.fused_lm_head else None  # refusals before any launch
 
-        old_rewards, reward_advantages, reward_returns, row_stats = kl_rewards(
-            self, reward, old_log_probs, ref_log_probs, old_reward_values, sequence_mask, start)
-        if returns is not None:
-            reward_advantages, reward_returns = returns(old_rewards, sequence_mask, start, row_stats)
+        old_rewards, reward_advantages, reward_returns, row_stats = step_advantages(
+            self, training_batch, sequence_mask, start, returns)
 
         actor_loss, actor_loss32, entropy_mean, clip_frac, kl_loss = actor_loss_node(
             self, inference_batch, input_ids, old_log_probs, reward_advantages, sequence_mask, start=start, head=head,

@@ -8,7 +8,7 @@
  * function(s) whose arithmetic it replaces (file:line relative to the reference's
  * align_anything/ directory); the Python mirror in align_anything_b200/ keeps the
  * reference's names and signatures and calls these through ctypes (INTEGRATION.md).
- * 58 entry points, ABI version 3.
+ * 64 entry points, ABI version 3.
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
@@ -51,7 +51,8 @@ enum {
   AA_STATUS_LABEL_OOB = 1,      /* a label outside [0, V): torch.gather would raise           */
   AA_STATUS_SHORT_SEQUENCE = 2, /* fewer non-pad tokens than response_len (dpo.py:135-137)   */
   AA_STATUS_EMPTY_MASK = 4,     /* a mask row with no True: m.nonzero()[-1] would raise       */
-  AA_STATUS_DIVERGE_RANGE = 8   /* simpo.py:72-73 `assert 0 <= diverge_index <= end_index` fails */
+  AA_STATUS_DIVERGE_RANGE = 8,  /* simpo.py:72-73 `assert 0 <= diverge_index <= end_index` fails */
+  AA_STATUS_WHITEN_COUNT = 16   /* fewer than 2 masked advantages to whiten (verl's masked_var raises) */
 };
 
 /* Descriptor of the one-shot NVLink all-reduce fused into the metric-producing kernels (multi-GPU only).
@@ -397,6 +398,29 @@ int aa_ppo_returns(const void *rewards, int rew_dtype, int64_t rew_row_stride, c
                    int64_t mask_row_stride, int32_t B, int32_t W, int32_t start, int estimator,
                    int32_t n_samples_per_prompt, float gamma, int mode, int mask_outputs, void *advantages,
                    void *returns, int out_dtype, float *row_stats, void *stream);
+
+/* ---------------------------------------------------------------------------------------
+ * Advantage whitening over a rollout: TRL's / verl's masked_whiten(A, m, shift_mean=True) over the advantages A
+ * and the actor-loss mask m of EVERY micro-batch of one rollout (and every data-parallel rank):
+ *   n = sum m,  mean = sum m A / n,  var = sum m (A - mean)^2 / (n - 1),
+ *   A' = (A - mean) * rsqrt(var + 1e-8) where m, 0 where not m.
+ * The statistics are fp64; mean and rstd are formed once in fp64 and rounded to fp32; (A - mean) * rstd is fp32,
+ * rounded once to the advantages' dtype.  Every sum has a fixed order (no floating-point atomics): a run gives the
+ * same bits every time.  For K micro-batches:
+ *   aa_whiten_moments x K : micro-batch k's (B, W) advantages (bf16 / f16 / f32, row stride in elements) and
+ *                           torch.bool mask -> its fp64 (n, sum A, sum A^2) in moments[3k .. 3k + 2] of a
+ *                           caller-owned (K, 3) buffer (one CTA per launch)
+ *   aa_whiten_reduce      : total (3,) = the K slots summed in slot order; across ranks the caller all-reduces
+ *                           (SUM) this fixed-size triple before the applies
+ *   aa_whiten_apply x K   : rewrites micro-batch k's advantages in place from `total`.  n < 2 sets
+ *                           AA_STATUS_WHITEN_COUNT in `status` and leaves the advantages unchanged.
+ * ------------------------------------------------------------------------------------- */
+int aa_whiten_moments(const void *advantages, int adv_dtype, int64_t adv_row_stride, const uint8_t *mask,
+                      int64_t mask_row_stride, int32_t B, int32_t W, double *moments, int32_t k, int32_t K,
+                      void *stream);
+int aa_whiten_reduce(const double *moments, int32_t K, double *total, void *stream);
+int aa_whiten_apply(void *advantages, int adv_dtype, int64_t adv_row_stride, const uint8_t *mask,
+                    int64_t mask_row_stride, int32_t B, int32_t W, const double *total, int32_t *status, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * K5  PPO losses, forward AND backward in one launch each (the backward is elementwise).
