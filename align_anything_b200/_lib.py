@@ -139,6 +139,14 @@ _SIGS = {
     'aa_grpo_loss_seq': (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int, _P, _P, c_int64, c_int64, c_int32, c_int32,
                                  c_float, c_float, c_float, c_float, c_int, c_int, c_int, _P, _P, c_int64, _P, _P, _P, _P,
                                  _P]),
+    'aa_grpo_loss_topent': (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int, _P, _P, c_int64, c_int64, c_int32,
+                                    c_int32, c_float, c_float, c_float, c_float, c_int, c_int, c_int, c_int, _P, _P,
+                                    c_int64, _P, _P, c_int64, _P, _P, _P, _P, _P]),
+    'aa_grpo_row_end': (c_int, [_P, c_int64, c_int64, c_int32, c_int32, _P, _P, _P, _P]),
+    'aa_entropy_hist_hi': (c_int, [_P, c_int64, _P, _P, c_int64, c_int32, c_int32, _P, _P]),
+    'aa_entropy_select_hi': (c_int, [_P, c_float, _P, _P]),
+    'aa_entropy_hist_lo': (c_int, [_P, c_int64, _P, _P, c_int64, c_int32, c_int32, _P, _P, _P]),
+    'aa_entropy_select_lo': (c_int, [_P, _P, _P, _P]),
     'aa_nll_mean': (c_int, [_P, c_int, _P, c_int64, c_int64, _P, _P, _P, _P, _P]),
     'aa_masked_mean': (c_int, [_P, c_int, c_int64, _P, c_int64, c_int32, c_int32, _P, _P, _P, _P]),
     'aa_ppo_pack_metrics': (c_int, [_P, _P, _P, _P, _P, c_int32, _P, POINTER(AaColl), _P, _P]),

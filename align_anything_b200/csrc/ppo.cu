@@ -10,6 +10,8 @@
 //                          (trainers/text_to_text/multi_ppo.py:510-591) on K4's shaped rewards.
 //     aa_ppo_pack_metrics: the ten local scalars of :360-381 packed for ONE all-reduce.
 //     aa_whiten_moments / aa_whiten_reduce / aa_whiten_apply: masked_whiten of a rollout's advantages.
+//     aa_grpo_row_end, aa_entropy_hist_hi / _select_hi / _hist_lo / _select_lo: the exact entropy quantile of the
+//                          top-entropy mask, and aa_grpo_loss_topent: GRPO's loss under that mask.
 //
 // These touch ~10 floats per token: latency-bound, not bandwidth-bound.  The point is launch
 // count (thousands -> five) and zero host syncs; each sample is owned by one warp / CTA.
@@ -641,6 +643,11 @@ struct GrpoObjParams {
   int agg;
   float *clip_frac;  // optional fp32[2]; row_scratch then holds 4 * B floats
   int kl_est;        // the per-token KL's estimator (AA_KL_*; aa_grpo_loss_obj: AA_KL_K3)
+  // the top-entropy mask (TOPENT, aa_grpo_loss_topent): the policy's fp32 entropy (row stride ent_stride) and the
+  // device threshold thr[0] of aa_entropy_select_lo; a counted token keeps s iff entropy >= thr
+  const float *entropy;
+  int64_t ent_stride;
+  const float *thr;
 };
 
 // GRPO's loss and d loss / d lp, one block per row, the last block to arrive reduces the rows.  OBJECTIVE: the clipped
@@ -648,10 +655,14 @@ struct GrpoObjParams {
 // (grpo_token, aa_grpo_loss), which passes agg = token-mean, old = clip_frac = nullptr: g_t = 1 / total, the row
 // partial is the fp32 row sum and the loss acc / total, as the reference computes them.  SEQUENCE (with OBJECTIVE,
 // aa_grpo_loss_seq, old != nullptr): GSPO's sequence-level ratio -- the block first folds its row's summed log-ratio,
-// then every token takes the row's objective and ratio coefficient (grpo_seq_row, grpo_seq_token)
-template <int THREADS, bool OBJECTIVE, bool SEQUENCE = false>
+// then every token takes the row's objective and ratio coefficient (grpo_seq_row, grpo_seq_token).  TOPENT (with
+// OBJECTIVE, aa_grpo_loss_topent): the top-entropy mask -- a counted token with entropy < thr keeps only its KL term
+// (keep = 0 in grpo_obj_token; at sequence level s * keep, and s's gradient reaches the row's ratio from the kept
+// tokens alone, n_s of grpo_seq_row)
+template <int THREADS, bool OBJECTIVE, bool SEQUENCE = false, bool TOPENT = false>
 __global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoObjParams q) {
   static_assert(OBJECTIVE || !SEQUENCE, "the sequence-level ratio is an option of the clipped objective");
+  static_assert(OBJECTIVE || !TOPENT, "the top-entropy mask is an option of the clipped objective");
   __shared__ float scratch[33];
   const GrpoParams &p = q.base;
   const int b = blockIdx.x, tid = threadIdx.x, r = p.r_lp;
@@ -659,30 +670,38 @@ __global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoObjParams 
   const float total = p.total[0];
   const float A = p.adv[b];
   const float g_t = grpo_agg_coeff(q.agg, total, static_cast<float>(end), p.B, p.K);
+  float thr = 0.f;
+  if constexpr (TOPENT) thr = *q.thr;
   float row = 0.f, n_clip = 0.f, n_dual = 0.f;
   float s_seq = 0.f, coef_seq = 0.f;
   int why_seq = 0;
   if constexpr (SEQUENCE) {  // the masked-out tokens add (lp - old) * 0: nothing
-    float lr = 0.f;
-    for (int t = tid; t < end; t += THREADS)
+    float lr = 0.f, kept = 0.f;
+    for (int t = tid; t < end; t += THREADS) {
       lr += round_to(load_as_float(p.lp, b * p.lp_stride + t, p.dtype) -
                          load_as_float(q.old, b * q.old_stride + t, p.dtype),
                      r);
+      if constexpr (TOPENT) kept += (q.entropy[b * q.ent_stride + t] >= thr) ? 1.f : 0.f;
+    }
     const float S = round_to(block_sum<THREADS>(lr, scratch), r);
-    grpo_seq_row(S, static_cast<float>(end), A, g_t, q.clip_lo, q.clip_hi, q.dual, r, s_seq, coef_seq, why_seq);
+    float n_s = static_cast<float>(end);
+    if constexpr (TOPENT) n_s = block_sum<THREADS>(kept, scratch);
+    grpo_seq_row(S, static_cast<float>(end), n_s, A, g_t, q.clip_lo, q.clip_hi, q.dual, r, s_seq, coef_seq, why_seq);
   }
   for (int t = tid; t < p.K; t += THREADS) {
     const bool on = t < end;
     const float lp = load_as_float(p.lp, b * p.lp_stride + t, p.dtype);
     const float rf = load_as_float(p.ref_lp, b * p.ref_stride + t, p.dtype);
+    float keep = 1.f;
+    if constexpr (TOPENT) keep = (on && q.entropy[b * q.ent_stride + t] >= thr) ? 1.f : 0.f;
     float ptl, g;
     int why = 0;
     if constexpr (SEQUENCE) {
-      grpo_seq_token(lp, rf, s_seq, coef_seq, on, g_t, p.beta, q.kl_est, r, ptl, g);
+      grpo_seq_token(lp, rf, s_seq * keep, coef_seq, on, g_t, p.beta, q.kl_est, r, ptl, g);
       why = why_seq;
     } else if constexpr (OBJECTIVE) {
       const float old = q.old ? load_as_float(q.old, b * q.old_stride + t, p.dtype) : lp;
-      grpo_obj_token(lp, old, rf, A, on, g_t, p.beta, q.clip_lo, q.clip_hi, q.dual, q.kl_est, r, ptl, g, why);
+      grpo_obj_token(lp, old, rf, A, on, g_t, p.beta, q.clip_lo, q.clip_hi, q.dual, q.kl_est, r, ptl, g, why, keep);
     } else {
       grpo_token(lp, rf, A, on, g_t, p.beta, r, ptl, g);
     }
@@ -816,6 +835,168 @@ __global__ void __launch_bounds__(32)
 
 __global__ void __launch_bounds__(32) allreduce_packed_kernel(const float *src, float *dst, int n, CollParams coll) {
   p2p_allreduce_packed(coll, src, dst, n);
+}
+
+// ---- top-entropy token masking: the exact entropy quantile (TRL's top_entropy_quantile) ------------------------------
+// thr = torch.quantile(H[counted], q) over every counted token of every rank, without a host sync: a radix select on
+// order-preserving uint32 keys, 16 bits at a time.  aa_entropy_hist_hi counts the keys' high halves (and the NaNs),
+// aa_entropy_select_hi finds the count N, the two ranks lo = floor(rank) and hi = ceil(rank) of rank = q * (N - 1) in
+// fp32, and the high-half bucket of each; aa_entropy_hist_lo counts the low halves inside those one or two buckets and
+// aa_entropy_select_lo reads the two values off and interpolates as ATen's lerp.  The histograms are integer counts, so
+// the caller's all_reduce(SUM) between the passes gives every rank the same bits in any order.
+constexpr int kEntBins = 1 << 16;         // bins of one 16-bit half
+constexpr int kEntSelectThreads = 1024;   // one block scans the 2^16 bins, 64 per thread
+constexpr uint32_t kEntSkip = 0xffffffffu;
+
+// the float order as an unsigned order: -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf (NaNs are counted apart)
+__device__ __forceinline__ uint32_t entropy_key(float x) {
+  const uint32_t u = __float_as_uint(x);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+__device__ __forceinline__ float entropy_key_value(uint32_t k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+// sel[] of aa_entropy_select_hi: N, the NaN count, (bucket, rank inside it) of lo and of hi, and the weight's bits
+enum { kSelN = 0, kSelNan, kSelLoBucket, kSelLoRank, kSelHiBucket, kSelHiRank, kSelWeight, kSelWords = 8 };
+
+// HI: bin = the key's high half, or kEntBins for a NaN.  LO: the low half of a key whose high half is the lo bucket
+// (bins [0, 2^16)) or else the hi bucket (bins [2^16, 2^17)); nothing when the select has no value to find.  One warp
+// folds equal bins (__match_any_sync) into one integer atomic.  counted: t < row_end[b], or mask[b, t] != 0.
+template <bool LO>
+__global__ void __launch_bounds__(256)
+    entropy_hist_kernel(const float *__restrict__ entropy, int64_t ent_stride, const int32_t *__restrict__ row_end,
+                        const uint8_t *__restrict__ mask, int64_t mask_stride, int B, int K,
+                        const uint32_t *__restrict__ sel, uint32_t *__restrict__ hist) {
+  uint32_t lo_bucket = 0, hi_bucket = 0;
+  if constexpr (LO) {
+    if (sel[kSelN] == 0u || sel[kSelNan] != 0u) return;
+    lo_bucket = sel[kSelLoBucket];
+    hi_bucket = sel[kSelHiBucket];
+  }
+  const int64_t n = static_cast<int64_t>(B) * K;
+  const int lane = threadIdx.x & (kWarp - 1);
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t base = static_cast<int64_t>(blockIdx.x) * blockDim.x + (threadIdx.x & ~(kWarp - 1)); base < n;
+       base += stride) {
+    const int64_t i = base + lane;
+    uint32_t bin = kEntSkip;
+    if (i < n) {
+      const int b = static_cast<int>(i / K), t = static_cast<int>(i - static_cast<int64_t>(b) * K);
+      const bool counted = mask ? mask[b * mask_stride + t] != 0 : t < row_end[b];
+      if (counted) {
+        const float h = entropy[b * ent_stride + t];
+        if constexpr (!LO) {
+          bin = (h != h) ? static_cast<uint32_t>(kEntBins) : entropy_key(h) >> 16;
+        } else if (h == h) {
+          const uint32_t k = entropy_key(h);
+          if ((k >> 16) == lo_bucket)
+            bin = k & 0xffffu;
+          else if ((k >> 16) == hi_bucket)
+            bin = kEntBins + (k & 0xffffu);
+        }
+      }
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, bin);
+    if (bin != kEntSkip && lane == __ffs(peers) - 1) atomicAdd(&hist[bin], static_cast<uint32_t>(__popc(peers)));
+  }
+}
+
+// The whole block: the bin of h[0 .. 2^16) that holds rank r (0-based, r < the bins' sum) and r's rank inside it, to
+// *bin / *rank_in (shared).  Also returns the bins' sum to every thread.
+__device__ __forceinline__ uint32_t entropy_find_rank(const uint32_t *__restrict__ h, uint32_t r, uint32_t *bin, uint32_t *rank_in,
+                                      uint32_t *warp_tot) {
+  const int tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid >> 5;
+  constexpr int per = kEntBins / kEntSelectThreads;
+  const uint32_t *mine = h + tid * per;
+  uint32_t s = 0;
+#pragma unroll 8
+  for (int j = 0; j < per; ++j) s += mine[j];
+  uint32_t inc = s;  // inclusive scan: lanes, then warps
+  for (int d = 1; d < kWarp; d <<= 1) {
+    const uint32_t v = __shfl_up_sync(0xffffffffu, inc, d);
+    if (lane >= d) inc += v;
+  }
+  __syncthreads();  // warp_tot may still be read by a previous call
+  if (lane == kWarp - 1) warp_tot[warp] = inc;
+  __syncthreads();
+  uint32_t before = 0, all = 0;
+#pragma unroll 4
+  for (int w = 0; w < kEntSelectThreads / kWarp; ++w) {
+    const uint32_t v = warp_tot[w];
+    before += (w < warp) ? v : 0u;
+    all += v;
+  }
+  const uint32_t excl = before + inc - s;
+  if (r >= excl && r - excl < s) {
+    uint32_t c = excl;
+#pragma unroll 1
+    for (int j = 0; j < per; ++j) {
+      if (r - c < mine[j]) {
+        *bin = static_cast<uint32_t>(tid * per + j);
+        *rank_in = r - c;
+        break;
+      }
+      c += mine[j];
+    }
+  }
+  __syncthreads();
+  return all;
+}
+
+// One block: N, the two ranks and their high-half buckets (sel[]).  rank = q * (N - 1) as ATen's quantile forms it
+// (fp32 q times the count, rounded once), lo = floor(rank), hi = ceil(rank), both at most N - 1; weight = rank - lo.
+__global__ void __launch_bounds__(kEntSelectThreads)
+    entropy_select_hi_kernel(const uint32_t *__restrict__ hist, float q, uint32_t *__restrict__ sel) {
+  __shared__ uint32_t warp_tot[kEntSelectThreads / kWarp];
+  __shared__ uint32_t res[4];
+  const int tid = threadIdx.x;
+  const uint32_t N = entropy_find_rank(hist, 0xffffffffu, &res[0], &res[1], warp_tot);  // the sum alone
+  if (N == 0u) {
+    if (tid < kSelWords) sel[tid] = (tid == kSelNan) ? hist[kEntBins] : 0u;
+    return;
+  }
+  const float rank = q * static_cast<float>(N - 1u);
+  const double rk = static_cast<double>(rank);
+  const uint32_t lo = rk >= static_cast<double>(N - 1u) ? N - 1u : static_cast<uint32_t>(rk);
+  const double ce = ceil(rk);
+  const uint32_t hi = ce >= static_cast<double>(N - 1u) ? N - 1u : static_cast<uint32_t>(ce);
+  entropy_find_rank(hist, lo, &res[0], &res[1], warp_tot);
+  entropy_find_rank(hist, hi, &res[2], &res[3], warp_tot);
+  if (tid == 0) {
+    sel[kSelN] = N;
+    sel[kSelNan] = hist[kEntBins];
+    sel[kSelLoBucket] = res[0];
+    sel[kSelLoRank] = res[1];
+    sel[kSelHiBucket] = res[2];
+    sel[kSelHiRank] = res[3];
+    sel[kSelWeight] = __float_as_uint(rank - static_cast<float>(lo));
+    sel[7] = 0u;
+  }
+}
+
+// One block: the two values and thr = lerp(v_lo, v_hi, w) as ATen's lerp forms it (w < 0.5: v_lo + w * (v_hi - v_lo),
+// else v_hi - (v_hi - v_lo) * (1 - w), each a fused multiply-add); NaN when a counted entropy is NaN, and when nothing
+// is counted (then no token is kept).
+__global__ void __launch_bounds__(kEntSelectThreads)
+    entropy_select_lo_kernel(const uint32_t *__restrict__ hist, const uint32_t *__restrict__ sel, float *thr) {
+  __shared__ uint32_t warp_tot[kEntSelectThreads / kWarp];
+  __shared__ uint32_t res[4];
+  if (sel[kSelN] == 0u || sel[kSelNan] != 0u) {
+    if (threadIdx.x == 0) thr[0] = __uint_as_float(0x7fc00000u);
+    return;
+  }
+  const uint32_t lo_b = sel[kSelLoBucket], hi_b = sel[kSelHiBucket];
+  entropy_find_rank(hist, sel[kSelLoRank], &res[0], &res[1], warp_tot);
+  entropy_find_rank(hist + (hi_b == lo_b ? 0 : kEntBins), sel[kSelHiRank], &res[2], &res[3], warp_tot);
+  if (threadIdx.x == 0) {
+    const float v_lo = entropy_key_value((lo_b << 16) | res[0]);
+    const float v_hi = entropy_key_value((hi_b << 16) | res[2]);
+    const float w = __uint_as_float(sel[kSelWeight]);
+    const float d = v_hi - v_lo;
+    thr[0] = (fabsf(w) < 0.5f) ? fmaf(w, d, v_lo) : fmaf(-d, 1.f - w, v_hi);
+  }
 }
 
 // ---- advantage whitening over a rollout (TRL's / verl's masked_whiten, shift_mean=True) -----------------------------
@@ -1144,13 +1325,17 @@ static int grpo_loss(const char *who, bool objective, const void *log_probs, int
                      const float *advantages, const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id,
                      int32_t B, int32_t K, float beta, float clip_low, float clip_high, float dual_clip, int loss_agg,
                      int kl_estimator, int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac,
-                     int32_t *row_end, float *scratch, uint32_t *counter, void *stream, bool sequence = false) {
+                     int32_t *row_end, float *scratch, uint32_t *counter, void *stream, bool sequence = false,
+                     bool topent = false, const float *entropy = nullptr, int64_t ent_stride = 0,
+                     const float *thr = nullptr) {
   AA_REQUIRE(B > 0 && K > 0 && log_probs && ref_log_probs && advantages && completion_tokens && loss && row_end &&
                  scratch && counter,
              AA_ERR_ARG, "%s: bad arguments", who);
   AA_REQUIRE(dtype_ok(lp_dtype), AA_ERR_DTYPE, "%s: bad dtype", who);
   AA_REQUIRE(!sequence || old_log_probs, AA_ERR_ARG,
              "%s: the sequence-level ratio needs old_log_probs (without them w = 1: use aa_grpo_loss_kl)", who);
+  AA_REQUIRE(!topent || (entropy && thr && ent_stride >= K), AA_ERR_ARG,
+             "%s: the top-entropy mask needs entropy (row stride >= K) and thr", who);
   if (objective) {
     AA_REQUIRE(grpo_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
                "%s: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a known loss_agg; got "
@@ -1165,8 +1350,13 @@ static int grpo_loss(const char *who, bool objective, const void *log_probs, int
   GrpoObjParams q{GrpoParams{log_probs, ref_log_probs, lp_dtype, lp_stride, ref_stride, advantages, row_end, scratch, B,
                              K, beta, (mode == AA_MODE_FAITHFUL) ? lp_dtype : AA_F32, loss, grad, grad_stride,
                              scratch + 1, counter + 1},
-                  old_log_probs, old_stride, clip_low, clip_high, dual_clip, loss_agg, clip_frac, kl_estimator};
-  if (sequence)
+                  old_log_probs, old_stride, clip_low, clip_high, dual_clip, loss_agg, clip_frac, kl_estimator,
+                  entropy, ent_stride, thr};
+  if (topent && sequence)
+    grpo_loss_kernel<128, true, true, true><<<B, 128, 0, st>>>(q);
+  else if (topent)
+    grpo_loss_kernel<128, true, false, true><<<B, 128, 0, st>>>(q);
+  else if (sequence)
     grpo_loss_kernel<128, true, true><<<B, 128, 0, st>>>(q);
   else if (objective)
     grpo_loss_kernel<128, true><<<B, 128, 0, st>>>(q);
@@ -1228,6 +1418,85 @@ extern "C" int aa_grpo_loss_seq(const void *log_probs, int64_t lp_stride, const 
                    lp_dtype, advantages, completion_tokens, tok_stride, eos_id, B, K, beta, clip_low, clip_high,
                    dual_clip, loss_agg, kl_estimator, mode, loss, grad, grad_stride, clip_frac, row_end, scratch,
                    counter, stream, true);
+}
+
+extern "C" int aa_grpo_loss_topent(const void *log_probs, int64_t lp_stride, const void *ref_log_probs,
+                                   int64_t ref_stride, const void *old_log_probs, int64_t old_stride, int lp_dtype,
+                                   const float *advantages, const int64_t *completion_tokens, int64_t tok_stride,
+                                   int64_t eos_id, int32_t B, int32_t K, float beta, float clip_low, float clip_high,
+                                   float dual_clip, int loss_agg, int kl_estimator, int sequence, int mode, float *loss,
+                                   void *grad, int64_t grad_stride, float *clip_frac, const float *entropy,
+                                   int64_t ent_stride, const float *thr, int32_t *row_end, float *scratch,
+                                   uint32_t *counter, void *stream) {
+  AA_REQUIRE(sequence == 0 || sequence == 1, AA_ERR_ARG, "aa_grpo_loss_topent: sequence must be 0 or 1, got %d",
+             sequence);
+  return grpo_loss("aa_grpo_loss_topent", true, log_probs, lp_stride, ref_log_probs, ref_stride, old_log_probs,
+                   old_stride, lp_dtype, advantages, completion_tokens, tok_stride, eos_id, B, K, beta, clip_low,
+                   clip_high, dual_clip, loss_agg, kl_estimator, mode, loss, grad, grad_stride, clip_frac, row_end,
+                   scratch, counter, stream, sequence == 1, true, entropy, ent_stride, thr);
+}
+
+extern "C" int aa_grpo_row_end(const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B,
+                               int32_t K, int32_t *row_end, float *total, uint32_t *counter, void *stream) {
+  AA_REQUIRE(B > 0 && K > 0 && completion_tokens && row_end && total && counter, AA_ERR_ARG,
+             "aa_grpo_row_end: bad arguments");
+  grpo_mask_kernel<128><<<B, 128, 0, static_cast<cudaStream_t>(stream)>>>(completion_tokens, tok_stride, B, K, eos_id,
+                                                                          row_end, total, counter);
+  return check_launch("aa_grpo_row_end");
+}
+
+// the checks both histogram passes share: exactly one of row_end / mask, sizes and strides
+static int entropy_hist_args(const char *who, const float *entropy, int64_t ent_stride, const int32_t *row_end,
+                             const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t K, const uint32_t *hist) {
+  AA_REQUIRE(entropy && hist, AA_ERR_ARG, "%s: null pointer", who);
+  AA_REQUIRE((row_end != nullptr) != (mask != nullptr), AA_ERR_ARG, "%s: give exactly one of row_end and mask", who);
+  AA_REQUIRE(B > 0 && K > 0 && static_cast<int64_t>(B) * K <= INT32_MAX, AA_ERR_ARG, "%s: bad sizes (B=%d K=%d)", who,
+             B, K);
+  AA_REQUIRE(ent_stride >= K && (!mask || mask_stride >= K), AA_ERR_ARG, "%s: row strides must be >= K", who);
+  return AA_OK;
+}
+
+static unsigned entropy_hist_grid(int32_t B, int32_t K) {
+  const int64_t blocks = (static_cast<int64_t>(B) * K + 255) / 256;
+  return static_cast<unsigned>(blocks < 1024 ? blocks : 1024);
+}
+
+extern "C" int aa_entropy_hist_hi(const float *entropy, int64_t ent_stride, const int32_t *row_end,
+                                  const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t K, uint32_t *hist,
+                                  void *stream) {
+  int rc = entropy_hist_args("aa_entropy_hist_hi", entropy, ent_stride, row_end, mask, mask_stride, B, K, hist);
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaMemsetAsync(hist, 0, sizeof(uint32_t) * (kEntBins + 1), st);
+  entropy_hist_kernel<false><<<entropy_hist_grid(B, K), 256, 0, st>>>(entropy, ent_stride, row_end, mask, mask_stride,
+                                                                      B, K, nullptr, hist);
+  return check_launch("aa_entropy_hist_hi");
+}
+
+extern "C" int aa_entropy_select_hi(const uint32_t *hist, float q, uint32_t *sel, void *stream) {
+  AA_REQUIRE(hist && sel, AA_ERR_ARG, "aa_entropy_select_hi: null pointer");
+  AA_REQUIRE(q >= 0.f && q <= 1.f, AA_ERR_ARG, "aa_entropy_select_hi: q must lie in [0, 1], got %g", q);
+  entropy_select_hi_kernel<<<1, kEntSelectThreads, 0, static_cast<cudaStream_t>(stream)>>>(hist, q, sel);
+  return check_launch("aa_entropy_select_hi");
+}
+
+extern "C" int aa_entropy_hist_lo(const float *entropy, int64_t ent_stride, const int32_t *row_end,
+                                  const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t K, const uint32_t *sel,
+                                  uint32_t *hist, void *stream) {
+  int rc = entropy_hist_args("aa_entropy_hist_lo", entropy, ent_stride, row_end, mask, mask_stride, B, K, hist);
+  if (rc) return rc;
+  AA_REQUIRE(sel, AA_ERR_ARG, "aa_entropy_hist_lo: null pointer");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaMemsetAsync(hist, 0, sizeof(uint32_t) * 2 * kEntBins, st);
+  entropy_hist_kernel<true><<<entropy_hist_grid(B, K), 256, 0, st>>>(entropy, ent_stride, row_end, mask, mask_stride,
+                                                                     B, K, sel, hist);
+  return check_launch("aa_entropy_hist_lo");
+}
+
+extern "C" int aa_entropy_select_lo(const uint32_t *hist, const uint32_t *sel, float *thr, void *stream) {
+  AA_REQUIRE(hist && sel && thr, AA_ERR_ARG, "aa_entropy_select_lo: null pointer");
+  entropy_select_lo_kernel<<<1, kEntSelectThreads, 0, static_cast<cudaStream_t>(stream)>>>(hist, sel, thr);
+  return check_launch("aa_entropy_select_lo");
 }
 
 extern "C" int aa_nll_mean(const void *logp, int dtype, const int64_t *labels, int64_t n, int64_t ignore_index,

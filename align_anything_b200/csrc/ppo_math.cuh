@@ -183,14 +183,16 @@ __device__ __forceinline__ float grpo_agg_coeff(int agg, float total, float cnt,
 // order (the ratio is created after the KL, as the reference creates its exp(lp - lp.detach()) term).  est: the KL
 // estimator (AA_KL_K3 is the reference's; kl_value / kl_grad).
 //   why: actor_token's clip-fraction bits
+// keep: the top-entropy mask (aa_grpo_loss_topent), 1 or 0: the per-token loss is -(s * keep - beta * KL), so a
+// masked token (keep 0) carries the KL term alone and s sends it no gradient; the clip-fraction bits stay the token's
 __device__ __forceinline__ void grpo_obj_token(float lp, float old, float rf, float A, bool on, float g_t, float beta,
                                                float eps_lo, float eps_hi, float dual, int est, int r, float &ptl,
-                                               float &grad, int &why) {
+                                               float &grad, int &why, float keep = 1.f) {
   float s, ga, aux;
-  actor_token(lp, old, A, on, -g_t, eps_lo, eps_hi, dual, r, AA_F32, AA_F32, s, ga, why);
+  actor_token(lp, old, A, on, -g_t * keep, eps_lo, eps_hi, dual, r, AA_F32, AA_F32, s, ga, why);
   const float kl = kl_value(lp, rf, est, r, aux);
   const float bk = round_to(beta * kl, r);
-  ptl = -(s - bk);
+  ptl = -(s * keep - bk);
   grad = 0.f;
   if (on) grad = kl_grad(ga, round_to(round_to(g_t, r) * beta, r), est, aux, r);
 }
@@ -202,11 +204,13 @@ __device__ __forceinline__ void grpo_obj_token(float lp, float old, float rf, fl
 // g_t: d loss / d per-token loss of a counted token (grpo_agg_coeff), so d loss / d s = -n * g_t, the sum of the
 // row's per-token coefficients.  coef = d loss / d lp_t through the ratio, the same for every masked-in token:
 // ExpBackward (gs * w), DivBackward by n, cast once to `r` at the backward of the sum.  why: clipped_ratio's bits.
-__device__ __forceinline__ void grpo_seq_row(float S, float n, float A, float g_t, float eps_lo, float eps_hi,
-                                             float dual, int r, float &s, float &coef, int &why) {
+// n_s: the counted tokens whose per-token loss takes s -- n, or under the top-entropy mask the row's kept tokens, so
+// d loss / d s = -n_s * g_t while the ratio's gradient still reaches every counted token through the row's mean.
+__device__ __forceinline__ void grpo_seq_row(float S, float n, float n_s, float A, float g_t, float eps_lo,
+                                             float eps_hi, float dual, int r, float &s, float &coef, int &why) {
   const float w = expf(S / n);
   float gs;
-  clipped_ratio(w, 1.f - eps_lo, 1.f + eps_hi, A, true, -(n * g_t), dual, AA_F32, AA_F32, AA_F32, s, gs, why);
+  clipped_ratio(w, 1.f - eps_lo, 1.f + eps_hi, A, true, -(n_s * g_t), dual, AA_F32, AA_F32, AA_F32, s, gs, why);
   coef = round_to((gs * w) / n, r);
 }
 

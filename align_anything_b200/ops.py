@@ -1260,14 +1260,14 @@ class _GrpoLossFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj=None, old=None, clip_frac=None,
-                sequence=False):
+                sequence=False, topent=None):
         B, K = lp.shape
         dev = lp.device
         loss = torch.empty(1, dtype=torch.float32, device=dev)
         grad = torch.empty((B, K), dtype=lp.dtype, device=dev)
         row_end = torch.empty(B, dtype=torch.int32, device=dev)
         _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
-                          sequence=sequence)
+                          sequence=sequence, topent=topent)
         ctx.save_for_backward(grad)
         ctx.mark_non_differentiable(row_end)
         return loss[0], row_end
@@ -1275,15 +1275,16 @@ class _GrpoLossFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g, _):
         (grad,) = ctx.saved_tensors
-        return (grad.float() * g.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None, None
+        return (grad.float() * g.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None, None, None
 
 
 def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
-                      scratch=None, sequence=False):
+                      scratch=None, sequence=False, topent=None):
     """GRPO's loss kernel, writing loss, row_end and (unless None) grad.  obj None: the reference loss (aa_grpo_loss);
     otherwise obj = _grpo_objective_args(...) for aa_grpo_loss_obj (aa_grpo_loss_kl unless the KL is k3), old = the old log-probs (None: the log-probs
     themselves, ratio 1) and clip_frac = an fp32[2] tensor for the clip fractions or None.  sequence (see
-    _sequence_level; old is then given): GSPO's sequence-level ratio, aa_grpo_loss_seq.  scratch (fp32): the token
+    _sequence_level; old is then given): GSPO's sequence-level ratio, aa_grpo_loss_seq.  topent: (entropy (B, K) fp32,
+    thr fp32[1]) for the top-entropy mask, aa_grpo_loss_topent at either level (obj is then given).  scratch (fp32): the token
     count and the row sums, B + 1 values, and under the objective the rows' clip counts too, 1 + 4 B; None allocates it."""
     B, K = lp.shape
     dev = lp.device
@@ -1296,6 +1297,11 @@ def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old
     tail = (row_end.data_ptr(), scratch.data_ptr(), _device_scratch(dev)['counter'][5:7].data_ptr(), L.stream_ptr(dev))
     if obj is None:
         L.check(lib.aa_grpo_loss(*lps, *rows, mode_code, *out, *tail))
+    elif topent is not None:
+        ent, thr = topent
+        L.check(lib.aa_grpo_loss_topent(*lps, L.ptr(old), old.stride(0) if old is not None else 0, *rows, *obj,
+                                        int(bool(sequence)), mode_code, *out, L.ptr(clip_frac), ent.data_ptr(),
+                                        ent.stride(0), thr.data_ptr(), *tail))
     elif sequence:
         L.check(lib.aa_grpo_loss_seq(*lps, old.data_ptr(), old.stride(0), *rows, *obj, mode_code, *out,
                                      L.ptr(clip_frac), *tail))
@@ -1327,6 +1333,101 @@ def _sequence_level(objective, old) -> bool:
     return old is not None and getattr(objective, 'sequence_level', False)
 
 
+def _top_entropy(objective) -> bool:
+    """Whether the top-entropy mask runs (top_entropy_quantile < 1).  Every token's gradient needs the global entropy
+    threshold first, so it runs on the composed path (selection -> aa_grpo_loss_topent), never on K1f's single pass."""
+    return getattr(objective, 'top_entropy_quantile', 1.0) < 1.0
+
+
+def grpo_row_end(completion_tokens: torch.Tensor, eos_token_id: int) -> torch.Tensor:
+    """GRPO's completion mask as counted tokens per row: int32 (B,), row_end[b] = the tokens up to and including the
+    first eos (K without one).  The GRPO loss kernels' own mask pass (aa_grpo_row_end), one launch."""
+    L.require_cuda(completion_tokens)
+    if completion_tokens.dim() != 2 or completion_tokens.numel() == 0:
+        raise ValueError(f'completion tokens must be a non-empty (B, K) tensor, got {tuple(completion_tokens.shape)}')
+    tok = _contiguous_last(completion_tokens.to(torch.int64))
+    B, K = tok.shape
+    dev = tok.device
+    row_end = torch.empty(B, dtype=torch.int32, device=dev)
+    total = torch.empty(1, dtype=torch.float32, device=dev)
+    L.check(L.lib().aa_grpo_row_end(tok.data_ptr(), tok.stride(0), int(eos_token_id), B, K, row_end.data_ptr(),
+                                    total.data_ptr(), _device_scratch(dev)['counter'][5:6].data_ptr(),
+                                    L.stream_ptr(dev)))
+    return row_end
+
+
+_ENT_BINS = 1 << 16  # include/aa_b200.h aa_entropy_hist_hi / _lo: 16 bits a pass
+
+
+def entropy_quantile_threshold(entropy: torch.Tensor, row_end_or_mask: torch.Tensor, q: float,
+                               group=None) -> torch.Tensor:
+    """torch.quantile(entropy[counted], q) (linear interpolation) over the counted tokens of every rank of `group`
+    (torch.distributed; None: the default group) when torch.distributed is initialised with more than one rank, else
+    over the local ones -> fp32 (1,) on the device.  entropy: fp32 (B, K); row_end_or_mask: int (B,) counted tokens per
+    row (t < row_end[b], GRPO's completion mask: grpo_row_end) or a bool / integer (B, K) mask.  NaN when nothing is
+    counted or a counted entropy is NaN (then `entropy >= thr` keeps nothing).
+    Exact: a radix select on order-preserving keys, 16 bits a pass (aa_entropy_hist_hi, aa_entropy_select_hi,
+    aa_entropy_hist_lo, aa_entropy_select_lo), the rank fp32 q * (N - 1) and ATen's lerp, so the value equals CUDA
+    torch.quantile's wherever that accepts the input (up to 2^24 values) and keeps its formula beyond.  Across ranks
+    the two histograms (integer counts) are all-reduced with SUM; no host sync.  Bad arguments raise ValueError here,
+    before any launch."""
+    if isinstance(q, bool) or not isinstance(q, (int, float)) or not 0.0 <= float(q) <= 1.0:
+        raise ValueError(f'entropy_quantile_threshold: q must be a number in [0, 1], got {q!r}')
+    if not isinstance(entropy, torch.Tensor) or entropy.dim() != 2 or entropy.numel() == 0 or \
+            entropy.dtype != torch.float32:
+        raise ValueError(f'entropy_quantile_threshold: entropy must be a non-empty fp32 (B, K) tensor, got '
+                         f'{getattr(entropy, "dtype", None)} {tuple(getattr(entropy, "shape", ()))}')
+    B, K = entropy.shape
+    if B * K > 2 ** 31 - 1:
+        raise ValueError(f'entropy_quantile_threshold: B * K = {B * K} exceeds 2^31 - 1')
+    m = row_end_or_mask
+    if not isinstance(m, torch.Tensor) or tuple(m.shape) not in ((B,), (B, K)) or \
+            (m.dim() == 1 and (m.dtype.is_floating_point or m.dtype == torch.bool)):
+        raise ValueError(f'entropy_quantile_threshold: row_end_or_mask must be integer (B,) = ({B},) row ends or a '
+                         f'(B, K) = ({B}, {K}) mask, got {getattr(m, "dtype", None)} {tuple(getattr(m, "shape", ()))}')
+    try:
+        L.require_cuda(entropy, m)
+    except RuntimeError as e:
+        raise ValueError(f'entropy_quantile_threshold: {e}') from None
+    dev = entropy.device
+    ent = _contiguous_last(entropy.detach())
+    if m.dim() == 1:
+        row_end, mask, mask_stride = m.to(torch.int32).contiguous(), None, 0
+    else:
+        row_end, mask = None, _contiguous_last((m != 0).to(torch.uint8))
+        mask_stride = mask.stride(0)
+    hist_hi = torch.empty(_ENT_BINS + 1, dtype=torch.int32, device=dev)  # uint32 counts; + the NaN count
+    hist_lo = torch.empty(2 * _ENT_BINS, dtype=torch.int32, device=dev)
+    sel = torch.empty(8, dtype=torch.int32, device=dev)
+    thr = torch.empty(1, dtype=torch.float32, device=dev)
+    lib, stream = L.lib(), L.stream_ptr(dev)
+    counted = (L.ptr(row_end), L.ptr(mask), mask_stride, B, K)
+    dist = torch.distributed
+    many = dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1
+    L.check(lib.aa_entropy_hist_hi(ent.data_ptr(), ent.stride(0), *counted, hist_hi.data_ptr(), stream))
+    if many:
+        dist.all_reduce(hist_hi, op=dist.ReduceOp.SUM, group=group)
+    L.check(lib.aa_entropy_select_hi(hist_hi.data_ptr(), float(q), sel.data_ptr(), stream))
+    L.check(lib.aa_entropy_hist_lo(ent.data_ptr(), ent.stride(0), *counted, sel.data_ptr(), hist_lo.data_ptr(), stream))
+    if many:
+        dist.all_reduce(hist_lo, op=dist.ReduceOp.SUM, group=group)
+    L.check(lib.aa_entropy_select_lo(hist_lo.data_ptr(), sel.data_ptr(), thr.data_ptr(), stream))
+    return thr
+
+
+def _top_entropy_args(objective, entropy, tok, eos_token_id, shape):
+    """(entropy, thr) of the top-entropy mask for _grpo_loss_launch, or None when the objective keeps every token.
+    thr: entropy_quantile_threshold at q = 1 - top_entropy_quantile over GRPO's completion mask."""
+    if not _top_entropy(objective):
+        return None
+    if not isinstance(entropy, torch.Tensor) or tuple(entropy.shape) != tuple(shape):
+        raise ValueError(f'top_entropy_quantile < 1 needs the policy entropy, a {tuple(shape)} tensor; got '
+                         f'{tuple(getattr(entropy, "shape", ())) if entropy is not None else None}')
+    ent = _contiguous_last(entropy.detach().float())
+    thr = entropy_quantile_threshold(ent, grpo_row_end(tok, eos_token_id), 1.0 - objective.top_entropy_quantile)
+    return ent, thr
+
+
 def _old_log_probs(old, shape, dtype):
     """The rollout-time policy log-probs for the objective kernels: detached, contiguous, in the log-probs' dtype."""
     if old is None:
@@ -1339,14 +1440,17 @@ def _old_log_probs(old, shape, dtype):
 def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, advantages: torch.Tensor,
               completion_tokens: torch.Tensor, eos_token_id: int, beta: float, mode: str | None = None, *,
               objective: GrpoObjective | None = None, old_per_token_logps: torch.Tensor | None = None,
-              return_clip_fraction: bool = False):
+              return_clip_fraction: bool = False, entropy: torch.Tensor | None = None):
     """The loss of GRPOTrainer.train_step (trainers/text_to_text/grpo.py:290-312): per-token k3 KL, per-token loss
     -(exp(lp - lp.detach()) * A - beta * KL), completion mask up to the first eos, token mean -> fp32 scalar,
     differentiable in per_token_logps.  Returns (loss, counted_tokens_per_row).
     objective (ops.GrpoObjective) / old_per_token_logps (the rollout-time policy log-probs, (B, K)): GRPO's clipped
     objective (aa_grpo_loss_obj) with ratio exp(lp - old); without old_per_token_logps the ratio is 1.  A sequence-level
     objective with old_per_token_logps: GSPO's one ratio per sequence (aa_grpo_loss_seq).  None / default fields and no
-    old log-probs: today's launch.  return_clip_fraction appends the fp32[2] clip fractions."""
+    old log-probs: today's launch.  return_clip_fraction appends the fp32[2] clip fractions.
+    An objective with top_entropy_quantile = rho < 1 also needs `entropy`, the policy's fp32 entropy (B, K) of the same
+    pass: only the counted tokens with entropy >= entropy_quantile_threshold(entropy, row_end, 1 - rho) (over every
+    data-parallel rank) keep the policy term s; the others carry the KL term alone (aa_grpo_loss_topent)."""
     L.require_cuda(per_token_logps, ref_per_token_logps, advantages, completion_tokens)
     obj = _grpo_objective_args(objective, old_per_token_logps, return_clip_fraction)
     if per_token_logps.dim() != 2 or per_token_logps.shape != ref_per_token_logps.shape or \
@@ -1360,8 +1464,9 @@ def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, 
     old = _old_log_probs(old_per_token_logps, lp.shape, lp.dtype)
     tok = _contiguous_last(completion_tokens.to(torch.int64))
     cf = torch.zeros(2, dtype=torch.float32, device=lp.device) if return_clip_fraction else None
+    topent = _top_entropy_args(objective, entropy, tok, eos_token_id, lp.shape)
     out = _GrpoLossFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype), obj, old, cf,
-                            _sequence_level(objective, old))
+                            _sequence_level(objective, old), topent)
     return out + (cf,) if return_clip_fraction else out
 
 
@@ -1477,25 +1582,27 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
     composed path K1's entropy variant -> grpo_loss -> K1b's entropy variant.
     objective / old_per_token_logps: GRPO's clipped objective as in grpo_loss (K1f's objective entry point, or K1 ->
     aa_grpo_loss_obj -> K1b); the entropy bonus stays a token mean over the completion mask.  A sequence-level objective
-    with old log-probs always takes the composed path (K1 -> aa_grpo_loss_seq -> K1b, see _sequence_level).
-    return_clip_fraction appends the fp32[2] clip fractions last.  None / default fields and no old log-probs: today's
+    with old log-probs always takes the composed path (K1 -> aa_grpo_loss_seq -> K1b, see _sequence_level), and so does
+    top_entropy_quantile < 1 (K1's entropy variant -> the entropy threshold -> aa_grpo_loss_topent -> K1b, see
+    _top_entropy).  return_clip_fraction appends the fp32[2] clip fractions last.  None / default fields and no old log-probs: today's
     launches."""
     L.require_cuda(logits, input_ids, ref_per_token_logps, advantages)
     obj = _grpo_objective_args(objective, old_per_token_logps, return_clip_fraction)
     K = int(logits_to_keep)
     tokens = input_ids[:, -K:]
     coeff = float(entropy_coeff)
-    if _sequence_level(objective, old_per_token_logps) or \
+    topent = _top_entropy(objective)
+    if _sequence_level(objective, old_per_token_logps) or topent or \
             not _single_pass_ok(logits, _FUSED_GRPO, torch.is_grad_enabled() and logits.requires_grad):
         ent = None
-        if return_entropy or coeff != 0.0:
+        if return_entropy or coeff != 0.0 or topent:
             lp, ent = tail_token_log_probs(logits, input_ids, K, mode=mode, return_entropy=True,
                                            entropy_grad=coeff != 0.0)
         else:
             lp = tail_token_log_probs(logits, input_ids, K, mode=mode)
         scored = grpo_loss(lp, ref_per_token_logps, advantages, tokens, eos_token_id, beta, mode=mode,
                            objective=objective, old_per_token_logps=old_per_token_logps,
-                           return_clip_fraction=return_clip_fraction)
+                           return_clip_fraction=return_clip_fraction, **({'entropy': ent} if topent else {}))
         loss, row_end = scored[0], scored[1]
         out = (loss, lp.detach(), row_end)
         if coeff != 0.0:
@@ -2275,12 +2382,17 @@ class GrpoObjective(ActorObjective):
     or 'k1' / 'k2': KL_ESTIMATORS).  importance_sampling_level: 'token' (the ratio above) or 'sequence' (GSPO, Zheng et
     al. 2025; TRL's importance_sampling_level): one fp32 ratio per sequence, w = exp(sum((lp - old) * mask) / n) with
     n = the sequence's counted tokens, clipped in place of each token's ratio (aa_grpo_loss_seq).  Without old
-    log-probs w is 1 and the token-level launches run.  Checked on the host when constructed."""
+    log-probs w is 1 and the token-level launches run.  top_entropy_quantile rho in [0, 1] (Wang et al. 2025; TRL's
+    top_entropy_quantile): only the counted tokens whose policy entropy H is >= torch.quantile(H[counted], 1 - rho)
+    over every rank keep s, per-token loss = -(s * keep - beta * KL); the denominators, the KL term, the entropy bonus,
+    GSPO's ratio and the clip fractions stay over the whole completion mask.  1 (the default) masks nothing.  Checked
+    on the host when constructed."""
 
     loss_agg_mode: str = 'token-mean'
     clip_range_ratio: float = 0.2
     kl_estimator: str = 'k3'
     importance_sampling_level: str = 'token'
+    top_entropy_quantile: float = 1.0
     _MODES = GRPO_LOSS_AGG_MODES
 
     def __post_init__(self):
@@ -2290,13 +2402,16 @@ class GrpoObjective(ActorObjective):
         if self.importance_sampling_level not in IMPORTANCE_SAMPLING_LEVELS:
             raise ValueError(f'importance_sampling_level must be one of {IMPORTANCE_SAMPLING_LEVELS}, got '
                              f'{self.importance_sampling_level!r}')
+        rho = self.top_entropy_quantile
+        if isinstance(rho, bool) or not isinstance(rho, (int, float)) or not 0.0 <= float(rho) <= 1.0:
+            raise ValueError(f'top_entropy_quantile must be a number in [0, 1], got {rho!r}')
 
     @property
     def is_default(self) -> bool:
         """The reference's loss when the ratio is 1: the kernels run today's launches."""
         return (self.clip_range_ratio_low is None and self.clip_range_ratio_high is None and self.dual_clip_ratio is None
                 and self.loss_agg_mode == 'token-mean' and self.kl_estimator == 'k3'
-                and self.importance_sampling_level == 'token')
+                and self.importance_sampling_level == 'token' and self.top_entropy_quantile == 1.0)
 
     @property
     def sequence_level(self) -> bool:

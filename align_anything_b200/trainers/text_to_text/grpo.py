@@ -16,7 +16,7 @@ from .ppo import entropy_coeff_of, hidden_log_probs, lm_head_of, switch_of
 __all__ = ['GRPOTrainer']
 
 GRPO_OBJECTIVE_KEYS = ('clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio',
-                       'loss_agg_mode', 'kl_estimator', 'importance_sampling_level')
+                       'loss_agg_mode', 'kl_estimator', 'importance_sampling_level', 'top_entropy_quantile')
 
 
 def num_iterations_of(tr) -> int:
@@ -79,13 +79,20 @@ class GRPOTrainer:
     # place of the token ratios.  It acts from update 2 on, so it wants num_iterations > 1; the first update (ratio 1)
     # runs the token-level launches.  `cfgs.train_cfgs.importance_sampling_level` overrides it.
     importance_sampling_level = 'token'
+    # High-entropy token masking (Wang et al. 2025, "Beyond the 80/20 Rule"; TRL's top_entropy_quantile): rho in [0, 1].
+    # Each update, only the top-rho fraction of the completion tokens by policy entropy (over every data-parallel rank)
+    # keep the policy-gradient term; the others carry the KL term alone.  1 (the default) masks nothing and runs
+    # today's launches; rho < 1 takes the composed path with the exact entropy quantile (ops.entropy_quantile_threshold)
+    # on both the tile and the fused_lm_head paths.  `cfgs.train_cfgs.top_entropy_quantile` overrides it.
+    top_entropy_quantile = 1.0
     # Opt-in: train/actor_clip_fraction (and train/actor_dual_clip_fraction with dual-clip), the mean over the updates,
     # in the step's one packed all-reduce
     log_clip_fraction = False
     # the class attributes above that the grafted methods read: patch.install() copies them onto the reference's class
     SWITCHES = ('mode', 'fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'num_iterations',
                 'clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode',
-                'scale_rewards', 'log_clip_fraction', 'kl_estimator', 'importance_sampling_level')
+                'scale_rewards', 'log_clip_fraction', 'kl_estimator', 'importance_sampling_level',
+                'top_entropy_quantile')
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, tokenizer=None, *, beta=None,
                  num_generations=None) -> None:
@@ -190,14 +197,15 @@ def policy_update(tr, sequences, attention_mask, logits_to_keep, ref_per_token_l
     coeff = entropy_coeff_of(tr)
     entropy_mean = plain = None  # with the bonus: its entropy term and GRPO's loss without it
     if tr.fused_lm_head:  # the composed path: K1f needs a logits tile
-        want_entropy = tr.log_entropy or coeff != 0.0
+        topent = ops._top_entropy(kw.get('objective'))  # the mask's threshold is taken from this pass's entropy
+        want_entropy = tr.log_entropy or coeff != 0.0 or topent
         per_token_logps = tr._get_per_token_logps(tr.actor_model, sequences, attention_mask, logits_to_keep,
                                                     return_entropy=want_entropy, entropy_grad=coeff != 0.0)
         if want_entropy:
             per_token_logps, entropy = per_token_logps
         scored = ops.grpo_loss(per_token_logps, ref_per_token_logps, advantages,
                                sequences[:, -logits_to_keep:], tr.tokenizer.eos_token_id, tr.beta,
-                               mode=tr.mode, **kw)
+                               mode=tr.mode, **kw, **({'entropy': entropy} if topent else {}))
         loss, row_end = scored[0], scored[1]
         if kw.get('return_clip_fraction'):
             cf = scored[2]
@@ -206,6 +214,8 @@ def policy_update(tr, sequences, attention_mask, logits_to_keep, ref_per_token_l
             entropy_mean = ops._completion_mean(entropy, row_end)
             plain, loss = loss, loss - coeff * entropy_mean
             entropy, entropy_mean = entropy.detach(), entropy_mean.detach()
+        if not tr.log_entropy and coeff == 0.0:
+            entropy = None  # taken for the mask alone
     else:
         logits = tr.actor_model(input_ids=sequences, attention_mask=attention_mask).logits
         scored = ops.grpo_loss_from_logits(logits, sequences, logits_to_keep, ref_per_token_logps, advantages,

@@ -8,7 +8,7 @@
  * function(s) whose arithmetic it replaces (file:line relative to the reference's
  * align_anything/ directory); the Python mirror in align_anything_b200/ keeps the
  * reference's names and signatures and calls these through ctypes (INTEGRATION.md).
- * 64 entry points, ABI version 3.
+ * 70 entry points, ABI version 3.
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
@@ -717,6 +717,44 @@ int aa_grpo_loss_seq(const void *log_probs, int64_t lp_stride, const void *ref_l
                      float beta, float clip_low, float clip_high, float dual_clip, int loss_agg, int kl_estimator,
                      int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac, int32_t *row_end,
                      float *scratch, uint32_t *counter, void *stream);
+/* aa_grpo_loss_seq's objective (sequence 1) or aa_grpo_loss_kl's (sequence 0; old_log_probs may then be NULL: ratio
+ * 1) under the top-entropy mask (Wang et al. 2025; TRL's top_entropy_quantile): a counted token with
+ * entropy[b * ent_stride + t] < thr[0] (fp32, e.g. from aa_entropy_select_lo; NaN keeps nothing) has the per-token loss
+ * -(s * 0 - beta * KL), so s sends it no gradient.  At sequence level s's gradient reaches the row's ratio from the
+ * kept tokens only, and through the ratio every counted token's log-prob, as autograd of the masked loss gives it.
+ * The KL term, the aggregation's denominators and the clip fractions are the unmasked ones.  Arguments are checked
+ * before any CUDA call. */
+int aa_grpo_loss_topent(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
+                        const void *old_log_probs, int64_t old_stride, int lp_dtype, const float *advantages,
+                        const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B, int32_t K,
+                        float beta, float clip_low, float clip_high, float dual_clip, int loss_agg, int kl_estimator,
+                        int sequence, int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac,
+                        const float *entropy, int64_t ent_stride, const float *thr, int32_t *row_end, float *scratch,
+                        uint32_t *counter, void *stream);
+
+/* Top-entropy threshold: thr = torch.quantile(H[counted], q) (linear interpolation) over every counted token of every
+ * rank, as an exact radix select on order-preserving keys, with no host sync.
+ *   aa_grpo_row_end      : GRPO's completion mask pass alone (row_end[b] = tokens up to and including the first eos,
+ *                          total[0] = their fp32 count), the rule aa_grpo_loss* apply.
+ *   aa_entropy_hist_hi   : hist (uint32[65537], zeroed here) = counts of the high 16 bits of the counted entropies' keys,
+ *                          hist[65536] = their NaNs.  counted: t < row_end[b], or mask[b * mask_stride + t] != 0 (give
+ *                          exactly one); entropy fp32 (B, K), row stride ent_stride.  B * K < 2^31.
+ *   (across ranks the caller all-reduces hist with SUM)
+ *   aa_entropy_select_hi : one block; sel (uint32[8]) = the count N, the NaN count, and for lo = floor(rank) and
+ *                          hi = ceil(rank) (rank = fp32 q * (N - 1), at most N - 1) the bucket and the rank inside it.
+ *                          q in [0, 1].  N must be < 2^32 over all ranks.
+ *   aa_entropy_hist_lo   : hist (uint32[2 * 65536], zeroed here) = the low 16 bits inside lo's and hi's buckets.
+ *   (across ranks the caller all-reduces hist with SUM)
+ *   aa_entropy_select_lo : one block; thr[0] = lerp(v_lo, v_hi, rank - lo) as ATen forms it; NaN when N == 0 or a
+ *                          counted entropy is NaN (torch.quantile's NaN). */
+int aa_grpo_row_end(const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B, int32_t K,
+                    int32_t *row_end, float *total, uint32_t *counter, void *stream);
+int aa_entropy_hist_hi(const float *entropy, int64_t ent_stride, const int32_t *row_end, const uint8_t *mask,
+                       int64_t mask_stride, int32_t B, int32_t K, uint32_t *hist, void *stream);
+int aa_entropy_select_hi(const uint32_t *hist, float q, uint32_t *sel, void *stream);
+int aa_entropy_hist_lo(const float *entropy, int64_t ent_stride, const int32_t *row_end, const uint8_t *mask,
+                       int64_t mask_stride, int32_t B, int32_t K, const uint32_t *sel, uint32_t *hist, void *stream);
+int aa_entropy_select_lo(const uint32_t *hist, const uint32_t *sel, float *thr, void *stream);
 
 /* masked_mean (utils/tools.py:460-467): mean over rows of masked row means -> out[0];
  * mask == NULL: plain mean. */
