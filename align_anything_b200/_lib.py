@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_uint32, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_uint32, c_void_p
 
 import torch
 
@@ -147,6 +147,19 @@ _SIGS = {
     'aa_entropy_select_hi': (c_int, [_P, c_float, _P, _P]),
     'aa_entropy_hist_lo': (c_int, [_P, c_int64, _P, _P, c_int64, c_int32, c_int32, _P, _P, _P]),
     'aa_entropy_select_lo': (c_int, [_P, _P, _P, _P]),
+    'aa_cov_moments': (c_int, [_P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, _P, c_int32, c_int32, _P, _P]),
+    'aa_cov_keys': (c_int, [c_int, _P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, _P, c_int32,
+                            c_int32, c_float, c_float, c_float, c_float, c_uint32, c_int, _P, _P, _P, _P, _P]),
+    'aa_cov_select_hi': (c_int, [_P, POINTER(c_double), _P, _P]),
+    'aa_cov_hist_lo': (c_int, [_P, _P, c_int64, _P, _P, _P]),
+    'aa_cov_select_lo': (c_int, [_P, _P, _P, _P]),
+    'aa_cov_mark': (c_int, [_P, _P, c_int32, c_int32, _P, _P, _P, c_int64, _P]),
+    'aa_ppo_actor_loss_cov': (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, c_int32,
+                                      c_int32, c_float, c_float, c_int, c_int, c_float, _P, c_int64, c_int, _P,
+                                      c_int64, c_float, c_int, _P, _P, _P, c_int64, _P, _P, _P, _P]),
+    'aa_grpo_loss_cov': (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int, _P, _P, c_int64, c_int64, c_int32,
+                                 c_int32, c_float, c_float, c_float, c_int, c_int, c_int, c_float, _P, c_int64, c_int,
+                                 _P, _P, c_int64, _P, _P, _P, _P, _P]),
     'aa_nll_mean': (c_int, [_P, c_int, _P, c_int64, c_int64, _P, _P, _P, _P, _P]),
     'aa_masked_mean': (c_int, [_P, c_int, c_int64, _P, c_int64, c_int32, c_int32, _P, _P, _P, _P]),
     'aa_ppo_pack_metrics': (c_int, [_P, _P, _P, _P, _P, c_int32, _P, POINTER(AaColl), _P, _P]),

@@ -12,6 +12,8 @@
 //     aa_whiten_moments / aa_whiten_reduce / aa_whiten_apply: masked_whiten of a rollout's advantages.
 //     aa_grpo_row_end, aa_entropy_hist_hi / _select_hi / _hist_lo / _select_lo: the exact entropy quantile of the
 //                          top-entropy mask, and aa_grpo_loss_topent: GRPO's loss under that mask.
+//     aa_cov_moments / _keys / _select_hi / _hist_lo / _select_lo / _mark: the exact top-k covariance selection of
+//                          Clip-Cov and KL-Cov, and aa_ppo_actor_loss_cov / aa_grpo_loss_cov: the losses under it.
 //
 // These touch ~10 floats per token: latency-bound, not bandwidth-bound.  The point is launch
 // count (thousands -> five) and zero host syncs; each sample is owned by one warp / CTA.
@@ -398,10 +400,17 @@ struct LossParams {
   float kl_coeff;
   int kl_est;
   float *kl_loss;
+  // Clip-Cov / KL-Cov (COV, aa_ppo_actor_loss_cov): the selection of aa_cov_mark (uint8, row stride sel_stride) and
+  // KL-Cov's coefficient (cov_token)
+  const uint8_t *sel;
+  int64_t sel_stride;
+  float cov_coef;
 };
 
-template <int THREADS, bool ACTOR>
+// COV (actor only, aa_ppo_actor_loss_cov): AA_COV_CLIP / AA_COV_KL, the token's objective is cov_token's
+template <int THREADS, bool ACTOR, int COV = 0>
 __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
+  static_assert(ACTOR || COV == 0, "Clip-Cov and KL-Cov are actor objectives");
   __shared__ float scratch[33];
   const int b = blockIdx.x, tid = threadIdx.x;
   const int Wm = p.Wm, rx = p.r_x, rp = p.r_p;
@@ -439,7 +448,11 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
     float obj, grad;
     if (ACTOR) {
       int why;
-      actor_token(x, old, aux, on, g_rs, p.clip, p.clip_hi, p.dual, rx, rp, p.r_a, obj, grad, why);
+      if constexpr (COV != 0)
+        cov_token(COV, x, old, aux, on, on && p.sel[b * p.sel_stride + t] != 0, g_rs, p.clip, p.clip_hi, p.cov_coef,
+                  rx, rp, obj, grad, why);
+      else
+        actor_token(x, old, aux, on, g_rs, p.clip, p.clip_hi, p.dual, rx, rp, p.r_a, obj, grad, why);
       if (on) {
         n_clip += (why & 1) ? 1.f : 0.f;
         n_dual += (why & 2) ? 1.f : 0.f;
@@ -648,6 +661,10 @@ struct GrpoObjParams {
   const float *entropy;
   int64_t ent_stride;
   const float *thr;
+  // Clip-Cov / KL-Cov (COV, aa_grpo_loss_cov): as LossParams' sel, sel_stride, cov_coef
+  const uint8_t *sel;
+  int64_t sel_stride;
+  float cov_coef;
 };
 
 // GRPO's loss and d loss / d lp, one block per row, the last block to arrive reduces the rows.  OBJECTIVE: the clipped
@@ -658,11 +675,13 @@ struct GrpoObjParams {
 // then every token takes the row's objective and ratio coefficient (grpo_seq_row, grpo_seq_token).  TOPENT (with
 // OBJECTIVE, aa_grpo_loss_topent): the top-entropy mask -- a counted token with entropy < thr keeps only its KL term
 // (keep = 0 in grpo_obj_token; at sequence level s * keep, and s's gradient reaches the row's ratio from the kept
-// tokens alone, n_s of grpo_seq_row)
-template <int THREADS, bool OBJECTIVE, bool SEQUENCE = false, bool TOPENT = false>
+// tokens alone, n_s of grpo_seq_row).  COV (with OBJECTIVE at token level, aa_grpo_loss_cov): Clip-Cov / KL-Cov
+// (grpo_cov_token)
+template <int THREADS, bool OBJECTIVE, bool SEQUENCE = false, bool TOPENT = false, int COV = 0>
 __global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoObjParams q) {
   static_assert(OBJECTIVE || !SEQUENCE, "the sequence-level ratio is an option of the clipped objective");
   static_assert(OBJECTIVE || !TOPENT, "the top-entropy mask is an option of the clipped objective");
+  static_assert(COV == 0 || (OBJECTIVE && !SEQUENCE && !TOPENT), "Clip-Cov and KL-Cov are token-level objectives");
   __shared__ float scratch[33];
   const GrpoParams &p = q.base;
   const int b = blockIdx.x, tid = threadIdx.x, r = p.r_lp;
@@ -699,6 +718,10 @@ __global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoObjParams 
     if constexpr (SEQUENCE) {
       grpo_seq_token(lp, rf, s_seq * keep, coef_seq, on, g_t, p.beta, q.kl_est, r, ptl, g);
       why = why_seq;
+    } else if constexpr (COV != 0) {
+      const float old = q.old ? load_as_float(q.old, b * q.old_stride + t, p.dtype) : lp;
+      grpo_cov_token(COV, lp, old, rf, A, on, on && q.sel[b * q.sel_stride + t] != 0, g_t, p.beta, q.clip_lo,
+                     q.clip_hi, q.cov_coef, q.kl_est, r, ptl, g, why);
     } else if constexpr (OBJECTIVE) {
       const float old = q.old ? load_as_float(q.old, b * q.old_stride + t, p.dtype) : lp;
       grpo_obj_token(lp, old, rf, A, on, g_t, p.beta, q.clip_lo, q.clip_hi, q.dual, q.kl_est, r, ptl, g, why, keep);
@@ -1088,6 +1111,255 @@ __global__ void __launch_bounds__(256)
   store_from_float(adv, i, dtype, v);
 }
 
+// ---- Clip-Cov / KL-Cov: the exact top-k covariance selection (verl's clip_cov / kl_cov) -----------------------------
+// The k largest uint32 keys of the eligible tokens of one loss call, without a host sync: the fp64 means (one block,
+// fixed order), the keys with the high-half histogram, a radix select 16 bits a pass (entropy_find_rank on the
+// threshold's ascending rank E - k), then a mark pass that takes the keys above the threshold T and, among the keys
+// equal to T, the first `need` by flat index (a per-row tie count and an exclusive scan over the rows).
+enum { kCovN = 0, kCovE, kCovK, kCovBucket, kCovRank, kCovT, kCovNeed, kCovMeanA, kCovMeanLp, kCovWords = 16 };
+constexpr int kCovThreads = 256;
+
+// MurmurHash3's 32-bit finaliser: a bijection of uint32
+__host__ __device__ __forceinline__ uint32_t fmix32(uint32_t h) {
+  h ^= h >> 16;
+  h *= 0x85ebca6bu;
+  h ^= h >> 13;
+  h *= 0xc2b2ae35u;
+  h ^= h >> 16;
+  return h;
+}
+
+// the float order as an unsigned order, -0.0 folded onto +0.0 and every NaN above +inf (torch.topk's order)
+__device__ __forceinline__ uint32_t cov_key(float x) {
+  if (x != x) return 0xffffffffu;
+  const uint32_t u = __float_as_uint(x == 0.f ? 0.f : x);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// the counted tokens and their advantages: mask (B, W) with advantages (B, W) of adv_dtype, or row_end with fp32
+// per-row advantages
+struct CovRows {
+  const void *lp;
+  int64_t lp_stride;
+  int lp_dtype;
+  const void *adv;
+  int64_t adv_stride;
+  int adv_dtype;
+  const uint8_t *mask;
+  int64_t mask_stride;
+  const int32_t *row_end;
+  int B, W;
+  __device__ __forceinline__ bool counted(int b, int t) const {
+    return mask ? mask[b * mask_stride + t] != 0 : t < row_end[b];
+  }
+  __device__ __forceinline__ float advantage(int b, int t) const {
+    return mask ? load_as_float(adv, b * adv_stride + t, adv_dtype) : static_cast<const float *>(adv)[b];
+  }
+};
+
+// One block: (N, sum A, sum lp) in fp64, each thread over its elements in index order, then block_sum_f64's fixed
+// tree; the loads are unconditional and masked by a select, so an uncounted NaN never enters the sums
+__global__ void __launch_bounds__(kWhitenThreads) cov_moments_kernel(const CovRows c, uint32_t *state) {
+  __shared__ double scratch[33];
+  double n = 0.0, sa = 0.0, sl = 0.0;
+  const uint32_t total = static_cast<uint32_t>(c.B) * static_cast<uint32_t>(c.W);
+  for (uint32_t i = threadIdx.x; i < total; i += kWhitenThreads) {
+    const int b = static_cast<int>(i / static_cast<uint32_t>(c.W)), t = static_cast<int>(i - b * static_cast<uint32_t>(c.W));
+    const bool on = c.counted(b, t);
+    const double a = c.advantage(b, t);
+    const double l = load_as_float(c.lp, b * c.lp_stride + t, c.lp_dtype);
+    n += on ? 1.0 : 0.0;
+    sa += on ? a : 0.0;
+    sl += on ? l : 0.0;
+  }
+  n = block_sum_f64<kWhitenThreads>(n, scratch);
+  sa = block_sum_f64<kWhitenThreads>(sa, scratch);
+  sl = block_sum_f64<kWhitenThreads>(sl, scratch);
+  if (threadIdx.x == 0) {
+    state[kCovN] = static_cast<uint32_t>(n);
+    state[kCovMeanA] = __float_as_uint(static_cast<float>(sa / n));
+    state[kCovMeanLp] = __float_as_uint(static_cast<float>(sl / n));
+  }
+}
+
+struct CovKeyParams {
+  CovRows c;
+  const void *old;
+  int64_t old_stride;
+  float clip_lo, clip_hi, lb, ub;
+  uint32_t seed;
+  int rx, rp;
+  const uint32_t *state;
+  uint32_t *keys;
+  uint8_t *elig;
+  uint32_t *hist;
+};
+
+// keys, eligibility and the high-half histogram; one warp folds equal bins (__match_any_sync) into one atomic
+template <int MODE>
+__global__ void __launch_bounds__(kCovThreads) cov_keys_kernel(const CovKeyParams p) {
+  const CovRows &c = p.c;
+  const float mean_a = __uint_as_float(p.state[kCovMeanA]), mean_lp = __uint_as_float(p.state[kCovMeanLp]);
+  const int64_t n = static_cast<int64_t>(c.B) * c.W;
+  const int lane = threadIdx.x & (kWarp - 1);
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t base = static_cast<int64_t>(blockIdx.x) * blockDim.x + (threadIdx.x & ~(kWarp - 1)); base < n;
+       base += stride) {
+    const int64_t i = base + lane;
+    uint32_t bin = kEntSkip;
+    if (i < n) {
+      const int b = static_cast<int>(i / c.W), t = static_cast<int>(i - static_cast<int64_t>(b) * c.W);
+      const bool on = c.counted(b, t);
+      const float a = c.advantage(b, t), lp = load_as_float(c.lp, b * c.lp_stride + t, c.lp_dtype);
+      const float cov = __fmul_rn(__fsub_rn(a, mean_a), __fsub_rn(lp, mean_lp));
+      bool e;
+      uint32_t key;
+      if constexpr (MODE == AA_COV_KL) {
+        e = on;
+        key = cov_key(cov);
+      } else {
+        const float old = p.old ? load_as_float(p.old, b * p.old_stride + t, c.lp_dtype) : lp;
+        float obj, g;
+        int why;
+        actor_token(lp, old, a, false, 0.f, p.clip_lo, p.clip_hi, 0.f, p.rx, p.rp, p.rp, obj, g, why);
+        e = on && !(why & 1) && cov > p.lb && cov < p.ub;
+        key = fmix32(static_cast<uint32_t>(i) ^ p.seed);
+      }
+      p.keys[i] = key;
+      p.elig[i] = e ? 1 : 0;
+      if (e) bin = key >> 16;
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, bin);
+    if (bin != kEntSkip && lane == __ffs(peers) - 1) atomicAdd(&p.hist[bin], static_cast<uint32_t>(__popc(peers)));
+  }
+}
+
+// One block: E = the eligible count, k, and the bucket of ascending rank E - k (the k-th largest key)
+__global__ void __launch_bounds__(kEntSelectThreads)
+    cov_select_hi_kernel(const uint32_t *__restrict__ hist, double ratio, uint32_t *__restrict__ state) {
+  __shared__ uint32_t warp_tot[kEntSelectThreads / kWarp];
+  __shared__ uint32_t res[2];
+  const uint32_t E = entropy_find_rank(hist, 0xffffffffu, &res[0], &res[1], warp_tot);  // the sum alone
+  uint32_t k = 0;
+  if (E > 0u) {
+    const long long m = static_cast<long long>(ratio * static_cast<double>(state[kCovN]));  // Python's int()
+    k = static_cast<uint32_t>(m < 1 ? 1 : (m > static_cast<long long>(E) ? static_cast<long long>(E) : m));
+    entropy_find_rank(hist, E - k, &res[0], &res[1], warp_tot);
+  }
+  if (threadIdx.x == 0) {
+    state[kCovE] = E;
+    state[kCovK] = k;
+    state[kCovBucket] = k ? res[0] : 0u;
+    state[kCovRank] = k ? res[1] : 0u;
+  }
+}
+
+__global__ void __launch_bounds__(kCovThreads)
+    cov_hist_lo_kernel(const uint32_t *__restrict__ keys, const uint8_t *__restrict__ elig, int64_t n,
+                       const uint32_t *__restrict__ state, uint32_t *__restrict__ hist) {
+  if (state[kCovK] == 0u) return;
+  const uint32_t bucket = state[kCovBucket];
+  const int lane = threadIdx.x & (kWarp - 1);
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t base = static_cast<int64_t>(blockIdx.x) * blockDim.x + (threadIdx.x & ~(kWarp - 1)); base < n;
+       base += stride) {
+    const int64_t i = base + lane;
+    uint32_t bin = kEntSkip;
+    if (i < n && elig[i] && (keys[i] >> 16) == bucket) bin = keys[i] & 0xffffu;
+    const unsigned peers = __match_any_sync(0xffffffffu, bin);
+    if (bin != kEntSkip && lane == __ffs(peers) - 1) atomicAdd(&hist[bin], static_cast<uint32_t>(__popc(peers)));
+  }
+}
+
+// One block: the threshold key T and need = how many of the keys equal to T are selected; share = k / N
+__global__ void __launch_bounds__(kEntSelectThreads)
+    cov_select_lo_kernel(const uint32_t *__restrict__ hist, uint32_t *__restrict__ state, float *share) {
+  __shared__ uint32_t warp_tot[kEntSelectThreads / kWarp];
+  __shared__ uint32_t res[2];
+  const uint32_t k = state[kCovK], N = state[kCovN];
+  if (k == 0u) {
+    if (threadIdx.x == 0) {
+      state[kCovT] = 0xffffffffu;
+      state[kCovNeed] = 0u;
+      share[0] = 0.f;
+    }
+    return;
+  }
+  entropy_find_rank(hist, state[kCovRank], &res[0], &res[1], warp_tot);
+  if (threadIdx.x == 0) {
+    state[kCovT] = (state[kCovBucket] << 16) | res[0];
+    state[kCovNeed] = hist[res[0]] - res[1];
+    share[0] = static_cast<float>(static_cast<double>(k) / static_cast<double>(N));
+  }
+}
+
+// Integer block sum (kCovThreads threads), valid in every thread; `scratch` >= kCovThreads / kWarp + 1 words
+__device__ __forceinline__ uint32_t cov_block_sum(uint32_t v, uint32_t *scratch) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) scratch[threadIdx.x >> 5] = v;
+  __syncthreads();
+  uint32_t s = 0;
+#pragma unroll
+  for (int w = 0; w < kCovThreads / kWarp; ++w) s += scratch[w];
+  __syncthreads();
+  return s;
+}
+
+// One block per row: the row's keys equal to T
+__global__ void __launch_bounds__(kCovThreads)
+    cov_tie_kernel(const uint32_t *__restrict__ keys, const uint8_t *__restrict__ elig, int W,
+                   const uint32_t *__restrict__ state, int32_t *__restrict__ tie_rows) {
+  __shared__ uint32_t scratch[kCovThreads / kWarp];
+  const int b = blockIdx.x;
+  const uint32_t T = state[kCovT];
+  const int64_t row = static_cast<int64_t>(b) * W;
+  uint32_t c = 0;
+  if (state[kCovK] != 0u)
+    for (int t = threadIdx.x; t < W; t += kCovThreads) c += (elig[row + t] && keys[row + t] == T) ? 1u : 0u;
+  c = cov_block_sum(c, scratch);
+  if (threadIdx.x == 0) tie_rows[b] = static_cast<int32_t>(c);
+}
+
+// One block per row: the ties of the rows before this one, then the row in chunks of kCovThreads, each tie's rank
+// the exclusive scan of the tie bits in flat-index order
+__global__ void __launch_bounds__(kCovThreads)
+    cov_mark_kernel(const uint32_t *__restrict__ keys, const uint8_t *__restrict__ elig, int W,
+                    const uint32_t *__restrict__ state, const int32_t *__restrict__ tie_rows, uint8_t *__restrict__ sel,
+                    int64_t sel_stride) {
+  __shared__ uint32_t scratch[kCovThreads / kWarp];
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & (kWarp - 1), warp = tid >> 5;
+  const uint32_t k = state[kCovK], T = state[kCovT], need = state[kCovNeed];
+  const int64_t row = static_cast<int64_t>(b) * W;
+  uint8_t *out = sel + static_cast<int64_t>(b) * sel_stride;
+  if (k == 0u) {
+    for (int t = tid; t < W; t += kCovThreads) out[t] = 0;
+    return;
+  }
+  uint32_t before = 0;
+  for (int j = tid; j < b; j += kCovThreads) before += static_cast<uint32_t>(tie_rows[j]);
+  before = cov_block_sum(before, scratch);
+  for (int t0 = 0; t0 < W; t0 += kCovThreads) {
+    const int t = t0 + tid;
+    const bool e = t < W && elig[row + t];
+    const uint32_t key = e ? keys[row + t] : 0u;
+    const bool tie = e && key == T;
+    const unsigned bits = __ballot_sync(0xffffffffu, tie);
+    if (lane == 0) scratch[warp] = __popc(bits);
+    __syncthreads();
+    uint32_t rank = before + __popc(bits & ((1u << lane) - 1u)), chunk = 0;
+#pragma unroll
+    for (int w = 0; w < kCovThreads / kWarp; ++w) {
+      const uint32_t v = scratch[w];
+      rank += (w < warp) ? v : 0u;
+      chunk += v;
+    }
+    __syncthreads();
+    if (t < W) out[t] = (e && (key > T || (tie && rank < need))) ? 1 : 0;
+    before += chunk;
+  }
+}
+
 static bool dtype_ok(int d) { return d == AA_BF16 || d == AA_F16 || d == AA_F32; }
 
 }  // namespace aa
@@ -1327,7 +1599,8 @@ static int grpo_loss(const char *who, bool objective, const void *log_probs, int
                      int kl_estimator, int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac,
                      int32_t *row_end, float *scratch, uint32_t *counter, void *stream, bool sequence = false,
                      bool topent = false, const float *entropy = nullptr, int64_t ent_stride = 0,
-                     const float *thr = nullptr) {
+                     const float *thr = nullptr, int cov = 0, float cov_coef = 0.f, const uint8_t *sel = nullptr,
+                     int64_t sel_stride = 0) {
   AA_REQUIRE(B > 0 && K > 0 && log_probs && ref_log_probs && advantages && completion_tokens && loss && row_end &&
                  scratch && counter,
              AA_ERR_ARG, "%s: bad arguments", who);
@@ -1351,8 +1624,12 @@ static int grpo_loss(const char *who, bool objective, const void *log_probs, int
                              K, beta, (mode == AA_MODE_FAITHFUL) ? lp_dtype : AA_F32, loss, grad, grad_stride,
                              scratch + 1, counter + 1},
                   old_log_probs, old_stride, clip_low, clip_high, dual_clip, loss_agg, clip_frac, kl_estimator,
-                  entropy, ent_stride, thr};
-  if (topent && sequence)
+                  entropy, ent_stride, thr, sel, sel_stride, cov_coef};
+  if (cov == AA_COV_CLIP)
+    grpo_loss_kernel<128, true, false, false, AA_COV_CLIP><<<B, 128, 0, st>>>(q);
+  else if (cov == AA_COV_KL)
+    grpo_loss_kernel<128, true, false, false, AA_COV_KL><<<B, 128, 0, st>>>(q);
+  else if (topent && sequence)
     grpo_loss_kernel<128, true, true, true><<<B, 128, 0, st>>>(q);
   else if (topent)
     grpo_loss_kernel<128, true, false, true><<<B, 128, 0, st>>>(q);
@@ -1497,6 +1774,166 @@ extern "C" int aa_entropy_select_lo(const uint32_t *hist, const uint32_t *sel, f
   AA_REQUIRE(hist && sel && thr, AA_ERR_ARG, "aa_entropy_select_lo: null pointer");
   entropy_select_lo_kernel<<<1, kEntSelectThreads, 0, static_cast<cudaStream_t>(stream)>>>(hist, sel, thr);
   return check_launch("aa_entropy_select_lo");
+}
+
+// the checks aa_cov_moments and aa_cov_keys share: exactly one of mask / row_end, sizes, strides and dtypes (fp32
+// per-row advantages with row_end)
+static int cov_rows(const char *who, const void *log_probs, int64_t lp_stride, int lp_dtype, const void *advantages,
+                    int64_t adv_stride, int adv_dtype, const uint8_t *mask, int64_t mask_stride,
+                    const int32_t *row_end, int32_t B, int32_t W, CovRows *out) {
+  AA_REQUIRE(log_probs && advantages, AA_ERR_ARG, "%s: null pointer", who);
+  AA_REQUIRE((row_end != nullptr) != (mask != nullptr), AA_ERR_ARG, "%s: give exactly one of row_end and mask", who);
+  AA_REQUIRE(B > 0 && W > 0 && static_cast<int64_t>(B) * W <= INT32_MAX, AA_ERR_ARG, "%s: bad sizes (B=%d W=%d)", who,
+             B, W);
+  AA_REQUIRE(lp_stride >= W && (!mask || (mask_stride >= W && adv_stride >= W)), AA_ERR_ARG,
+             "%s: row strides must be >= W", who);
+  AA_REQUIRE(dtype_ok(lp_dtype) && dtype_ok(adv_dtype) && (mask || adv_dtype == AA_F32), AA_ERR_DTYPE,
+             "%s: bad dtype (per-row advantages are fp32)", who);
+  *out = CovRows{log_probs, lp_stride, lp_dtype, advantages, adv_stride, adv_dtype, mask, mask_stride, row_end, B, W};
+  return AA_OK;
+}
+
+static unsigned cov_grid(int64_t n) {
+  const int64_t blocks = (n + kCovThreads - 1) / kCovThreads;
+  return static_cast<unsigned>(blocks < 1024 ? blocks : 1024);
+}
+
+extern "C" int aa_cov_moments(const void *log_probs, int64_t lp_stride, int lp_dtype, const void *advantages,
+                              int64_t adv_stride, int adv_dtype, const uint8_t *mask, int64_t mask_stride,
+                              const int32_t *row_end, int32_t B, int32_t W, uint32_t *state, void *stream) {
+  CovRows c;
+  int rc = cov_rows("aa_cov_moments", log_probs, lp_stride, lp_dtype, advantages, adv_stride, adv_dtype, mask,
+                    mask_stride, row_end, B, W, &c);
+  if (rc) return rc;
+  AA_REQUIRE(state, AA_ERR_ARG, "aa_cov_moments: null state");
+  cov_moments_kernel<<<1, kWhitenThreads, 0, static_cast<cudaStream_t>(stream)>>>(c, state);
+  return check_launch("aa_cov_moments");
+}
+
+extern "C" int aa_cov_keys(int cov_mode, const void *log_probs, int64_t lp_stride, const void *old_log_probs,
+                           int64_t old_stride, int lp_dtype, const void *advantages, int64_t adv_stride, int adv_dtype,
+                           const uint8_t *mask, int64_t mask_stride, const int32_t *row_end, int32_t B, int32_t W,
+                           float clip_low, float clip_high, float lb, float ub, uint32_t hash_seed, int mode,
+                           const uint32_t *state, uint32_t *keys, uint8_t *elig, uint32_t *hist, void *stream) {
+  CovRows c;
+  int rc = cov_rows("aa_cov_keys", log_probs, lp_stride, lp_dtype, advantages, adv_stride, adv_dtype, mask,
+                    mask_stride, row_end, B, W, &c);
+  if (rc) return rc;
+  AA_REQUIRE(state && keys && elig && hist, AA_ERR_ARG, "aa_cov_keys: null pointer");
+  AA_REQUIRE(cov_mode == AA_COV_CLIP || cov_mode == AA_COV_KL, AA_ERR_ARG, "aa_cov_keys: unknown cov_mode %d",
+             cov_mode);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_cov_keys: bad mode");
+  AA_REQUIRE(!old_log_probs || old_stride >= W, AA_ERR_ARG, "aa_cov_keys: old_stride must be >= W");
+  AA_REQUIRE(cov_mode == AA_COV_KL || (actor_objective_ok(clip_low, clip_high, 0.f, AA_AGG_TOKEN_MEAN) && lb < ub &&
+                                       isfinite(lb) && isfinite(ub)),
+             AA_ERR_ARG, "aa_cov_keys: bad Clip-Cov arguments (need 0 <= clip_low < 1, clip_high >= 0, finite lb < ub; "
+             "got %g %g %g %g)", clip_low, clip_high, lb, ub);
+  const bool f = mode == AA_MODE_FAITHFUL;
+  const CovKeyParams p{c, old_log_probs, old_stride, clip_low, clip_high, lb, ub, hash_seed,
+                       f ? lp_dtype : AA_F32, f ? promote(lp_dtype, adv_dtype) : AA_F32, state, keys, elig, hist};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaMemsetAsync(hist, 0, sizeof(uint32_t) * kEntBins, st);
+  const unsigned grid = cov_grid(static_cast<int64_t>(B) * W);
+  if (cov_mode == AA_COV_KL)
+    cov_keys_kernel<AA_COV_KL><<<grid, kCovThreads, 0, st>>>(p);
+  else
+    cov_keys_kernel<AA_COV_CLIP><<<grid, kCovThreads, 0, st>>>(p);
+  return check_launch("aa_cov_keys");
+}
+
+extern "C" int aa_cov_select_hi(const uint32_t *hist, const double *ratio_host, uint32_t *state, void *stream) {
+  AA_REQUIRE(hist && state && ratio_host, AA_ERR_ARG, "aa_cov_select_hi: null pointer");
+  const double ratio = *ratio_host;
+  AA_REQUIRE(ratio > 0.0 && ratio <= 1.0, AA_ERR_ARG, "aa_cov_select_hi: ratio must lie in (0, 1], got %g", ratio);
+  cov_select_hi_kernel<<<1, kEntSelectThreads, 0, static_cast<cudaStream_t>(stream)>>>(hist, ratio, state);
+  return check_launch("aa_cov_select_hi");
+}
+
+extern "C" int aa_cov_hist_lo(const uint32_t *keys, const uint8_t *elig, int64_t n, const uint32_t *state,
+                              uint32_t *hist, void *stream) {
+  AA_REQUIRE(keys && elig && state && hist, AA_ERR_ARG, "aa_cov_hist_lo: null pointer");
+  AA_REQUIRE(n > 0 && n <= INT32_MAX, AA_ERR_ARG, "aa_cov_hist_lo: bad size %lld", static_cast<long long>(n));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaMemsetAsync(hist, 0, sizeof(uint32_t) * kEntBins, st);
+  cov_hist_lo_kernel<<<cov_grid(n), kCovThreads, 0, st>>>(keys, elig, n, state, hist);
+  return check_launch("aa_cov_hist_lo");
+}
+
+extern "C" int aa_cov_select_lo(const uint32_t *hist, uint32_t *state, float *share, void *stream) {
+  AA_REQUIRE(hist && state && share, AA_ERR_ARG, "aa_cov_select_lo: null pointer");
+  cov_select_lo_kernel<<<1, kEntSelectThreads, 0, static_cast<cudaStream_t>(stream)>>>(hist, state, share);
+  return check_launch("aa_cov_select_lo");
+}
+
+extern "C" int aa_cov_mark(const uint32_t *keys, const uint8_t *elig, int32_t B, int32_t W, const uint32_t *state,
+                           int32_t *tie_rows, uint8_t *sel, int64_t sel_stride, void *stream) {
+  AA_REQUIRE(keys && elig && state && tie_rows && sel, AA_ERR_ARG, "aa_cov_mark: null pointer");
+  AA_REQUIRE(B > 0 && W > 0 && static_cast<int64_t>(B) * W <= INT32_MAX && sel_stride >= W, AA_ERR_ARG,
+             "aa_cov_mark: bad sizes (B=%d W=%d sel_stride=%lld)", B, W, static_cast<long long>(sel_stride));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cov_tie_kernel<<<B, kCovThreads, 0, st>>>(keys, elig, W, state, tie_rows);
+  int rc = check_launch("aa_cov_mark(ties)");
+  if (rc) return rc;
+  cov_mark_kernel<<<B, kCovThreads, 0, st>>>(keys, elig, W, state, tie_rows, sel, sel_stride);
+  return check_launch("aa_cov_mark");
+}
+
+extern "C" int aa_ppo_actor_loss_cov(const void *log_probs, int64_t lp_stride, const void *old_log_probs,
+                                     int64_t old_stride, int lp_dtype, const void *advantages, int64_t adv_stride,
+                                     int adv_dtype, const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t Wm,
+                                     float clip_low, float clip_high, int loss_agg, int cov_mode, float cov_coef,
+                                     const uint8_t *sel, int64_t sel_stride, int mode, const void *ref_log_probs,
+                                     int64_t ref_stride, float kl_loss_coeff, int kl_estimator, float *loss,
+                                     float *kl_loss, void *grad, int64_t grad_stride, float *clip_frac,
+                                     float *row_scratch, uint32_t *counter, void *stream) {
+  const char *who = "aa_ppo_actor_loss_cov";
+  AA_REQUIRE(B > 0 && Wm > 0, AA_ERR_ARG, "%s: bad sizes", who);
+  AA_REQUIRE(log_probs && old_log_probs && advantages && mask && sel && loss && row_scratch && counter, AA_ERR_ARG,
+             "%s: null pointer", who);
+  AA_REQUIRE(dtype_ok(lp_dtype) && dtype_ok(adv_dtype), AA_ERR_DTYPE, "%s: bad dtype", who);
+  AA_REQUIRE(actor_objective_ok(clip_low, clip_high, 0.f, loss_agg), AA_ERR_ARG,
+             "%s: bad objective (need 0 <= clip_low < 1, clip_high >= 0, a known loss_agg; got %g %g %d)", who,
+             clip_low, clip_high, loss_agg);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "%s: bad mode", who);
+  AA_REQUIRE(cov_mode == AA_COV_CLIP || cov_mode == AA_COV_KL, AA_ERR_ARG, "%s: unknown cov_mode %d", who, cov_mode);
+  AA_REQUIRE(isfinite(cov_coef) && cov_coef >= 0.f, AA_ERR_ARG, "%s: cov_coef must be finite and >= 0, got %g", who,
+             cov_coef);
+  AA_REQUIRE(sel_stride >= Wm, AA_ERR_ARG, "%s: sel_stride must be >= Wm", who);
+  if (ref_log_probs) {
+    AA_REQUIRE(kl_estimator_ok(kl_estimator), AA_ERR_ARG, "%s: unknown kl_estimator code %d", who, kl_estimator);
+    AA_REQUIRE(kl_loss_term_ok(kl_loss_coeff) && kl_loss, AA_ERR_ARG,
+               "%s: a KL loss term needs kl_loss_coeff finite and > 0 (got %g) and kl_loss", who, kl_loss_coeff);
+  }
+  const bool f = (mode == AA_MODE_FAITHFUL);
+  LossParams p{log_probs, lp_stride, old_log_probs, old_stride, lp_dtype, advantages, adv_stride, adv_dtype,
+               mask, mask_stride, B, Wm, clip_low, f ? lp_dtype : AA_F32,
+               f ? promote(lp_dtype, adv_dtype) : AA_F32, loss, grad, grad_stride, nullptr, row_scratch, counter, nullptr, 0,
+               clip_high, 0.f, f ? adv_dtype : AA_F32, loss_agg, clip_frac, ref_log_probs, ref_stride,
+               ref_log_probs ? kl_loss_coeff : 0.f, kl_estimator, kl_loss, sel, sel_stride, cov_coef};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (cov_mode == AA_COV_KL)
+    ppo_loss_kernel<128, true, AA_COV_KL><<<B, 128, 0, st>>>(p);
+  else
+    ppo_loss_kernel<128, true, AA_COV_CLIP><<<B, 128, 0, st>>>(p);
+  return check_launch(who);
+}
+
+extern "C" int aa_grpo_loss_cov(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
+                                const void *old_log_probs, int64_t old_stride, int lp_dtype, const float *advantages,
+                                const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B,
+                                int32_t K, float beta, float clip_low, float clip_high, int loss_agg, int kl_estimator,
+                                int cov_mode, float cov_coef, const uint8_t *sel, int64_t sel_stride, int mode,
+                                float *loss, void *grad, int64_t grad_stride, float *clip_frac, int32_t *row_end,
+                                float *scratch, uint32_t *counter, void *stream) {
+  AA_REQUIRE(cov_mode == AA_COV_CLIP || cov_mode == AA_COV_KL, AA_ERR_ARG, "aa_grpo_loss_cov: unknown cov_mode %d",
+             cov_mode);
+  AA_REQUIRE(isfinite(cov_coef) && cov_coef >= 0.f, AA_ERR_ARG,
+             "aa_grpo_loss_cov: cov_coef must be finite and >= 0, got %g", cov_coef);
+  AA_REQUIRE(sel && sel_stride >= K, AA_ERR_ARG, "aa_grpo_loss_cov: sel must be given with a row stride >= K");
+  return grpo_loss("aa_grpo_loss_cov", true, log_probs, lp_stride, ref_log_probs, ref_stride, old_log_probs, old_stride,
+                   lp_dtype, advantages, completion_tokens, tok_stride, eos_id, B, K, beta, clip_low, clip_high, 0.f,
+                   loss_agg, kl_estimator, mode, loss, grad, grad_stride, clip_frac, row_end, scratch, counter, stream,
+                   false, false, nullptr, 0, nullptr, cov_mode, cov_coef, sel, sel_stride);
 }
 
 extern "C" int aa_nll_mean(const void *logp, int dtype, const int64_t *labels, int64_t n, int64_t ignore_index,

@@ -102,6 +102,34 @@ __device__ __forceinline__ void actor_token(float x, float old, float aux, bool 
   grad = round_to(gs * ratio, rx);  // ExpBackward: grad * result
 }
 
+// One token of Clip-Cov / KL-Cov (verl's compute_policy_loss_clip_cov / _kl_cov; tests/cov_port.py is the
+// specification), `sel` the token's bit of the covariance selection:
+//   AA_COV_CLIP  actor_token's clip-higher objective (no dual-clip); a selected token's objective and gradient are 0
+//   AA_COV_KL    the unclipped s = adv * ratio; a selected token takes s - kl_coef * |x - old|, whose gradient
+//                through |.| is sign(x - old) (0 at 0)
+// x, old, aux, on, g_rs, rx, rp, obj, grad, why: as actor_token's (KL-Cov clips nothing: why = 0).
+__device__ __forceinline__ void cov_token(int mode, float x, float old, float aux, bool on, bool sel, float g_rs,
+                                          float eps_lo, float eps_hi, float kl_coef, int rx, int rp, float &obj,
+                                          float &grad, int &why) {
+  if (mode == AA_COV_CLIP) {
+    actor_token(x, old, aux, on, g_rs, eps_lo, eps_hi, 0.f, rx, rp, rp, obj, grad, why);
+    if (sel) obj = grad = 0.f;
+    return;
+  }
+  const float d = round_to(x - old, rx);
+  const float ratio = round_to(expf(d), rx);
+  obj = round_to(aux * ratio, rp);
+  why = 0;
+  grad = 0.f;
+  if (sel) obj = round_to(obj - round_to(kl_coef * fabsf(d), rx), rp);
+  if (!on) return;
+  grad = round_to(round_to(round_to(g_rs * aux, rp), rx) * ratio, rx);  // through the ratio (ExpBackward)
+  if (sel && d != 0.f) {  // through -kl_coef * |d|: MulBackward by the scalar, then AbsBackward's sign
+    const float ga = round_to(-g_rs * kl_coef, rx);
+    grad = round_to(grad + (d > 0.f ? ga : -ga), rx);
+  }
+}
+
 // ---- KL estimators (ops.KL_ESTIMATORS; tests/kl_objective_port.py is their specification) ---------------------
 // One token's estimate of KL(policy || reference) from the log-probs lp and rf, each op rounded to `r` as the eager
 // expression rounds it:
@@ -193,6 +221,19 @@ __device__ __forceinline__ void grpo_obj_token(float lp, float old, float rf, fl
   const float kl = kl_value(lp, rf, est, r, aux);
   const float bk = round_to(beta * kl, r);
   ptl = -(s * keep - bk);
+  grad = 0.f;
+  if (on) grad = kl_grad(ga, round_to(round_to(g_t, r) * beta, r), est, aux, r);
+}
+
+// One token of GRPO under Clip-Cov / KL-Cov (aa_grpo_loss_cov): -(s - beta * KL) with cov_token's s (fp32, as
+// grpo_obj_token's) and grpo_obj_token's KL and accumulation order
+__device__ __forceinline__ void grpo_cov_token(int mode, float lp, float old, float rf, float A, bool on, bool sel,
+                                               float g_t, float beta, float eps_lo, float eps_hi, float kl_coef,
+                                               int est, int r, float &ptl, float &grad, int &why) {
+  float s, ga, aux;
+  cov_token(mode, lp, old, A, on, sel, -g_t, eps_lo, eps_hi, kl_coef, r, AA_F32, s, ga, why);
+  const float kl = kl_value(lp, rf, est, r, aux);
+  ptl = -(s - round_to(beta * kl, r));
   grad = 0.f;
   if (on) grad = kl_grad(ga, round_to(round_to(g_t, r) * beta, r), est, aux, r);
 }

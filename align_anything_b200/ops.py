@@ -11,6 +11,7 @@ plumbing only; all arithmetic on the path runs in the hand-written sm_90a kernel
 """
 from __future__ import annotations
 
+import ctypes
 import dataclasses
 import functools
 import math
@@ -1260,14 +1261,14 @@ class _GrpoLossFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj=None, old=None, clip_frac=None,
-                sequence=False, topent=None):
+                sequence=False, topent=None, cov=None):
         B, K = lp.shape
         dev = lp.device
         loss = torch.empty(1, dtype=torch.float32, device=dev)
         grad = torch.empty((B, K), dtype=lp.dtype, device=dev)
         row_end = torch.empty(B, dtype=torch.int32, device=dev)
         _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
-                          sequence=sequence, topent=topent)
+                          sequence=sequence, topent=topent, cov=cov)
         ctx.save_for_backward(grad)
         ctx.mark_non_differentiable(row_end)
         return loss[0], row_end
@@ -1275,17 +1276,20 @@ class _GrpoLossFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g, _):
         (grad,) = ctx.saved_tensors
-        return (grad.float() * g.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None, None, None
+        return (grad.float() * g.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None, None, None, \
+            None
 
 
 def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
-                      scratch=None, sequence=False, topent=None):
+                      scratch=None, sequence=False, topent=None, cov=None):
     """GRPO's loss kernel, writing loss, row_end and (unless None) grad.  obj None: the reference loss (aa_grpo_loss);
     otherwise obj = _grpo_objective_args(...) for aa_grpo_loss_obj (aa_grpo_loss_kl unless the KL is k3), old = the old log-probs (None: the log-probs
     themselves, ratio 1) and clip_frac = an fp32[2] tensor for the clip fractions or None.  sequence (see
     _sequence_level; old is then given): GSPO's sequence-level ratio, aa_grpo_loss_seq.  topent: (entropy (B, K) fp32,
     thr fp32[1]) for the top-entropy mask, aa_grpo_loss_topent at either level (obj is then given).  scratch (fp32): the token
-    count and the row sums, B + 1 values, and under the objective the rows' clip counts too, 1 + 4 B; None allocates it."""
+    count and the row sums, B + 1 values, and under the objective the rows' clip counts too, 1 + 4 B; None allocates it.
+    cov (_CovTerm, obj given, token level): Clip-Cov / KL-Cov, the selection over GRPO's completion mask
+    (grpo_row_end) then aa_grpo_loss_cov."""
     B, K = lp.shape
     dev = lp.device
     if scratch is None:
@@ -1297,6 +1301,11 @@ def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old
     tail = (row_end.data_ptr(), scratch.data_ptr(), _device_scratch(dev)['counter'][5:7].data_ptr(), L.stream_ptr(dev))
     if obj is None:
         L.check(lib.aa_grpo_loss(*lps, *rows, mode_code, *out, *tail))
+    elif cov is not None:
+        sel = _cov_select(lp, adv, old, None, grpo_row_end(tokens, eos_id), cov, obj[0], obj[1], mode_code)
+        L.check(lib.aa_grpo_loss_cov(*lps, L.ptr(old), old.stride(0) if old is not None else 0, *rows, obj[0], obj[1],
+                                     obj[3], obj[4], cov.code, cov.coef, sel.data_ptr(), sel.stride(0), mode_code, *out,
+                                     L.ptr(clip_frac), *tail))
     elif topent is not None:
         ent, thr = topent
         L.check(lib.aa_grpo_loss_topent(*lps, L.ptr(old), old.stride(0) if old is not None else 0, *rows, *obj,
@@ -1440,7 +1449,7 @@ def _old_log_probs(old, shape, dtype):
 def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, advantages: torch.Tensor,
               completion_tokens: torch.Tensor, eos_token_id: int, beta: float, mode: str | None = None, *,
               objective: GrpoObjective | None = None, old_per_token_logps: torch.Tensor | None = None,
-              return_clip_fraction: bool = False, entropy: torch.Tensor | None = None):
+              return_clip_fraction: bool = False, entropy: torch.Tensor | None = None, cov_seed: int = 0):
     """The loss of GRPOTrainer.train_step (trainers/text_to_text/grpo.py:290-312): per-token k3 KL, per-token loss
     -(exp(lp - lp.detach()) * A - beta * KL), completion mask up to the first eos, token mean -> fp32 scalar,
     differentiable in per_token_logps.  Returns (loss, counted_tokens_per_row).
@@ -1450,7 +1459,10 @@ def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, 
     old log-probs: today's launch.  return_clip_fraction appends the fp32[2] clip fractions.
     An objective with top_entropy_quantile = rho < 1 also needs `entropy`, the policy's fp32 entropy (B, K) of the same
     pass: only the counted tokens with entropy >= entropy_quantile_threshold(entropy, row_end, 1 - rho) (over every
-    data-parallel rank) keep the policy term s; the others carry the KL term alone (aa_grpo_loss_topent)."""
+    data-parallel rank) keep the policy term s; the others carry the KL term alone (aa_grpo_loss_topent).
+    An objective with policy_loss_mode clip_cov / kl_cov: the selection of cov_token_selection over the completion mask
+    (Clip-Cov hashes with cov_seed, see cov_hash_seed), then aa_grpo_loss_cov; its fp32 (1,) selected share follows
+    row_end, before the clip fractions."""
     L.require_cuda(per_token_logps, ref_per_token_logps, advantages, completion_tokens)
     obj = _grpo_objective_args(objective, old_per_token_logps, return_clip_fraction)
     if per_token_logps.dim() != 2 or per_token_logps.shape != ref_per_token_logps.shape or \
@@ -1465,8 +1477,11 @@ def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, 
     tok = _contiguous_last(completion_tokens.to(torch.int64))
     cf = torch.zeros(2, dtype=torch.float32, device=lp.device) if return_clip_fraction else None
     topent = _top_entropy_args(objective, entropy, tok, eos_token_id, lp.shape)
+    cov = _cov_term(_objective(objective, GrpoObjective), cov_seed, lp.device)
     out = _GrpoLossFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype), obj, old, cf,
-                            _sequence_level(objective, old), topent)
+                            _sequence_level(objective, old), topent, cov)
+    if cov is not None:
+        out += (cov.share,)
     return out + (cf,) if return_clip_fraction else out
 
 
@@ -1570,7 +1585,7 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
                           ref_per_token_logps: torch.Tensor, advantages: torch.Tensor, eos_token_id: int, beta: float,
                           mode: str | None = None, return_entropy: bool = False, entropy_coeff: float = 0.0, *,
                           objective: GrpoObjective | None = None, old_per_token_logps: torch.Tensor | None = None,
-                          return_clip_fraction: bool = False):
+                          return_clip_fraction: bool = False, cov_seed: int = 0):
     """`_get_per_token_logps` of the policy + the loss of GRPOTrainer.train_step (trainers/text_to_text/grpo.py:205-210,
     290-312) from the policy's logits; the reference model's per-token log-probs must already be there.
     -> (loss fp32 scalar, policy per-token log-probs (B, K), counted tokens per row).  With a gradient: one pass over the
@@ -1584,15 +1599,17 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
     aa_grpo_loss_obj -> K1b); the entropy bonus stays a token mean over the completion mask.  A sequence-level objective
     with old log-probs always takes the composed path (K1 -> aa_grpo_loss_seq -> K1b, see _sequence_level), and so does
     top_entropy_quantile < 1 (K1's entropy variant -> the entropy threshold -> aa_grpo_loss_topent -> K1b, see
-    _top_entropy).  return_clip_fraction appends the fp32[2] clip fractions last.  None / default fields and no old log-probs: today's
-    launches."""
+    _top_entropy), and so does policy_loss_mode clip_cov / kl_cov (K1 -> selection -> aa_grpo_loss_cov -> K1b, seeded
+    by cov_seed; the fp32 (1,) selected share is appended before the clip fractions).  return_clip_fraction appends
+    the fp32[2] clip fractions last.  None / default fields and no old log-probs: today's launches."""
     L.require_cuda(logits, input_ids, ref_per_token_logps, advantages)
     obj = _grpo_objective_args(objective, old_per_token_logps, return_clip_fraction)
     K = int(logits_to_keep)
     tokens = input_ids[:, -K:]
     coeff = float(entropy_coeff)
     topent = _top_entropy(objective)
-    if _sequence_level(objective, old_per_token_logps) or topent or \
+    cov = getattr(objective, 'policy_loss_mode', 'vanilla') != 'vanilla'
+    if _sequence_level(objective, old_per_token_logps) or topent or cov or \
             not _single_pass_ok(logits, _FUSED_GRPO, torch.is_grad_enabled() and logits.requires_grad):
         ent = None
         if return_entropy or coeff != 0.0 or topent:
@@ -1602,7 +1619,8 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
             lp = tail_token_log_probs(logits, input_ids, K, mode=mode)
         scored = grpo_loss(lp, ref_per_token_logps, advantages, tokens, eos_token_id, beta, mode=mode,
                            objective=objective, old_per_token_logps=old_per_token_logps,
-                           return_clip_fraction=return_clip_fraction, **({'entropy': ent} if topent else {}))
+                           return_clip_fraction=return_clip_fraction, cov_seed=cov_seed,
+                           **({'entropy': ent} if topent else {}))
         loss, row_end = scored[0], scored[1]
         out = (loss, lp.detach(), row_end)
         if coeff != 0.0:
@@ -1610,7 +1628,9 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
             out = (loss - coeff * h_mean, lp.detach(), row_end, h_mean.detach(), loss.detach())
         if return_entropy:
             out += (ent.detach(),)
-        return out + (scored[2],) if return_clip_fraction else out
+        if cov:
+            out += (scored[2],)
+        return out + (scored[-1],) if return_clip_fraction else out
     B, seq, _ = logits.shape
     if not 0 < K < seq:
         raise ValueError('logits_to_keep must lie in (0, L)')
@@ -2309,6 +2329,9 @@ def whiten_advantages(advantages: list[torch.Tensor], masks: list[torch.Tensor],
 
 
 LOSS_AGG_MODES = {'seq-mean-token-mean': 0, 'token-mean': 1}  # include/aa_b200.h AA_AGG_*
+POLICY_LOSS_MODES = {'vanilla': 0, 'clip_cov': 1, 'kl_cov': 2}  # include/aa_b200.h AA_COV_*
+# verl's defaults of the Clip-Cov / KL-Cov keys (ActorObjective: None takes these)
+COV_DEFAULTS = {'clip_cov_ratio': 2e-4, 'clip_cov_lb': 1.0, 'clip_cov_ub': 5.0, 'kl_cov_ratio': 2e-4, 'ppo_kl_coef': 1.0}
 
 
 @dataclasses.dataclass(frozen=True)
@@ -2322,12 +2345,27 @@ class ActorObjective:
              = -(s * mask).sum() / mask.sum()       ('token-mean': mean over the micro-batch's response tokens)
 
     clip_range_ratio_low / _high: None takes the trainer's clip_range_ratio (clip-higher: high > low); dual_clip_ratio:
-    None = off, otherwise c > 1.  The fields are checked here, on the host, before anything is launched."""
+    None = off, otherwise c > 1.
+    policy_loss_mode (Cui et al. 2025; verl's policy_loss.loss_mode): 'vanilla' (the above), 'clip_cov' or 'kl_cov'.
+    Over the counted tokens of one loss call, cov_t = (A_t - mean A) * (lp_t - mean lp) (fp64 means rounded to fp32,
+    the product fp32; cov_token_selection).  'clip_cov': among the counted, unclipped tokens with
+    clip_cov_lb < cov_t < clip_cov_ub, max(int(clip_cov_ratio * N), 1) (N = counted tokens) chosen by a hash of the
+    flat index and the seed lose their objective term and its gradient.  'kl_cov': the objective is unclipped, s = A *
+    ratio, and the max(1, int(kl_cov_ratio * N)) tokens with the largest cov_t take s - ppo_kl_coef * |lp - old|.  The
+    five keys are None for their defaults (2e-4, 1.0, 5.0, 2e-4, 1.0) and refused under 'vanilla'; neither mode takes
+    dual_clip_ratio, and 'kl_cov' refuses an explicit clip range, which it would ignore.  The fields are checked here,
+    on the host, before anything is launched."""
 
     clip_range_ratio_low: float | None = None
     clip_range_ratio_high: float | None = None
     dual_clip_ratio: float | None = None
     loss_agg_mode: str = 'seq-mean-token-mean'
+    policy_loss_mode: str = 'vanilla'
+    clip_cov_ratio: float | None = None
+    clip_cov_lb: float | None = None
+    clip_cov_ub: float | None = None
+    kl_cov_ratio: float | None = None
+    ppo_kl_coef: float | None = None
     _MODES = LOSS_AGG_MODES  # the aggregations this objective takes (a class attribute, not a field)
 
     def __post_init__(self):
@@ -2340,12 +2378,45 @@ class ActorObjective:
             raise ValueError(f'dual_clip_ratio must be None (off) or a finite value > 1, got {c!r}')
         if self.loss_agg_mode not in self._MODES:
             raise ValueError(f'loss_agg_mode must be one of {sorted(self._MODES)}, got {self.loss_agg_mode!r}')
+        self._check_cov()
+
+    def _check_cov(self):
+        mode = self.policy_loss_mode
+        if mode not in POLICY_LOSS_MODES:
+            raise ValueError(f'policy_loss_mode must be one of {tuple(POLICY_LOSS_MODES)}, got {mode!r}')
+        keys = {k: getattr(self, k) for k in COV_DEFAULTS}
+        if mode == 'vanilla':
+            given = [k for k, v in keys.items() if v is not None]
+            if given:
+                raise ValueError(f'{", ".join(given)} need policy_loss_mode clip_cov or kl_cov (it is vanilla)')
+            return
+        for k, v in keys.items():
+            if v is not None and (isinstance(v, bool) or not isinstance(v, (int, float))):
+                raise ValueError(f'{k} must be a number, got {v!r}')
+        if self.dual_clip_ratio is not None:
+            raise ValueError(f'policy_loss_mode {mode!r} has no dual-clip: dual_clip_ratio must be unset')
+        if mode == 'kl_cov' and (self.clip_range_ratio_low is not None or self.clip_range_ratio_high is not None):
+            raise ValueError('policy_loss_mode kl_cov is unclipped: clip_range_ratio_low / _high would be ignored')
+        for k in ('clip_cov_ratio', 'kl_cov_ratio'):
+            if not 0.0 < self.cov_value(k) <= 1.0:
+                raise ValueError(f'{k} must lie in (0, 1], got {keys[k]!r}')
+        lb, ub = self.cov_value('clip_cov_lb'), self.cov_value('clip_cov_ub')
+        if not (math.isfinite(lb) and math.isfinite(ub) and lb < ub):
+            raise ValueError(f'clip_cov_lb < clip_cov_ub must be finite, got {lb!r}, {ub!r}')
+        c = self.cov_value('ppo_kl_coef')
+        if not (math.isfinite(c) and c >= 0.0):
+            raise ValueError(f'ppo_kl_coef must be finite and >= 0, got {c!r}')
+
+    def cov_value(self, key: str) -> float:
+        """One of the Clip-Cov / KL-Cov keys in effect: the field, or its default (COV_DEFAULTS) when None."""
+        v = getattr(self, key)
+        return float(COV_DEFAULTS[key] if v is None else v)
 
     @property
     def is_default(self) -> bool:
         """The reference's objective: the kernels run today's launches."""
         return (self.clip_range_ratio_low is None and self.clip_range_ratio_high is None and self.dual_clip_ratio is None
-                and self.loss_agg_mode == 'seq-mean-token-mean')
+                and self.loss_agg_mode == 'seq-mean-token-mean' and self.policy_loss_mode == 'vanilla')
 
     @property
     def token_mean(self) -> bool:
@@ -2385,8 +2456,10 @@ class GrpoObjective(ActorObjective):
     log-probs w is 1 and the token-level launches run.  top_entropy_quantile rho in [0, 1] (Wang et al. 2025; TRL's
     top_entropy_quantile): only the counted tokens whose policy entropy H is >= torch.quantile(H[counted], 1 - rho)
     over every rank keep s, per-token loss = -(s * keep - beta * KL); the denominators, the KL term, the entropy bonus,
-    GSPO's ratio and the clip fractions stay over the whole completion mask.  1 (the default) masks nothing.  Checked
-    on the host when constructed."""
+    GSPO's ratio and the clip fractions stay over the whole completion mask.  1 (the default) masks nothing.
+    policy_loss_mode 'clip_cov' / 'kl_cov' (ActorObjective) over the completion mask with the row's advantage, per-token
+    loss -(s - beta * KL); token level only.  On the first update (ratio 1) KL-Cov selects tokens but changes nothing:
+    |lp - old| = 0 and its gradient sign(0) = 0.  Checked on the host when constructed."""
 
     loss_agg_mode: str = 'token-mean'
     clip_range_ratio: float = 0.2
@@ -2405,13 +2478,17 @@ class GrpoObjective(ActorObjective):
         rho = self.top_entropy_quantile
         if isinstance(rho, bool) or not isinstance(rho, (int, float)) or not 0.0 <= float(rho) <= 1.0:
             raise ValueError(f'top_entropy_quantile must be a number in [0, 1], got {rho!r}')
+        if self.policy_loss_mode != 'vanilla' and (self.sequence_level or rho < 1.0):
+            raise ValueError(f'policy_loss_mode {self.policy_loss_mode!r} is token-level and takes every token: it '
+                             f'refuses importance_sampling_level="sequence" and top_entropy_quantile < 1')
 
     @property
     def is_default(self) -> bool:
         """The reference's loss when the ratio is 1: the kernels run today's launches."""
         return (self.clip_range_ratio_low is None and self.clip_range_ratio_high is None and self.dual_clip_ratio is None
                 and self.loss_agg_mode == 'token-mean' and self.kl_estimator == 'k3'
-                and self.importance_sampling_level == 'token' and self.top_entropy_quantile == 1.0)
+                and self.importance_sampling_level == 'token' and self.top_entropy_quantile == 1.0
+                and self.policy_loss_mode == 'vanilla')
 
     @property
     def sequence_level(self) -> bool:
@@ -2431,19 +2508,152 @@ def _objective(objective: ActorObjective | None, cls: type = ActorObjective) -> 
     return None if objective.is_default else objective
 
 
+_U32 = 0xffffffff
+
+
+def _fmix32(h: int) -> int:
+    """MurmurHash3's 32-bit finaliser (the device's fmix32)."""
+    h &= _U32
+    h ^= h >> 16
+    h = (h * 0x85ebca6b) & _U32
+    h ^= h >> 13
+    h = (h * 0xc2b2ae35) & _U32
+    return h ^ (h >> 16)
+
+
+def cov_hash_seed(seed: int, rank: int, call: int) -> int:
+    """Clip-Cov's 32-bit hash seed s = fmix32(fmix32(fmix32(seed) ^ rank) ^ call): `seed` the run's seed, `rank` the
+    data-parallel rank, `call` the count of the trainer's earlier Clip-Cov loss calls.  Token t of the call is chosen
+    by its key fmix32(t ^ s), so the choice is reproducible without RNG state (and differs from verl's
+    torch.randperm stream)."""
+    return _fmix32(_fmix32(_fmix32(int(seed)) ^ (int(rank) & _U32)) ^ (int(call) & _U32))
+
+
+class _CovTerm:
+    """Clip-Cov / KL-Cov of one loss call: the mode's AA_COV_* code, the selection ratio, Clip-Cov's bounds and
+    KL-Cov's coefficient (an ActorObjective's values in effect), the hash seed, and `share`, the fp32[1] the selection
+    writes the selected share of the counted tokens into."""
+
+    def __init__(self, objective: ActorObjective, seed: int, device):
+        self.code = POLICY_LOSS_MODES[objective.policy_loss_mode]
+        clip = self.code == POLICY_LOSS_MODES['clip_cov']
+        self.ratio = objective.cov_value('clip_cov_ratio' if clip else 'kl_cov_ratio')
+        self.lb, self.ub = objective.cov_value('clip_cov_lb'), objective.cov_value('clip_cov_ub')
+        self.coef = 0.0 if clip else objective.cov_value('ppo_kl_coef')
+        self.seed = int(seed) & _U32
+        self.share = torch.empty(1, dtype=torch.float32, device=device)
+
+
+def _cov_term(objective, seed: int, device) -> _CovTerm | None:
+    """None unless the objective's policy_loss_mode is clip_cov or kl_cov."""
+    if objective is None or objective.policy_loss_mode == 'vanilla':
+        return None
+    return _CovTerm(objective, seed, device)
+
+
+def _cov_select(x, aux, old, mask, row_end, cov: _CovTerm, clip_lo: float, clip_hi: float, mode_code: int):
+    """The selection of one loss call -> uint8 (B, W), and cov.share: aa_cov_moments -> aa_cov_keys ->
+    aa_cov_select_hi -> aa_cov_hist_lo -> aa_cov_select_lo -> aa_cov_mark, no host sync.  x: the log-probs the loss
+    kernel reads; with `mask` (PPO) aux holds (B, W) advantages, with `row_end` (GRPO) fp32 (B,) ones."""
+    B, W = x.shape
+    dev = x.device
+    state = torch.empty(16, dtype=torch.int32, device=dev)  # uint32 words
+    keys = torch.empty(B * W, dtype=torch.int32, device=dev)
+    elig = torch.empty(B * W, dtype=torch.uint8, device=dev)
+    hist = torch.empty(_ENT_BINS, dtype=torch.int32, device=dev)
+    ties = torch.empty(B, dtype=torch.int32, device=dev)
+    sel = torch.empty((B, W), dtype=torch.uint8, device=dev)
+    lib, stream = L.lib(), L.stream_ptr(dev)
+    rows = (x.data_ptr(), x.stride(0), L.dtype_code(x.dtype), aux.data_ptr(), aux.stride(0) if mask is not None else 0,
+            L.dtype_code(aux.dtype), L.ptr(mask), mask.stride(0) if mask is not None else 0, L.ptr(row_end), B, W)
+    L.check(lib.aa_cov_moments(*rows, state.data_ptr(), stream))
+    L.check(lib.aa_cov_keys(cov.code, *rows[:2], L.ptr(old), old.stride(0) if old is not None else 0, *rows[2:],
+                            float(clip_lo), float(clip_hi), cov.lb, cov.ub, cov.seed, mode_code, state.data_ptr(),
+                            keys.data_ptr(), elig.data_ptr(), hist.data_ptr(), stream))
+    L.check(lib.aa_cov_select_hi(hist.data_ptr(), ctypes.byref(ctypes.c_double(cov.ratio)), state.data_ptr(), stream))
+    L.check(lib.aa_cov_hist_lo(keys.data_ptr(), elig.data_ptr(), B * W, state.data_ptr(), hist.data_ptr(), stream))
+    L.check(lib.aa_cov_select_lo(hist.data_ptr(), state.data_ptr(), cov.share.data_ptr(), stream))
+    L.check(lib.aa_cov_mark(keys.data_ptr(), elig.data_ptr(), B, W, state.data_ptr(), ties.data_ptr(), sel.data_ptr(),
+                            sel.stride(0), stream))
+    return sel
+
+
+def cov_token_selection(log_probs: torch.Tensor, advantages: torch.Tensor, mask_or_row_end: torch.Tensor,
+                        policy_loss_mode: str, *, old_log_probs: torch.Tensor | None = None,
+                        clip_range_ratio_low: float = 0.2, clip_range_ratio_high: float = 0.2,
+                        clip_cov_ratio: float | None = None, clip_cov_lb: float | None = None,
+                        clip_cov_ub: float | None = None, kl_cov_ratio: float | None = None, seed: int = 0,
+                        mode: str | None = None, return_share: bool = False):
+    """The tokens Clip-Cov or KL-Cov selects in one loss call (see ActorObjective) -> uint8 (B, W), 1 = selected;
+    return_share: and the fp32 (1,) selected share of the counted tokens (0 when none is counted).
+    log_probs (B, W) fp32 / bf16 / fp16, the current log-probs as the loss kernel reads them; mask_or_row_end: a
+    (B, W) mask with (B, W) advantages (PPO), or int (B,) counted tokens per row (t < row_end[b], GRPO's completion
+    mask: grpo_row_end) with one advantage per row.  Clip-Cov: old_log_probs (None: ratio 1) and the clip range give
+    the clipped tokens, `seed` the 32-bit hash seed (cov_hash_seed), `mode` the ratio's rounding.  The selection is
+    local to this call (no collective) and exact: a radix select on 32-bit keys with ties to the smaller flat index.
+    Bad arguments raise ValueError here, before any launch."""
+    keys = {'clip_cov_ratio': clip_cov_ratio, 'clip_cov_lb': clip_cov_lb, 'clip_cov_ub': clip_cov_ub,
+            'kl_cov_ratio': kl_cov_ratio}
+    if policy_loss_mode not in ('clip_cov', 'kl_cov'):
+        raise ValueError(f'cov_token_selection: policy_loss_mode must be clip_cov or kl_cov, got {policy_loss_mode!r}')
+    objective = ActorObjective(policy_loss_mode=policy_loss_mode, **keys)
+    for name, t in (('log_probs', log_probs), ('advantages', advantages), ('mask_or_row_end', mask_or_row_end)):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f'cov_token_selection: {name} must be a tensor')
+    if log_probs.dim() != 2 or log_probs.numel() == 0 or log_probs.dtype not in (torch.float32, torch.bfloat16,
+                                                                                 torch.float16):
+        raise ValueError(f'cov_token_selection: log_probs must be a non-empty fp32 / bf16 / fp16 (B, W) tensor, got '
+                         f'{log_probs.dtype} {tuple(log_probs.shape)}')
+    B, W = log_probs.shape
+    if B * W > 2 ** 31 - 1:
+        raise ValueError(f'cov_token_selection: B * W = {B * W} exceeds 2^31 - 1')
+    m = mask_or_row_end
+    if tuple(m.shape) == (B, W):
+        if tuple(advantages.shape) != (B, W):
+            raise ValueError(f'cov_token_selection: with a mask the advantages must be (B, W) = ({B}, {W})')
+        mask, row_end = _contiguous_last((m != 0).to(torch.uint8)), None
+        aux = _contiguous_last(advantages.detach())
+        if aux.dtype not in (torch.float32, torch.bfloat16, torch.float16):
+            aux = aux.float()
+    elif tuple(m.shape) == (B,) and not m.dtype.is_floating_point and m.dtype != torch.bool:
+        if advantages.numel() != B:
+            raise ValueError(f'cov_token_selection: with row ends one advantage per row ({B}) is expected')
+        mask, row_end = None, m.to(torch.int32).contiguous()
+        aux = advantages.detach().float().contiguous().view(-1)
+    else:
+        raise ValueError(f'cov_token_selection: mask_or_row_end must be a (B, W) = ({B}, {W}) mask or integer (B,) row '
+                         f'ends, got {m.dtype} {tuple(m.shape)}')
+    if old_log_probs is not None and tuple(old_log_probs.shape) != (B, W):
+        raise ValueError(f'cov_token_selection: old_log_probs must be (B, W) = ({B}, {W})')
+    lo, hi = float(clip_range_ratio_low), float(clip_range_ratio_high)
+    if not (0.0 <= lo < 1.0 and hi >= 0.0):
+        raise ValueError(f'cov_token_selection: clip range [1 - {lo}, 1 + {hi}]: need 0 <= low < 1 and high >= 0')
+    try:
+        L.require_cuda(log_probs, advantages, m, *((old_log_probs,) if old_log_probs is not None else ()))
+    except RuntimeError as e:
+        raise ValueError(f'cov_token_selection: {e}') from None
+    x = _contiguous_last(log_probs.detach())
+    old = _contiguous_last(old_log_probs.detach().to(x.dtype)) if old_log_probs is not None else None
+    cov = _CovTerm(objective, seed, x.device)
+    sel = _cov_select(x, aux, old, mask, row_end, cov, lo, hi, _mode_code(mode, x.dtype))
+    return (sel, cov.share) if return_share else sel
+
+
 def token_mean(x: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
     """(x * mask).sum() / mask.sum() over the whole (B, W) tensor -> fp32 scalar (NaN without a masked-in token): the
     masked_mean kernel on the tensor as one row, differentiable in x."""
     return masked_mean(x.reshape(1, -1), mask.reshape(1, -1))
 
 
-def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=None, obj=None, clip_frac=None, kl=None):
+def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=None, obj=None, clip_frac=None, kl=None,
+                     cov=None):
     """K5: -> (loss fp32[2], loss as a 0-dim tensor of the promoted dtype (a view, no launch), grad (B, Wm), row_mean).
     x_tail = (DeviceLens, src_width): `x` is the raw (B, src_width) tensor and the kernel reads the per-sample tails.
     Actor only: obj = ActorObjective.args(...) (None: the reference's objective), clip_frac = an fp32[2] tensor the
     kernel fills with the clip fractions (aa_ppo_actor_loss_obj); kl = _KlLossTerm: the KL loss term
     (aa_ppo_actor_loss_kl: grad is d (loss + coeff * agg(KL)) / d x, kl.out receives agg(KL), `loss` stays the
-    clipped objective)."""
+    clipped objective).  cov = _CovTerm (obj given): Clip-Cov / KL-Cov, the selection (_cov_select) then
+    aa_ppo_actor_loss_cov, with the KL loss term when kl is given."""
     B, Wm = old.shape
     dev = x.device
     loss = torch.empty(2, dtype=torch.float32, device=dev)
@@ -2452,7 +2662,19 @@ def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=Non
     row_mean = torch.empty(B, dtype=torch.float32, device=dev)
     sc = _device_scratch(dev)
     lib = L.lib()
-    if actor and kl is not None:
+    if actor and cov is not None:
+        lo, hi, _, agg = obj
+        sel = _cov_select(x, aux, old, mask, None, cov, lo, hi, mode_code)
+        rows = torch.empty(5 * B, dtype=torch.float32, device=dev)
+        L.check(lib.aa_ppo_actor_loss_cov(
+            x.data_ptr(), x.stride(0), old.data_ptr(), old.stride(0), L.dtype_code(x.dtype), aux.data_ptr(),
+            aux.stride(0), L.dtype_code(aux.dtype), mask.data_ptr(), mask.stride(0), B, Wm, float(lo), float(hi),
+            int(agg), cov.code, cov.coef, sel.data_ptr(), sel.stride(0), mode_code,
+            kl.ref.data_ptr() if kl is not None else None, kl.ref.stride(0) if kl is not None else 0,
+            kl.coeff if kl is not None else 0.0, kl.estimator if kl is not None else 0, loss.data_ptr(),
+            kl.out.data_ptr() if kl is not None else None, grad.data_ptr(), grad.stride(0), L.ptr(clip_frac),
+            rows.data_ptr(), sc['counter'][2:3].data_ptr(), L.stream_ptr(dev)))
+    elif actor and kl is not None:
         lo, hi, dual, agg = obj if obj is not None else (clip, clip, 0.0, 0)
         rows = torch.empty(5 * B, dtype=torch.float32, device=dev)
         L.check(lib.aa_ppo_actor_loss_kl(
@@ -2492,9 +2714,9 @@ class _PpoLossFn(torch.autograd.Function):
     (kl, actor only) the first output is  loss + kl.coeff * agg(KL)  (fp32) and its gradient is K5's."""
 
     @staticmethod
-    def forward(ctx, x, old, aux, mask, clip, mode_code, actor: bool, obj=None, clip_frac=None, kl=None):
+    def forward(ctx, x, old, aux, mask, clip, mode_code, actor: bool, obj=None, clip_frac=None, kl=None, cov=None):
         loss, cast, grad, row_mean = _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor, obj=obj,
-                                                      clip_frac=clip_frac, kl=kl)
+                                                      clip_frac=clip_frac, kl=kl, cov=cov)
         ctx.save_for_backward(grad)
         ctx.mark_non_differentiable(row_mean, loss)
         return (cast if kl is None else kl.regularised(loss[0])), row_mean, loss
@@ -2502,7 +2724,7 @@ class _PpoLossFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_loss, _g, _l):
         (grad,) = ctx.saved_tensors
-        return (grad.float() * g_loss.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None
+        return (grad.float() * g_loss.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None, None
 
 
 def _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, grad, obj, coeff, ent, kl=None):
@@ -2552,11 +2774,13 @@ class _TailActorLossFn(torch.autograd.Function):
     (aa_ppo_actor_loss_obj); under token-mean the entropy term is a token mean too.  clip_frac: an fp32[2] tensor K5
     fills with the clip fractions.  kl (_KlLossTerm): the node's loss gains  + kl.coeff * agg(KL)  (fp32; the third
     output stays the actor loss without it), K1f's KL entry point (aa_logprob_actor_fused_kl) writes its gradient into
-    the tile, K5's (aa_ppo_actor_loss_kl) the loss value, agg(KL) into kl.out and, for K1b, d total / d log-probs."""
+    the tile, K5's (aa_ppo_actor_loss_kl) the loss value, agg(KL) into kl.out and, for K1b, d total / d log-probs.
+    cov (_CovTerm, with single_pass False): Clip-Cov / KL-Cov -- the selection needs every log-prob of the call first,
+    so K1 -> selection -> aa_ppo_actor_loss_cov -> K1b."""
 
     @staticmethod
     def forward(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, single_pass, entropy_coeff=0.0, objective=None,
-                clip_frac=None, kl=None):
+                clip_frac=None, kl=None, cov=None):
         out_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         dev = logits.device
         coeff = float(entropy_coeff)
@@ -2574,7 +2798,7 @@ class _TailActorLossFn(torch.autograd.Function):
             stats = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=dev)
             _launch_fwd(logits, ids, plan, lp, stats[0], stats[1], entropy=ent)
         loss, cast, grad_lp, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True, obj=obj, clip_frac=clip_frac,
-                                                  kl=kl)
+                                                  kl=kl, cov=cov)
         tm = objective is not None and objective.token_mean
         if not ctx.fused:
             if ctx.bonus:
@@ -2599,7 +2823,7 @@ class _TailActorLossFn(torch.autograd.Function):
     def backward(ctx, g_loss, *_unused):
         if ctx.fused:
             (grad,) = _hand_over_once(ctx, g_loss, *ctx.saved_tensors)
-            return grad, None, None, None, None, None, None, None, None, None, None, None, None
+            return grad, None, None, None, None, None, None, None, None, None, None, None, None, None
         scale = g_loss.detach().reshape(1)
         if scale.dtype not in (torch.float32, torch.bfloat16, torch.float16):
             scale = scale.float()
@@ -2611,7 +2835,7 @@ class _TailActorLossFn(torch.autograd.Function):
         grad = torch.empty(logits.shape, dtype=logits.dtype, device=logits.device)
         _launch_bwd(logits, ids, ctx.plan, stats[0], stats[1], grad_lp, None, scale, grad, ctx.mode_code, entropy=ent,
                     grad_entropy=g_h)
-        return grad, None, None, None, None, None, None, None, None, None, None, None, None
+        return grad, None, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 class _TailCriticLossFn(torch.autograd.Function):
@@ -2706,33 +2930,40 @@ def _loss_inputs(x, old, aux, mask):
 
 def actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio: float, mode: str | None = None,
                objective: ActorObjective | None = None, return_clip_fraction: bool = False, ref_log_probs=None,
-               kl_loss_coeff: float = 0.0, kl_loss_estimator: str = 'k3'):
+               kl_loss_coeff: float = 0.0, kl_loss_estimator: str = 'k3', cov_seed: int = 0):
     """PPOTrainer.actor_loss_fn (trainers/text_to_text/ppo.py:291-307), differentiable in log_probs.
     objective: an ActorObjective (None: the reference's).  return_clip_fraction: -> (loss, fp32[2] device tensor: the
     clipped fraction and the dual-clip fraction, aggregated like the loss; see aa_ppo_actor_loss_obj).
     kl_loss_coeff != 0 (a KL loss term, see _actor_loss): the loss is  actor_loss + kl_loss_coeff * agg(KL)  (fp32)
-    and the detached agg(KL) follows it, before the clip fractions."""
-    loss, _, kl, cf = _actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio, mode, objective,
-                                  return_clip_fraction, ref_log_probs, kl_loss_coeff, kl_loss_estimator)
-    out = (loss,) + ((kl,) if kl is not None else ()) + ((cf,) if return_clip_fraction else ())
+    and the detached agg(KL) follows it, before the clip fractions.  An objective with policy_loss_mode clip_cov /
+    kl_cov: the selection of cov_token_selection (Clip-Cov hashes with cov_seed, see cov_hash_seed) and K5's Cov entry
+    point; its fp32 (1,) selected share follows agg(KL), before the clip fractions."""
+    loss, _, kl, cf, share = _actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio, mode, objective,
+                                         return_clip_fraction, ref_log_probs, kl_loss_coeff, kl_loss_estimator, cov_seed)
+    out = (loss,) + ((kl,) if kl is not None else ()) + ((share,) if share is not None else ()) + \
+        ((cf,) if return_clip_fraction else ())
     return out if len(out) > 1 else loss
 
 
 def _actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio, mode, objective, return_clip_fraction,
-                ref_log_probs, kl_loss_coeff, kl_loss_estimator):
+                ref_log_probs, kl_loss_coeff, kl_loss_estimator, cov_seed: int = 0):
     """actor_loss -> (loss, the actor loss without the KL term for ppo_pack_metrics (the loss itself without the term,
-    K5's fp32[2] with it), the detached agg(KL) or None, clip fractions or None).  The KL loss term: KL(lp, ref) by
-    `kl_loss_estimator` (KL_ESTIMATORS), aggregated over the same mask as the objective (its loss_agg_mode), its
-    gradient added to K5's (aa_ppo_actor_loss_kl)."""
+    K5's fp32[2] with it), the detached agg(KL) or None, clip fractions or None, the Clip-Cov / KL-Cov selected share
+    or None).  The KL loss term: KL(lp, ref) by `kl_loss_estimator` (KL_ESTIMATORS), aggregated over the same mask as
+    the objective (its loss_agg_mode), its gradient added to K5's (aa_ppo_actor_loss_kl, or aa_ppo_actor_loss_cov
+    under Clip-Cov / KL-Cov)."""
     objective = _objective(objective)
     x, old, aux, m = _loss_inputs(log_probs, old_log_probs, advantages, mask)
     kl = _kl_loss_term(ref_log_probs, old_log_probs, kl_loss_coeff, kl_loss_estimator, x.dtype)
     obj = objective.args(clip_range_ratio) if objective is not None else None
+    cov = _cov_term(objective, cov_seed, x.device)
     cf = torch.zeros(2, dtype=torch.float32, device=x.device) if return_clip_fraction else None
-    loss, _, loss32 = _PpoLossFn.apply(x, old, aux, m, clip_range_ratio, _mode_code(mode, x.dtype), True, obj, cf, kl)
+    loss, _, loss32 = _PpoLossFn.apply(x, old, aux, m, clip_range_ratio, _mode_code(mode, x.dtype), True, obj, cf, kl,
+                                       cov)
+    share = cov.share if cov is not None else None
     if kl is None:
-        return loss, loss, None, cf
-    return loss, loss32, kl.out[0], cf
+        return loss, loss, None, cf, share
+    return loss, loss32, kl.out[0], cf, share
 
 
 def critic_loss(values, old_values, returns, mask, clip_range_value: float, mode: str | None = None,
@@ -2746,15 +2977,17 @@ def critic_loss(values, old_values, returns, mask, clip_range_value: float, mode
 def tail_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, lens, old_log_probs, advantages, mask,
                     clip_range_ratio: float, mode: str | None = None, entropy_coeff: float = 0.0,
                     objective: ActorObjective | None = None, return_clip_fraction: bool = False, ref_log_probs=None,
-                    kl_loss_coeff: float = 0.0, kl_loss_estimator: str = 'k3'):
+                    kl_loss_coeff: float = 0.0, kl_loss_estimator: str = 'k3', cov_seed: int = 0):
     """response_tail_log_probs + actor_loss as one autograd node (see _TailActorLossFn).
     -> (actor loss, new log-probs (B, W), the loss as fp32[2] for ppo_pack_metrics).  entropy_coeff != 0: the first
     output is  actor_loss - entropy_coeff * masked_mean(H, mask)  (fp32), the third stays the actor loss without the
     bonus, and the detached masked-mean entropy follows as a fourth.  objective: an ActorObjective (None: the
     reference's; under token-mean the entropy term is a token mean too).  kl_loss_coeff != 0 (a KL loss term, as
     actor_loss; ref_log_probs (B, W) aligned with old_log_probs): the first output gains  + kl_loss_coeff * agg(KL),
-    the third stays without it and the detached agg(KL) follows the entropy mean (if any).  return_clip_fraction: the
-    fp32[2] clip fractions (see actor_loss) follow as the last output."""
+    the third stays without it and the detached agg(KL) follows the entropy mean (if any).  An objective with
+    policy_loss_mode clip_cov / kl_cov (seeded by cov_seed, as actor_loss) runs the composed path, K1 -> selection ->
+    aa_ppo_actor_loss_cov -> K1b, and its fp32 (1,) selected share follows agg(KL).  return_clip_fraction: the fp32[2]
+    clip fractions (see actor_loss) follow as the last output."""
     objective = _objective(objective)
     L.require_cuda(logits, input_ids, old_log_probs, advantages, mask)
     lens = as_device_lens(lens, logits.device)
@@ -2769,13 +3002,15 @@ def tail_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, lens, old_log
     old, aux, m = _k5_operands(old_log_probs, advantages, mask, lp_dtype)
     kl = _kl_loss_term(ref_log_probs, old_log_probs, kl_loss_coeff, kl_loss_estimator, lp_dtype)
     plan = device_tail_plan(lens, K, logits.stride(0), logits.stride(1), ids.stride(0), ids.size(1), 0, -1, lens.bound)
-    single_pass = _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad)
+    cov = _cov_term(objective, cov_seed, logits.device)
+    single_pass = cov is None and _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad)
     if objective is not None:
         objective.args(clip_range_ratio)  # a bad clip range fails here, before the node launches anything
     cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
     out = _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass,
-                                 float(entropy_coeff), objective, cf, kl)
-    return (*out, *((kl.out[0],) if kl is not None else ()), *((cf,) if return_clip_fraction else ()))
+                                 float(entropy_coeff), objective, cf, kl, cov)
+    return (*out, *((kl.out[0],) if kl is not None else ()), *((cov.share,) if cov is not None else ()),
+            *((cf,) if return_clip_fraction else ()))
 
 
 @functools.lru_cache(maxsize=64)
@@ -2790,7 +3025,7 @@ def _dense_actor_plan(B: int, L: int, start: int, sb: int, sl: int, lab_sb: int,
 def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, old_log_probs, advantages, mask,
                      clip_range_ratio: float, mode: str | None = None, entropy_coeff: float = 0.0,
                      objective: ActorObjective | None = None, return_clip_fraction: bool = False, ref_log_probs=None,
-                     kl_loss_coeff: float = 0.0, kl_loss_estimator: str = 'k3'):
+                     kl_loss_coeff: float = 0.0, kl_loss_estimator: str = 'k3', cov_seed: int = 0):
     """The actor half of the text rl_step (trainers/text_to_text/ppo.py:336-349) as one autograd node:
     `gather_log_probabilities(logits[:, :-1], ids[:, 1:])[:, start:]` -> `actor_loss_fn` -> backward up to d logits.
     Only the rows `[start, L - 1)` are read (the reference scores every position and slices afterwards); with a
@@ -2802,7 +3037,10 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
     single pass is K1f's entropy-gradient variant, the composed path K1's entropy variant -> K5 + masked_mean -> K1b's
     entropy variant.  objective / return_clip_fraction / the KL loss term (ref_log_probs (B, L - 1 - start),
     kl_loss_coeff, kl_loss_estimator): as tail_actor_loss (agg(KL) after the entropy mean, the clip fractions last);
-    the composed path runs K5's KL entry point, whose gradient K1b carries to the tile."""
+    the composed path runs K5's KL entry point, whose gradient K1b carries to the tile.  An objective with
+    policy_loss_mode clip_cov / kl_cov always takes the composed path (K1 -> selection -> aa_ppo_actor_loss_cov ->
+    K1b; the selection needs every log-prob of the call first) and its selected share follows agg(KL), as
+    tail_actor_loss."""
     objective = _objective(objective)
     L.require_cuda(logits, input_ids, old_log_probs, advantages, mask)
     if logits.dim() != 3 or input_ids.shape != logits.shape[:2]:
@@ -2816,7 +3054,8 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
         raise ValueError('old_log_probs, advantages and mask must all be (B, L - 1 - start)')
     if objective is not None:
         objective.args(clip_range_ratio)  # a bad clip range fails here, before any launch
-    if not _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad):
+    cov_mode = objective is not None and objective.policy_loss_mode != 'vanilla'
+    if cov_mode or not _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad):
         # short rows, fp16, no gradient: the composed ops (K1 over the response rows -> K5, which takes the objective;
         # backward K1b)
         rows, labels = logits[:, start:-1], input_ids[:, start + 1:]
@@ -2825,9 +3064,11 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
             lp, ent = gather_log_probabilities_with_entropy(rows, labels, mode=mode, entropy_grad=True)
         else:
             lp = gather_log_probabilities(rows, labels, mode=mode)
-        loss, loss32, kl, cf = _actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, mode, objective,
-                                           return_clip_fraction, ref_log_probs, kl_loss_coeff, kl_loss_estimator)
-        tail = ((kl,) if kl is not None else ()) + ((cf,) if return_clip_fraction else ())
+        loss, loss32, kl, cf, share = _actor_loss(lp, old_log_probs, advantages, mask, clip_range_ratio, mode, objective,
+                                                  return_clip_fraction, ref_log_probs, kl_loss_coeff, kl_loss_estimator,
+                                                  cov_seed)
+        tail = ((kl,) if kl is not None else ()) + ((share,) if share is not None else ()) + \
+            ((cf,) if return_clip_fraction else ())
         if entropy_coeff == 0.0:
             return (loss, lp.detach(), loss32, *tail)
         m = mask.to(torch.bool)

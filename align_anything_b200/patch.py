@@ -23,7 +23,7 @@ swaps, without touching any reference file,
     `kl_loss_estimator`, unset: the reference's penalty and no KL term in the actor loss, and `whiten_advantages`, off;
     the GRPO class also the GRPO-objective switches `num_iterations`, `clip_range_ratio`,
     `clip_range_ratio_low`, `clip_range_ratio_high`, `dual_clip_ratio`, `loss_agg_mode`, `scale_rewards`,
-    `log_clip_fraction`, `kl_estimator`, `importance_sampling_level` and `top_entropy_quantile`, at the reference's single-update loss), RMTrainer.{loss, train_step} of the text /
+    `log_clip_fraction`, `kl_estimator`, `importance_sampling_level`, `top_entropy_quantile` and the Clip-Cov / KL-Cov keys, at the reference's single-update loss), RMTrainer.{loss, train_step} of the text /
     audio / video trainers (the audio and video trainers override `loss` with the text arithmetic, so their own `loss`
     is replaced too; the image trainers inherit both) and CMTrainer.{loss, train_step} of the text cost-model
     trainer (Safe RLHF's signed cost loss in one launch; the image cost-model trainer inherits both),

@@ -160,7 +160,7 @@ class PPOTrainer(_TextPPOTrainer):
         old_rewards, reward_advantages, reward_returns, row_stats = step_advantages(self, training_batch, sequence_mask, 0)
 
         # actor: K1 over the response tails + K5 as ONE autograd node; its backward is K1b alone (:296-316)
-        actor_loss, actor_loss32, entropy_mean, clip_frac, kl_loss = actor_loss_node(
+        actor_loss, actor_loss32, entropy_mean, clip_frac, kl_loss, cov_share = actor_loss_node(
             self, self.infer_batch(inference_batch), input_ids, old_log_probs, reward_advantages, sequence_mask,
             lens=lens, ref_log_probs=ref_log_probs)
         self.actor_model.backward(actor_loss)
@@ -177,4 +177,4 @@ class PPOTrainer(_TextPPOTrainer):
             self, row_stats, reward, value_row_mean, actor_loss32, critic_loss32,
             {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns},
             entropy=training_batch['entropy'] if self.log_entropy else None, mask=sequence_mask,
-            entropy_mean=entropy_mean, clip_frac=clip_frac, kl_loss=kl_loss)
+            entropy_mean=entropy_mean, clip_frac=clip_frac, kl_loss=kl_loss, cov_share=cov_share)

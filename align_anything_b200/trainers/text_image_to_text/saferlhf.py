@@ -42,6 +42,15 @@ def refuse_kl_switches(tr) -> None:
             raise ValueError(f'{name}={v!r}: Safe RLHF-V keeps the reference KL penalty (k1, a fixed kl_coeff)')
 
 
+def refuse_cov_switches(tr) -> None:
+    """Safe RLHF-V keeps the reference's clipped actor objective: the Clip-Cov / KL-Cov switches it inherits from the
+    PPO trainers raise here, before anything runs, when set (policy_loss_mode to anything but vanilla)."""
+    for name in ('policy_loss_mode', 'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef'):
+        v = switch_of(tr, name)
+        if v is not None and not (name == 'policy_loss_mode' and v == 'vanilla'):
+            raise ValueError(f'{name}={v!r}: Safe RLHF-V keeps the reference\'s clipped actor objective')
+
+
 def refuse_whitening(tr) -> None:
     """Safe RLHF-V mixes its reward and cost advantages with the Lagrange multiplier as the reference does, unwhitened:
     `whiten_advantages` set to True (or to anything but a bool) raises here, before anything runs."""
@@ -82,6 +91,7 @@ class SafeRLHFVTrainer(_MMPPOTrainer):
     # ---- saferlhf.py:453-481 ---------------------------------------------------------------------------
     def add_kl_divergence_regularization_with_cost(self, reward, cost, log_probs, ref_log_probs, sequence_mask):
         refuse_kl_switches(self)
+        refuse_cov_switches(self)
         zeros = torch.zeros_like(log_probs)
         rewards = ops.kl_rewards_and_gae(reward, log_probs, ref_log_probs, zeros, sequence_mask, 0, self.kl_coeff,
                                          self.clip_range_score, self.gamma, self.gae_lambda, mode=self.mode)[0]
@@ -120,6 +130,7 @@ class SafeRLHFVTrainer(_MMPPOTrainer):
     # ---- saferlhf.py:483-675 ---------------------------------------------------------------------------
     def rl_step(self, inference_batch, training_batch) -> dict[str, Any]:
         refuse_kl_switches(self)
+        refuse_cov_switches(self)
         refuse_whitening(self)
         self._lambda_step()
         lens = ops.as_device_lens(training_batch['response_lens'], training_batch['log_probs'].device)

@@ -11,12 +11,13 @@ import torch
 
 from ... import ops
 from ...utils.multi_process import all_reduce_packed
-from .ppo import entropy_coeff_of, hidden_log_probs, lm_head_of, switch_of
+from .ppo import cov_seed_of, entropy_coeff_of, hidden_log_probs, lm_head_of, switch_of
 
 __all__ = ['GRPOTrainer']
 
 GRPO_OBJECTIVE_KEYS = ('clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio',
-                       'loss_agg_mode', 'kl_estimator', 'importance_sampling_level', 'top_entropy_quantile')
+                       'loss_agg_mode', 'kl_estimator', 'importance_sampling_level', 'top_entropy_quantile',
+                       'policy_loss_mode', 'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef')
 
 
 def num_iterations_of(tr) -> int:
@@ -85,6 +86,17 @@ class GRPOTrainer:
     # today's launches; rho < 1 takes the composed path with the exact entropy quantile (ops.entropy_quantile_threshold)
     # on both the tile and the fused_lm_head paths.  `cfgs.train_cfgs.top_entropy_quantile` overrides it.
     top_entropy_quantile = 1.0
+    # Clip-Cov / KL-Cov (Cui et al. 2025; verl's policy_loss.loss_mode, see ops.ActorObjective / ops.GrpoObjective):
+    # policy_loss_mode 'clip_cov' or 'kl_cov' (None = 'vanilla') and their keys (None = verl's defaults), token level
+    # only.  Each update selects over its own completion tokens on the device, on the composed path (tile and
+    # fused_lm_head); train/actor_cov_fraction reports the selected share, the mean over the updates.  On the first
+    # update (ratio 1) KL-Cov changes nothing.  `cfgs.train_cfgs.<key>` overrides each when set.
+    policy_loss_mode = None
+    clip_cov_ratio = None
+    clip_cov_lb = None
+    clip_cov_ub = None
+    kl_cov_ratio = None
+    ppo_kl_coef = None
     # Opt-in: train/actor_clip_fraction (and train/actor_dual_clip_fraction with dual-clip), the mean over the updates,
     # in the step's one packed all-reduce
     log_clip_fraction = False
@@ -92,7 +104,8 @@ class GRPOTrainer:
     SWITCHES = ('mode', 'fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'num_iterations',
                 'clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode',
                 'scale_rewards', 'log_clip_fraction', 'kl_estimator', 'importance_sampling_level',
-                'top_entropy_quantile')
+                'top_entropy_quantile', 'policy_loss_mode', 'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub',
+                'kl_cov_ratio', 'ppo_kl_coef')
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, tokenizer=None, *, beta=None,
                  num_generations=None) -> None:
@@ -141,11 +154,14 @@ class GRPOTrainer:
         if log_cf:
             kw['return_clip_fraction'] = True
         old = None  # updates 2..mu: the first update's log-probs
-        plains, entropies, entropy_means, fracs = [], [], [], []
+        plains, entropies, entropy_means, fracs, shares = [], [], [], [], []
+        cov = objective is not None and objective.policy_loss_mode != 'vanilla'
         for _ in range(mu):
             if old is not None:
                 kw['old_per_token_logps'] = old
-            loss, plain, entropy, entropy_mean, cf, lp, row_end = policy_update(
+            if cov:
+                kw['cov_seed'] = cov_seed_of(self, objective)
+            loss, plain, entropy, entropy_mean, cf, lp, row_end, share = policy_update(
                 self, sequences, attention_mask, logits_to_keep, ref_per_token_logps, advantages, kw)
             if old is None and mu > 1:
                 old = lp
@@ -153,6 +169,7 @@ class GRPOTrainer:
             entropies.append(entropy)
             entropy_means.append(entropy_mean)
             fracs.append(cf)
+            shares.append(share)
         with torch.no_grad():
             # train/loss is GRPO's loss without the bonus, the mean over the updates; lane 2 = device status word, MAX
             packed = [torch.stack([_mean(plains), rewards.float().mean()]), ops.status_lane(loss.device)]
@@ -167,6 +184,8 @@ class GRPOTrainer:
                 lanes['train/actor_clip_fraction'] = cf[:1]
                 if objective is not None and objective.dual_clip_ratio is not None:
                     lanes['train/actor_dual_clip_fraction'] = cf[1:2]
+            if cov:  # the share of completion tokens Clip-Cov / KL-Cov selected
+                lanes['train/actor_cov_fraction'] = _mean(shares)
             # ONE collective, ONE sync per rollout (reference: 2 + 2 per update)
             v = all_reduce_packed(torch.cat([*packed, *lanes.values()]), max_lanes=(2,)).tolist()
         ops.raise_for_status(v[2], loss.device)
@@ -191,9 +210,9 @@ def _mean(xs):
 def policy_update(tr, sequences, attention_mask, logits_to_keep, ref_per_token_logps, advantages, kw):
     """One policy pass, backward and optimizer step of the trainer `tr` on the rollout -> (loss, GRPO's loss without
     the bonus (fp32, detached), entropy or None, entropy term or None, clip fractions or None, detached log-probs,
-    row_end).  A function rather than a method, so that the grafted step_from_rollout of the reference's class finds
+    row_end, the Clip-Cov / KL-Cov selected share or None).  A function rather than a method, so that the grafted step_from_rollout of the reference's class finds
     it without being grafted itself."""
-    entropy = cf = None
+    entropy = cf = share = None
     coeff = entropy_coeff_of(tr)
     entropy_mean = plain = None  # with the bonus: its entropy term and GRPO's loss without it
     if tr.fused_lm_head:  # the composed path: K1f needs a logits tile
@@ -208,7 +227,9 @@ def policy_update(tr, sequences, attention_mask, logits_to_keep, ref_per_token_l
                                mode=tr.mode, **kw, **({'entropy': entropy} if topent else {}))
         loss, row_end = scored[0], scored[1]
         if kw.get('return_clip_fraction'):
-            cf = scored[2]
+            cf = scored[-1]
+        if 'cov_seed' in kw:
+            share = scored[2]
         lp = per_token_logps.detach()
         if coeff != 0.0:  # K6b adds the entropy's gradient in its epilogue
             entropy_mean = ops._completion_mean(entropy, row_end)
@@ -224,6 +245,8 @@ def policy_update(tr, sequences, attention_mask, logits_to_keep, ref_per_token_l
                                            **({'entropy_coeff': coeff} if coeff != 0.0 else {}), **kw)
         if kw.get('return_clip_fraction'):
             scored, cf = scored[:-1], scored[-1]
+        if 'cov_seed' in kw:
+            scored, share = scored[:-1], scored[-1]
         loss, lp, row_end = scored[0], scored[1], scored[2]
         if coeff != 0.0:
             entropy_mean, plain = scored[3], scored[4]
@@ -233,4 +256,4 @@ def policy_update(tr, sequences, attention_mask, logits_to_keep, ref_per_token_l
     tr.actor_model.backward(loss)
     tr.actor_model.step()
     plain = (loss if plain is None else plain).detach().float()
-    return loss, plain, entropy, entropy_mean, cf, lp, row_end
+    return loss, plain, entropy, entropy_mean, cf, lp, row_end, share

@@ -163,7 +163,8 @@ def whiten_rollout(tr, training_batches, sequence_masks, starts, returns=None) -
         training['advantages'] = adv
 
 
-OBJECTIVE_KEYS = ('clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode')
+OBJECTIVE_KEYS = ('clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode',
+                  'policy_loss_mode', 'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef')
 
 
 def actor_objective_of(tr) -> ops.ActorObjective | None:
@@ -174,12 +175,28 @@ def actor_objective_of(tr) -> ops.ActorObjective | None:
     return ops.ActorObjective(**fields) if fields else None
 
 
+def cov_seed_of(tr, objective) -> int:
+    """The hash seed of this loss call under Clip-Cov (ops.cov_hash_seed of `train_cfgs.seed` (0 when absent), the
+    data-parallel rank and tr's count of earlier Clip-Cov calls, which this advances); 0 for any other objective."""
+    if objective is None or objective.policy_loss_mode != 'clip_cov':
+        return 0
+    tc = getattr(getattr(tr, 'cfgs', None), 'train_cfgs', None)
+    seed = getattr(tc, 'seed', None)
+    dist = torch.distributed
+    rank = dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
+    n = getattr(tr, 'cov_calls', 0)
+    tr.cov_calls = n + 1
+    return ops.cov_hash_seed(int(seed or 0), rank, n)
+
+
 def objective_kwargs(tr) -> dict:
     """The ops keywords of the actor objective switches: empty when they are all at their defaults (today's call)."""
     kw = {}
     objective = actor_objective_of(tr)
     if objective is not None:
         kw['objective'] = objective
+        if objective.policy_loss_mode != 'vanilla':
+            kw['cov_seed'] = cov_seed_of(tr, objective)
     if tr.log_clip_fraction:
         kw['return_clip_fraction'] = True
     return kw
@@ -188,7 +205,8 @@ def objective_kwargs(tr) -> dict:
 def actor_loss_node(tr, batch, input_ids, old_log_probs, advantages, mask, *, start=0, head=None, lens=None,
                     ref_log_probs=None):
     """The actor loss of an rl_step -> (loss, the loss for ppo_pack_metrics, the masked-mean entropy or None, the
-    fp32[2] clip fractions or None, agg(KL) of the KL loss term or None).  The rows scored are those of the text
+    fp32[2] clip fractions or None, agg(KL) of the KL loss term or None, the Clip-Cov / KL-Cov selected share or
+    None).  The rows scored are those of the text
     layout, `[start:]` of every row, or with `lens` the response tails of the multimodal layout (`old_log_probs`,
     `ref_log_probs`, `advantages` and `mask` already (B, W)).
     `head`: the lm_head weight of the text layout's fused path.  With an entropy bonus (entropy_coeff_of(tr) != 0) the loss is
@@ -200,7 +218,7 @@ def actor_loss_node(tr, batch, input_ids, old_log_probs, advantages, mask, *, st
     being grafted itself."""
     coeff = entropy_coeff_of(tr)
     kw = objective_kwargs(tr)
-    cf = kl = None
+    cf = kl = share = None
     if lens is None:
         old_log_probs, mask = old_log_probs[:, start:], mask[:, start:]
     term = kl_loss_of(tr)
@@ -218,15 +236,15 @@ def actor_loss_node(tr, batch, input_ids, old_log_probs, advantages, mask, *, st
         if coeff != 0.0:
             log_probs, ent = log_probs
         # ops.actor_loss, with the actor loss without the KL term beside the loss
-        loss, loss32, kl, cf = ops._actor_loss(
+        loss, loss32, kl, cf, share = ops._actor_loss(
             log_probs, old_log_probs, advantages, mask, tr.clip_range_ratio, tr.mode, kw.get('objective'),
             kw.get('return_clip_fraction', False), kw.get('ref_log_probs'), kw.get('kl_loss_coeff', 0.0),
-            kw.get('kl_loss_estimator', 'k3'))
+            kw.get('kl_loss_estimator', 'k3'), kw.get('cov_seed', 0))
         if coeff == 0.0:
-            return loss, loss32, None, cf, kl
+            return loss, loss32, None, cf, kl, share
         token = 'objective' in kw and kw['objective'].token_mean
         h_mean = (ops.token_mean if token else ops.masked_mean)(ent, mask)
-        return loss - coeff * h_mean, loss32, h_mean.detach(), cf, kl
+        return loss - coeff * h_mean, loss32, h_mean.detach(), cf, kl, share
     # One autograd node (K1f): log-probs, d loss / d log-prob and the gradient tile in a single pass over the scored
     # rows.  The text layout reads only the rows `[start:]` the reference keeps after scoring every position
     # (:338-346); the prompt rows of the tile are written as zeros by the same kernel.
@@ -242,13 +260,15 @@ def actor_loss_node(tr, batch, input_ids, old_log_probs, advantages, mask, *, st
                                   mode=tr.mode, **kw)
     if kw.get('return_clip_fraction'):
         out, cf = out[:-1], out[-1]
+    if 'cov_seed' in kw:
+        out, share = out[:-1], out[-1]
     if term is not None:
         out, kl = out[:-1], out[-1]
-    return out[0], out[2], (out[3] if coeff != 0.0 else None), cf, kl
+    return out[0], out[2], (out[3] if coeff != 0.0 else None), cf, kl, share
 
 
 def ppo_metrics(tr, row_stats, reward, value_row_mean, actor_loss, critic_loss, tensors, *, entropy=None, mask=None,
-                entropy_mean=None, clip_frac=None, kl_loss=None) -> dict[str, Any]:
+                entropy_mean=None, clip_frac=None, kl_loss=None, cov_share=None) -> dict[str, Any]:
     """The metric dict of a PPO rl_step from ONE packed collective and ONE host sync (reference: 10 all-reduces, a
     barrier and 12 .item()).  ppo_pack_metrics packs the ten metrics of METRIC_KEYS, the device status word (lane 10,
     MAX-reduced with lane 9) and a spare lane 11 (0).  Optional AVG lanes follow, each read back under its key:
@@ -257,7 +277,8 @@ def ppo_metrics(tr, row_stats, reward, value_row_mean, actor_loss, critic_loss, 
       * `entropy_mean`, the entropy term of the bonus (train/actor_entropy);
       * `clip_frac`, K5's clip fraction (train/actor_clip_fraction) and with dual-clip its dual-clip fraction
         (train/actor_dual_clip_fraction);
-      * `kl_loss`, agg(KL) of the KL loss term without its coefficient (train/actor_kl_loss).
+      * `kl_loss`, agg(KL) of the KL loss term without its coefficient (train/actor_kl_loss);
+      * `cov_share`, the share of counted tokens Clip-Cov / KL-Cov selected (train/actor_cov_fraction).
     Sets `tr.last_rl_tensors = tensors` (per-token tensors stay out of the dict: the reference hands it to Logger.log,
     which takes scalars only).  With `kl_target` set (kl_controller_of) the step's train/kl_coeff goes into the dict and
     tr.kl_coeff takes the adaptive controller's update from the step's (all-reduced) train/kl_divergence and its
@@ -265,7 +286,8 @@ def ppo_metrics(tr, row_stats, reward, value_row_mean, actor_loss, critic_loss, 
     with torch.no_grad():
         # an optional lane is filled in before the one packed all-reduce, so the NVLink reduction fused into
         # ppo_pack_metrics (which reduces the vector as it writes it) gives way to all_reduce_packed
-        extra = entropy is not None or entropy_mean is not None or clip_frac is not None or kl_loss is not None
+        extra = entropy is not None or entropy_mean is not None or clip_frac is not None or kl_loss is not None or \
+            cov_share is not None
         fused = fused_allreduce(row_stats.device) if not extra else None
         stats = ops.ppo_pack_metrics(row_stats, reward, value_row_mean, actor_loss, critic_loss,
                                      coll=fused.next((9, 10)) if fused is not None else None)
@@ -281,6 +303,8 @@ def ppo_metrics(tr, row_stats, reward, value_row_mean, actor_loss, critic_loss, 
                 lanes['train/actor_dual_clip_fraction'] = clip_frac[1:2]
         if kl_loss is not None:
             lanes['train/actor_kl_loss'] = kl_loss.detach().float().reshape(1)
+        if cov_share is not None:
+            lanes['train/actor_cov_fraction'] = cov_share.reshape(1)
         first = 11 if entropy is not None else 12  # the entropy takes the spare lane 11
         if lanes:
             stats = torch.cat([stats[:first], *lanes.values()])
@@ -344,6 +368,16 @@ class PPOTrainer:
     # train/actor_loss stays the clipped objective, train/actor_kl_loss reports agg(KL).
     kl_loss_coeff = 0.0
     kl_loss_estimator = None
+    # Clip-Cov / KL-Cov (Cui et al. 2025; verl's policy_loss.loss_mode, see ops.ActorObjective): policy_loss_mode
+    # 'clip_cov' or 'kl_cov' (None = 'vanilla'), and their keys clip_cov_ratio, clip_cov_lb, clip_cov_ub, kl_cov_ratio
+    # and ppo_kl_coef (None = verl's defaults).  The selection runs on the device, local to each micro-batch's loss;
+    # train/actor_cov_fraction reports the selected share.  `cfgs.train_cfgs.<key>` overrides each when set.
+    policy_loss_mode = None
+    clip_cov_ratio = None
+    clip_cov_lb = None
+    clip_cov_ub = None
+    kl_cov_ratio = None
+    ppo_kl_coef = None
     # Advantage whitening (TRL's / verl's masked_whiten): rollout() forms every micro-batch's advantages with the
     # kl_coeff in effect then (K4, and K4r for Multi-PPO's other estimators) and whitens them with ONE mean and std over
     # the whole rollout's actor-loss mask, on every data-parallel rank (ops.whiten_advantages); rl_step reuses them (all
@@ -353,7 +387,8 @@ class PPOTrainer:
     # the class attributes above that the grafted methods read: patch.install() copies them onto the reference's classes
     SWITCHES = ('mode', 'fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'clip_range_ratio_low',
                 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode', 'log_clip_fraction', 'kl_estimator',
-                'kl_target', 'kl_horizon', 'kl_loss_coeff', 'kl_loss_estimator', 'whiten_advantages')
+                'kl_target', 'kl_horizon', 'kl_loss_coeff', 'kl_loss_estimator', 'whiten_advantages', 'policy_loss_mode',
+                'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef')
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, reward_model=None,
                  reward_critic_model=None, tokenizer=None, reward_tokenizer=None, *, kl_coeff=0.02,
@@ -526,7 +561,7 @@ class PPOTrainer:
         old_rewards, reward_advantages, reward_returns, row_stats = step_advantages(
             self, training_batch, sequence_mask, start, returns)
 
-        actor_loss, actor_loss32, entropy_mean, clip_frac, kl_loss = actor_loss_node(
+        actor_loss, actor_loss32, entropy_mean, clip_frac, kl_loss, cov_share = actor_loss_node(
             self, inference_batch, input_ids, old_log_probs, reward_advantages, sequence_mask, start=start, head=head,
             ref_log_probs=ref_log_probs)
         self.actor_model.backward(actor_loss)
@@ -544,4 +579,4 @@ class PPOTrainer:
             self, row_stats, reward, value_row_mean, actor_loss32, reward_critic_loss,
             {'old_rewards': old_rewards, 'advantages': reward_advantages, 'returns': reward_returns},
             entropy=training_batch['entropy'][:, start:] if self.log_entropy else None, mask=sequence_mask[:, start:],
-            entropy_mean=entropy_mean, clip_frac=clip_frac, kl_loss=kl_loss)
+            entropy_mean=entropy_mean, clip_frac=clip_frac, kl_loss=kl_loss, cov_share=cov_share)

@@ -8,7 +8,7 @@
  * function(s) whose arithmetic it replaces (file:line relative to the reference's
  * align_anything/ directory); the Python mirror in align_anything_b200/ keeps the
  * reference's names and signatures and calls these through ctypes (INTEGRATION.md).
- * 70 entry points, ABI version 3.
+ * 78 entry points, ABI version 3.
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
@@ -755,6 +755,68 @@ int aa_entropy_select_hi(const uint32_t *hist, float q, uint32_t *sel, void *str
 int aa_entropy_hist_lo(const float *entropy, int64_t ent_stride, const int32_t *row_end, const uint8_t *mask,
                        int64_t mask_stride, int32_t B, int32_t K, const uint32_t *sel, uint32_t *hist, void *stream);
 int aa_entropy_select_lo(const uint32_t *hist, const uint32_t *sel, float *thr, void *stream);
+
+/* Clip-Cov and KL-Cov (Cui et al. 2025; verl's policy_loss.loss_mode 'clip_cov' / 'kl_cov'): the tokens whose
+ * covariance cov_t = (A_t - mean A) * (lp_t - mean lp) over the counted tokens is largest lose their policy term
+ * (Clip-Cov, a random share of the eligible ones) or take a |lp - old| penalty (KL-Cov, the top share).  The
+ * selection runs on the device with no host sync, local to one loss call:
+ *   aa_cov_moments   : one block; fixed-order fp64 (N, sum A, sum lp) over the counted tokens, each mean rounded once
+ *                      to fp32 -> state.  Counted: mask[b * mask_stride + t] != 0 with advantages (B, W) of adv_dtype
+ *                      and row stride adv_stride (PPO), or t < row_end[b] with fp32 per-row advantages adv[b] (GRPO);
+ *                      give exactly one of mask and row_end.  log_probs (B, W) of lp_dtype.  B * W < 2^31.
+ *   aa_cov_keys      : a uint32 key and a uint8 eligibility bit per flat index i = b * W + t (keys / elig, B * W
+ *                      each), and hist (uint32[65536], zeroed here) = the counts of the eligible keys' high halves.
+ *                      AA_COV_KL: every counted token is eligible, key = the order of fp32 cov_t (-0 = +0, NaN above
+ *                      +inf).  AA_COV_CLIP: eligible = counted, not clipped (aa_ppo_actor_loss_obj's clip-fraction
+ *                      predicate at [1 - clip_low, 1 + clip_high], old_log_probs NULL: ratio 1) and lb < cov_t < ub;
+ *                      key = fmix32(i ^ hash_seed) (MurmurHash3's finaliser: a bijection, no ties).  mode: AA_MODE_*,
+ *                      the loss kernel's rounding of the ratio.
+ *   aa_cov_select_hi : one block; k = min(E, max(1, (int64)(ratio * (double)N))) of the E eligible tokens (0 when
+ *                      E == 0), and the high-half bucket of the k-th largest key.  ratio = *ratio_host, a double
+ *                      in (0, 1] (the product rounds as Python's int(ratio * N) does).
+ *   aa_cov_hist_lo   : hist (uint32[65536], zeroed here) = the low halves of the eligible keys in that bucket.
+ *   aa_cov_select_lo : one block; the threshold key T, the number of keys == T to take, and share[0] = k / N (fp32,
+ *                      0 when N == 0).
+ *   aa_cov_mark      : sel[b * sel_stride + t] = 1 for the k eligible tokens with the largest keys, ties at T going to
+ *                      the smaller flat index; 0 elsewhere.  tie_rows: int32 [B] scratch.
+ * state: uint32[16], written and read by these calls only.  Arguments are checked before any CUDA call. */
+enum { AA_COV_CLIP = 1, AA_COV_KL = 2 };
+int aa_cov_moments(const void *log_probs, int64_t lp_stride, int lp_dtype, const void *advantages, int64_t adv_stride,
+                   int adv_dtype, const uint8_t *mask, int64_t mask_stride, const int32_t *row_end, int32_t B,
+                   int32_t W, uint32_t *state, void *stream);
+int aa_cov_keys(int cov_mode, const void *log_probs, int64_t lp_stride, const void *old_log_probs, int64_t old_stride,
+                int lp_dtype, const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
+                int64_t mask_stride, const int32_t *row_end, int32_t B, int32_t W, float clip_low, float clip_high,
+                float lb, float ub, uint32_t hash_seed, int mode, const uint32_t *state, uint32_t *keys,
+                uint8_t *elig, uint32_t *hist, void *stream);
+int aa_cov_select_hi(const uint32_t *hist, const double *ratio_host, uint32_t *state, void *stream);
+int aa_cov_hist_lo(const uint32_t *keys, const uint8_t *elig, int64_t n, const uint32_t *state, uint32_t *hist,
+                   void *stream);
+int aa_cov_select_lo(const uint32_t *hist, uint32_t *state, float *share, void *stream);
+int aa_cov_mark(const uint32_t *keys, const uint8_t *elig, int32_t B, int32_t W, const uint32_t *state,
+                int32_t *tie_rows, uint8_t *sel, int64_t sel_stride, void *stream);
+
+/* aa_ppo_actor_loss_kl's objective under Clip-Cov or KL-Cov (cov_mode AA_COV_*), sel (uint8 (B, Wm), row stride
+ * sel_stride) the selection of aa_cov_mark: Clip-Cov is the clip-higher objective with a selected token's term and
+ * gradient 0; KL-Cov is the unclipped s = adv * ratio with s - cov_coef * |lp - old| on a selected token (cov_coef
+ * finite, >= 0).  There is no dual-clip.  ref_log_probs NULL: no KL loss term (kl_loss may then be NULL).  The clip
+ * fractions count the clipped branch as aa_ppo_actor_loss_obj does (0 under KL-Cov).  row_scratch: fp32 [5 * B]. */
+int aa_ppo_actor_loss_cov(const void *log_probs, int64_t lp_stride, const void *old_log_probs, int64_t old_stride,
+                          int lp_dtype, const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
+                          int64_t mask_stride, int32_t B, int32_t Wm, float clip_low, float clip_high, int loss_agg,
+                          int cov_mode, float cov_coef, const uint8_t *sel, int64_t sel_stride, int mode,
+                          const void *ref_log_probs, int64_t ref_stride, float kl_loss_coeff, int kl_estimator,
+                          float *loss, float *kl_loss, void *grad, int64_t grad_stride, float *clip_frac,
+                          float *row_scratch, uint32_t *counter, void *stream);
+/* aa_grpo_loss_kl's token-level objective under Clip-Cov or KL-Cov, as aa_ppo_actor_loss_cov defines them, with the
+ * per-token loss -(s - beta * KL); old_log_probs NULL: ratio 1 (KL-Cov then changes nothing).  dual_clip must be 0. */
+int aa_grpo_loss_cov(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
+                     const void *old_log_probs, int64_t old_stride, int lp_dtype, const float *advantages,
+                     const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B, int32_t K,
+                     float beta, float clip_low, float clip_high, int loss_agg, int kl_estimator, int cov_mode,
+                     float cov_coef, const uint8_t *sel, int64_t sel_stride, int mode, float *loss, void *grad,
+                     int64_t grad_stride, float *clip_frac, int32_t *row_end, float *scratch, uint32_t *counter,
+                     void *stream);
 
 /* masked_mean (utils/tools.py:460-467): mean over rows of masked row means -> out[0];
  * mask == NULL: plain mean. */
