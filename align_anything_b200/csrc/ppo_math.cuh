@@ -124,8 +124,10 @@ __device__ __forceinline__ void cov_token(int mode, float x, float old, float au
   if (sel) obj = round_to(obj - round_to(kl_coef * fabsf(d), rx), rp);
   if (!on) return;
   grad = round_to(round_to(round_to(g_rs * aux, rp), rx) * ratio, rx);  // through the ratio (ExpBackward)
-  if (sel && d != 0.f) {  // through -kl_coef * |d|: MulBackward by the scalar, then AbsBackward's sign
-    const float ga = round_to(-g_rs * kl_coef, rx);
+  if (sel && d != 0.f) {  // through -kl_coef * |d|: MulBackward by the scalar, then AbsBackward's sign.  kl_coef * |d|
+    // has the log-probs' dtype, so the gradient reaching it is rounded to rx first (a no-op unless rp is wider, as
+    // with GRPO's or PPO's fp32 advantages under 16-bit log-probs)
+    const float ga = round_to(round_to(-g_rs, rx) * kl_coef, rx);
     grad = round_to(grad + (d > 0.f ? ga : -ga), rx);
   }
 }

@@ -102,9 +102,58 @@ def ppo_loss(mode, lp, old, adv, mask, sel, agg='seq-mean-token-mean', lo=0.2, h
     return aggregate(pg_losses(mode, lp, old, adv, sel, lo, hi, coef), mask, agg)
 
 
-def grpo_loss(mode, lp, ref, old, adv, mask, sel, beta, agg='token-mean', lo=0.2, hi=0.2, coef=1.0):
-    """GRPO under Clip-Cov / KL-Cov: per-token loss pg + beta * k3 KL, `old` None: the ratio is 1."""
+def grpo_loss(mode, lp, ref, old, adv, mask, sel, beta, agg='token-mean', lo=0.2, hi=0.2, coef=1.0, estimator=None):
+    """GRPO under Clip-Cov / KL-Cov: per-token loss pg + beta * k3 KL, `old` None: the ratio is 1.  estimator 'k1' /
+    'k2' / 'k3': the KL of kl_objective_port.kl_estimate instead (op for op the kernel's, created before the ratio)."""
     old = lp.detach() if old is None else old
-    d = ref - lp
-    kl = torch.exp(d) - d - 1
+    if estimator is None:
+        d = ref - lp
+        kl = torch.exp(d) - d - 1
+    else:
+        from kl_objective_port import kl_estimate
+        kl = kl_estimate(lp, ref, estimator)
     return aggregate(pg_losses(mode, lp, old, adv.view(-1, 1), sel, lo, hi, coef) + beta * kl, mask, agg)
+
+
+def ppo_loss_kl(mode, lp, old, adv, mask, sel, agg, lo, hi, coef, ref, kl_coeff: float, estimator: str):
+    """-> (the Cov objective's loss, agg(KL), the total loss + kl_coeff * agg(KL)).  The KL is created before the
+    ratio, so autograd adds its gradient to lp after the objective's (kl_loss_port's order, K5's kl_grad)."""
+    from kl_loss_port import kl_loss
+
+    kl = kl_loss(lp, ref, mask, estimator, agg)
+    loss = ppo_loss(mode, lp, old, adv, mask, sel, agg, lo, hi, coef)
+    return loss, kl, loss + kl_coeff * kl
+
+
+def stable_clip(lp, old, adv, lo: float, hi: float, ulps: int = 4):
+    """True where `clipped` cannot change when exp moves by up to `ulps` fp32 ulps.  The kernel's expf and ATen's exp
+    may differ by one fp32 ulp; where that ulp lands the dtype-rounded ratio on the other side of a clip bound the
+    kernel and the port disagree by design.  The band is narrow (fp32 ulps of exp, not dtype ulps of the ratio): the
+    ratios one dtype ulp from a bound stay, and with them the tokens on which the ratio's rounding dtype decides."""
+    d = (lp - old).double()
+    r = torch.exp(d)
+    a = adv.to(torch.promote_types(lp.dtype, adv.dtype))
+    out = []
+    for f in (1.0 - ulps * 2.0 ** -24, 1.0 + ulps * 2.0 ** -24):
+        rr = (r * f).float().to(lp.dtype)
+        out.append(a * torch.clamp(rr, 1 - lo, 1 + hi) < a * rr)
+    return out[0] == out[1]
+
+
+def clear_clip_band(lp, old, adv, lo: float, hi: float, ulps: int = 4):
+    """`old` with old = lp (ratio exactly 1, never clipped) on every token stable_clip rejects."""
+    return torch.where(stable_clip(lp, old, adv, lo, hi, ulps), old, lp)
+
+
+def state_words(keys, eligible, ratio: float, n: int):
+    """The selection's state words of the reference: (E, k, T, need), as aa_cov_select_hi / _lo leave them.  keys: the
+    int64 uint32 keys, eligible: bool, both over every token; k = min(max(int(ratio * N), 1), E), 0 when E = 0 (then
+    T = 0xffffffff and need = 0); T is the k-th largest eligible key and need how many keys equal to T are taken."""
+    ek = keys.reshape(-1)[eligible.reshape(-1).bool()]
+    E = int(ek.numel())
+    k = min(n_select(ratio, n), E)
+    if k == 0:
+        return E, 0, U32, 0
+    top = torch.sort(ek, descending=True).values[:k]
+    T = int(top[-1])
+    return E, k, T, int((top == T).sum())
