@@ -160,6 +160,20 @@ _SIGS = {
     'aa_grpo_loss_cov': (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int, _P, _P, c_int64, c_int64, c_int32,
                                  c_int32, c_float, c_float, c_float, c_int, c_int, c_int, c_float, _P, c_int64, c_int,
                                  _P, _P, c_int64, _P, _P, _P, _P, _P]),
+    'aa_ppo_actor_loss_pm': (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int, _P, c_int64, c_int32,
+                                     c_int32, c_float, c_int, c_int, c_float, c_float, c_int, _P, c_int64, c_float,
+                                     c_int, _P, _P, _P, c_int64, _P, _P, _P, _P]),
+    'aa_grpo_loss_pm': (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int, _P, _P, c_int64, c_int64, c_int32,
+                                c_int32, c_float, c_float, c_int, c_int, c_int, c_float, c_float, c_int, _P, _P,
+                                c_int64, _P, _P, _P, _P, _P]),
+    'aa_logprob_actor_fused_pm': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P,
+                                          c_int, _P, _P, _P, c_int64, _P, c_int64, c_int, _P, c_int64, c_int32, c_float,
+                                          c_int, c_int, c_float, c_float, c_int, _P, c_int64, _P, _P, c_float, _P, _P,
+                                          c_float, c_int, _P]),
+    'aa_logprob_grpo_fused_pm': (c_int, [_P, c_int, c_int64, c_int32, _P, c_int32, _P, _P, _P, _P, _P, c_int64, _P,
+                                         c_int, _P, c_int64, _P, _P, _P, c_int64, c_int64, c_int32, c_float, c_float,
+                                         c_int, c_int, c_int, c_float, c_float, c_int, _P, c_int64, _P, _P, _P, _P, _P,
+                                         _P, c_float, _P]),
     'aa_nll_mean': (c_int, [_P, c_int, _P, c_int64, c_int64, _P, _P, _P, _P, _P]),
     'aa_masked_mean': (c_int, [_P, c_int, c_int64, _P, c_int64, c_int32, c_int32, _P, _P, _P, _P]),
     'aa_ppo_pack_metrics': (c_int, [_P, _P, _P, _P, _P, c_int32, _P, POINTER(AaColl), _P, _P]),

@@ -36,18 +36,25 @@ struct FusedActorParams {
   const void *logits;
   int64_t row_stride;
   int V;
+  // PM kernels (aa_logprob_actor_fused_pm, aa_logprob_grpo_fused_pm): kinds 0 and 3 take CISPO or SAPO (pm, AA_PM_*)
+  // with SAPO's temperatures tau_pos / tau_neg in place of the clipped ratio (ppo_math.cuh, pm_token / grpo_pm_token),
+  // and rp is s's dtype.  The three fields sit in the struct's alignment holes, so that the parameter block keeps its
+  // size and layout and the other kernels their code.
+  int pm;
   const int64_t *labels;
   RowMap map;
   const int64_t *seg_tile_row;
   int seq;  // tile rows per segment (n_tile_rows / n_seg)
   void *out;
   int out_dtype;
+  float tau_pos;  // PM
   float *stat_max, *stat_logsum;  // optional
   const void *old;
   int64_t old_stride;
   const void *adv;
   int64_t adv_stride;
   int adv_dtype;
+  float tau_neg;  // PM
   const uint8_t *mask;
   int64_t mask_stride;
   int W;
@@ -106,6 +113,7 @@ struct __align__(16) FusedRec {
   int32_t on;       // mask bit
 };
 static_assert(sizeof(FusedRec) == 48, "FusedRec is read as three 16-byte vectors");
+static_assert(sizeof(FusedActorParams) == 344, "the PM fields fill alignment holes: the parameter block keeps its size");
 
 // grid (ceil(seq / 256), n_seg): block (c, seg) resolves tile rows [256 c, 256 c + 256) of sample `seg`.
 template <bool EGRAD = false>
@@ -226,7 +234,10 @@ __device__ __forceinline__ uint4 vec_grad_pk(const uint4 &v, const GradConsts &k
 }
 
 // EGRAD (implies ENT): phase B adds the entropy's gradient (logprob_math.cuh, vec_grad_ent) to rows with g_H != 0.
-template <typename T, int CONSUMERS, int STAGES, int UNROLL, int LAG, bool FAITHFUL, bool ENT = false, bool EGRAD = false>
+// PM: kinds 0 and 3 run the policy loss p.pm (CISPO / SAPO) at the boundary; a flag of its own, so that the other
+// instantiations keep their code.
+template <typename T, int CONSUMERS, int STAGES, int UNROLL, int LAG, bool FAITHFUL, bool ENT = false, bool EGRAD = false,
+          bool PM = false>
 __global__ void __launch_bounds__(CONSUMERS + 32)
     logprob_actor_fused_kernel(const FusedActorParams p, const FusedRec *__restrict__ rec, int64_t n_work) {
   constexpr int E = Traits<T>::kVec;
@@ -459,7 +470,10 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
         int why;
         if (p.kind == 0) {
           const float lpr = round_to(lp, p.out_dtype);
-          actor_token(lpr, old, adv, on, g_rs, p.clip, p.clip_hi, p.dual, p.rx, p.rp, p.ra, obj, g, why);
+          if constexpr (PM)
+            pm_token(p.pm, lpr, old, adv, on, g_rs, p.clip_hi, p.tau_pos, p.tau_neg, p.rx, p.rp, obj, g, why);
+          else
+            actor_token(lpr, old, adv, on, g_rs, p.clip, p.clip_hi, p.dual, p.rx, p.rp, p.ra, obj, g, why);
           if (p.kl_coeff != 0.f && on) {  // the KL term: its gradient is added after the ratio's (as in K5)
             float kaux;
             kl_value(lpr, load_as_float(p.ref, out_idx, p.out_dtype), p.kl_est, p.rx, kaux);
@@ -470,8 +484,12 @@ __global__ void __launch_bounds__(CONSUMERS + 32)
         if (p.kind == 3) {
           const float lpr = round_to(lp, p.out_dtype);
           const float po = p.old_pol ? load_as_float(p.old_pol, out_idx, p.out_dtype) : lpr;
-          grpo_obj_token(lpr, po, old, adv, on, g_rs, p.clip, p.clip_lo, p.clip_hi, p.dual, p.kl_est, p.rx, obj, g,
-                         why);
+          if constexpr (PM)
+            grpo_pm_token(p.pm, lpr, po, old, adv, on, g_rs, p.clip, p.clip_hi, p.tau_pos, p.tau_neg, p.kl_est, p.rx,
+                          obj, g, why);
+          else
+            grpo_obj_token(lpr, po, old, adv, on, g_rs, p.clip, p.clip_lo, p.clip_hi, p.dual, p.kl_est, p.rx, obj, g,
+                           why);
         }
         sh_b[0] = m;
         sh_b[1] = logsum;
@@ -604,13 +622,13 @@ __global__ void __launch_bounds__(256) scale_tile_kernel(T *__restrict__ tile, i
 // two passes, inside the 50 MB L2, so the second pass is an L2 hit; with two rows in flight per SM part of it misses.
 // The kernel is bound by the MUFU / conversion pipe and instruction issue (two exp per logit + the bf16 pack) rather
 // than by HBM.
-template <typename T, bool ENT = false, bool EGRAD = false>
+template <typename T, bool ENT = false, bool EGRAD = false, bool PM = false>
 static int launch_fused_kernel(const FusedActorParams &p, int mode, FusedRec *rec, int64_t n_work, cudaStream_t st) {
   constexpr int CONSUMERS = 992, STAGES = 6, UNROLL = 2, LAG = 4;
   constexpr size_t smem = static_cast<size_t>(STAGES + 1) * CONSUMERS * UNROLL * 16 + STAGES * (8 + 8 + 8 + 4) + 16;
   const bool faithful = (mode == AA_MODE_FAITHFUL) && sizeof(T) == 2;
-  auto kf = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, true, ENT, EGRAD>;
-  auto kn = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, false, ENT, EGRAD>;
+  auto kf = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, true, ENT, EGRAD, PM>;
+  auto kn = logprob_actor_fused_kernel<T, CONSUMERS, STAGES, UNROLL, LAG, false, ENT, EGRAD, PM>;
   static std::atomic<bool> configured{false};  // the attribute is idempotent: a race sets it twice, harmlessly
   if (!configured.load(std::memory_order_relaxed)) {
     cudaError_t e = cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -637,30 +655,38 @@ static int launch_fused_kernel(const FusedActorParams &p, int mode, FusedRec *re
 }
 
 // egrad: the entropy-bonus kernels (p.entropy set)
-static int launch_fused(const FusedActorParams &p, int logits_dtype, int mode, FusedRec *rec, int64_t n_work,
-                        cudaStream_t st, bool egrad = false) {
+template <bool PM>
+static int launch_fused_of(const FusedActorParams &p, int logits_dtype, int mode, FusedRec *rec, int64_t n_work,
+                           cudaStream_t st, bool egrad) {
   if (egrad) {
     switch (logits_dtype) {
-      case AA_BF16: return launch_fused_kernel<__nv_bfloat16, true, true>(p, mode, rec, n_work, st);
-      case AA_F16: return launch_fused_kernel<__half, true, true>(p, mode, rec, n_work, st);
-      case AA_F32: return launch_fused_kernel<float, true, true>(p, mode, rec, n_work, st);
+      case AA_BF16: return launch_fused_kernel<__nv_bfloat16, true, true, PM>(p, mode, rec, n_work, st);
+      case AA_F16: return launch_fused_kernel<__half, true, true, PM>(p, mode, rec, n_work, st);
+      case AA_F32: return launch_fused_kernel<float, true, true, PM>(p, mode, rec, n_work, st);
     }
     return AA_ERR_DTYPE;
   }
   if (p.entropy) {
     switch (logits_dtype) {
-      case AA_BF16: return launch_fused_kernel<__nv_bfloat16, true>(p, mode, rec, n_work, st);
-      case AA_F16: return launch_fused_kernel<__half, true>(p, mode, rec, n_work, st);
-      case AA_F32: return launch_fused_kernel<float, true>(p, mode, rec, n_work, st);
+      case AA_BF16: return launch_fused_kernel<__nv_bfloat16, true, false, PM>(p, mode, rec, n_work, st);
+      case AA_F16: return launch_fused_kernel<__half, true, false, PM>(p, mode, rec, n_work, st);
+      case AA_F32: return launch_fused_kernel<float, true, false, PM>(p, mode, rec, n_work, st);
     }
     return AA_ERR_DTYPE;
   }
   switch (logits_dtype) {
-    case AA_BF16: return launch_fused_kernel<__nv_bfloat16>(p, mode, rec, n_work, st);
-    case AA_F16: return launch_fused_kernel<__half>(p, mode, rec, n_work, st);
-    case AA_F32: return launch_fused_kernel<float>(p, mode, rec, n_work, st);
+    case AA_BF16: return launch_fused_kernel<__nv_bfloat16, false, false, PM>(p, mode, rec, n_work, st);
+    case AA_F16: return launch_fused_kernel<__half, false, false, PM>(p, mode, rec, n_work, st);
+    case AA_F32: return launch_fused_kernel<float, false, false, PM>(p, mode, rec, n_work, st);
   }
   return AA_ERR_DTYPE;
+}
+
+// p.pm != 0: the PM kernels
+static int launch_fused(const FusedActorParams &p, int logits_dtype, int mode, FusedRec *rec, int64_t n_work,
+                        cudaStream_t st, bool egrad = false) {
+  return p.pm ? launch_fused_of<true>(p, logits_dtype, mode, rec, n_work, st, egrad)
+              : launch_fused_of<false>(p, logits_dtype, mode, rec, n_work, st, egrad);
 }
 
 // The fields every kind sets; each entry point adds its own and the kind.
@@ -701,6 +727,12 @@ struct ActorKlTerm {
   int est;
 };
 
+// the policy loss of the PM entry points (AA_PM_*) and SAPO's temperatures
+struct PolicyLoss {
+  int mode;
+  float tau_pos, tau_neg;
+};
+
 // aa_logprob_actor_fused{,_entropy,_obj,_kl}: entropy == nullptr runs the plain kernels; kl == nullptr: no KL term
 static int logprob_actor_fused(const char *who, float *entropy, float entropy_coeff, const void *logits, int logits_dtype,
                                int64_t row_stride, int32_t V, const int64_t *labels, int32_t n_segments,
@@ -710,7 +742,8 @@ static int logprob_actor_fused(const char *who, float *entropy, float entropy_co
                                int64_t old_stride, const void *advantages, int64_t adv_stride, int adv_dtype,
                                const uint8_t *mask, int64_t mask_stride, int32_t W, float clip_low, float clip_high,
                                float dual_clip, int loss_agg, int mode, void *grad_logits, int64_t grad_row_stride,
-                               void *row_scratch, int32_t *status, void *stream, const ActorKlTerm *kl = nullptr) {
+                               void *row_scratch, int32_t *status, void *stream, const ActorKlTerm *kl = nullptr,
+                               const PolicyLoss *pm = nullptr) {
   AA_REQUIRE(V > 0 && n_segments > 0 && W > 0 && n_tile_rows > 0 && n_tile_rows % n_segments == 0, AA_ERR_ARG,
              "%s: bad sizes (the gradient tile holds n_tile_rows / n_segments rows per sample)", who);
   AA_REQUIRE(logits && labels && seg_logit_off && seg_label_off && seg_out_off && seg_cum && seg_tile_row && log_probs &&
@@ -747,6 +780,12 @@ static int logprob_actor_fused(const char *who, float *entropy, float entropy_co
   p.rx = f ? lp_dtype : AA_F32;
   p.rp = f ? promote_dt(lp_dtype, adv_dtype) : AA_F32;
   p.ra = f ? adv_dtype : AA_F32;
+  if (pm) {
+    p.pm = pm->mode;
+    p.tau_pos = pm->tau_pos;
+    p.tau_neg = pm->tau_neg;
+    if (pm->mode == AA_PM_SAPO) p.rp = AA_F32;  // SAPO's s is fp32 (its temperature tensor is)
+  }
   FusedRec *rec = static_cast<FusedRec *>(row_scratch);
   if (entropy) {
     p.entropy = entropy;
@@ -874,11 +913,12 @@ extern "C" int aa_logprob_ce_fused(const void *logits, int logits_dtype, int64_t
   return launch_fused(p, logits_dtype, AA_MODE_F32, static_cast<FusedRec *>(row_scratch), n_tile_rows, st);
 }
 
-// the objective of aa_logprob_grpo_fused_obj (kind 3)
+// the objective of aa_logprob_grpo_fused_obj (kind 3); pm: the policy loss of aa_logprob_grpo_fused_pm (0: clipped)
 struct GrpoObjective {
   const void *old_pol;
   float clip_lo, clip_hi, dual;
   int agg, kl_est;
+  PolicyLoss pm;
 };
 
 // aa_logprob_grpo_fused{,_entropy,_obj}: entropy == nullptr runs the plain kernels; obj == nullptr: kind 2
@@ -930,6 +970,9 @@ static int logprob_grpo_fused(float *entropy, float entropy_coeff, bool egrad, c
     p.dual = obj->dual;
     p.agg = obj->agg;
     p.kl_est = obj->kl_est;
+    p.pm = obj->pm.mode;
+    p.tau_pos = obj->pm.tau_pos;
+    p.tau_neg = obj->pm.tau_neg;
   }
   return launch_fused(p, logits_dtype, mode, static_cast<FusedRec *>(row_scratch), n_tile_rows, st, egrad);
 }
@@ -996,14 +1039,15 @@ static int logprob_grpo_fused_objective(const char *who, const void *logits, int
                                         float beta, float clip_low, float clip_high, float dual_clip, int loss_agg,
                                         int kl_estimator, int mode, void *grad_logits, int64_t grad_row_stride,
                                         void *row_scratch, int32_t *row_end, float *total, uint32_t *counter,
-                                        int32_t *status, float *entropy, float entropy_coeff, void *stream) {
+                                        int32_t *status, float *entropy, float entropy_coeff, void *stream,
+                                        PolicyLoss pm = PolicyLoss{0, 1.f, 1.f}) {
   AA_REQUIRE(grpo_objective_ok(clip_low, clip_high, dual_clip, loss_agg), AA_ERR_ARG,
              "%s: bad objective (need 0 <= clip_low < 1, clip_high >= 0, dual_clip 0 or > 1, a known loss_agg; got %g "
              "%g %g %d)", who, clip_low, clip_high, dual_clip, loss_agg);
   AA_REQUIRE(kl_estimator_ok(kl_estimator), AA_ERR_ARG, "%s: unknown kl_estimator code %d", who, kl_estimator);
   AA_REQUIRE(entropy_coeff == entropy_coeff, AA_ERR_ARG, "%s: entropy_coeff is NaN", who);
   AA_REQUIRE(entropy || entropy_coeff == 0.f, AA_ERR_ARG, "%s: entropy_coeff needs entropy", who);
-  GrpoObjective obj{old_log_probs, clip_low, clip_high, dual_clip, loss_agg, kl_estimator};
+  GrpoObjective obj{old_log_probs, clip_low, clip_high, dual_clip, loss_agg, kl_estimator, pm};
   return logprob_grpo_fused(entropy, entropy_coeff, entropy && entropy_coeff != 0.f, who, logits, logits_dtype,
                             row_stride, V, labels, n_segments, seg_logit_off, seg_label_off, seg_out_off, seg_cum,
                             seg_tile_row, n_tile_rows, log_probs, lp_dtype, ref_log_probs, ref_stride, advantages,
@@ -1047,6 +1091,63 @@ extern "C" int aa_logprob_grpo_fused_kl(const void *logits, int logits_dtype, in
                                       advantages, completion_tokens, tok_stride, eos_id, K, beta, clip_low, clip_high,
                                       dual_clip, loss_agg, kl_estimator, mode, grad_logits, grad_row_stride,
                                       row_scratch, row_end, total, counter, status, entropy, entropy_coeff, stream);
+}
+
+extern "C" int aa_logprob_actor_fused_pm(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                         const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                         const int64_t *seg_label_off, const int64_t *seg_out_off,
+                                         const int64_t *seg_cum, const int64_t *seg_tile_row, int64_t n_tile_rows,
+                                         void *log_probs, int lp_dtype, float *stat_max, float *stat_logsum,
+                                         const void *old_log_probs, int64_t old_stride, const void *advantages,
+                                         int64_t adv_stride, int adv_dtype, const uint8_t *mask, int64_t mask_stride,
+                                         int32_t W, float clip_high, int loss_agg, int pm_mode, float tau_pos,
+                                         float tau_neg, int mode, void *grad_logits, int64_t grad_row_stride,
+                                         void *row_scratch, int32_t *status, float entropy_coeff, float *entropy,
+                                         const void *ref_log_probs, float kl_loss_coeff, int kl_estimator,
+                                         void *stream) {
+  const char *who = "aa_logprob_actor_fused_pm";
+  AA_REQUIRE(pm_mode_ok(pm_mode), AA_ERR_ARG, "%s: unknown pm_mode %d", who, pm_mode);
+  AA_REQUIRE(actor_objective_ok(0.f, clip_high, 0.f, loss_agg), AA_ERR_ARG,
+             "%s: bad objective (need clip_high >= 0 and a known loss_agg; got %g %d)", who, clip_high, loss_agg);
+  AA_REQUIRE(sapo_temperature_ok(tau_pos) && sapo_temperature_ok(tau_neg), AA_ERR_ARG,
+             "%s: tau_pos and tau_neg must be finite and > 0 (got %g %g)", who, tau_pos, tau_neg);
+  AA_REQUIRE(entropy_coeff == entropy_coeff, AA_ERR_ARG, "%s: entropy_coeff is NaN", who);
+  AA_REQUIRE(entropy || entropy_coeff == 0.f, AA_ERR_ARG, "%s: entropy_coeff needs entropy", who);
+  if (ref_log_probs) {
+    AA_REQUIRE(kl_estimator_ok(kl_estimator), AA_ERR_ARG, "%s: unknown kl_estimator code %d", who, kl_estimator);
+    AA_REQUIRE(kl_loss_term_ok(kl_loss_coeff), AA_ERR_ARG, "%s: kl_loss_coeff must be finite and > 0 (got %g)", who,
+               kl_loss_coeff);
+  }
+  const ActorKlTerm kl{ref_log_probs, kl_loss_coeff, kl_estimator};
+  const PolicyLoss pm{pm_mode, tau_pos, tau_neg};
+  return logprob_actor_fused(who, entropy, entropy_coeff, logits, logits_dtype, row_stride, V, labels, n_segments,
+                             seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row, n_tile_rows, log_probs,
+                             lp_dtype, stat_max, stat_logsum, old_log_probs, old_stride, advantages, adv_stride,
+                             adv_dtype, mask, mask_stride, W, 0.f, clip_high, 0.f, loss_agg, mode, grad_logits,
+                             grad_row_stride, row_scratch, status, stream, ref_log_probs ? &kl : nullptr, &pm);
+}
+
+extern "C" int aa_logprob_grpo_fused_pm(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                                        const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                                        const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
+                                        const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
+                                        const void *ref_log_probs, int64_t ref_stride, const void *old_log_probs,
+                                        const float *advantages, const int64_t *completion_tokens, int64_t tok_stride,
+                                        int64_t eos_id, int32_t K, float beta, float clip_high, int loss_agg,
+                                        int kl_estimator, int pm_mode, float tau_pos, float tau_neg, int mode,
+                                        void *grad_logits, int64_t grad_row_stride, void *row_scratch,
+                                        int32_t *row_end, float *total, uint32_t *counter, int32_t *status,
+                                        float *entropy, float entropy_coeff, void *stream) {
+  AA_REQUIRE(pm_mode_ok(pm_mode), AA_ERR_ARG, "aa_logprob_grpo_fused_pm: unknown pm_mode %d", pm_mode);
+  AA_REQUIRE(sapo_temperature_ok(tau_pos) && sapo_temperature_ok(tau_neg), AA_ERR_ARG,
+             "aa_logprob_grpo_fused_pm: tau_pos and tau_neg must be finite and > 0 (got %g %g)", tau_pos, tau_neg);
+  return logprob_grpo_fused_objective("aa_logprob_grpo_fused_pm", logits, logits_dtype, row_stride, V, labels,
+                                      n_segments, seg_logit_off, seg_label_off, seg_out_off, seg_cum, seg_tile_row,
+                                      n_tile_rows, log_probs, lp_dtype, ref_log_probs, ref_stride, old_log_probs,
+                                      advantages, completion_tokens, tok_stride, eos_id, K, beta, 0.f, clip_high, 0.f,
+                                      loss_agg, kl_estimator, mode, grad_logits, grad_row_stride, row_scratch,
+                                      row_end, total, counter, status, entropy, entropy_coeff, stream,
+                                      PolicyLoss{pm_mode, tau_pos, tau_neg});
 }
 
 extern "C" int aa_scale_tile(void *tile, int dtype, int64_t n, const void *scale, int scale_dtype, void *stream) {

@@ -14,6 +14,7 @@
 //                          top-entropy mask, and aa_grpo_loss_topent: GRPO's loss under that mask.
 //     aa_cov_moments / _keys / _select_hi / _hist_lo / _select_lo / _mark: the exact top-k covariance selection of
 //                          Clip-Cov and KL-Cov, and aa_ppo_actor_loss_cov / aa_grpo_loss_cov: the losses under it.
+//     aa_ppo_actor_loss_pm / aa_grpo_loss_pm: the CISPO and SAPO policy losses (ppo_math.cuh, pm_token).
 //
 // These touch ~10 floats per token: latency-bound, not bandwidth-bound.  The point is launch
 // count (thousands -> five) and zero host syncs; each sample is owned by one warp / CTA.
@@ -405,9 +406,12 @@ struct LossParams {
   const uint8_t *sel;
   int64_t sel_stride;
   float cov_coef;
+  // CISPO / SAPO (COV = AA_PM_*, aa_ppo_actor_loss_pm): SAPO's temperatures (pm_token); r_p is then s's dtype
+  float tau_pos, tau_neg;
 };
 
-// COV (actor only, aa_ppo_actor_loss_cov): AA_COV_CLIP / AA_COV_KL, the token's objective is cov_token's
+// COV (actor only): AA_COV_CLIP / AA_COV_KL (aa_ppo_actor_loss_cov), the token's objective is cov_token's;
+// AA_PM_CISPO / AA_PM_SAPO (aa_ppo_actor_loss_pm), pm_token's
 template <int THREADS, bool ACTOR, int COV = 0>
 __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
   static_assert(ACTOR || COV == 0, "Clip-Cov and KL-Cov are actor objectives");
@@ -448,7 +452,9 @@ __global__ void __launch_bounds__(THREADS) ppo_loss_kernel(const LossParams p) {
     float obj, grad;
     if (ACTOR) {
       int why;
-      if constexpr (COV != 0)
+      if constexpr (COV == AA_PM_CISPO || COV == AA_PM_SAPO)
+        pm_token(COV, x, old, aux, on, g_rs, p.clip_hi, p.tau_pos, p.tau_neg, rx, rp, obj, grad, why);
+      else if constexpr (COV != 0)
         cov_token(COV, x, old, aux, on, on && p.sel[b * p.sel_stride + t] != 0, g_rs, p.clip, p.clip_hi, p.cov_coef,
                   rx, rp, obj, grad, why);
       else
@@ -665,6 +671,8 @@ struct GrpoObjParams {
   const uint8_t *sel;
   int64_t sel_stride;
   float cov_coef;
+  // CISPO / SAPO (COV = AA_PM_*, aa_grpo_loss_pm): SAPO's temperatures
+  float tau_pos, tau_neg;
 };
 
 // GRPO's loss and d loss / d lp, one block per row, the last block to arrive reduces the rows.  OBJECTIVE: the clipped
@@ -675,8 +683,8 @@ struct GrpoObjParams {
 // then every token takes the row's objective and ratio coefficient (grpo_seq_row, grpo_seq_token).  TOPENT (with
 // OBJECTIVE, aa_grpo_loss_topent): the top-entropy mask -- a counted token with entropy < thr keeps only its KL term
 // (keep = 0 in grpo_obj_token; at sequence level s * keep, and s's gradient reaches the row's ratio from the kept
-// tokens alone, n_s of grpo_seq_row).  COV (with OBJECTIVE at token level, aa_grpo_loss_cov): Clip-Cov / KL-Cov
-// (grpo_cov_token)
+// tokens alone, n_s of grpo_seq_row).  COV (with OBJECTIVE at token level): Clip-Cov / KL-Cov (AA_COV_*,
+// aa_grpo_loss_cov, grpo_cov_token) or CISPO / SAPO (AA_PM_*, aa_grpo_loss_pm, grpo_pm_token)
 template <int THREADS, bool OBJECTIVE, bool SEQUENCE = false, bool TOPENT = false, int COV = 0>
 __global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoObjParams q) {
   static_assert(OBJECTIVE || !SEQUENCE, "the sequence-level ratio is an option of the clipped objective");
@@ -718,6 +726,9 @@ __global__ void __launch_bounds__(THREADS) grpo_loss_kernel(const GrpoObjParams 
     if constexpr (SEQUENCE) {
       grpo_seq_token(lp, rf, s_seq * keep, coef_seq, on, g_t, p.beta, q.kl_est, r, ptl, g);
       why = why_seq;
+    } else if constexpr (COV == AA_PM_CISPO || COV == AA_PM_SAPO) {
+      const float old = q.old ? load_as_float(q.old, b * q.old_stride + t, p.dtype) : lp;
+      grpo_pm_token(COV, lp, old, rf, A, on, g_t, p.beta, q.clip_hi, q.tau_pos, q.tau_neg, q.kl_est, r, ptl, g, why);
     } else if constexpr (COV != 0) {
       const float old = q.old ? load_as_float(q.old, b * q.old_stride + t, p.dtype) : lp;
       grpo_cov_token(COV, lp, old, rf, A, on, on && q.sel[b * q.sel_stride + t] != 0, g_t, p.beta, q.clip_lo,
@@ -1600,7 +1611,7 @@ static int grpo_loss(const char *who, bool objective, const void *log_probs, int
                      int32_t *row_end, float *scratch, uint32_t *counter, void *stream, bool sequence = false,
                      bool topent = false, const float *entropy = nullptr, int64_t ent_stride = 0,
                      const float *thr = nullptr, int cov = 0, float cov_coef = 0.f, const uint8_t *sel = nullptr,
-                     int64_t sel_stride = 0) {
+                     int64_t sel_stride = 0, float tau_pos = 1.f, float tau_neg = 1.f) {
   AA_REQUIRE(B > 0 && K > 0 && log_probs && ref_log_probs && advantages && completion_tokens && loss && row_end &&
                  scratch && counter,
              AA_ERR_ARG, "%s: bad arguments", who);
@@ -1624,8 +1635,12 @@ static int grpo_loss(const char *who, bool objective, const void *log_probs, int
                              K, beta, (mode == AA_MODE_FAITHFUL) ? lp_dtype : AA_F32, loss, grad, grad_stride,
                              scratch + 1, counter + 1},
                   old_log_probs, old_stride, clip_low, clip_high, dual_clip, loss_agg, clip_frac, kl_estimator,
-                  entropy, ent_stride, thr, sel, sel_stride, cov_coef};
-  if (cov == AA_COV_CLIP)
+                  entropy, ent_stride, thr, sel, sel_stride, cov_coef, tau_pos, tau_neg};
+  if (cov == AA_PM_CISPO)
+    grpo_loss_kernel<128, true, false, false, AA_PM_CISPO><<<B, 128, 0, st>>>(q);
+  else if (cov == AA_PM_SAPO)
+    grpo_loss_kernel<128, true, false, false, AA_PM_SAPO><<<B, 128, 0, st>>>(q);
+  else if (cov == AA_COV_CLIP)
     grpo_loss_kernel<128, true, false, false, AA_COV_CLIP><<<B, 128, 0, st>>>(q);
   else if (cov == AA_COV_KL)
     grpo_loss_kernel<128, true, false, false, AA_COV_KL><<<B, 128, 0, st>>>(q);
@@ -1934,6 +1949,60 @@ extern "C" int aa_grpo_loss_cov(const void *log_probs, int64_t lp_stride, const 
                    lp_dtype, advantages, completion_tokens, tok_stride, eos_id, B, K, beta, clip_low, clip_high, 0.f,
                    loss_agg, kl_estimator, mode, loss, grad, grad_stride, clip_frac, row_end, scratch, counter, stream,
                    false, false, nullptr, 0, nullptr, cov_mode, cov_coef, sel, sel_stride);
+}
+
+extern "C" int aa_ppo_actor_loss_pm(const void *log_probs, int64_t lp_stride, const void *old_log_probs,
+                                    int64_t old_stride, int lp_dtype, const void *advantages, int64_t adv_stride,
+                                    int adv_dtype, const uint8_t *mask, int64_t mask_stride, int32_t B, int32_t Wm,
+                                    float clip_high, int loss_agg, int pm_mode, float tau_pos, float tau_neg, int mode,
+                                    const void *ref_log_probs, int64_t ref_stride, float kl_loss_coeff,
+                                    int kl_estimator, float *loss, float *kl_loss, void *grad, int64_t grad_stride,
+                                    float *clip_frac, float *row_scratch, uint32_t *counter, void *stream) {
+  const char *who = "aa_ppo_actor_loss_pm";
+  AA_REQUIRE(B > 0 && Wm > 0, AA_ERR_ARG, "%s: bad sizes", who);
+  AA_REQUIRE(log_probs && old_log_probs && advantages && mask && loss && row_scratch && counter, AA_ERR_ARG,
+             "%s: null pointer", who);
+  AA_REQUIRE(dtype_ok(lp_dtype) && dtype_ok(adv_dtype), AA_ERR_DTYPE, "%s: bad dtype", who);
+  AA_REQUIRE(pm_mode_ok(pm_mode), AA_ERR_ARG, "%s: unknown pm_mode %d", who, pm_mode);
+  AA_REQUIRE(actor_objective_ok(0.f, clip_high, 0.f, loss_agg), AA_ERR_ARG,
+             "%s: bad objective (need clip_high >= 0 and a known loss_agg; got %g %d)", who, clip_high, loss_agg);
+  AA_REQUIRE(sapo_temperature_ok(tau_pos) && sapo_temperature_ok(tau_neg), AA_ERR_ARG,
+             "%s: tau_pos and tau_neg must be finite and > 0 (got %g %g)", who, tau_pos, tau_neg);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "%s: bad mode", who);
+  if (ref_log_probs) {
+    AA_REQUIRE(kl_estimator_ok(kl_estimator), AA_ERR_ARG, "%s: unknown kl_estimator code %d", who, kl_estimator);
+    AA_REQUIRE(kl_loss_term_ok(kl_loss_coeff) && kl_loss, AA_ERR_ARG,
+               "%s: a KL loss term needs kl_loss_coeff finite and > 0 (got %g) and kl_loss", who, kl_loss_coeff);
+  }
+  const bool f = (mode == AA_MODE_FAITHFUL);
+  // s's dtype: the promoted one under CISPO, fp32 under SAPO (its temperature tensor is fp32)
+  const int rp = (f && pm_mode == AA_PM_CISPO) ? promote(lp_dtype, adv_dtype) : AA_F32;
+  LossParams p{log_probs, lp_stride, old_log_probs, old_stride, lp_dtype, advantages, adv_stride, adv_dtype,
+               mask, mask_stride, B, Wm, 0.f, f ? lp_dtype : AA_F32, rp, loss, grad, grad_stride, nullptr, row_scratch,
+               counter, nullptr, 0, clip_high, 0.f, f ? adv_dtype : AA_F32, loss_agg, clip_frac, ref_log_probs,
+               ref_stride, ref_log_probs ? kl_loss_coeff : 0.f, kl_estimator, kl_loss, nullptr, 0, 0.f, tau_pos,
+               tau_neg};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (pm_mode == AA_PM_SAPO)
+    ppo_loss_kernel<128, true, AA_PM_SAPO><<<B, 128, 0, st>>>(p);
+  else
+    ppo_loss_kernel<128, true, AA_PM_CISPO><<<B, 128, 0, st>>>(p);
+  return check_launch(who);
+}
+
+extern "C" int aa_grpo_loss_pm(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
+                               const void *old_log_probs, int64_t old_stride, int lp_dtype, const float *advantages,
+                               const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B,
+                               int32_t K, float beta, float clip_high, int loss_agg, int kl_estimator, int pm_mode,
+                               float tau_pos, float tau_neg, int mode, float *loss, void *grad, int64_t grad_stride,
+                               float *clip_frac, int32_t *row_end, float *scratch, uint32_t *counter, void *stream) {
+  AA_REQUIRE(pm_mode_ok(pm_mode), AA_ERR_ARG, "aa_grpo_loss_pm: unknown pm_mode %d", pm_mode);
+  AA_REQUIRE(sapo_temperature_ok(tau_pos) && sapo_temperature_ok(tau_neg), AA_ERR_ARG,
+             "aa_grpo_loss_pm: tau_pos and tau_neg must be finite and > 0 (got %g %g)", tau_pos, tau_neg);
+  return grpo_loss("aa_grpo_loss_pm", true, log_probs, lp_stride, ref_log_probs, ref_stride, old_log_probs, old_stride,
+                   lp_dtype, advantages, completion_tokens, tok_stride, eos_id, B, K, beta, 0.f, clip_high, 0.f,
+                   loss_agg, kl_estimator, mode, loss, grad, grad_stride, clip_frac, row_end, scratch, counter, stream,
+                   false, false, nullptr, 0, nullptr, pm_mode, 0.f, nullptr, 0, tau_pos, tau_neg);
 }
 
 extern "C" int aa_nll_mean(const void *logp, int dtype, const int64_t *labels, int64_t n, int64_t ignore_index,

@@ -132,6 +132,44 @@ __device__ __forceinline__ void cov_token(int mode, float x, float old, float au
   }
 }
 
+// ---- CISPO and SAPO (ops.POLICY_LOSS_MODES 'cispo' / 'sapo'; tests/policy_loss_port.py is the specification) ----
+// the argument checks of the AA_PM_* entry points (ops.ActorObjective checks the same on the host)
+inline bool pm_mode_ok(int pm) { return pm == AA_PM_CISPO || pm == AA_PM_SAPO; }
+inline bool sapo_temperature_ok(float tau) { return tau > 0.f && tau <= 3.402823466e38f; }
+
+// One token of CISPO (MiniMax-M1) or SAPO (Qwen's Soft Adaptive Policy Optimization).  x, old, aux, on, g_rs, rx, obj,
+// grad: as actor_token's; rp: the dtype of s (the promoted dtype under CISPO; fp32 under SAPO, whose temperature
+// tensor is fp32).  ratio = exp(x - old) in rx.
+//   AA_PM_CISPO  w = clamp(ratio, max = round_rx(1 + eps_hi)), detached (NaN stays NaN);  obj = s = (w * aux) * x
+//                grad = round_rx(round_rp(g_rs * (w * aux)))      (MulBackward; nothing reaches the ratio)
+//                why bit 0: ratio > the bound (the clip-fraction counter)
+//   AA_PM_SAPO   tau = aux > 0 ? tau_pos : tau_neg;  sig = 1 / (1 + exp(-(tau * (ratio - 1))));  obj = ((sig * 4) / tau) * aux
+//                the backward op for op: Mul by aux, Div by tau, Mul by 4, SigmoidBackward ((g * (1 - sig)) * sig), Mul by
+//                tau (cast to rx), ExpBackward (* ratio);  why = 0
+__device__ __forceinline__ void pm_token(int pm, float x, float old, float aux, bool on, float g_rs, float eps_hi,
+                                         float tau_pos, float tau_neg, int rx, int rp, float &obj, float &grad,
+                                         int &why) {
+  const float ratio = round_to(expf(round_to(x - old, rx)), rx);
+  grad = 0.f;
+  why = 0;
+  if (pm == AA_PM_CISPO) {
+    const float hi = round_to(1.f + eps_hi, rx);
+    const bool over = ratio > hi;
+    const float wa = round_to((over ? hi : ratio) * aux, rp);
+    obj = round_to(wa * x, rp);
+    why = over ? 1 : 0;
+    if (on) grad = round_to(round_to(g_rs * wa, rp), rx);
+    return;
+  }
+  const float tau = aux > 0.f ? tau_pos : tau_neg;
+  const float sig = 1.f / (1.f + expf(-(tau * round_to(ratio - 1.f, rx))));
+  obj = ((sig * 4.f) / tau) * aux;
+  if (on) {
+    const float gu = ((((g_rs * aux) / tau) * 4.f) * (1.f - sig)) * sig;
+    grad = round_to(round_to(gu * tau, rx) * ratio, rx);
+  }
+}
+
 // ---- KL estimators (ops.KL_ESTIMATORS; tests/kl_objective_port.py is their specification) ---------------------
 // One token's estimate of KL(policy || reference) from the log-probs lp and rf, each op rounded to `r` as the eager
 // expression rounds it:
@@ -234,6 +272,19 @@ __device__ __forceinline__ void grpo_cov_token(int mode, float lp, float old, fl
                                                int est, int r, float &ptl, float &grad, int &why) {
   float s, ga, aux;
   cov_token(mode, lp, old, A, on, sel, -g_t, eps_lo, eps_hi, kl_coef, r, AA_F32, s, ga, why);
+  const float kl = kl_value(lp, rf, est, r, aux);
+  ptl = -(s - round_to(beta * kl, r));
+  grad = 0.f;
+  if (on) grad = kl_grad(ga, round_to(round_to(g_t, r) * beta, r), est, aux, r);
+}
+
+// One token of GRPO under CISPO / SAPO (aa_grpo_loss_pm, K1f's kind 3 with the mode): -(s - beta * KL) with
+// pm_token's s (fp32: the advantage is fp32) and grpo_obj_token's KL and accumulation order
+__device__ __forceinline__ void grpo_pm_token(int pm, float lp, float old, float rf, float A, bool on, float g_t,
+                                              float beta, float eps_hi, float tau_pos, float tau_neg, int est, int r,
+                                              float &ptl, float &grad, int &why) {
+  float s, ga, aux;
+  pm_token(pm, lp, old, A, on, -g_t, eps_hi, tau_pos, tau_neg, r, AA_F32, s, ga, why);
   const float kl = kl_value(lp, rf, est, r, aux);
   ptl = -(s - round_to(beta * kl, r));
   grad = 0.f;

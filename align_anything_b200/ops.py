@@ -1261,14 +1261,14 @@ class _GrpoLossFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj=None, old=None, clip_frac=None,
-                sequence=False, topent=None, cov=None):
+                sequence=False, topent=None, cov=None, pm=None):
         B, K = lp.shape
         dev = lp.device
         loss = torch.empty(1, dtype=torch.float32, device=dev)
         grad = torch.empty((B, K), dtype=lp.dtype, device=dev)
         row_end = torch.empty(B, dtype=torch.int32, device=dev)
         _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
-                          sequence=sequence, topent=topent, cov=cov)
+                          sequence=sequence, topent=topent, cov=cov, pm=pm)
         ctx.save_for_backward(grad)
         ctx.mark_non_differentiable(row_end)
         return loss[0], row_end
@@ -1277,11 +1277,11 @@ class _GrpoLossFn(torch.autograd.Function):
     def backward(ctx, g, _):
         (grad,) = ctx.saved_tensors
         return (grad.float() * g.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None, None, None, \
-            None
+            None, None
 
 
 def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, grad, clip_frac, row_end,
-                      scratch=None, sequence=False, topent=None, cov=None):
+                      scratch=None, sequence=False, topent=None, cov=None, pm=None):
     """GRPO's loss kernel, writing loss, row_end and (unless None) grad.  obj None: the reference loss (aa_grpo_loss);
     otherwise obj = _grpo_objective_args(...) for aa_grpo_loss_obj (aa_grpo_loss_kl unless the KL is k3), old = the old log-probs (None: the log-probs
     themselves, ratio 1) and clip_frac = an fp32[2] tensor for the clip fractions or None.  sequence (see
@@ -1289,7 +1289,7 @@ def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old
     thr fp32[1]) for the top-entropy mask, aa_grpo_loss_topent at either level (obj is then given).  scratch (fp32): the token
     count and the row sums, B + 1 values, and under the objective the rows' clip counts too, 1 + 4 B; None allocates it.
     cov (_CovTerm, obj given, token level): Clip-Cov / KL-Cov, the selection over GRPO's completion mask
-    (grpo_row_end) then aa_grpo_loss_cov."""
+    (grpo_row_end) then aa_grpo_loss_cov.  pm (_PmTerm, obj given, token level): CISPO / SAPO, aa_grpo_loss_pm."""
     B, K = lp.shape
     dev = lp.device
     if scratch is None:
@@ -1301,6 +1301,9 @@ def _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old
     tail = (row_end.data_ptr(), scratch.data_ptr(), _device_scratch(dev)['counter'][5:7].data_ptr(), L.stream_ptr(dev))
     if obj is None:
         L.check(lib.aa_grpo_loss(*lps, *rows, mode_code, *out, *tail))
+    elif pm is not None:
+        L.check(lib.aa_grpo_loss_pm(*lps, L.ptr(old), old.stride(0) if old is not None else 0, *rows, obj[1], obj[3],
+                                    obj[4], pm.code, pm.tau_pos, pm.tau_neg, mode_code, *out, L.ptr(clip_frac), *tail))
     elif cov is not None:
         sel = _cov_select(lp, adv, old, None, grpo_row_end(tokens, eos_id), cov, obj[0], obj[1], mode_code)
         L.check(lib.aa_grpo_loss_cov(*lps, L.ptr(old), old.stride(0) if old is not None else 0, *rows, obj[0], obj[1],
@@ -1479,7 +1482,7 @@ def grpo_loss(per_token_logps: torch.Tensor, ref_per_token_logps: torch.Tensor, 
     topent = _top_entropy_args(objective, entropy, tok, eos_token_id, lp.shape)
     cov = _cov_term(_objective(objective, GrpoObjective), cov_seed, lp.device)
     out = _GrpoLossFn.apply(lp, rlp, adv, tok, eos_token_id, beta, _mode_code(mode, lp.dtype), obj, old, cf,
-                            _sequence_level(objective, old), topent, cov)
+                            _sequence_level(objective, old), topent, cov, _pm_term(_objective(objective, GrpoObjective)))
     if cov is not None:
         out += (cov.share,)
     return out + (cf,) if return_clip_fraction else out
@@ -1513,9 +1516,10 @@ class _GrpoFusedFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, logits, labels, plan, ref_lp, adv, tokens, eos_id, beta, mode_code, entropy=None,
-                entropy_coeff=0.0, obj=None, old=None, clip_frac=None):
+                entropy_coeff=0.0, obj=None, old=None, clip_frac=None, pm=None):
         """obj: GrpoObjective.args() for aa_logprob_grpo_fused_obj + aa_grpo_loss_obj (old: the old log-probs or None,
-        clip_frac: an fp32[2] tensor for the clip fractions or None); None: today's launches."""
+        clip_frac: an fp32[2] tensor for the clip fractions or None); None: today's launches.  pm (_PmTerm, obj
+        given): CISPO / SAPO, aa_logprob_grpo_fused_pm + aa_grpo_loss_pm."""
         dev = logits.device
         B, K = plan.out_shape
         lp_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
@@ -1526,9 +1530,9 @@ class _GrpoFusedFn(torch.autograd.Function):
         scratch = torch.empty(B + 1, dtype=torch.float32, device=dev)  # K1f's token count; aa_grpo_loss's scratch too
         loss = torch.empty(1, dtype=torch.float32, device=dev)
         _k1f_grpo_launch(logits, labels, plan, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, grad, rows, row_end,
-                         scratch, entropy, entropy_coeff, obj, old)
+                         scratch, entropy, entropy_coeff, obj, old, pm)
         _grpo_loss_launch(lp, ref_lp, adv, tokens, eos_id, beta, mode_code, obj, old, loss, None, clip_frac, row_end,
-                          scratch if obj is None else None)
+                          scratch if obj is None else None, pm=pm)
         ctx.save_for_backward(grad)
         if entropy_coeff == 0.0:
             ctx.mark_non_differentiable(lp, row_end)
@@ -1541,14 +1545,15 @@ class _GrpoFusedFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g, *_unused):
         (grad,) = _hand_over_once(ctx, g, *ctx.saved_tensors)
-        return grad, None, None, None, None, None, None, None, None, None, None, None, None, None
+        return grad, None, None, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 def _k1f_grpo_launch(logits, labels, plan, lp, ref_lp, adv, tokens, eos_id, beta, mode_code, grad, rows, row_end,
-                     total, entropy, entropy_coeff, obj, old):
+                     total, entropy, entropy_coeff, obj, old, pm=None):
     """K1f over GRPO's completion rows (`rows`: its int64 row records, 6 per tile row), writing lp, row_end, the token
     count `total[0]`, the gradient tile `grad` and (unless None) the fp32 entropy.  obj: GrpoObjective.args() for the objective entry point (aa_logprob_grpo_fused_obj, old: the old
-    log-probs or None); None: the reference loss, plain, with the entropy, or with the entropy bonus's gradient."""
+    log-probs or None); None: the reference loss, plain, with the entropy, or with the entropy bonus's gradient.
+    pm (_PmTerm, obj given): CISPO / SAPO's entry point (aa_logprob_grpo_fused_pm)."""
     dev = logits.device
     K = plan.out_shape[1]
     sc = _device_scratch(dev)
@@ -1560,7 +1565,11 @@ def _k1f_grpo_launch(logits, labels, plan, lp, ref_lp, adv, tokens, eos_id, beta
     mid = (adv.data_ptr(), tokens.data_ptr(), tokens.stride(0), int(eos_id), K, float(beta))
     tail = (mode_code, grad.data_ptr(), logits.size(-1), rows.data_ptr(), row_end.data_ptr(), total.data_ptr(),
             sc['counter'][5:6].data_ptr(), sc['status'].data_ptr())
-    if obj is not None and obj[4] == KL_ESTIMATORS['k3']:
+    if pm is not None:
+        L.check(lib.aa_logprob_grpo_fused_pm(*head, L.ptr(old), *mid, obj[1], obj[3], obj[4], pm.code, pm.tau_pos,
+                                             pm.tau_neg, *tail, L.ptr(entropy), float(entropy_coeff),
+                                             L.stream_ptr(dev)))
+    elif obj is not None and obj[4] == KL_ESTIMATORS['k3']:
         L.check(lib.aa_logprob_grpo_fused_obj(*head, L.ptr(old), *mid, *obj[:4], *tail, L.ptr(entropy),
                                               float(entropy_coeff), L.stream_ptr(dev)))
     elif obj is not None:  # another KL estimator: the same kernel with the estimator's code
@@ -1608,7 +1617,7 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
     tokens = input_ids[:, -K:]
     coeff = float(entropy_coeff)
     topent = _top_entropy(objective)
-    cov = getattr(objective, 'policy_loss_mode', 'vanilla') != 'vanilla'
+    cov = getattr(objective, 'policy_loss_mode', 'vanilla') in COV_MODES
     if _sequence_level(objective, old_per_token_logps) or topent or cov or \
             not _single_pass_ok(logits, _FUSED_GRPO, torch.is_grad_enabled() and logits.requires_grad):
         ent = None
@@ -1651,7 +1660,7 @@ def grpo_loss_from_logits(logits: torch.Tensor, input_ids: torch.Tensor, logits_
     ent = torch.zeros((B, K), dtype=torch.float32, device=logits.device) if return_entropy or coeff != 0.0 else None
     cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
     out = _GrpoFusedFn.apply(logits, labels, plan, rlp, adv, tok, int(eos_token_id), float(beta), mode_code, ent, coeff,
-                             obj, old, cf)
+                             obj, old, cf, _pm_term(_objective(objective, GrpoObjective)))
     if return_entropy:
         out += (ent,)
     return out + (cf,) if return_clip_fraction else out
@@ -2329,9 +2338,14 @@ def whiten_advantages(advantages: list[torch.Tensor], masks: list[torch.Tensor],
 
 
 LOSS_AGG_MODES = {'seq-mean-token-mean': 0, 'token-mean': 1}  # include/aa_b200.h AA_AGG_*
-POLICY_LOSS_MODES = {'vanilla': 0, 'clip_cov': 1, 'kl_cov': 2}  # include/aa_b200.h AA_COV_*
+# include/aa_b200.h AA_COV_* (clip_cov, kl_cov) and AA_PM_* (cispo, sapo)
+POLICY_LOSS_MODES = {'vanilla': 0, 'clip_cov': 1, 'kl_cov': 2, 'cispo': 3, 'sapo': 4}
+COV_MODES = ('clip_cov', 'kl_cov')  # the modes that select tokens by covariance (_cov_term)
+PM_MODES = ('cispo', 'sapo')  # the per-token policy losses of the AA_PM_* entry points (_pm_term)
 # verl's defaults of the Clip-Cov / KL-Cov keys (ActorObjective: None takes these)
 COV_DEFAULTS = {'clip_cov_ratio': 2e-4, 'clip_cov_lb': 1.0, 'clip_cov_ub': 5.0, 'kl_cov_ratio': 2e-4, 'ppo_kl_coef': 1.0}
+# TRL's defaults of SAPO's temperatures (ActorObjective: None takes these)
+SAPO_DEFAULTS = {'sapo_temperature_pos': 1.0, 'sapo_temperature_neg': 1.05}
 
 
 @dataclasses.dataclass(frozen=True)
@@ -2352,9 +2366,20 @@ class ActorObjective:
     clip_cov_lb < cov_t < clip_cov_ub, max(int(clip_cov_ratio * N), 1) (N = counted tokens) chosen by a hash of the
     flat index and the seed lose their objective term and its gradient.  'kl_cov': the objective is unclipped, s = A *
     ratio, and the max(1, int(kl_cov_ratio * N)) tokens with the largest cov_t take s - ppo_kl_coef * |lp - old|.  The
-    five keys are None for their defaults (2e-4, 1.0, 5.0, 2e-4, 1.0) and refused under 'vanilla'; neither mode takes
-    dual_clip_ratio, and 'kl_cov' refuses an explicit clip range, which it would ignore.  The fields are checked here,
-    on the host, before anything is launched."""
+    five keys are None for their defaults (2e-4, 1.0, 5.0, 2e-4, 1.0) and refused under any other mode; neither mode
+    takes dual_clip_ratio, and 'kl_cov' refuses an explicit clip range, which it would ignore.
+    policy_loss_mode 'cispo' (MiniMax-M1, 2025) and 'sapo' (Qwen's Soft Adaptive Policy Optimization, 2025; TRL's
+    GRPO loss_type 'cispo' / 'sapo') replace the clipped ratio per token, with s the negated loss term aggregated as
+    above (tests/policy_loss_port.py is the specification):
+        'cispo'  w = clamp(ratio, max = 1 + clip_range_ratio_high).detach() ;  s = w * A * lp     (every token keeps
+                 the gradient w * A; train/actor_clip_fraction counts ratio > 1 + clip_range_ratio_high)
+        'sapo'   tau = sapo_temperature_pos where A > 0, else sapo_temperature_neg ;
+                 s = sigmoid(tau * (ratio - 1)) * 4 / tau * A                                     (fp32; nothing clipped)
+    Neither takes dual_clip_ratio; 'cispo' refuses clip_range_ratio_low and 'sapo' any clip range, which they would
+    ignore.  sapo_temperature_pos / _neg: None for 1.0 / 1.05, finite and > 0 as fp32 (the kernels' type), refused
+    under any mode but 'sapo'.
+    Both stay on K1f's single pass: each token's loss and gradient need that token alone.  The fields are checked
+    here, on the host, before anything is launched."""
 
     clip_range_ratio_low: float | None = None
     clip_range_ratio_high: float | None = None
@@ -2366,6 +2391,8 @@ class ActorObjective:
     clip_cov_ub: float | None = None
     kl_cov_ratio: float | None = None
     ppo_kl_coef: float | None = None
+    sapo_temperature_pos: float | None = None
+    sapo_temperature_neg: float | None = None
     _MODES = LOSS_AGG_MODES  # the aggregations this objective takes (a class attribute, not a field)
 
     def __post_init__(self):
@@ -2384,19 +2411,37 @@ class ActorObjective:
         mode = self.policy_loss_mode
         if mode not in POLICY_LOSS_MODES:
             raise ValueError(f'policy_loss_mode must be one of {tuple(POLICY_LOSS_MODES)}, got {mode!r}')
+        temps = {k: getattr(self, k) for k in SAPO_DEFAULTS}
+        given = [k for k, v in temps.items() if v is not None]
+        if given and mode != 'sapo':
+            raise ValueError(f'{", ".join(given)} need policy_loss_mode sapo (it is {mode})')
+        for k, v in temps.items():
+            # the kernels take the temperature as an fp32: it must stay finite and > 0 there too (1e39 is inf and
+            # 1e-50 is 0 in fp32, which the C argument checks refuse)
+            if v is not None and (isinstance(v, bool) or not isinstance(v, (int, float)) or
+                                  not (math.isfinite(ctypes.c_float(float(v)).value) and
+                                       ctypes.c_float(float(v)).value > 0.0)):
+                raise ValueError(f'{k} must be a finite number > 0 in fp32, got {v!r}')
         keys = {k: getattr(self, k) for k in COV_DEFAULTS}
-        if mode == 'vanilla':
+        if mode not in COV_MODES:
             given = [k for k, v in keys.items() if v is not None]
             if given:
-                raise ValueError(f'{", ".join(given)} need policy_loss_mode clip_cov or kl_cov (it is vanilla)')
+                raise ValueError(f'{", ".join(given)} need policy_loss_mode clip_cov or kl_cov (it is {mode})')
+        if mode == 'vanilla':
+            return
+        if self.dual_clip_ratio is not None:
+            raise ValueError(f'policy_loss_mode {mode!r} has no dual-clip: dual_clip_ratio must be unset')
+        if mode in ('kl_cov', 'sapo') and (self.clip_range_ratio_low is not None or
+                                           self.clip_range_ratio_high is not None):
+            raise ValueError(f'policy_loss_mode {mode} is unclipped: clip_range_ratio_low / _high would be ignored')
+        if mode == 'cispo' and self.clip_range_ratio_low is not None:
+            raise ValueError('policy_loss_mode cispo truncates the ratio from above only: clip_range_ratio_low would be '
+                             'ignored')
+        if mode in PM_MODES:
             return
         for k, v in keys.items():
             if v is not None and (isinstance(v, bool) or not isinstance(v, (int, float))):
                 raise ValueError(f'{k} must be a number, got {v!r}')
-        if self.dual_clip_ratio is not None:
-            raise ValueError(f'policy_loss_mode {mode!r} has no dual-clip: dual_clip_ratio must be unset')
-        if mode == 'kl_cov' and (self.clip_range_ratio_low is not None or self.clip_range_ratio_high is not None):
-            raise ValueError('policy_loss_mode kl_cov is unclipped: clip_range_ratio_low / _high would be ignored')
         for k in ('clip_cov_ratio', 'kl_cov_ratio'):
             if not 0.0 < self.cov_value(k) <= 1.0:
                 raise ValueError(f'{k} must lie in (0, 1], got {keys[k]!r}')
@@ -2406,6 +2451,11 @@ class ActorObjective:
         c = self.cov_value('ppo_kl_coef')
         if not (math.isfinite(c) and c >= 0.0):
             raise ValueError(f'ppo_kl_coef must be finite and >= 0, got {c!r}')
+
+    def sapo_value(self, key: str) -> float:
+        """One of SAPO's temperatures in effect: the field, or its default (SAPO_DEFAULTS) when None."""
+        v = getattr(self, key)
+        return float(SAPO_DEFAULTS[key] if v is None else v)
 
     def cov_value(self, key: str) -> float:
         """One of the Clip-Cov / KL-Cov keys in effect: the field, or its default (COV_DEFAULTS) when None."""
@@ -2546,9 +2596,27 @@ class _CovTerm:
 
 def _cov_term(objective, seed: int, device) -> _CovTerm | None:
     """None unless the objective's policy_loss_mode is clip_cov or kl_cov."""
-    if objective is None or objective.policy_loss_mode == 'vanilla':
+    if objective is None or objective.policy_loss_mode not in COV_MODES:
         return None
     return _CovTerm(objective, seed, device)
+
+
+class _PmTerm:
+    """CISPO / SAPO of one loss call: the mode's AA_PM_* code and SAPO's temperatures in effect (CISPO ignores them).
+    `sapo`: s, and so the loss, is fp32 whatever the dtypes (the temperature tensor is fp32)."""
+
+    def __init__(self, objective: ActorObjective):
+        self.code = POLICY_LOSS_MODES[objective.policy_loss_mode]
+        self.sapo = objective.policy_loss_mode == 'sapo'
+        self.tau_pos = objective.sapo_value('sapo_temperature_pos')
+        self.tau_neg = objective.sapo_value('sapo_temperature_neg')
+
+
+def _pm_term(objective) -> _PmTerm | None:
+    """None unless the objective's policy_loss_mode is cispo or sapo."""
+    if objective is None or objective.policy_loss_mode not in PM_MODES:
+        return None
+    return _PmTerm(objective)
 
 
 def _cov_select(x, aux, old, mask, row_end, cov: _CovTerm, clip_lo: float, clip_hi: float, mode_code: int):
@@ -2646,14 +2714,15 @@ def token_mean(x: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
 
 
 def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=None, obj=None, clip_frac=None, kl=None,
-                     cov=None):
+                     cov=None, pm=None):
     """K5: -> (loss fp32[2], loss as a 0-dim tensor of the promoted dtype (a view, no launch), grad (B, Wm), row_mean).
     x_tail = (DeviceLens, src_width): `x` is the raw (B, src_width) tensor and the kernel reads the per-sample tails.
     Actor only: obj = ActorObjective.args(...) (None: the reference's objective), clip_frac = an fp32[2] tensor the
     kernel fills with the clip fractions (aa_ppo_actor_loss_obj); kl = _KlLossTerm: the KL loss term
     (aa_ppo_actor_loss_kl: grad is d (loss + coeff * agg(KL)) / d x, kl.out receives agg(KL), `loss` stays the
     clipped objective).  cov = _CovTerm (obj given): Clip-Cov / KL-Cov, the selection (_cov_select) then
-    aa_ppo_actor_loss_cov, with the KL loss term when kl is given."""
+    aa_ppo_actor_loss_cov, with the KL loss term when kl is given.  pm = _PmTerm (obj given): CISPO / SAPO,
+    aa_ppo_actor_loss_pm, with the KL loss term when kl is given (SAPO's loss is fp32)."""
     B, Wm = old.shape
     dev = x.device
     loss = torch.empty(2, dtype=torch.float32, device=dev)
@@ -2662,7 +2731,18 @@ def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=Non
     row_mean = torch.empty(B, dtype=torch.float32, device=dev)
     sc = _device_scratch(dev)
     lib = L.lib()
-    if actor and cov is not None:
+    if actor and pm is not None:
+        _, hi, _, agg = obj
+        rows = torch.empty(5 * B, dtype=torch.float32, device=dev)
+        L.check(lib.aa_ppo_actor_loss_pm(
+            x.data_ptr(), x.stride(0), old.data_ptr(), old.stride(0), L.dtype_code(x.dtype), aux.data_ptr(),
+            aux.stride(0), L.dtype_code(aux.dtype), mask.data_ptr(), mask.stride(0), B, Wm, float(hi), int(agg),
+            pm.code, pm.tau_pos, pm.tau_neg, mode_code, kl.ref.data_ptr() if kl is not None else None,
+            kl.ref.stride(0) if kl is not None else 0, kl.coeff if kl is not None else 0.0,
+            kl.estimator if kl is not None else 0, loss.data_ptr(), kl.out.data_ptr() if kl is not None else None,
+            grad.data_ptr(), grad.stride(0), L.ptr(clip_frac), rows.data_ptr(), sc['counter'][2:3].data_ptr(),
+            L.stream_ptr(dev)))
+    elif actor and cov is not None:
         lo, hi, _, agg = obj
         sel = _cov_select(x, aux, old, mask, None, cov, lo, hi, mode_code)
         rows = torch.empty(5 * B, dtype=torch.float32, device=dev)
@@ -2704,7 +2784,8 @@ def _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor: bool, x_tail=Non
             mode_code, loss.data_ptr(), grad.data_ptr(), grad.stride(0), row_mean.data_ptr(), rows.data_ptr(),
             sc['counter'][3:4].data_ptr(), x_tail[0].dev.data_ptr() if x_tail else None, int(x_tail[1]) if x_tail else 0,
             L.stream_ptr(dev)))
-    out_dtype = _promote(x.dtype, aux.dtype) if mode_code == L.MODE_FAITHFUL else torch.float32
+    faithful = mode_code == L.MODE_FAITHFUL and not (pm is not None and pm.sapo)
+    out_dtype = _promote(x.dtype, aux.dtype) if faithful else torch.float32
     cast = loss[0] if out_dtype == torch.float32 else loss[1:2].view(out_dtype)[0]
     return loss, cast, grad, row_mean
 
@@ -2714,9 +2795,10 @@ class _PpoLossFn(torch.autograd.Function):
     (kl, actor only) the first output is  loss + kl.coeff * agg(KL)  (fp32) and its gradient is K5's."""
 
     @staticmethod
-    def forward(ctx, x, old, aux, mask, clip, mode_code, actor: bool, obj=None, clip_frac=None, kl=None, cov=None):
+    def forward(ctx, x, old, aux, mask, clip, mode_code, actor: bool, obj=None, clip_frac=None, kl=None, cov=None,
+                pm=None):
         loss, cast, grad, row_mean = _ppo_loss_launch(x, old, aux, mask, clip, mode_code, actor, obj=obj,
-                                                      clip_frac=clip_frac, kl=kl, cov=cov)
+                                                      clip_frac=clip_frac, kl=kl, cov=cov, pm=pm)
         ctx.save_for_backward(grad)
         ctx.mark_non_differentiable(row_mean, loss)
         return (cast if kl is None else kl.regularised(loss[0])), row_mean, loss
@@ -2724,18 +2806,21 @@ class _PpoLossFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_loss, _g, _l):
         (grad,) = ctx.saved_tensors
-        return (grad.float() * g_loss.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None, None
+        return (grad.float() * g_loss.float()).to(grad.dtype), None, None, None, None, None, None, None, None, None, \
+            None, None
 
 
-def _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, grad, obj, coeff, ent, kl=None):
+def _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, grad, obj, coeff, ent, kl=None, pm=None):
     """K1f over the actor's scored rows, writing lp and the gradient tile `grad`.  obj: ActorObjective.args(...) for
     the objective entry point (aa_logprob_actor_fused_obj), None for the reference's objective -- with an entropy
     bonus (`ent`, the fp32 entropy out) the entropy-gradient entry point, otherwise the plain one.  kl (_KlLossTerm):
-    the KL loss term's entry point (aa_logprob_actor_fused_kl), whatever the objective."""
+    the KL loss term's entry point (aa_logprob_actor_fused_kl), whatever the objective.  pm (_PmTerm, obj given):
+    CISPO / SAPO's entry point (aa_logprob_actor_fused_pm), with the KL loss term and the entropy as given."""
     dev = logits.device
     # 48 bytes per tile row (the row records); the entropy-gradient and objective forms add 4 per segment (the rows'
     # g_H coefficients), the KL form 8 (and the rows' KL coefficients)
-    extra = plan.n_seg if kl is not None else (plan.n_seg + 1) // 2 if obj is not None or ent is not None else 0
+    extra = plan.n_seg if kl is not None or pm is not None else \
+        (plan.n_seg + 1) // 2 if obj is not None or ent is not None else 0
     scratch = torch.empty(plan.n_tile_rows * 6 + extra, dtype=torch.int64, device=dev)
     p = plan.ptrs()
     lib = L.lib()
@@ -2744,7 +2829,12 @@ def _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, gr
             None, old.data_ptr(), old.stride(0), aux.data_ptr(), aux.stride(0), L.dtype_code(aux.dtype),
             mask.data_ptr(), mask.stride(0), lp.size(1))
     tail = (mode_code, grad.data_ptr(), logits.size(-1), scratch.data_ptr(), _device_scratch(dev)['status'].data_ptr())
-    if kl is not None:
+    if pm is not None:
+        L.check(lib.aa_logprob_actor_fused_pm(*head, float(obj[1]), int(obj[3]), pm.code, pm.tau_pos, pm.tau_neg,
+                                              *tail, coeff, L.ptr(ent), L.ptr(kl.ref if kl is not None else None),
+                                              kl.coeff if kl is not None else 0.0, kl.estimator if kl is not None else 0,
+                                              L.stream_ptr(dev)))
+    elif kl is not None:
         L.check(lib.aa_logprob_actor_fused_kl(*head, *(obj if obj is not None else (clip, clip, 0.0, 0)), *tail, coeff,
                                               L.ptr(ent), kl.ref.data_ptr(), kl.coeff, kl.estimator, L.stream_ptr(dev)))
     elif obj is not None:
@@ -2776,11 +2866,12 @@ class _TailActorLossFn(torch.autograd.Function):
     output stays the actor loss without it), K1f's KL entry point (aa_logprob_actor_fused_kl) writes its gradient into
     the tile, K5's (aa_ppo_actor_loss_kl) the loss value, agg(KL) into kl.out and, for K1b, d total / d log-probs.
     cov (_CovTerm, with single_pass False): Clip-Cov / KL-Cov -- the selection needs every log-prob of the call first,
-    so K1 -> selection -> aa_ppo_actor_loss_cov -> K1b."""
+    so K1 -> selection -> aa_ppo_actor_loss_cov -> K1b.  pm (_PmTerm): CISPO / SAPO, K1f's and K5's PM entry points
+    (aa_logprob_actor_fused_pm, aa_ppo_actor_loss_pm), or K1 -> aa_ppo_actor_loss_pm -> K1b."""
 
     @staticmethod
     def forward(ctx, logits, ids, plan, old, aux, mask, clip, mode_code, single_pass, entropy_coeff=0.0, objective=None,
-                clip_frac=None, kl=None, cov=None):
+                clip_frac=None, kl=None, cov=None, pm=None):
         out_dtype = logits.dtype if mode_code == L.MODE_FAITHFUL else torch.float32
         dev = logits.device
         coeff = float(entropy_coeff)
@@ -2792,13 +2883,13 @@ class _TailActorLossFn(torch.autograd.Function):
         ent = torch.zeros(plan.out_shape, dtype=torch.float32, device=dev) if ctx.bonus else None
         if ctx.fused:
             grad = torch.empty(logits.shape, dtype=logits.dtype, device=dev)
-            _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, grad, obj, coeff, ent, kl)
+            _k1f_actor_launch(logits, ids, plan, lp, old, aux, mask, clip, mode_code, grad, obj, coeff, ent, kl, pm)
             ctx.save_for_backward(grad)
         else:
             stats = torch.empty((2, max(plan.n_rows, 1)), dtype=torch.float32, device=dev)
             _launch_fwd(logits, ids, plan, lp, stats[0], stats[1], entropy=ent)
         loss, cast, grad_lp, _ = _ppo_loss_launch(lp, old, aux, mask, clip, mode_code, True, obj=obj, clip_frac=clip_frac,
-                                                  kl=kl, cov=cov)
+                                                  kl=kl, cov=cov, pm=pm)
         tm = objective is not None and objective.token_mean
         if not ctx.fused:
             if ctx.bonus:
@@ -2823,7 +2914,7 @@ class _TailActorLossFn(torch.autograd.Function):
     def backward(ctx, g_loss, *_unused):
         if ctx.fused:
             (grad,) = _hand_over_once(ctx, g_loss, *ctx.saved_tensors)
-            return grad, None, None, None, None, None, None, None, None, None, None, None, None, None
+            return grad, None, None, None, None, None, None, None, None, None, None, None, None, None, None
         scale = g_loss.detach().reshape(1)
         if scale.dtype not in (torch.float32, torch.bfloat16, torch.float16):
             scale = scale.float()
@@ -2835,7 +2926,7 @@ class _TailActorLossFn(torch.autograd.Function):
         grad = torch.empty(logits.shape, dtype=logits.dtype, device=logits.device)
         _launch_bwd(logits, ids, ctx.plan, stats[0], stats[1], grad_lp, None, scale, grad, ctx.mode_code, entropy=ent,
                     grad_entropy=g_h)
-        return grad, None, None, None, None, None, None, None, None, None, None, None, None, None
+        return grad, None, None, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 class _TailCriticLossFn(torch.autograd.Function):
@@ -2959,7 +3050,7 @@ def _actor_loss(log_probs, old_log_probs, advantages, mask, clip_range_ratio, mo
     cov = _cov_term(objective, cov_seed, x.device)
     cf = torch.zeros(2, dtype=torch.float32, device=x.device) if return_clip_fraction else None
     loss, _, loss32 = _PpoLossFn.apply(x, old, aux, m, clip_range_ratio, _mode_code(mode, x.dtype), True, obj, cf, kl,
-                                       cov)
+                                       cov, _pm_term(objective))
     share = cov.share if cov is not None else None
     if kl is None:
         return loss, loss, None, cf, share
@@ -3008,7 +3099,7 @@ def tail_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, lens, old_log
         objective.args(clip_range_ratio)  # a bad clip range fails here, before the node launches anything
     cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
     out = _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, single_pass,
-                                 float(entropy_coeff), objective, cf, kl, cov)
+                                 float(entropy_coeff), objective, cf, kl, cov, _pm_term(objective))
     return (*out, *((kl.out[0],) if kl is not None else ()), *((cov.share,) if cov is not None else ()),
             *((cf,) if return_clip_fraction else ()))
 
@@ -3054,7 +3145,7 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
         raise ValueError('old_log_probs, advantages and mask must all be (B, L - 1 - start)')
     if objective is not None:
         objective.args(clip_range_ratio)  # a bad clip range fails here, before any launch
-    cov_mode = objective is not None and objective.policy_loss_mode != 'vanilla'
+    cov_mode = objective is not None and objective.policy_loss_mode in COV_MODES
     if cov_mode or not _single_pass_ok(logits, _FUSED_ACTOR, torch.is_grad_enabled() and logits.requires_grad):
         # short rows, fp16, no gradient: the composed ops (K1 over the response rows -> K5, which takes the objective;
         # backward K1b)
@@ -3084,7 +3175,7 @@ def dense_actor_loss(logits: torch.Tensor, input_ids: torch.Tensor, start: int, 
     plan = _dense_actor_plan(B, Lq, start, logits.stride(0), logits.stride(1), ids.stride(0), str(logits.device))
     cf = torch.zeros(2, dtype=torch.float32, device=logits.device) if return_clip_fraction else None
     out = _TailActorLossFn.apply(logits, ids, plan, old, aux, m, clip_range_ratio, mode_code, True,
-                                 float(entropy_coeff), objective, cf, kl)
+                                 float(entropy_coeff), objective, cf, kl, None, _pm_term(objective))
     return (*out, *((kl.out[0],) if kl is not None else ()), *((cf,) if return_clip_fraction else ()))
 
 

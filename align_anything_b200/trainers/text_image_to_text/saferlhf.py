@@ -44,8 +44,10 @@ def refuse_kl_switches(tr) -> None:
 
 def refuse_cov_switches(tr) -> None:
     """Safe RLHF-V keeps the reference's clipped actor objective: the Clip-Cov / KL-Cov switches it inherits from the
-    PPO trainers raise here, before anything runs, when set (policy_loss_mode to anything but vanilla)."""
-    for name in ('policy_loss_mode', 'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef'):
+    PPO trainers raise here, before anything runs, when set (policy_loss_mode to anything but vanilla), and so do the
+    CISPO / SAPO keys."""
+    for name in ('policy_loss_mode', 'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef',
+                 'sapo_temperature_pos', 'sapo_temperature_neg'):
         v = switch_of(tr, name)
         if v is not None and not (name == 'policy_loss_mode' and v == 'vanilla'):
             raise ValueError(f'{name}={v!r}: Safe RLHF-V keeps the reference\'s clipped actor objective')

@@ -17,7 +17,8 @@ __all__ = ['GRPOTrainer']
 
 GRPO_OBJECTIVE_KEYS = ('clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio',
                        'loss_agg_mode', 'kl_estimator', 'importance_sampling_level', 'top_entropy_quantile',
-                       'policy_loss_mode', 'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef')
+                       'policy_loss_mode', 'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef',
+                       'sapo_temperature_pos', 'sapo_temperature_neg')
 
 
 def num_iterations_of(tr) -> int:
@@ -97,6 +98,11 @@ class GRPOTrainer:
     clip_cov_ub = None
     kl_cov_ratio = None
     ppo_kl_coef = None
+    # CISPO / SAPO (TRL's GRPO loss_type 'cispo' / 'sapo', see ops.GrpoObjective): policy_loss_mode 'cispo' or 'sapo',
+    # token level only, on K1f's single pass whenever it runs; SAPO's temperatures sapo_temperature_pos / _neg (None =
+    # 1.0 / 1.05).  `cfgs.train_cfgs.<key>` overrides each when set.
+    sapo_temperature_pos = None
+    sapo_temperature_neg = None
     # Opt-in: train/actor_clip_fraction (and train/actor_dual_clip_fraction with dual-clip), the mean over the updates,
     # in the step's one packed all-reduce
     log_clip_fraction = False
@@ -105,7 +111,7 @@ class GRPOTrainer:
                 'clip_range_ratio', 'clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode',
                 'scale_rewards', 'log_clip_fraction', 'kl_estimator', 'importance_sampling_level',
                 'top_entropy_quantile', 'policy_loss_mode', 'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub',
-                'kl_cov_ratio', 'ppo_kl_coef')
+                'kl_cov_ratio', 'ppo_kl_coef', 'sapo_temperature_pos', 'sapo_temperature_neg')
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, tokenizer=None, *, beta=None,
                  num_generations=None) -> None:
@@ -155,7 +161,7 @@ class GRPOTrainer:
             kw['return_clip_fraction'] = True
         old = None  # updates 2..mu: the first update's log-probs
         plains, entropies, entropy_means, fracs, shares = [], [], [], [], []
-        cov = objective is not None and objective.policy_loss_mode != 'vanilla'
+        cov = objective is not None and objective.policy_loss_mode in ops.COV_MODES
         for _ in range(mu):
             if old is not None:
                 kw['old_per_token_logps'] = old

@@ -164,7 +164,8 @@ def whiten_rollout(tr, training_batches, sequence_masks, starts, returns=None) -
 
 
 OBJECTIVE_KEYS = ('clip_range_ratio_low', 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode',
-                  'policy_loss_mode', 'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef')
+                  'policy_loss_mode', 'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef',
+                  'sapo_temperature_pos', 'sapo_temperature_neg')
 
 
 def actor_objective_of(tr) -> ops.ActorObjective | None:
@@ -195,7 +196,7 @@ def objective_kwargs(tr) -> dict:
     objective = actor_objective_of(tr)
     if objective is not None:
         kw['objective'] = objective
-        if objective.policy_loss_mode != 'vanilla':
+        if objective.policy_loss_mode in ops.COV_MODES:
             kw['cov_seed'] = cov_seed_of(tr, objective)
     if tr.log_clip_fraction:
         kw['return_clip_fraction'] = True
@@ -378,6 +379,12 @@ class PPOTrainer:
     clip_cov_ub = None
     kl_cov_ratio = None
     ppo_kl_coef = None
+    # CISPO / SAPO (TRL's loss_type 'cispo' / 'sapo', see ops.ActorObjective): policy_loss_mode 'cispo' truncates the
+    # importance weight at 1 + clip_range_ratio_high (None = clip_range_ratio) and stops its gradient; 'sapo' gates the
+    # ratio with a sigmoid of temperature sapo_temperature_pos (A > 0) or sapo_temperature_neg (None = 1.0 / 1.05).  Both
+    # keep K1f's single pass.  `cfgs.train_cfgs.<key>` overrides each when set.
+    sapo_temperature_pos = None
+    sapo_temperature_neg = None
     # Advantage whitening (TRL's / verl's masked_whiten): rollout() forms every micro-batch's advantages with the
     # kl_coeff in effect then (K4, and K4r for Multi-PPO's other estimators) and whitens them with ONE mean and std over
     # the whole rollout's actor-loss mask, on every data-parallel rank (ops.whiten_advantages); rl_step reuses them (all
@@ -388,7 +395,8 @@ class PPOTrainer:
     SWITCHES = ('mode', 'fused_lm_head', 'lm_head_chunk_rows', 'log_entropy', 'entropy_coeff', 'clip_range_ratio_low',
                 'clip_range_ratio_high', 'dual_clip_ratio', 'loss_agg_mode', 'log_clip_fraction', 'kl_estimator',
                 'kl_target', 'kl_horizon', 'kl_loss_coeff', 'kl_loss_estimator', 'whiten_advantages', 'policy_loss_mode',
-                'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef')
+                'clip_cov_ratio', 'clip_cov_lb', 'clip_cov_ub', 'kl_cov_ratio', 'ppo_kl_coef', 'sapo_temperature_pos',
+                'sapo_temperature_neg')
 
     def __init__(self, cfgs=None, actor_model=None, actor_reference_model=None, reward_model=None,
                  reward_critic_model=None, tokenizer=None, reward_tokenizer=None, *, kl_coeff=0.02,

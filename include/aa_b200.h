@@ -8,7 +8,7 @@
  * function(s) whose arithmetic it replaces (file:line relative to the reference's
  * align_anything/ directory); the Python mirror in align_anything_b200/ keeps the
  * reference's names and signatures and calls these through ctypes (INTEGRATION.md).
- * 78 entry points, ABI version 3.
+ * 82 entry points, ABI version 3.
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
@@ -817,6 +817,57 @@ int aa_grpo_loss_cov(const void *log_probs, int64_t lp_stride, const void *ref_l
                      float cov_coef, const uint8_t *sel, int64_t sel_stride, int mode, float *loss, void *grad,
                      int64_t grad_stride, float *clip_frac, int32_t *row_end, float *scratch, uint32_t *counter,
                      void *stream);
+
+/* CISPO and SAPO (TRL's GRPO loss_type 'cispo' / 'sapo'; ops.POLICY_LOSS_MODES), policy losses in place of the
+ * clipped ratio, with r = exp(lp - old) rounded as aa_ppo_actor_loss_obj rounds it and s the negated loss term that
+ * loss_agg aggregates:
+ *   AA_PM_CISPO  w = clamp(r, max = 1 + clip_high) with its gradient stopped;  s = w * A * lp;  d s / d lp = w * A.
+ *                The clip fractions count r > 1 + clip_high (the dual-clip lane is 0).
+ *   AA_PM_SAPO   tau = tau_pos where A > 0, else tau_neg;  s = sigmoid(tau * (r - 1)) * 4 / tau * A (fp32: the loss
+ *                and its aggregation are fp32 whatever the dtypes);  d s / d lp = 4 sigma (1 - sigma) r A.  The clip
+ *                fractions are 0.
+ * The modes are kept apart from AA_COV_*: the Cov entry points refuse these codes.  clip_high >= 0; tau_pos / tau_neg
+ * finite and > 0 (SAPO; CISPO ignores them).  There is no dual-clip and no lower bound.  Every other argument is as in
+ * aa_ppo_actor_loss_cov (ref_log_probs NULL: no KL loss term; row_scratch fp32 [5 * B]) and aa_grpo_loss_kl
+ * (old_log_probs NULL: ratio 1).  Arguments are checked before any launch. */
+enum { AA_PM_CISPO = 3, AA_PM_SAPO = 4 };
+int aa_ppo_actor_loss_pm(const void *log_probs, int64_t lp_stride, const void *old_log_probs, int64_t old_stride,
+                         int lp_dtype, const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
+                         int64_t mask_stride, int32_t B, int32_t Wm, float clip_high, int loss_agg, int pm_mode,
+                         float tau_pos, float tau_neg, int mode, const void *ref_log_probs, int64_t ref_stride,
+                         float kl_loss_coeff, int kl_estimator, float *loss, float *kl_loss, void *grad,
+                         int64_t grad_stride, float *clip_frac, float *row_scratch, uint32_t *counter, void *stream);
+int aa_grpo_loss_pm(const void *log_probs, int64_t lp_stride, const void *ref_log_probs, int64_t ref_stride,
+                    const void *old_log_probs, int64_t old_stride, int lp_dtype, const float *advantages,
+                    const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t B, int32_t K,
+                    float beta, float clip_high, int loss_agg, int kl_estimator, int pm_mode, float tau_pos,
+                    float tau_neg, int mode, float *loss, void *grad, int64_t grad_stride, float *clip_frac,
+                    int32_t *row_end, float *scratch, uint32_t *counter, void *stream);
+/* K1f's actor node (aa_logprob_actor_fused_kl) and GRPO node (aa_logprob_grpo_fused_kl) under CISPO / SAPO, as
+ * aa_ppo_actor_loss_pm / aa_grpo_loss_pm define them: the log-probs are bit-identical to the other K1f entry points',
+ * the gradient tile carries the mode's d loss / d log-prob.  ref_log_probs (actor) NULL: no KL loss term; entropy
+ * NULL: no entropy (entropy_coeff must then be 0); entropy_coeff != 0 adds the entropy bonus's gradient as the
+ * _obj entry points do.  row_scratch as aa_logprob_actor_fused_kl's / aa_logprob_grpo_fused_kl's. */
+int aa_logprob_actor_fused_pm(const void *logits, int logits_dtype, int64_t row_stride, int32_t V,
+                              const int64_t *labels, int32_t n_segments, const int64_t *seg_logit_off,
+                              const int64_t *seg_label_off, const int64_t *seg_out_off, const int64_t *seg_cum,
+                              const int64_t *seg_tile_row, int64_t n_tile_rows, void *log_probs, int lp_dtype,
+                              float *stat_max, float *stat_logsum, const void *old_log_probs, int64_t old_stride,
+                              const void *advantages, int64_t adv_stride, int adv_dtype, const uint8_t *mask,
+                              int64_t mask_stride, int32_t W, float clip_high, int loss_agg, int pm_mode,
+                              float tau_pos, float tau_neg, int mode, void *grad_logits, int64_t grad_row_stride,
+                              void *row_scratch, int32_t *status, float entropy_coeff, float *entropy,
+                              const void *ref_log_probs, float kl_loss_coeff, int kl_estimator, void *stream);
+int aa_logprob_grpo_fused_pm(const void *logits, int logits_dtype, int64_t row_stride, int32_t V, const int64_t *labels,
+                             int32_t n_segments, const int64_t *seg_logit_off, const int64_t *seg_label_off,
+                             const int64_t *seg_out_off, const int64_t *seg_cum, const int64_t *seg_tile_row,
+                             int64_t n_tile_rows, void *log_probs, int lp_dtype, const void *ref_log_probs,
+                             int64_t ref_stride, const void *old_log_probs, const float *advantages,
+                             const int64_t *completion_tokens, int64_t tok_stride, int64_t eos_id, int32_t K,
+                             float beta, float clip_high, int loss_agg, int kl_estimator, int pm_mode, float tau_pos,
+                             float tau_neg, int mode, void *grad_logits, int64_t grad_row_stride, void *row_scratch,
+                             int32_t *row_end, float *total, uint32_t *counter, int32_t *status, float *entropy,
+                             float entropy_coeff, void *stream);
 
 /* masked_mean (utils/tools.py:460-467): mean over rows of masked row means -> out[0];
  * mask == NULL: plain mean. */
