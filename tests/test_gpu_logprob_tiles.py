@@ -18,7 +18,11 @@ checks:
   * zero rows are exactly 0, rows outside a scored-only plan, pad columns and guards are bit for bit unchanged;
   * both kernels, and the host-layout route (memset spans + listed zero rows) and the tile route (the kernel zero-fills
     every unscored row), write byte-identical buffers, guards included;
-  * the forward writes every scored log-prob, 0 for ignored rows, and nothing else.
+  * the forward writes every scored log-prob, 0 for ignored rows, and nothing else;
+  * grad_entropy: K1b's entropy-gradient variant on the same case leaves the rows with g_H == 0 bit-identical to
+    aa_logprob_bwd's and puts the float64 tile formula with the entropy term in the others.  It runs once per case and
+    mode, through the case's first route: aa_logprob_bwd_entropy is always TMA-staged (the LDG row kernel has no
+    entropy variant), so there is no LDG run to compare.
 K1f (the single-pass nodes) is checked against K1 -> loss kernel -> K1b on the same inputs, both into guarded tiles.
 """
 import ctypes
@@ -263,8 +267,10 @@ class Case:
     def routes(self):
         return [True, False] if self.kind == 'host' else [None]  # _ZERO_SPANS: host layout, tile mode
 
-    def run(self, ops, mode_code, kernel, zero_spans, monkeypatch):
-        """One forward + backward into freshly poisoned buffers -> (tile guard object, out, stats, status word)."""
+    def run(self, ops, mode_code, kernel, zero_spans, monkeypatch, grad_entropy=None):
+        """One forward + backward into freshly poisoned buffers -> (tile guard object, out, stats, status word).
+        grad_entropy (fp32, laid out like the log-probs): K1b's entropy-gradient variant, fed the float64 entropy of
+        the scored rows rounded to fp32."""
         if zero_spans is not None:
             monkeypatch.setattr(ops, '_ZERO_SPANS', zero_spans)
         out_dtype = self.dtype if mode_code == Lb.MODE_FAITHFUL else torch.float32
@@ -274,10 +280,17 @@ class Case:
         ig = IGNORE if self.ignore else None
         _status_take()
         ops._launch_fwd(self.logits, self.labels, self.plan, out, stats[0], stats[1], ignore_index=ig)
+        ent = None
+        if grad_entropy is not None:
+            from test_gpu_entropy import entropy64
+
+            ent = torch.zeros(self.out_shape, dtype=torch.float32, device=DEV)
+            ent.view(-1)[self.out_idx.to(DEV)] = entropy64(self.logits[self.tile_row.to(DEV)]).float()
         _set_bwd_kernel(kernel)
         try:
             ops._launch_bwd(self.logits, self.labels, self.plan, stats[0], stats[1], self.grad_rows, self.grad_seg,
-                            self.grad_scale, tile.tile, mode_code, ignore_index=ig, grad_row_stride=self.gpitch)
+                            self.grad_scale, tile.tile, mode_code, ignore_index=ig, grad_row_stride=self.gpitch,
+                            entropy=ent, grad_entropy=grad_entropy)
         finally:
             _set_bwd_kernel(-1)
         torch.cuda.synchronize()
@@ -378,6 +391,45 @@ def test_backward_tile_contract(ops, case_args, monkeypatch):
             flagged = bool(case.plan_status & Lb.STATUS_SHORT_SEQUENCE)
             assert flagged == any(r < 0 for r in case.lens), 'a negative length is clamped to 0 and flagged'
         _check_against_reference(case, mode_code, tile0, out0, stats0, status0)
+        _check_entropy_gradient(ops, case, mode_code, runs[0][0][1], tile0, monkeypatch)
+
+
+def _check_entropy_gradient(ops, case, mode_code, route, plain, monkeypatch):
+    """The grad_entropy axis: aa_logprob_bwd_entropy (always TMA-staged) on the case's rows with g_H != 0 on most
+    scored rows, the g == 0 row included.  Rows with g_H == 0, the rows outside the plan, pad columns and guards are
+    bit-identical to aa_logprob_bwd's buffer; the others hold test_gpu_entropy_bonus._tile64's
+    g (onehot - p) - g_H p (l + H) (FAITHFUL: the rounded log-softmax) at its _close bar."""
+    from test_gpu_entropy_bonus import EPS, _tile64
+
+    k = case.tile_row.numel()
+    gh = torch.tensor([0.0, 0.5, -1.25, 0.0, 2.0, -0.375])[torch.arange(k) % 6]
+    gh[8] = 0.75  # g == 0: the row carries the entropy's gradient alone
+    gh[case.ignored | case.oob | case.nan_g] = 0.0
+    gh_rows = torch.zeros(case.out_shape, dtype=torch.float32)
+    gh_rows.view(-1)[case.out_idx] = gh
+    tile, out, stats, status = case.run(ops, mode_code, TMA, route, monkeypatch, grad_entropy=gh_rows.to(DEV))
+    what = f'{_case_id((case.dtype, case.V, case.kind, case.layout, "", case.ignore, case.B, case.S))} mode {mode_code}'
+    hot = torch.zeros(case.R, dtype=torch.bool)
+    hot[case.tile_row[gh != 0]] = True
+    keep = tile.outside()
+    assert torch.equal(tile.bits[keep], plain.bits[keep]), f'{what}: grad_entropy changed a guard or pad column'
+    cold = torch.nonzero(~hot).flatten().to(DEV)
+    assert torch.equal(tile.row_bits(cold), plain.row_bits(cold)), f'{what}: a row with g_H == 0 differs from K1b'
+    sel = gh != 0
+    rows = case.tile_row[sel].to(DEV)
+    x = case.logits[rows].float()
+    y = case.y[sel].to(DEV)
+    faithful = case.dtype if (mode_code == Lb.MODE_FAITHFUL and case.dtype != torch.float32) else None
+    g_h = gh[sel].to(DEV) * (-0.5 if case.grad_scale is not None else 1.0)  # grad_scale multiplies g_H too
+    g = case.g[sel].to(DEV)
+    want = _tile64(x, y, g, g_h, faithful)
+    # test_gpu_entropy_bonus._close's bar, its floor relative to the larger of the row's largest element, |g| and |g_H|
+    # (a one-column row has want == 0 and p rounded from an fp32 exp)
+    scale = torch.maximum(want.abs().amax(-1), torch.maximum(g.abs(), g_h.abs()).double())[:, None]
+    eps = EPS[case.dtype]
+    err = (tile.tile[rows].double() - want).abs()
+    bad = ~(err <= eps * want.abs() + max(eps, 2e-5) * scale)
+    assert not bool(bad.any()), f'{what} grad_entropy: {int(bad.sum())} elements beyond tolerance'
 
 
 def test_pitched_tile_host_layout_keeps_pad_columns(ops, monkeypatch):
