@@ -236,55 +236,99 @@ struct Welford {
   float mean, m2, nf;
 };
 __device__ __forceinline__ Welford welford_one(float x) { return {x, 0.f, 1.f}; }
+// WelfordOps::reduce (one element into a running state; {0, 0, 0} + x is exactly welford_one(x))
+__device__ __forceinline__ Welford welford_add(Welford a, float x) {
+  const float nf = __fadd_rn(a.nf, 1.f), d = __fsub_rn(x, a.mean), m = __fadd_rn(a.mean, __fdiv_rn(d, nf));
+  return {m, __fmaf_rn(d, __fsub_rn(x, m), a.m2), nf};
+}
+// WelfordOps::combine of two non-empty states
 __device__ __forceinline__ Welford welford_combine(Welford a, Welford b) {
   const float d = __fsub_rn(b.mean, a.mean), nn = __fadd_rn(a.nf, b.nf), r = __fdiv_rn(b.nf, nn);
   return {__fmaf_rn(d, r, a.mean), __fmaf_rn(__fmul_rn(__fmul_rn(d, d), a.nf), r, __fadd_rn(a.m2, b.m2)), nn};
 }
 
-// Group sum and unbiased std of the n flat elements from g0, in the order ATen's reduction combines them for a
-// contiguous inner dimension of n < 16: bw = largest power of two <= n lanes, lane j holds elements j and j + bw,
-// then a shuffle tree over the lanes.  Larger groups are folded sequentially (the same value up to fp32 rounding).
+// group_stats (below) for n >= 16
+__device__ __forceinline__ void group_stats_wide(const ReturnsParams &p, int64_t g0, bool want_std, float &sum,
+                                                 float &sd) {
+  const int n = p.n;
+  const int bw = n >= 32 ? 32 : 16;
+  float ls[5], s = 0.f;  // ls[l]: the open subtree of 2^l partials
+  Welford lw[5], w = {0.f, 0.f, 0.f};
+#pragma unroll 1
+  for (int j = 0; j < bw; ++j) {
+    float a[4] = {0.f, 0.f, 0.f, 0.f};
+    Welford acc[2] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+    for (int i = j; i < n; i += 4 * bw) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        if (i + q * bw < n) {
+          const float x = masked_reward(p, g0 + i + q * bw);
+          a[q] = __fadd_rn(a[q], x);
+          if (want_std) acc[q & 1] = welford_add(acc[q & 1], x);
+        }
+      }
+    }
+    s = __fadd_rn(__fadd_rn(__fadd_rn(a[0], a[1]), a[2]), a[3]);
+    if (want_std) w = acc[1].nf == 0.f ? acc[0] : welford_combine(acc[0], acc[1]);
+    bool open = true;
+#pragma unroll
+    for (int l = 0; l < 5; ++l) {
+      if (open && ((j >> l) & 1)) {
+        s = __fadd_rn(ls[l], s);
+        if (want_std) w = welford_combine(lw[l], w);
+      } else if (open) {
+        ls[l] = s;
+        lw[l] = w;
+        open = false;
+      }
+    }
+  }
+  sum = s;  // after partial bw - 1 (s, w): the whole tree
+  sd = want_std ? __fsqrt_rn(__fdiv_rn(w.m2, static_cast<float>(n - 1))) : 0.f;
+}
+
+// Group sum and unbiased std of the n flat elements from g0, in the block-x layout Reduce.cuh describes for a
+// contiguous inner dimension of n < 128 with at least 16 groups (larger n vectorises the loads, fewer groups widen
+// the block past a warp): bw = min(largest power of two <= n, 32) threads; thread j folds elements j + k * bw, in k
+// order, into accumulator k % 4 (the sum: vt0 = 4, from 0) or k % 2 (Welford: vt0 = 2), then combines its
+// accumulators in index order; then a shuffle-down tree over the bw threads, lower index on the left.  The tree is
+// evaluated here as a left-to-right pairwise fold over the threads' partials: partial j closes every subtree whose last
+// leaf it is (one per trailing 1 bit of j), so ls / lw hold at most one open subtree per level.
+// This is the layout as read, not confirmed at the bit level: on an H100 with torch 2.11, ATen's fp32 group sums equal
+// it for n <= 3 only (for n = 4..8 they equal a 2-thread, 2-accumulator fold instead, and for n >= 12 no layout
+// tried), so fp32 results match eager ATen on 75-90 % of the elements; 16-bit rounding hides the order (DESIGN
+// section 4, "Multi-PPO (K4r)").  tests/test_gpu_returns_pin.py holds this order bit for bit against a float32
+// restatement of it.
 __device__ __forceinline__ void group_stats(const ReturnsParams &p, int64_t g0, bool want_std, float &sum, float &sd) {
   const int n = p.n;
-  if (n >= 16) {
-    Welford w = welford_one(masked_reward(p, g0));
-    sum = w.mean;
-    for (int k = 1; k < n; ++k) {
-      const float v = masked_reward(p, g0 + k);
-      sum = __fadd_rn(sum, v);
-      if (want_std) {
-        const float nf = __fadd_rn(w.nf, 1.f), d = __fsub_rn(v, w.mean);
-        const float m = __fadd_rn(w.mean, __fdiv_rn(d, nf));
-        w = {m, __fmaf_rn(d, __fsub_rn(v, m), w.m2), nf};
+  if (n < 16) {  // the same layout unrolled: bw <= 8 threads of at most two elements, a three-level tree
+    const int bw = n >= 8 ? 8 : n >= 4 ? 4 : 2;
+    float s[8];
+    Welford w[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if (j < bw) {
+        const float a = masked_reward(p, g0 + j);
+        const float b = (j + bw < n) ? masked_reward(p, g0 + j + bw) : 0.f;
+        s[j] = (j + bw < n) ? __fadd_rn(a, b) : a;
+        w[j] = (j + bw < n) ? welford_combine(welford_one(a), welford_one(b)) : welford_one(a);
       }
     }
-    sd = __fsqrt_rn(__fdiv_rn(w.m2, static_cast<float>(n - 1)));
+#pragma unroll
+    for (int off = 1; off < 8; off <<= 1) {
+#pragma unroll
+      for (int j = 0; j + off < 8; j += 2 * off) {
+        if (j + off < bw) {
+          s[j] = __fadd_rn(s[j], s[j + off]);
+          if (want_std) w[j] = welford_combine(w[j], w[j + off]);
+        }
+      }
+    }
+    sum = s[0];
+    sd = want_std ? __fsqrt_rn(__fdiv_rn(w[0].m2, static_cast<float>(n - 1))) : 0.f;
     return;
   }
-  const int bw = n >= 8 ? 8 : n >= 4 ? 4 : n >= 2 ? 2 : 1;
-  float s[8];
-  Welford w[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    if (j < bw) {
-      const float a = masked_reward(p, g0 + j);
-      const float b = (j + bw < n) ? masked_reward(p, g0 + j + bw) : 0.f;
-      s[j] = (j + bw < n) ? __fadd_rn(a, b) : a;
-      w[j] = (j + bw < n) ? welford_combine(welford_one(a), welford_one(b)) : welford_one(a);
-    }
-  }
-#pragma unroll
-  for (int off = 1; off < 8; off <<= 1) {
-#pragma unroll
-    for (int j = 0; j + off < 8; j += 2 * off) {
-      if (j + off < bw) {
-        s[j] = __fadd_rn(s[j], s[j + off]);
-        if (want_std) w[j] = welford_combine(w[j], w[j + off]);
-      }
-    }
-  }
-  sum = s[0];
-  sd = want_std ? __fsqrt_rn(__fdiv_rn(w[0].m2, static_cast<float>(n - 1))) : 0.f;
+  group_stats_wide(p, g0, want_std, sum, sd);
 }
 
 // the estimator's value at flat index f, with the rounding points of the eager ops (r = rounding code):

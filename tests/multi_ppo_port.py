@@ -33,8 +33,9 @@ def cumulative_returns(rewards, mask, start: int, gamma: float):
 
 
 def advantages_and_returns(values, rewards, sequence_mask, start: int, estimator: str, n: int, gamma: float,
-                           gae_lambda: float = 0.95):
-    """multi_ppo.py:510-570."""
+                           gae_lambda: float = 0.95, mask_outputs: bool = True):
+    """multi_ppo.py:510-570.  mask_outputs=False leaves out the final `*= sequence_mask` (`cumulative_returns` on its
+    own, as `ops.estimator_returns(..., mask_outputs=False)` computes it)."""
     values = values * sequence_mask
     rewards = rewards * sequence_mask
     if estimator == 'gae':
@@ -60,12 +61,13 @@ def advantages_and_returns(values, rewards, sequence_mask, start: int, estimator
         advantages = returns.clone()
     else:
         raise ValueError(f'Unknown estimator: {estimator}')
-    advantages *= sequence_mask[:, start:]
-    returns *= sequence_mask[:, start:]
+    if mask_outputs:
+        advantages *= sequence_mask[:, start:]
+        returns *= sequence_mask[:, start:]
     return advantages, returns
 
 
-def returns_f64(rewards, mask, start: int, estimator: str, n: int, gamma: float) -> np.ndarray:
+def returns_f64(rewards, mask, start: int, estimator: str, n: int, gamma: float, mask_outputs: bool = True) -> np.ndarray:
     """The four non-GAE estimators in float64, group by group over the flat (B, W) index."""
     r = rewards.detach().double().cpu().numpy() * mask.cpu().numpy()
     B, W = r.shape
@@ -88,7 +90,7 @@ def returns_f64(rewards, mask, start: int, estimator: str, n: int, gamma: float)
         for t in range(W - 1, start - 1, -1):
             c = x[b, t] + gamma * c
             out[b, t - start] = c
-    return out * mask.cpu().numpy()[:, start:]
+    return out * mask.cpu().numpy()[:, start:] if mask_outputs else out
 
 
 def rl_step(rollout, new_actor_logits, new_critic_scores, input_ids, attention_mask, start: int, estimator: str,
