@@ -915,7 +915,10 @@ int aa_linear_logprob_fwd(const void *hidden, int64_t n_rows, int32_t H, int64_t
  * (bf16-rounded in FAITHFUL mode, the fp32 accumulators in F32 mode), never rounded.  The (max, sum-exp, entropy sum)
  * merge across the quad and across vocabulary splits uses t' = alpha (t + (m - m') s); `partial` then holds FOUR floats
  * per (row, split): 4 * 132 * 128 always suffices on a 132-SM H100 (with fewer floats the split count is lowered as for
- * K6).  out, stat_max and stat_logsum are bit-identical to aa_linear_logprob_fwd. */
+ * K6).  out, stat_max and stat_logsum are bit-identical to aa_linear_logprob_fwd's when both launches split the
+ * vocabulary the same way: `partial` NULL, or partial_floats >= 4 * n_rows * splits for the split count `splits` that
+ * aa_linear_logprob_fwd picks.  A buffer sized at 3 floats per split for the plain launch can make this launch split
+ * fewer ways; the statistics are then merged in another order and may differ in the last bits. */
 int aa_linear_logprob_fwd_entropy(const void *hidden, int64_t n_rows, int32_t H, int64_t hidden_row_stride,
                                   const void *weight, int32_t V, int64_t weight_row_stride, const int64_t *labels,
                                   void *out, int out_dtype, float *stat_max, float *stat_logsum, float *partial,

@@ -159,9 +159,11 @@ def _headroom(what, err, tol):
     print(f'HEADROOM {what}: max err {err:.3e}, bar {tol:.3e}')
 
 
-def schedule(n, V, may_split, partial_floats):
-    """The host schedule of linear_logprob.cu restated: -> (splits, tiles per split, row units per group)."""
-    S = torch.cuda.get_device_properties(0).multi_processor_count
+def schedule(n, V, may_split, partial_floats, per_split=3, sms=None):
+    """The host schedule of linear_logprob.cu restated: -> (splits, tiles per split, row units per group).
+    per_split: floats of `partial` per (row, split) -- 3 for K6, 4 for its entropy variant; sms: the SM count (default:
+    the device's)."""
+    S = sms or torch.cuda.get_device_properties(0).multi_processor_count
     units = -(-n // BM)
     all_tiles = -(-V // BN)
     splits, group = 1, units
@@ -178,7 +180,7 @@ def schedule(n, V, may_split, partial_floats):
                     best, best_cost = s, cost
             splits, group = best, S // best
         splits = max(1, min(splits, all_tiles))
-        while partial_floats >= 0 and splits > 1 and n * splits * 3 > partial_floats:
+        while partial_floats >= 0 and splits > 1 and n * splits * per_split > partial_floats:
             splits -= 1
         group = max(1, min(group, units))
     tps = -(-all_tiles // splits)
