@@ -67,6 +67,8 @@ _SIGS = {
                             _P, _P, _P, _P, POINTER(AaColl), _P, _P, _P]),
     'aa_dpo_loss_obj': (c_int, [_P, _P, c_int, c_int32, c_int32, c_int64, c_float, c_int, c_int, c_float, c_float, _P,
                                 _P, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),
+    'aa_dpo_loss_ext': (c_int, [_P, _P, c_int, c_int32, c_int32, c_int64, c_float, c_int, c_int, c_float, c_float, c_int,
+                                c_float, c_float, c_float, c_float, _P, _P, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),
     'aa_pair_slices': (c_int, [_P, c_int64, _P, c_int, c_int64, c_int32, c_int32, _P, _P, _P]),
     'aa_slice_sums': (c_int, [_P, c_int, c_int64, c_int32, c_int32, _P, c_int, _P, _P]),
     'aa_rm_pair_loss': (c_int, [_P, c_int32, c_float, _P, _P, _P]),

@@ -240,10 +240,192 @@ __device__ __forceinline__ float2 dpo_obj_backward(int type, float gl, float s0,
   }
 }
 
+// ---- K2 extended objective: f-divergences, EXO, DiscoPOP and AOT (DESIGN section 4.13) -----------------------------
+// Each restates tests/dpo_ext_port.py op for op, with the conventions of the objective variant above.  The
+// per-pair thread keeps (a, b) in grad_seg and the last block re-runs the pair's forward next to its backward; AOT
+// keeps its two sort keys there instead and is sorted, and its loss formed, by the last block.
+struct DpoExtParams : DpoObjParams {
+  int fdiv;       // AA_DPO_FDIV_*
+  float f_alpha;  // alpha-divergence coefficient
+  float tau;      // DiscoPOP temperature
+  float exp_cap;  // cap_exp's clamp, floor(log(finfo(log-prob dtype).max) * 1e4) / 1e4
+  float exo_c1, exo_c2;  // EXO's log(1 - e') and log(e'), formed by the caller in double and rounded to fp32 once
+};
+
+// ATen softplus (beta 1, threshold 20) and its backward g * z / (z + 1), z = exp(x), each in fp32 and rounded once
+__device__ __forceinline__ float softplus_f(float x) { return x > 20.f ? x : log1pf(expf(x)); }
+__device__ __forceinline__ float dsoftplus(float g, float x, int rd) {
+  const float z = expf(x);
+  return round_to(x > 20.f ? g : __fdiv_rn(__fmul_rn(g, z), z + 1.f), rd);
+}
+
+// exp(clamp(x, max = cap)): clamp passes NaN through and rounds its fp32 result
+__device__ __forceinline__ float cap_exp(float x, float cap, int rd) {
+  return round_to(expf(round_to(x != x ? x : fminf(x, cap), rd)), rd);
+}
+
+// h from a and b under the f-divergence
+__device__ __forceinline__ float fdiv_forward(const DpoExtParams &p, float a, float b, int rd) {
+  if (p.fdiv == AA_DPO_FDIV_ALPHA) {
+    const float eb = cap_exp(round_to(__fmul_rn(b, -p.f_alpha), rd), p.exp_cap, rd);
+    const float ea = cap_exp(round_to(__fmul_rn(a, -p.f_alpha), rd), p.exp_cap, rd);
+    return round_to(__fmul_rn(round_to(eb - ea, rd), 1.f / p.f_alpha), rd);
+  }
+  const float h = round_to(a - b, rd);
+  if (p.fdiv == AA_DPO_FDIV_JS) return round_to(h - round_to(round_to(softplus_f(a), rd) - round_to(softplus_f(b), rd), rd), rd);
+  return h;
+}
+
+// (d / d a, d / d b) from d / d h.  Alpha: ExpBackward (grad * result), then no gradient where the clamp is active.
+__device__ __forceinline__ float2 fdiv_backward(const DpoExtParams &p, float gh, float a, float b, int rd) {
+  if (p.fdiv == AA_DPO_FDIV_ALPHA) {
+    const float gd = round_to(__fmul_rn(gh, 1.f / p.f_alpha), rd);
+    const float ta = round_to(__fmul_rn(a, -p.f_alpha), rd), tb = round_to(__fmul_rn(b, -p.f_alpha), rd);
+    const float gta = ta <= p.exp_cap ? round_to(__fmul_rn(-gd, cap_exp(ta, p.exp_cap, rd)), rd) : 0.f;
+    const float gtb = tb <= p.exp_cap ? round_to(__fmul_rn(gd, cap_exp(tb, p.exp_cap, rd)), rd) : 0.f;
+    return make_float2(round_to(__fmul_rn(gta, -p.f_alpha), rd), round_to(__fmul_rn(gtb, -p.f_alpha), rd));
+  }
+  if (p.fdiv == AA_DPO_FDIV_JS)  // h = a - b and softplus(a) both reach a: two terms, added once
+    return make_float2(round_to(gh + dsoftplus(-gh, a, rd), rd), round_to(-gh + dsoftplus(gh, b, rd), rd));
+  return make_float2(gh, -gh);
+}
+
+// EXO (pair form) and DiscoPOP of h: (loss, d (gl * loss) / d h).  z reaches the loss along three paths; autograd adds
+// their gradients in the order its engine runs them (the latest-created node first), so the sums below follow it.
+__device__ __forceinline__ float2 exo_discopop(const DpoExtParams &p, float h, float gl, int rd) {
+  const float z = round_to(__fmul_rn(p.beta, h), rd);
+  if (p.loss_type == AA_DPO_EXO_PAIR) {
+    const float c1 = p.exo_c1, c2 = p.exo_c2;
+    const float s1 = round_to(sigmoid_f(z), rd), t1 = round_to(round_to(log_sigmoid(z), rd) - c1, rd);
+    const float s2 = round_to(sigmoid_f(-z), rd), t2 = round_to(round_to(log_sigmoid(-z), rd) - c2, rd);
+    const float loss = round_to(round_to(__fmul_rn(s1, t1), rd) + round_to(__fmul_rn(s2, t2), rd), rd);
+    const float g_nz = round_to(round_to(__fmul_rn(round_to(__fmul_rn(gl, s2), rd), dlog_sigmoid(-z)), rd) +
+                                    dsigmoid(round_to(__fmul_rn(gl, t2), rd), s2, rd), rd);
+    const float g_l1 = round_to(__fmul_rn(round_to(__fmul_rn(gl, s1), rd), dlog_sigmoid(z)), rd);
+    const float gz = round_to(round_to(-g_nz + g_l1, rd) + dsigmoid(round_to(__fmul_rn(gl, t1), rd), s1, rd), rd);
+    return make_float2(loss, round_to(__fmul_rn(gz, p.beta), rd));
+  }
+  // AA_DPO_DISCOPOP: m = sigmoid(z / tau), loss = -logsigmoid(z) * (1 - m) + exp(-z) * m
+  const float inv_tau = 1.f / p.tau;
+  const float m = round_to(sigmoid_f(round_to(__fmul_rn(z, inv_tau), rd)), rd);
+  const float lc = -round_to(log_sigmoid(z), rd), ec = round_to(expf(-z), rd), om = round_to(1.f - m, rd);
+  const float loss = round_to(round_to(__fmul_rn(lc, om), rd) + round_to(__fmul_rn(ec, m), rd), rd);
+  const float gm = round_to(round_to(__fmul_rn(gl, ec), rd) - round_to(__fmul_rn(gl, lc), rd), rd);
+  const float g_e = -round_to(__fmul_rn(round_to(__fmul_rn(gl, m), rd), ec), rd);
+  const float g_l = round_to(__fmul_rn(-round_to(__fmul_rn(gl, om), rd), dlog_sigmoid(z)), rd);
+  const float g_t = round_to(__fmul_rn(dsigmoid(gm, m, rd), inv_tau), rd);
+  const float gz = round_to(round_to(g_e + g_l, rd) + g_t, rd);
+  return make_float2(loss, round_to(__fmul_rn(gz, p.beta), rd));
+}
+
+__device__ __forceinline__ bool dpo_aot(int type) { return type == AA_DPO_AOT || type == AA_DPO_AOT_PAIR; }
+// the types and f-divergences aa_dpo_loss_obj already has: the same arithmetic, the same stored operands
+__device__ __forceinline__ bool dpo_obj_arith(const DpoExtParams &p) {
+  return p.loss_type <= AA_DPO_APO_DOWN && p.fdiv == AA_DPO_FDIV_REVERSE_KL;
+}
+
+// A pair of a non-AOT new type or f-divergence: (loss, d (gl * loss) / d a, d (gl * loss) / d b)
+__device__ __forceinline__ float3 dpo_ext_pair(const DpoExtParams &p, float a, float b, float gl, int rd) {
+  const float h = fdiv_forward(p, a, b, rd);
+  float2 r;
+  if (p.loss_type == AA_DPO_EXO_PAIR || p.loss_type == AA_DPO_DISCOPOP) {
+    r = exo_discopop(p, h, gl, rd);
+  } else {  // SIGMOID / ROBUST / HINGE of the f-divergence's h: a = h, b = 0 makes their h - 0 = h exactly
+    const DpoPairFwd f = dpo_obj_forward(p.loss_type, h, 0.f, p.beta, p.eps, rd);
+    r = make_float2(f.loss, dpo_obj_backward(p.loss_type, gl, f.s0, f.s1, p.beta, p.eps, 0.f, 0.f, rd).x);
+  }
+  const float2 g = fdiv_backward(p, r.y, a, b, rd);
+  return make_float3(r.x, g.x, g.y);
+}
+
+// The per-pair thread: the loss and the two operands the last block reads back (AOT: its sort keys, loss 0 for now)
+__device__ __forceinline__ DpoPairFwd dpo_ext_forward(const DpoExtParams &p, float a, float b, float pc, float pr,
+                                                      float rc, float rr, int rd) {
+  if (p.loss_type == AA_DPO_AOT) return DpoPairFwd{0.f, round_to(pc - pr, rd), round_to(rc - rr, rd)};
+  if (p.loss_type == AA_DPO_AOT_PAIR) return DpoPairFwd{0.f, a, b};
+  if (dpo_obj_arith(p)) return dpo_obj_forward(p.loss_type, a, b, p.beta, p.eps, rd);
+  return DpoPairFwd{dpo_ext_pair(p, a, b, 0.f, rd).x, a, b};
+}
+
+// AOT in the last block: a stable rank sort of the kept pairs' two keys (torch.sort(stable=True): NaN last, ties to the
+// smaller pair index), exact and deterministic; then delta_k = key1_(k) - key2_(k) and the sigmoid loss of each
+// position k.  per_pair[0][i] becomes the loss at the position of pair i's first key.
+struct DpoAotSmem {
+  float key1[AA_DPO_AOT_MAX_PAIRS], key2[AA_DPO_AOT_MAX_PAIRS];
+  float pos[AA_DPO_AOT_MAX_PAIRS];  // the sorted second keys, then z = beta * delta_k at each position k
+  int rank1[AA_DPO_AOT_MAX_PAIRS], rank2[AA_DPO_AOT_MAX_PAIRS];  // -1: a skipped pair
+  unsigned char keep[AA_DPO_AOT_MAX_PAIRS];
+};
+__device__ __forceinline__ DpoAotSmem &dpo_aot_smem() {
+  __shared__ DpoAotSmem s;
+  return s;
+}
+
+__device__ __forceinline__ bool sorts_before(float xj, int j, float xi, int i) {
+  if (xi != xi) return xj == xj || j < i;
+  if (xj != xj) return false;
+  return xj < xi || (xj == xi && j < i);
+}
+
+template <int THREADS>
+__device__ void dpo_aot_sort(const DpoExtParams &p) {
+  DpoAotSmem &s = dpo_aot_smem();
+  const int B = p.n_pairs, rd = p.round_dt, tid = threadIdx.x;
+  const volatile float *v_key = p.grad_seg, *v_valid = p.per_pair + 4 * B;
+  for (int k = tid; k < B; k += THREADS) {
+    s.key1[k] = v_key[k];
+    s.key2[k] = v_key[B + k];
+    s.keep[k] = v_valid[k] != 0.f;
+  }
+  __syncthreads();
+  for (int i = tid; i < B; i += THREADS) {
+    int r1 = -1, r2 = -1;
+    if (s.keep[i]) {
+      r1 = r2 = 0;
+      const float x1 = s.key1[i], x2 = s.key2[i];
+      for (int j = 0; j < B; ++j) {
+        if (s.keep[j]) {
+          r1 += sorts_before(s.key1[j], j, x1, i);
+          r2 += sorts_before(s.key2[j], j, x2, i);
+        }
+      }
+    }
+    s.rank1[i] = r1;
+    s.rank2[i] = r2;
+  }
+  __syncthreads();
+  for (int i = tid; i < B; i += THREADS)
+    if (s.rank2[i] >= 0) s.pos[s.rank2[i]] = s.key2[i];
+  __syncthreads();
+  for (int i = tid; i < B; i += THREADS) {
+    const int k = s.rank1[i];
+    if (k >= 0) {  // position k is read and rewritten by this thread alone (the ranks are a permutation)
+      const DpoPairFwd f = dpo_obj_forward(AA_DPO_SIGMOID, round_to(s.key1[i] - s.pos[k], rd), 0.f, p.beta, p.eps, rd);
+      p.per_pair[i] = f.loss;
+      s.pos[k] = f.s0;
+    }
+  }
+  __syncthreads();
+}
+
+// (d / d chosen sum, d / d rejected sum) of a kept pair k of the extended variant; s0, s1: what its forward stored
+__device__ __forceinline__ float2 dpo_ext_backward(const DpoExtParams &p, int k, float gl, float s0, float s1,
+                                                   float inv_nc, float inv_nr, int rd) {
+  if (dpo_aot(p.loss_type)) {  // SortBackward: each key takes the gradient of the position it landed in
+    const DpoAotSmem &s = dpo_aot_smem();
+    const float g1 = dpo_obj_backward(AA_DPO_SIGMOID, gl, s.pos[s.rank1[k]], 0.f, p.beta, p.eps, 0.f, 0.f, rd).x;
+    if (p.loss_type == AA_DPO_AOT) return make_float2(g1, -g1);  // key1 = pc - pr
+    return make_float2(g1, -dpo_obj_backward(AA_DPO_SIGMOID, gl, s.pos[s.rank2[k]], 0.f, p.beta, p.eps, 0.f, 0.f, rd).x);
+  }
+  if (dpo_obj_arith(p)) return dpo_obj_backward(p.loss_type, gl, s0, s1, p.beta, p.eps, inv_nc, inv_nr, rd);
+  const float3 r = dpo_ext_pair(p, s0, s1, gl, rd);
+  return make_float2(r.y, r.z);
+}
+
 // The last block of the objective variant, after the metric means: the RPO NLL term (alpha > 0), then the seeds.
 // per_pair[3] holds each pair's chosen sum and grad_seg the forward's (s0, s1) until they are replaced here.
-template <int THREADS>
-__device__ __forceinline__ void dpo_obj_finish(const DpoObjParams &p, float sum_loss_over_n, float inv_n, float *scratch) {
+template <int THREADS, class Params>
+__device__ __forceinline__ void dpo_obj_finish(const Params &p, float sum_loss_over_n, float inv_n, float *scratch) {
   const int B = p.n_pairs, rd = p.round_dt, tid = threadIdx.x;
   volatile float *v_g = p.per_pair + 3 * B, *v_seg = p.grad_seg;
   const volatile float *v_valid = p.per_pair + 4 * B;
@@ -271,9 +453,14 @@ __device__ __forceinline__ void dpo_obj_finish(const DpoObjParams &p, float sum_
     float gc = 0.f, gr = -0.f;  // a skipped pair: the seeds aa_dpo_loss writes (+0, -0)
     if (v_valid[k] != 0.f) {
       const bool ipo = p.loss_type == AA_DPO_IPO;
-      const float2 g = dpo_obj_backward(p.loss_type, gl, v_seg[k], v_seg[B + k], p.beta, p.eps,
-                                        ipo ? 1.f / static_cast<float>(p.counts[k]) : 0.f,
-                                        ipo ? 1.f / static_cast<float>(p.counts[B + k]) : 0.f, rd);
+      float2 g;
+      if constexpr (std::is_same<Params, DpoExtParams>::value)
+        g = dpo_ext_backward(p, k, gl, v_seg[k], v_seg[B + k], ipo ? 1.f / static_cast<float>(p.counts[k]) : 0.f,
+                             ipo ? 1.f / static_cast<float>(p.counts[B + k]) : 0.f, rd);
+      else
+        g = dpo_obj_backward(p.loss_type, gl, v_seg[k], v_seg[B + k], p.beta, p.eps,
+                             ipo ? 1.f / static_cast<float>(p.counts[k]) : 0.f,
+                             ipo ? 1.f / static_cast<float>(p.counts[B + k]) : 0.f, rd);
       gc = p.alpha > 0.f ? round_to(g.x + g_nll, rd) : g.x;
       gr = g.y;
     }
@@ -285,7 +472,8 @@ __device__ __forceinline__ void dpo_obj_finish(const DpoObjParams &p, float sum_
 
 template <int THREADS, class Params>
 __global__ void __launch_bounds__(THREADS) dpo_loss_kernel(const Params p) {
-  constexpr bool OBJ = std::is_same<Params, DpoObjParams>::value;
+  constexpr bool OBJ = std::is_base_of<DpoObjParams, Params>::value;
+  constexpr bool EXT = std::is_same<Params, DpoExtParams>::value;
   __shared__ float scratch[33];
   __shared__ int same_flag;
   const int i = blockIdx.x, tid = threadIdx.x;
@@ -325,7 +513,11 @@ __global__ void __launch_bounds__(THREADS) dpo_loss_kernel(const Params p) {
         a = round_to(round_to(__fmul_rn(pc, inv_c), rd) - round_to(__fmul_rn(rc, inv_c), rd), rd);
         b = round_to(round_to(__fmul_rn(pr, inv_r), rd) - round_to(__fmul_rn(rr, inv_r), rd), rd);
       }
-      const DpoPairFwd f = dpo_obj_forward(p.loss_type, a, b, p.beta, p.eps, rd);
+      DpoPairFwd f;
+      if constexpr (EXT)
+        f = dpo_ext_forward(p, a, b, pc, pr, rc, rr, rd);
+      else
+        f = dpo_obj_forward(p.loss_type, a, b, p.beta, p.eps, rd);
       loss_i[i] = f.loss;
       better_i[i] = round_to(p.beta * ratio_c, rd);  // the metrics keep the summed ratios for every loss type
       worse_i[i] = round_to(p.beta * ratio_r, rd);
@@ -343,6 +535,9 @@ __global__ void __launch_bounds__(THREADS) dpo_loss_kernel(const Params p) {
   }
 
   if (!last_block_arrives(p.counter, gridDim.x)) return;
+  if constexpr (EXT) {
+    if (dpo_aot(p.loss_type)) dpo_aot_sort<THREADS>(p);
+  }
 
   // ---- final reduction over pairs (fixed order -> deterministic) ----
   // other blocks' results: read through volatile so no stale L1 line can be used
@@ -381,7 +576,7 @@ __global__ void __launch_bounds__(THREADS) dpo_loss_kernel(const Params p) {
     p.stats[7] = p.status ? static_cast<float>(*reinterpret_cast<const volatile int32_t *>(p.status)) : 0.f;
   }
   if constexpr (OBJ) {
-    dpo_obj_finish<THREADS>(p, s_loss * inv_n, inv_n, scratch);
+    dpo_obj_finish<THREADS, Params>(p, s_loss * inv_n, inv_n, scratch);
     return;
   }
   if (p.coll.world > 1 && p.stats_global) {
@@ -695,4 +890,61 @@ extern "C" int aa_dpo_loss_obj(const void *policy_lp, const void *ref_lp, int lp
                  loss_type, label_smoothing, rpo_alpha, counts};
   dpo_loss_kernel<128, DpoObjParams><<<n_pairs, 128, 0, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("aa_dpo_loss_obj");
+}
+
+extern "C" int aa_dpo_loss_ext(const void *policy_lp, const void *ref_lp, int lp_dtype, int32_t n_pairs,
+                               int32_t width, int64_t lp_row_stride, float scale_coeff, int mode, int loss_type,
+                               float label_smoothing, float rpo_alpha, int f_divergence, float f_alpha_coef,
+                               float discopop_tau, float exo_log_keep, float exo_log_smooth, const int32_t *counts, const int64_t *input_ids, int32_t L,
+                               int64_t ids_row_stride, float *per_pair, float *grad_seg, float *stats,
+                               uint32_t *counter, const int32_t *status, void *stream) {
+  AA_REQUIRE(n_pairs > 0 && width >= 0, AA_ERR_ARG, "aa_dpo_loss_ext: bad sizes");
+  AA_REQUIRE(policy_lp && per_pair && grad_seg && stats && counter, AA_ERR_ARG, "aa_dpo_loss_ext: null pointer");
+  AA_REQUIRE(lp_dtype == AA_BF16 || lp_dtype == AA_F16 || lp_dtype == AA_F32, AA_ERR_DTYPE,
+             "aa_dpo_loss_ext: bad dtype %d", lp_dtype);
+  AA_REQUIRE(mode == AA_MODE_FAITHFUL || mode == AA_MODE_F32, AA_ERR_ARG, "aa_dpo_loss_ext: bad mode %d", mode);
+  AA_REQUIRE(loss_type >= AA_DPO_SIGMOID && loss_type <= AA_DPO_AOT_PAIR, AA_ERR_ARG,
+             "aa_dpo_loss_ext: bad objective: loss_type %d", loss_type);
+  AA_REQUIRE(f_divergence >= AA_DPO_FDIV_REVERSE_KL && f_divergence <= AA_DPO_FDIV_ALPHA, AA_ERR_ARG,
+             "aa_dpo_loss_ext: bad objective: f_divergence %d", f_divergence);
+  const bool smoothable = loss_type == AA_DPO_SIGMOID || loss_type == AA_DPO_ROBUST || loss_type == AA_DPO_EXO_PAIR ||
+                          loss_type == AA_DPO_AOT || loss_type == AA_DPO_AOT_PAIR;
+  AA_REQUIRE(label_smoothing >= 0.f && label_smoothing < 0.5f && (smoothable || label_smoothing == 0.f), AA_ERR_ARG,
+             "aa_dpo_loss_ext: bad objective: label_smoothing %g with loss_type %d", label_smoothing, loss_type);
+  AA_REQUIRE(rpo_alpha >= 0.f && isfinite(rpo_alpha), AA_ERR_ARG, "aa_dpo_loss_ext: bad objective: rpo_alpha %g",
+             rpo_alpha);
+  AA_REQUIRE((loss_type != AA_DPO_IPO && loss_type != AA_DPO_SPPO_HARD) || (scale_coeff > 0.f && isfinite(scale_coeff)),
+             AA_ERR_ARG, "aa_dpo_loss_ext: bad objective: loss_type %d needs scale_coeff > 0, got %g", loss_type,
+             scale_coeff);
+  const bool reads_h = loss_type == AA_DPO_SIGMOID || loss_type == AA_DPO_ROBUST || loss_type == AA_DPO_HINGE ||
+                       loss_type == AA_DPO_EXO_PAIR;
+  AA_REQUIRE(f_divergence == AA_DPO_FDIV_REVERSE_KL || reads_h, AA_ERR_ARG,
+             "aa_dpo_loss_ext: bad objective: f_divergence %d with loss_type %d", f_divergence, loss_type);
+  AA_REQUIRE(f_alpha_coef > 0.f && isfinite(f_alpha_coef) && (f_alpha_coef == 1.f || f_divergence == AA_DPO_FDIV_ALPHA),
+             AA_ERR_ARG, "aa_dpo_loss_ext: bad objective: f_alpha_coef %g with f_divergence %d", f_alpha_coef,
+             f_divergence);
+  AA_REQUIRE(discopop_tau > 0.f && isfinite(discopop_tau) && (discopop_tau == 0.05f || loss_type == AA_DPO_DISCOPOP),
+             AA_ERR_ARG, "aa_dpo_loss_ext: bad objective: discopop_tau %g with loss_type %d", discopop_tau, loss_type);
+  AA_REQUIRE(loss_type != AA_DPO_EXO_PAIR || (exo_log_keep < 0.f && exo_log_smooth < 0.f && isfinite(exo_log_smooth)),
+             AA_ERR_ARG, "aa_dpo_loss_ext: bad objective: EXO's log(1 - e') %g and log(e') %g", exo_log_keep,
+             exo_log_smooth);
+  AA_REQUIRE((loss_type != AA_DPO_AOT && loss_type != AA_DPO_AOT_PAIR) || n_pairs <= AA_DPO_AOT_MAX_PAIRS, AA_ERR_ARG,
+             "aa_dpo_loss_ext: AOT sorts at most %d pairs, got %d", AA_DPO_AOT_MAX_PAIRS, n_pairs);
+  AA_REQUIRE(counts || (loss_type != AA_DPO_IPO && rpo_alpha == 0.f), AA_ERR_ARG,
+             "aa_dpo_loss_ext: loss_type %d with rpo_alpha %g needs the row counts", loss_type, rpo_alpha);
+  const double dt_max = lp_dtype == AA_F16 ? 65504.0 : lp_dtype == AA_BF16 ? 3.3895313892515355e38 : 3.4028234663852886e38;
+  DpoExtParams p;
+  static_cast<DpoObjParams &>(p) =
+      DpoObjParams{{policy_lp, ref_lp, lp_dtype, n_pairs, width, lp_row_stride, scale_coeff,
+                    mode == AA_MODE_FAITHFUL ? lp_dtype : AA_F32, input_ids, L, ids_row_stride, per_pair, grad_seg,
+                    stats, counter, nullptr, CollParams{nullptr, 0, 1, 0u, 0u}, status},
+                   loss_type, label_smoothing, rpo_alpha, counts};
+  p.fdiv = f_divergence;
+  p.f_alpha = f_alpha_coef;
+  p.tau = discopop_tau;
+  p.exp_cap = static_cast<float>(floor(log(dt_max) * 1e4) / 1e4);
+  p.exo_c1 = exo_log_keep;
+  p.exo_c2 = exo_log_smooth;
+  dpo_loss_kernel<128, DpoExtParams><<<n_pairs, 128, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("aa_dpo_loss_ext");
 }

@@ -928,7 +928,10 @@ def sequence_log_probs(logits: torch.Tensor, input_ids: torch.Tensor, response_l
 
 
 DPO_LOSS_TYPES = {'sigmoid': 0, 'robust': 1, 'hinge': 2, 'ipo': 3, 'sppo_hard': 4, 'nca_pair': 5, 'apo_zero': 6,
-                  'apo_down': 7}  # include/aa_b200.h AA_DPO_*
+                  'apo_down': 7, 'exo_pair': 8, 'discopop': 9, 'aot': 10, 'aot_pair': 11}  # include/aa_b200.h AA_DPO_*
+DPO_F_DIVERGENCES = {'reverse_kl': 0, 'js_divergence': 1, 'alpha_divergence': 2}  # include/aa_b200.h AA_DPO_FDIV_*
+DPO_AOT_MAX_PAIRS = 1024  # include/aa_b200.h AA_DPO_AOT_MAX_PAIRS: the pairs one rank's AOT sort takes
+_DPO_EXT_TYPES = ('exo_pair', 'discopop', 'aot', 'aot_pair')  # aa_dpo_loss_ext's own types
 
 
 @dataclasses.dataclass(frozen=True)
@@ -945,15 +948,30 @@ class DpoObjective:
         nca_pair   -logsigmoid(beta a) - logsigmoid(-beta a) / 2 - logsigmoid(-beta b) / 2
         apo_zero   (1 - sigmoid(beta a)) + sigmoid(beta b)
         apo_down   sigmoid(beta a) + (1 - sigmoid(beta h))
+        exo_pair   sigmoid(z) (logsigmoid(z) - log(1 - e')) + sigmoid(-z) (logsigmoid(-z) - log e'), e' = eps or 1e-3
+        discopop   -logsigmoid(z) (1 - m) + exp(-z) m, m = sigmoid(z / discopop_tau)
+        aot_pair   the kept pairs' a and, separately, their b sorted ascending (stable, NaN last); with
+                   d_k = a_(k) - b_(k) the loss at position k is -(1 - eps) logsigmoid(beta d_k) - eps logsigmoid(-beta d_k)
+        aot        the same with pc - pr and rc - rr sorted in place of a and b
+
+    f_divergence_type replaces h before a loss type that reads z = beta * h (sigmoid, robust, hinge, exo_pair) does:
+    'reverse_kl' keeps h = a - b, 'js_divergence' takes h - (softplus(a) - softplus(b)), 'alpha_divergence' takes
+    (cap_exp(-alpha b) - cap_exp(-alpha a)) / alpha with alpha = f_alpha_divergence_coef and cap_exp(x) =
+    exp(min(x, floor(log(finfo(dtype).max) * 1e4) / 1e4)) in the log-prob dtype (no gradient where the clamp holds).
+    A field away from its default on a type that does not read it raises.
 
     The loss is the mean over the kept pairs; rpo_alpha > 0 adds rpo_alpha * NLL, NLL = -sum(pc) / sum(R_c - 1) over
     the kept pairs' chosen rows (RPO), reported as train/nll_loss.  reference_free: rc = rr = 0 and no reference model
-    runs.  The metrics keep the reference's definitions for every loss type.  Checked here, before anything runs."""
+    runs.  The metrics keep the reference's definitions for every loss type (from the unsorted ratios under AOT).
+    Checked here, before anything runs."""
 
     loss_type: str = 'sigmoid'
     label_smoothing: float = 0.0
     rpo_alpha: float = 0.0
     reference_free: bool = False
+    f_divergence_type: str = 'reverse_kl'
+    f_alpha_divergence_coef: float = 1.0
+    discopop_tau: float = 0.05
 
     def __post_init__(self):
         if self.loss_type not in DPO_LOSS_TYPES:
@@ -961,18 +979,38 @@ class DpoObjective:
         eps, alpha = float(self.label_smoothing), float(self.rpo_alpha)
         if not 0.0 <= eps < 0.5:
             raise ValueError(f'label_smoothing must lie in [0, 0.5), got {self.label_smoothing!r}')
-        if eps > 0.0 and self.loss_type not in ('sigmoid', 'robust'):
-            raise ValueError(f"label_smoothing applies to loss_type 'sigmoid' and 'robust' only, not {self.loss_type!r}")
+        if eps > 0.0 and self.loss_type not in ('sigmoid', 'robust', 'exo_pair', 'aot', 'aot_pair'):
+            raise ValueError(f"label_smoothing applies to loss_type 'sigmoid', 'robust', 'exo_pair', 'aot' and 'aot_pair' "
+                             f"only, not {self.loss_type!r}")
         if not (alpha >= 0.0 and math.isfinite(alpha)):
             raise ValueError(f'rpo_alpha must be a finite value >= 0, got {self.rpo_alpha!r}')
         if not isinstance(self.reference_free, bool):
             raise ValueError(f'reference_free must be a bool, got {self.reference_free!r}')
+        if self.f_divergence_type not in DPO_F_DIVERGENCES:
+            raise ValueError(f'f_divergence_type must be one of {sorted(DPO_F_DIVERGENCES)}, got {self.f_divergence_type!r}')
+        if self.f_divergence_type != 'reverse_kl' and self.loss_type not in ('sigmoid', 'robust', 'hinge', 'exo_pair'):
+            raise ValueError(f"f_divergence_type {self.f_divergence_type!r} applies to loss_type 'sigmoid', 'robust', "
+                             f"'hinge' and 'exo_pair' only, not {self.loss_type!r}")
+        coef, tau = float(self.f_alpha_divergence_coef), float(self.discopop_tau)
+        if not (coef > 0.0 and math.isfinite(coef)):
+            raise ValueError(f'f_alpha_divergence_coef must be a finite value > 0, got {self.f_alpha_divergence_coef!r}')
+        if coef != 1.0 and self.f_divergence_type != 'alpha_divergence':
+            raise ValueError("f_alpha_divergence_coef applies to f_divergence_type 'alpha_divergence' only")
+        if not (tau > 0.0 and math.isfinite(tau)):
+            raise ValueError(f'discopop_tau must be a finite value > 0, got {self.discopop_tau!r}')
+        if tau != 0.05 and self.loss_type != 'discopop':
+            raise ValueError(f"discopop_tau applies to loss_type 'discopop' only, not {self.loss_type!r}")
 
     @property
     def is_default(self) -> bool:
         """The reference's objective: K2 runs today's launch."""
         return (self.loss_type == 'sigmoid' and float(self.label_smoothing) == 0.0 and float(self.rpo_alpha) == 0.0
-                and not self.reference_free)
+                and not self.reference_free and not self.needs_ext)
+
+    @property
+    def needs_ext(self) -> bool:
+        """A loss type or f-divergence of K2's extended variant (aa_dpo_loss_ext)."""
+        return self.loss_type in _DPO_EXT_TYPES or self.f_divergence_type != 'reverse_kl'
 
     @property
     def needs_counts(self) -> bool:
@@ -999,7 +1037,8 @@ def _dpo_counts(obj: DpoObjective | None, response_lens, device):
 def _dpo_launch(policy_lp, ref_lp, scale_coeff, mode_code, input_ids, want_grad_seg, coll=None, obj=None, counts=None):
     """coll: an `_lib.AaColl` descriptor (utils.multi_process.FusedPackedAllReduce.next()) -> K2's last block
     also all-reduces the stats over NVLink; the reduced vector comes back as a 4th result.  obj: a non-default
-    DpoObjective -> aa_dpo_loss_obj (ref_lp None when reference-free; stats gets a 9th lane, the NLL, with rpo_alpha)."""
+    DpoObjective -> aa_dpo_loss_obj, or aa_dpo_loss_ext for its f-divergences and the types only that entry has (ref_lp
+    None when reference-free; stats gets a 9th lane, the NLL, with rpo_alpha)."""
     import ctypes
 
     dev = policy_lp.device
@@ -1016,11 +1055,20 @@ def _dpo_launch(policy_lp, ref_lp, scale_coeff, mode_code, input_ids, want_grad_
     if obj is not None:
         if coll is not None:
             raise ValueError('the DPO objective options have no in-kernel collective: all-reduce the stats instead')
-        L.check(L.lib().aa_dpo_loss_obj(
-            policy_lp.data_ptr(), L.ptr(ref_lp), L.dtype_code(policy_lp.dtype), B, W, policy_lp.stride(0),
-            float(scale_coeff), mode_code, DPO_LOSS_TYPES[obj.loss_type], float(obj.label_smoothing),
-            float(obj.rpo_alpha), L.ptr(counts), *ids_args, per_pair.data_ptr(), grad_seg.data_ptr(), stats.data_ptr(),
-            sc['counter'][0:1].data_ptr(), sc['status'].data_ptr(), L.stream_ptr(dev)))
+        head = (policy_lp.data_ptr(), L.ptr(ref_lp), L.dtype_code(policy_lp.dtype), B, W, policy_lp.stride(0),
+                float(scale_coeff), mode_code, DPO_LOSS_TYPES[obj.loss_type], float(obj.label_smoothing),
+                float(obj.rpo_alpha))
+        tail = (L.ptr(counts), *ids_args, per_pair.data_ptr(), grad_seg.data_ptr(), stats.data_ptr(),
+                sc['counter'][0:1].data_ptr(), sc['status'].data_ptr(), L.stream_ptr(dev))
+        if obj.needs_ext:
+            if obj.loss_type in ('aot', 'aot_pair') and B > DPO_AOT_MAX_PAIRS:
+                raise ValueError(f'{obj.loss_type} sorts at most {DPO_AOT_MAX_PAIRS} pairs per rank, got {B}')
+            e = float(obj.label_smoothing) or 1e-3  # EXO's constants in double, as TRL forms them from the Python value
+            L.check(L.lib().aa_dpo_loss_ext(*head, DPO_F_DIVERGENCES[obj.f_divergence_type],
+                                            float(obj.f_alpha_divergence_coef), float(obj.discopop_tau),
+                                            math.log(1 - e), math.log(e), *tail))
+        else:
+            L.check(L.lib().aa_dpo_loss_obj(*head, *tail))
         return per_pair, stats, grad_seg
     stats_global = torch.empty(8, dtype=torch.float32, device=dev) if coll is not None else None
     L.check(L.lib().aa_dpo_loss(

@@ -6,8 +6,8 @@ swaps, without touching any reference file,
   * align_anything.utils.tools.{gather_log_probabilities, masked_mean, move_padding_left}
     (and the names re-imported by the trainer modules),
   * DPOTrainer.{compute_log_probs, loss, train_step} of the text / image / audio / video trainers (the classes also
-    get the objective switches `loss_type`, `label_smoothing`, `rpo_alpha` and `reference_free`, unset: the
-    reference's loss),
+    get the objective switches `loss_type`, `label_smoothing`, `rpo_alpha`, `reference_free`, `f_divergence_type`,
+    `f_alpha_divergence_coef` and `discopop_tau`, unset: the reference's loss),
   * PPOTrainer.{rollout, actor_loss_fn, critic_loss_fn, add_kl_divergence_regularization,
     get_advantages_and_returns, rl_step, ptx_step} of the text / image / audio / video trainers, and the
     multimodal trainers' actor_step (its post-generate bookkeeping); `reward_model_step` and the text trainer's

@@ -21,12 +21,17 @@ __all__ = ['DPOTrainer', 'strip_pad']
 
 METRIC_KEYS = ('train/loss', 'train/reward', 'train/better_sample_reward', 'train/worse_sample_reward',
                'train/reward_accuracy', 'train/reward_margin')
-DPO_OBJECTIVE_KEYS = ('loss_type', 'label_smoothing', 'rpo_alpha', 'reference_free')
+DPO_OBJECTIVE_KEYS = ('loss_type', 'label_smoothing', 'rpo_alpha', 'reference_free', 'f_divergence_type',
+                      'f_alpha_divergence_coef', 'discopop_tau')
 
 
 def dpo_objective_of(tr) -> ops.DpoObjective | None:
     """The DPO objective in effect (switch_of each of DPO_OBJECTIVE_KEYS), or None when every key is unset: the
-    reference's loss and today's launches.  A bad value raises ValueError here, before anything runs."""
+    reference's loss and today's launches.  A bad value raises ValueError here, before anything runs, and so does
+    TRL's `use_weighting` (WPO), which this trainer does not implement: a recipe that sets it must not silently train
+    unweighted DPO."""
+    if switch_of(tr, 'use_weighting'):
+        raise ValueError('use_weighting (WPO) is not supported by this DPO trainer: unset it, or set it to false')
     fields = {k: switch_of(tr, k) for k in DPO_OBJECTIVE_KEYS}
     fields = {k: v for k, v in fields.items() if v is not None}
     return ops.DpoObjective(**fields) if fields else None
@@ -50,16 +55,22 @@ class DPOTrainer:
     fused_lm_head = False
     lm_head_chunk_rows = None
     # The objective (ops.DpoObjective, TRL's DPOConfig names): loss_type ('sigmoid', 'robust', 'hinge', 'ipo',
-    # 'sppo_hard', 'nca_pair', 'apo_zero', 'apo_down'), label_smoothing (cDPO / robust), rpo_alpha (RPO's NLL term on
-    # the chosen responses, logged as train/nll_loss) and reference_free (no reference model forward).  None: the
-    # reference's loss; `cfgs.train_cfgs.<name>` overrides each when set.
+    # 'sppo_hard', 'nca_pair', 'apo_zero', 'apo_down', 'exo_pair', 'discopop', 'aot', 'aot_pair'), label_smoothing
+    # (cDPO / robust / EXO / AOT), rpo_alpha (RPO's NLL term on the chosen responses, logged as train/nll_loss),
+    # reference_free (no reference model forward), f_divergence_type ('reverse_kl', 'js_divergence',
+    # 'alpha_divergence') with f_alpha_divergence_coef, and discopop_tau.  None: the reference's loss;
+    # `cfgs.train_cfgs.<name>` overrides each when set.
     loss_type = None
     label_smoothing = None
     rpo_alpha = None
     reference_free = None
+    f_divergence_type = None
+    f_alpha_divergence_coef = None
+    discopop_tau = None
     # the class attributes above that the grafted methods read: patch.install() copies them onto the reference's classes
     SWITCHES = ('strip_pad_tokens', 'skip_identical_pairs', 'mode', 'fused_lm_head', 'lm_head_chunk_rows', 'loss_type',
-                'label_smoothing', 'rpo_alpha', 'reference_free')
+                'label_smoothing', 'rpo_alpha', 'reference_free', 'f_divergence_type', 'f_alpha_divergence_coef',
+                'discopop_tau')
 
     def __init__(self, cfgs, model, reference_model, tokenizer, infer_batch=None) -> None:
         self.cfgs = cfgs

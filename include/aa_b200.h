@@ -271,6 +271,44 @@ int aa_dpo_loss_obj(const void *policy_lp, const void *ref_lp, int lp_dtype, int
                     const int32_t *status, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * K2 with the further objectives of TRL's DPOConfig (DESIGN.md section 4.13): aa_dpo_loss_obj's arguments and
+ * arithmetic, plus f-divergences (f_divergence_type) and the loss types below.  With a, b, h as above and
+ * e = label_smoothing:
+ *   f_divergence (replaces h; only for SIGMOID, ROBUST, HINGE and EXO_PAIR):
+ *     AA_DPO_FDIV_REVERSE_KL  h = a - b                                       (aa_dpo_loss_obj's h)
+ *     AA_DPO_FDIV_JS          h = (a - b) - (softplus(a) - softplus(b))
+ *     AA_DPO_FDIV_ALPHA       h = (cap_exp(-f_alpha_coef b) - cap_exp(-f_alpha_coef a)) / f_alpha_coef,
+ *                             cap_exp(x) = exp(min(x, floor(log(finfo(lp dtype).max) * 1e4) / 1e4)): no gradient
+ *                             where the clamp is active
+ *   AA_DPO_EXO_PAIR  sig(z) (logsig(z) - log(1 - e')) + sig(-z) (logsig(-z) - log e'), e' = e if e > 0 else 1e-3
+ *   AA_DPO_DISCOPOP  -logsig(z) (1 - m) + exp(-z) m, m = sigmoid(z / discopop_tau)
+ *   AA_DPO_AOT_PAIR  the kept pairs' a and, separately, their b sorted ascending (stable: NaN last, ties to the
+ *                    smaller pair index); delta_k = a_(k) - b_(k); -(1-e) logsig(beta delta_k) - e logsig(-beta delta_k)
+ *   AA_DPO_AOT       the same with pc - pr and rc - rr sorted in place of a and b
+ * AOT: per_pair[0][i] is the loss at the sorted position of pair i's first key (a_i, or pc_i - pr_i), each row's
+ * grad_seg entry the gradient at the position its key landed in; n_pairs <= AA_DPO_AOT_MAX_PAIRS.
+ * label_smoothing is also legal for EXO_PAIR, AOT and AOT_PAIR.  exo_log_keep = log(1 - e') and exo_log_smooth =
+ * log(e'): EXO's two constants, formed by the caller in double from its own label_smoothing (an fp32 copy of 0.1 is
+ * not 0.1), both < 0; read by EXO_PAIR only.  f_alpha_coef (> 0, finite) must be 1 unless
+ * f_divergence is ALPHA; discopop_tau (> 0, finite) must be 0.05 unless the type is DISCOPOP.  With f_divergence
+ * REVERSE_KL and a type of aa_dpo_loss_obj the results are aa_dpo_loss_obj's, bit for bit.
+ * ------------------------------------------------------------------------------------- */
+enum {
+  AA_DPO_EXO_PAIR = 8,
+  AA_DPO_DISCOPOP = 9,
+  AA_DPO_AOT = 10,
+  AA_DPO_AOT_PAIR = 11,
+  AA_DPO_AOT_MAX_PAIRS = 1024
+};
+enum { AA_DPO_FDIV_REVERSE_KL = 0, AA_DPO_FDIV_JS = 1, AA_DPO_FDIV_ALPHA = 2 };
+int aa_dpo_loss_ext(const void *policy_lp, const void *ref_lp, int lp_dtype, int32_t n_pairs, int32_t width,
+                    int64_t lp_row_stride, float scale_coeff, int mode, int loss_type, float label_smoothing,
+                    float rpo_alpha, int f_divergence, float f_alpha_coef, float discopop_tau, float exo_log_keep,
+                    float exo_log_smooth, const int32_t *counts,
+                    const int64_t *input_ids, int32_t L, int64_t ids_row_stride, float *per_pair, float *grad_seg,
+                    float *stats, uint32_t *counter, const int32_t *status, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Pair bookkeeping and slice sums of SimPO / ORPO / KTO (SURVEY.md 8f row 2).
  * aa_pair_slices: trainers/text_to_text/simpo.py:61-77 (orpo.py:61-77, kto.py:111-125): identical-pair test, last
  *   attended index of both rows, first index where the id rows differ -> out int32 [4][n_pairs] =
