@@ -431,16 +431,22 @@ __device__ __forceinline__ void dpo_obj_finish(const Params &p, float sum_loss_o
   const volatile float *v_valid = p.per_pair + 4 * B;
   float g_nll = 0.f;
   if (p.alpha > 0.f) {  // NLL = -(sum of the kept chosen sums) / (their scored rows): the token mean, as in RPO
-    float s_pc = 0.f, s_cnt = 0.f;
+    // the count is summed in integers and rounded to fp32 once, as ATen converts the reference's exact Python count:
+    // an fp32 sum past 2^24 rounds at every level of the tree
+    __shared__ unsigned long long cnt_total;
+    if (tid == 0) cnt_total = 0ull;
+    float s_pc = 0.f;
+    long long s_cnt = 0;
     for (int k = tid; k < B; k += THREADS) {
       if (v_valid[k] != 0.f) {
         s_pc += v_g[k];
-        s_cnt += static_cast<float>(p.counts[k]);
+        s_cnt += p.counts[k];
       }
     }
-    s_pc = block_sum<THREADS>(s_pc, scratch);
-    s_cnt = block_sum<THREADS>(s_cnt, scratch);
-    const float inv_cnt = 1.f / s_cnt;  // x / int: x * (1 / n)
+    s_pc = block_sum<THREADS>(s_pc, scratch);  // its barriers order the zeroing above before the adds below
+    atomicAdd(&cnt_total, static_cast<unsigned long long>(s_cnt));
+    __syncthreads();
+    const float inv_cnt = 1.f / static_cast<float>(static_cast<long long>(cnt_total));  // x / int: x * (1 / n)
     const float nll = -round_to(__fmul_rn(round_to(s_pc, rd), inv_cnt), rd);
     g_nll = round_to(__fmul_rn(-round_to(p.alpha, rd), inv_cnt), rd);  // Add -> Mul(alpha) -> Neg -> Div -> Sum
     if (tid == 0) {
